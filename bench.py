@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py - rows/sec of the tabular-DNN train step (BASELINE.json metric) on N B200s.
+"""bench.py - rows/sec of the tabular-DNN train step (BASELINE.json metric) on N H100s.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--config cfg2|cfg1|cfg0] [--impl b200|reference]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
            bench.py --gpus N --steps K --warmup W
 
@@ -19,6 +20,10 @@ reported under `also`.
              resolved" .. "last CTA exit"), so that the kernel times are the in-step times and sum to <= ms_per_step
   eval       BASELINE config 5: batch scoring of the trained 2000-col net, device-resident 100 M rows and host-buffer e2e
   cpu_baseline / --impl reference   the reference-equivalent CPU worker (oracle port on torch-CPU) on the host cores
+  --dump-outputs DIR   after the timed steps of the headline config (rank 0): what the last timed step handed back,
+             DIR/params.npy (float32, the flat parameter vector after its update) and DIR/loss.npy (float64, its loss).
+             Inputs and initial parameters are seeded, so two builds run with the same arguments can be compared output
+             for output (up to the summation order of the atomically reduced gradients).
 
 Weak scaling: every rank owns its own `batch` rows per step.  PyTorch is plumbing only (rendezvous, barrier, max-reduce,
 events, synthetic device data for the eval leg); all compute is libshifu_b200.so.
@@ -73,7 +78,7 @@ def synth_dataset(cfg, rank, n_batches=None):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -142,7 +147,7 @@ def config_block(name, cfg, world):
     return {"workload": "%s: %d cols x %d rows/GPU/step, MLP %s relu, %s, MSE-on-sigmoid loss" %
                         (name, cfg["F"], cfg["batch"], cfg["hidden"], cfg["optimizer"]),
             "global_batch": cfg["batch"] * world, "rows_per_gpu": cfg["batch"], "parallelism": "dp%d" % world,
-            "resident_set": "%d batches (%.0f MB fp32 per GPU) cycled, larger than the 126 MB L2 (no L2 flush needed)" %
+            "resident_set": "%d batches (%.0f MB fp32 per GPU) cycled, larger than the 50 MB L2 (no L2 flush needed)" %
                             (cfg["n_batches"], cfg["n_batches"] * cfg["batch"] * cfg["F"] * 4 / 1e6)}
 
 
@@ -264,6 +269,8 @@ def main():
     ap.add_argument("--sustained-seconds", type=float, default=3.0)
     ap.add_argument("--e2e-steps", type=int, default=0, help="steps of the host-buffer leg (default: min(steps, 50))")
     ap.add_argument("--also", default="cfg1", help="second config measured on the resident leg only and reported under 'also' ('' = none)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the parameters and loss of the last timed step of the headline config to DIR/*.npy")
     args = ap.parse_args()
     cfg = CONFIGS[args.config]
     rank = int(os.environ.get("RANK", "0"))
@@ -302,16 +309,10 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak_tf = float(peaks.get("bf16_tflops", 1590.0))
-    peak_sus = float(peaks.get("bf16_tflops_sustained", 1400.0))
-    peak_src = "measured burst (MEASURED_PEAKS.json bf16_tflops)" if peaks else "fallback 1.59 PF (B200_PROFILING.md)"
-    # dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` capture of this command
-    # (scripts/summarize_ncu.py writes the file); null when no capture of the current build has been committed
-    traffic_db = {}
-    try:
-        traffic_db = json.load(open(os.path.join(ROOT, "profiles", "ncu_r02_traffic.json")))
-    except Exception:
-        pass
+    # without measured peaks: NVIDIA's H100 SXM data-sheet figures (dense BF16, 700 W card), not reached rates
+    peak_tf = float(peaks.get("bf16_tflops", 989.0))
+    peak_sus = float(peaks.get("bf16_tflops_sustained", 989.0))
+    peak_src = "measured burst (MEASURED_PEAKS.json bf16_tflops)" if peaks else "H100 SXM data sheet, 989 TFLOP/s dense BF16"
 
     sampler = ClockSampler(local_rank).start() if rank == 0 else None
 
@@ -373,6 +374,12 @@ def main():
         ms, wall0, wall1 = timed_run(args.steps, args.warmup)
         clk = sampler.window(wall0, wall1) if (sampler and full) else None
         last_loss = t.last_loss()
+        if full and args.dump_outputs:
+            params = t.get_params()      # (sharded update: every rank takes part)
+            if rank == 0:
+                os.makedirs(args.dump_outputs, exist_ok=True)
+                np.save(os.path.join(args.dump_outputs, "params.npy"), np.asarray(params, np.float32))
+                np.save(os.path.join(args.dump_outputs, "loss.npy"), np.asarray([last_loss], np.float64))
         value = world * B * args.steps / (ms / 1e3)
         res = {"value": value, "ms_per_step": ms / args.steps, "last_loss": last_loss, "clocks": clk,
                "gradient_exchange": exchange, "gpu_launches": t.kernels_per_step(B) * args.steps,
@@ -386,7 +393,7 @@ def main():
             res["sustained"] = {"value": world * B * n_sus / (ms_s / 1e3), "unit": "rows/s", "steps": n_sus, "seconds": ms_s / 1e3,
                                 "ms_per_step": ms_s / n_sus, "clocks": sampler.window(w0 + 0.5, w1) if sampler else None,
                                 "step_fraction_of_sustained_peak": (B * n_sus / (ms_s / 1e3) * f_train / 1e12) / peak_sus,
-                                "peak": peak_sus, "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (4 s cuBLAS loop)"}
+                                "peak": peak_sus, "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else peak_src}
 
         # ---------------- roofline: in-graph kernel spans ----------------
         roofline = None
@@ -404,11 +411,9 @@ def main():
                 gem = [k for k in tl["kernels"] if k["flops"]]
                 top = max(gem, key=lambda k: k["us"])
                 sum_us = sum(k["us"] for k in gem)
-                key = "%s/%s" % (name, top["kernel"])
                 roofline = {"bound": "tensor", "achieved": top["tflops"], "peak": peak_tf, "unit": "TFLOP/s",
-                            "frac": top["tflops"] / peak_tf, "traffic": traffic_db.get(key),
-                            "traffic_source": "profiles/ncu_r02_traffic.json (ncu --set full capture of this command)" if key in traffic_db else None,
-                            "kernel": "gemm_tc_kernel %s (tcgen05 + TMA), the longest GEMM of the step" % top["kernel"],
+                            "frac": top["tflops"] / peak_tf, "traffic": None,
+                            "kernel": "gemm_tc_kernel %s (wgmma + TMA), the longest GEMM of the step" % top["kernel"],
                             "flops_per_launch": top["flops"], "kernel_us": top["us"], "peak_source": peak_src,
                             "method": "%globaltimer stamps inside the captured step graph of a second, traced trainer: dependencies "
                                       "resolved (CTA 0) .. last CTA exit of every kernel; no profiler, no extra launches",
@@ -478,7 +483,7 @@ def main():
         # ---------------- ingest leg: load_data's per-cell float() loop on the GPU (SURVEY 8f rank 1) ----------------
         res["ingest"] = None
         if rank == 0 and world == 1 and not args.no_ingest:
-            res["ingest"] = ingest_leg(sb, local_rank, float(peaks.get("hbm_gbs", 6650.0)))
+            res["ingest"] = ingest_leg(sb, local_rank, float(peaks.get("hbm_gbs", 3350.0)))
 
         # ---------------- CPU baseline (rank 0, N = 1 only) ----------------
         res["cpu_baseline"] = None
@@ -556,7 +561,7 @@ def ingest_leg(sb, device, hbm_gbs):
 
 
 def eval_leg(sb, torch, c, trained_params, X_host, world, rank, local_rank, barrier, max_over_ranks, peak_tf):
-    """BASELINE config 5 (TensorflowModel.compute, TensorflowModel.java:53-94, 100 M rows of the 2000-col net on one B200):
+    """BASELINE config 5 (TensorflowModel.compute, TensorflowModel.java:53-94, 100 M rows of the 2000-col net on one H100):
     rows are sharded over the ranks with no collective (strong scaling of the 100 M-row job).
       device-resident  synthetic fp32 rows generated on the device in 1 Mi-row chunks (8.4 GB, >> L2), scored with
                        sb_model_score_device (cast + forward GEMMs + output layer), CUDA events on the model's stream

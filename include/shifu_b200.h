@@ -1,5 +1,5 @@
 /*
- * shifu_b200.h - C ABI of the B200-native tabular-DNN train/score hot path.
+ * shifu_b200.h - C ABI of the H100-native tabular-DNN train/score hot path.
  *
  * This is the drop-in boundary (SURVEY.md section 8b, seam B3).  The reference has no
  * native boundary of its own for this path: its arithmetic is reached through
@@ -21,7 +21,7 @@
  *     i.e. the variables weight_hidden_layer{l}, biases_hidden_layer{l}, weight_shifu_output_0,
  *     biases_shifu_output_0 of ssgd_monitor.py:59,64,99-104,121.
  *   - there is NO CPU fallback: every compute entry point fails with SB_ERR_CUDA when no
- *     sm_100 device is present.
+ *     sm_90 device is present.
  */
 #ifndef SHIFU_B200_H
 #define SHIFU_B200_H
@@ -52,10 +52,10 @@ typedef enum { SB_LOSS_MSE = 0, SB_LOSS_SIGMOID_CE = 1 } sb_loss;
 /* ADADELTA: ssgd_monitor.py:138; ADAM: ssgd.py:57; SGD: ssgd_monitor_bk.py:81; MOMENTUM: north star */
 typedef enum { SB_OPT_ADADELTA = 0, SB_OPT_ADAM = 1, SB_OPT_SGD = 2, SB_OPT_MOMENTUM = 3 } sb_optimizer;
 /* SB_PREC_FP32: fp32 operands and fp32 accumulation end to end (what TF-CPU computes) - parity mode (CUDA cores).
- * SB_PREC_BF16: bf16 operands on tcgen05 tensor cores, fp32 accumulation in TMEM, fp32 master
+ * SB_PREC_BF16: bf16 operands on the tensor cores (wgmma), fp32 accumulation, fp32 master
  *               weights and optimizer state - performance mode.
  * SB_PREC_FP32_TC: fp32-class accuracy ON the tensor cores: every fp32 operand value is split into three bf16 parts
- *               (v = p0 + p1 + p2, exact to ~2^-24), the six part products with i + j < 3 accumulate in fp32 TMEM.  Same
+ *               (v = p0 + p1 + p2, exact to ~2^-24), the six part products with i + j < 3 accumulate in fp32.  Same
  *               kernels as SB_PREC_BF16 over a six times longer K axis; meets the fp32 tolerances (loss / gradients
  *               1e-4, scores 1e-5).  Parity mode that is not a CUDA-core program.
  * SB_PREC_BF16X2: two parts, three products (~2^-17 relative per product): half the cost of FP32_TC. */
@@ -286,7 +286,7 @@ int sb_savedmodel_read(const char* saved_model_dir, const char* input_name, cons
                        int64_t* n_params);
 
 /* ---- kernel-level test hooks (parity tests of single kernels through the C ABI) ---- */
-/* D[M,N] = A[M,K] * B[N,K]^T on the tcgen05 path: A, B are fp32 host arrays that are rounded to
+/* D[M,N] = A[M,K] * B[N,K]^T on the wgmma path: A, B are fp32 host arrays that are rounded to
  * bf16 on the device; D fp32 host.  split_k >= 1. */
 int sb_debug_gemm_bf16(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K,
                        int32_t split_k, int device);
@@ -294,8 +294,9 @@ int sb_debug_gemm_bf16(const float* A, const float* B, float* D, int32_t M, int3
  * B ([N,K] or [K,N]).  Instantiated combinations: (0,0) dA GEMM, (0,1) forward GEMM, (1,1) dW GEMM. */
 int sb_debug_gemm_bf16_ex(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K,
                           int32_t split_k, int32_t a_mn, int32_t b_mn, int device);
-/* same, forcing the tile configuration: cfg_cg = 1 (one CTA per 128 x cfg_bn tile, cfg_bn 64|128) or 2 (CTA pair per
- * 256 x cfg_bn tile, tcgen05 cta_group::2, cfg_bn 128|256); cfg_cg = 0 lets the planner choose. */
+/* same, forcing the tile configuration: cfg_cg = 1 (one CTA per 128 x cfg_bn tile, cfg_bn 64|128) or 2 (cluster of two
+ * CTAs per 256 x cfg_bn tile, B multicast, cfg_bn 128|256; not with sb_debug_gemm_bench); cfg_cg = 0 lets the planner
+ * choose. */
 int sb_debug_gemm_bf16_cfg(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K,
                            int32_t split_k, int32_t a_mn, int32_t b_mn, int32_t cfg_cg, int32_t cfg_bn, int device);
 

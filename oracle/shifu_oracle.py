@@ -450,9 +450,9 @@ def bf16_round(a: np.ndarray) -> np.ndarray:
 def loss_and_grads_bf16(net: NetDesc, params, X, y, w, loss=LOSS_MSE, fused_out=True):
     """The SAME math as loss_and_grads, with a bf16 rounding wherever the CUDA performance mode stores an
     operand as bf16 (DESIGN.md 'precision modes'): X, hidden-layer W, every activation A_l and every dZ_l that is
-    fed to a tensor-core GEMM.  Accumulation stays in higher precision (fp64 here vs fp32 in TMEM), the output
+    fed to a tensor-core GEMM.  Accumulation stays in higher precision (fp64 here vs fp32 in the GEMM), the output
     layer uses fp32 w_o, and bias gradients / dw_o are summed from the un-rounded values exactly like the kernels
-    do.  Lets the tests check the tcgen05 path to ~1e-5 instead of the loose bf16-vs-fp32 bound.
+    do.  Lets the tests check the tensor-core path to ~1e-5 instead of the loose bf16-vs-fp32 bound.
     fused_out=True (training steps with h_L <= 256): the last hidden activation A_L never leaves the GEMM epilogue, so
     it is NOT rounded to bf16 before the output layer; fused_out=False is the forward-only / scoring path."""
     q = bf16_round

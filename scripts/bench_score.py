@@ -8,6 +8,11 @@ import shifu_tensorflow_b200 as sb
 from oracle import shifu_oracle as so
 
 F, hidden = 2000, [1024, 512, 256]
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+try:      # the same peak source as bench.py: measured peaks, else the H100 SXM data-sheet dense bf16 rate
+    PEAK = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("bf16_tflops", 989.0)) * 1e12
+except Exception:
+    PEAK = 989e12
 net = so.NetDesc(F, hidden, [so.ACT_RELU] * 3)
 flat = so.flatten_params(so.xavier_init(net, 1))
 out = {}
@@ -37,7 +42,7 @@ for prec, name in ((sb.PREC_BF16, "bf16"), (sb.PREC_FP32, "fp32")):
     Xh = torch.randn(hrows, F).clamp_(-4, 4).pin_memory().numpy()
     m.score(Xh[:1024])
     t0 = time.perf_counter(); m.score(Xh); th = time.perf_counter() - t0
-    out[name] = {"device_resident_rows_per_s": rps, "tflops": rps * 5407232 / 1e12, "frac_of_peak": rps * 5407232 / 1689.8e12,
+    out[name] = {"device_resident_rows_per_s": rps, "tflops": rps * 5407232 / 1e12, "frac_of_peak": rps * 5407232 / PEAK,
                  "seconds_per_100M_rows": 1e8 / rps, "max_abs_err_vs_oracle": err, "host_rows_per_s": hrows / th}
     m.close()
 print(json.dumps({"metric": "rows/sec batch scoring, cfg2 net (2000 -> 1024 -> 512 -> 256 -> 1)", "n_gpus": 1, **out}))

@@ -1,5 +1,5 @@
 // Peer-memory link probe (2+ GPUs of one node): what the exchange kernels of csrc/xchg_p2p.cuh can expect from the fabric.
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o scripts/p2p_probe scripts/p2p_probe.cu && scripts/p2p_probe
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o scripts/p2p_probe scripts/p2p_probe.cu && scripts/p2p_probe
 // Prints: peer attributes, copy-engine bandwidth, SM-issued peer load / store bandwidth by grid size and bytes in flight,
 // flag round trip (st.release.sys into the peer -> peer spins locally -> answers).
 #include <cuda_runtime.h>

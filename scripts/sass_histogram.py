@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""cuobjdump -sass of libshifu_b200.so -> opcode histogram per kernel family (evidence for B200_PROFILING.md's
-"what proves a Blackwell-native kernel": UTC*MMA = tcgen05.mma, LDTM = tcgen05.ld, UTMALDG/UTMASTG = TMA, HMMA = legacy).
+"""cuobjdump -sass of libshifu_b200.so -> opcode histogram per kernel family (what shows a Hopper-native kernel:
+HGMMA = wgmma, UTMALDG/UTMASTG = TMA, SYNCS = mbarrier, HMMA = the older warp-level mma).
 
-    python scripts/sass_histogram.py > profiles/sass_r02_gemm_tc.txt
+    python scripts/sass_histogram.py
 """
 import collections
 import os
@@ -36,7 +36,7 @@ def main():
     tot = collections.Counter()
     for name, cnt in fam.items():
         keep = {k: v for k, v in cnt.items() if any(k.startswith(p) for p in KEY)}
-        if not any(k.startswith(("UTC", "LDTM", "UTMA", "MULTIMEM", "HMMA")) for k in keep) and "gemm" not in name and "xchg" not in name and "allreduce" not in name:
+        if not any(k.startswith(("HGMMA", "UTMA", "MULTIMEM", "HMMA")) for k in keep) and "gemm" not in name and "xchg" not in name and "allreduce" not in name:
             continue
         print("\n%s   [%d SASS instructions]" % (name, cnt["#instructions"]))
         for k in sorted(keep):
@@ -45,8 +45,8 @@ def main():
     print("\n# totals over the listed kernels")
     for k in sorted(tot):
         print("    %-44s %6d" % (k, tot[k]))
-    legacy = sum(v for k, v in tot.items() if k.startswith(("HMMA", "HGMMA")))
-    print("\n# legacy tensor path (HMMA/HGMMA) instructions: %d" % legacy)
+    legacy = sum(v for k, v in tot.items() if k.startswith("HMMA"))
+    print("\n# warp-level tensor path (HMMA) instructions: %d" % legacy)
 
 
 if __name__ == "__main__":

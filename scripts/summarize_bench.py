@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Print the numbers of bench.py JSON lines the results table quotes:  python scripts/summarize_bench.py <json> [...]"""
+"""Print the headline numbers of bench.py JSON lines:  python scripts/summarize_bench.py <json> [...]"""
 import json
 import sys
 

@@ -1,7 +1,7 @@
-"""shifu-tensorflow_b200: B200-native tabular-DNN train / score hot path behind shifu-tensorflow's plug-in seams.
+"""shifu-tensorflow_b200: H100-native tabular-DNN train / score hot path behind shifu-tensorflow's plug-in seams.
 
 Only what the path needs lives here:
-  csrc/        CUDA kernels (sm_100a: tcgen05 / TMEM / TMA) + the C-ABI (include/shifu_b200.h)
+  csrc/        CUDA kernels (sm_90a: wgmma / TMA / mbarrier) + the C-ABI (include/shifu_b200.h)
   _capi.py     ctypes binding of that C-ABI
   trainer.py   host mirror of the reference worker script (ssgd_monitor.py): env-var contract, ModelConfig.json,
                load_data, batch schedule, metrics socket line, SavedModel export

@@ -577,7 +577,7 @@ def savedmodel_read(saved_model_dir: str, input_name: str, output_name: str, tag
 
 def debug_gemm_bf16(A: np.ndarray, B: np.ndarray, split_k: int = 1, device: int = 0, a_mn: bool = False,
                     b_mn: bool = False, cg: int = 0, bn: int = 0) -> np.ndarray:
-    """D[M,N] = sum_k A(m,k) B(n,k) through the tcgen05 kernel (operands rounded to bf16 on the device).
+    """D[M,N] = sum_k A(m,k) B(n,k) through the wgmma kernel (operands rounded to bf16 on the device).
     A is [M,K] (K-major) or, with a_mn, [K,M] (MN-major); B is [N,K] or, with b_mn, [K,N]."""
     A, B = _f32(A), _f32(B)
     (K, M) = A.shape if a_mn else A.shape[::-1]
@@ -589,7 +589,7 @@ def debug_gemm_bf16(A: np.ndarray, B: np.ndarray, split_k: int = 1, device: int 
 
 
 def debug_gemm_split(A: np.ndarray, B: np.ndarray, np_parts: int, device: int = 0) -> np.ndarray:
-    """D[M,N] = A[M,K] B[N,K]^T on the tcgen05 path with every fp32 value split into np_parts bf16 parts"""
+    """D[M,N] = A[M,K] B[N,K]^T on the wgmma path with every fp32 value split into np_parts bf16 parts"""
     A, B = _f32(A), _f32(B)
     M, K = A.shape
     N, K2 = B.shape

@@ -1,4 +1,4 @@
-"""Build libshifu_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libshifu_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python shifu-tensorflow_b200/build.py [--force]
 
@@ -17,7 +17,7 @@ LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libshifu_b200.so")
 SOURCES = ["net.cu", "capi.cu", "text_ingest.cu", "savedmodel.cpp"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function",
 ]
 
@@ -61,7 +61,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         if p.returncode != 0:
             raise RuntimeError("nvcc failed on %s:\n%s" % (src, out))
     tmp = LIB + ".tmp.%d" % os.getpid()      # link beside the target and rename: a snapshot never sees a half-written library
-    cmd = [nvcc, "-shared", "-o", tmp] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart_static", "-ldl", "-lpthread", "-lrt"]
+    cmd = [nvcc, "-shared", "-o", tmp] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart_static", "-ldl", "-lpthread", "-lrt"]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n" + r.stdout)

@@ -77,7 +77,7 @@ struct sb_trainer {
   cudaEvent_t ev_copied[2] = {nullptr, nullptr}, ev_consumed[2] = {nullptr, nullptr};
   unsigned long long async_steps = 0;
   // resident steps: the batch descriptor of step i+1 is written on `prep` while step i still runs (two descriptor /
-  // scalar pairs, one captured graph per pair), so set_batch_kernel leaves the critical path (-2.9 us per cfg1 step)
+  // scalar pairs, one captured graph per pair), so set_batch_kernel leaves the critical path
   BatchDesc* descs[2] = {nullptr, nullptr};
   float* scals[2] = {nullptr, nullptr};
   cudaStream_t prep = nullptr;
@@ -179,18 +179,19 @@ static int enqueue_xchg(sb_trainer* t, int slot_mask, cudaStream_t st, bool publ
     }
   const int U = t->world <= 2 ? 2 : 1;      // runs per block iteration of the update phase (xchg_update_kernel)
   const int want = std::max((runs + U - 1) / U, (all_runs - runs + 3) / 4);   // ... and 4 per iteration of the gather phase
-  // one block per SM and launch: it fits beside a forward GEMM CTA, and two launches fit beside a dW GEMM CTA (xchg_p2p.cuh;
-  // with two blocks per SM the chunk exchanges crowded dW_1 out: 15 -> 27 us, measured).  Blocks that find no room wait for
-  // GEMM CTAs to leave - those never wait for an exchange, so this cannot deadlock, only be slow.
+  // one block per SM and launch.  A GEMM CTA takes a whole SM (registers and shared memory, gemm_tc.cuh), so exchange
+  // blocks run only on SMs no GEMM CTA holds and otherwise wait for GEMM CTAs to leave - those never wait for an exchange,
+  // so this cannot deadlock, only be slow.  The schedule below was tuned where an exchange block fitted beside a GEMM CTA;
+  // on H100 it has not been measured with more than one GPU.
   // (alone: nothing but other exchange launches runs beside this one - two blocks per SM, all loads of a phase in one round)
   int grid = t->xchg_blocks > 0 ? t->xchg_blocks : (alone ? 2 : 1) * n.num_sms;
   if (t->peers_share_device && grid > 32) grid = 32;    // replicas on ONE device: leave registers to the replica being waited for
   if (grid > want) grid = want;
   if (grid < 1) grid = 1;
   const dim3 g(static_cast<unsigned>(grid)), b(256);
-  // SB_XCHG_LL = all (default) | last | none: which launches use the LL protocol (flags inside the data).  Measured on 2 x B200,
-  // cfg2: all 163.8 us/step, last (only the launch nothing runs beside) 168.2, none 171.4; an LL launch takes 21-28 us where
-  // the flag-and-pull kernel takes 32-47, at the price of 2-4 us on the GEMM beside it (polling, doubled store traffic).
+  // SB_XCHG_LL = all (default) | last | none: which launches use the LL protocol (flags inside the data).  An LL launch needs
+  // fewer round trips than the flag-and-pull kernel, at the price of polling and doubled store traffic beside the GEMM it
+  // runs with; "last" keeps it for the launch nothing runs beside.
   static const int ll_mode = [] {
     const char* e = getenv("SB_XCHG_LL");
     if (e == nullptr) return 2;
@@ -260,8 +261,8 @@ static int enqueue_step_body(sb_trainer* t, int rows, int kind, bool resident = 
   static const bool one_xchg = getenv("SB_XCHG_ONE") != nullptr;    // experiment: one exchange launch for everything after a join
   const bool split_tail = !old_sched && kind == G_STEP && (t->world == 1 || (t->p2p_ready && !one_xchg)) && !pipelined &&
                           n.concurrent_bwd && !n.profiling && n.side != nullptr && n.tc() && n.L > 1;
-  // Peer exchange (world > 1): one exchange launch costs 20-30 us through NVSwitch however little data it moves (fabric latency,
-  // xchg_p2p.cuh) - hidden when a GEMM follows it, exposed in full behind the last GEMM.  Default order ("first"):
+  // Peer exchange (world > 1): one exchange launch costs several fabric round trips however little data it moves (xchg_p2p.cuh)
+  // - hidden when a GEMM follows it, exposed in full behind the last GEMM.  Default order ("first"):
   //   main:  ... dA_1 -> dW_1 -> dW_0 chunk 0 -> dW_0 chunk 1 | wait A, B0, B1 | next step
   //   side:  ... dW_2 ...     A ------------->
   //   comm:                             B0 ---------------->    B1 ------>
@@ -271,7 +272,7 @@ static int enqueue_step_body(sb_trainer* t, int rows, int kind, bool resident = 
   // may read this rank's gradient buffer until then - the buffer is cleared by layer 1's forward GEMM instead of layer 0's.
   const bool xsched = split_tail && t->world > 1;
   // SB_XCHG_ORDER: "first" (default) = dW_1 in front of dW_0: slot A and chunk 0 hide behind dW_0's chunks, the LAST chunk's
-  // exchange runs on an otherwise idle GPU - an exchange kernel beside a GEMM takes 40-47 us, alone ~25 (measured, 2 x B200);
+  // exchange runs on an otherwise idle GPU, where an exchange kernel is faster than beside a GEMM;
   // "last" = dW_1 behind dW_0 as cover for the last chunk, slot A beside the next step's layer-0 forward.
   static const bool order_last_env = getenv("SB_XCHG_ORDER") != nullptr && strcmp(getenv("SB_XCHG_ORDER"), "last") == 0;
   // (replicas that share ONE device - tests - keep the "last" order: with three exchange launches of both replicas waiting
@@ -287,8 +288,8 @@ static int enqueue_step_body(sb_trainer* t, int rows, int kind, bool resident = 
   if (resident) {
     // no load kernel: the batch is read by TMA from the bf16 resident set; set_batch_kernel already published n_nz.
     // The gradient buffer is first written by the last forward layer's epilogue, so with more than one hidden layer the
-    // layer-0 forward GEMM clears it (its epilogue warps idle until their first accumulator completes); a memset node
-    // at the head of the chain cost ~3 us per step.
+    // layer-0 forward GEMM clears it (its producer warpgroup's idle warps, beside the main loop) instead of a memset node
+    // at the head of the chain.
     if (n.L > 1) {
       n.zero_buf = reinterpret_cast<float4*>(t->grad);   // cudaMalloc'ed, padded to xch_n4 float4
       n.zero_n4 = t->xch_n4;
@@ -305,9 +306,8 @@ static int enqueue_step_body(sb_trainer* t, int rows, int kind, bool resident = 
   // flat segment [W_l, b_l] (+ the output layer for l = L-1) is all-reduced and its optimizer update applied on the
   // comm stream while the remaining dA / dW GEMMs still run - the role SyncReplicasOptimizer's accumulator + apply
   // play in the reference (res/ssgd_monitor.py:136-142), without the parameter server.
-  // Measured on 2x B200 (profiles/scaling_r01.md): with NCCL as the exchange, ONE all-reduce of the whole flat gradient
-  // after the backward pass beats per-layer / per-chunk calls (each NCCL launch costs ~20-50 us and its CTAs evict
-  // persistent GEMM CTAs), so the pipelined variant is opt-in (SB_PIPELINE_AR=1).
+  // With NCCL as the exchange, the default is ONE all-reduce of the whole flat gradient after the backward pass: each NCCL
+  // launch has a fixed cost and its CTAs evict persistent GEMM CTAs, so the pipelined variant is opt-in (SB_PIPELINE_AR=1).
   if (pipelined) {
     n.on_layer_grads = [t](int l, cudaStream_t cs, int phase, long long e0, long long e1) -> int {
       Net& nn = t->net;
@@ -335,8 +335,7 @@ static int enqueue_step_body(sb_trainer* t, int rows, int kind, bool resident = 
   cudaStream_t comms[2] = {n.comm2, n.comm};
   if (xsched) {
     // dW_1 leaves the side stream: in front of dW_0 ("first") or behind it ("last").  (SB_XCHG_BESIDE=1 keeps it beside dW_0
-    // like the single-GPU schedule; measured on 2 x B200: the chunks of dW_0 then share the SMs with dW_1 - 31 + 19 us
-    // instead of 18 + 19.)
+    // like the single-GPU schedule, where the chunks of dW_0 share the SMs with dW_1.)
     static const bool beside = getenv("SB_XCHG_BESIDE") != nullptr;
     n.dw0_chunks = t->x_chunks;
     n.dw1_last = !beside && order_last;
@@ -386,7 +385,7 @@ static int enqueue_step_body(sb_trainer* t, int rows, int kind, bool resident = 
     // Deferred (multi-step graphs): the launch goes ON the main stream, as dW_1's programmatic dependent.  It releases ITS
     // dependents at its start, the next step's layer-0 forward GEMM skips its dependency wait (all it needs - B0, B1 - are
     // full dependencies) and so runs beside the exchange; layer 1's forward is a plain in-stream launch behind both.
-    // (As a node on another stream that nothing on the main chain waited for, the graph executor started the exchange 18 us
+    // (As a node on another stream that nothing on the main chain waited for, the graph executor started the exchange well
     // after B1 had ENDED - whichever stream carried it, with or without a waited-for marker kernel in front.)
     const bool a_on_main = defer_A && n.dw1_last && !t->peers_share_device;
     if (t->x_sent & XSEG_A) {
@@ -577,7 +576,7 @@ static int stage_host_batch(sb_trainer* t, const float* X, const float* y, const
 
 extern "C" {
 
-const char* sb_version(void) { return "shifu_b200 0.1 (sm_100a)"; }
+const char* sb_version(void) { return "shifu_b200 0.1 (sm_90a)"; }
 const char* sb_last_error(void) { return last_error_ref().c_str(); }
 
 int sb_device_count(void) {
@@ -586,7 +585,7 @@ int sb_device_count(void) {
   int ok = 0;
   for (int i = 0; i < n; ++i) {
     cudaDeviceProp p;
-    if (cudaGetDeviceProperties(&p, i) == cudaSuccess && p.major == 10) ++ok;
+    if (cudaGetDeviceProperties(&p, i) == cudaSuccess && p.major == 9 && p.minor == 0) ++ok;
   }
   return ok;
 }
@@ -738,7 +737,6 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
       snprintf(buf, sizeof(buf), "%d", nccl_ctas);
       setenv("NCCL_MAX_CTAS", buf, 0);
       n.gemm_sms = n.num_sms - nccl_ctas;
-      n.gemm_sms -= n.gemm_sms & 1;  // CTA pairs
       n.dw_chunk_bytes = 2500000;
       if (const char* e = getenv("SB_DW_CHUNK_BYTES")) n.dw_chunk_bytes = atoll(e);
     }
@@ -1722,7 +1720,7 @@ static int debug_gemm_impl(const float* A, const float* B, float* D, int32_t M, 
   SB_CHECK(cudaGetDeviceCount(&n_dev) == cudaSuccess && n_dev > 0, SB_ERR_CUDA, "no CUDA device available");
   cudaDeviceProp prop;
   SB_CUDA(cudaGetDeviceProperties(&prop, device));
-  SB_CHECK(prop.major == 10, SB_ERR_CUDA, "device is sm_%d%d, need sm_100", prop.major, prop.minor);
+  SB_CHECK(prop.major == 9 && prop.minor == 0, SB_ERR_CUDA, "device is sm_%d%d, need sm_90", prop.major, prop.minor);
   SB_CUDA(cudaSetDevice(device));
   // stored shapes: K-major [R, K]; MN-major [K, R]
   const int a_rows = a_mn ? K : M, a_cols = a_mn ? M : K;
@@ -1776,6 +1774,7 @@ static int debug_gemm_impl(const float* A, const float* B, float* D, int32_t M, 
     else if (!a_mn) s = set_gemm_tc_attrs<EPI_F32, false, true>();
     else s = set_gemm_tc_attrs<EPI_F32, true, true>();
     if (s == SB_OK) s = launch();
+    if (s == SB_OK && iters > 0 && pl.cg != 1) s = set_error(SB_ERR_INVALID, "CTA-pair tiles exist with the fp32 test epilogue only");
     if (s == SB_OK && iters > 0) {
       // benchmark with the REAL epilogue of the layout's use: KM -> forward (bias + relu -> bf16), KK -> dA
       // (act' * , bf16 store, column sums), MM -> dW (fp32 red.add)
@@ -1860,7 +1859,7 @@ int sb_debug_gemm_split(const float* A, const float* B, float* D, int32_t M, int
   SB_CHECK(cudaGetDeviceCount(&n_dev) == cudaSuccess && n_dev > 0, SB_ERR_CUDA, "no CUDA device available");
   cudaDeviceProp prop;
   SB_CUDA(cudaGetDeviceProperties(&prop, device));
-  SB_CHECK(prop.major == 10, SB_ERR_CUDA, "device is sm_%d%d, need sm_100", prop.major, prop.minor);
+  SB_CHECK(prop.major == 9 && prop.minor == 0, SB_ERR_CUDA, "device is sm_%d%d, need sm_90", prop.major, prop.minor);
   SB_CUDA(cudaSetDevice(device));
   const int ld = round_up(K, 8);
   const long long a_ps = static_cast<long long>(M) * ld, b_ps = static_cast<long long>(N) * ld;

@@ -1,10 +1,10 @@
-// tcgen05 / TMEM / TMA dense-layer GEMM for sm_100a with fused epilogues.
+// wgmma / TMA dense-layer GEMM for sm_90a with fused epilogues.
 //
-//   D[M,N] = sum_k A(m,k) * B(n,k)      A, B bf16, fp32 accumulation in TMEM
+//   D[M,N] = sum_k A(m,k) * B(n,k)      A, B bf16, fp32 accumulation in registers
 //
 // Each operand is consumed in the layout it already has in HBM - no transposed copies anywhere:
-//   K-major  : element (r,k) at r*ld + k   (row-major [M|N, K]);  TMA box 64(K) x rows, UMMA K-major descriptor
-//   MN-major : element (r,k) at k*ld + r   (row-major [K, M|N]);  TMA boxes 64(MN) x 64(K), UMMA MN-major descriptor
+//   K-major  : element (r,k) at r*ld + k   (row-major [M|N, K]);  TMA box 64(K) x rows, wgmma K-major descriptor
+//   MN-major : element (r,k) at k*ld + r   (row-major [K, M|N]);  TMA boxes 64(MN) x 64(K), wgmma MN-major descriptor
 //
 // One kernel covers every dense contraction of the tabular-DNN step (the TF ops behind nn_layer,
 // res/ssgd_monitor.py:57-71, and their gradients built by opt.minimize, :142):
@@ -15,23 +15,24 @@
 //                                    batch, fp32 red.add into the flat gradient
 //   EPI_F32 : plain fp32 store (kernel-level parity test hook)
 //   EPI_FWD_OUT : last hidden layer of a TRAINING step, output layer fused into the epilogue (K2 + K3 + K4 + output
-//                 backward in one kernel; needs N = h_L <= BN so a CTA holds whole rows of A_L in TMEM):
+//                 backward in one kernel; needs N = h_L <= BN so a CTA holds whole rows of A_L):
 //                 pass 1  a = act(acc + bias), z = a . w_o + b_o, y_hat = sigmoid(z), loss term, d z_hat
-//                 pass 2  (accumulator re-read from TMEM) dZ_L = dz * w_o * act'(a) -> bf16, db_L / dw_o column sums,
-//                         db_o, loss sum.  A_L itself never goes to HBM.
+//                 pass 2  (accumulator staged again from registers) dZ_L = dz * w_o * act'(a) -> bf16, db_L / dw_o column
+//                         sums, db_o, loss sum.  A_L itself never goes to HBM.
 //
-// Two tile configurations (template CG):
-//   CG = 1 : one CTA owns a 128 x BN tile (tcgen05.mma.cta_group::1, M = 128)         - small / narrow problems
-//   CG = 2 : a CTA PAIR (cluster of 2 on one TPC) owns a 256 x BN tile: tcgen05.mma.cta_group::2 with M = 256.
-//            Each CTA stages its own 128 rows of A and HALF of the B tile, so every byte fetched from L2 feeds
-//            twice the MMA work of CG = 1 - the 128x128 single-CTA tile is L2->SM bandwidth bound at ~45 % of the
-//            tensor peak on this part (measured, DESIGN.md), the pair tile is not.
+// Tile: one CTA owns 128 x BN (BN = 64 | 128 | 256).  CG = 2: a cluster of two CTAs owns 256 x BN; both need the same B tile,
+// so each loads half of it and TMA multicasts that half into both CTAs' shared memory (half the B traffic from L2 per CTA).
+// A stage is then refilled only after the consumers of BOTH CTAs have released it (remote mbarrier arrivals).
 //
-// Structure (persistent, one CTA per SM, 320 threads):
-//   warp 0     : TMA producer   - cp.async.bulk.tensor 128B-swizzled tiles into a STAGES-deep smem ring
-//   warp 1     : MMA issuer     - one thread (of the leader CTA when CG = 2) issues tcgen05.mma, commits to mbarriers
-//   warps 2..9 : epilogue       - tcgen05.ld the accumulator (double-buffered in TMEM) and apply the epilogue;
-//                                 two warps per TMEM lane quarter, each taking every other 32-column chunk
+// Structure (persistent, one CTA per SM, 384 threads = three warpgroups):
+//   warps 0..7 : two consumer warpgroups.  Warpgroup g multiplies rows 64 g .. 64 g + 63 of the tile with wgmma.m64nBNk16
+//                (accumulator in registers, one wgmma group in flight while the stage before it is released), then both
+//                run the epilogue.  The epilogue is written thread-owns-row: warp w takes the 32 rows of quarter w & 3 and
+//                every other 32-column chunk (parity w >> 2).  The accumulator reaches that layout through a padded
+//                128 x 64 fp32 block in shared memory, one 64-column block at a time.
+//   warps 8..11: producer warpgroup; one thread issues cp.async.bulk.tensor 128B-swizzled tiles into a STAGES-deep smem
+//                ring and runs ahead into the next tile while the consumers are in the epilogue.  The group gives its
+//                registers to the consumers (setmaxnreg), whose 128 x BN accumulator lives in registers.
 // M/N/K tails need no special code on the load side: TMA zero-fills out-of-bounds box elements.
 #pragma once
 #include <cuda.h>
@@ -70,14 +71,14 @@ struct GemmTcParams {
   int loss;                 // sb_loss
   float *g_wo, *g_bo, *g_bL;  // gradient slots: dw_o [N], db_o [1], db_L [N]
   const BatchDesc* a_rows;  // non-null: operand A lives in the HBM-resident set; add a_rows->row0 to its row coordinate
-  // optional: the epilogue warps clear this buffer (16-byte units) while they wait for their first accumulator.  Used by
-  // the layer-0 forward GEMM of a resident step to clear the step's gradient buffer (no memset node on the chain).
+  // optional: the producer warpgroup's idle warps clear this buffer (16-byte units) beside the main loop.  Used by the
+  // layer-0 forward GEMM of a resident step to clear the step's gradient buffer (no memset node on the chain).
   float4* zero_buf;
   long long zero_n4;
   unsigned long long* trace;  // debug: CTA 0 writes %globaltimer stamps of its pipeline milestones (nullable)
   // Split-precision modes (SB_PREC_FP32_TC / SB_PREC_BF16X2, net.cuh): every fp32 operand value is held as np bf16 PARTS
   // v = p0 + p1 (+ p2) in np equally shaped arrays; the contraction is then a plain bf16 GEMM over an EXTENDED K axis that
-  // walks the part pairs (a_i, b_j) with i + j < np one after the other, all accumulating into the same fp32 TMEM tile:
+  // walks the part pairs (a_i, b_j) with i + j < np one after the other, all accumulating into the same fp32 tile:
   //   np = 2 : a0b0 + a0b1 + a1b0                        (relative error ~2^-17 per product)
   //   np = 3 : a0b0 + a0b1 + a1b0 + a0b2 + a1b1 + a2b0   (~2^-24: fp32-class, what TF-CPU's fp32 GEMM delivers)
   // The MMA issuer does not know about it; the TMA producer picks the pair's tensor maps per k-block.
@@ -116,25 +117,28 @@ struct GemmTcCfg {
   static constexpr int BK = 64;         // 64 bf16 = 128 B = one swizzle row
   static constexpr int BN_CTA = BN / CG;  // B rows staged by one CTA
   static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = BN_CTA * BK * 2;
+  static constexpr int B_BYTES = BN * BK * 2;    // (pair: this CTA's BN_CTA rows and the peer's, multicast)
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  // accumulator staging block: 128 rows x 64 fp32 columns, rows padded by 16 B so that both the fragment stores and the
+  // row-wise 16-byte loads are free of bank conflicts
+  static constexpr int ACC_LD = 64 + 4;
+  static constexpr int ACC_BYTES = BM * ACC_LD * 4;
   // shared memory besides the operand ring: align slack, barriers, epilogue scratch, bias (+ w_o), per-warp transpose tiles
-  // (only the epilogues without TMA staging use them), column-sum accumulators, TMA staging tiles (XB)
+  // (only the epilogues without TMA staging use them), column-sum accumulators, TMA staging tiles (XB), accumulator block
   static constexpr int TR_BYTES = XB > 0 ? 0 : 8 * 2048;
-  static constexpr int FIXED_BYTES = 1024 + 256 + 2048 + 2048 + TR_BYTES + 4096 + XB;
-  static constexpr int RING_BUDGET = (XB > 0 ? 232448 - FIXED_BYTES : 200 * 1024);   // (the un-staged kernels keep their round-1 depth)
+  static constexpr int FIXED_BYTES = 1024 + 256 + 2048 + 2048 + TR_BYTES + 4096 + XB + ACC_BYTES;
+  static constexpr int RING_BUDGET = 232448 - FIXED_BYTES;   // 227 KB of dynamic shared memory per block
   static constexpr int STAGES = RING_BUDGET / STAGE_BYTES > 8 ? 8 : RING_BUDGET / STAGE_BYTES;
-  static constexpr int TMEM_COLS = (2 * BN <= 32) ? 32 : (2 * BN <= 64 ? 64 : (2 * BN <= 128 ? 128 : (2 * BN <= 256 ? 256 : 512)));
+  static_assert(STAGES >= 2, "operand ring");
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED_BYTES;
   static_assert(SMEM_BYTES <= 232448, "shared memory budget");
-  // Epilogue warps.  The dA epilogue (the longest: A_{l-1} tile in, act', column sums, dZ tile out) runs SIXTEEN warps in two
-  // groups of eight that work on alternate 64-column blocks (cfg2 dA_1 19.7 -> 18.8 us, dA_2 7.9 -> 6.8 us; the forward
-  // epilogue gained nothing and keeps eight: 320 threads x <= 115 registers leave room for an exchange block on the same SM,
-  // see xchg_p2p.cuh).
-  static constexpr int EPI_WARPS = XB >= 4 * 16384 ? 16 : 8;
-  static constexpr int EPI_GROUPS = EPI_WARPS / 8;
+  static constexpr int EPI_WARPS = 8;                 // the two consumer warpgroups
   static constexpr int EPI_THREADS = 32 * EPI_WARPS;
-  static constexpr int THREADS = 64 + EPI_THREADS;
+  static constexpr int PRODUCER_WARP = EPI_WARPS;     // first warp of the producer warpgroup
+  static constexpr int THREADS = EPI_THREADS + 128;
+  // per-thread registers after setmaxnreg: 2 x 128 x 232 + 128 x 40 <= 64 K
+  static constexpr int CONSUMER_REGS = 232;
+  static constexpr int PRODUCER_REGS = 40;
 };
 
 // ---- epilogue element functions, specialised per activation so the switch is hoisted out of the element loop
@@ -149,14 +153,13 @@ __device__ __forceinline__ void epi_da_chunk(float (&v)[32], const __nv_bfloat16
   for (int j = 0; j < 32; ++j) v[j] *= act_grad_from_out(__bfloat162float(ah[j]), ACT);
 }
 
-// ACT_T: activation fixed at compile time (EPI_FWD_OUT: its two-pass epilogue with every activation variant inlined was
-// 7.4 k instructions and spent 38 % of its warp samples waiting for instruction fetch, profiles/ncu_r01_*), or
-// SB_ACT_AT_RUNTIME = read p.act.
+// ACT_T: activation fixed at compile time (EPI_FWD_OUT: its two-pass epilogue with every activation variant inlined is
+// several thousand instructions, and instruction fetch then dominates), or SB_ACT_AT_RUNTIME = read p.act.
 constexpr int SB_ACT_AT_RUNTIME = -100;
 
-// GENERIC = false: the plain-bf16 epilogues (performance mode; their instruction footprint decides the epilogue speed - a
-// 7.4 k-instruction epilogue spent 38 % of its issue slots waiting for instruction fetch).  GENERIC = true adds the cold
-// features at compile time: split-precision part stores / loads (np > 1) and the fp32 addend of the wide+deep first layer.
+// GENERIC = false: the plain-bf16 epilogues (performance mode; their instruction footprint decides the epilogue speed).
+// GENERIC = true adds the cold features at compile time: split-precision part stores / loads (np > 1) and the fp32 addend
+// of the wide+deep first layer.
 template <int BN, int EPI, bool A_MN, bool B_MN, int CG, int ACT_T = SB_ACT_AT_RUNTIME, bool GENERIC = false>
 __global__ void __launch_bounds__((GemmTcCfg<BN, CG, epi_tma_bytes(EPI, GENERIC)>::THREADS), 1)
 gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
@@ -168,14 +171,12 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B needs 1024 B alignment
   const uint32_t xbuf_base = smem_base + STAGES * Cfg::STAGE_BYTES;            // TMA staging tiles (1024-byte aligned)
-  const uint32_t bar_base = xbuf_base + epi_tma_bytes(EPI, GENERIC);
-  // barrier layout (8 B each): full[STAGES], empty[STAGES], tmem_full[2], tmem_empty[2], then tmem base slot.
-  // CG = 2: full[] and tmem_empty[] are only used in the leader CTA (rank 0); empty[] / tmem_full[] in both.
+  const uint32_t accs_base = xbuf_base + epi_tma_bytes(EPI, GENERIC);          // accumulator staging block
+  const uint32_t bar_base = accs_base + Cfg::ACC_BYTES;
+  // barrier layout (8 B each): full[STAGES], empty[STAGES]; then scratch (EPI_FWD_OUT partial dot products / dA TMA barriers)
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
+  const uint32_t scratch = bar_base + 8u * (2 * STAGES) + 16u;
   auto smem_a = [&](int s) { return smem_base + s * Cfg::STAGE_BYTES; };
   auto smem_b = [&](int s) { return smem_base + s * Cfg::STAGE_BYTES + Cfg::A_BYTES; };
 
@@ -184,38 +185,21 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
   const bool tracing = p.trace != nullptr && blockIdx.x == 0;
   auto stamp = [&](int slot) { if (tracing) p.trace[slot] = globaltimer_ns(); };
   if (threadIdx.x == 0) stamp(0);  // kernel entry
-  const uint32_t rank = (CG == 2) ? cluster_ctarank() : 0u;  // CTA rank inside the pair
-  const bool leader = rank == 0;
 
   const int n_pairs = p.n_pairs > 0 ? p.n_pairs : 1;
-  if (warp == 0 && lane == 0) {
+  if (warp == Cfg::PRODUCER_WARP && lane == 0) {
     tma_prefetch_desc(&tms.a[0]);
     tma_prefetch_desc(&tms.b[0]);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), CG);  // CG = 2: leader producer's arrive.expect_tx + peer producer's remote arrive
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), Cfg::EPI_WARPS * CG);  // one arrival per epilogue warp (of both CTAs)
+      mbar_init(full_bar(s), 1);   // the producer's arrive.expect_tx
+      mbar_init(empty_bar(s), 2 * CG);  // one arrival per consumer warpgroup (of both CTAs of a pair)
     }
     fence_barrier_init();
   }
-  __syncwarp();
-  if constexpr (CG == 2) cluster_sync_all();  // both CTAs alive before the pair-wide TMEM allocation
-  if (warp == 2) {
-    if constexpr (CG == 2) tmem_alloc_cg2<Cfg::TMEM_COLS>(tmem_slot);
-    else tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  }
-  tcgen05_fence_before();
-  if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
-  tcgen05_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
-  // PDL: everything above (barrier init, TMEM allocation, descriptor prefetch) overlapped the previous kernel's tail;
-  // from here on global memory written by it is touched.
+  const uint32_t rank = (CG == 2) ? cluster_ctarank() : 0u;  // CTA rank inside the pair
+  if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();   // (pair: the peer's barriers exist before any multicast)
+  // PDL: everything above (barrier init, descriptor prefetch) overlapped the previous kernel's tail; from here on global
+  // memory written by it is touched.
   if (threadIdx.x == 0) stamp(1);  // setup done
   if (!p.no_dep_wait) pdl_wait();
   pdl_launch_dependents();
@@ -227,12 +211,13 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
   const int n_work = n_tiles * p.split_k;
   const int part_kb = (p.K + BK - 1) / BK;         // k-blocks of ONE part pair
   const int total_kb = part_kb * n_pairs;          // extended K axis: the pairs one after the other
-  const int w_first = (CG == 2) ? (blockIdx.x >> 1) : blockIdx.x;   // work items are per CTA (CG=1) or per pair (CG=2)
-  const int w_step = (CG == 2) ? (gridDim.x >> 1) : gridDim.x;
+  const int w_first = blockIdx.x / CG;             // work items are per CTA (CG = 1) or per pair (CG = 2)
+  const int w_step = gridDim.x / CG;
 
-  if (warp == 0) {
-    // ================= TMA producer (every CTA) =================
-    if (lane == 0) {
+  if (warp >= Cfg::PRODUCER_WARP) {
+    // ================= TMA producer =================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::PRODUCER_REGS));
+    if (warp == Cfg::PRODUCER_WARP && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       const int a_row0 = (p.a_rows != nullptr) ? p.a_rows->row0 : 0;  // batch position inside the resident set
@@ -250,11 +235,8 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
           const CUtensorMap* tmB = &tms.b[n_pairs > 1 ? p.pair_b[pp] : 0];
           mbar_wait(empty_bar(stage), phase ^ 1);
           const uint32_t fb = full_bar(stage);
-          if (leader) mbar_arrive_expect_tx(fb, Cfg::STAGE_BYTES * CG);
-          auto load = [&](uint32_t dst, const CUtensorMap* tm_, int c0, int c1) {
-            if constexpr (CG == 2) tma_load_2d_cg2(dst, tm_, fb, c0, c1);
-            else tma_load_2d(dst, tm_, fb, c0, c1);
-          };
+          mbar_arrive_expect_tx(fb, Cfg::STAGE_BYTES);
+          auto load = [&](uint32_t dst, const CUtensorMap* tm_, int c0, int c1) { tma_load_2d(dst, tm_, fb, c0, c1); };
           if constexpr (A_MN) {
 #pragma unroll
             for (int i = 0; i < BM / 64; ++i)  // 64(MN) x 64(K) boxes, 8 KB each, side by side along MN
@@ -262,92 +244,56 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
           } else {
             load(smem_a(stage), tmA, kb * BK, m0 + a_row0);
           }
-          if constexpr (B_MN) {
+          if constexpr (CG == 2) {   // this CTA's half of the B tile, into both CTAs
+            if constexpr (B_MN) {
+#pragma unroll
+              for (int j = 0; j < BN_CTA / 64; ++j)
+                tma_load_2d_mc(smem_b(stage) + (rank * (BN_CTA / 64) + j) * 8192, tmB, fb, n0 + j * 64, kb * BK, 3);
+            } else {
+              tma_load_2d_mc(smem_b(stage) + rank * BN_CTA * 128, tmB, fb, kb * BK, n0, 3);
+            }
+          } else if constexpr (B_MN) {
 #pragma unroll
             for (int i = 0; i < BN_CTA / 64; ++i)
               load(smem_b(stage) + i * 8192, tmB, n0 + i * 64, kb * BK);
           } else {
             load(smem_b(stage), tmB, kb * BK, n0);
           }
-          if constexpr (CG == 2) {
-            if (!leader) mbar_arrive_cluster(fb, 0);  // second arrival on the leader's full barrier
-          }
           if (kbx == kb0 && w == w_first) stamp(3);  // first TMA issued
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
-    __syncwarp();   // the whole warp reaches the final block barrier together (bar.sync counts warps, not lanes)
-  } else if (warp == 1) {
-    // ================= MMA issuer (leader CTA only when CG = 2) =================
-    if (lane == 0 && leader) {
-      constexpr uint32_t idesc = make_idesc_bf16(TILE_M, BN, A_MN ? 1u : 0u, B_MN ? 1u : 0u);
-      // descriptor step for 16 elements along K: K-major = 32 B inside the swizzle row; MN-major = 16 rows of 128 B
-      constexpr uint32_t a_kstep = A_MN ? (2048u >> 4) : (32u >> 4);
-      constexpr uint32_t b_kstep = B_MN ? (2048u >> 4) : (32u >> 4);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int w = w_first; w < n_work; w += w_step, ++it) {
-        const int ks = w / n_tiles;
-        const int kb0 = ks * p.kb_per_split;
-        const int kb1 = min(total_kb, kb0 + p.kb_per_split);
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1);  // epilogue(s) have drained this accumulator
-        tcgen05_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * BN;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(full_bar(stage), phase);  // TMA bytes of both CTAs have landed
-          tcgen05_fence_after();
-          if (kb == kb0 && w == w_first) stamp(4);  // first stage landed
-          const uint64_t da = A_MN ? make_mnmajor_sw128_desc(smem_a(stage), 8192u) : make_kmajor_sw128_desc(smem_a(stage));
-          const uint64_t db = B_MN ? make_mnmajor_sw128_desc(smem_b(stage), 8192u) : make_kmajor_sw128_desc(smem_b(stage));
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint32_t accumulate = (kb > kb0 || k > 0) ? 1u : 0u;
-            if constexpr (CG == 2) umma_bf16_cg2(tmem_d, da + a_kstep * k, db + b_kstep * k, idesc, accumulate);
-            else umma_bf16(tmem_d, da + a_kstep * k, db + b_kstep * k, idesc, accumulate);
-          }
-          // frees the smem slot (in both CTAs) once these MMAs have read it
-          if constexpr (CG == 2) umma_commit_cg2(empty_bar(stage)); else umma_commit(empty_bar(stage));
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        // accumulator complete -> epilogue (of both CTAs)
-        if constexpr (CG == 2) umma_commit_cg2(tfull_bar(acc)); else umma_commit(tfull_bar(acc));
-        if (w == w_first) stamp(5);  // all MMAs of the first tile issued
-      }
-    }
-    __syncwarp();
-  } else {
-    // ================= epilogue warps (2..9), every CTA: its own 128 rows x BN columns =================
-    const int quarter = warp & 3;        // TMEM lane quarter this warp may access
-    const int half = ((warp - 2) >> 2) & 1;    // which of the two warps (of a group) sharing the quarter
-    const int grp = (warp - 2) >> 3;           // TMA-staged epilogues: group 0 / 1 takes the even / odd 64-column blocks
-    const int et = static_cast<int>(threadIdx.x) - 64;   // 0 .. EPI_THREADS-1 over all epilogue warps
-    constexpr int ET = Cfg::EPI_THREADS;
-    constexpr int NGRP = Cfg::EPI_GROUPS;
-    auto bar_all = [&]() { asm volatile("bar.sync 1, %0;" ::"n"(Cfg::EPI_THREADS) : "memory"); };    // every epilogue warp
-    auto bar_grp = [&]() { asm volatile("bar.sync %0, 256;" ::"r"(2 + grp) : "memory"); };              // the eight warps of a group
-    if (p.zero_buf != nullptr) {
-      // idle time before the first accumulator completes: clear the step's gradient buffer (read by nobody before the
-      // next kernel boundary)
+    if (warp > Cfg::PRODUCER_WARP && p.zero_buf != nullptr) {
+      // the producer warpgroup's other three warps clear the step's gradient buffer beside the main loop (read by nobody
+      // before the next kernel boundary)
       const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (long long i = static_cast<long long>(blockIdx.x) * ET + et; i < p.zero_n4; i += static_cast<long long>(gridDim.x) * ET) p.zero_buf[i] = z4;
+      const long long zt = static_cast<long long>(threadIdx.x) - 32 * (Cfg::PRODUCER_WARP + 1), zn = 32 * 3;
+      for (long long i = static_cast<long long>(blockIdx.x) * zn + zt; i < p.zero_n4; i += static_cast<long long>(gridDim.x) * zn)
+        p.zero_buf[i] = z4;
     }
-    // EPI_FWD_OUT: bias and w_o of the (single) n-tile staged in shared memory once, before the accumulator wait, so the
-    // two epilogue passes read them with broadcast ld.shared instead of dependent global loads
-    const uint32_t sm_vec = bar_base + 8u * (2 * STAGES + 4) + 16u + 2048u;   // [bias BN floats][w_o BN floats]
-    // Coalescing: tcgen05.ld hands thread t the 32 columns of ROW t, so a direct 16-byte access per thread touches 32
+    __syncwarp();   // the whole warp reaches the final block barrier together (bar.sync counts warps, not lanes)
+  } else {
+    // ================= consumer warpgroups (warps 0..7): MMA, then the epilogue of the tile =================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::CONSUMER_REGS));
+    const int wg = warp >> 2;                  // MMA: rows 64 wg .. 64 wg + 63 of the tile
+    const int quarter = warp & 3;              // epilogue: rows 32 quarter .. 32 quarter + 31 of the tile
+    const int half = (warp >> 2) & 1;          // epilogue: which of the two warps sharing the quarter (chunk parity)
+    const int et = static_cast<int>(threadIdx.x);   // 0 .. EPI_THREADS-1 over all consumer warps
+    constexpr int ET = Cfg::EPI_THREADS;
+    auto bar_all = [&]() { asm volatile("bar.sync 1, %0;" ::"n"(Cfg::EPI_THREADS) : "memory"); };    // every consumer warp
+    // EPI_FWD_OUT: bias and w_o of the (single) n-tile staged in shared memory once, before the first tile, so the two
+    // epilogue passes read them with broadcast ld.shared instead of dependent global loads
+    const uint32_t sm_vec = scratch + 2048u;   // [bias BN floats][w_o BN floats]
+    // Coalescing: the epilogue hands thread t the 32 columns of ROW t, so a direct 16-byte access per thread touches 32
     // different rows (32 L1 wavefronts per instruction).  Every global access of the epilogue therefore goes through a
     // warp-private 32 x 64 B tile in shared memory (16-byte pieces XOR-swizzled by row pair -> conflict-free on both
     // sides): on the global side lane l handles piece (l & 3) of rows 8 i + (l >> 2), i = 0..3, i.e. four lanes cover
     // 64 contiguous bytes of a row and one instruction touches 8 rows instead of 32.
-    const uint32_t sm_stage = sm_vec + 2048u + static_cast<uint32_t>(warp - 2) * 2048u;
+    const uint32_t sm_stage = sm_vec + 2048u + static_cast<uint32_t>(warp) * 2048u;
     // Column sums (bias gradients; dw_o of the fused output layer) are accumulated per CTA in shared memory and flushed to
-    // the flat gradient ONCE per tile and column: one red.global per column per 128 rows instead of one per 32 rows.  With
-    // one red per warp and chunk, the 8192 x 1024 dA GEMM of cfg2 sent 262 k reds to 32 cache lines and spent 3/4 of its time
-    // waiting for the L2 atomic units (tensor pipe 25 % active, profiles/ncu_r01_cfg2_gemm_full.txt).
+    // the flat gradient ONCE per tile and column: one red.global per column per 128 rows instead of one per 32 rows (with
+    // one red per warp and chunk, the wide dA GEMMs wait on the L2 atomic units).
     // layout: [buffer (tile parity)][array 0: db | array 1: dw_o][BN] floats
     const uint32_t sm_col = sm_vec + 2048u + static_cast<uint32_t>(Cfg::TR_BYTES);
     // TMA-staged epilogue (plain-bf16 forward / dA): the 128 x BN tile leaves in 64-column blocks.  Block k: every thread
@@ -357,13 +303,13 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
     // with the same swizzle.  No ld.shared / st.global per element, no transposes, M / N tails clipped by the tensor map.
     auto xo = [&](int b) { return xbuf_base + static_cast<uint32_t>(b) * 16384u; };
     auto xa = [&](int b) { return xbuf_base + 32768u + static_cast<uint32_t>(b) * 16384u; };
-    auto aux_bar = [&](int b) { return bar_base + 8u * (2 * STAGES + 4) + 16u + 8u * static_cast<uint32_t>(b); };   // (scratch of EPI_FWD_OUT, unused here)
+    auto aux_bar = [&](int b) { return scratch + 8u * static_cast<uint32_t>(b); };   // (scratch of EPI_FWD_OUT, unused here)
     const int rt = quarter * 32 + lane;                                   // row of this thread inside the CTA's 128 rows
     auto piece = [&](int half_, int i) { return static_cast<uint32_t>(rt) * 128u + static_cast<uint32_t>(((half_ * 4 + i) ^ (rt & 7)) << 4); };
-    const bool xthread = (((warp - 2) & 7) == 0 && lane == 0);            // first lane of a group: issues its TMA loads / stores
-    unsigned xblk = 0;                                                    // 64-column blocks processed so far by this GROUP
+    const bool xthread = (warp == 0 && lane == 0);                        // issues the epilogue's TMA loads / stores
+    unsigned xblk = 0;                                                    // 64-column blocks processed so far
     if constexpr (TMA_EPI && EPI == EPI_DA) {
-      if (warp == 2 && lane == 0) { mbar_init(aux_bar(0), 1); mbar_init(aux_bar(1), 1); fence_barrier_init(); }
+      if (warp == 0 && lane == 0) { mbar_init(aux_bar(0), 1); mbar_init(aux_bar(1), 1); fence_barrier_init(); }
       bar_all();
     }
     auto col_slot = [&](int buf, int arr, int j) { return sm_col + static_cast<uint32_t>(((buf * 2 + arr) * BN + j) * 4); };
@@ -424,21 +370,61 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
       }
       bar_all();
     }
+
+    // ---- accumulator: registers of the wgmma fragment, handed to the epilogue one 64-column block at a time
+    float acc[BN / 2];
+    // write columns 64 j .. 64 j + 63 of the fragment to the staging block (every consumer warp calls this together; the
+    // first barrier waits for the readers of the previous block).  j selects among unrolled copies so that acc[] stays in
+    // registers.
+    auto stage_block = [&](int j) {
+      bar_all();
+      const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+      for (int jj = 0; jj < BN / 64; ++jj) {
+        if (jj == j) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int n8 = jj * 8 + i;
+            const uint32_t col = static_cast<uint32_t>(8 * i + 2 * (lane & 3));
+            const uint32_t a0 = accs_base + (static_cast<uint32_t>(r0) * Cfg::ACC_LD + col) * 4u;
+            const uint32_t a1 = a0 + 8u * Cfg::ACC_LD * 4u;
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a0), "f"(acc[4 * n8]), "f"(acc[4 * n8 + 1]) : "memory");
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a1), "f"(acc[4 * n8 + 2]), "f"(acc[4 * n8 + 3]) : "memory");
+          }
+        }
+      }
+      bar_all();
+    };
+    // chunk c (32 columns; its block c / 2 is staged): row rt of this thread
+    auto acc_ld = [&](int c, uint32_t (&raw)[32]) {
+      const uint32_t a = accs_base + (static_cast<uint32_t>(rt) * Cfg::ACC_LD + static_cast<uint32_t>((c & 1) * 32)) * 4u;
+#pragma unroll
+      for (int q = 0; q < 8; ++q)
+        asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
+                     : "=r"(raw[4 * q]), "=r"(raw[4 * q + 1]), "=r"(raw[4 * q + 2]), "=r"(raw[4 * q + 3])
+                     : "r"(a + 16u * q) : "memory");
+    };
+
+    // descriptor step for 16 elements along K: K-major = 32 B inside the swizzle row; MN-major = 16 rows of 128 B
+    constexpr uint32_t a_kstep = A_MN ? (2048u >> 4) : (32u >> 4);
+    constexpr uint32_t b_kstep = B_MN ? (2048u >> 4) : (32u >> 4);
+    // this warpgroup's 64 rows of the A stage: K-major = 64 rows of 128 B further; MN-major = the second 64-wide MN atom
+    const uint32_t a_wg_off = static_cast<uint32_t>(wg) * 8192u;
+    int stage = 0;
+    uint32_t phase = 0;
     int it = 0;
     for (int w = w_first; w < n_work; w += w_step, ++it) {
-      const int tile = w % n_tiles;
+      const int tile = w % n_tiles, ks = w / n_tiles;
       const int tm = tile / tiles_n, tn = tile % tiles_n;
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
+      const int kb0 = ks * p.kb_per_split;
+      const int kb1 = min(total_kb, kb0 + p.kb_per_split);
       const int row = tm * TILE_M + static_cast<int>(rank) * BM + quarter * 32 + lane;  // output row of this thread
       const bool row_ok = row < p.M;
-      // operands of the epilogue that do not depend on the accumulator are fetched BEFORE waiting for it (the epilogue
-      // warps idle during the main loop): per-row label / weight / n_nz / b_o of the fused output layer, and the first
-      // chunk of A_{l-1} of the dA epilogue (the next chunk's is fetched while the current one is processed)
+      // operands of the epilogue that do not depend on the accumulator are fetched BEFORE the main loop: per-row label /
+      // weight / n_nz / b_o of the fused output layer, and the A_{l-1} tiles of the dA epilogue
       float pre_y = 0.f, pre_w = 0.f, pre_nnz = 0.f, pre_bo = 0.f;
-      // dA epilogue: A_{l-1} of EVERY chunk this warp will handle is fetched before the accumulator wait (the loads do not
-      // depend on it) and kept in registers as a shift queue, so that one L2 / HBM latency is paid per tile instead of one
-      // per 32-column chunk (the chunk-ahead prefetch left this epilogue latency bound: 5 us per 256 x 256 tile at cfg2)
+      // dA epilogue without TMA staging: A_{l-1} of EVERY chunk this warp will handle is fetched before the main loop and
+      // kept in registers as a shift queue, so that one L2 / HBM latency is paid per tile instead of one per chunk
       constexpr int AUXQ = (EPI == EPI_DA && !TMA_EPI) ? (BN / 64 > 0 ? BN / 64 : 1) : 1;
       uint4 aux_q[AUXQ][4];
       const int row_base = tm * TILE_M + static_cast<int>(rank) * BM + quarter * 32;   // first row of this warp's 32
@@ -504,18 +490,11 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
       const int nblk = (tile_cols + 63) / 64;
       const int x_row0 = tm * TILE_M + static_cast<int>(rank) * BM;      // TMA row coordinate of this CTA's 128 rows
       if constexpr (TMA_EPI && EPI == EPI_DA) {
-        if constexpr (NGRP == 2) {
-          if (xthread && grp < nblk) {       // A_{l-1} of this group's first block (its buffer is free: the group has left the previous tile)
-            mbar_arrive_expect_tx(aux_bar(grp), 16384u);
-            tma_load_2d(xa(grp), &tms.x, aux_bar(grp), tn * BN + grp * 64, x_row0);
-          }
-        } else {
-          if (xthread) {
-            for (int k = 0; k < 2 && k < nblk; ++k) {       // A_{l-1} of the first two blocks (buffers free: every warp has left the previous tile)
-              const int b = (xblk + k) & 1;
-              mbar_arrive_expect_tx(aux_bar(b), 16384u);
-              tma_load_2d(xa(b), &tms.x, aux_bar(b), tn * BN + k * 64, x_row0);
-            }
+        if (xthread) {
+          for (int k = 0; k < 2 && k < nblk; ++k) {       // A_{l-1} of the first two blocks (buffers free: every warp has left the previous tile)
+            const int b = (xblk + k) & 1;
+            mbar_arrive_expect_tx(aux_bar(b), 16384u);
+            tma_load_2d(xa(b), &tms.x, aux_bar(b), tn * BN + k * 64, x_row0);
           }
         }
       }
@@ -530,12 +509,39 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
         }
         bar_all();
       }
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tcgen05_fence_after();
-      if (w == w_first && warp == 2 && lane == 0) stamp(6);  // first accumulator complete
+
+      // ---------- main loop: wgmma over the k-blocks of this work item ----------
+      // one arrival per warpgroup on the stage's empty barrier - in both CTAs of a pair, whose producers both fill it
+      auto release = [&](int s_) {
+        if ((warp & 3) == 0 && lane == 0) {
+          mbar_arrive(empty_bar(s_));
+          if constexpr (CG == 2) mbar_arrive_cluster(empty_bar(s_), rank ^ 1u);
+        }
+      };
+      int prev_stage = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(full_bar(stage), phase);  // the stage's TMA bytes have landed
+        if (kb == kb0 && w == w_first && threadIdx.x == 0) stamp(4);  // first stage landed
+        const uint32_t sa = smem_a(stage) + a_wg_off, sbb = smem_b(stage);
+        const uint64_t da = A_MN ? make_mnmajor_sw128_desc(sa, 8192u) : make_kmajor_sw128_desc(sa);
+        const uint64_t db = B_MN ? make_mnmajor_sw128_desc(sbb, 8192u) : make_kmajor_sw128_desc(sbb);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)
+          wgmma_bf16<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da + a_kstep * k, db + b_kstep * k, (kb > kb0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous k-block's wgmma group has finished reading its stage
+        if (prev_stage >= 0) release(prev_stage);
+        prev_stage = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if (prev_stage >= 0) release(prev_stage);
+      if (w == w_first && threadIdx.x == 0) { stamp(5); stamp(6); }  // first tile's accumulator complete
+
       if constexpr (EPI == EPI_FWD_OUT) {
-        // ---------- fused output layer (tiles_n == 1: this CTA's TMEM holds complete rows of A_L) ----------
-        const uint32_t zs = bar_base + 8u * (2 * STAGES + 4) + 16u + static_cast<uint32_t>(it & 1) * 1024u;  // zpart[2][128]
+        // ---------- fused output layer (tiles_n == 1: this CTA's accumulator holds complete rows of A_L) ----------
+        const uint32_t zs = scratch + static_cast<uint32_t>(it & 1) * 1024u;  // zpart[2][128]
         const int rl = quarter * 32 + lane;
         // 32 consecutive fp32 of the staged bias (which = 0) / w_o (which = 1): 8 broadcast 16-byte ld.shared
         auto load_vec32 = [&](int which, int col0, float (&o)[32]) {
@@ -549,8 +555,7 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
         auto load_act = [&](int c, float (&v)[32]) {   // a = act(acc + bias) for chunk c; 0 beyond N
           const int col0 = c * 32;
           uint32_t raw[32];
-          tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN + c * 32, raw);
-          tmem_ld_wait();
+          acc_ld(c, raw);
           float b[32];
           load_vec32(0, col0, b);
 #pragma unroll
@@ -571,8 +576,9 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
         // pass 1: partial dot product of this thread's row with w_o over this warp's chunks
         float zp = 0.f;
 #pragma unroll 1
-        for (int c = half; c < BN / 32; c += 2) {
-          if (c * 32 >= p.N) break;
+        for (int c = half; (c >> 1) < nblk; c += 2) {
+          stage_block(c >> 1);
+          if (c * 32 >= p.N) continue;
           float v[32], wv[32];
           load_act(c, v);
           load_vec32(1, c * 32, wv);
@@ -580,7 +586,7 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
           for (int j = 0; j < 32; ++j) zp = fmaf(v[j], wv[j], zp);
         }
         asm volatile("st.shared.f32 [%0], %1;" ::"r"(zs + static_cast<uint32_t>(half * 128 + rl) * 4u), "f"(zp) : "memory");
-        asm volatile("bar.sync 1, 256;" ::: "memory");   // the 8 epilogue warps only
+        bar_all();
         float z0, z1;
         asm volatile("ld.shared.f32 %0, [%1];" : "=f"(z0) : "r"(zs + static_cast<uint32_t>(rl) * 4u) : "memory");
         asm volatile("ld.shared.f32 %0, [%1];" : "=f"(z1) : "r"(zs + static_cast<uint32_t>(128 + rl) * 4u) : "memory");
@@ -606,9 +612,10 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
         }
         // pass 2: rank-1 backward of the output layer through act'
 #pragma unroll 1
-        for (int c = half; c < BN / 32; c += 2) {
+        for (int c = half; (c >> 1) < nblk; c += 2) {
+          if (nblk > 1) stage_block(c >> 1);   // (one block: still staged from pass 1)
           const int col0 = c * 32;
-          if (col0 >= p.N) break;
+          if (col0 >= p.N) continue;
           float v[32], g[32];
           load_act(c, v);
           load_vec32(1, col0, g);      // g starts as w_o (0 beyond N)
@@ -629,28 +636,20 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
           red_shared(col_slot(it & 1, 0, col0 + lane), sb_);       // columns beyond N carry zeros
           red_shared(col_slot(it & 1, 1, col0 + lane), sw_);
         }
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if constexpr (CG == 2) mbar_arrive_cluster(tempty_bar(acc), 0);
-          else mbar_arrive(tempty_bar(acc));
-        }
         flush_cols(it, 0, p.g_bL, p.g_wo);
         continue;
       }
 #pragma unroll 1
-      for (int c = TMA_EPI ? 2 * grp + half : half; c < BN / 32; c += (TMA_EPI ? 2 * NGRP : 2)) {
+      for (int c = half; (c >> 1) < nblk; c += 2) {
+        stage_block(c >> 1);
         const int col0 = tn * BN + c * 32;
-        if constexpr (TMA_EPI) {
-          if ((c >> 1) >= nblk) break;          // same trip count for the eight warps of a group
-        } else {
-          if (col0 >= p.N) break;  // whole chunk out of range (warp-uniform)
-        }
         const bool chunk_ok = col0 < p.N;       // (TMA path: a warp whose 32 columns lie beyond N only joins the barriers)
+        if constexpr (!TMA_EPI) {
+          if (!chunk_ok) continue;  // whole chunk out of range (warp-uniform)
+        }
         uint32_t raw[32];
         if (chunk_ok) {
-          tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN + c * 32, raw);
-          tmem_ld_wait();
+          acc_ld(c, raw);
         } else {
 #pragma unroll
           for (int j = 0; j < 32; ++j) raw[j] = 0u;
@@ -659,8 +658,7 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
 #pragma unroll
         for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(raw[j]);
         const bool full = col0 + 32 <= p.N;  // warp-uniform fast path
-        // staging tiles: two groups -> each owns one output and one A_{l-1} tile; one group -> it alternates between two
-        const int xb = NGRP == 2 ? grp : static_cast<int>(xblk & 1u);
+        const int xb = static_cast<int>(xblk & 1u);   // staging tiles: the two alternate
 
         if constexpr (EPI == EPI_FWD) {
           if (GENERIC && p.addend != nullptr && row_ok) {
@@ -677,7 +675,7 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
                 if (col0 + j < p.N) v[j] += __ldg(ad + j);
             }
           }
-          float b[32];   // staged before the accumulator wait (0 beyond N)
+          float b[32];   // staged before the main loop (0 beyond N)
 #pragma unroll
           for (int q = 0; q < 8; ++q)
             asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
@@ -691,10 +689,10 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
             default: epi_fwd_chunk<SB_ACT_NONE>(v, b); break;
           }
         } else if constexpr (EPI == EPI_DA) {
-          // multiply by act'(A_{l-1}[row, col]) read as bf16 (64 B per thread per chunk, fetched one chunk ahead)
+          // multiply by act'(A_{l-1}[row, col]) read as bf16
           uint4 a4[4];
           if constexpr (TMA_EPI) {
-            mbar_wait(aux_bar(xb), (NGRP == 2 ? xblk : (xblk >> 1)) & 1u);   // this block's A_{l-1} tile has landed
+            mbar_wait(aux_bar(xb), (xblk >> 1) & 1u);   // this block's A_{l-1} tile has landed
 #pragma unroll
             for (int i = 0; i < 4; ++i) a4[i] = lds4(xa(xb) + piece(half, i));
           } else {
@@ -747,19 +745,17 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
               o[q].z = pack_bf16x2(v[q * 8 + 4], v[q * 8 + 5]);
               o[q].w = pack_bf16x2(v[q * 8 + 6], v[q * 8 + 7]);
             }
-            if (xthread) {                                         // the last store out of this tile has finished reading it ...
-              if constexpr (NGRP == 2) tma_store_wait_read<0>(); else tma_store_wait_read<1>();
-            }
-            bar_grp();                                             // (B) ... which every warp of the group may now overwrite
+            if (xthread) tma_store_wait_read<1>();                 // the store issued from this tile two blocks ago has read it ...
+            bar_all();                                             // (B) ... so every warp may now overwrite it
 #pragma unroll
             for (int q = 0; q < 4; ++q) sts4(xo(xb) + piece(half, q), o[q]);
             fence_proxy_async();                                   // generic-proxy writes -> visible to the TMA engine
-            bar_grp();                                             // (A) the block's tile is complete; A_{l-1} tile consumed
+            bar_all();                                             // (A) the block's tile is complete; A_{l-1} tile consumed
             if (xthread) {
               tma_store_2d(&tms.o, xo(xb), tn * BN + (c >> 1) * 64, x_row0);
               tma_store_commit();
               if constexpr (EPI == EPI_DA) {
-                if ((c >> 1) + 2 < nblk) {                         // A_{l-1} of the group's next block, into the tile just consumed
+                if ((c >> 1) + 2 < nblk) {                         // A_{l-1} of the block after next, into the tile just consumed
                   mbar_arrive_expect_tx(aux_bar(xb), 16384u);
                   tma_load_2d(xa(xb), &tms.x, aux_bar(xb), tn * BN + ((c >> 1) + 2) * 64, x_row0);
                 }
@@ -818,34 +814,22 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
           }
         }
       }
-      // release the accumulator back to the MMA warp: one arrival per warp on the leader's barrier
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (CG == 2) mbar_arrive_cluster(tempty_bar(acc), 0);
-        else mbar_arrive(tempty_bar(acc));
-      }
       if constexpr (EPI == EPI_DA) {
         if (p.colsum != nullptr) flush_cols(it, tn, p.colsum, nullptr);
       }
-      if (w == w_first && warp == 2 && lane == 0) stamp(7);  // first tile's epilogue done
+      if (w == w_first && threadIdx.x == 0) stamp(7);  // first tile's epilogue done
+    }
+    if constexpr (TMA_EPI) {
+      if (xthread) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // the last tiles are in global memory
     }
   }
 
-  if constexpr (TMA_EPI) {
-    if (warp >= 2 && ((warp - 2) & 7) == 0 && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // the last tiles are in global memory
-  }
-  tcgen05_fence_before();
+  // (pair: no CTA exits while its peer may still multicast into it or arrive on its barriers)
   if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
   if (threadIdx.x == 0) stamp(8);  // all roles finished
   // in-graph kernel span: slot 2 (dependencies resolved, CTA 0) .. slot 10 (latest exit over ALL CTAs; %globaltimer only
   // grows, so atomicMax needs no reset between steps)
   if (p.trace != nullptr && threadIdx.x == 0) atomicMax(p.trace + 10, static_cast<unsigned long long>(globaltimer_ns()));
-  if (warp == 2) {
-    tcgen05_fence_after();
-    if constexpr (CG == 2) tmem_dealloc_cg2<Cfg::TMEM_COLS>(tmem_base);
-    else tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-  }
 }
 
 // ------------------------------------------------------------------ host side
@@ -866,7 +850,7 @@ void set_part_pairs(GemmTcParams* p, int np);
 
 // Tile configuration chosen per problem.
 struct GemmPlan {
-  int cg;            // 1 or 2
+  int cg;            // 1, or 2: a cluster of two CTAs per 256 x bn tile, B multicast
   int bn;            // 64 / 128 / 256
   int split_k, kb_per_split;
   int grid;          // CTAs to launch (a multiple of cg)

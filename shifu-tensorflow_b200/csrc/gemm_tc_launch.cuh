@@ -62,8 +62,6 @@ int launch_gemm_tc(const GemmPlan& pl, const TmapSet& tms, GemmTcParams p, cudaS
       } else {
         if (pl.cg == 1 && pl.bn == 64) return launch_gemm_tc_one<64, EPI, A_MN, B_MN, 1, ACT_G, true>(pl, tms, p, st, pdl);
         if (pl.cg == 1 && pl.bn == 128) return launch_gemm_tc_one<128, EPI, A_MN, B_MN, 1, ACT_G, true>(pl, tms, p, st, pdl);
-        if (pl.cg == 2 && pl.bn == 128) return launch_gemm_tc_one<128, EPI, A_MN, B_MN, 2, ACT_G, true>(pl, tms, p, st, pdl);
-        if (pl.cg == 2 && pl.bn == 256) return launch_gemm_tc_one<256, EPI, A_MN, B_MN, 2, ACT_G, true>(pl, tms, p, st, pdl);
       }
       return set_error(SB_ERR_INVALID, "no generic gemm_tc instantiation for cg=%d bn=%d", pl.cg, pl.bn);
     }
@@ -76,8 +74,10 @@ int launch_gemm_tc(const GemmPlan& pl, const TmapSet& tms, GemmTcParams p, cudaS
   } else {
   if (pl.cg == 1 && pl.bn == 64) return launch_gemm_tc_one<64, EPI, A_MN, B_MN, 1>(pl, tms, p, st, pdl);
   if (pl.cg == 1 && pl.bn == 128) return launch_gemm_tc_one<128, EPI, A_MN, B_MN, 1>(pl, tms, p, st, pdl);
+  if constexpr (EPI == EPI_F32) {   // CTA pairs: the tile-configuration hook's (the planner does not pick them)
   if (pl.cg == 2 && pl.bn == 128) return launch_gemm_tc_one<128, EPI, A_MN, B_MN, 2>(pl, tms, p, st, pdl);
   if (pl.cg == 2 && pl.bn == 256) return launch_gemm_tc_one<256, EPI, A_MN, B_MN, 2>(pl, tms, p, st, pdl);
+  }
   return set_error(SB_ERR_INVALID, "no gemm_tc instantiation for cg=%d bn=%d", pl.cg, pl.bn);
   }
 }
@@ -104,13 +104,14 @@ int set_gemm_tc_attrs() {
 #define SB_ATTR(BN, CG)                                                                                            \
   SB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI, A_MN, B_MN, CG>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
                                (GemmTcCfg<BN, CG, epi_tma_bytes(EPI, false)>::SMEM_BYTES)))
-  SB_ATTR(64, 1); SB_ATTR(128, 1); SB_ATTR(128, 2); SB_ATTR(256, 2);
+  SB_ATTR(64, 1); SB_ATTR(128, 1);
+  if constexpr (EPI == EPI_F32) { SB_ATTR(128, 2); SB_ATTR(256, 2); }
 #undef SB_ATTR
   if constexpr (EPI == EPI_FWD || EPI == EPI_DA) {
 #define SB_ATTR_G(BN, CG)                                                                                            \
   SB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI, A_MN, B_MN, CG, SB_ACT_AT_RUNTIME, true>,                      \
                                cudaFuncAttributeMaxDynamicSharedMemorySize, GemmTcCfg<BN, CG>::SMEM_BYTES))
-    SB_ATTR_G(64, 1); SB_ATTR_G(128, 1); SB_ATTR_G(128, 2); SB_ATTR_G(256, 2);
+    SB_ATTR_G(64, 1); SB_ATTR_G(128, 1);
 #undef SB_ATTR_G
   }
   return SB_OK;

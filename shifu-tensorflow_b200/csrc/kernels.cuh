@@ -253,8 +253,8 @@ out_layer_kernel(const OutLayerParams p) {
 // the block's slice); lane i owns columns [256 c + 8 i, +8) of every 256-column chunk c of every row, moved with 16-byte
 // loads / stores.  Because the lane <-> column mapping is the same for every row, the row's dot product is one xor-shuffle
 // reduction and the dw_o / db_L column sums stay in registers over all rows of the warp; a block reduces them through
-// shared memory and issues ONE atomic per column (the 32-rows-per-block kernel above read A_L twice with 2-byte
-// accesses and took 20 us at cfg2 sizes, scripts/step_timeline.py).
+// shared memory and issues ONE atomic per column (the 32-rows-per-block kernel above reads A_L twice with 2-byte
+// accesses).
 template <int NCH>
 __global__ void __launch_bounds__(256)
 out_layer_rows_kernel(const OutLayerParams p, int rows_per_block) {
@@ -443,7 +443,7 @@ optimizer_kernel(const OptWork* __restrict__ work, const BatchDesc* __restrict__
   pdl_launch_dependents();
   if (trace != nullptr && blockIdx.x == 0 && threadIdx.x == 0) trace[2] = globaltimer_ns();   // dependencies resolved
   // last kernel of a step: publish the step scalars (loss sum, n_nz) straight into mapped pinned host memory - a posted
-  // PCIe write off the critical path instead of a D2H copy node between two steps (measured: -8.7 us per cfg1 step)
+  // PCIe write off the critical path instead of a D2H copy node between two steps
   if (host_scal != nullptr && blockIdx.x == 0 && threadIdx.x < SCAL_COUNT) {
     host_scal[threadIdx.x] = scal[threadIdx.x];
     if (threadIdx.x == 0 && desc->hist != nullptr) *desc->hist = make_float2(scal[SCAL_LOSS_SUM], scal[SCAL_NNZ]);   // loss curve

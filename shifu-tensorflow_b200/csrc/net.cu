@@ -67,37 +67,15 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rows, int cols, int l
   return SB_OK;
 }
 
-// Tile configuration, rules fitted to the on-device sweep in profiles/gemm_sweep_r01.txt (scripts/gemm_sweep.py):
-//   - the single-CTA 128x128 tile is L2->SM bandwidth bound (~46 B/cycle/SM with every SM pulling, i.e. ~45 % of the
-//     tensor peak); the CTA-pair 256x256 tile (cta_group::2) halves the bytes per flop and reaches ~64 %;
-//   - the pair tile only pays when there are enough pair tiles to fill the 74 SM pairs AND the K loop is deep
-//     enough (>= 8 k-blocks per tile) to amortise its larger fill / epilogue;
+// Tile configuration (persistent grid, one CTA per SM, 128 x BN tiles):
+//   - BN = 128 (64 for a layer at most 64 wide).  A 128 x 256 tile would fetch fewer operand bytes per flop, but its
+//     128-register accumulator plus the epilogue does not fit the consumer threads' registers without spills; only the
+//     fused output layer, which needs whole rows, uses it;
+//   - no CTA pairs: the 256 x BN cluster tile with B multicast (cg = 2, gemm_tc.cuh) is the tile-configuration hook's,
+//     instantiated with the fp32 test epilogue only;
 //   - split-K (dW GEMMs, reduction over the batch): fill the machine but keep >= 8 k-blocks per split.
 GemmPlan plan_gemm(int M, int N, int K, int num_sms, bool allow_split) {
   const int total_kb = (K + 63) / 64;
-  GemmPlan pl = {};
-  auto finish = [&](int cg, int bn, int want_split) {
-    const int slots = num_sms / cg;
-    const int tiles = ((M + 128 * cg - 1) / (128 * cg)) * ((N + bn - 1) / bn);
-    if (want_split < 1) want_split = 1;
-    if (want_split > total_kb) want_split = total_kb;
-    pl.cg = cg; pl.bn = bn;
-    pl.kb_per_split = (total_kb + want_split - 1) / want_split;
-    pl.split_k = (total_kb + pl.kb_per_split - 1) / pl.kb_per_split;
-    const int work = tiles * pl.split_k;
-    pl.grid = (work < slots ? work : slots) * cg;
-  };
-  const int pairs = num_sms / 2;
-  const int pair_tiles = ((M + 255) / 256) * ((N + 255) / 256);
-  if (N >= 512 && M >= 512) {
-    if (!allow_split) {
-      if (pair_tiles * 5 >= pairs * 4 && total_kb >= 8) { finish(2, 256, 1); return pl; }
-    } else {
-      int split = pairs / pair_tiles;
-      if (split < 1) split = 1;
-      if (pair_tiles * split * 5 >= pairs * 4 && total_kb / split >= 32) { finish(2, 256, split); return pl; }
-    }
-  }
   const int bn = N <= 64 ? 64 : 128;
   const int tiles = ((M + 127) / 128) * ((N + bn - 1) / bn);
   int split = 1;
@@ -107,7 +85,13 @@ GemmPlan plan_gemm(int M, int N, int K, int num_sms, bool allow_split) {
     if (split > cap) split = cap;
     if (split < 1) split = 1;
   }
-  finish(1, bn, split);
+  if (split > total_kb) split = total_kb;
+  GemmPlan pl = {};
+  pl.cg = 1; pl.bn = bn;
+  pl.kb_per_split = (total_kb + split - 1) / split;
+  pl.split_k = (total_kb + pl.kb_per_split - 1) / pl.kb_per_split;
+  const int work = tiles * pl.split_k;
+  pl.grid = work < num_sms ? work : num_sms;
   return pl;
 }
 
@@ -137,8 +121,8 @@ static int check_device(int device, int* num_sms) {
   SB_CHECK(device >= 0 && device < n, SB_ERR_INVALID, "device %d out of range [0,%d)", device, n);
   cudaDeviceProp prop;
   SB_CUDA(cudaGetDeviceProperties(&prop, device));
-  SB_CHECK(prop.major == 10, SB_ERR_CUDA, "device %d is sm_%d%d; this library is built for sm_100a only", device,
-           prop.major, prop.minor);
+  SB_CHECK(prop.major == 9 && prop.minor == 0, SB_ERR_CUDA, "device %d is sm_%d%d; this library is built for sm_90a only",
+           device, prop.major, prop.minor);
   *num_sms = prop.multiProcessorCount;
   return SB_OK;
 }
@@ -420,8 +404,7 @@ int Net::enqueue_hidden_forward(int rows, float* grad, bool* fused_out) {
         // K2 + K3 + K4 + output backward in one kernel: one n-tile must cover the whole layer width
         GemmPlan fp = pl;
         fp.split_k = 1; fp.kb_per_split = ((k_in + 63) / 64) * pairs_of(nparts);
-        // (a 256-wide PAIR tile measured slower than GEMM + out_layer kernel in round 1; the single-CTA 128 x 256 tile keeps
-        // whole rows of A_L in one CTA's TMEM - 2 x 256 columns, double-buffered - and needs no second kernel)
+        // (the 128 x 256 tile keeps whole rows of A_L in one CTA's accumulator and needs no second kernel)
         if (ly.out <= 64) { fp.cg = 1; fp.bn = 64; }
         else if (ly.out <= 128) { fp.cg = 1; fp.bn = 128; }
         else { fp.cg = 1; fp.bn = 256; }
@@ -509,20 +492,21 @@ int Net::enqueue_backward(int rows, float* grad) {
   // overlap the dA chain (they are each well under one wave at cfg1 sizes).  Not while profiling (clean times).
   const bool fork = concurrent_bwd && !profiling && side != nullptr && tc();
   // dW_1 (side stream) and dW_0 (main stream) run at the same time, one CTA per SM each.  If their natural grids do not
-  // fit the machine together, dW_1's second wave only starts when dW_0's CTAs exit (measured: the side optimizer then
-  // finishes 4 us after the main one, scripts/step_timeline.py).  Compare, in k-blocks per CTA, "natural grids, dW_1
+  // fit the machine together, dW_1's second wave only starts when dW_0's CTAs exit.  Compare, in k-blocks per CTA, "natural grids, dW_1
   // finishing after dW_0" against "dW_1 on a third of the SMs, dW_0 on the rest" and take the shorter.
   int dw_sms[2] = {gemm_sms, gemm_sms};
   static const bool no_budget = getenv("SB_NO_DW_BUDGET") != nullptr;
   // dw1_serial_auto (single-GPU tail): when the natural grids of dW_0 and dW_1 do not fit the machine together, dW_1 runs IN
-  // FRONT of dW_0 on the main stream instead of beside it - side by side the two persistent grids take turns on the SMs
-  // (cfg2: 47.9 us for both; alone 13.9 + 29.0 us, profiles/ncu_r02_cfg2_launches.txt); small layers (cfg1) stay side by side
+  // FRONT of dW_0 on the main stream instead of beside it - side by side the two persistent grids take turns on the SMs;
+  // small layers (cfg1) stay side by side.  Only when dW_0 alone fills every SM: on one H100, cfg2 (dW_0 = 128 tiles on 132
+  // SMs, budget split below) measured within 1 % of both dW_1 in front and the natural grids, while moving dW_1 in front
+  // once dW_0 fills >= 90 % of the SMs made cfg1 4 % slower
   bool dw1_front = dw1_first;
   if (fork && dw0_on_main && L > 1 && !on_layer_grads && !no_budget && !dw1_last && !dw1_first) {
     const int kx = round_up(rows, 64) * pairs_of(nparts);
     const GemmPlan n0 = plan_gemm(layers[0].in, layers[0].out, kx, gemm_sms, true);
     const GemmPlan n1 = plan_gemm(layers[1].in, layers[1].out, kx, gemm_sms, true);
-    if (n0.grid + n1.grid > gemm_sms && dw1_serial_auto && n0.cg == 2) {      // (pair tiles = a GEMM of several waves, plan_gemm)
+    if (n0.grid + n1.grid > gemm_sms && dw1_serial_auto && n0.grid == gemm_sms) {      // (dW_0 alone fills the machine)
       dw1_front = true;
     } else if (n0.grid + n1.grid > gemm_sms) {
       const GemmPlan b1 = plan_gemm(layers[1].in, layers[1].out, kx, gemm_sms / 3, true);
@@ -550,7 +534,7 @@ int Net::enqueue_backward(int rows, float* grad) {
         if (xchg_chunks) n_chunks = dw0_chunks;
         int chunk_rows = xchg_chunks ? dw0_chunk_rows() : round_up((ly.in + n_chunks - 1) / n_chunks, 128);
         // dW_0 has nothing to overlap with (no dA_0): PDL-chained on the main stream right behind the last dA GEMM it
-        // starts ~6 us earlier than as a cross-stream launch (measured, scripts/step_timeline.py)
+        // starts earlier than as a cross-stream launch
         const bool on_main = !fork || (l == 0 && dw0_on_main && L > 1) || force_main;
         if (!on_main) {
           SB_CUDA(cudaEventRecord(ev_dz[l], stream));

@@ -21,7 +21,7 @@ struct Layer {
 };
 
 struct Net {
-  int device = 0, num_sms = 148;
+  int device = 0, num_sms = 132;
   cudaStream_t stream = nullptr;
   cudaStream_t side = nullptr;               // dW GEMMs run here, concurrently with the dA chain on `stream`
   std::vector<cudaEvent_t> ev_dz;            // ev_dz[l]: dZ_l is complete on `stream`

@@ -1,4 +1,4 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM).
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma.
 // No CUTLASS / CuTe dependency: everything the kernels need is spelled out here.
 #pragma once
 #include <cuda_bf16.h>
@@ -76,51 +76,56 @@ __device__ __forceinline__ void tma_store_wait_read() {
   asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// ---------------------------------------------------------------- wgmma (warpgroup MMA, accumulator in registers)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// Whole warp.  Writes the TMEM base address of the allocation to *dst_smem.
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "n"(COLS) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
+// D[64 x N] (+)= A[64 x 16, smem desc] * B[16 x N, smem desc]^T, issued by the four warps of a warpgroup.  TA / TB = 1: the
+// operand tile is MN-major in shared memory (transposed read).  scale_d = 0 overwrites D (first k-step of a tile).
+// Accumulator fragment: warp w of the group, lane l holds for n8 block i: d[4i + 0/1] = row 16 w + l / 4, columns
+// 8 i + 2 (l % 4) + 0/1; d[4i + 2/3] = row + 8, same columns.
+// accumulator operands d[i .. i + 7] of a wgmma asm statement
+#define SB_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+  static_assert(N == 64 || N == 128 || N == 256, "wgmma N");
+  if constexpr (N == 64) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, %35, %36;\n\t}"
+        : SB_F8(0), SB_F8(8), SB_F8(16), SB_F8(24)
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d), "n"(TA), "n"(TB));
+  }
+  if constexpr (N == 128) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, %67, %68;\n\t}"
+        : SB_F8(0), SB_F8(8), SB_F8(16), SB_F8(24), SB_F8(32), SB_F8(40), SB_F8(48), SB_F8(56)
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d), "n"(TA), "n"(TB));
+  }
+  if constexpr (N == 256) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+        "%128, %129, p, 1, 1, %131, %132;\n\t}"
+        : SB_F8(0), SB_F8(8), SB_F8(16), SB_F8(24), SB_F8(32), SB_F8(40), SB_F8(48), SB_F8(56), SB_F8(64), SB_F8(72), SB_F8(80), SB_F8(88), SB_F8(96), SB_F8(104), SB_F8(112), SB_F8(120)
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d), "n"(TA), "n"(TB));
+  }
 }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Make the mbarrier track completion of all prior tcgen05 ops of this thread (implies fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
+#undef SB_F8
 
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp receives row (lane base + i), v[j] = column j.
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---------------------------------------------------------------- CTA pairs (cta_group::2, cluster of 2)
+// ---------------------------------------------------------------- CTA pairs (cluster of 2)
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -139,51 +144,25 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_local, uint32_t
       ::"r"(bar_local), "r"(cta)
       : "memory");
 }
-// 2-CTA TMA load: data lands in THIS CTA's smem, the transaction bytes are signalled on the LEADER CTA's
-// mbarrier (peer bit 24 of the shared::cluster address cleared).
-__device__ __forceinline__ void tma_load_2d_cg2(uint32_t dst_smem, const void* tmap, uint32_t bar, int c0, int c1) {
+// The same load, multicast: the box lands at this smem offset in every CTA of the cluster named in cta_mask, and each of
+// them gets the bytes signalled on its mbarrier at offset `bar`.
+__device__ __forceinline__ void tma_load_2d_mc(uint32_t dst_smem, const void* tmap, uint32_t bar, int c0, int c1, uint16_t cta_mask) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst_smem), "l"(tmap), "r"(bar & 0xFEFFFFFFu), "r"(c0), "r"(c1)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(dst_smem), "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
-}
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_alloc_cg2(uint32_t dst_smem) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "n"(COLS) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_dealloc_cg2(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[256 rows: 128 from each CTA's smem] * B[N: N/2 from each CTA's smem]; leader thread only.
-__device__ __forceinline__ void umma_bf16_cg2(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit + arrive on the mbarrier at this offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit_cg2(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"(static_cast<uint16_t>(3))
-               : "memory");
 }
 
 // ---------------------------------------------------------------- descriptors
 // Shared-memory matrix descriptor for a K-major bf16 operand tile staged by TMA with 128-byte swizzle:
 // rows of 64 bf16 (128 B), 8-row swizzle atoms of 1024 B stacked along M/N (SBO = 1024), LBO unused.
 //   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4   bits [46,48) descriptor version (1 on sm_100)
-//   bits [61,64) layout type (2 = SWIZZLE_128B)
+//   bits [32,46) stride byte offset >> 4   bits [62,64) layout type (1 = SWIZZLE_128B)
 __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
   d |= static_cast<uint64_t>(1024u >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 // MN-major bf16 operand tile (rows of 64 MN-elements = 128 B along MN, stacked along K), 128-byte swizzle.
@@ -194,15 +173,8 @@ __device__ __forceinline__ uint64_t make_mnmajor_sw128_desc(uint32_t smem_addr, 
   d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>(1024u >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
-}
-// Instruction descriptor, kind::f16: D = fp32, A = B = bf16.
-//   [4,6) c_format (1 = F32)  [7,10) a_format (1 = BF16)  [10,13) b_format (1 = BF16)
-//   [15] a_major (0 = K)  [16] b_major (0 = K)  [17,23) N >> 3  [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn_major = 0, uint32_t b_mn_major = 0) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
 }
 
 // ---------------------------------------------------------------- programmatic dependent launch

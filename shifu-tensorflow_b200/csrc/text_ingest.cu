@@ -246,7 +246,7 @@ int sb_device_gather_rows(const float* d_src, int32_t n_cols, const int64_t* row
   cudaError_t e = cudaMemcpy(d_rows, rows_host, sizeof(long long) * static_cast<size_t>(n), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) {
     long long blocks = (n * n_cols + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > 132 * 32) blocks = 132 * 32;
     gather_rows_kernel<<<static_cast<unsigned>(blocks), 256>>>(d_src, n_cols, d_rows, n, d_dst);
     e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaDeviceSynchronize();

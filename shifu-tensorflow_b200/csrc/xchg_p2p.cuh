@@ -135,12 +135,10 @@ __device__ __forceinline__ bool xchg_wait(const unsigned int* slots, int world, 
 }
 
 // W = compile-time upper bound of `world`; a block iteration handles U consecutive runs with every load of the iteration in
-// flight before the first add.  <= 85 registers per thread: one block (21 k registers) fits beside ANY of the
-// persistent GEMM CTAs that may be resident while an exchange runs - the dW GEMMs of the same step (320 threads x 64) and
-// the next step's layer-0 forward (320 x <= 115) - so the exchange really overlaps them.
-// Measured on 2 x B200 through NVSwitch (scripts/p2p_probe.cu, profiles/p2p_probe_r02.txt): a flag takes 2.7 us one way, a
-// P2P load round trip ~5 us, bandwidth 750 GB/s only beyond ~16 MB in flight (4 MB: 14 us).  The chain arrive -> loads ->
-// stores + fence -> done therefore costs ~17 us however little data moves: the schedule (capi.cu) hides it behind GEMMs.
+// flight before the first add.  <= 85 registers per thread (one block = 21 k registers).  A persistent GEMM CTA takes a
+// whole SM (registers and shared memory), so an exchange overlaps a GEMM on the SMs that GEMM's grid leaves free.
+// The chain arrive -> loads -> stores + fence -> done costs several P2P round trips however little data moves: the
+// schedule (capi.cu) hides it behind GEMMs.
 template <int W>
 static __global__ void __launch_bounds__(256, W <= 8 ? 3 : 2)
 xchg_update_kernel(const XchgParams p) {
@@ -180,8 +178,7 @@ xchg_update_kernel(const XchgParams p) {
   if (p.trace != nullptr && blockIdx.x == 0 && threadIdx.x == 0) p.trace[3] = globaltimer_ns();
   // ---- owned runs of every slot of the launch ----
   // (every load of an iteration - the peers' gradients, the local master and state - is issued before the first store, so a
-  // thread pays the fabric round trip once per iteration; the first version interleaved them run by run and took 20 us for
-  // 512 runs beside a GEMM)
+  // thread pays the fabric round trip once per iteration instead of once per run)
   if (alive) {
 #pragma unroll 1
     for (int slot = 0; slot < p.n_slots; ++slot) {
@@ -281,13 +278,13 @@ xchg_update_kernel(const XchgParams p) {
   }
   stamp_max(4);
   // ---- updated: my owned runs carry the new values (local stores only, so this fence does not wait for the fabric) ----
-  // (ONE fence per block, behind the barrier that orders the block's stores before it: a fence per thread serialised the
-  // eight warps' MEMBAR.SYS and took 12-14 us on an SM that shares its memory pipeline with a GEMM CTA)
+  // (ONE fence per block, behind the barrier that orders the block's stores before it: a fence per thread serialises the
+  // eight warps' MEMBAR.SYS)
   __syncthreads();
   if (threadIdx.x == 0) {
     // every store of phase 1 went to LOCAL memory, whose point of coherence - this GPU's L2 - also serves the peers' P2P
-    // loads, so a gpu-scope fence is enough to order them before the flag: 2 us instead of the 9-11 us MEMBAR.SYS took on an
-    // SM that shares its memory pipeline with a GEMM CTA (measured; replicas stay bit-identical, tests/test_multi_gpu.py).
+    // loads, so a gpu-scope fence is enough to order them before the flag, and much cheaper than MEMBAR.SYS (replicas stay
+    // bit-identical, tests/test_multi_gpu.py).
     // fence_gpu = 0 (SB_XCHG_FENCE_SYS=1) uses the sys scope the PTX memory model asks for between devices.
     if (p.fence_gpu) __threadfence(); else __threadfence_system();
     sh_last = (atomicAdd(&mine->blocks_done[sync], 1u) == gridDim.x - 1) ? 1u : 0u;
@@ -305,8 +302,8 @@ xchg_update_kernel(const XchgParams p) {
   }
   stamp_max(5);
   // ---- all-gather by P2P LOADS: every run somebody else owns is pulled from its owner once that owner has updated ----
-  // (a pushed all-gather has to fence its remote stores before it may raise a flag: 12 us per launch on 2 x B200 while the
-  // peer's GEMMs kept its L2 busy; a pull needs no fence, and a peer's "updated" flag also tells that it has finished
+  // (a pushed all-gather has to fence its remote stores before it may raise a flag, which is slow while the peer's GEMMs
+  // keep its L2 busy; a pull needs no fence, and a peer's "updated" flag also tells that it has finished
   // reading MY gradient - on exit my operands are final and my gradient buffer is free)
   if (alive) alive = xchg_wait(mine->done[sync], p.world, epoch, p, sync, &sh_fail);
   if (p.trace != nullptr && blockIdx.x == 0 && threadIdx.x == 0) p.trace[6] = globaltimer_ns();
@@ -398,8 +395,8 @@ xchg_update_kernel(const XchgParams p) {
 //           parameters; runs without a shadow: fp32 theta, two stores)
 //   gather  runs others own: poll sbuf, unpack into my shadow / theta
 //
-// The chain is  store latency (2.7 us) + 2 x bytes / bandwidth, twice - about half of the flag-and-pull protocol above,
-// whose three fabric round trips cost ~27 us beside a GEMM however little data they moved (profiles/results_r02.md).
+// The chain is  store latency + 2 x bytes / bandwidth, twice - fewer fabric round trips than the flag-and-pull protocol
+// above, whose three round trips cost the same however little data they move.
 // Buffers (arena, behind the flag block): gbuf = world x n4 entries, sbuf = n4 entries of 32 bytes, entry i = parameters
 // 4 i .. 4 i + 3 as four 8-byte units {value bits, epoch} (two 16-byte halves in two planes, see the kernel); a shadow
 // entry uses the first half {2 x bf16, epoch, 2 x bf16, epoch}.

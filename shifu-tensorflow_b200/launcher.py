@@ -2,11 +2,11 @@
 
 The stock executor starts ONE python process per worker container (TensorflowTaskExecutor.java:300-317) and the
 application master expects ONE metrics line per worker container and epoch (SocketServer.java:71-89,
-TensorflowSession.java:515-549).  A B200 node has 8 GPUs, so this script is what
+TensorflowSession.java:515-549).  An H100 node has up to 8 GPUs, so this script is what
 `shifu.application.python-script-path` points at when a container owns more than one GPU: it is started with the
 executor's usual environment (the same contract `trainer.py` honours) and
 
-  * starts G local ranks (`python -m shifu_tensorflow_b200.trainer`), G = $SB_LOCAL_GPUS or the number of sm_100
+  * starts G local ranks (`python -m shifu_tensorflow_b200.trainer`), G = $SB_LOCAL_GPUS or the number of sm_90
     devices, with the contract rewritten for a world of WORKER_CNT * G ranks:
         WORKER_CNT'   = WORKER_CNT * G          TASK_ID' = TASK_ID * G + g          LOCAL_RANK = SB_DEVICE = g
         CLUSTER_SPEC' = every worker address repeated G times (only worker[0], the NCCL-id rendezvous of global

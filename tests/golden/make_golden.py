@@ -1,5 +1,5 @@
-"""Generates tests/golden/*.json|npz from the reference's OWN artefacts, in the build container only
-(/root/reference does not exist on the GPU box).  Run:  python tests/golden/make_golden.py
+"""Generates tests/golden/* from the reference's OWN artefacts, so that the tests need no copy of the reference.  Run:
+    python tests/golden/make_golden.py <shifu-tensorflow checkout>/shifu-tensorflow-eval/src/test/resources/dummydl
 
 dummydl_known_answers.json : forward outputs of the reference's SavedModel fixture
     (shifu-tensorflow-eval/src/test/resources/dummydl, loaded by TensorflowModelTest.java:35-60) computed by the
@@ -9,10 +9,17 @@ dummydl_op_attrs.json : for every op type in the fixture's GraphDef (written by 
     nodes carry, plus the attribute keys of the SignatureDef / SaverDef plumbing - the structural reference our own
     SavedModel writer is linted against (tests/test_formats.py).
 dummydl_head.npz : the first 3 and the last layer of that model + a 16-row input/output pair, small enough to
-    commit, so the GPU box can check the scorer kernels against the fixture's real weights.
+    commit, so the scorer kernels can be checked against the fixture's real weights.
+dummydl_saved_model.pb.xz, dummydl_variables.index : the fixture's GraphDef and tensor-bundle index exactly as TF wrote
+    them (xz-compressed graph).  With the stored tensors written at the index's offsets into a (sparse) data file they make
+    the fixture again: tests/test_formats.py rebuilds it so that both readers run on a TF-written model.
+dummydl_mlp_mid.npz : layers 3..19 of the MLP as the oracle reader extracts it (dummydl_head.npz holds the others), with
+    the variable names and activations of all 21 layers; checked against the index's crcs.
 """
 import json
+import lzma
 import os
+import shutil
 import sys
 
 import numpy as np
@@ -21,10 +28,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
 from oracle import tf_formats as tff  # noqa: E402
 
-FIXTURE = "/root/reference/shifu-tensorflow-eval/src/test/resources/dummydl"
 
 
-def main():
+def main(fixture):
+    FIXTURE = fixture
     layers, names = tff.extract_mlp(FIXTURE, "dense_46_input", "dense_66/Sigmoid")
     cases = []
     for value in (0.5, 0.0):
@@ -47,8 +54,16 @@ def main():
     json.dump({"source": "dummydl/saved_model.pb (TF-written GraphDef), via oracle/tf_formats.read_graph_nodes",
                "op_attr_keys": {op: sorted(keys) for op, keys in sorted(ops.items())}, "signatures": sorted(sigs)},
               open(os.path.join(HERE, "dummydl_op_attrs.json"), "w"), indent=1)
+    shutil.copyfile(os.path.join(FIXTURE, "variables", "variables.index"), os.path.join(HERE, "dummydl_variables.index"))
+    with open(os.path.join(FIXTURE, "saved_model.pb"), "rb") as f, lzma.open(os.path.join(HERE, "dummydl_saved_model.pb.xz"), "wb",
+                                                                          preset=9 | lzma.PRESET_EXTREME) as g:
+        g.write(f.read())
+    mid = {i: l for i, l in enumerate(layers) if 3 <= i < len(layers) - 1}
+    np.savez_compressed(os.path.join(HERE, "dummydl_mlp_mid.npz"), acts=np.array([l[2] for l in layers], np.int32),
+                        names=np.array([n for pair in names for n in pair]),
+                        **{"W%d" % i: l[0] for i, l in mid.items()}, **{"b%d" % i: l[1] for i, l in mid.items()})
     print("wrote", os.listdir(HERE))
 
 
 if __name__ == "__main__":
-    main()
+    main(sys.argv[1])

@@ -1,5 +1,5 @@
 """No-GPU checks of the drop-in boundary: the library loads, exports every symbol include/shifu_b200.h declares,
-and every compute entry point fails loudly (never falls back) when no sm_100 device is present."""
+and every compute entry point fails loudly (never falls back) when no sm_90 device is present."""
 import ctypes
 import os
 import re

@@ -1,6 +1,7 @@
-"""SavedModel / tensor-bundle formats on the CPU: oracle reader vs the reference's own fixture (when present),
+"""SavedModel / tensor-bundle formats on the CPU: oracle reader vs the reference's own fixture (rebuilt from tests/golden),
 product C++ reader vs oracle reader, product writer -> both readers, golden known answers."""
 import json
+import lzma
 import os
 
 import numpy as np
@@ -9,9 +10,40 @@ import pytest
 from oracle import shifu_oracle as so
 from oracle import tf_formats as tff
 
-FIXTURE = "/root/reference/shifu-tensorflow-eval/src/test/resources/dummydl"
-GOLDEN = os.path.join(os.path.dirname(__file__), "golden", "dummydl_known_answers.json")
-have_fixture = pytest.mark.skipif(not os.path.isdir(FIXTURE), reason="reference fixture only exists in the build container")
+GOLDEN_DIR = os.path.join(os.path.dirname(__file__), "golden")
+GOLDEN = os.path.join(GOLDEN_DIR, "dummydl_known_answers.json")
+
+
+@pytest.fixture(scope="module")
+def fixture_dir(tmp_path_factory):
+    """The reference's dummydl SavedModel (eval/test/resources/dummydl) rebuilt from tests/golden: TF's own GraphDef and
+    tensor-bundle index, and the 21 layers' tensors written at the offsets that index gives into a sparse data file (the
+    Adam slots and other variables the MLP does not use read as zeros)."""
+    d = tmp_path_factory.mktemp("dummydl")
+    os.makedirs(d / "variables")
+    with lzma.open(os.path.join(GOLDEN_DIR, "dummydl_saved_model.pb.xz")) as f:
+        (d / "saved_model.pb").write_bytes(f.read())
+    index = open(os.path.join(GOLDEN_DIR, "dummydl_variables.index"), "rb").read()
+    (d / "variables" / "variables.index").write_bytes(index)
+    head = np.load(os.path.join(GOLDEN_DIR, "dummydl_head.npz"))
+    mid = np.load(os.path.join(GOLDEN_DIR, "dummydl_mlp_mid.npz"))
+    names = [str(n) for n in mid["names"]]
+    n = len(names) // 2
+    layer = lambda i: (head["W%d" % min(i, 3)], head["b%d" % min(i, 3)]) if i < 3 or i == n - 1 else (mid["W%d" % i], mid["b%d" % i])
+    tensors = {nm: arr for i in range(n) for nm, arr in zip(names[2 * i:2 * i + 2], layer(i))}
+    entries = {}
+    for key, val in tff.read_table(str(d / "variables" / "variables.index")):
+        if key:
+            m = tff.parse_proto(val)
+            entries[key.decode()] = ([v for fn, _, v in m if fn == 4] or [0])[0], ([v for fn, _, v in m if fn == 5] or [0])[0]
+    with open(d / "variables" / "variables.data-00000-of-00001", "wb") as f:
+        f.truncate(max(off + size for off, size in entries.values()))
+        for nm, arr in tensors.items():
+            off, size = entries[nm]
+            assert size == arr.nbytes, nm
+            f.seek(off)
+            f.write(np.ascontiguousarray(arr, "<f4").tobytes())
+    return str(d)
 
 
 def test_crc32c_known_answers():
@@ -19,10 +51,9 @@ def test_crc32c_known_answers():
     assert tff.crc32c(b"\x00" * 32) == 0x8A9136AA           # RFC 3720 B.4
 
 
-@have_fixture
-def test_oracle_reader_on_reference_fixture_matches_golden():
+def test_oracle_reader_on_reference_fixture_matches_golden(fixture_dir):
     """TensorflowModelTest.java:35-60 loads this model (inputs dense_46_input, output dense_66/Sigmoid)."""
-    layers, names = tff.extract_mlp(FIXTURE, "dense_46_input", "dense_66/Sigmoid")
+    layers, names = tff.extract_mlp(fixture_dir, "dense_46_input", "dense_66/Sigmoid")
     assert len(layers) == 21 and layers[0][0].shape == (1522, 100) and layers[-1][0].shape == (100, 1)
     assert [l[2] for l in layers] == [so.ACT_RELU] * 20 + [so.ACT_SIGMOID]
     g = json.load(open(GOLDEN))
@@ -35,22 +66,20 @@ def test_oracle_reader_on_reference_fixture_matches_golden():
         np.testing.assert_allclose(got, np.asarray(case["expected"], np.float32), atol=2e-6)
 
 
-@have_fixture
-def test_bundle_crcs_of_reference_fixture():
-    b = tff.read_bundle(os.path.join(FIXTURE, "variables", "variables"), verify_crc=False)
+def test_bundle_crcs_of_reference_fixture(fixture_dir):
+    b = tff.read_bundle(os.path.join(fixture_dir, "variables", "variables"), verify_crc=False)
     assert b["dense_46/kernel"].shape == (1522, 100)
-    # verify the stored per-tensor crc32c of two tensors (full verify of 27 MB in pure python is slow)
-    entries = dict(tff.read_table(os.path.join(FIXTURE, "variables", "variables.index")))
-    for key in (b"dense_66/bias", b"dense_66/kernel"):
+    # every MLP tensor the fixture was rebuilt from carries the per-tensor crc32c TF stored for it
+    entries = dict(tff.read_table(os.path.join(fixture_dir, "variables", "variables.index")))
+    for key in [("dense_%d/%s" % (i, k)).encode() for i in range(46, 67) for k in ("kernel", "bias")]:
         m = tff.parse_proto(entries[key])
         stored = [v for f, _, v in m if f == 6][0]
         assert tff.crc_mask(tff.crc32c(b[key.decode()].tobytes())) == stored
 
 
-@have_fixture
-def test_cpp_reader_equals_oracle_reader_on_fixture(sb):
-    F, hidden, acts, out_act, flat = sb.capi.savedmodel_read(FIXTURE, "dense_46_input", "dense_66/Sigmoid")
-    layers, _ = tff.extract_mlp(FIXTURE, "dense_46_input", "dense_66/Sigmoid")
+def test_cpp_reader_equals_oracle_reader_on_fixture(sb, fixture_dir):
+    F, hidden, acts, out_act, flat = sb.capi.savedmodel_read(fixture_dir, "dense_46_input", "dense_66/Sigmoid")
+    layers, _ = tff.extract_mlp(fixture_dir, "dense_46_input", "dense_66/Sigmoid")
     assert F == 1522 and hidden == [100] * 20 and acts == [so.ACT_RELU] * 20 and out_act == so.ACT_SIGMOID
     ref = np.concatenate([np.concatenate([W.ravel(), b.ravel()]) for W, b, _ in layers])
     np.testing.assert_array_equal(flat, ref)

@@ -1,5 +1,5 @@
 """The tensor-core parity GEMM (SB_PREC_FP32_TC / SB_PREC_BF16X2): fp32 operands held as 3 / 2 bf16 parts, the part
-products with i + j < np accumulated in fp32 TMEM by the SAME tcgen05 kernel over an extended K axis.  Checked against a
+products with i + j < np accumulated in fp32 by the SAME wgmma kernel over an extended K axis.  Checked against a
 float64 contraction of the fp32 inputs; the bound is relative to sum_k |a_k b_k| (what an fp32 dot product is held to)."""
 import numpy as np
 import pytest

@@ -1,7 +1,7 @@
-"""Kernel-level parity of the tcgen05 GEMM (gemm_tc.cuh) through the C-ABI test hook.
+"""Kernel-level parity of the wgmma GEMM (gemm_tc.cuh) through the C-ABI test hook.
 
 Oracle: float64 matmul of the bf16-rounded operands (the kernel multiplies exact bf16 products and accumulates
-in fp32 in TMEM, so the only difference is fp32 summation order/rounding)."""
+in fp32 registers, so the only difference is fp32 summation order/rounding)."""
 import numpy as np
 import pytest
 
@@ -17,7 +17,7 @@ SHAPES = [
     (1000, 512, 4096, 4),     # cfg1 layer-0 dW as split-K over the batch
     (512, 256, 4096, 16),     # deeper split
     (130, 129, 72, 2),        # everything ragged + split
-    (8192, 1024, 2000, 1),    # cfg2 layer-0 forward (persistent: > 148 tiles, TMEM double buffering)
+    (8192, 1024, 2000, 1),    # cfg2 layer-0 forward (persistent: > 132 tiles, several per CTA)
 ]
 
 
@@ -42,7 +42,7 @@ def test_gemm_bf16_matches_fp64(sb, M, N, K, split_k, layout):
     assert err <= 2e-5 * scale * 4, "max abs err %g (K=%d)" % (err, K)
 
 
-TILES = [(1, 64), (1, 128), (2, 128), (2, 256)]   # (cta_group, BN)
+TILES = [(1, 64), (1, 128), (2, 128), (2, 256)]   # (CTAs per tile, BN)
 
 
 @pytest.mark.gpu
@@ -50,8 +50,8 @@ TILES = [(1, 64), (1, 128), (2, 128), (2, 256)]   # (cta_group, BN)
 @pytest.mark.parametrize("layout", sorted(LAYOUTS))
 @pytest.mark.parametrize("M,N,K,split_k", [(300, 200, 136, 1), (1000, 512, 1024, 2), (2048, 1024, 512, 1)])
 def test_gemm_every_tile_configuration(sb, M, N, K, split_k, layout, cg, bn):
-    """each instantiated tile shape (single CTA 128xBN, CTA pair 256xBN with cta_group::2) on ragged and multi-wave
-    problems, forced through the debug hook (the planner would not pick every one of them at these sizes)"""
+    """each instantiated tile shape (single CTA 128xBN, CTA pair 256xBN: a cluster of two sharing B by TMA multicast) on
+    ragged and multi-wave problems, forced through the debug hook (the planner would not pick every one of them here)"""
     if bn == 64 and N > 64:
         N = 64
     a_mn, b_mn = LAYOUTS[layout]

@@ -24,7 +24,7 @@ def _one_step(sb, n_features, hidden, acts, rows, loss, optimizer, precision, we
 
 
 # the two parity modes: fp32 FFMA on the CUDA cores, and fp32-class accuracy on the tensor cores (three bf16 parts per value,
-# six tcgen05 products per contraction) - both must meet the north star's fp32 tolerances
+# six wgmma products per contraction) - both must meet the north star's fp32 tolerances
 FP32_MODES = [0, 2]     # sb.PREC_FP32, sb.PREC_FP32_TC
 
 
@@ -103,7 +103,7 @@ def _bf16_case(sb, F, hidden, acts, rows, loss, weights, seed=3):
 @pytest.mark.parametrize("cfg_name,F,hidden,rows", [("cfg0", 200, [100, 50], 100), ("cfg1", 1000, [512, 256, 128], 4096),
                                                     ("cfg2", 2000, [1024, 512, 256], 8192)])
 def test_bf16_step_against_bf16_oracle(sb, cfg_name, F, hidden, rows):
-    """tcgen05 path (bf16 operands, fp32 TMEM accumulation) against the oracle that rounds to bf16 at exactly the
+    """tensor-core path (bf16 operands, fp32 accumulation) against the oracle that rounds to bf16 at exactly the
     points the kernels do (oracle.loss_and_grads_bf16).  What is left is fp32-vs-fp64 accumulation order, so the
     bound is tight: 1e-5 absolute on the loss, 2e-3 of the gradient's max magnitude on gradients (an activation
     sitting on a rounding boundary may flip one bf16 ulp).  The distance to the pure fp32 oracle is the bf16
