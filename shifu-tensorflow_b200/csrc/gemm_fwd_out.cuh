@@ -1,0 +1,401 @@
+// Last hidden layer of a TRAINING step with the output layer fused into its epilogue (K2 + K3 + K4 + output backward in
+// one kernel, res/ssgd_monitor.py:121,129; h_L = N <= 256, so one CTA holds whole rows of A_L):
+//   a     = act(A_{L-1} W_L + b_L)                 fp32, never rounded, never leaves the registers
+//   z     = a . w_o + b_o,  y_hat = sigmoid(z),  loss term,  dz
+//   dZ_L  = dz * w_o * act'(a)  -> bf16 (or its split-precision parts), by TMA store
+//   db_L / dw_o column sums, db_o and the loss sum by atomics into the flat gradient / the step scalars
+//
+// Tile: 64 rows x BN (BN = 64 | 128 | 256 >= N).  The 64-row tile puts twice as many CTAs on the machine as a 128-row one
+// (cfg2: 128 of 132 SMs at 8192 rows), and the two consumer warpgroups split N instead of M: warpgroup g multiplies the
+// same 64 rows against columns g BN/2 .. g BN/2 + BN/2 - 1 with wgmma.m64n(BN/2)k16, so its accumulator is BN/4 registers
+// per thread (64 at BN = 256).  The epilogue runs in the wgmma fragment layout itself - no fp32 staging through shared
+// memory: thread (warp w of the group, lane l) holds rows 16 w + l/4 and +8 at the column pairs 8 i + 2 (l % 4).
+//   row dot products  : per-thread partials, shuffle over the 4 lanes of a row, the two warpgroups' halves through shared
+//                       memory (one consumer barrier)
+//   column sums       : each thread adds its two rows, a reduce-scatter over the 8 row groups of the warp (3 shuffle
+//                       rounds that halve the data each time), red.shared across the 4 warps of the group; flushed to
+//                       the flat gradient once per CTA
+//   dZ_L              : bf16 pairs into BN/64 128-byte-swizzled 64 x 64 tiles (the output tensor map's layout; conflict
+//                       free for the fragment), one cp.async.bulk.tensor store per tile
+// Producer warpgroup, operand ring, TMA zero fill of the M / N / K tails, setmaxnreg split and PDL as in gemm_tc.cuh.
+#pragma once
+#include "gemm_tc.cuh"
+
+namespace sb {
+
+// tensor maps of the split-precision parts (np = 1: index 0 only); one kernel parameter of 1152 B
+struct FwdOutTmaps {
+  CUtensorMap a[3];   // A_{L-1} [rows, K] K-major: box 64 (K) x 64 rows
+  CUtensorMap b[3];   // W_L [K, N] MN-major: box 64 (N) x 64 (K)
+  CUtensorMap o[3];   // dZ_L [rows, N]: box 64 columns x 64 rows (store)
+};
+
+template <int BN>
+struct FwdOutCfg {
+  static_assert(BN == 64 || BN == 128 || BN == 256, "tile N");
+  static constexpr int BM = 64;
+  static constexpr int BK = 64;
+  static constexpr int WN = BN / 2;                 // columns of one consumer warpgroup
+  static constexpr int A_BYTES = BM * BK * 2;       // 8 KB
+  static constexpr int B_BYTES = BN * BK * 2;       // BN / 64 MN-major 64 x 64 boxes
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int X_BYTES = BM * BN * 2;       // dZ_L staging tiles
+  // besides the ring: align slack, barriers, bias + w_o, the two column-sum arrays, z partials [tile parity][group][64]
+  static constexpr int FIXED_BYTES = 1024 + 256 + 2 * BN * 4 + 2 * BN * 4 + 2 * 2 * BM * 4 + X_BYTES;
+  static constexpr int RING_BUDGET = 232448 - FIXED_BYTES;   // 227 KB of dynamic shared memory per block
+  static constexpr int STAGES = RING_BUDGET / STAGE_BYTES > 8 ? 8 : RING_BUDGET / STAGE_BYTES;
+  static_assert(STAGES >= 4, "operand ring");
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED_BYTES;
+  static constexpr int EPI_THREADS = 256;           // the two consumer warpgroups
+  static constexpr int PRODUCER_WARP = 8;
+  static constexpr int THREADS = EPI_THREADS + 128;
+  static constexpr int CONSUMER_REGS = 232;
+  static constexpr int PRODUCER_REGS = 40;
+};
+
+// Sums of N_ column values over the 8 row groups of a warp (lane bits 2..4).  Every round sends half of the values that
+// are still open to the partner lane and keeps the other half, so on return lane l holds the complete sums of the
+// N_ / 8 values q N_ / 8 .. q N_ / 8 + N_ / 8 - 1, q = l / 4, in v[0 .. N_ / 8 - 1].
+template <int LEN, int N_>
+__device__ __forceinline__ void colsum_halve(float (&v)[N_], int lane, int m) {   // one round: v[0 .. 2 LEN) -> v[0 .. LEN)
+  const bool upper = (lane & m) != 0;
+#pragma unroll
+  for (int i = 0; i < LEN; ++i) {
+    const float send = upper ? v[i] : v[i + LEN];
+    const float keep = upper ? v[i + LEN] : v[i];
+    v[i] = keep + __shfl_xor_sync(0xffffffffu, send, m);
+  }
+}
+template <int N_>
+__device__ __forceinline__ void colsum_row_groups(float (&v)[N_], int lane) {
+  static_assert(N_ % 8 == 0, "three halving rounds");
+  colsum_halve<N_ / 2>(v, lane, 16);
+  colsum_halve<N_ / 4>(v, lane, 8);
+  colsum_halve<N_ / 8>(v, lane, 4);
+}
+
+template <int BN, int ACT>
+__global__ void __launch_bounds__(FwdOutCfg<BN>::THREADS, 1)
+gemm_fwd_out_kernel(const __grid_constant__ FwdOutTmaps tms, const GemmTcParams p) {
+  using Cfg = FwdOutCfg<BN>;
+  constexpr int BM = Cfg::BM, BK = Cfg::BK, STAGES = Cfg::STAGES, WN = Cfg::WN;
+
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // SWIZZLE_128B needs 1024 B alignment
+  const uint32_t xs_base = smem_base + STAGES * Cfg::STAGE_BYTES;     // dZ_L staging tiles (1024-byte aligned)
+  const uint32_t bar_base = xs_base + Cfg::X_BYTES;                   // full[STAGES], empty[STAGES] (8 B each)
+  const uint32_t sm_vec = bar_base + 256u;                            // [bias BN][w_o BN] fp32, 0 beyond N
+  const uint32_t sm_col = sm_vec + 2u * BN * 4u;                      // [db_L BN][dw_o BN] fp32 column sums
+  const uint32_t sm_z = sm_col + 2u * BN * 4u;                        // z partials [tile parity][group][64 rows]
+  auto full_bar = [&](int s) { return bar_base + 8u * s; };
+  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+  auto smem_a = [&](int s) { return smem_base + s * Cfg::STAGE_BYTES; };
+  auto smem_b = [&](int s) { return smem_base + s * Cfg::STAGE_BYTES + Cfg::A_BYTES; };
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const bool tracing = p.trace != nullptr && blockIdx.x == 0;
+  auto stamp = [&](int slot) { if (tracing) p.trace[slot] = globaltimer_ns(); };
+  if (threadIdx.x == 0) stamp(0);  // kernel entry
+
+  const int np = p.np > 0 ? p.np : 1;
+  const int n_pairs = p.n_pairs > 0 ? p.n_pairs : 1;
+  if (warp == Cfg::PRODUCER_WARP && lane == 0) {
+    tma_prefetch_desc(&tms.a[0]);
+    tma_prefetch_desc(&tms.b[0]);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(full_bar(s), 1);    // the producer's arrive.expect_tx
+      mbar_init(empty_bar(s), 2);   // one arrival per consumer warpgroup
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) stamp(1);  // setup done
+  pdl_wait();
+  pdl_launch_dependents();
+  if (threadIdx.x == 0) stamp(2);  // dependencies resolved
+
+  const int tiles = (p.M + BM - 1) / BM;
+  const int part_kb = (p.K + BK - 1) / BK;         // k-blocks of ONE part pair
+  const int total_kb = part_kb * n_pairs;          // extended K axis: the pairs one after the other
+
+  if (warp >= Cfg::PRODUCER_WARP) {
+    // ================= TMA producer =================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::PRODUCER_REGS));
+    if (warp == Cfg::PRODUCER_WARP && lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      const int a_row0 = (p.a_rows != nullptr) ? p.a_rows->row0 : 0;  // batch position inside the resident set
+      for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+        for (int kbx = 0; kbx < total_kb; ++kbx) {
+          const int pp = (n_pairs > 1) ? kbx / part_kb : 0;     // which part pair this k-block belongs to
+          const int kb = kbx - pp * part_kb;
+          const CUtensorMap* tmA = &tms.a[n_pairs > 1 ? p.pair_a[pp] : 0];
+          const CUtensorMap* tmB = &tms.b[n_pairs > 1 ? p.pair_b[pp] : 0];
+          mbar_wait(empty_bar(stage), phase ^ 1);
+          const uint32_t fb = full_bar(stage);
+          mbar_arrive_expect_tx(fb, Cfg::STAGE_BYTES);
+          tma_load_2d(smem_a(stage), tmA, fb, kb * BK, t * BM + a_row0);
+#pragma unroll
+          for (int j = 0; j < BN / 64; ++j) tma_load_2d(smem_b(stage) + j * 8192, tmB, fb, j * 64, kb * BK);
+          if (kbx == 0 && t == static_cast<int>(blockIdx.x)) stamp(3);  // first TMA issued
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+    __syncwarp();   // the whole warp reaches the final block barrier together (bar.sync counts warps, not lanes)
+  } else {
+    // ================= consumer warpgroups (warps 0..7): MMA, then the fused epilogue of the tile =================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::CONSUMER_REGS));
+    const int wg = warp >> 2;                 // columns wg WN .. wg WN + WN - 1 of the tile
+    const int et = static_cast<int>(threadIdx.x);
+    auto bar_all = [&]() { asm volatile("bar.sync 1, %0;" ::"n"(Cfg::EPI_THREADS) : "memory"); };
+    const bool xthread = (warp == 0 && lane == 0);   // issues the dZ_L stores
+    auto lds = [](uint32_t a) { float v; asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a) : "memory"); return v; };
+    auto lds2 = [](uint32_t a) {
+      float2 v;
+      asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(a) : "memory");
+      return v;
+    };
+    auto sts = [](uint32_t a, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(v) : "memory"); };
+    // bias and w_o staged once (broadcast ld.shared in the epilogue), column sums cleared
+    for (int j = et; j < 2 * BN; j += Cfg::EPI_THREADS) {
+      const int col = j < BN ? j : j - BN;
+      const float* src = j < BN ? p.bias : p.wo;
+      sts(sm_vec + static_cast<uint32_t>(j) * 4u, col < p.N ? __ldg(src + col) : 0.f);
+      sts(sm_col + static_cast<uint32_t>(j) * 4u, 0.f);
+    }
+    bar_all();
+    const float b_o = __ldg(p.bo);
+    const float nnz = p.scal[SCAL_NNZ];
+    const float inv_nnz = nnz > 0.f ? 1.f / nnz : 0.f;
+    float loss_acc = 0.f, dz_acc = 0.f;   // this warp's loss / db_o contributions over all its tiles (group 0 only)
+
+    // fragment: rows r0 = 16 (warp & 3) + lane / 4 and r0 + 8; n8 block i holds columns c0 + 8 i + {0, 1}
+    const int r0 = (warp & 3) * 16 + (lane >> 2);
+    const int c0 = wg * WN + 2 * (lane & 3);
+    float acc[WN / 2];
+    // descriptor steps for 16 elements along K: A K-major = 32 B inside the swizzle row; B MN-major = 16 rows of 128 B.
+    // This group's B columns: the next 64-wide MN atom(s), or for WN = 32 the second half of the 128-byte swizzle rows
+    // (the swizzle is a function of the address, so a start 64 B into the row reads columns 32..63).
+    constexpr uint32_t a_kstep = 32u >> 4, b_kstep = 2048u >> 4;
+    const uint32_t b_wg_off = WN >= 64 ? static_cast<uint32_t>(wg) * (WN / 64) * 8192u : static_cast<uint32_t>(wg) * 64u;
+    int stage = 0;
+    uint32_t phase = 0;
+    int it = 0;
+    for (int t = blockIdx.x; t < tiles; t += gridDim.x, ++it) {
+      const int row0 = t * BM + r0, row1 = row0 + 8;
+      const bool ok0 = row0 < p.M, ok1 = row1 < p.M;
+      // per-row label / weight fetched before the main loop
+      const float y0 = ok0 ? __ldg(p.desc->y + row0) : 0.f, w0 = ok0 ? __ldg(p.desc->w + row0) : 0.f;
+      const float y1 = ok1 ? __ldg(p.desc->y + row1) : 0.f, w1 = ok1 ? __ldg(p.desc->w + row1) : 0.f;
+
+      // ---------- main loop: wgmma over the k-blocks ----------
+      auto release = [&](int s_) { if ((warp & 3) == 0 && lane == 0) mbar_arrive(empty_bar(s_)); };
+      int prev_stage = -1;
+      for (int kb = 0; kb < total_kb; ++kb) {
+        mbar_wait(full_bar(stage), phase);  // the stage's TMA bytes have landed
+        if (kb == 0 && it == 0 && threadIdx.x == 0) stamp(4);  // first stage landed
+        const uint64_t da = make_kmajor_sw128_desc(smem_a(stage));
+        const uint64_t db = make_mnmajor_sw128_desc(smem_b(stage) + b_wg_off, 8192u);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)
+          wgmma_bf16<WN, 0, 1>(acc, da + a_kstep * k, db + b_kstep * k, (kb > 0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous k-block's wgmma group has finished reading its stage
+        if (prev_stage >= 0) release(prev_stage);
+        prev_stage = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if (prev_stage >= 0) release(prev_stage);
+      if (it == 0 && threadIdx.x == 0) { stamp(5); stamp(6); }  // first tile's accumulator complete
+
+      // ---------- (1) a = act(acc + bias), 0 beyond N;  (2) row partials of a . w_o ----------
+      float zp0 = 0.f, zp1 = 0.f;
+#pragma unroll
+      for (int i = 0; i < WN / 8; ++i) {
+        const int c = c0 + 8 * i;
+        const float2 b = lds2(sm_vec + static_cast<uint32_t>(c) * 4u);
+        const float2 wo = lds2(sm_vec + static_cast<uint32_t>(BN + c) * 4u);
+        acc[4 * i + 0] = act_apply(acc[4 * i + 0] + b.x, ACT);
+        acc[4 * i + 1] = act_apply(acc[4 * i + 1] + b.y, ACT);
+        acc[4 * i + 2] = act_apply(acc[4 * i + 2] + b.x, ACT);
+        acc[4 * i + 3] = act_apply(acc[4 * i + 3] + b.y, ACT);
+        if (p.N < BN) {
+          if (c >= p.N) { acc[4 * i + 0] = 0.f; acc[4 * i + 2] = 0.f; }
+          if (c + 1 >= p.N) { acc[4 * i + 1] = 0.f; acc[4 * i + 3] = 0.f; }
+        }
+        zp0 = fmaf(acc[4 * i + 0], wo.x, zp0); zp0 = fmaf(acc[4 * i + 1], wo.y, zp0);
+        zp1 = fmaf(acc[4 * i + 2], wo.x, zp1); zp1 = fmaf(acc[4 * i + 3], wo.y, zp1);
+      }
+#pragma unroll
+      for (int m = 1; m <= 2; m <<= 1) {
+        zp0 += __shfl_xor_sync(0xffffffffu, zp0, m);
+        zp1 += __shfl_xor_sync(0xffffffffu, zp1, m);
+      }
+      const uint32_t zs = sm_z + static_cast<uint32_t>(it & 1) * (2u * BM * 4u);   // [group][64]
+      if ((lane & 3) == 0) {
+        sts(zs + static_cast<uint32_t>(wg * BM + r0) * 4u, zp0);
+        sts(zs + static_cast<uint32_t>(wg * BM + r0 + 8) * 4u, zp1);
+      }
+      if (xthread) tma_store_wait_read<0>();   // the previous tile's dZ_L stores have read the staging tiles
+      bar_all();
+      const float z0 = lds(zs + static_cast<uint32_t>(r0) * 4u) + lds(zs + static_cast<uint32_t>(BM + r0) * 4u) + b_o;
+      const float z1 = lds(zs + static_cast<uint32_t>(r0 + 8) * 4u) + lds(zs + static_cast<uint32_t>(BM + r0 + 8) * 4u) + b_o;
+
+      // ---------- (3) per row: y_hat, loss term, dz (a rolled loop over the two rows: one copy of the code) ----------
+      float dz0 = 0.f, dz1 = 0.f;
+#pragma unroll 1
+      for (int h = 0; h < 2; ++h) {
+        const float z = h ? z1 : z0, y = h ? y1 : y0, wgt = h ? w1 : w0;
+        float dz = 0.f, lossv = 0.f;
+        if (h ? ok1 : ok0) {
+          const float yh = sigmoidf_stable(z);
+          if (p.loss == SB_LOSS_MSE) {
+            const float d = yh - y;
+            lossv = wgt * d * d;
+            dz = 2.f * wgt * d * yh * (1.f - yh) * inv_nnz;
+          } else {
+            lossv = wgt * (fmaxf(z, 0.f) - z * y + log1pf(expf(-fabsf(z))));
+            dz = wgt * (yh - y) * inv_nnz;
+          }
+        }
+        if (h) dz1 = dz; else dz0 = dz;
+        if (wg == 0 && (lane & 3) == 0) { loss_acc += lossv; dz_acc += dz; }   // each row once
+      }
+
+      // ---------- (4) g = dz w_o act'(a) (replaces a in acc), column sums of g and dz a over the two rows ----------
+      float sdb[WN / 4], sdw[WN / 4];
+#pragma unroll
+      for (int i = 0; i < WN / 8; ++i) {
+        const float2 wo = lds2(sm_vec + static_cast<uint32_t>(BN + c0 + 8 * i) * 4u);
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float w = e ? wo.y : wo.x;
+          const float a0 = acc[4 * i + e], a1 = acc[4 * i + 2 + e];
+          const float g0 = dz0 * w * act_grad_from_out(a0, ACT);
+          const float g1 = dz1 * w * act_grad_from_out(a1, ACT);
+          sdb[2 * i + e] = g0 + g1;
+          sdw[2 * i + e] = a0 * dz0 + a1 * dz1;
+          acc[4 * i + e] = g0;
+          acc[4 * i + 2 + e] = g1;
+        }
+      }
+      // ---------- (5) over the warp's 16 rows, then across the group's 4 warps in shared memory ----------
+      colsum_row_groups(sdb, lane);
+      colsum_row_groups(sdw, lane);
+#pragma unroll
+      for (int j = 0; j < WN / 32; ++j) {
+        const int k = (lane >> 2) * (WN / 32) + j;   // value index 2 i + e of the thread's columns
+        const uint32_t col = static_cast<uint32_t>(c0 + 8 * (k >> 1) + (k & 1));
+        asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(sm_col + col * 4u), "f"(sdb[j]) : "memory");
+        asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(sm_col + (BN + col) * 4u), "f"(sdw[j]) : "memory");
+      }
+
+      // ---------- (6) dZ_L: bf16, TMA store.  Split modes: part k = bf16 of the residual after parts 0..k-1 (acc keeps
+      //            the residual) ----------
+#pragma unroll 1
+      for (int part = 0; part < np; ++part) {
+        if (part > 0) {
+#pragma unroll
+          for (int j = 0; j < WN / 2; ++j) acc[j] -= __bfloat162float(__float2bfloat16_rn(acc[j]));
+          if (xthread) tma_store_wait_read<0>();   // the previous part's stores have read the staging tiles
+          bar_all();
+        }
+#pragma unroll
+        for (int i = 0; i < WN / 8; ++i) {
+          const int c = c0 + 8 * i;   // tile column; 64 x 64 tile c / 64, 16-byte piece (c % 64) / 8, swizzled by row
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = r0 + 8 * h;
+            const uint32_t a = xs_base + static_cast<uint32_t>((c >> 6) * 8192 + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4) + (c & 7) * 2);
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(pack_bf16x2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1])) : "memory");
+          }
+        }
+        fence_proxy_async();   // generic-proxy writes -> visible to the TMA engine
+        bar_all();
+        if (xthread) {
+#pragma unroll
+          for (int x = 0; x < BN / 64; ++x)
+            if (x * 64 < p.N) tma_store_2d(&tms.o[part], xs_base + x * 8192, x * 64, t * BM);
+          tma_store_commit();
+        }
+      }
+      if (it == 0 && threadIdx.x == 0) stamp(7);  // first tile's epilogue done
+    }
+    // loss sum and db_o: one atomic pair per warp; db_L / dw_o: one red.global per column and CTA
+    if (wg == 0) {
+      const float ls = warp_sum(loss_acc), ds = warp_sum(dz_acc);
+      if (lane == 0) { atomicAdd(p.scal + SCAL_LOSS_SUM, ls); atomicAdd(p.g_bo, ds); }
+    }
+    bar_all();
+    for (int j = et; j < BN && j < p.N; j += Cfg::EPI_THREADS) {
+      const float db = lds(sm_col + static_cast<uint32_t>(j) * 4u), dw = lds(sm_col + static_cast<uint32_t>(BN + j) * 4u);
+      if (db != 0.f) red_add_f32(p.g_bL + j, db);
+      if (dw != 0.f) red_add_f32(p.g_wo + j, dw);
+    }
+    if (xthread) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // the last tiles are in global memory
+  }
+
+  __syncthreads();
+  if (threadIdx.x == 0) stamp(8);  // all roles finished
+  // in-graph kernel span: slot 2 (dependencies resolved, CTA 0) .. slot 10 (latest exit over ALL CTAs; %globaltimer only
+  // grows, so atomicMax needs no reset between steps)
+  if (p.trace != nullptr && threadIdx.x == 0) atomicMax(p.trace + 10, static_cast<unsigned long long>(globaltimer_ns()));
+}
+
+// ------------------------------------------------------------------ host side
+template <int BN, int ACT>
+static int launch_gemm_fwd_out_one(int grid, const FwdOutTmaps& tms, const GemmTcParams& p, cudaStream_t st, bool pdl) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(static_cast<unsigned>(grid));
+  cfg.blockDim = dim3(FwdOutCfg<BN>::THREADS);
+  cfg.dynamicSmemBytes = FwdOutCfg<BN>::SMEM_BYTES;
+  cfg.stream = st;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = pdl ? 1 : 0;
+  SB_CUDA(cudaLaunchKernelEx(&cfg, gemm_fwd_out_kernel<BN, ACT>, tms, p));
+  return SB_OK;
+}
+
+template <int BN>
+static int launch_gemm_fwd_out_bn(int grid, const FwdOutTmaps& tms, const GemmTcParams& p, cudaStream_t st, bool pdl) {
+  switch (p.act) {
+    case SB_ACT_SIGMOID: return launch_gemm_fwd_out_one<BN, SB_ACT_SIGMOID>(grid, tms, p, st, pdl);
+    case SB_ACT_TANH: return launch_gemm_fwd_out_one<BN, SB_ACT_TANH>(grid, tms, p, st, pdl);
+    case SB_ACT_RELU: return launch_gemm_fwd_out_one<BN, SB_ACT_RELU>(grid, tms, p, st, pdl);
+    case SB_ACT_LEAKYRELU: return launch_gemm_fwd_out_one<BN, SB_ACT_LEAKYRELU>(grid, tms, p, st, pdl);
+    default: return launch_gemm_fwd_out_one<BN, SB_ACT_NONE>(grid, tms, p, st, pdl);
+  }
+}
+
+// the narrowest tile that holds a whole row of A_L (N <= 256); one CTA per SM and 64-row tile
+static inline int fwd_out_bn(int N) { return N <= 64 ? 64 : (N <= 128 ? 128 : 256); }
+
+static int launch_gemm_fwd_out(int grid, const FwdOutTmaps& tms, const GemmTcParams& p, cudaStream_t st, bool pdl) {
+  SB_CHECK(p.N <= 256, SB_ERR_INVALID, "fused output layer: last hidden layer %d wider than 256", p.N);
+  switch (fwd_out_bn(p.N)) {
+    case 64: return launch_gemm_fwd_out_bn<64>(grid, tms, p, st, pdl);
+    case 128: return launch_gemm_fwd_out_bn<128>(grid, tms, p, st, pdl);
+    default: return launch_gemm_fwd_out_bn<256>(grid, tms, p, st, pdl);
+  }
+}
+
+// opt in to > 48 KB dynamic shared memory (once per process, outside of stream capture)
+static int set_gemm_fwd_out_attrs() {
+#define SB_ATTR_ACT(BN, ACT) \
+  SB_CUDA(cudaFuncSetAttribute(gemm_fwd_out_kernel<BN, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdOutCfg<BN>::SMEM_BYTES))
+#define SB_ATTR_ALL(BN) SB_ATTR_ACT(BN, SB_ACT_NONE); SB_ATTR_ACT(BN, SB_ACT_SIGMOID); SB_ATTR_ACT(BN, SB_ACT_TANH); \
+                        SB_ATTR_ACT(BN, SB_ACT_RELU); SB_ATTR_ACT(BN, SB_ACT_LEAKYRELU)
+  SB_ATTR_ALL(64); SB_ATTR_ALL(128); SB_ATTR_ALL(256);
+#undef SB_ATTR_ALL
+#undef SB_ATTR_ACT
+  return SB_OK;
+}
+
+}  // namespace sb

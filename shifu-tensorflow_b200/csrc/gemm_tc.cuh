@@ -14,11 +14,7 @@
 //   EPI_DW  : dW_l = A_{l-1}^T dZ_l  A = A_{l-1} [rows,in] MN-major, B = dZ_l [rows,out] MN-major; split-K over the
 //                                    batch, fp32 red.add into the flat gradient
 //   EPI_F32 : plain fp32 store (kernel-level parity test hook)
-//   EPI_FWD_OUT : last hidden layer of a TRAINING step, output layer fused into the epilogue (K2 + K3 + K4 + output
-//                 backward in one kernel; needs N = h_L <= BN so a CTA holds whole rows of A_L):
-//                 pass 1  a = act(acc + bias), z = a . w_o + b_o, y_hat = sigmoid(z), loss term, d z_hat
-//                 pass 2  (accumulator staged again from registers) dZ_L = dz * w_o * act'(a) -> bf16, db_L / dw_o column
-//                         sums, db_o, loss sum.  A_L itself never goes to HBM.
+// The last hidden GEMM of a training step, with the output layer fused into its epilogue, is gemm_fwd_out.cuh.
 //
 // Tile: one CTA owns 128 x BN (BN = 64 | 128 | 256).  CG = 2: a cluster of two CTAs owns 256 x BN; both need the same B tile,
 // so each loads half of it and TMA multicasts that half into both CTAs' shared memory (half the B traffic from L2 per CTA).
@@ -42,7 +38,7 @@
 
 namespace sb {
 
-enum { EPI_FWD = 0, EPI_DA = 1, EPI_DW = 2, EPI_F32 = 3, EPI_FWD_OUT = 4 };
+enum { EPI_FWD = 0, EPI_DA = 1, EPI_DW = 2, EPI_F32 = 3 };
 
 struct GemmTcParams {
   int M, N, K;
@@ -63,7 +59,7 @@ struct GemmTcParams {
   float* accum;  // [M, ld_acc] fp32
   int ld_acc;
   int acc_vec4;  // 1 if 16-byte aligned rows -> red.global.add.v4.f32
-  // EPI_FWD_OUT (output layer + loss + its backward, res/ssgd_monitor.py:121,129)
+  // fused output layer (gemm_fwd_out_kernel: output layer + loss + its backward, res/ssgd_monitor.py:121,129)
   const float* wo;          // [N] output-layer weights (fp32)
   const float* bo;          // [1]
   const BatchDesc* desc;    // y, w of the current batch
@@ -123,7 +119,7 @@ struct GemmTcCfg {
   // row-wise 16-byte loads are free of bank conflicts
   static constexpr int ACC_LD = 64 + 4;
   static constexpr int ACC_BYTES = BM * ACC_LD * 4;
-  // shared memory besides the operand ring: align slack, barriers, epilogue scratch, bias (+ w_o), per-warp transpose tiles
+  // shared memory besides the operand ring: align slack, barriers, epilogue scratch, bias, per-warp transpose tiles
   // (only the epilogues without TMA staging use them), column-sum accumulators, TMA staging tiles (XB), accumulator block
   static constexpr int TR_BYTES = XB > 0 ? 0 : 8 * 2048;
   static constexpr int FIXED_BYTES = 1024 + 256 + 2048 + 2048 + TR_BYTES + 4096 + XB + ACC_BYTES;
@@ -153,19 +149,15 @@ __device__ __forceinline__ void epi_da_chunk(float (&v)[32], const __nv_bfloat16
   for (int j = 0; j < 32; ++j) v[j] *= act_grad_from_out(__bfloat162float(ah[j]), ACT);
 }
 
-// ACT_T: activation fixed at compile time (EPI_FWD_OUT: its two-pass epilogue with every activation variant inlined is
-// several thousand instructions, and instruction fetch then dominates), or SB_ACT_AT_RUNTIME = read p.act.
-constexpr int SB_ACT_AT_RUNTIME = -100;
-
 // GENERIC = false: the plain-bf16 epilogues (performance mode; their instruction footprint decides the epilogue speed).
 // GENERIC = true adds the cold features at compile time: split-precision part stores / loads (np > 1) and the fp32 addend
 // of the wide+deep first layer.
-template <int BN, int EPI, bool A_MN, bool B_MN, int CG, int ACT_T = SB_ACT_AT_RUNTIME, bool GENERIC = false>
+template <int BN, int EPI, bool A_MN, bool B_MN, int CG, bool GENERIC = false>
 __global__ void __launch_bounds__((GemmTcCfg<BN, CG, epi_tma_bytes(EPI, GENERIC)>::THREADS), 1)
 gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
   using Cfg = GemmTcCfg<BN, CG, epi_tma_bytes(EPI, GENERIC)>;
   constexpr bool TMA_EPI = epi_tma_bytes(EPI, GENERIC) > 0;
-  const int act_sel = (ACT_T == SB_ACT_AT_RUNTIME) ? p.act : ACT_T;
+  const int act_sel = p.act;
   constexpr int BM = Cfg::BM, BK = Cfg::BK, STAGES = Cfg::STAGES, TILE_M = Cfg::TILE_M, BN_CTA = Cfg::BN_CTA;
 
   extern __shared__ uint8_t smem_raw[];
@@ -173,7 +165,7 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
   const uint32_t xbuf_base = smem_base + STAGES * Cfg::STAGE_BYTES;            // TMA staging tiles (1024-byte aligned)
   const uint32_t accs_base = xbuf_base + epi_tma_bytes(EPI, GENERIC);          // accumulator staging block
   const uint32_t bar_base = accs_base + Cfg::ACC_BYTES;
-  // barrier layout (8 B each): full[STAGES], empty[STAGES]; then scratch (EPI_FWD_OUT partial dot products / dA TMA barriers)
+  // barrier layout (8 B each): full[STAGES], empty[STAGES]; then scratch (dA TMA barriers)
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
   const uint32_t scratch = bar_base + 8u * (2 * STAGES) + 16u;
@@ -282,19 +274,18 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
     const int et = static_cast<int>(threadIdx.x);   // 0 .. EPI_THREADS-1 over all consumer warps
     constexpr int ET = Cfg::EPI_THREADS;
     auto bar_all = [&]() { asm volatile("bar.sync 1, %0;" ::"n"(Cfg::EPI_THREADS) : "memory"); };    // every consumer warp
-    // EPI_FWD_OUT: bias and w_o of the (single) n-tile staged in shared memory once, before the first tile, so the two
-    // epilogue passes read them with broadcast ld.shared instead of dependent global loads
-    const uint32_t sm_vec = scratch + 2048u;   // [bias BN floats][w_o BN floats]
+    // EPI_FWD: the tile's bias staged in shared memory (broadcast ld.shared instead of dependent global loads)
+    const uint32_t sm_vec = scratch + 2048u;   // [tile parity][bias BN floats]
     // Coalescing: the epilogue hands thread t the 32 columns of ROW t, so a direct 16-byte access per thread touches 32
     // different rows (32 L1 wavefronts per instruction).  Every global access of the epilogue therefore goes through a
     // warp-private 32 x 64 B tile in shared memory (16-byte pieces XOR-swizzled by row pair -> conflict-free on both
     // sides): on the global side lane l handles piece (l & 3) of rows 8 i + (l >> 2), i = 0..3, i.e. four lanes cover
     // 64 contiguous bytes of a row and one instruction touches 8 rows instead of 32.
     const uint32_t sm_stage = sm_vec + 2048u + static_cast<uint32_t>(warp) * 2048u;
-    // Column sums (bias gradients; dw_o of the fused output layer) are accumulated per CTA in shared memory and flushed to
-    // the flat gradient ONCE per tile and column: one red.global per column per 128 rows instead of one per 32 rows (with
-    // one red per warp and chunk, the wide dA GEMMs wait on the L2 atomic units).
-    // layout: [buffer (tile parity)][array 0: db | array 1: dw_o][BN] floats
+    // Column sums (bias gradients) are accumulated per CTA in shared memory and flushed to the flat gradient ONCE per tile
+    // and column: one red.global per column per 128 rows instead of one per 32 rows (with one red per warp and chunk, the
+    // wide dA GEMMs wait on the L2 atomic units).
+    // layout: [buffer (tile parity)][BN] floats
     const uint32_t sm_col = sm_vec + 2048u + static_cast<uint32_t>(Cfg::TR_BYTES);
     // TMA-staged epilogue (plain-bf16 forward / dA): the 128 x BN tile leaves in 64-column blocks.  Block k: every thread
     // writes the 32 bf16 of its row-chunk as four 16-byte pieces into the 128-byte-swizzled 128 x 64 tile xo[k & 1] (the layout
@@ -303,7 +294,7 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
     // with the same swizzle.  No ld.shared / st.global per element, no transposes, M / N tails clipped by the tensor map.
     auto xo = [&](int b) { return xbuf_base + static_cast<uint32_t>(b) * 16384u; };
     auto xa = [&](int b) { return xbuf_base + 32768u + static_cast<uint32_t>(b) * 16384u; };
-    auto aux_bar = [&](int b) { return scratch + 8u * static_cast<uint32_t>(b); };   // (scratch of EPI_FWD_OUT, unused here)
+    auto aux_bar = [&](int b) { return scratch + 8u * static_cast<uint32_t>(b); };
     const int rt = quarter * 32 + lane;                                   // row of this thread inside the CTA's 128 rows
     auto piece = [&](int half_, int i) { return static_cast<uint32_t>(rt) * 128u + static_cast<uint32_t>(((half_ * 4 + i) ^ (rt & 7)) << 4); };
     const bool xthread = (warp == 0 && lane == 0);                        // issues the epilogue's TMA loads / stores
@@ -312,26 +303,21 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
       if (warp == 0 && lane == 0) { mbar_init(aux_bar(0), 1); mbar_init(aux_bar(1), 1); fence_barrier_init(); }
       bar_all();
     }
-    auto col_slot = [&](int buf, int arr, int j) { return sm_col + static_cast<uint32_t>(((buf * 2 + arr) * BN + j) * 4); };
+    auto col_slot = [&](int buf, int j) { return sm_col + static_cast<uint32_t>((buf * BN + j) * 4); };
     auto red_shared = [](uint32_t a, float v) { asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(a), "f"(v) : "memory"); };
-    if constexpr (EPI == EPI_DA || EPI == EPI_FWD_OUT) {
-      for (int j = et; j < 4 * BN; j += ET) asm volatile("st.shared.f32 [%0], %1;" ::"r"(sm_col + static_cast<uint32_t>(j) * 4u), "f"(0.f) : "memory");
+    if constexpr (EPI == EPI_DA) {
+      for (int j = et; j < 2 * BN; j += ET) asm volatile("st.shared.f32 [%0], %1;" ::"r"(sm_col + static_cast<uint32_t>(j) * 4u), "f"(0.f) : "memory");
       bar_all();
     }
     // after every epilogue warp has added its sums of tile `it`: one thread per column flushes and clears buffer it & 1
-    auto flush_cols = [&](int it_, int tn_, float* dst0, float* dst1) {
+    auto flush_cols = [&](int it_, int tn_, float* dst) {
       bar_all();
       for (int j = et; j < BN; j += ET) {
         const int col = tn_ * BN + j;
-#pragma unroll
-        for (int arr = 0; arr < 2; ++arr) {
-          float* dst = arr == 0 ? dst0 : dst1;
-          if (dst == nullptr) continue;
-          float vsum;
-          asm volatile("ld.shared.f32 %0, [%1];" : "=f"(vsum) : "r"(col_slot(it_ & 1, arr, j)) : "memory");
-          asm volatile("st.shared.f32 [%0], %1;" ::"r"(col_slot(it_ & 1, arr, j)), "f"(0.f) : "memory");
-          if (col < p.N && vsum != 0.f) red_add_f32(dst + col, vsum);
-        }
+        float vsum;
+        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(vsum) : "r"(col_slot(it_ & 1, j)) : "memory");
+        asm volatile("st.shared.f32 [%0], %1;" ::"r"(col_slot(it_ & 1, j)), "f"(0.f) : "memory");
+        if (col < p.N && vsum != 0.f) red_add_f32(dst + col, vsum);
       }
     };
     const int lrow = lane >> 2, lpc = lane & 3;
@@ -360,16 +346,6 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
       for (int q = 0; q < 4; ++q) mine[q] = lds4(stg(lane, q));
       __syncwarp();
     };
-    if constexpr (EPI == EPI_FWD_OUT) {
-#pragma unroll
-      for (int j = et; j < 2 * BN; j += ET) {
-        const int col = (j < BN) ? j : j - BN;
-        const float* src = (j < BN) ? p.bias : p.wo;
-        const float v = (col < p.N) ? __ldg(src + col) : 0.f;
-        asm volatile("st.shared.f32 [%0], %1;" ::"r"(sm_vec + static_cast<uint32_t>(j) * 4u), "f"(v) : "memory");
-      }
-      bar_all();
-    }
 
     // ---- accumulator: registers of the wgmma fragment, handed to the epilogue one 64-column block at a time
     float acc[BN / 2];
@@ -420,9 +396,8 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
       const int kb1 = min(total_kb, kb0 + p.kb_per_split);
       const int row = tm * TILE_M + static_cast<int>(rank) * BM + quarter * 32 + lane;  // output row of this thread
       const bool row_ok = row < p.M;
-      // operands of the epilogue that do not depend on the accumulator are fetched BEFORE the main loop: per-row label /
-      // weight / n_nz / b_o of the fused output layer, and the A_{l-1} tiles of the dA epilogue
-      float pre_y = 0.f, pre_w = 0.f, pre_nnz = 0.f, pre_bo = 0.f;
+      // operands of the epilogue that do not depend on the accumulator are fetched BEFORE the main loop: the A_{l-1} tiles
+      // of the dA epilogue
       // dA epilogue without TMA staging: A_{l-1} of EVERY chunk this warp will handle is fetched before the main loop and
       // kept in registers as a shift queue, so that one L2 / HBM latency is paid per tile instead of one per chunk
       constexpr int AUXQ = (EPI == EPI_DA && !TMA_EPI) ? (BN / 64 > 0 ? BN / 64 : 1) : 1;
@@ -476,11 +451,6 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
           }
         }
       };
-      if constexpr (EPI == EPI_FWD_OUT) {
-        if (row_ok) { pre_y = __ldg(p.desc->y + row); pre_w = __ldg(p.desc->w + row); }
-        pre_nnz = p.scal[SCAL_NNZ];
-        pre_bo = __ldg(p.bo);
-      }
       if constexpr (EPI == EPI_DA && !TMA_EPI) {
 #pragma unroll
         for (int i = 0; i < AUXQ; ++i) load_aux(half + 2 * i, aux_q[i]);
@@ -539,106 +509,6 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
       if (prev_stage >= 0) release(prev_stage);
       if (w == w_first && threadIdx.x == 0) { stamp(5); stamp(6); }  // first tile's accumulator complete
 
-      if constexpr (EPI == EPI_FWD_OUT) {
-        // ---------- fused output layer (tiles_n == 1: this CTA's accumulator holds complete rows of A_L) ----------
-        const uint32_t zs = scratch + static_cast<uint32_t>(it & 1) * 1024u;  // zpart[2][128]
-        const int rl = quarter * 32 + lane;
-        // 32 consecutive fp32 of the staged bias (which = 0) / w_o (which = 1): 8 broadcast 16-byte ld.shared
-        auto load_vec32 = [&](int which, int col0, float (&o)[32]) {
-          const uint32_t a = sm_vec + static_cast<uint32_t>(which * BN + col0) * 4u;
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
-                         : "=f"(o[4 * q]), "=f"(o[4 * q + 1]), "=f"(o[4 * q + 2]), "=f"(o[4 * q + 3])
-                         : "r"(a + 16u * q));
-        };
-        auto load_act = [&](int c, float (&v)[32]) {   // a = act(acc + bias) for chunk c; 0 beyond N
-          const int col0 = c * 32;
-          uint32_t raw[32];
-          acc_ld(c, raw);
-          float b[32];
-          load_vec32(0, col0, b);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(raw[j]);
-          switch (act_sel) {
-            case SB_ACT_RELU: epi_fwd_chunk<SB_ACT_RELU>(v, b); break;
-            case SB_ACT_SIGMOID: epi_fwd_chunk<SB_ACT_SIGMOID>(v, b); break;
-            case SB_ACT_TANH: epi_fwd_chunk<SB_ACT_TANH>(v, b); break;
-            case SB_ACT_LEAKYRELU: epi_fwd_chunk<SB_ACT_LEAKYRELU>(v, b); break;
-            default: epi_fwd_chunk<SB_ACT_NONE>(v, b); break;
-          }
-          if (col0 + 32 > p.N) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (col0 + j >= p.N) v[j] = 0.f;
-          }
-        };
-        // pass 1: partial dot product of this thread's row with w_o over this warp's chunks
-        float zp = 0.f;
-#pragma unroll 1
-        for (int c = half; (c >> 1) < nblk; c += 2) {
-          stage_block(c >> 1);
-          if (c * 32 >= p.N) continue;
-          float v[32], wv[32];
-          load_act(c, v);
-          load_vec32(1, c * 32, wv);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) zp = fmaf(v[j], wv[j], zp);
-        }
-        asm volatile("st.shared.f32 [%0], %1;" ::"r"(zs + static_cast<uint32_t>(half * 128 + rl) * 4u), "f"(zp) : "memory");
-        bar_all();
-        float z0, z1;
-        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(z0) : "r"(zs + static_cast<uint32_t>(rl) * 4u) : "memory");
-        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(z1) : "r"(zs + static_cast<uint32_t>(128 + rl) * 4u) : "memory");
-        const float z = z0 + z1 + pre_bo;
-        float dz = 0.f, lossv = 0.f;
-        if (row_ok) {
-          const float nnz = pre_nnz;
-          const float inv_nnz = nnz > 0.f ? 1.f / nnz : 0.f;
-          const float yh = sigmoidf_stable(z);
-          const float y = pre_y, wgt = pre_w;
-          if (p.loss == SB_LOSS_MSE) {
-            const float d = yh - y;
-            lossv = wgt * d * d;
-            dz = 2.f * wgt * d * yh * (1.f - yh) * inv_nnz;
-          } else {
-            lossv = wgt * (fmaxf(z, 0.f) - z * y + log1pf(expf(-fabsf(z))));
-            dz = wgt * (yh - y) * inv_nnz;
-          }
-        }
-        if (half == 0) {
-          const float ls = warp_sum(lossv), ds = warp_sum(dz);
-          if (lane == 0) { atomicAdd(p.scal + SCAL_LOSS_SUM, ls); atomicAdd(p.g_bo, ds); }
-        }
-        // pass 2: rank-1 backward of the output layer through act'
-#pragma unroll 1
-        for (int c = half; (c >> 1) < nblk; c += 2) {
-          if (nblk > 1) stage_block(c >> 1);   // (one block: still staged from pass 1)
-          const int col0 = c * 32;
-          if (col0 >= p.N) continue;
-          float v[32], g[32];
-          load_act(c, v);
-          load_vec32(1, col0, g);      // g starts as w_o (0 beyond N)
-          switch (act_sel) {
-#define SB_G(ACT) _Pragma("unroll") for (int j = 0; j < 32; ++j) g[j] = dz * g[j] * act_grad_from_out(v[j], ACT);
-            case SB_ACT_RELU: SB_G(SB_ACT_RELU) break;
-            case SB_ACT_SIGMOID: SB_G(SB_ACT_SIGMOID) break;
-            case SB_ACT_TANH: SB_G(SB_ACT_TANH) break;
-            case SB_ACT_LEAKYRELU: SB_G(SB_ACT_LEAKYRELU) break;
-            default: SB_G(SB_ACT_NONE) break;
-#undef SB_G
-          }
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] *= dz;          // dz * a  -> dw_o contributions (0 for rows >= M)
-          store_parts(g, p.out, p.out_ps, p.ld_out, col0, false);       // dZ_L (bf16, or its parts)
-          const float sb_ = warp_colsum_32x32(g, lane);
-          const float sw_ = warp_colsum_32x32(v, lane);
-          red_shared(col_slot(it & 1, 0, col0 + lane), sb_);       // columns beyond N carry zeros
-          red_shared(col_slot(it & 1, 1, col0 + lane), sw_);
-        }
-        flush_cols(it, 0, p.g_bL, p.g_wo);
-        continue;
-      }
 #pragma unroll 1
       for (int c = half; (c >> 1) < nblk; c += 2) {
         stage_block(c >> 1);
@@ -770,7 +640,7 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
             if (p.colsum != nullptr) {
               // bias gradient: per-column sum over this warp's 32 rows, accumulated per CTA in shared memory
               const float s = warp_colsum_32x32(v, lane);
-              red_shared(col_slot(it & 1, 0, c * 32 + lane), s);     // columns beyond N / rows beyond M were zeroed above
+              red_shared(col_slot(it & 1, c * 32 + lane), s);     // columns beyond N / rows beyond M were zeroed above
             }
           }
         } else if constexpr (EPI == EPI_DW) {
@@ -815,7 +685,7 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
         }
       }
       if constexpr (EPI == EPI_DA) {
-        if (p.colsum != nullptr) flush_cols(it, tn, p.colsum, nullptr);
+        if (p.colsum != nullptr) flush_cols(it, tn, p.colsum);
       }
       if (w == w_first && threadIdx.x == 0) stamp(7);  // first tile's epilogue done
     }

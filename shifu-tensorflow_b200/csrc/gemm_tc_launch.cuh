@@ -4,7 +4,7 @@
 
 namespace sb {
 
-template <int BN, int EPI, bool A_MN, bool B_MN, int CG, int ACT_T = SB_ACT_AT_RUNTIME, bool GENERIC = false>
+template <int BN, int EPI, bool A_MN, bool B_MN, int CG, bool GENERIC = false>
 static int launch_gemm_tc_one(const GemmPlan& pl, const TmapSet& tms, const GemmTcParams& p, cudaStream_t st,
                               bool pdl) {
   using Cfg = GemmTcCfg<BN, CG, epi_tma_bytes(EPI, GENERIC)>;
@@ -27,21 +27,8 @@ static int launch_gemm_tc_one(const GemmPlan& pl, const TmapSet& tms, const Gemm
   }
   cfg.attrs = at;
   cfg.numAttrs = na;
-  SB_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, EPI, A_MN, B_MN, CG, ACT_T, GENERIC>, tms, p));
+  SB_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, EPI, A_MN, B_MN, CG, GENERIC>, tms, p));
   return SB_OK;
-}
-
-// EPI_FWD_OUT: one instantiation per (tile width 64 | 128 | 256, activation), single CTAs only
-template <int BN, bool A_MN, bool B_MN>
-static int launch_fwd_out_act(const GemmPlan& pl, const TmapSet& tms, const GemmTcParams& p, cudaStream_t st,
-                              bool pdl) {
-  switch (p.act) {
-    case SB_ACT_SIGMOID: return launch_gemm_tc_one<BN, EPI_FWD_OUT, A_MN, B_MN, 1, SB_ACT_SIGMOID>(pl, tms, p, st, pdl);
-    case SB_ACT_TANH: return launch_gemm_tc_one<BN, EPI_FWD_OUT, A_MN, B_MN, 1, SB_ACT_TANH>(pl, tms, p, st, pdl);
-    case SB_ACT_RELU: return launch_gemm_tc_one<BN, EPI_FWD_OUT, A_MN, B_MN, 1, SB_ACT_RELU>(pl, tms, p, st, pdl);
-    case SB_ACT_LEAKYRELU: return launch_gemm_tc_one<BN, EPI_FWD_OUT, A_MN, B_MN, 1, SB_ACT_LEAKYRELU>(pl, tms, p, st, pdl);
-    default: return launch_gemm_tc_one<BN, EPI_FWD_OUT, A_MN, B_MN, 1, SB_ACT_NONE>(pl, tms, p, st, pdl);
-  }
 }
 
 template <int EPI, bool A_MN, bool B_MN>
@@ -50,28 +37,14 @@ int launch_gemm_tc(const GemmPlan& pl, const TmapSet& tms, GemmTcParams p, cudaS
   if (p.n_pairs < 1) p.n_pairs = 1;
   p.split_k = pl.split_k;
   p.kb_per_split = pl.kb_per_split;
-  // split-precision parts or an fp32 addend: the GENERIC instantiations (the fused output layer reads its activation at run
-  // time there - three kernels instead of fifteen)
-  if constexpr (EPI == EPI_FWD || EPI == EPI_DA || EPI == EPI_FWD_OUT) {
+  // split-precision parts or an fp32 addend: the GENERIC instantiations
+  if constexpr (EPI == EPI_FWD || EPI == EPI_DA) {
     if (p.np > 1 || p.addend != nullptr) {
-      constexpr int ACT_G = SB_ACT_AT_RUNTIME;
-      if constexpr (EPI == EPI_FWD_OUT) {
-        if (pl.cg == 1 && pl.bn == 64) return launch_gemm_tc_one<64, EPI, A_MN, B_MN, 1, ACT_G, true>(pl, tms, p, st, pdl);
-        if (pl.cg == 1 && pl.bn == 128) return launch_gemm_tc_one<128, EPI, A_MN, B_MN, 1, ACT_G, true>(pl, tms, p, st, pdl);
-        if (pl.cg == 1 && pl.bn == 256) return launch_gemm_tc_one<256, EPI, A_MN, B_MN, 1, ACT_G, true>(pl, tms, p, st, pdl);
-      } else {
-        if (pl.cg == 1 && pl.bn == 64) return launch_gemm_tc_one<64, EPI, A_MN, B_MN, 1, ACT_G, true>(pl, tms, p, st, pdl);
-        if (pl.cg == 1 && pl.bn == 128) return launch_gemm_tc_one<128, EPI, A_MN, B_MN, 1, ACT_G, true>(pl, tms, p, st, pdl);
-      }
+      if (pl.cg == 1 && pl.bn == 64) return launch_gemm_tc_one<64, EPI, A_MN, B_MN, 1, true>(pl, tms, p, st, pdl);
+      if (pl.cg == 1 && pl.bn == 128) return launch_gemm_tc_one<128, EPI, A_MN, B_MN, 1, true>(pl, tms, p, st, pdl);
       return set_error(SB_ERR_INVALID, "no generic gemm_tc instantiation for cg=%d bn=%d", pl.cg, pl.bn);
     }
   }
-  if constexpr (EPI == EPI_FWD_OUT) {
-    if (pl.cg == 1 && pl.bn == 64) return launch_fwd_out_act<64, A_MN, B_MN>(pl, tms, p, st, pdl);
-    if (pl.cg == 1 && pl.bn == 128) return launch_fwd_out_act<128, A_MN, B_MN>(pl, tms, p, st, pdl);
-    if (pl.cg == 1 && pl.bn == 256) return launch_fwd_out_act<256, A_MN, B_MN>(pl, tms, p, st, pdl);
-    return set_error(SB_ERR_INVALID, "fused output layer: no instantiation for cg=%d bn=%d", pl.cg, pl.bn);
-  } else {
   if (pl.cg == 1 && pl.bn == 64) return launch_gemm_tc_one<64, EPI, A_MN, B_MN, 1>(pl, tms, p, st, pdl);
   if (pl.cg == 1 && pl.bn == 128) return launch_gemm_tc_one<128, EPI, A_MN, B_MN, 1>(pl, tms, p, st, pdl);
   if constexpr (EPI == EPI_F32) {   // CTA pairs: the tile-configuration hook's (the planner does not pick them)
@@ -79,28 +52,11 @@ int launch_gemm_tc(const GemmPlan& pl, const TmapSet& tms, GemmTcParams p, cudaS
   if (pl.cg == 2 && pl.bn == 256) return launch_gemm_tc_one<256, EPI, A_MN, B_MN, 2>(pl, tms, p, st, pdl);
   }
   return set_error(SB_ERR_INVALID, "no gemm_tc instantiation for cg=%d bn=%d", pl.cg, pl.bn);
-  }
 }
 
 // opt in to > 48 KB dynamic shared memory (once per process per instantiation, outside of stream capture)
 template <int EPI, bool A_MN, bool B_MN>
 int set_gemm_tc_attrs() {
-  if constexpr (EPI == EPI_FWD_OUT) {
-#define SB_ATTR_ACT(BN, ACT)                                                                                          \
-  SB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI_FWD_OUT, A_MN, B_MN, 1, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                               GemmTcCfg<BN, 1>::SMEM_BYTES))
-#define SB_ATTR_ALL(BN) SB_ATTR_ACT(BN, SB_ACT_NONE); SB_ATTR_ACT(BN, SB_ACT_SIGMOID); SB_ATTR_ACT(BN, SB_ACT_TANH); \
-                        SB_ATTR_ACT(BN, SB_ACT_RELU); SB_ATTR_ACT(BN, SB_ACT_LEAKYRELU)
-    SB_ATTR_ALL(64); SB_ATTR_ALL(128); SB_ATTR_ALL(256);
-#undef SB_ATTR_ALL
-#undef SB_ATTR_ACT
-#define SB_ATTR_G(BN)                                                                                                \
-  SB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI_FWD_OUT, A_MN, B_MN, 1, SB_ACT_AT_RUNTIME, true>,              \
-                               cudaFuncAttributeMaxDynamicSharedMemorySize, GemmTcCfg<BN, 1>::SMEM_BYTES))
-    SB_ATTR_G(64); SB_ATTR_G(128); SB_ATTR_G(256);
-#undef SB_ATTR_G
-    return SB_OK;
-  } else {
 #define SB_ATTR(BN, CG)                                                                                            \
   SB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI, A_MN, B_MN, CG>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
                                (GemmTcCfg<BN, CG, epi_tma_bytes(EPI, false)>::SMEM_BYTES)))
@@ -109,13 +65,12 @@ int set_gemm_tc_attrs() {
 #undef SB_ATTR
   if constexpr (EPI == EPI_FWD || EPI == EPI_DA) {
 #define SB_ATTR_G(BN, CG)                                                                                            \
-  SB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI, A_MN, B_MN, CG, SB_ACT_AT_RUNTIME, true>,                      \
+  SB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI, A_MN, B_MN, CG, true>,                                        \
                                cudaFuncAttributeMaxDynamicSharedMemorySize, GemmTcCfg<BN, CG>::SMEM_BYTES))
     SB_ATTR_G(64, 1); SB_ATTR_G(128, 1);
 #undef SB_ATTR_G
   }
   return SB_OK;
-  }
 }
 
 // box rows of the tensor map of a K-major B operand / tile geometry helpers

@@ -6,6 +6,7 @@
 #include <algorithm>
 #include "net.cuh"
 #include "gemm_tc_launch.cuh"
+#include "gemm_fwd_out.cuh"
 
 namespace sb {
 
@@ -69,8 +70,10 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rows, int cols, int l
 
 // Tile configuration (persistent grid, one CTA per SM, 128 x BN tiles):
 //   - BN = 128 (64 for a layer at most 64 wide).  A 128 x 256 tile would fetch fewer operand bytes per flop, but its
-//     128-register accumulator plus the epilogue does not fit the consumer threads' registers without spills; only the
-//     fused output layer, which needs whole rows, uses it;
+//     128-register accumulator plus the epilogue does not fit the consumer threads' registers without spills.  The fused
+//     output layer (gemm_fwd_out.cuh) is planned apart: it needs whole rows of A_L in one CTA, so it takes 64 x h_L tiles
+//     (h_L <= 256, the two consumer warpgroups split the columns: 64 accumulator registers per thread) and
+//     ceil(rows / 64) CTAs - twice the CTAs a 128-row tile would give the narrow last layer;
 //   - no CTA pairs: the 256 x BN cluster tile with B multicast (cg = 2, gemm_tc.cuh) is the tile-configuration hook's,
 //     instantiated with the fp32 test epilogue only;
 //   - split-K (dW GEMMs, reduction over the batch): fill the machine but keep >= 8 k-blocks per split.
@@ -272,7 +275,7 @@ int Net::init(const sb_net_desc* d, int device_, bool training_) {
   // opt in to > 48 KB dynamic shared memory once, outside of any stream capture
   if (bf) {
     SB_TRY((set_gemm_tc_attrs<EPI_FWD, false, true>()));
-    SB_TRY((set_gemm_tc_attrs<EPI_FWD_OUT, false, true>()));
+    SB_TRY(set_gemm_fwd_out_attrs());
     SB_TRY((set_gemm_tc_attrs<EPI_DA, false, false>()));
     SB_TRY((set_gemm_tc_attrs<EPI_DW, true, true>()));
     // keep the SMs in the GEMMs' shared-memory carve-out for every kernel of the step, so that no launch in the chain
@@ -400,24 +403,20 @@ int Net::enqueue_hidden_forward(int rows, float* grad, bool* fused_out) {
       p.bias = theta + ly.b_off; p.act = ly.act;
       p.out = A[l]; p.ld_out = ly.ld_out; p.out_ps = A_ps[l];
       p.a_rows = res0 ? desc : nullptr;
-      if (l == L - 1 && grad != nullptr && fuse_out_layer && training && ly.out <= fuse_out_max) {
-        // K2 + K3 + K4 + output backward in one kernel: one n-tile must cover the whole layer width
-        GemmPlan fp = pl;
-        fp.split_k = 1; fp.kb_per_split = ((k_in + 63) / 64) * pairs_of(nparts);
-        // (the 128 x 256 tile keeps whole rows of A_L in one CTA's accumulator and needs no second kernel)
-        if (ly.out <= 64) { fp.cg = 1; fp.bn = 64; }
-        else if (ly.out <= 128) { fp.cg = 1; fp.bn = 128; }
-        else { fp.cg = 1; fp.bn = 256; }
-        const int slots = gemm_sms / fp.cg;
-        const int tiles = (rows + 128 * fp.cg - 1) / (128 * fp.cg);
-        fp.grid = (tiles < slots ? tiles : slots) * fp.cg;
+      if (l == L - 1 && grad != nullptr && fuse_out_layer && training && ly.out <= fuse_out_max && p.addend == nullptr) {
+        // K2 + K3 + K4 + output backward in one kernel (gemm_fwd_out.cuh): 64-row tiles of whole rows of A_L
+        FwdOutTmaps ft;
+        SB_TRY(make_tmaps_bf16(ft.a, src, src_ps, nparts, res0 ? static_cast<int>(resident_rows) : rows, k_in, ld_k, 64));
+        for (int i = 0; i < 3; ++i) ft.b[i] = tm.b[i];
+        SB_TRY(make_tmaps_bf16(ft.o, dZ[l], A_ps[l], nparts, rows, ly.out, ly.ld_out, 64));
+        const int tiles = (rows + 63) / 64;
+        const int grid = tiles < gemm_sms ? tiles : gemm_sms;
         Layer& ol = layers[L];
-        p.out = dZ[l];
         p.wo = theta + ol.w_off; p.bo = theta + ol.b_off;
         p.desc = desc; p.scal = scal; p.loss = loss;
         p.g_wo = grad + ol.w_off; p.g_bo = grad + ol.b_off; p.g_bL = grad + ly.b_off;
         p.trace = next_trace("fwd_out", l, rows, ly.out, k_in);
-        SB_TRY((launch_gemm_tc<EPI_FWD_OUT, false, true>(fp, tm, p, stream, use_pdl)));
+        SB_TRY(launch_gemm_fwd_out(grid, ft, p, stream, use_pdl));
         if (fused_out) *fused_out = true;
         mark("gemm_fwd_out");
         continue;

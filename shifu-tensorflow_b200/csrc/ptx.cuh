@@ -90,7 +90,17 @@ __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sy
 #define SB_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
 template <int N, int TA, int TB>
 __device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
-  static_assert(N == 64 || N == 128 || N == 256, "wgmma N");
+  static_assert(N == 32 || N == 64 || N == 128 || N == 256, "wgmma N");
+  if constexpr (N == 32) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "%16, %17, p, 1, 1, %19, %20;\n\t}"
+        : SB_F8(0), SB_F8(8)
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d), "n"(TA), "n"(TB));
+  }
   if constexpr (N == 64) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
