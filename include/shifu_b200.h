@@ -315,6 +315,18 @@ int sb_debug_gemm_bench(const float* A, const float* B, float* D, int32_t M, int
                         int32_t a_mn, int32_t b_mn, int32_t cfg_cg, int32_t cfg_bn, int device, int32_t iters,
                         float* ms_out);
 
+/* One plain-bf16 forward (da = 0) or dA (da = 1) GEMM of a training step through the kernel the step plans for it, with
+ * its fused epilogue.  Operands are fp32 on the host, rounded to bf16 on the device:
+ *   forward: out = bf16(act(A W + bias))               A [M,K], W [K,N], bias [N]
+ *   dA     : out = bf16((A W^T) * act'(aux)),          A [M,K], W [N,K], aux [M,N] (an activation output);
+ *            colsum[N] = column sums of the fp32 product before rounding (nullable)
+ * out [M,N] receives the bf16 results widened to fp32.  bm_wg = 0 lets the planner choose the rows of a warpgroup tile,
+ * 64 or 128 forces them.  iters > 0: afterwards, average device milliseconds per launch over `iters` back-to-back
+ * launches into *ms_out. */
+int sb_debug_gemm_epilogue(const float* A, const float* W, const float* bias, const float* aux, float* out, float* colsum,
+                           int32_t M, int32_t N, int32_t K, int32_t da, int32_t act, int32_t bm_wg, int device,
+                           int32_t iters, float* ms_out);
+
 #ifdef __cplusplus
 }
 #endif

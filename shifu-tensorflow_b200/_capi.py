@@ -154,6 +154,8 @@ PROTOTYPES = {
                                       C.c_int32, C.c_int32, C.c_int, C.c_int32, _f32p]),
     "sb_debug_gemm_bf16_cfg": (C.c_int, [_f32p, _f32p, _f32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                          C.c_int32, C.c_int32, C.c_int]),
+    "sb_debug_gemm_epilogue": (C.c_int, [_f32p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                         C.c_int32, C.c_int32, C.c_int, C.c_int32, _f32p]),
 }
 
 
@@ -610,6 +612,26 @@ def debug_gemm_bench(M: int, N: int, K: int, split_k: int = 1, a_mn: bool = Fals
     check(lib().sb_debug_gemm_bench(_ptr(A), _ptr(B), _ptr(D), M, N, K, split_k, int(a_mn), int(b_mn), cg, bn, device,
                                     iters, C.byref(ms)))
     return float(ms.value)
+
+
+def debug_gemm_epilogue(A: np.ndarray, W: np.ndarray, act: int, bias: Optional[np.ndarray] = None,
+                        aux: Optional[np.ndarray] = None, bm_wg: int = 0, iters: int = 0, device: int = 0):
+    """One plain-bf16 forward (aux None: act(A W + bias), W [K,N]) or dA (aux given: (A W^T) * act'(aux), W [N,K]) GEMM
+    with its fused epilogue -> (out [M,N] fp32 of the bf16 results, column sums [N] or None, ms per launch or None)"""
+    A, W = _f32(A), _f32(W)
+    M, K = A.shape
+    da = aux is not None
+    N = W.shape[0] if da else W.shape[1]
+    assert W.shape == ((N, K) if da else (K, N))
+    bias = _f32(bias) if bias is not None else None
+    aux = _f32(aux) if da else None
+    out = np.zeros((M, N), np.float32)
+    cs = np.zeros(N, np.float32) if da else None
+    ms = C.c_float()
+    check(lib().sb_debug_gemm_epilogue(_ptr(A), _ptr(W), _ptr(bias) if bias is not None else None,
+                                       _ptr(aux) if da else None, _ptr(out), _ptr(cs) if da else None, M, N, K, int(da),
+                                       act, bm_wg, device, iters, C.byref(ms)))
+    return out, cs, (float(ms.value) if iters > 0 else None)
 
 
 def text_parse_device(text: bytes, col_map: Sequence[int], n_feat: int, delim: str = "|", device: int = 0, flag_cap: int = 65536):

@@ -8,6 +8,7 @@
 #include <random>
 #include "net.cuh"
 #include "gemm_tc_launch.cuh"
+#include "gemm_pp.cuh"
 #include "savedmodel.h"
 #include "xchg_p2p.cuh"
 
@@ -1789,17 +1790,22 @@ static int debug_gemm_impl(const float* A, const float* B, float* D, int32_t M, 
       GemmTcParams q = p;
       q.bias = d_bias; q.act = SB_ACT_RELU; q.out = d_out; q.ld_out = ldn; q.aux = d_aux; q.ld_aux = ldn; q.colsum = d_colsum;
       q.acc_vec4 = (N % 4 == 0) ? 1 : 0;
-      if (s == SB_OK) s = make_tmap_bf16(&tms.o, d_out, M, N, ldn, 128);
-      if (s == SB_OK) s = make_tmap_bf16(&tms.x, d_aux, M, N, ldn, 128);
+      // KM / KK: the ping-pong kernel the step plans for the shape
+      const PpPlan pp = plan_gemm_pp(M, N, K, prop.multiProcessorCount);
+      PpTmaps pt;
+      if (!a_mn) {
+        if (s == SB_OK) s = make_tmap_bf16(&pt.a, dA, a_rows, a_cols, lda, pp.bm_wg);
+        if (s == SB_OK) s = make_tmap_bf16(&pt.b, dB, b_rows, b_cols, ldb, b_mn ? 64 : pp.bn);
+        if (s == SB_OK) s = make_tmap_bf16(&pt.o, d_out, M, N, ldn, pp.bm_wg);
+        if (s == SB_OK) s = make_tmap_bf16(&pt.x, d_aux, M, N, ldn, pp.bm_wg);
+      }
       const bool bench_pdl = getenv("SB_BENCH_PDL") != nullptr;
       auto real = [&]() -> int {
-        if (!a_mn && !b_mn) return launch_gemm_tc<EPI_DA, false, false>(pl, tms, q, 0, bench_pdl);
-        if (!a_mn) return launch_gemm_tc<EPI_FWD, false, true>(pl, tms, q, 0, bench_pdl);
+        if (!a_mn && !b_mn) return launch_gemm_pp<EPI_DA>(pp, pt, q, 0, bench_pdl);
+        if (!a_mn) return launch_gemm_pp<EPI_FWD>(pp, pt, q, 0, bench_pdl);
         return launch_gemm_tc<EPI_DW, true, true>(pl, tms, q, 0, bench_pdl);
       };
-      if (!a_mn && !b_mn) s = set_gemm_tc_attrs<EPI_DA, false, false>();
-      else if (!a_mn) s = set_gemm_tc_attrs<EPI_FWD, false, true>();
-      else s = set_gemm_tc_attrs<EPI_DW, true, true>();
+      if (s == SB_OK) s = a_mn ? set_gemm_tc_attrs<EPI_DW, true, true>() : set_gemm_pp_attrs();
       cudaEvent_t e0, e1;
       cudaEventCreate(&e0); cudaEventCreate(&e1);
       for (int i = 0; i < 3 && s == SB_OK; ++i) s = real();
@@ -1829,8 +1835,12 @@ static int debug_gemm_impl(const float* A, const float* B, float* D, int32_t M, 
         cudaEventElapsedTime(&one, t0, t1);
         unsigned long long h[16];
         cudaMemcpy(h, d_tr, sizeof(h), cudaMemcpyDeviceToHost);
-        fprintf(stderr, "[trace] M=%d N=%d K=%d cg=%d bn=%d split=%d single-launch %.2f us | ns since entry:", M, N, K, pl.cg, pl.bn,
-                pl.split_k, one * 1e3f);
+        if (a_mn)
+          fprintf(stderr, "[trace] M=%d N=%d K=%d cg=%d bn=%d split=%d single-launch %.2f us | ns since entry:", M, N, K, pl.cg, pl.bn,
+                  pl.split_k, one * 1e3f);
+        else
+          fprintf(stderr, "[trace] M=%d N=%d K=%d ping-pong bm_wg=%d bn=%d single-launch %.2f us | ns since entry:", M, N, K, pp.bm_wg,
+                  pp.bn, one * 1e3f);
         const char* nm[9] = {"entry", "setup", "deps", "tma0", "land0", "mma_done", "acc_ready", "epi_done", "exit"};
         for (int i = 1; i < 9; ++i) fprintf(stderr, " %s=%lld", nm[i], (long long)(h[i] - h[0]));
         fprintf(stderr, "\n");
@@ -1902,6 +1912,97 @@ int sb_debug_gemm_bf16_ex(const float* A, const float* B, float* D, int32_t M, i
 }
 int sb_debug_gemm_bf16(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K, int32_t split_k, int device) {
   return sb_debug_gemm_bf16_cfg(A, B, D, M, N, K, split_k, 0, 0, 0, 0, device);
+}
+
+int sb_debug_gemm_epilogue(const float* A, const float* W, const float* bias, const float* aux, float* out, float* colsum,
+                           int32_t M, int32_t N, int32_t K, int32_t da, int32_t act, int32_t bm_wg, int device,
+                           int32_t iters, float* ms_out) {
+  SB_CHECK(A && W && out && M > 0 && N > 0 && K > 0 && (da == 0 || da == 1), SB_ERR_INVALID, "bad argument");
+  SB_CHECK(da ? aux != nullptr : bias != nullptr, SB_ERR_INVALID, "the forward GEMM needs a bias, the dA GEMM an aux matrix");
+  SB_CHECK(act >= SB_ACT_NONE && act <= SB_ACT_LEAKYRELU, SB_ERR_INVALID, "act invalid");
+  SB_CHECK(bm_wg == 0 || bm_wg == 64 || bm_wg == 128, SB_ERR_INVALID, "bm_wg must be 0, 64 or 128 (got %d)", bm_wg);
+  SB_CHECK(iters >= 0 && (iters == 0 || ms_out != nullptr), SB_ERR_INVALID, "iters / ms_out");
+  int n_dev = 0;
+  SB_CHECK(cudaGetDeviceCount(&n_dev) == cudaSuccess && n_dev > 0, SB_ERR_CUDA, "no CUDA device available");
+  cudaDeviceProp prop;
+  SB_CUDA(cudaGetDeviceProperties(&prop, device));
+  SB_CHECK(prop.major == 9 && prop.minor == 0, SB_ERR_CUDA, "device is sm_%d%d, need sm_90", prop.major, prop.minor);
+  SB_CUDA(cudaSetDevice(device));
+  // stored shapes: A [M, K]; W [K, N] (forward, MN-major operand) or [N, K] (dA, K-major operand)
+  const int w_rows = da ? N : K, w_cols = da ? K : N;
+  const int lda = round_up(K, 8), ldw = round_up(w_cols, 8), ldn = round_up(N, 8);
+  const size_t mn = static_cast<size_t>(M) * N;
+  float *dA32 = nullptr, *dW32 = nullptr, *dX32 = nullptr, *d_bias = nullptr, *d_col = nullptr;
+  __nv_bfloat16 *dA = nullptr, *dW = nullptr, *d_out = nullptr, *d_aux = nullptr;
+  SB_CUDA(cudaMalloc(&dA32, sizeof(float) * M * K));
+  SB_CUDA(cudaMalloc(&dW32, sizeof(float) * N * K));
+  SB_CUDA(cudaMalloc(&dX32, sizeof(float) * mn));
+  SB_CUDA(cudaMalloc(&d_bias, sizeof(float) * N));
+  SB_CUDA(cudaMalloc(&d_col, sizeof(float) * N));
+  SB_CUDA(cudaMalloc(&dA, sizeof(__nv_bfloat16) * M * lda));
+  SB_CUDA(cudaMalloc(&dW, sizeof(__nv_bfloat16) * w_rows * ldw));
+  SB_CUDA(cudaMalloc(&d_out, sizeof(__nv_bfloat16) * M * ldn));
+  SB_CUDA(cudaMalloc(&d_aux, sizeof(__nv_bfloat16) * M * ldn));
+  SB_CUDA(cudaMemset(dA, 0, sizeof(__nv_bfloat16) * M * lda));
+  SB_CUDA(cudaMemset(dW, 0, sizeof(__nv_bfloat16) * w_rows * ldw));
+  SB_CUDA(cudaMemset(d_out, 0, sizeof(__nv_bfloat16) * M * ldn));
+  SB_CUDA(cudaMemset(d_aux, 0, sizeof(__nv_bfloat16) * M * ldn));
+  SB_CUDA(cudaMemset(d_bias, 0, sizeof(float) * N));
+  SB_CUDA(cudaMemset(d_col, 0, sizeof(float) * N));
+  SB_CUDA(cudaMemcpy(dA32, A, sizeof(float) * M * K, cudaMemcpyHostToDevice));
+  SB_CUDA(cudaMemcpy(dW32, W, sizeof(float) * N * K, cudaMemcpyHostToDevice));
+  if (bias) SB_CUDA(cudaMemcpy(d_bias, bias, sizeof(float) * N, cudaMemcpyHostToDevice));
+  cast_bf16_kernel<<<static_cast<unsigned>((static_cast<long long>(M) * K + 255) / 256), 256>>>(dA32, M, K, dA, lda);
+  cast_bf16_kernel<<<static_cast<unsigned>((static_cast<long long>(N) * K + 255) / 256), 256>>>(dW32, w_rows, w_cols, dW, ldw);
+  if (aux) {
+    SB_CUDA(cudaMemcpy(dX32, aux, sizeof(float) * mn, cudaMemcpyHostToDevice));
+    cast_bf16_kernel<<<static_cast<unsigned>((mn + 255) / 256), 256>>>(dX32, M, N, d_aux, ldn);
+  }
+  const PpPlan pp = plan_gemm_pp(M, N, K, prop.multiProcessorCount, bm_wg);
+  PpTmaps pt;
+  int s = make_tmap_bf16(&pt.a, dA, M, K, lda, pp.bm_wg);
+  if (s == SB_OK) s = make_tmap_bf16(&pt.b, dW, w_rows, w_cols, ldw, da ? pp.bn : 64);
+  if (s == SB_OK) s = make_tmap_bf16(&pt.o, d_out, M, N, ldn, pp.bm_wg);
+  if (s == SB_OK) s = make_tmap_bf16(&pt.x, d_aux, M, N, ldn, pp.bm_wg);
+  GemmTcParams p = {};
+  p.M = M; p.N = N; p.K = K;
+  p.act = act; p.bias = d_bias; p.colsum = colsum ? d_col : nullptr;
+  auto launch = [&]() { return da ? launch_gemm_pp<EPI_DA>(pp, pt, p, 0, false) : launch_gemm_pp<EPI_FWD>(pp, pt, p, 0, false); };
+  if (s == SB_OK) s = set_gemm_pp_attrs();
+  if (s == SB_OK) s = launch();
+  if (s == SB_OK) {
+    cudaError_t e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) s = set_error(SB_ERR_CUDA, "gemm_pp_kernel failed: %s", cudaGetErrorString(e));
+  }
+  if (s == SB_OK) {
+    std::vector<uint16_t> h(static_cast<size_t>(M) * ldn);
+    if (cudaMemcpy(h.data(), d_out, sizeof(uint16_t) * h.size(), cudaMemcpyDeviceToHost) != cudaSuccess) s = set_error(SB_ERR_CUDA, "D2H failed");
+    for (int r = 0; r < M && s == SB_OK; ++r)
+      for (int c = 0; c < N; ++c) {
+        const uint32_t u = static_cast<uint32_t>(h[static_cast<size_t>(r) * ldn + c]) << 16;   // bf16 -> fp32, exact
+        memcpy(out + static_cast<size_t>(r) * N + c, &u, 4);
+      }
+    if (s == SB_OK && colsum && cudaMemcpy(colsum, d_col, sizeof(float) * N, cudaMemcpyDeviceToHost) != cudaSuccess)
+      s = set_error(SB_ERR_CUDA, "D2H failed");
+  }
+  if (s == SB_OK && iters > 0) {
+    cudaEvent_t e0, e1;
+    cudaEventCreate(&e0); cudaEventCreate(&e1);
+    for (int i = 0; i < 3 && s == SB_OK; ++i) s = launch();
+    cudaEventRecord(e0, 0);
+    for (int i = 0; i < iters && s == SB_OK; ++i) s = launch();
+    cudaEventRecord(e1, 0);
+    cudaEventSynchronize(e1);
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, e0, e1);
+    *ms_out = ms / iters;
+    cudaEventDestroy(e0); cudaEventDestroy(e1);
+    cudaError_t e = cudaDeviceSynchronize();
+    if (s == SB_OK && e != cudaSuccess) s = set_error(SB_ERR_CUDA, "gemm_pp_kernel failed: %s", cudaGetErrorString(e));
+  }
+  cudaFree(dA32); cudaFree(dW32); cudaFree(dX32); cudaFree(d_bias); cudaFree(d_col);
+  cudaFree(dA); cudaFree(dW); cudaFree(d_out); cudaFree(d_aux);
+  return s;
 }
 
 }  // extern "C"

@@ -88,4 +88,25 @@ __device__ __forceinline__ float warp_colsum_32x32(float (&v)[32], int lane) {
   return v[0];
 }
 
+// Sums of N_ column values over the 8 row groups of a warp (lane bits 2..4) of a wgmma accumulator fragment.  Every round
+// sends half of the values that are still open to the partner lane and keeps the other half, so on return lane l holds
+// the complete sums of the N_ / 8 values q N_ / 8 .. q N_ / 8 + N_ / 8 - 1, q = l / 4, in v[0 .. N_ / 8 - 1].
+template <int LEN, int N_>
+__device__ __forceinline__ void colsum_halve(float (&v)[N_], int lane, int m) {   // one round: v[0 .. 2 LEN) -> v[0 .. LEN)
+  const bool upper = (lane & m) != 0;
+#pragma unroll
+  for (int i = 0; i < LEN; ++i) {
+    const float send = upper ? v[i] : v[i + LEN];
+    const float keep = upper ? v[i + LEN] : v[i];
+    v[i] = keep + __shfl_xor_sync(0xffffffffu, send, m);
+  }
+}
+template <int N_>
+__device__ __forceinline__ void colsum_row_groups(float (&v)[N_], int lane) {
+  static_assert(N_ % 8 == 0, "three halving rounds");
+  colsum_halve<N_ / 2>(v, lane, 16);
+  colsum_halve<N_ / 4>(v, lane, 8);
+  colsum_halve<N_ / 8>(v, lane, 4);
+}
+
 }  // namespace sb

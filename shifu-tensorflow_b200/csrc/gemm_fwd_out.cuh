@@ -13,8 +13,9 @@
 //   row dot products  : per-thread partials, shuffle over the 4 lanes of a row, the two warpgroups' halves through shared
 //                       memory (one consumer barrier)
 //   column sums       : each thread adds its two rows, a reduce-scatter over the 8 row groups of the warp (3 shuffle
-//                       rounds that halve the data each time), red.shared across the 4 warps of the group; flushed to
-//                       the flat gradient once per CTA
+//                       rounds that halve the data each time), red.shared into the warp's own slots; the 4 slots are
+//                       added in a fixed order and flushed to the flat gradient once per CTA (as are the loss sum and
+//                       db_o), so a step's result does not depend on warp timing
 //   dZ_L              : bf16 pairs into BN/64 128-byte-swizzled 64 x 64 tiles (the output tensor map's layout; conflict
 //                       free for the fragment), one cp.async.bulk.tensor store per tile
 // Producer warpgroup, operand ring, TMA zero fill of the M / N / K tails, setmaxnreg split and PDL as in gemm_tc.cuh.
@@ -40,8 +41,9 @@ struct FwdOutCfg {
   static constexpr int B_BYTES = BN * BK * 2;       // BN / 64 MN-major 64 x 64 boxes
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int X_BYTES = BM * BN * 2;       // dZ_L staging tiles
-  // besides the ring: align slack, barriers, bias + w_o, the two column-sum arrays, z partials [tile parity][group][64]
-  static constexpr int FIXED_BYTES = 1024 + 256 + 2 * BN * 4 + 2 * BN * 4 + 2 * 2 * BM * 4 + X_BYTES;
+  // besides the ring: align slack, barriers, bias + w_o, the two column-sum arrays per warp of a group, z partials
+  // [tile parity][group][64], loss / db_o per warp of group 0
+  static constexpr int FIXED_BYTES = 1024 + 256 + 2 * BN * 4 + 4 * 2 * BN * 4 + 2 * 2 * BM * 4 + 32 + X_BYTES;
   static constexpr int RING_BUDGET = 232448 - FIXED_BYTES;   // 227 KB of dynamic shared memory per block
   static constexpr int STAGES = RING_BUDGET / STAGE_BYTES > 8 ? 8 : RING_BUDGET / STAGE_BYTES;
   static_assert(STAGES >= 4, "operand ring");
@@ -52,27 +54,6 @@ struct FwdOutCfg {
   static constexpr int CONSUMER_REGS = 232;
   static constexpr int PRODUCER_REGS = 40;
 };
-
-// Sums of N_ column values over the 8 row groups of a warp (lane bits 2..4).  Every round sends half of the values that
-// are still open to the partner lane and keeps the other half, so on return lane l holds the complete sums of the
-// N_ / 8 values q N_ / 8 .. q N_ / 8 + N_ / 8 - 1, q = l / 4, in v[0 .. N_ / 8 - 1].
-template <int LEN, int N_>
-__device__ __forceinline__ void colsum_halve(float (&v)[N_], int lane, int m) {   // one round: v[0 .. 2 LEN) -> v[0 .. LEN)
-  const bool upper = (lane & m) != 0;
-#pragma unroll
-  for (int i = 0; i < LEN; ++i) {
-    const float send = upper ? v[i] : v[i + LEN];
-    const float keep = upper ? v[i + LEN] : v[i];
-    v[i] = keep + __shfl_xor_sync(0xffffffffu, send, m);
-  }
-}
-template <int N_>
-__device__ __forceinline__ void colsum_row_groups(float (&v)[N_], int lane) {
-  static_assert(N_ % 8 == 0, "three halving rounds");
-  colsum_halve<N_ / 2>(v, lane, 16);
-  colsum_halve<N_ / 4>(v, lane, 8);
-  colsum_halve<N_ / 8>(v, lane, 4);
-}
 
 template <int BN, int ACT>
 __global__ void __launch_bounds__(FwdOutCfg<BN>::THREADS, 1)
@@ -85,8 +66,9 @@ gemm_fwd_out_kernel(const __grid_constant__ FwdOutTmaps tms, const GemmTcParams 
   const uint32_t xs_base = smem_base + STAGES * Cfg::STAGE_BYTES;     // dZ_L staging tiles (1024-byte aligned)
   const uint32_t bar_base = xs_base + Cfg::X_BYTES;                   // full[STAGES], empty[STAGES] (8 B each)
   const uint32_t sm_vec = bar_base + 256u;                            // [bias BN][w_o BN] fp32, 0 beyond N
-  const uint32_t sm_col = sm_vec + 2u * BN * 4u;                      // [db_L BN][dw_o BN] fp32 column sums
-  const uint32_t sm_z = sm_col + 2u * BN * 4u;                        // z partials [tile parity][group][64 rows]
+  const uint32_t sm_col = sm_vec + 2u * BN * 4u;                      // [warp & 3][db_L BN][dw_o BN] fp32 column sums
+  const uint32_t sm_z = sm_col + 4u * 2u * BN * 4u;                   // z partials [tile parity][group][64 rows]
+  const uint32_t sm_lw = sm_z + 2u * 2u * BM * 4u;                    // [warp][loss, db_o] of group 0
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
   auto smem_a = [&](int s) { return smem_base + s * Cfg::STAGE_BYTES; };
@@ -163,8 +145,8 @@ gemm_fwd_out_kernel(const __grid_constant__ FwdOutTmaps tms, const GemmTcParams 
       const int col = j < BN ? j : j - BN;
       const float* src = j < BN ? p.bias : p.wo;
       sts(sm_vec + static_cast<uint32_t>(j) * 4u, col < p.N ? __ldg(src + col) : 0.f);
-      sts(sm_col + static_cast<uint32_t>(j) * 4u, 0.f);
     }
+    for (int j = et; j < 4 * 2 * BN; j += Cfg::EPI_THREADS) sts(sm_col + static_cast<uint32_t>(j) * 4u, 0.f);
     bar_all();
     const float b_o = __ldg(p.bo);
     const float nnz = p.scal[SCAL_NNZ];
@@ -283,15 +265,16 @@ gemm_fwd_out_kernel(const __grid_constant__ FwdOutTmaps tms, const GemmTcParams 
           acc[4 * i + 2 + e] = g1;
         }
       }
-      // ---------- (5) over the warp's 16 rows, then across the group's 4 warps in shared memory ----------
+      // ---------- (5) over the warp's 16 rows, then into the warp's slots (one writer per address) ----------
       colsum_row_groups(sdb, lane);
       colsum_row_groups(sdw, lane);
+      const uint32_t cw = sm_col + static_cast<uint32_t>(warp & 3) * 2u * BN * 4u;
 #pragma unroll
       for (int j = 0; j < WN / 32; ++j) {
         const int k = (lane >> 2) * (WN / 32) + j;   // value index 2 i + e of the thread's columns
         const uint32_t col = static_cast<uint32_t>(c0 + 8 * (k >> 1) + (k & 1));
-        asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(sm_col + col * 4u), "f"(sdb[j]) : "memory");
-        asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(sm_col + (BN + col) * 4u), "f"(sdw[j]) : "memory");
+        asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(cw + col * 4u), "f"(sdb[j]) : "memory");
+        asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(cw + (BN + col) * 4u), "f"(sdw[j]) : "memory");
       }
 
       // ---------- (6) dZ_L: bf16, TMA store.  Split modes: part k = bf16 of the residual after parts 0..k-1 (acc keeps
@@ -325,14 +308,24 @@ gemm_fwd_out_kernel(const __grid_constant__ FwdOutTmaps tms, const GemmTcParams 
       }
       if (it == 0 && threadIdx.x == 0) stamp(7);  // first tile's epilogue done
     }
-    // loss sum and db_o: one atomic pair per warp; db_L / dw_o: one red.global per column and CTA
+    // loss sum and db_o: one atomic pair per CTA; db_L / dw_o: one red.global per column and CTA (warps added in order)
     if (wg == 0) {
       const float ls = warp_sum(loss_acc), ds = warp_sum(dz_acc);
-      if (lane == 0) { atomicAdd(p.scal + SCAL_LOSS_SUM, ls); atomicAdd(p.g_bo, ds); }
+      if (lane == 0) { sts(sm_lw + warp * 8u, ls); sts(sm_lw + warp * 8u + 4u, ds); }
     }
     bar_all();
+    if (et == 0) {
+      float ls = 0.f, ds = 0.f;
+      for (int w = 0; w < 4; ++w) { ls += lds(sm_lw + w * 8u); ds += lds(sm_lw + w * 8u + 4u); }
+      atomicAdd(p.scal + SCAL_LOSS_SUM, ls);
+      atomicAdd(p.g_bo, ds);
+    }
     for (int j = et; j < BN && j < p.N; j += Cfg::EPI_THREADS) {
-      const float db = lds(sm_col + static_cast<uint32_t>(j) * 4u), dw = lds(sm_col + static_cast<uint32_t>(BN + j) * 4u);
+      float db = 0.f, dw = 0.f;
+      for (int w = 0; w < 4; ++w) {
+        db += lds(sm_col + static_cast<uint32_t>(w * 2 * BN + j) * 4u);
+        dw += lds(sm_col + static_cast<uint32_t>(w * 2 * BN + BN + j) * 4u);
+      }
       if (db != 0.f) red_add_f32(p.g_bL + j, db);
       if (dw != 0.f) red_add_f32(p.g_wo + j, dw);
     }

@@ -1,0 +1,382 @@
+// Ping-pong wgmma / TMA GEMM for the plain-bf16 forward and dA GEMMs of a training step and the forward GEMMs of scoring:
+//   EPI_FWD : A_l      = act(A_{l-1} W_l + b_l)                 A K-major [rows, in], B = W_l [in, out] MN-major
+//   EPI_DA  : dZ_{l-1} = (dZ_l W_l^T) * act'(A_{l-1}),  db_{l-1} += column sums     A K-major [rows, out], B = W_l K-major
+//
+// Structure (persistent, one CTA per SM, 384 threads = three warpgroups):
+//   warps 8..11: producer warpgroup; one thread fills a STAGES-deep ring of 128-byte-swizzled TMA tiles with the k-blocks of
+//                the CTA's tiles in tile order.  Its other three warps clear the step's gradient buffer when asked to.
+//   warps 0..7 : two consumer warpgroups.  Each owns WHOLE tiles of BM_WG x BN: the CTA's tiles alternate between them
+//                (local tile 0, 2, 4, ... -> group 0; 1, 3, 5, ... -> group 1).  A group skips the other's k-blocks when it
+//                advances its ring position.  An ordered pair of named barriers makes the groups take turns issuing their
+//                main loops, so one group's wgmma run while the other runs its epilogue: the tensor cores are not idle
+//                for the length of an epilogue, and the epilogue no longer shares the SM with its own group's next fill.
+// Accumulator: BM_WG / 64 wgmma.m64nBNk16 per k16 step (128 registers per thread at 128 x 128).
+// Epilogues run in the wgmma fragment layout (thread = warp w of the group, lane l: rows 64 mi + 16 w + l / 4 (+ 8),
+// columns 8 i + 2 (l % 4) + {0, 1}); nothing fp32 is staged through shared memory.  Each group has one epilogue buffer of
+// BM_WG x BN bf16: BN / 64 tiles of BM_WG x 64 in the 128-byte swizzle the output tensor map expects.  A bf16 pair per
+// thread and n8 block is a conflict-free 4-byte access in that layout.
+//   forward: bias (staged in shared memory before the main loop) + activation in place, bf16 pairs into the buffer,
+//            cp.async.bulk.tensor stores
+//   dA     : A_{l-1}'s tile arrives by TMA into the buffer during the main loop, act' is applied to the accumulator and
+//            dZ_{l-1} is written over A_{l-1} in place, then stored by TMA.  Column sums: each thread adds its rows, a
+//            reduce-scatter over the warp's 8 row groups (colsum_row_groups), one shared-memory slot per warp, the 4 warps
+//            added in a fixed order (a step's result does not depend on warp timing), one red.global per column and tile.
+// M / N / K tails: TMA zero fill on the load side (so out-of-range accumulator rows and columns are 0 and add nothing to the
+// column sums), tensor-map clipping on the store side.
+#pragma once
+#include "gemm_tc.cuh"
+
+namespace sb {
+
+// tensor maps of one ping-pong GEMM (plain bf16: one part per operand)
+struct PpTmaps {
+  CUtensorMap a;   // K-major: box 64 (K) x BM_WG rows
+  CUtensorMap b;   // forward: MN-major, box 64 (N) x 64 (K); dA: K-major, box 64 (K) x BN rows
+  CUtensorMap o;   // output [M, N] bf16: box 64 columns x BM_WG rows (store)
+  CUtensorMap x;   // dA: A_{l-1} [M, N] bf16, same box (load)
+};
+
+template <int BM_WG, int BN>
+struct GemmPpCfg {
+  static_assert(BM_WG == 64 || BM_WG == 128, "warpgroup tile rows");
+  static_assert(BN == 64 || BN == 128, "tile N");
+  static constexpr int BK = 64;
+  static constexpr int A_BYTES = BM_WG * BK * 2;
+  static constexpr int B_BYTES = BN * BK * 2;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int X_TILE = BM_WG * 128;               // one BM_WG x 64 bf16 swizzled tile
+  static constexpr int X_BYTES = X_TILE * (BN / 64);       // one group's epilogue buffer
+  // besides the ring and the two epilogue buffers: align slack, barriers, bias [group][BN], column sums
+  // [group][parity][warp][BN]
+  static constexpr int FIXED_BYTES = 1024 + 256 + 2 * BN * 4 + 16 * BN * 4;
+  static constexpr int RING_BUDGET = 232448 - FIXED_BYTES - 2 * X_BYTES;   // 227 KB of dynamic shared memory per block
+  static constexpr int STAGES = RING_BUDGET / STAGE_BYTES > 8 ? 8 : RING_BUDGET / STAGE_BYTES;
+  static_assert(STAGES >= 4, "operand ring");
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * X_BYTES + FIXED_BYTES;
+  static constexpr int PRODUCER_WARP = 8;
+  static constexpr int THREADS = 384;
+  static constexpr int CONSUMER_REGS = 232;
+  static constexpr int PRODUCER_REGS = 40;
+};
+
+template <int BM_WG, int BN, int EPI, int ACT>
+__global__ void __launch_bounds__(384, 1)
+gemm_pp_kernel(const __grid_constant__ PpTmaps tms, const GemmTcParams p) {
+  static_assert(EPI == EPI_FWD || EPI == EPI_DA, "forward or dA");
+  using Cfg = GemmPpCfg<BM_WG, BN>;
+  constexpr int BK = Cfg::BK, STAGES = Cfg::STAGES, MI = BM_WG / 64;
+  constexpr bool B_MN = EPI == EPI_FWD;
+
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // SWIZZLE_128B needs 1024 B alignment
+  const uint32_t xs_base = smem_base + STAGES * Cfg::STAGE_BYTES;     // [group] epilogue buffers (1024-byte aligned)
+  const uint32_t bar_base = xs_base + 2 * Cfg::X_BYTES;               // full[STAGES], empty[STAGES], aux[2] (8 B each)
+  const uint32_t sm_bias = bar_base + 256u;                           // [group][BN] fp32
+  const uint32_t sm_col = sm_bias + 2u * BN * 4u;                     // [group][tile parity][warp][BN] fp32
+  auto full_bar = [&](int s) { return bar_base + 8u * s; };
+  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+  auto aux_bar = [&](int g) { return bar_base + 8u * (2 * STAGES + g); };
+  auto smem_a = [&](int s) { return smem_base + s * Cfg::STAGE_BYTES; };
+  auto smem_b = [&](int s) { return smem_base + s * Cfg::STAGE_BYTES + Cfg::A_BYTES; };
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const bool tracing = p.trace != nullptr && blockIdx.x == 0;
+  auto stamp = [&](int slot) { if (tracing) p.trace[slot] = globaltimer_ns(); };
+  if (threadIdx.x == 0) stamp(0);  // kernel entry
+
+  if (threadIdx.x == 0) {   // (not the producer thread: its predicate would stay live across the consumer code)
+    tma_prefetch_desc(&tms.a);
+    tma_prefetch_desc(&tms.b);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(full_bar(s), 1);    // the producer's arrive.expect_tx
+      mbar_init(empty_bar(s), 1);   // the owning consumer warpgroup
+    }
+    mbar_init(aux_bar(0), 1);
+    mbar_init(aux_bar(1), 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) stamp(1);  // setup done
+  if (!p.no_dep_wait) pdl_wait();
+  pdl_launch_dependents();
+  if (threadIdx.x == 0) stamp(2);  // dependencies resolved
+
+  const int tiles_m = (p.M + BM_WG - 1) / BM_WG;
+  const int tiles_n = (p.N + BN - 1) / BN;
+  const int n_tiles = tiles_m * tiles_n;
+  const int kb_n = (p.K + BK - 1) / BK;
+
+  if (warp >= Cfg::PRODUCER_WARP) {
+    // ================= TMA producer =================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::PRODUCER_REGS));
+    if (warp == Cfg::PRODUCER_WARP && lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      const int a_row0 = (p.a_rows != nullptr) ? p.a_rows->row0 : 0;  // batch position inside the resident set
+      for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        const int m0 = (t / tiles_n) * BM_WG, n0 = (t % tiles_n) * BN;
+        for (int kb = 0; kb < kb_n; ++kb) {
+          mbar_wait(empty_bar(stage), phase ^ 1);
+          const uint32_t fb = full_bar(stage);
+          mbar_arrive_expect_tx(fb, Cfg::STAGE_BYTES);
+          tma_load_2d(smem_a(stage), &tms.a, fb, kb * BK, m0 + a_row0);
+          if constexpr (B_MN) {
+#pragma unroll
+            for (int j = 0; j < BN / 64; ++j) tma_load_2d(smem_b(stage) + j * 8192, &tms.b, fb, n0 + j * 64, kb * BK);
+          } else {
+            tma_load_2d(smem_b(stage), &tms.b, fb, kb * BK, n0);
+          }
+          if (kb == 0 && t == static_cast<int>(blockIdx.x)) stamp(3);  // first TMA issued
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+    if (warp > Cfg::PRODUCER_WARP && p.zero_buf != nullptr) {
+      // the producer warpgroup's other three warps clear the step's gradient buffer beside the main loop (read by nobody
+      // before the next kernel boundary)
+      const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+      const long long zt = static_cast<long long>(threadIdx.x) - 32 * (Cfg::PRODUCER_WARP + 1), zn = 32 * 3;
+      for (long long i = static_cast<long long>(blockIdx.x) * zn + zt; i < p.zero_n4; i += static_cast<long long>(gridDim.x) * zn)
+        p.zero_buf[i] = z4;
+    }
+    __syncwarp();   // the whole warp reaches the final block barrier together (bar.sync counts warps, not lanes)
+  } else {
+    // ================= consumer warpgroups: whole tiles, alternating =================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::CONSUMER_REGS));
+    const int g = warp >> 2;                      // this group's tiles: local tile g, g + 2, ...
+    const int gt = static_cast<int>(threadIdx.x) & 127;
+    const bool xthread = gt == 0;                 // issues the group's epilogue TMA and its ring releases
+    // named barriers: 2 + g = this group's 128 threads; 4 + g = "group g may issue its main loop" (group g syncs, the other
+    // group arrives once it has issued the main loop of the tile before)
+    auto bar_wg = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(2 + g) : "memory"); };
+    const uint32_t xs = xs_base + static_cast<uint32_t>(g) * Cfg::X_BYTES;
+    const uint32_t bias_s = sm_bias + static_cast<uint32_t>(g) * BN * 4u;
+    const uint32_t col_w = sm_col + static_cast<uint32_t>(g * 8 + (warp & 3)) * BN * 4u;   // this warp's column-sum slots
+    const int r0 = (warp & 3) * 16 + (lane >> 2);   // fragment rows r0 + 8 h + 64 mi
+    const int c0 = 2 * (lane & 3);                  // fragment columns c0 + 8 i + {0, 1}
+    // byte offset of the bf16 pair at (row r, column c) of the group's buffer: tile c / 64, 16-byte piece swizzled by r % 8
+    auto xaddr = [&](int r, int c) {
+      return xs + static_cast<uint32_t>((c >> 6) * Cfg::X_TILE + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4) + (c & 7) * 2);
+    };
+    const bool do_cols = EPI == EPI_DA && p.colsum != nullptr;
+
+    float acc[MI][BN / 2];
+    // descriptor steps for 16 elements along K: K-major = 32 B inside the swizzle row; MN-major = 16 rows of 128 B
+    constexpr uint32_t a_kstep = 32u >> 4;
+    constexpr uint32_t b_kstep = B_MN ? (2048u >> 4) : (32u >> 4);
+    for (int lt = g;; lt += 2) {
+      const int t = static_cast<int>(blockIdx.x) + lt * static_cast<int>(gridDim.x);
+      if (t >= n_tiles) break;
+      const int it = lt >> 1;                      // tiles this group has done
+      const int m0 = (t / tiles_n) * BM_WG, n0 = (t % tiles_n) * BN;
+      const int nx = min(BN / 64, (p.N - n0 + 63) / 64);   // 64-column tiles inside N
+
+      // ---------- before the main loop: the buffer is free once this group's previous stores have read it ----------
+      if (xthread) tma_store_wait_read<0>();
+      if constexpr (EPI == EPI_FWD) {
+        for (int j = gt; j < BN; j += 128) {
+          const float bv = (n0 + j < p.N) ? __ldg(p.bias + n0 + j) : 0.f;
+          asm volatile("st.shared.f32 [%0], %1;" ::"r"(bias_s + j * 4u), "f"(bv) : "memory");
+        }
+        bar_wg();   // bias staged; every thread may now overwrite the buffer
+      } else {
+        if (xthread) {   // A_{l-1}'s tile, landing during the main loop
+          mbar_arrive_expect_tx(aux_bar(g), static_cast<uint32_t>(nx * Cfg::X_TILE));
+          for (int x = 0; x < nx; ++x) tma_load_2d(xs + x * Cfg::X_TILE, &tms.x, aux_bar(g), n0 + x * 64, m0);
+        }
+      }
+
+      // ---------- main loop, in turn with the other group ----------
+      if (lt >= 1) asm volatile("bar.sync %0, 256;" ::"r"(4 + g) : "memory");
+      const int kb_first = lt * kb_n;              // ring position: the k-blocks of every earlier tile of the CTA
+      int stage = kb_first % STAGES;
+      uint32_t phase = static_cast<uint32_t>(kb_first / STAGES) & 1u;
+      int prev_stage = -1;
+      for (int kb = 0; kb < kb_n; ++kb) {
+        mbar_wait(full_bar(stage), phase);  // the stage's TMA bytes have landed
+        if (kb == 0 && lt == 0 && threadIdx.x == 0) stamp(4);  // first stage landed
+        const uint64_t da = make_kmajor_sw128_desc(smem_a(stage));
+        const uint64_t db = B_MN ? make_mnmajor_sw128_desc(smem_b(stage), 8192u) : make_kmajor_sw128_desc(smem_b(stage));
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+#pragma unroll
+          for (int mi = 0; mi < MI; ++mi)   // rows 64 mi .. 64 mi + 63: 64 rows of 128 B further
+            wgmma_bf16<BN, 0, B_MN ? 1 : 0>(acc[mi], da + (8192u >> 4) * mi + a_kstep * k, db + b_kstep * k, (kb > 0 || k > 0) ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous k-block's wgmma group has finished reading its stage
+        if (prev_stage >= 0 && xthread) mbar_arrive(empty_bar(prev_stage));
+        prev_stage = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      // the other group's next tile (local tile lt + 1) may issue now
+      if (t + static_cast<int>(gridDim.x) < n_tiles) asm volatile("bar.arrive %0, 256;" ::"r"(4 + (g ^ 1)) : "memory");
+      wgmma_wait<0>();
+      if (prev_stage >= 0 && xthread) mbar_arrive(empty_bar(prev_stage));
+      if (lt == 0 && threadIdx.x == 0) { stamp(5); stamp(6); }  // first tile's accumulator complete
+
+      // ---------- epilogue in the fragment layout ----------
+      if constexpr (EPI == EPI_FWD) {
+#pragma unroll
+        for (int i = 0; i < BN / 8; ++i) {
+          const int c = c0 + 8 * i;
+          float2 b;
+          asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(b.x), "=f"(b.y) : "r"(bias_s + c * 4u) : "memory");
+#pragma unroll
+          for (int mi = 0; mi < MI; ++mi) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const float v0 = act_apply(acc[mi][4 * i + 2 * h] + b.x, ACT);
+              const float v1 = act_apply(acc[mi][4 * i + 2 * h + 1] + b.y, ACT);
+              asm volatile("st.shared.b32 [%0], %1;" ::"r"(xaddr(64 * mi + r0 + 8 * h, c)), "r"(pack_bf16x2(v0, v1)) : "memory");
+            }
+          }
+        }
+      } else {
+        mbar_wait(aux_bar(g), static_cast<uint32_t>(it) & 1u);   // A_{l-1}'s tile has landed
+        const uint32_t cb = col_w + static_cast<uint32_t>(it & 1) * 4u * BN * 4u;
+#pragma unroll
+        for (int x = 0; x < BN / 64; ++x) {   // one 64-column tile at a time (keeps the column sums at 16 registers)
+          float cs[16];   // per column pair of the thread in this tile: the sum over its rows
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int c = 64 * x + c0 + 8 * i;
+            float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+            for (int mi = 0; mi < MI; ++mi) {
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const uint32_t a = xaddr(64 * mi + r0 + 8 * h, c);
+                uint32_t raw;
+                asm volatile("ld.shared.b32 %0, [%1];" : "=r"(raw) : "r"(a) : "memory");
+                const float x0 = __uint_as_float(raw << 16), x1 = __uint_as_float(raw & 0xFFFF0000u);   // bf16 pair -> fp32
+                const float v0 = acc[mi][32 * x + 4 * i + 2 * h] * act_grad_from_out(x0, ACT);
+                const float v1 = acc[mi][32 * x + 4 * i + 2 * h + 1] * act_grad_from_out(x1, ACT);
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(pack_bf16x2(v0, v1)) : "memory");
+                s0 += v0;
+                s1 += v1;
+              }
+            }
+            cs[2 * i] = s0;
+            cs[2 * i + 1] = s1;
+          }
+          if (do_cols) {
+            colsum_row_groups(cs, lane);
+            // values 2 q, 2 q + 1 (q = lane / 4) = the column pair 8 q + c0 of this tile
+            const uint32_t col = static_cast<uint32_t>(64 * x + c0 + 8 * (lane >> 2));
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(cb + col * 4u), "f"(cs[0]), "f"(cs[1]) : "memory");
+          }
+        }
+      }
+      fence_proxy_async();   // generic-proxy writes -> visible to the TMA engine
+      bar_wg();              // the tile is complete in the buffer; the column sums of every warp are in
+      if (xthread) {
+        for (int x = 0; x < nx; ++x) tma_store_2d(&tms.o, xs + x * Cfg::X_TILE, n0 + x * 64, m0);
+        tma_store_commit();
+      }
+      if (do_cols) {
+        // the 4 warps' sums in a fixed order, one red.global per column and tile; the slots of this parity are rewritten two
+        // tiles later, after the next bar_wg
+        const uint32_t cb = col_w + static_cast<uint32_t>((it & 1) * 4 - (warp & 3)) * BN * 4u;   // warp 0's slot
+        for (int j = gt; j < BN; j += 128) {
+          float v = 0.f;
+#pragma unroll
+          for (int w = 0; w < 4; ++w) {
+            float x;
+            asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(cb + (w * BN + j) * 4u) : "memory");
+            v += x;
+          }
+          if (n0 + j < p.N && v != 0.f) red_add_f32(p.colsum + n0 + j, v);
+        }
+      }
+      if (lt == 0 && threadIdx.x == 0) stamp(7);  // first tile's epilogue done
+    }
+    if (xthread) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // the last tiles are in global memory
+  }
+
+  __syncthreads();
+  if (threadIdx.x == 0) stamp(8);  // all roles finished
+  // in-graph kernel span: slot 2 (dependencies resolved, CTA 0) .. slot 10 (latest exit over ALL CTAs; %globaltimer only
+  // grows, so atomicMax needs no reset between steps)
+  if (p.trace != nullptr && threadIdx.x == 0) atomicMax(p.trace + 10, static_cast<unsigned long long>(globaltimer_ns()));
+}
+
+// ------------------------------------------------------------------ host side
+struct PpPlan {
+  int bm_wg;   // rows of one warpgroup's tile: 128, or 64 when 128-row tiles would leave warpgroups without a tile
+  int bn;      // 64 / 128
+  int grid;
+};
+
+// bm_wg = 0: chosen from the tile count.  A CTA needs two tiles for both of its warpgroups to have work, so with no more
+// 128-row tiles than SMs 64-row tiles give each CTA two to four.  Except when 128-row tiles still cover nearly every SM
+// and the main loop is long (>= 8 k-blocks): there the taller tile's operand reuse wins over the overlapped epilogue
+// (one H100 SXM, 132 SMs: 4096 x 512 x 1000 takes 11.7 us with 128-row tiles, 13.2 us with 64; 8192 x 256 x 512 7.6 vs
+// 9.1 us; 4096 x 512 x 256, 4 k-blocks, 7.8 vs 7.4 us).
+static inline PpPlan plan_gemm_pp(int M, int N, int K, int num_sms, int bm_wg = 0) {
+  PpPlan pl = {};
+  pl.bn = N <= 64 ? 64 : 128;
+  const int tiles_n = (N + pl.bn - 1) / pl.bn;
+  const int tiles128 = ((M + 127) / 128) * tiles_n;
+  const bool tall = tiles128 > num_sms || (8 * tiles128 >= 7 * num_sms && (K + 63) / 64 >= 8);
+  pl.bm_wg = bm_wg > 0 ? bm_wg : (tall ? 128 : 64);
+  const int tiles = ((M + pl.bm_wg - 1) / pl.bm_wg) * tiles_n;
+  pl.grid = tiles < num_sms ? tiles : num_sms;
+  return pl;
+}
+
+template <int BM_WG, int BN, int EPI, int ACT>
+static int launch_gemm_pp_one(const PpPlan& pl, const PpTmaps& tms, const GemmTcParams& p, cudaStream_t st, bool pdl) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(static_cast<unsigned>(pl.grid));
+  cfg.blockDim = dim3(GemmPpCfg<BM_WG, BN>::THREADS);
+  cfg.dynamicSmemBytes = GemmPpCfg<BM_WG, BN>::SMEM_BYTES;
+  cfg.stream = st;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = pdl ? 1 : 0;
+  SB_CUDA(cudaLaunchKernelEx(&cfg, gemm_pp_kernel<BM_WG, BN, EPI, ACT>, tms, p));
+  return SB_OK;
+}
+
+template <int BM_WG, int BN, int EPI>
+static int launch_gemm_pp_act(const PpPlan& pl, const PpTmaps& tms, const GemmTcParams& p, cudaStream_t st, bool pdl) {
+  switch (p.act) {
+    case SB_ACT_SIGMOID: return launch_gemm_pp_one<BM_WG, BN, EPI, SB_ACT_SIGMOID>(pl, tms, p, st, pdl);
+    case SB_ACT_TANH: return launch_gemm_pp_one<BM_WG, BN, EPI, SB_ACT_TANH>(pl, tms, p, st, pdl);
+    case SB_ACT_RELU: return launch_gemm_pp_one<BM_WG, BN, EPI, SB_ACT_RELU>(pl, tms, p, st, pdl);
+    case SB_ACT_LEAKYRELU: return launch_gemm_pp_one<BM_WG, BN, EPI, SB_ACT_LEAKYRELU>(pl, tms, p, st, pdl);
+    default: return launch_gemm_pp_one<BM_WG, BN, EPI, SB_ACT_NONE>(pl, tms, p, st, pdl);
+  }
+}
+
+// tensor maps (pl.bm_wg-row boxes) must have been made for the same plan
+template <int EPI>
+static int launch_gemm_pp(const PpPlan& pl, const PpTmaps& tms, const GemmTcParams& p, cudaStream_t st, bool pdl) {
+  if (pl.bm_wg == 128 && pl.bn == 128) return launch_gemm_pp_act<128, 128, EPI>(pl, tms, p, st, pdl);
+  if (pl.bm_wg == 128 && pl.bn == 64) return launch_gemm_pp_act<128, 64, EPI>(pl, tms, p, st, pdl);
+  if (pl.bm_wg == 64 && pl.bn == 128) return launch_gemm_pp_act<64, 128, EPI>(pl, tms, p, st, pdl);
+  if (pl.bm_wg == 64 && pl.bn == 64) return launch_gemm_pp_act<64, 64, EPI>(pl, tms, p, st, pdl);
+  return set_error(SB_ERR_INVALID, "no gemm_pp instantiation for bm_wg=%d bn=%d", pl.bm_wg, pl.bn);
+}
+
+// opt in to > 48 KB dynamic shared memory (once per process, outside of stream capture)
+static int set_gemm_pp_attrs() {
+#define SB_ATTR_ACT(BM, BN, EPI, ACT) \
+  SB_CUDA(cudaFuncSetAttribute(gemm_pp_kernel<BM, BN, EPI, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmPpCfg<BM, BN>::SMEM_BYTES))
+#define SB_ATTR_ALL(BM, BN, EPI) SB_ATTR_ACT(BM, BN, EPI, SB_ACT_NONE); SB_ATTR_ACT(BM, BN, EPI, SB_ACT_SIGMOID); \
+  SB_ATTR_ACT(BM, BN, EPI, SB_ACT_TANH); SB_ATTR_ACT(BM, BN, EPI, SB_ACT_RELU); SB_ATTR_ACT(BM, BN, EPI, SB_ACT_LEAKYRELU)
+#define SB_ATTR_EPI(EPI) SB_ATTR_ALL(128, 128, EPI); SB_ATTR_ALL(128, 64, EPI); SB_ATTR_ALL(64, 128, EPI); SB_ATTR_ALL(64, 64, EPI)
+  SB_ATTR_EPI(EPI_FWD);
+  SB_ATTR_EPI(EPI_DA);
+#undef SB_ATTR_EPI
+#undef SB_ATTR_ALL
+#undef SB_ATTR_ACT
+  return SB_OK;
+}
+
+}  // namespace sb

@@ -14,7 +14,9 @@
 //   EPI_DW  : dW_l = A_{l-1}^T dZ_l  A = A_{l-1} [rows,in] MN-major, B = dZ_l [rows,out] MN-major; split-K over the
 //                                    batch, fp32 red.add into the flat gradient
 //   EPI_F32 : plain fp32 store (kernel-level parity test hook)
-// The last hidden GEMM of a training step, with the output layer fused into its epilogue, is gemm_fwd_out.cuh.
+// Here EPI_FWD / EPI_DA are the split-precision parts and the wide+deep addend (GENERIC); the plain-bf16 forward and dA
+// GEMMs are gemm_pp.cuh, the last hidden GEMM of a training step with the output layer fused into its epilogue is
+// gemm_fwd_out.cuh.
 //
 // Tile: one CTA owns 128 x BN (BN = 64 | 128 | 256).  CG = 2: a cluster of two CTAs owns 256 x BN; both need the same B tile,
 // so each loads half of it and TMA multicasts that half into both CTAs' shared memory (half the B traffic from L2 per CTA).
@@ -93,17 +95,9 @@ struct GemmTcParams {
 struct TmapSet {
   CUtensorMap a[3];
   CUtensorMap b[3];
-  CUtensorMap o;   // TMA-staged epilogues: the bf16 output matrix [M, N] (box 64 columns x 128 rows, 128-byte swizzle)
-  CUtensorMap x;   // EPI_DA: A_{l-1} [M, N], same box
 };
 
-// bytes of TMA staging the epilogue of an instantiation needs: the plain-bf16 forward and dA epilogues move their global
-// data through 128 x 64 bf16 tiles (16 KB) with TMA - output tile double-buffered, dA additionally its A_{l-1} tile
-__host__ __device__ constexpr int epi_tma_bytes(int EPI, bool GENERIC) {
-  return GENERIC ? 0 : (EPI == 0 /*EPI_FWD*/ ? 2 * 16384 : (EPI == 1 /*EPI_DA*/ ? 4 * 16384 : 0));
-}
-
-template <int BN, int CG, int XB = 0>
+template <int BN, int CG>
 struct GemmTcCfg {
   static_assert(CG == 1 || CG == 2, "cta group");
   static_assert(BN == 64 || BN == 128 || BN == 256, "tile N");
@@ -119,10 +113,10 @@ struct GemmTcCfg {
   // row-wise 16-byte loads are free of bank conflicts
   static constexpr int ACC_LD = 64 + 4;
   static constexpr int ACC_BYTES = BM * ACC_LD * 4;
-  // shared memory besides the operand ring: align slack, barriers, epilogue scratch, bias, per-warp transpose tiles
-  // (only the epilogues without TMA staging use them), column-sum accumulators, TMA staging tiles (XB), accumulator block
-  static constexpr int TR_BYTES = XB > 0 ? 0 : 8 * 2048;
-  static constexpr int FIXED_BYTES = 1024 + 256 + 2048 + 2048 + TR_BYTES + 4096 + XB + ACC_BYTES;
+  // shared memory besides the operand ring: align slack, barriers, epilogue scratch, bias, per-warp transpose tiles,
+  // column-sum accumulators, accumulator block
+  static constexpr int TR_BYTES = 8 * 2048;
+  static constexpr int FIXED_BYTES = 1024 + 256 + 2048 + 2048 + TR_BYTES + 4096 + ACC_BYTES;
   static constexpr int RING_BUDGET = 232448 - FIXED_BYTES;   // 227 KB of dynamic shared memory per block
   static constexpr int STAGES = RING_BUDGET / STAGE_BYTES > 8 ? 8 : RING_BUDGET / STAGE_BYTES;
   static_assert(STAGES >= 2, "operand ring");
@@ -149,23 +143,20 @@ __device__ __forceinline__ void epi_da_chunk(float (&v)[32], const __nv_bfloat16
   for (int j = 0; j < 32; ++j) v[j] *= act_grad_from_out(__bfloat162float(ah[j]), ACT);
 }
 
-// GENERIC = false: the plain-bf16 epilogues (performance mode; their instruction footprint decides the epilogue speed).
 // GENERIC = true adds the cold features at compile time: split-precision part stores / loads (np > 1) and the fp32 addend
-// of the wide+deep first layer.
+// of the wide+deep first layer.  EPI_FWD / EPI_DA are instantiated with it only.
 template <int BN, int EPI, bool A_MN, bool B_MN, int CG, bool GENERIC = false>
-__global__ void __launch_bounds__((GemmTcCfg<BN, CG, epi_tma_bytes(EPI, GENERIC)>::THREADS), 1)
+__global__ void __launch_bounds__((GemmTcCfg<BN, CG>::THREADS), 1)
 gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
-  using Cfg = GemmTcCfg<BN, CG, epi_tma_bytes(EPI, GENERIC)>;
-  constexpr bool TMA_EPI = epi_tma_bytes(EPI, GENERIC) > 0;
+  using Cfg = GemmTcCfg<BN, CG>;
   const int act_sel = p.act;
   constexpr int BM = Cfg::BM, BK = Cfg::BK, STAGES = Cfg::STAGES, TILE_M = Cfg::TILE_M, BN_CTA = Cfg::BN_CTA;
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B needs 1024 B alignment
-  const uint32_t xbuf_base = smem_base + STAGES * Cfg::STAGE_BYTES;            // TMA staging tiles (1024-byte aligned)
-  const uint32_t accs_base = xbuf_base + epi_tma_bytes(EPI, GENERIC);          // accumulator staging block
+  const uint32_t accs_base = smem_base + STAGES * Cfg::STAGE_BYTES;            // accumulator staging block
   const uint32_t bar_base = accs_base + Cfg::ACC_BYTES;
-  // barrier layout (8 B each): full[STAGES], empty[STAGES]; then scratch (dA TMA barriers)
+  // barrier layout (8 B each): full[STAGES], empty[STAGES]; then scratch
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
   const uint32_t scratch = bar_base + 8u * (2 * STAGES) + 16u;
@@ -287,22 +278,7 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
     // wide dA GEMMs wait on the L2 atomic units).
     // layout: [buffer (tile parity)][BN] floats
     const uint32_t sm_col = sm_vec + 2048u + static_cast<uint32_t>(Cfg::TR_BYTES);
-    // TMA-staged epilogue (plain-bf16 forward / dA): the 128 x BN tile leaves in 64-column blocks.  Block k: every thread
-    // writes the 32 bf16 of its row-chunk as four 16-byte pieces into the 128-byte-swizzled 128 x 64 tile xo[k & 1] (the layout
-    // the output tensor map expects; a quarter-warp covers all 32 banks), one thread issues cp.async.bulk.tensor (store) for
-    // the tile; dA additionally gets its A_{l-1} block by TMA load into xa[k & 1] (issued two blocks ahead) and reads it back
-    // with the same swizzle.  No ld.shared / st.global per element, no transposes, M / N tails clipped by the tensor map.
-    auto xo = [&](int b) { return xbuf_base + static_cast<uint32_t>(b) * 16384u; };
-    auto xa = [&](int b) { return xbuf_base + 32768u + static_cast<uint32_t>(b) * 16384u; };
-    auto aux_bar = [&](int b) { return scratch + 8u * static_cast<uint32_t>(b); };
     const int rt = quarter * 32 + lane;                                   // row of this thread inside the CTA's 128 rows
-    auto piece = [&](int half_, int i) { return static_cast<uint32_t>(rt) * 128u + static_cast<uint32_t>(((half_ * 4 + i) ^ (rt & 7)) << 4); };
-    const bool xthread = (warp == 0 && lane == 0);                        // issues the epilogue's TMA loads / stores
-    unsigned xblk = 0;                                                    // 64-column blocks processed so far
-    if constexpr (TMA_EPI && EPI == EPI_DA) {
-      if (warp == 0 && lane == 0) { mbar_init(aux_bar(0), 1); mbar_init(aux_bar(1), 1); fence_barrier_init(); }
-      bar_all();
-    }
     auto col_slot = [&](int buf, int j) { return sm_col + static_cast<uint32_t>((buf * BN + j) * 4); };
     auto red_shared = [](uint32_t a, float v) { asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(a), "f"(v) : "memory"); };
     if constexpr (EPI == EPI_DA) {
@@ -400,7 +376,7 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
       // of the dA epilogue
       // dA epilogue without TMA staging: A_{l-1} of EVERY chunk this warp will handle is fetched before the main loop and
       // kept in registers as a shift queue, so that one L2 / HBM latency is paid per tile instead of one per chunk
-      constexpr int AUXQ = (EPI == EPI_DA && !TMA_EPI) ? (BN / 64 > 0 ? BN / 64 : 1) : 1;
+      constexpr int AUXQ = EPI == EPI_DA ? (BN / 64 > 0 ? BN / 64 : 1) : 1;
       uint4 aux_q[AUXQ][4];
       const int row_base = tm * TILE_M + static_cast<int>(rank) * BM + quarter * 32;   // first row of this warp's 32
       // store a 32 x 64 B tile held one-row-per-thread (4 pieces each) to a row-major bf16 matrix, coalesced
@@ -451,23 +427,13 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
           }
         }
       };
-      if constexpr (EPI == EPI_DA && !TMA_EPI) {
+      if constexpr (EPI == EPI_DA) {
 #pragma unroll
         for (int i = 0; i < AUXQ; ++i) load_aux(half + 2 * i, aux_q[i]);
       }
       // blocks of 64 columns this tile really has (the same number for every warp: the block loop contains barriers)
       const int tile_cols = (p.N - tn * BN) < BN ? (p.N - tn * BN) : BN;
       const int nblk = (tile_cols + 63) / 64;
-      const int x_row0 = tm * TILE_M + static_cast<int>(rank) * BM;      // TMA row coordinate of this CTA's 128 rows
-      if constexpr (TMA_EPI && EPI == EPI_DA) {
-        if (xthread) {
-          for (int k = 0; k < 2 && k < nblk; ++k) {       // A_{l-1} of the first two blocks (buffers free: every warp has left the previous tile)
-            const int b = (xblk + k) & 1;
-            mbar_arrive_expect_tx(aux_bar(b), 16384u);
-            tma_load_2d(xa(b), &tms.x, aux_bar(b), tn * BN + k * 64, x_row0);
-          }
-        }
-      }
       const uint32_t sm_bias = sm_vec + static_cast<uint32_t>(it & 1) * (BN * 4u);   // EPI_FWD: this tile's bias, double-buffered
       if constexpr (EPI == EPI_FWD) {
         // (a warp reaches this barrier only after finishing the previous tile, so buffer it & 1 is no longer read)
@@ -513,22 +479,13 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
       for (int c = half; (c >> 1) < nblk; c += 2) {
         stage_block(c >> 1);
         const int col0 = tn * BN + c * 32;
-        const bool chunk_ok = col0 < p.N;       // (TMA path: a warp whose 32 columns lie beyond N only joins the barriers)
-        if constexpr (!TMA_EPI) {
-          if (!chunk_ok) continue;  // whole chunk out of range (warp-uniform)
-        }
+        if (col0 >= p.N) continue;  // whole chunk out of range (warp-uniform)
         uint32_t raw[32];
-        if (chunk_ok) {
-          acc_ld(c, raw);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) raw[j] = 0u;
-        }
+        acc_ld(c, raw);
         float v[32];
 #pragma unroll
         for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(raw[j]);
         const bool full = col0 + 32 <= p.N;  // warp-uniform fast path
-        const int xb = static_cast<int>(xblk & 1u);   // staging tiles: the two alternate
 
         if constexpr (EPI == EPI_FWD) {
           if (GENERIC && p.addend != nullptr && row_ok) {
@@ -561,17 +518,11 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
         } else if constexpr (EPI == EPI_DA) {
           // multiply by act'(A_{l-1}[row, col]) read as bf16
           uint4 a4[4];
-          if constexpr (TMA_EPI) {
-            mbar_wait(aux_bar(xb), (xblk >> 1) & 1u);   // this block's A_{l-1} tile has landed
+          lanes_to_row(aux_q[0], a4);
 #pragma unroll
-            for (int i = 0; i < 4; ++i) a4[i] = lds4(xa(xb) + piece(half, i));
-          } else {
-            lanes_to_row(aux_q[0], a4);
+          for (int i = 0; i + 1 < AUXQ; ++i) {
 #pragma unroll
-            for (int i = 0; i + 1 < AUXQ; ++i) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k) aux_q[i][k] = aux_q[i + 1][k];
-            }
+            for (int k = 0; k < 4; ++k) aux_q[i][k] = aux_q[i + 1][k];
           }
           __nv_bfloat16* ah = reinterpret_cast<__nv_bfloat16*>(a4);
           if (GENERIC && p.np > 1 && (act_sel == SB_ACT_SIGMOID || act_sel == SB_ACT_TANH)) {
@@ -606,36 +557,8 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
         }
 
         if constexpr (EPI == EPI_FWD || EPI == EPI_DA) {
-          if constexpr (TMA_EPI) {
-            uint4 o[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              o[q].x = pack_bf16x2(v[q * 8 + 0], v[q * 8 + 1]);
-              o[q].y = pack_bf16x2(v[q * 8 + 2], v[q * 8 + 3]);
-              o[q].z = pack_bf16x2(v[q * 8 + 4], v[q * 8 + 5]);
-              o[q].w = pack_bf16x2(v[q * 8 + 6], v[q * 8 + 7]);
-            }
-            if (xthread) tma_store_wait_read<1>();                 // the store issued from this tile two blocks ago has read it ...
-            bar_all();                                             // (B) ... so every warp may now overwrite it
-#pragma unroll
-            for (int q = 0; q < 4; ++q) sts4(xo(xb) + piece(half, q), o[q]);
-            fence_proxy_async();                                   // generic-proxy writes -> visible to the TMA engine
-            bar_all();                                             // (A) the block's tile is complete; A_{l-1} tile consumed
-            if (xthread) {
-              tma_store_2d(&tms.o, xo(xb), tn * BN + (c >> 1) * 64, x_row0);
-              tma_store_commit();
-              if constexpr (EPI == EPI_DA) {
-                if ((c >> 1) + 2 < nblk) {                         // A_{l-1} of the block after next, into the tile just consumed
-                  mbar_arrive_expect_tx(aux_bar(xb), 16384u);
-                  tma_load_2d(xa(xb), &tms.x, aux_bar(xb), tn * BN + ((c >> 1) + 2) * 64, x_row0);
-                }
-              }
-            }
-            ++xblk;
-          } else {
-            // row-major bf16 (ld_out is a multiple of 8, pad columns belong to the buffer); split modes: np part arrays
-            store_parts(v, p.out, p.out_ps, p.ld_out, col0, full);
-          }
+          // row-major bf16 (ld_out is a multiple of 8, pad columns belong to the buffer); split modes: np part arrays
+          store_parts(v, p.out, p.out_ps, p.ld_out, col0, full);
           if constexpr (EPI == EPI_DA) {
             if (p.colsum != nullptr) {
               // bias gradient: per-column sum over this warp's 32 rows, accumulated per CTA in shared memory
@@ -688,9 +611,6 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
         if (p.colsum != nullptr) flush_cols(it, tn, p.colsum);
       }
       if (w == w_first && threadIdx.x == 0) stamp(7);  // first tile's epilogue done
-    }
-    if constexpr (TMA_EPI) {
-      if (xthread) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // the last tiles are in global memory
     }
   }
 

@@ -7,6 +7,7 @@
 #include "net.cuh"
 #include "gemm_tc_launch.cuh"
 #include "gemm_fwd_out.cuh"
+#include "gemm_pp.cuh"
 
 namespace sb {
 
@@ -69,7 +70,8 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rows, int cols, int l
 }
 
 // Tile configuration (persistent grid, one CTA per SM, 128 x BN tiles):
-//   - BN = 128 (64 for a layer at most 64 wide).  A 128 x 256 tile would fetch fewer operand bytes per flop, but its
+//   - BN = 128 (64 for a layer at most 64 wide).  The plain-bf16 forward and dA GEMMs are planned apart (plan_gemm_pp,
+//     gemm_pp.cuh): two warpgroups per CTA with whole tiles each, 128 or 64 rows.  A 128 x 256 tile would fetch fewer operand bytes per flop, but its
 //     128-register accumulator plus the epilogue does not fit the consumer threads' registers without spills.  The fused
 //     output layer (gemm_fwd_out.cuh) is planned apart: it needs whole rows of A_L in one CTA, so it takes 64 x h_L tiles
 //     (h_L <= 256, the two consumer warpgroups split the columns: 64 accumulator registers per thread) and
@@ -276,6 +278,7 @@ int Net::init(const sb_net_desc* d, int device_, bool training_) {
   if (bf) {
     SB_TRY((set_gemm_tc_attrs<EPI_FWD, false, true>()));
     SB_TRY(set_gemm_fwd_out_attrs());
+    SB_TRY(set_gemm_pp_attrs());
     SB_TRY((set_gemm_tc_attrs<EPI_DA, false, false>()));
     SB_TRY((set_gemm_tc_attrs<EPI_DW, true, true>()));
     // keep the SMs in the GEMMs' shared-memory carve-out for every kernel of the step, so that no launch in the chain
@@ -389,12 +392,11 @@ int Net::enqueue_hidden_forward(int rows, float* grad, bool* fused_out) {
     const int ld_k = sp0 ? ldD : ly.ld_in;
     if (tc()) {
       // Z = A_{l-1}[rows,in] (K-major) x W_l[in,out] (MN-major B operand: n contiguous)
-      const GemmPlan pl = plan_gemm(rows, ly.out, round_up(k_in, 64) * pairs_of(nparts), gemm_sms, false);
       TmapSet tm;
       const bool res0 = (l == 0) && from_resident;
       const __nv_bfloat16* src = (l == 0) ? (res0 ? resident_Xb : Xb) : A[l - 1];
       const long long src_ps = (l == 0) ? (res0 ? resident_ps : Xb_ps) : A_ps[l - 1];
-      SB_TRY(make_tmaps_bf16(tm.a, src, src_ps, nparts, res0 ? static_cast<int>(resident_rows) : rows, k_in, ld_k, 128));
+      const int src_rows = res0 ? static_cast<int>(resident_rows) : rows;
       SB_TRY(make_tmaps_bf16(tm.b, ly.Wn, Wn_ps[l], nparts, k_in, ly.out, ly.ld_out, 64));
       GemmTcParams p = {};
       set_part_pairs(&p, nparts);
@@ -406,7 +408,7 @@ int Net::enqueue_hidden_forward(int rows, float* grad, bool* fused_out) {
       if (l == L - 1 && grad != nullptr && fuse_out_layer && training && ly.out <= fuse_out_max && p.addend == nullptr) {
         // K2 + K3 + K4 + output backward in one kernel (gemm_fwd_out.cuh): 64-row tiles of whole rows of A_L
         FwdOutTmaps ft;
-        SB_TRY(make_tmaps_bf16(ft.a, src, src_ps, nparts, res0 ? static_cast<int>(resident_rows) : rows, k_in, ld_k, 64));
+        SB_TRY(make_tmaps_bf16(ft.a, src, src_ps, nparts, src_rows, k_in, ld_k, 64));
         for (int i = 0; i < 3; ++i) ft.b[i] = tm.b[i];
         SB_TRY(make_tmaps_bf16(ft.o, dZ[l], A_ps[l], nparts, rows, ly.out, ly.ld_out, 64));
         const int tiles = (rows + 63) / 64;
@@ -426,10 +428,20 @@ int Net::enqueue_hidden_forward(int rows, float* grad, bool* fused_out) {
         zero_buf = nullptr;
       }
       p.trace = next_trace("fwd", l, rows, ly.out, k_in);
-      if (nparts == 1 && p.addend == nullptr)      // plain bf16: the epilogue stores its tiles by TMA
-        SB_TRY(make_tmap_bf16(&tm.o, A[l], rows, ly.out, ly.ld_out, 128));
       if (beside_prev_xchg && l == 0) p.no_dep_wait = 1;
-      SB_TRY((launch_gemm_tc<EPI_FWD, false, true>(pl, tm, p, stream, use_pdl && !(beside_prev_xchg && l == 1))));
+      const bool pdl = use_pdl && !(beside_prev_xchg && l == 1);
+      if (nparts == 1 && p.addend == nullptr) {    // plain bf16: the ping-pong kernel
+        const PpPlan pp = plan_gemm_pp(rows, ly.out, k_in, gemm_sms);
+        PpTmaps pt;
+        SB_TRY(make_tmap_bf16(&pt.a, src, src_rows, k_in, ld_k, pp.bm_wg));
+        pt.b = tm.b[0];
+        SB_TRY(make_tmap_bf16(&pt.o, A[l], rows, ly.out, ly.ld_out, pp.bm_wg));
+        SB_TRY(launch_gemm_pp<EPI_FWD>(pp, pt, p, stream, pdl));
+      } else {
+        const GemmPlan pl = plan_gemm(rows, ly.out, round_up(k_in, 64) * pairs_of(nparts), gemm_sms, false);
+        SB_TRY(make_tmaps_bf16(tm.a, src, src_ps, nparts, src_rows, k_in, ld_k, 128));
+        SB_TRY((launch_gemm_tc<EPI_FWD, false, true>(pl, tm, p, stream, pdl)));
+      }
     } else {
       GemmF32Params p = {};
       p.M = rows; p.N = ly.out; p.K = k_in;
@@ -591,10 +603,6 @@ int Net::enqueue_backward(int rows, float* grad) {
       if (l > 0) {
         // dZ_{l-1}[rows,in] = (dZ_l[rows,out] (K-major) x W_l[in,out] (K-major B: k = out contiguous)) .* act'(A_{l-1})
         Layer& pl = layers[l - 1];
-        const GemmPlan gp = plan_gemm(rows, ly.in, round_up(ly.out, 64) * pairs_of(nparts), gemm_sms, false);
-        TmapSet tm;
-        SB_TRY(make_tmaps_bf16(tm.a, dZ[l], A_ps[l], nparts, rows, ly.out, ly.ld_out, 128));
-        SB_TRY(make_tmaps_bf16(tm.b, ly.Wn, Wn_ps[l], nparts, ly.in, ly.out, ly.ld_out, plan_box_rows_b(gp)));
         GemmTcParams p = {};
         set_part_pairs(&p, nparts);
         p.M = rows; p.N = ly.in; p.K = ly.out;
@@ -603,11 +611,21 @@ int Net::enqueue_backward(int rows, float* grad) {
         p.out = dZ[l - 1]; p.ld_out = pl.ld_out; p.out_ps = A_ps[l - 1];
         p.colsum = grad + pl.b_off;
         p.trace = next_trace("dA", l, rows, ly.in, ly.out);
-        if (nparts == 1) {                           // plain bf16: A_{l-1} in and dZ_{l-1} out move as TMA tiles
-          SB_TRY(make_tmap_bf16(&tm.o, dZ[l - 1], rows, ly.in, pl.ld_out, 128));
-          SB_TRY(make_tmap_bf16(&tm.x, A[l - 1], rows, ly.in, pl.ld_out, 128));
+        if (nparts == 1) {                           // plain bf16: the ping-pong kernel
+          const PpPlan pp = plan_gemm_pp(rows, ly.in, ly.out, gemm_sms);
+          PpTmaps pt;
+          SB_TRY(make_tmap_bf16(&pt.a, dZ[l], rows, ly.out, ly.ld_out, pp.bm_wg));
+          SB_TRY(make_tmap_bf16(&pt.b, ly.Wn, ly.in, ly.out, ly.ld_out, pp.bn));
+          SB_TRY(make_tmap_bf16(&pt.o, dZ[l - 1], rows, ly.in, pl.ld_out, pp.bm_wg));
+          SB_TRY(make_tmap_bf16(&pt.x, A[l - 1], rows, ly.in, pl.ld_out, pp.bm_wg));
+          SB_TRY(launch_gemm_pp<EPI_DA>(pp, pt, p, stream, use_pdl));
+        } else {
+          const GemmPlan gp = plan_gemm(rows, ly.in, round_up(ly.out, 64) * pairs_of(nparts), gemm_sms, false);
+          TmapSet tm;
+          SB_TRY(make_tmaps_bf16(tm.a, dZ[l], A_ps[l], nparts, rows, ly.out, ly.ld_out, 128));
+          SB_TRY(make_tmaps_bf16(tm.b, ly.Wn, Wn_ps[l], nparts, ly.in, ly.out, ly.ld_out, plan_box_rows_b(gp)));
+          SB_TRY((launch_gemm_tc<EPI_DA, false, false>(gp, tm, p, stream, use_pdl)));
         }
-        SB_TRY((launch_gemm_tc<EPI_DA, false, false>(gp, tm, p, stream, use_pdl)));
         mark("gemm_da");
         if (l == 1 && fork && defer_join) SB_CUDA(cudaEventRecord(ev_da_done, stream));
       }
