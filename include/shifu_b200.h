@@ -294,9 +294,8 @@ int sb_debug_gemm_bf16(const float* A, const float* B, float* D, int32_t M, int3
  * B ([N,K] or [K,N]).  Instantiated combinations: (0,0) dA GEMM, (0,1) forward GEMM, (1,1) dW GEMM. */
 int sb_debug_gemm_bf16_ex(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K,
                           int32_t split_k, int32_t a_mn, int32_t b_mn, int device);
-/* same, forcing the tile configuration: cfg_cg = 1 (one CTA per 128 x cfg_bn tile, cfg_bn 64|128) or 2 (cluster of two
- * CTAs per 256 x cfg_bn tile, B multicast, cfg_bn 128|256; not with sb_debug_gemm_bench); cfg_cg = 0 lets the planner
- * choose. */
+/* same, forcing the tile configuration: cfg_cg = 1 forces a 128 x cfg_bn tile (cfg_bn 64|128); cfg_cg = 0 lets the
+ * planner choose.  Any other cfg_cg is SB_ERR_INVALID. */
 int sb_debug_gemm_bf16_cfg(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K,
                            int32_t split_k, int32_t a_mn, int32_t b_mn, int32_t cfg_cg, int32_t cfg_bn, int device);
 

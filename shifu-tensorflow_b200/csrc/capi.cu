@@ -7,7 +7,6 @@
 #include <memory>
 #include <random>
 #include "net.cuh"
-#include "gemm_tc_launch.cuh"
 #include "gemm_pp.cuh"
 #include "savedmodel.h"
 #include "xchg_p2p.cuh"
@@ -123,9 +122,9 @@ static int enqueue_optimizer(sb_trainer* t, const float* g, int w0 = 0, int w1 =
   if (!st) st = n.stream;
   if (w1 <= w0) return SB_OK;
   // pdl = false: plain dependency (runs after a stream join / on the comm stream)
-  SB_TRY(n.launch(optimizer_kernel, dim3(static_cast<unsigned>(w1 - w0)), dim3(256), 0, st, pdl, n.work + w0, n.desc, t->hyper,
-                  n.theta, g, n.s1, n.s2, n.scal, publish_scalars ? t->d_hscal : static_cast<float*>(nullptr),
-                  n.next_trace(st == n.stream ? "opt" : "opt_side")));
+  SB_TRY(launch_kernel(optimizer_kernel, dim3(static_cast<unsigned>(w1 - w0)), dim3(256), 0, st, pdl, n.work + w0, n.desc, t->hyper,
+                       n.theta, g, n.s1, n.s2, n.scal, publish_scalars ? t->d_hscal : static_cast<float*>(nullptr),
+                       n.next_trace(st == n.stream ? "opt" : "opt_side")));
   n.mark("optimizer");
   return SB_OK;
 }
@@ -201,15 +200,15 @@ static int enqueue_xchg(sb_trainer* t, int slot_mask, cudaStream_t st, bool publ
   if (t->ll_ready && (ll_mode == 2 || (ll_mode == 1 && alone))) {
     LLParams lp;
     lp.x = p; lp.llg_off = t->llg_off; lp.lls_off = t->lls_off; lp.n4 = t->xch_n4;
-    if (t->world <= 2) SB_TRY(n.launch(xchg_ll_kernel<2>, g, b, 0, st, pdl, lp));
-    else if (t->world <= 4) SB_TRY(n.launch(xchg_ll_kernel<4>, g, b, 0, st, pdl, lp));
-    else if (t->world <= 8) SB_TRY(n.launch(xchg_ll_kernel<8>, g, b, 0, st, pdl, lp));
-    else SB_TRY(n.launch(xchg_ll_kernel<16>, g, b, 0, st, pdl, lp));
+    if (t->world <= 2) SB_TRY(launch_kernel(xchg_ll_kernel<2>, g, b, 0, st, pdl, lp));
+    else if (t->world <= 4) SB_TRY(launch_kernel(xchg_ll_kernel<4>, g, b, 0, st, pdl, lp));
+    else if (t->world <= 8) SB_TRY(launch_kernel(xchg_ll_kernel<8>, g, b, 0, st, pdl, lp));
+    else SB_TRY(launch_kernel(xchg_ll_kernel<16>, g, b, 0, st, pdl, lp));
   } else
-  if (t->world <= 2) SB_TRY(n.launch(xchg_update_kernel<2>, g, b, 0, st, pdl, p));
-  else if (t->world <= 4) SB_TRY(n.launch(xchg_update_kernel<4>, g, b, 0, st, pdl, p));
-  else if (t->world <= 8) SB_TRY(n.launch(xchg_update_kernel<8>, g, b, 0, st, pdl, p));
-  else SB_TRY(n.launch(xchg_update_kernel<16>, g, b, 0, st, pdl, p));
+  if (t->world <= 2) SB_TRY(launch_kernel(xchg_update_kernel<2>, g, b, 0, st, pdl, p));
+  else if (t->world <= 4) SB_TRY(launch_kernel(xchg_update_kernel<4>, g, b, 0, st, pdl, p));
+  else if (t->world <= 8) SB_TRY(launch_kernel(xchg_update_kernel<8>, g, b, 0, st, pdl, p));
+  else SB_TRY(launch_kernel(xchg_update_kernel<16>, g, b, 0, st, pdl, p));
   n.mark("xchg_update");
   t->master_stale = true;
   t->grad_sharded = true;
@@ -1712,8 +1711,8 @@ int sb_debug_gemm_bench(const float* A, const float* B, float* D, int32_t M, int
 
 static int debug_gemm_impl(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K, int32_t split_k,
                            int32_t a_mn, int32_t b_mn, int32_t cfg_cg, int32_t cfg_bn, int device, int iters, float* ms_out) {
-  SB_CHECK(cfg_cg == 0 || ((cfg_cg == 1 && (cfg_bn == 64 || cfg_bn == 128)) || (cfg_cg == 2 && (cfg_bn == 128 || cfg_bn == 256))),
-           SB_ERR_INVALID, "tile configuration cg=%d bn=%d not instantiated", cfg_cg, cfg_bn);
+  SB_CHECK(cfg_cg == 0 || (cfg_cg == 1 && (cfg_bn == 64 || cfg_bn == 128)), SB_ERR_INVALID,
+           "tile configuration cg=%d bn=%d not instantiated", cfg_cg, cfg_bn);
   SB_CHECK(A && B && D && M > 0 && N > 0 && K > 0, SB_ERR_INVALID, "bad argument");
   SB_CHECK((a_mn == 0 && b_mn == 0) || (a_mn == 0 && b_mn == 1) || (a_mn == 1 && b_mn == 1), SB_ERR_INVALID,
            "layout combination not instantiated (use KK, KM or MM)");
@@ -1742,26 +1741,18 @@ static int debug_gemm_impl(const float* A, const float* B, float* D, int32_t M, 
   cast_bf16_kernel<<<static_cast<unsigned>((static_cast<long long>(M) * K + 255) / 256), 256>>>(dA32, a_rows, a_cols, dA, lda);
   cast_bf16_kernel<<<static_cast<unsigned>((static_cast<long long>(N) * K + 255) / 256), 256>>>(dB32, b_rows, b_cols, dB, ldb);
   GemmPlan pl = plan_gemm(M, N, K, prop.multiProcessorCount, false);
-  if (cfg_cg > 0) {  // explicit tile configuration requested by the test
-    pl.cg = cfg_cg; pl.bn = cfg_bn;
-    const int tiles = ((M + 128 * pl.cg - 1) / (128 * pl.cg)) * ((N + pl.bn - 1) / pl.bn);
-    pl.split_k = 1; pl.kb_per_split = (K + 63) / 64;
-    const int slots = prop.multiProcessorCount / pl.cg;
-    pl.grid = (tiles < slots ? tiles : slots) * pl.cg;
-  }
+  if (cfg_cg > 0) pl.bn = cfg_bn;  // explicit tile configuration requested by the test
   {
     const int total_kb = (K + 63) / 64;
     int want = split_k < 1 ? 1 : (split_k > total_kb ? total_kb : split_k);
     pl.kb_per_split = (total_kb + want - 1) / want;
     pl.split_k = (total_kb + pl.kb_per_split - 1) / pl.kb_per_split;
-    const int tiles = ((M + 128 * pl.cg - 1) / (128 * pl.cg)) * ((N + pl.bn - 1) / pl.bn);
-    const int slots = prop.multiProcessorCount / pl.cg;
-    const int work = tiles * pl.split_k;
-    pl.grid = (work < slots ? work : slots) * pl.cg;
+    const int work = ((M + 127) / 128) * ((N + pl.bn - 1) / pl.bn) * pl.split_k;
+    pl.grid = work < prop.multiProcessorCount ? work : prop.multiProcessorCount;
   }
   TmapSet tms;
   int s = make_tmap_bf16(&tms.a[0], dA, a_rows, a_cols, lda, a_mn ? 64 : 128);
-  if (s == SB_OK) s = make_tmap_bf16(&tms.b[0], dB, b_rows, b_cols, ldb, b_mn ? 64 : plan_box_rows_b(pl));
+  if (s == SB_OK) s = make_tmap_bf16(&tms.b[0], dB, b_rows, b_cols, ldb, b_mn ? 64 : pl.bn);
   if (s == SB_OK) {
     GemmTcParams p = {};
     p.M = M; p.N = N; p.K = K;
@@ -1775,7 +1766,6 @@ static int debug_gemm_impl(const float* A, const float* B, float* D, int32_t M, 
     else if (!a_mn) s = set_gemm_tc_attrs<EPI_F32, false, true>();
     else s = set_gemm_tc_attrs<EPI_F32, true, true>();
     if (s == SB_OK) s = launch();
-    if (s == SB_OK && iters > 0 && pl.cg != 1) s = set_error(SB_ERR_INVALID, "CTA-pair tiles exist with the fp32 test epilogue only");
     if (s == SB_OK && iters > 0) {
       // benchmark with the REAL epilogue of the layout's use: KM -> forward (bias + relu -> bf16), KK -> dA
       // (act' * , bf16 store, column sums), MM -> dW (fp32 red.add)
@@ -1836,8 +1826,8 @@ static int debug_gemm_impl(const float* A, const float* B, float* D, int32_t M, 
         unsigned long long h[16];
         cudaMemcpy(h, d_tr, sizeof(h), cudaMemcpyDeviceToHost);
         if (a_mn)
-          fprintf(stderr, "[trace] M=%d N=%d K=%d cg=%d bn=%d split=%d single-launch %.2f us | ns since entry:", M, N, K, pl.cg, pl.bn,
-                  pl.split_k, one * 1e3f);
+          fprintf(stderr, "[trace] M=%d N=%d K=%d bn=%d split=%d single-launch %.2f us | ns since entry:", M, N, K, pl.bn, pl.split_k,
+                  one * 1e3f);
         else
           fprintf(stderr, "[trace] M=%d N=%d K=%d ping-pong bm_wg=%d bn=%d single-launch %.2f us | ns since entry:", M, N, K, pp.bm_wg,
                   pp.bn, one * 1e3f);
@@ -1894,7 +1884,7 @@ int sb_debug_gemm_split(const float* A, const float* B, float* D, int32_t M, int
   const GemmPlan pl = plan_gemm(M, N, round_up(K, 64) * p.n_pairs, prop.multiProcessorCount, false);
   TmapSet tms;
   int s = make_tmaps_bf16(tms.a, dA, a_ps, np, M, K, ld, 128);
-  if (s == SB_OK) s = make_tmaps_bf16(tms.b, dB, b_ps, np, N, K, ld, plan_box_rows_b(pl));
+  if (s == SB_OK) s = make_tmaps_bf16(tms.b, dB, b_ps, np, N, K, ld, pl.bn);
   if (s == SB_OK) s = set_gemm_tc_attrs<EPI_F32, false, false>();
   if (s == SB_OK) s = launch_gemm_tc<EPI_F32, false, false>(pl, tms, p, 0);
   if (s == SB_OK) {

@@ -5,6 +5,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string>
+#include <type_traits>
 
 #include "../../include/shifu_b200.h"
 
@@ -35,6 +36,38 @@ int set_error(int code, const char* fmt, ...);
 
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// cudaLaunchKernelEx with the optional programmatic-stream-serialization (PDL) attribute
+template <typename... KArgs, typename... Args>
+int launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, Args... args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
+  SB_CUDA(cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...));
+  return SB_OK;
+}
+
+// opt a kernel in to more than 48 KB of dynamic shared memory (once per process, outside of stream capture)
+template <typename... KArgs>
+int set_max_smem(void (*kernel)(KArgs...), int bytes) {
+  SB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+  return SB_OK;
+}
+
+// f(std::integral_constant<int, act>()): calls the instantiation of f for a run-time activation
+template <typename F>
+int with_act(int act, F&& f) {
+  switch (act) {
+    case SB_ACT_SIGMOID: return f(std::integral_constant<int, SB_ACT_SIGMOID>());
+    case SB_ACT_TANH: return f(std::integral_constant<int, SB_ACT_TANH>());
+    case SB_ACT_RELU: return f(std::integral_constant<int, SB_ACT_RELU>());
+    case SB_ACT_LEAKYRELU: return f(std::integral_constant<int, SB_ACT_LEAKYRELU>());
+    default: return f(std::integral_constant<int, SB_ACT_NONE>());
+  }
+}
 
 // ---- activations (get_activation_fun, res/ssgd_monitor.py:74-88; tf.nn.leaky_relu alpha = 0.2) ----
 #define SB_LEAKY_ALPHA 0.2f

@@ -18,7 +18,7 @@
 //                       db_o), so a step's result does not depend on warp timing
 //   dZ_L              : bf16 pairs into BN/64 128-byte-swizzled 64 x 64 tiles (the output tensor map's layout; conflict
 //                       free for the fragment), one cp.async.bulk.tensor store per tile
-// Producer warpgroup, operand ring, TMA zero fill of the M / N / K tails, setmaxnreg split and PDL as in gemm_tc.cuh.
+// Producer warpgroup, operand ring, main loop, kernel entry and exit: gemm_ring.cuh.
 #pragma once
 #include "gemm_tc.cuh"
 
@@ -31,82 +31,46 @@ struct FwdOutTmaps {
   CUtensorMap o[3];   // dZ_L [rows, N]: box 64 columns x 64 rows (store)
 };
 
+// besides the ring: align slack, barriers, bias + w_o, the two column-sum arrays per warp of a group, z partials
+// [tile parity][group][64], loss / db_o per warp of group 0, dZ_L staging tiles (X_BYTES)
 template <int BN>
-struct FwdOutCfg {
+struct FwdOutCfg : RingCfg<64 * 64 * 2, BN * 64 * 2, 1024 + 256 + 2 * BN * 4 + 4 * 2 * BN * 4 + 2 * 2 * 64 * 4 + 32 + 64 * BN * 2> {
   static_assert(BN == 64 || BN == 128 || BN == 256, "tile N");
+  static_assert(FwdOutCfg::STAGES >= 4, "operand ring");
   static constexpr int BM = 64;
-  static constexpr int BK = 64;
   static constexpr int WN = BN / 2;                 // columns of one consumer warpgroup
-  static constexpr int A_BYTES = BM * BK * 2;       // 8 KB
-  static constexpr int B_BYTES = BN * BK * 2;       // BN / 64 MN-major 64 x 64 boxes
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int X_BYTES = BM * BN * 2;       // dZ_L staging tiles
-  // besides the ring: align slack, barriers, bias + w_o, the two column-sum arrays per warp of a group, z partials
-  // [tile parity][group][64], loss / db_o per warp of group 0
-  static constexpr int FIXED_BYTES = 1024 + 256 + 2 * BN * 4 + 4 * 2 * BN * 4 + 2 * 2 * BM * 4 + 32 + X_BYTES;
-  static constexpr int RING_BUDGET = 232448 - FIXED_BYTES;   // 227 KB of dynamic shared memory per block
-  static constexpr int STAGES = RING_BUDGET / STAGE_BYTES > 8 ? 8 : RING_BUDGET / STAGE_BYTES;
-  static_assert(STAGES >= 4, "operand ring");
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED_BYTES;
   static constexpr int EPI_THREADS = 256;           // the two consumer warpgroups
-  static constexpr int PRODUCER_WARP = 8;
-  static constexpr int THREADS = EPI_THREADS + 128;
-  static constexpr int CONSUMER_REGS = 232;
-  static constexpr int PRODUCER_REGS = 40;
 };
 
 template <int BN, int ACT>
 __global__ void __launch_bounds__(FwdOutCfg<BN>::THREADS, 1)
 gemm_fwd_out_kernel(const __grid_constant__ FwdOutTmaps tms, const GemmTcParams p) {
   using Cfg = FwdOutCfg<BN>;
-  constexpr int BM = Cfg::BM, BK = Cfg::BK, STAGES = Cfg::STAGES, WN = Cfg::WN;
+  constexpr int BM = Cfg::BM, BK = Cfg::BK, WN = Cfg::WN;
 
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // SWIZZLE_128B needs 1024 B alignment
-  const uint32_t xs_base = smem_base + STAGES * Cfg::STAGE_BYTES;     // dZ_L staging tiles (1024-byte aligned)
-  const uint32_t bar_base = xs_base + Cfg::X_BYTES;                   // full[STAGES], empty[STAGES] (8 B each)
-  const uint32_t sm_vec = bar_base + 256u;                            // [bias BN][w_o BN] fp32, 0 beyond N
+  const Ring<Cfg> ring(smem_raw, Cfg::X_BYTES);
+  const uint32_t xs_base = ring.end();                                // dZ_L staging tiles (1024-byte aligned)
+  const uint32_t sm_vec = ring.bars + 256u;                           // [bias BN][w_o BN] fp32, 0 beyond N
   const uint32_t sm_col = sm_vec + 2u * BN * 4u;                      // [warp & 3][db_L BN][dw_o BN] fp32 column sums
   const uint32_t sm_z = sm_col + 4u * 2u * BN * 4u;                   // z partials [tile parity][group][64 rows]
   const uint32_t sm_lw = sm_z + 2u * 2u * BM * 4u;                    // [warp][loss, db_o] of group 0
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto smem_a = [&](int s) { return smem_base + s * Cfg::STAGE_BYTES; };
-  auto smem_b = [&](int s) { return smem_base + s * Cfg::STAGE_BYTES + Cfg::A_BYTES; };
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const bool tracing = p.trace != nullptr && blockIdx.x == 0;
-  auto stamp = [&](int slot) { if (tracing) p.trace[slot] = globaltimer_ns(); };
-  if (threadIdx.x == 0) stamp(0);  // kernel entry
+  const bool tracing = ring_enter(ring, 2, 0, &tms.a[0], &tms.b[0], p);   // one empty arrival per consumer warpgroup
 
   const int np = p.np > 0 ? p.np : 1;
   const int n_pairs = p.n_pairs > 0 ? p.n_pairs : 1;
-  if (warp == Cfg::PRODUCER_WARP && lane == 0) {
-    tma_prefetch_desc(&tms.a[0]);
-    tma_prefetch_desc(&tms.b[0]);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), 1);    // the producer's arrive.expect_tx
-      mbar_init(empty_bar(s), 2);   // one arrival per consumer warpgroup
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) stamp(1);  // setup done
-  pdl_wait();
-  pdl_launch_dependents();
-  if (threadIdx.x == 0) stamp(2);  // dependencies resolved
-
   const int tiles = (p.M + BM - 1) / BM;
   const int part_kb = (p.K + BK - 1) / BK;         // k-blocks of ONE part pair
   const int total_kb = part_kb * n_pairs;          // extended K axis: the pairs one after the other
 
   if (warp >= Cfg::PRODUCER_WARP) {
-    // ================= TMA producer =================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::PRODUCER_REGS));
     if (warp == Cfg::PRODUCER_WARP && lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+      RingPos<Cfg::STAGES> pos;
       const int a_row0 = (p.a_rows != nullptr) ? p.a_rows->row0 : 0;  // batch position inside the resident set
       for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
         for (int kbx = 0; kbx < total_kb; ++kbx) {
@@ -114,18 +78,16 @@ gemm_fwd_out_kernel(const __grid_constant__ FwdOutTmaps tms, const GemmTcParams 
           const int kb = kbx - pp * part_kb;
           const CUtensorMap* tmA = &tms.a[n_pairs > 1 ? p.pair_a[pp] : 0];
           const CUtensorMap* tmB = &tms.b[n_pairs > 1 ? p.pair_b[pp] : 0];
-          mbar_wait(empty_bar(stage), phase ^ 1);
-          const uint32_t fb = full_bar(stage);
-          mbar_arrive_expect_tx(fb, Cfg::STAGE_BYTES);
-          tma_load_2d(smem_a(stage), tmA, fb, kb * BK, t * BM + a_row0);
+          ring_issue(ring, pos, [&](uint32_t fb, uint32_t sa, uint32_t sb) {
+            tma_load_2d(sa, tmA, fb, kb * BK, t * BM + a_row0);
 #pragma unroll
-          for (int j = 0; j < BN / 64; ++j) tma_load_2d(smem_b(stage) + j * 8192, tmB, fb, j * 64, kb * BK);
-          if (kbx == 0 && t == static_cast<int>(blockIdx.x)) stamp(3);  // first TMA issued
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * 8192, tmB, fb, j * 64, kb * BK);
+          });
+          if (kbx == 0 && t == static_cast<int>(blockIdx.x)) ring_stamp(p, tracing, 3);  // first TMA issued
         }
       }
     }
-    __syncwarp();   // the whole warp reaches the final block barrier together (bar.sync counts warps, not lanes)
+    ring_producer_tail<Cfg>(p);
   } else {
     // ================= consumer warpgroups (warps 0..7): MMA, then the fused epilogue of the tile =================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::CONSUMER_REGS));
@@ -156,14 +118,12 @@ gemm_fwd_out_kernel(const __grid_constant__ FwdOutTmaps tms, const GemmTcParams 
     // fragment: rows r0 = 16 (warp & 3) + lane / 4 and r0 + 8; n8 block i holds columns c0 + 8 i + {0, 1}
     const int r0 = (warp & 3) * 16 + (lane >> 2);
     const int c0 = wg * WN + 2 * (lane & 3);
-    float acc[WN / 2];
-    // descriptor steps for 16 elements along K: A K-major = 32 B inside the swizzle row; B MN-major = 16 rows of 128 B.
+    float acc_mi[1][WN / 2];
+    float (&acc)[WN / 2] = acc_mi[0];
     // This group's B columns: the next 64-wide MN atom(s), or for WN = 32 the second half of the 128-byte swizzle rows
     // (the swizzle is a function of the address, so a start 64 B into the row reads columns 32..63).
-    constexpr uint32_t a_kstep = 32u >> 4, b_kstep = 2048u >> 4;
     const uint32_t b_wg_off = WN >= 64 ? static_cast<uint32_t>(wg) * (WN / 64) * 8192u : static_cast<uint32_t>(wg) * 64u;
-    int stage = 0;
-    uint32_t phase = 0;
+    RingPos<Cfg::STAGES> pos;
     int it = 0;
     for (int t = blockIdx.x; t < tiles; t += gridDim.x, ++it) {
       const int row0 = t * BM + r0, row1 = row0 + 8;
@@ -172,27 +132,7 @@ gemm_fwd_out_kernel(const __grid_constant__ FwdOutTmaps tms, const GemmTcParams 
       const float y0 = ok0 ? __ldg(p.desc->y + row0) : 0.f, w0 = ok0 ? __ldg(p.desc->w + row0) : 0.f;
       const float y1 = ok1 ? __ldg(p.desc->y + row1) : 0.f, w1 = ok1 ? __ldg(p.desc->w + row1) : 0.f;
 
-      // ---------- main loop: wgmma over the k-blocks ----------
-      auto release = [&](int s_) { if ((warp & 3) == 0 && lane == 0) mbar_arrive(empty_bar(s_)); };
-      int prev_stage = -1;
-      for (int kb = 0; kb < total_kb; ++kb) {
-        mbar_wait(full_bar(stage), phase);  // the stage's TMA bytes have landed
-        if (kb == 0 && it == 0 && threadIdx.x == 0) stamp(4);  // first stage landed
-        const uint64_t da = make_kmajor_sw128_desc(smem_a(stage));
-        const uint64_t db = make_mnmajor_sw128_desc(smem_b(stage) + b_wg_off, 8192u);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k)
-          wgmma_bf16<WN, 0, 1>(acc, da + a_kstep * k, db + b_kstep * k, (kb > 0 || k > 0) ? 1u : 0u);
-        wgmma_commit();
-        wgmma_wait<1>();   // the previous k-block's wgmma group has finished reading its stage
-        if (prev_stage >= 0) release(prev_stage);
-        prev_stage = stage;
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      wgmma_wait<0>();
-      if (prev_stage >= 0) release(prev_stage);
-      if (it == 0 && threadIdx.x == 0) { stamp(5); stamp(6); }  // first tile's accumulator complete
+      ring_mma<WN, false, true>(ring, pos, total_kb, acc_mi, 0u, b_wg_off, (warp & 3) == 0 && lane == 0, it == 0, p, tracing);
 
       // ---------- (1) a = act(acc + bias), 0 beyond N;  (2) row partials of a . w_o ----------
       float zp0 = 0.f, zp1 = 0.f;
@@ -306,7 +246,7 @@ gemm_fwd_out_kernel(const __grid_constant__ FwdOutTmaps tms, const GemmTcParams 
           tma_store_commit();
         }
       }
-      if (it == 0 && threadIdx.x == 0) stamp(7);  // first tile's epilogue done
+      if (it == 0 && threadIdx.x == 0) ring_stamp(p, tracing, 7);  // first tile's epilogue done
     }
     // loss sum and db_o: one atomic pair per CTA; db_L / dw_o: one red.global per column and CTA (warps added in order)
     if (wg == 0) {
@@ -331,63 +271,34 @@ gemm_fwd_out_kernel(const __grid_constant__ FwdOutTmaps tms, const GemmTcParams 
     }
     if (xthread) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // the last tiles are in global memory
   }
-
-  __syncthreads();
-  if (threadIdx.x == 0) stamp(8);  // all roles finished
-  // in-graph kernel span: slot 2 (dependencies resolved, CTA 0) .. slot 10 (latest exit over ALL CTAs; %globaltimer only
-  // grows, so atomicMax needs no reset between steps)
-  if (p.trace != nullptr && threadIdx.x == 0) atomicMax(p.trace + 10, static_cast<unsigned long long>(globaltimer_ns()));
+  ring_exit(p, tracing);
 }
 
 // ------------------------------------------------------------------ host side
-template <int BN, int ACT>
-static int launch_gemm_fwd_out_one(int grid, const FwdOutTmaps& tms, const GemmTcParams& p, cudaStream_t st, bool pdl) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(static_cast<unsigned>(grid));
-  cfg.blockDim = dim3(FwdOutCfg<BN>::THREADS);
-  cfg.dynamicSmemBytes = FwdOutCfg<BN>::SMEM_BYTES;
-  cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = pdl ? 1 : 0;
-  SB_CUDA(cudaLaunchKernelEx(&cfg, gemm_fwd_out_kernel<BN, ACT>, tms, p));
-  return SB_OK;
+// f(integral_constant BN): the narrowest tile that holds a whole row of A_L (N <= 256); one CTA per SM and 64-row tile
+template <typename F>
+static int with_fwd_out_bn(int N, F&& f) {
+  SB_CHECK(N <= 256, SB_ERR_INVALID, "fused output layer: last hidden layer %d wider than 256", N);
+  if (N <= 64) return f(std::integral_constant<int, 64>());
+  if (N <= 128) return f(std::integral_constant<int, 128>());
+  return f(std::integral_constant<int, 256>());
 }
-
-template <int BN>
-static int launch_gemm_fwd_out_bn(int grid, const FwdOutTmaps& tms, const GemmTcParams& p, cudaStream_t st, bool pdl) {
-  switch (p.act) {
-    case SB_ACT_SIGMOID: return launch_gemm_fwd_out_one<BN, SB_ACT_SIGMOID>(grid, tms, p, st, pdl);
-    case SB_ACT_TANH: return launch_gemm_fwd_out_one<BN, SB_ACT_TANH>(grid, tms, p, st, pdl);
-    case SB_ACT_RELU: return launch_gemm_fwd_out_one<BN, SB_ACT_RELU>(grid, tms, p, st, pdl);
-    case SB_ACT_LEAKYRELU: return launch_gemm_fwd_out_one<BN, SB_ACT_LEAKYRELU>(grid, tms, p, st, pdl);
-    default: return launch_gemm_fwd_out_one<BN, SB_ACT_NONE>(grid, tms, p, st, pdl);
-  }
-}
-
-// the narrowest tile that holds a whole row of A_L (N <= 256); one CTA per SM and 64-row tile
-static inline int fwd_out_bn(int N) { return N <= 64 ? 64 : (N <= 128 ? 128 : 256); }
 
 static int launch_gemm_fwd_out(int grid, const FwdOutTmaps& tms, const GemmTcParams& p, cudaStream_t st, bool pdl) {
-  SB_CHECK(p.N <= 256, SB_ERR_INVALID, "fused output layer: last hidden layer %d wider than 256", p.N);
-  switch (fwd_out_bn(p.N)) {
-    case 64: return launch_gemm_fwd_out_bn<64>(grid, tms, p, st, pdl);
-    case 128: return launch_gemm_fwd_out_bn<128>(grid, tms, p, st, pdl);
-    default: return launch_gemm_fwd_out_bn<256>(grid, tms, p, st, pdl);
-  }
+  return with_fwd_out_bn(p.N, [&](auto BN) {
+    return with_act(p.act, [&](auto ACT) {
+      return launch_kernel(gemm_fwd_out_kernel<BN, ACT>, grid, FwdOutCfg<BN>::THREADS, FwdOutCfg<BN>::SMEM_BYTES, st, pdl, tms, p);
+    });
+  });
 }
 
 // opt in to > 48 KB dynamic shared memory (once per process, outside of stream capture)
 static int set_gemm_fwd_out_attrs() {
-#define SB_ATTR_ACT(BN, ACT) \
-  SB_CUDA(cudaFuncSetAttribute(gemm_fwd_out_kernel<BN, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdOutCfg<BN>::SMEM_BYTES))
-#define SB_ATTR_ALL(BN) SB_ATTR_ACT(BN, SB_ACT_NONE); SB_ATTR_ACT(BN, SB_ACT_SIGMOID); SB_ATTR_ACT(BN, SB_ACT_TANH); \
-                        SB_ATTR_ACT(BN, SB_ACT_RELU); SB_ATTR_ACT(BN, SB_ACT_LEAKYRELU)
-  SB_ATTR_ALL(64); SB_ATTR_ALL(128); SB_ATTR_ALL(256);
-#undef SB_ATTR_ALL
-#undef SB_ATTR_ACT
+  for (int n : {64, 128, 256})
+    for (int act = SB_ACT_NONE; act <= SB_ACT_LEAKYRELU; ++act)
+      SB_TRY(with_fwd_out_bn(n, [&](auto BN) {
+        return with_act(act, [&](auto ACT) { return set_max_smem(gemm_fwd_out_kernel<BN, ACT>, FwdOutCfg<BN>::SMEM_BYTES); });
+      }));
   return SB_OK;
 }
 

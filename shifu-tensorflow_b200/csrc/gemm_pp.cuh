@@ -2,9 +2,8 @@
 //   EPI_FWD : A_l      = act(A_{l-1} W_l + b_l)                 A K-major [rows, in], B = W_l [in, out] MN-major
 //   EPI_DA  : dZ_{l-1} = (dZ_l W_l^T) * act'(A_{l-1}),  db_{l-1} += column sums     A K-major [rows, out], B = W_l K-major
 //
-// Structure (persistent, one CTA per SM, 384 threads = three warpgroups):
-//   warps 8..11: producer warpgroup; one thread fills a STAGES-deep ring of 128-byte-swizzled TMA tiles with the k-blocks of
-//                the CTA's tiles in tile order.  Its other three warps clear the step's gradient buffer when asked to.
+// Producer warpgroup, operand ring, main loop, kernel entry and exit: gemm_ring.cuh.  The producer fills the ring with the
+// k-blocks of the CTA's tiles in tile order.
 //   warps 0..7 : two consumer warpgroups.  Each owns WHOLE tiles of BM_WG x BN: the CTA's tiles alternate between them
 //                (local tile 0, 2, 4, ... -> group 0; 1, 3, 5, ... -> group 1).  A group skips the other's k-blocks when it
 //                advances its ring position.  An ordered pair of named barriers makes the groups take turns issuing their
@@ -36,71 +35,36 @@ struct PpTmaps {
   CUtensorMap x;   // dA: A_{l-1} [M, N] bf16, same box (load)
 };
 
+// besides the ring: align slack, barriers, bias [group][BN], column sums [group][parity][warp][BN], the two epilogue
+// buffers (X_BYTES each)
 template <int BM_WG, int BN>
-struct GemmPpCfg {
+struct GemmPpCfg : RingCfg<BM_WG * 64 * 2, BN * 64 * 2, 1024 + 256 + 2 * BN * 4 + 16 * BN * 4 + 2 * BM_WG * BN * 2> {
   static_assert(BM_WG == 64 || BM_WG == 128, "warpgroup tile rows");
   static_assert(BN == 64 || BN == 128, "tile N");
-  static constexpr int BK = 64;
-  static constexpr int A_BYTES = BM_WG * BK * 2;
-  static constexpr int B_BYTES = BN * BK * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static_assert(GemmPpCfg::STAGES >= 4, "operand ring");
   static constexpr int X_TILE = BM_WG * 128;               // one BM_WG x 64 bf16 swizzled tile
   static constexpr int X_BYTES = X_TILE * (BN / 64);       // one group's epilogue buffer
-  // besides the ring and the two epilogue buffers: align slack, barriers, bias [group][BN], column sums
-  // [group][parity][warp][BN]
-  static constexpr int FIXED_BYTES = 1024 + 256 + 2 * BN * 4 + 16 * BN * 4;
-  static constexpr int RING_BUDGET = 232448 - FIXED_BYTES - 2 * X_BYTES;   // 227 KB of dynamic shared memory per block
-  static constexpr int STAGES = RING_BUDGET / STAGE_BYTES > 8 ? 8 : RING_BUDGET / STAGE_BYTES;
-  static_assert(STAGES >= 4, "operand ring");
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * X_BYTES + FIXED_BYTES;
-  static constexpr int PRODUCER_WARP = 8;
-  static constexpr int THREADS = 384;
-  static constexpr int CONSUMER_REGS = 232;
-  static constexpr int PRODUCER_REGS = 40;
 };
 
 template <int BM_WG, int BN, int EPI, int ACT>
-__global__ void __launch_bounds__(384, 1)
+__global__ void __launch_bounds__(GemmPpCfg<BM_WG, BN>::THREADS, 1)
 gemm_pp_kernel(const __grid_constant__ PpTmaps tms, const GemmTcParams p) {
   static_assert(EPI == EPI_FWD || EPI == EPI_DA, "forward or dA");
   using Cfg = GemmPpCfg<BM_WG, BN>;
-  constexpr int BK = Cfg::BK, STAGES = Cfg::STAGES, MI = BM_WG / 64;
+  constexpr int BK = Cfg::BK, MI = BM_WG / 64;
   constexpr bool B_MN = EPI == EPI_FWD;
 
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // SWIZZLE_128B needs 1024 B alignment
-  const uint32_t xs_base = smem_base + STAGES * Cfg::STAGE_BYTES;     // [group] epilogue buffers (1024-byte aligned)
-  const uint32_t bar_base = xs_base + 2 * Cfg::X_BYTES;               // full[STAGES], empty[STAGES], aux[2] (8 B each)
-  const uint32_t sm_bias = bar_base + 256u;                           // [group][BN] fp32
+  const Ring<Cfg> ring(smem_raw, 2 * Cfg::X_BYTES);
+  const uint32_t xs_base = ring.end();                                // [group] epilogue buffers (1024-byte aligned)
+  const uint32_t sm_bias = ring.bars + 256u;                          // [group][BN] fp32
   const uint32_t sm_col = sm_bias + 2u * BN * 4u;                     // [group][tile parity][warp][BN] fp32
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto aux_bar = [&](int g) { return bar_base + 8u * (2 * STAGES + g); };
-  auto smem_a = [&](int s) { return smem_base + s * Cfg::STAGE_BYTES; };
-  auto smem_b = [&](int s) { return smem_base + s * Cfg::STAGE_BYTES + Cfg::A_BYTES; };
+  auto aux_bar = [&](int g) { return ring.bar(g); };
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const bool tracing = p.trace != nullptr && blockIdx.x == 0;
-  auto stamp = [&](int slot) { if (tracing) p.trace[slot] = globaltimer_ns(); };
-  if (threadIdx.x == 0) stamp(0);  // kernel entry
-
-  if (threadIdx.x == 0) {   // (not the producer thread: its predicate would stay live across the consumer code)
-    tma_prefetch_desc(&tms.a);
-    tma_prefetch_desc(&tms.b);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), 1);    // the producer's arrive.expect_tx
-      mbar_init(empty_bar(s), 1);   // the owning consumer warpgroup
-    }
-    mbar_init(aux_bar(0), 1);
-    mbar_init(aux_bar(1), 1);
-    fence_barrier_init();
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) stamp(1);  // setup done
-  if (!p.no_dep_wait) pdl_wait();
-  pdl_launch_dependents();
-  if (threadIdx.x == 0) stamp(2);  // dependencies resolved
+  // empty: one arrival, by the warpgroup that owns the tile; two own barriers: aux_bar(0), aux_bar(1)
+  const bool tracing = ring_enter(ring, 1, 2, &tms.a, &tms.b, p);
 
   const int tiles_m = (p.M + BM_WG - 1) / BM_WG;
   const int tiles_n = (p.N + BN - 1) / BN;
@@ -108,39 +72,27 @@ gemm_pp_kernel(const __grid_constant__ PpTmaps tms, const GemmTcParams p) {
   const int kb_n = (p.K + BK - 1) / BK;
 
   if (warp >= Cfg::PRODUCER_WARP) {
-    // ================= TMA producer =================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::PRODUCER_REGS));
     if (warp == Cfg::PRODUCER_WARP && lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+      RingPos<Cfg::STAGES> pos;
       const int a_row0 = (p.a_rows != nullptr) ? p.a_rows->row0 : 0;  // batch position inside the resident set
       for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
         const int m0 = (t / tiles_n) * BM_WG, n0 = (t % tiles_n) * BN;
         for (int kb = 0; kb < kb_n; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1);
-          const uint32_t fb = full_bar(stage);
-          mbar_arrive_expect_tx(fb, Cfg::STAGE_BYTES);
-          tma_load_2d(smem_a(stage), &tms.a, fb, kb * BK, m0 + a_row0);
-          if constexpr (B_MN) {
+          ring_issue(ring, pos, [&](uint32_t fb, uint32_t sa, uint32_t sb) {
+            tma_load_2d(sa, &tms.a, fb, kb * BK, m0 + a_row0);
+            if constexpr (B_MN) {
 #pragma unroll
-            for (int j = 0; j < BN / 64; ++j) tma_load_2d(smem_b(stage) + j * 8192, &tms.b, fb, n0 + j * 64, kb * BK);
-          } else {
-            tma_load_2d(smem_b(stage), &tms.b, fb, kb * BK, n0);
-          }
-          if (kb == 0 && t == static_cast<int>(blockIdx.x)) stamp(3);  // first TMA issued
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+              for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * 8192, &tms.b, fb, n0 + j * 64, kb * BK);
+            } else {
+              tma_load_2d(sb, &tms.b, fb, kb * BK, n0);
+            }
+          });
+          if (kb == 0 && t == static_cast<int>(blockIdx.x)) ring_stamp(p, tracing, 3);  // first TMA issued
         }
       }
     }
-    if (warp > Cfg::PRODUCER_WARP && p.zero_buf != nullptr) {
-      // the producer warpgroup's other three warps clear the step's gradient buffer beside the main loop (read by nobody
-      // before the next kernel boundary)
-      const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
-      const long long zt = static_cast<long long>(threadIdx.x) - 32 * (Cfg::PRODUCER_WARP + 1), zn = 32 * 3;
-      for (long long i = static_cast<long long>(blockIdx.x) * zn + zt; i < p.zero_n4; i += static_cast<long long>(gridDim.x) * zn)
-        p.zero_buf[i] = z4;
-    }
-    __syncwarp();   // the whole warp reaches the final block barrier together (bar.sync counts warps, not lanes)
+    ring_producer_tail<Cfg>(p);
   } else {
     // ================= consumer warpgroups: whole tiles, alternating =================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::CONSUMER_REGS));
@@ -162,9 +114,6 @@ gemm_pp_kernel(const __grid_constant__ PpTmaps tms, const GemmTcParams p) {
     const bool do_cols = EPI == EPI_DA && p.colsum != nullptr;
 
     float acc[MI][BN / 2];
-    // descriptor steps for 16 elements along K: K-major = 32 B inside the swizzle row; MN-major = 16 rows of 128 B
-    constexpr uint32_t a_kstep = 32u >> 4;
-    constexpr uint32_t b_kstep = B_MN ? (2048u >> 4) : (32u >> 4);
     for (int lt = g;; lt += 2) {
       const int t = static_cast<int>(blockIdx.x) + lt * static_cast<int>(gridDim.x);
       if (t >= n_tiles) break;
@@ -189,33 +138,11 @@ gemm_pp_kernel(const __grid_constant__ PpTmaps tms, const GemmTcParams p) {
 
       // ---------- main loop, in turn with the other group ----------
       if (lt >= 1) asm volatile("bar.sync %0, 256;" ::"r"(4 + g) : "memory");
-      const int kb_first = lt * kb_n;              // ring position: the k-blocks of every earlier tile of the CTA
-      int stage = kb_first % STAGES;
-      uint32_t phase = static_cast<uint32_t>(kb_first / STAGES) & 1u;
-      int prev_stage = -1;
-      for (int kb = 0; kb < kb_n; ++kb) {
-        mbar_wait(full_bar(stage), phase);  // the stage's TMA bytes have landed
-        if (kb == 0 && lt == 0 && threadIdx.x == 0) stamp(4);  // first stage landed
-        const uint64_t da = make_kmajor_sw128_desc(smem_a(stage));
-        const uint64_t db = B_MN ? make_mnmajor_sw128_desc(smem_b(stage), 8192u) : make_kmajor_sw128_desc(smem_b(stage));
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-#pragma unroll
-          for (int mi = 0; mi < MI; ++mi)   // rows 64 mi .. 64 mi + 63: 64 rows of 128 B further
-            wgmma_bf16<BN, 0, B_MN ? 1 : 0>(acc[mi], da + (8192u >> 4) * mi + a_kstep * k, db + b_kstep * k, (kb > 0 || k > 0) ? 1u : 0u);
-        }
-        wgmma_commit();
-        wgmma_wait<1>();   // the previous k-block's wgmma group has finished reading its stage
-        if (prev_stage >= 0 && xthread) mbar_arrive(empty_bar(prev_stage));
-        prev_stage = stage;
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      // the other group's next tile (local tile lt + 1) may issue now
-      if (t + static_cast<int>(gridDim.x) < n_tiles) asm volatile("bar.arrive %0, 256;" ::"r"(4 + (g ^ 1)) : "memory");
-      wgmma_wait<0>();
-      if (prev_stage >= 0 && xthread) mbar_arrive(empty_bar(prev_stage));
-      if (lt == 0 && threadIdx.x == 0) { stamp(5); stamp(6); }  // first tile's accumulator complete
+      RingPos<Cfg::STAGES> pos = RingPos<Cfg::STAGES>::at(lt * kb_n);   // after the k-blocks of every earlier tile of the CTA
+      ring_mma<BN, false, B_MN>(ring, pos, kb_n, acc, 0u, 0u, xthread, lt == 0, p, tracing, [&] {
+        // the other group's next tile (local tile lt + 1) may issue now
+        if (t + static_cast<int>(gridDim.x) < n_tiles) asm volatile("bar.arrive %0, 256;" ::"r"(4 + (g ^ 1)) : "memory");
+      });
 
       // ---------- epilogue in the fragment layout ----------
       if constexpr (EPI == EPI_FWD) {
@@ -291,16 +218,11 @@ gemm_pp_kernel(const __grid_constant__ PpTmaps tms, const GemmTcParams p) {
           if (n0 + j < p.N && v != 0.f) red_add_f32(p.colsum + n0 + j, v);
         }
       }
-      if (lt == 0 && threadIdx.x == 0) stamp(7);  // first tile's epilogue done
+      if (lt == 0 && threadIdx.x == 0) ring_stamp(p, tracing, 7);  // first tile's epilogue done
     }
     if (xthread) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // the last tiles are in global memory
   }
-
-  __syncthreads();
-  if (threadIdx.x == 0) stamp(8);  // all roles finished
-  // in-graph kernel span: slot 2 (dependencies resolved, CTA 0) .. slot 10 (latest exit over ALL CTAs; %globaltimer only
-  // grows, so atomicMax needs no reset between steps)
-  if (p.trace != nullptr && threadIdx.x == 0) atomicMax(p.trace + 10, static_cast<unsigned long long>(globaltimer_ns()));
+  ring_exit(p, tracing);
 }
 
 // ------------------------------------------------------------------ host side
@@ -327,55 +249,40 @@ static inline PpPlan plan_gemm_pp(int M, int N, int K, int num_sms, int bm_wg = 
   return pl;
 }
 
-template <int BM_WG, int BN, int EPI, int ACT>
-static int launch_gemm_pp_one(const PpPlan& pl, const PpTmaps& tms, const GemmTcParams& p, cudaStream_t st, bool pdl) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(static_cast<unsigned>(pl.grid));
-  cfg.blockDim = dim3(GemmPpCfg<BM_WG, BN>::THREADS);
-  cfg.dynamicSmemBytes = GemmPpCfg<BM_WG, BN>::SMEM_BYTES;
-  cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = pdl ? 1 : 0;
-  SB_CUDA(cudaLaunchKernelEx(&cfg, gemm_pp_kernel<BM_WG, BN, EPI, ACT>, tms, p));
-  return SB_OK;
-}
-
-template <int BM_WG, int BN, int EPI>
-static int launch_gemm_pp_act(const PpPlan& pl, const PpTmaps& tms, const GemmTcParams& p, cudaStream_t st, bool pdl) {
-  switch (p.act) {
-    case SB_ACT_SIGMOID: return launch_gemm_pp_one<BM_WG, BN, EPI, SB_ACT_SIGMOID>(pl, tms, p, st, pdl);
-    case SB_ACT_TANH: return launch_gemm_pp_one<BM_WG, BN, EPI, SB_ACT_TANH>(pl, tms, p, st, pdl);
-    case SB_ACT_RELU: return launch_gemm_pp_one<BM_WG, BN, EPI, SB_ACT_RELU>(pl, tms, p, st, pdl);
-    case SB_ACT_LEAKYRELU: return launch_gemm_pp_one<BM_WG, BN, EPI, SB_ACT_LEAKYRELU>(pl, tms, p, st, pdl);
-    default: return launch_gemm_pp_one<BM_WG, BN, EPI, SB_ACT_NONE>(pl, tms, p, st, pdl);
-  }
+// f(integral_constant BM_WG, integral_constant BN) for a plan's tile shape
+template <typename F>
+static int with_pp_shape(int bm_wg, int bn, F&& f) {
+  using std::integral_constant;
+  if (bm_wg == 128 && bn == 128) return f(integral_constant<int, 128>(), integral_constant<int, 128>());
+  if (bm_wg == 128 && bn == 64) return f(integral_constant<int, 128>(), integral_constant<int, 64>());
+  if (bm_wg == 64 && bn == 128) return f(integral_constant<int, 64>(), integral_constant<int, 128>());
+  if (bm_wg == 64 && bn == 64) return f(integral_constant<int, 64>(), integral_constant<int, 64>());
+  return set_error(SB_ERR_INVALID, "no gemm_pp instantiation for bm_wg=%d bn=%d", bm_wg, bn);
 }
 
 // tensor maps (pl.bm_wg-row boxes) must have been made for the same plan
 template <int EPI>
 static int launch_gemm_pp(const PpPlan& pl, const PpTmaps& tms, const GemmTcParams& p, cudaStream_t st, bool pdl) {
-  if (pl.bm_wg == 128 && pl.bn == 128) return launch_gemm_pp_act<128, 128, EPI>(pl, tms, p, st, pdl);
-  if (pl.bm_wg == 128 && pl.bn == 64) return launch_gemm_pp_act<128, 64, EPI>(pl, tms, p, st, pdl);
-  if (pl.bm_wg == 64 && pl.bn == 128) return launch_gemm_pp_act<64, 128, EPI>(pl, tms, p, st, pdl);
-  if (pl.bm_wg == 64 && pl.bn == 64) return launch_gemm_pp_act<64, 64, EPI>(pl, tms, p, st, pdl);
-  return set_error(SB_ERR_INVALID, "no gemm_pp instantiation for bm_wg=%d bn=%d", pl.bm_wg, pl.bn);
+  return with_pp_shape(pl.bm_wg, pl.bn, [&](auto BM_WG, auto BN) {
+    return with_act(p.act, [&](auto ACT) {
+      using Cfg = GemmPpCfg<BM_WG, BN>;
+      return launch_kernel(gemm_pp_kernel<BM_WG, BN, EPI, ACT>, pl.grid, Cfg::THREADS, Cfg::SMEM_BYTES, st, pdl, tms, p);
+    });
+  });
 }
 
 // opt in to > 48 KB dynamic shared memory (once per process, outside of stream capture)
 static int set_gemm_pp_attrs() {
-#define SB_ATTR_ACT(BM, BN, EPI, ACT) \
-  SB_CUDA(cudaFuncSetAttribute(gemm_pp_kernel<BM, BN, EPI, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmPpCfg<BM, BN>::SMEM_BYTES))
-#define SB_ATTR_ALL(BM, BN, EPI) SB_ATTR_ACT(BM, BN, EPI, SB_ACT_NONE); SB_ATTR_ACT(BM, BN, EPI, SB_ACT_SIGMOID); \
-  SB_ATTR_ACT(BM, BN, EPI, SB_ACT_TANH); SB_ATTR_ACT(BM, BN, EPI, SB_ACT_RELU); SB_ATTR_ACT(BM, BN, EPI, SB_ACT_LEAKYRELU)
-#define SB_ATTR_EPI(EPI) SB_ATTR_ALL(128, 128, EPI); SB_ATTR_ALL(128, 64, EPI); SB_ATTR_ALL(64, 128, EPI); SB_ATTR_ALL(64, 64, EPI)
-  SB_ATTR_EPI(EPI_FWD);
-  SB_ATTR_EPI(EPI_DA);
-#undef SB_ATTR_EPI
-#undef SB_ATTR_ALL
-#undef SB_ATTR_ACT
+  for (int bm_wg : {64, 128})
+    for (int bn : {64, 128})
+      for (int act = SB_ACT_NONE; act <= SB_ACT_LEAKYRELU; ++act)
+        SB_TRY(with_pp_shape(bm_wg, bn, [&](auto BM_WG, auto BN) {
+          return with_act(act, [&](auto ACT) {
+            const int bytes = GemmPpCfg<BM_WG, BN>::SMEM_BYTES;
+            SB_TRY(set_max_smem(gemm_pp_kernel<BM_WG, BN, EPI_FWD, ACT>, bytes));
+            return set_max_smem(gemm_pp_kernel<BM_WG, BN, EPI_DA, ACT>, bytes);
+          });
+        }));
   return SB_OK;
 }
 

@@ -18,78 +18,17 @@
 // GEMMs are gemm_pp.cuh, the last hidden GEMM of a training step with the output layer fused into its epilogue is
 // gemm_fwd_out.cuh.
 //
-// Tile: one CTA owns 128 x BN (BN = 64 | 128 | 256).  CG = 2: a cluster of two CTAs owns 256 x BN; both need the same B tile,
-// so each loads half of it and TMA multicasts that half into both CTAs' shared memory (half the B traffic from L2 per CTA).
-// A stage is then refilled only after the consumers of BOTH CTAs have released it (remote mbarrier arrivals).
-//
-// Structure (persistent, one CTA per SM, 384 threads = three warpgroups):
-//   warps 0..7 : two consumer warpgroups.  Warpgroup g multiplies rows 64 g .. 64 g + 63 of the tile with wgmma.m64nBNk16
-//                (accumulator in registers, one wgmma group in flight while the stage before it is released), then both
-//                run the epilogue.  The epilogue is written thread-owns-row: warp w takes the 32 rows of quarter w & 3 and
-//                every other 32-column chunk (parity w >> 2).  The accumulator reaches that layout through a padded
-//                128 x 64 fp32 block in shared memory, one 64-column block at a time.
-//   warps 8..11: producer warpgroup; one thread issues cp.async.bulk.tensor 128B-swizzled tiles into a STAGES-deep smem
-//                ring and runs ahead into the next tile while the consumers are in the epilogue.  The group gives its
-//                registers to the consumers (setmaxnreg), whose 128 x BN accumulator lives in registers.
-// M/N/K tails need no special code on the load side: TMA zero-fills out-of-bounds box elements.
+// Tile: one CTA owns 128 x BN (BN = 64 | 128).  Producer warpgroup, operand ring, main loop, kernel entry and exit:
+// gemm_ring.cuh.  Warpgroup g multiplies rows 64 g .. 64 g + 63 of the tile with wgmma.m64nBNk16, then both run the
+// epilogue while the producer runs ahead into the next tile.  The epilogue is written thread-owns-row: warp w takes the
+// 32 rows of quarter w & 3 and every other 32-column chunk (parity w >> 2).  The accumulator reaches that layout through a
+// padded 128 x 64 fp32 block in shared memory, one 64-column block at a time.
 #pragma once
-#include <cuda.h>
-#include "common.cuh"
-#include "ptx.cuh"
-#include "kernels.cuh"
+#include "gemm_ring.cuh"
 
 namespace sb {
 
 enum { EPI_FWD = 0, EPI_DA = 1, EPI_DW = 2, EPI_F32 = 3 };
-
-struct GemmTcParams {
-  int M, N, K;
-  int kb_per_split;  // k-blocks (of 64) per split
-  int split_k;       // number of splits actually used (all non-empty)
-  int no_dep_wait;   // 1: do not wait for the programmatic primary (an exchange kernel this GEMM may run beside, capi.cu);
-                     // every real dependency of the launch is then a full one
-  // EPI_FWD
-  const float* bias;  // [N]
-  int act;            // FWD: activation applied; DA: activation whose derivative is applied
-  __nv_bfloat16* out;  // [M, ld_out] row-major (FWD, DA)
-  int ld_out;
-  // EPI_DA
-  const __nv_bfloat16* aux;  // activation output A_{l-1} [M, ld_aux]
-  int ld_aux;
-  float* colsum;  // [N] fp32, atomically accumulated (bias gradient), nullable
-  // EPI_DW / EPI_F32
-  float* accum;  // [M, ld_acc] fp32
-  int ld_acc;
-  int acc_vec4;  // 1 if 16-byte aligned rows -> red.global.add.v4.f32
-  // fused output layer (gemm_fwd_out_kernel: output layer + loss + its backward, res/ssgd_monitor.py:121,129)
-  const float* wo;          // [N] output-layer weights (fp32)
-  const float* bo;          // [1]
-  const BatchDesc* desc;    // y, w of the current batch
-  float* scal;              // SCAL_LOSS_SUM / SCAL_NNZ
-  int loss;                 // sb_loss
-  float *g_wo, *g_bo, *g_bL;  // gradient slots: dw_o [N], db_o [1], db_L [N]
-  const BatchDesc* a_rows;  // non-null: operand A lives in the HBM-resident set; add a_rows->row0 to its row coordinate
-  // optional: the producer warpgroup's idle warps clear this buffer (16-byte units) beside the main loop.  Used by the
-  // layer-0 forward GEMM of a resident step to clear the step's gradient buffer (no memset node on the chain).
-  float4* zero_buf;
-  long long zero_n4;
-  unsigned long long* trace;  // debug: CTA 0 writes %globaltimer stamps of its pipeline milestones (nullable)
-  // Split-precision modes (SB_PREC_FP32_TC / SB_PREC_BF16X2, net.cuh): every fp32 operand value is held as np bf16 PARTS
-  // v = p0 + p1 (+ p2) in np equally shaped arrays; the contraction is then a plain bf16 GEMM over an EXTENDED K axis that
-  // walks the part pairs (a_i, b_j) with i + j < np one after the other, all accumulating into the same fp32 tile:
-  //   np = 2 : a0b0 + a0b1 + a1b0                        (relative error ~2^-17 per product)
-  //   np = 3 : a0b0 + a0b1 + a1b0 + a0b2 + a1b1 + a2b0   (~2^-24: fp32-class, what TF-CPU's fp32 GEMM delivers)
-  // The MMA issuer does not know about it; the TMA producer picks the pair's tensor maps per k-block.
-  int np;                     // parts per value in `out` / `aux` (1 = plain bf16)
-  int n_pairs;                // part pairs accumulated (1, 3 or 6); 0 is read as 1
-  unsigned char pair_a[6], pair_b[6];
-  long long out_ps, aux_ps;   // element stride between consecutive parts of `out` / `aux`
-  // EPI_FWD, nullable: fp32 [M, ld_add] added to the pre-activation before bias + activation.  Wide+deep first layer:
-  // the sum of the embedding rows of the row's categorical values, i.e. the one-hot block of Z_0 = X W_0 evaluated as a
-  // gather (oracle/wide_deep.py) while this GEMM contracts only the dense columns.
-  const float* addend;
-  int ld_add;
-};
 
 // tensor maps of the parts of both operands (one kernel parameter, 768 B)
 struct TmapSet {
@@ -97,38 +36,19 @@ struct TmapSet {
   CUtensorMap b[3];
 };
 
-template <int BN, int CG>
-struct GemmTcCfg {
-  static_assert(CG == 1 || CG == 2, "cta group");
-  static_assert(BN == 64 || BN == 128 || BN == 256, "tile N");
-  static_assert(CG == 1 || BN >= 128, "pair tiles need BN >= 128 (each CTA stages BN/2 >= 64 rows of B)");
-  static constexpr int BM = 128;        // rows of the tile owned by ONE CTA
-  static constexpr int TILE_M = BM * CG;  // rows of the (pair) tile
-  static constexpr int BK = 64;         // 64 bf16 = 128 B = one swizzle row
-  static constexpr int BN_CTA = BN / CG;  // B rows staged by one CTA
-  static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = BN * BK * 2;    // (pair: this CTA's BN_CTA rows and the peer's, multicast)
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+// shared memory besides the ring: align slack, barriers, epilogue scratch, bias, per-warp transpose tiles (TR_BYTES),
+// column-sum accumulators, accumulator block (ACC_BYTES)
+template <int BN>
+struct GemmTcCfg : RingCfg<128 * 64 * 2, BN * 64 * 2, 1024 + 256 + 2048 + 2048 + 8 * 2048 + 4096 + 128 * (64 + 4) * 4> {
+  static_assert(BN == 64 || BN == 128, "tile N");
+  static_assert(GemmTcCfg::STAGES >= 2, "operand ring");
+  static constexpr int BM = 128;
   // accumulator staging block: 128 rows x 64 fp32 columns, rows padded by 16 B so that both the fragment stores and the
   // row-wise 16-byte loads are free of bank conflicts
   static constexpr int ACC_LD = 64 + 4;
   static constexpr int ACC_BYTES = BM * ACC_LD * 4;
-  // shared memory besides the operand ring: align slack, barriers, epilogue scratch, bias, per-warp transpose tiles,
-  // column-sum accumulators, accumulator block
   static constexpr int TR_BYTES = 8 * 2048;
-  static constexpr int FIXED_BYTES = 1024 + 256 + 2048 + 2048 + TR_BYTES + 4096 + ACC_BYTES;
-  static constexpr int RING_BUDGET = 232448 - FIXED_BYTES;   // 227 KB of dynamic shared memory per block
-  static constexpr int STAGES = RING_BUDGET / STAGE_BYTES > 8 ? 8 : RING_BUDGET / STAGE_BYTES;
-  static_assert(STAGES >= 2, "operand ring");
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED_BYTES;
-  static_assert(SMEM_BYTES <= 232448, "shared memory budget");
-  static constexpr int EPI_WARPS = 8;                 // the two consumer warpgroups
-  static constexpr int EPI_THREADS = 32 * EPI_WARPS;
-  static constexpr int PRODUCER_WARP = EPI_WARPS;     // first warp of the producer warpgroup
-  static constexpr int THREADS = EPI_THREADS + 128;
-  // per-thread registers after setmaxnreg: 2 x 128 x 232 + 128 x 40 <= 64 K
-  static constexpr int CONSUMER_REGS = 232;
-  static constexpr int PRODUCER_REGS = 40;
+  static constexpr int EPI_THREADS = 256;   // the two consumer warpgroups
 };
 
 // ---- epilogue element functions, specialised per activation so the switch is hoisted out of the element loop
@@ -145,117 +65,66 @@ __device__ __forceinline__ void epi_da_chunk(float (&v)[32], const __nv_bfloat16
 
 // GENERIC = true adds the cold features at compile time: split-precision part stores / loads (np > 1) and the fp32 addend
 // of the wide+deep first layer.  EPI_FWD / EPI_DA are instantiated with it only.
-template <int BN, int EPI, bool A_MN, bool B_MN, int CG, bool GENERIC = false>
-__global__ void __launch_bounds__((GemmTcCfg<BN, CG>::THREADS), 1)
+template <int BN, int EPI, bool A_MN, bool B_MN, bool GENERIC = false>
+__global__ void __launch_bounds__(GemmTcCfg<BN>::THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
-  using Cfg = GemmTcCfg<BN, CG>;
+  using Cfg = GemmTcCfg<BN>;
   const int act_sel = p.act;
-  constexpr int BM = Cfg::BM, BK = Cfg::BK, STAGES = Cfg::STAGES, TILE_M = Cfg::TILE_M, BN_CTA = Cfg::BN_CTA;
+  constexpr int BM = Cfg::BM, BK = Cfg::BK;
 
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B needs 1024 B alignment
-  const uint32_t accs_base = smem_base + STAGES * Cfg::STAGE_BYTES;            // accumulator staging block
-  const uint32_t bar_base = accs_base + Cfg::ACC_BYTES;
-  // barrier layout (8 B each): full[STAGES], empty[STAGES]; then scratch
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  const uint32_t scratch = bar_base + 8u * (2 * STAGES) + 16u;
-  auto smem_a = [&](int s) { return smem_base + s * Cfg::STAGE_BYTES; };
-  auto smem_b = [&](int s) { return smem_base + s * Cfg::STAGE_BYTES + Cfg::A_BYTES; };
+  const Ring<Cfg> ring(smem_raw, Cfg::ACC_BYTES);
+  const uint32_t accs_base = ring.end();            // accumulator staging block
+  const uint32_t scratch = ring.bar(0) + 16u;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const bool tracing = p.trace != nullptr && blockIdx.x == 0;
-  auto stamp = [&](int slot) { if (tracing) p.trace[slot] = globaltimer_ns(); };
-  if (threadIdx.x == 0) stamp(0);  // kernel entry
+  const bool tracing = ring_enter(ring, 2, 0, &tms.a[0], &tms.b[0], p);   // one empty arrival per consumer warpgroup
 
   const int n_pairs = p.n_pairs > 0 ? p.n_pairs : 1;
-  if (warp == Cfg::PRODUCER_WARP && lane == 0) {
-    tma_prefetch_desc(&tms.a[0]);
-    tma_prefetch_desc(&tms.b[0]);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), 1);   // the producer's arrive.expect_tx
-      mbar_init(empty_bar(s), 2 * CG);  // one arrival per consumer warpgroup (of both CTAs of a pair)
-    }
-    fence_barrier_init();
-  }
-  const uint32_t rank = (CG == 2) ? cluster_ctarank() : 0u;  // CTA rank inside the pair
-  if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();   // (pair: the peer's barriers exist before any multicast)
-  // PDL: everything above (barrier init, descriptor prefetch) overlapped the previous kernel's tail; from here on global
-  // memory written by it is touched.
-  if (threadIdx.x == 0) stamp(1);  // setup done
-  if (!p.no_dep_wait) pdl_wait();
-  pdl_launch_dependents();
-  if (threadIdx.x == 0) stamp(2);  // dependencies resolved
-
-  const int tiles_m = (p.M + TILE_M - 1) / TILE_M;
+  const int tiles_m = (p.M + BM - 1) / BM;
   const int tiles_n = (p.N + BN - 1) / BN;
   const int n_tiles = tiles_m * tiles_n;
   const int n_work = n_tiles * p.split_k;
   const int part_kb = (p.K + BK - 1) / BK;         // k-blocks of ONE part pair
   const int total_kb = part_kb * n_pairs;          // extended K axis: the pairs one after the other
-  const int w_first = blockIdx.x / CG;             // work items are per CTA (CG = 1) or per pair (CG = 2)
-  const int w_step = gridDim.x / CG;
+  const int w_first = blockIdx.x;
 
   if (warp >= Cfg::PRODUCER_WARP) {
-    // ================= TMA producer =================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::PRODUCER_REGS));
     if (warp == Cfg::PRODUCER_WARP && lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+      RingPos<Cfg::STAGES> pos;
       const int a_row0 = (p.a_rows != nullptr) ? p.a_rows->row0 : 0;  // batch position inside the resident set
-      for (int w = w_first; w < n_work; w += w_step) {
+      for (int w = w_first; w < n_work; w += gridDim.x) {
         const int tile = w % n_tiles, ks = w / n_tiles;
-        const int tm = tile / tiles_n, tn = tile % tiles_n;
+        const int m0 = (tile / tiles_n) * BM, n0 = (tile % tiles_n) * BN;
         const int kb0 = ks * p.kb_per_split;
         const int kb1 = min(total_kb, kb0 + p.kb_per_split);
-        const int m0 = tm * TILE_M + static_cast<int>(rank) * BM;      // this CTA's rows of A
-        const int n0 = tn * BN + static_cast<int>(rank) * BN_CTA;      // this CTA's share of the B tile
         for (int kbx = kb0; kbx < kb1; ++kbx) {
           const int pp = (n_pairs > 1) ? kbx / part_kb : 0;     // which part pair this k-block belongs to
           const int kb = kbx - pp * part_kb;
           const CUtensorMap* tmA = &tms.a[n_pairs > 1 ? p.pair_a[pp] : 0];
           const CUtensorMap* tmB = &tms.b[n_pairs > 1 ? p.pair_b[pp] : 0];
-          mbar_wait(empty_bar(stage), phase ^ 1);
-          const uint32_t fb = full_bar(stage);
-          mbar_arrive_expect_tx(fb, Cfg::STAGE_BYTES);
-          auto load = [&](uint32_t dst, const CUtensorMap* tm_, int c0, int c1) { tma_load_2d(dst, tm_, fb, c0, c1); };
-          if constexpr (A_MN) {
+          ring_issue(ring, pos, [&](uint32_t fb, uint32_t sa, uint32_t sb) {
+            if constexpr (A_MN) {
 #pragma unroll
-            for (int i = 0; i < BM / 64; ++i)  // 64(MN) x 64(K) boxes, 8 KB each, side by side along MN
-              load(smem_a(stage) + i * 8192, tmA, m0 + i * 64, kb * BK + a_row0);   // rows of the set = K here
-          } else {
-            load(smem_a(stage), tmA, kb * BK, m0 + a_row0);
-          }
-          if constexpr (CG == 2) {   // this CTA's half of the B tile, into both CTAs
+              for (int i = 0; i < BM / 64; ++i)  // 64(MN) x 64(K) boxes, 8 KB each, side by side along MN
+                tma_load_2d(sa + i * 8192, tmA, fb, m0 + i * 64, kb * BK + a_row0);   // rows of the set = K here
+            } else {
+              tma_load_2d(sa, tmA, fb, kb * BK, m0 + a_row0);
+            }
             if constexpr (B_MN) {
 #pragma unroll
-              for (int j = 0; j < BN_CTA / 64; ++j)
-                tma_load_2d_mc(smem_b(stage) + (rank * (BN_CTA / 64) + j) * 8192, tmB, fb, n0 + j * 64, kb * BK, 3);
+              for (int i = 0; i < BN / 64; ++i) tma_load_2d(sb + i * 8192, tmB, fb, n0 + i * 64, kb * BK);
             } else {
-              tma_load_2d_mc(smem_b(stage) + rank * BN_CTA * 128, tmB, fb, kb * BK, n0, 3);
+              tma_load_2d(sb, tmB, fb, kb * BK, n0);
             }
-          } else if constexpr (B_MN) {
-#pragma unroll
-            for (int i = 0; i < BN_CTA / 64; ++i)
-              load(smem_b(stage) + i * 8192, tmB, n0 + i * 64, kb * BK);
-          } else {
-            load(smem_b(stage), tmB, kb * BK, n0);
-          }
-          if (kbx == kb0 && w == w_first) stamp(3);  // first TMA issued
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          });
+          if (kbx == kb0 && w == w_first) ring_stamp(p, tracing, 3);  // first TMA issued
         }
       }
     }
-    if (warp > Cfg::PRODUCER_WARP && p.zero_buf != nullptr) {
-      // the producer warpgroup's other three warps clear the step's gradient buffer beside the main loop (read by nobody
-      // before the next kernel boundary)
-      const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
-      const long long zt = static_cast<long long>(threadIdx.x) - 32 * (Cfg::PRODUCER_WARP + 1), zn = 32 * 3;
-      for (long long i = static_cast<long long>(blockIdx.x) * zn + zt; i < p.zero_n4; i += static_cast<long long>(gridDim.x) * zn)
-        p.zero_buf[i] = z4;
-    }
-    __syncwarp();   // the whole warp reaches the final block barrier together (bar.sync counts warps, not lanes)
+    ring_producer_tail<Cfg>(p);
   } else {
     // ================= consumer warpgroups (warps 0..7): MMA, then the epilogue of the tile =================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::CONSUMER_REGS));
@@ -324,7 +193,8 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
     };
 
     // ---- accumulator: registers of the wgmma fragment, handed to the epilogue one 64-column block at a time
-    float acc[BN / 2];
+    float acc_mi[1][BN / 2];
+    float (&acc)[BN / 2] = acc_mi[0];
     // write columns 64 j .. 64 j + 63 of the fragment to the staging block (every consumer warp calls this together; the
     // first barrier waits for the readers of the previous block).  j selects among unrolled copies so that acc[] stays in
     // registers.
@@ -357,20 +227,16 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
                      : "r"(a + 16u * q) : "memory");
     };
 
-    // descriptor step for 16 elements along K: K-major = 32 B inside the swizzle row; MN-major = 16 rows of 128 B
-    constexpr uint32_t a_kstep = A_MN ? (2048u >> 4) : (32u >> 4);
-    constexpr uint32_t b_kstep = B_MN ? (2048u >> 4) : (32u >> 4);
     // this warpgroup's 64 rows of the A stage: K-major = 64 rows of 128 B further; MN-major = the second 64-wide MN atom
     const uint32_t a_wg_off = static_cast<uint32_t>(wg) * 8192u;
-    int stage = 0;
-    uint32_t phase = 0;
+    RingPos<Cfg::STAGES> pos;
     int it = 0;
-    for (int w = w_first; w < n_work; w += w_step, ++it) {
+    for (int w = w_first; w < n_work; w += gridDim.x, ++it) {
       const int tile = w % n_tiles, ks = w / n_tiles;
       const int tm = tile / tiles_n, tn = tile % tiles_n;
       const int kb0 = ks * p.kb_per_split;
       const int kb1 = min(total_kb, kb0 + p.kb_per_split);
-      const int row = tm * TILE_M + static_cast<int>(rank) * BM + quarter * 32 + lane;  // output row of this thread
+      const int row = tm * BM + quarter * 32 + lane;  // output row of this thread
       const bool row_ok = row < p.M;
       // operands of the epilogue that do not depend on the accumulator are fetched BEFORE the main loop: the A_{l-1} tiles
       // of the dA epilogue
@@ -378,7 +244,7 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
       // kept in registers as a shift queue, so that one L2 / HBM latency is paid per tile instead of one per chunk
       constexpr int AUXQ = EPI == EPI_DA ? (BN / 64 > 0 ? BN / 64 : 1) : 1;
       uint4 aux_q[AUXQ][4];
-      const int row_base = tm * TILE_M + static_cast<int>(rank) * BM + quarter * 32;   // first row of this warp's 32
+      const int row_base = tm * BM + quarter * 32;   // first row of this warp's 32
       // store a 32 x 64 B tile held one-row-per-thread (4 pieces each) to a row-major bf16 matrix, coalesced
       auto store_rows_bf16 = [&](const uint4 (&mine)[4], __nv_bfloat16* base, int ld, int col0_, bool all_cols) {
         uint4 oc[4];
@@ -446,34 +312,7 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
         bar_all();
       }
 
-      // ---------- main loop: wgmma over the k-blocks of this work item ----------
-      // one arrival per warpgroup on the stage's empty barrier - in both CTAs of a pair, whose producers both fill it
-      auto release = [&](int s_) {
-        if ((warp & 3) == 0 && lane == 0) {
-          mbar_arrive(empty_bar(s_));
-          if constexpr (CG == 2) mbar_arrive_cluster(empty_bar(s_), rank ^ 1u);
-        }
-      };
-      int prev_stage = -1;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(full_bar(stage), phase);  // the stage's TMA bytes have landed
-        if (kb == kb0 && w == w_first && threadIdx.x == 0) stamp(4);  // first stage landed
-        const uint32_t sa = smem_a(stage) + a_wg_off, sbb = smem_b(stage);
-        const uint64_t da = A_MN ? make_mnmajor_sw128_desc(sa, 8192u) : make_kmajor_sw128_desc(sa);
-        const uint64_t db = B_MN ? make_mnmajor_sw128_desc(sbb, 8192u) : make_kmajor_sw128_desc(sbb);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k)
-          wgmma_bf16<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da + a_kstep * k, db + b_kstep * k, (kb > kb0 || k > 0) ? 1u : 0u);
-        wgmma_commit();
-        wgmma_wait<1>();   // the previous k-block's wgmma group has finished reading its stage
-        if (prev_stage >= 0) release(prev_stage);
-        prev_stage = stage;
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      wgmma_wait<0>();
-      if (prev_stage >= 0) release(prev_stage);
-      if (w == w_first && threadIdx.x == 0) { stamp(5); stamp(6); }  // first tile's accumulator complete
+      ring_mma<BN, A_MN, B_MN>(ring, pos, kb1 - kb0, acc_mi, a_wg_off, 0u, (warp & 3) == 0 && lane == 0, w == w_first, p, tracing);
 
 #pragma unroll 1
       for (int c = half; (c >> 1) < nblk; c += 2) {
@@ -610,16 +449,10 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
       if constexpr (EPI == EPI_DA) {
         if (p.colsum != nullptr) flush_cols(it, tn, p.colsum);
       }
-      if (w == w_first && threadIdx.x == 0) stamp(7);  // first tile's epilogue done
+      if (w == w_first && threadIdx.x == 0) ring_stamp(p, tracing, 7);  // first tile's epilogue done
     }
   }
-
-  // (pair: no CTA exits while its peer may still multicast into it or arrive on its barriers)
-  if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
-  if (threadIdx.x == 0) stamp(8);  // all roles finished
-  // in-graph kernel span: slot 2 (dependencies resolved, CTA 0) .. slot 10 (latest exit over ALL CTAs; %globaltimer only
-  // grows, so atomicMax needs no reset between steps)
-  if (p.trace != nullptr && threadIdx.x == 0) atomicMax(p.trace + 10, static_cast<unsigned long long>(globaltimer_ns()));
+  ring_exit(p, tracing);
 }
 
 // ------------------------------------------------------------------ host side
@@ -631,7 +464,7 @@ PFN_encodeTiled get_encode_tiled();
 // Tensor map of a row-major bf16 matrix [rows, cols] with leading dimension ld (elements):
 // box = 64 columns x box_rows rows, 128-byte swizzle.  cols/rows are the LOGICAL extents (TMA zero-fills beyond
 // them), ld*2 must be a multiple of 16 bytes.  K-major operand: box_rows = rows one CTA stages (128 for A,
-// BN / CG for B); MN-major operand: 64.
+// BN for B); MN-major operand: 64.
 int make_tmap_bf16(CUtensorMap* out, const void* base, int rows, int cols, int ld, int box_rows);
 // the same map for each of np part arrays that lie part_stride ELEMENTS apart (np = 1: just the one)
 int make_tmaps_bf16(CUtensorMap* out3, const void* base, long long part_stride, int np, int rows, int cols, int ld, int box_rows);
@@ -640,13 +473,35 @@ void set_part_pairs(GemmTcParams* p, int np);
 
 // Tile configuration chosen per problem.
 struct GemmPlan {
-  int cg;            // 1, or 2: a cluster of two CTAs per 256 x bn tile, B multicast
-  int bn;            // 64 / 128 / 256
+  int bn;            // 64 / 128
   int split_k, kb_per_split;
-  int grid;          // CTAs to launch (a multiple of cg)
+  int grid;          // CTAs to launch
 };
 GemmPlan plan_gemm(int M, int N, int K, int num_sms, bool allow_split);
 
-// launch_gemm_tc<EPI, A_MN, B_MN>(plan, tmA, tmB, params, stream, pdl) lives in gemm_tc_launch.cuh
+template <int EPI, bool A_MN, bool B_MN>
+int launch_gemm_tc(const GemmPlan& pl, const TmapSet& tms, GemmTcParams p, cudaStream_t st, bool pdl = false) {
+  if (p.np < 1) p.np = 1;
+  if (p.n_pairs < 1) p.n_pairs = 1;
+  p.split_k = pl.split_k;
+  p.kb_per_split = pl.kb_per_split;
+  // forward / dA: split-precision parts or an fp32 addend, the GENERIC instantiations (plain bf16 is gemm_pp.cuh)
+  constexpr bool GENERIC = EPI == EPI_FWD || EPI == EPI_DA;
+  if (pl.bn == 64)
+    return launch_kernel(gemm_tc_kernel<64, EPI, A_MN, B_MN, GENERIC>, pl.grid, GemmTcCfg<64>::THREADS, GemmTcCfg<64>::SMEM_BYTES,
+                         st, pdl, tms, p);
+  if (pl.bn == 128)
+    return launch_kernel(gemm_tc_kernel<128, EPI, A_MN, B_MN, GENERIC>, pl.grid, GemmTcCfg<128>::THREADS,
+                         GemmTcCfg<128>::SMEM_BYTES, st, pdl, tms, p);
+  return set_error(SB_ERR_INVALID, "no gemm_tc instantiation for bn=%d", pl.bn);
+}
+
+// opt in to > 48 KB dynamic shared memory (once per process per instantiation, outside of stream capture)
+template <int EPI, bool A_MN, bool B_MN>
+int set_gemm_tc_attrs() {
+  constexpr bool GENERIC = EPI == EPI_FWD || EPI == EPI_DA;
+  SB_TRY(set_max_smem(gemm_tc_kernel<64, EPI, A_MN, B_MN, GENERIC>, GemmTcCfg<64>::SMEM_BYTES));
+  return set_max_smem(gemm_tc_kernel<128, EPI, A_MN, B_MN, GENERIC>, GemmTcCfg<128>::SMEM_BYTES);
+}
 
 }  // namespace sb

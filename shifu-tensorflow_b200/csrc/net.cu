@@ -5,7 +5,6 @@
 #include <string.h>
 #include <algorithm>
 #include "net.cuh"
-#include "gemm_tc_launch.cuh"
 #include "gemm_fwd_out.cuh"
 #include "gemm_pp.cuh"
 
@@ -76,8 +75,6 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rows, int cols, int l
 //     output layer (gemm_fwd_out.cuh) is planned apart: it needs whole rows of A_L in one CTA, so it takes 64 x h_L tiles
 //     (h_L <= 256, the two consumer warpgroups split the columns: 64 accumulator registers per thread) and
 //     ceil(rows / 64) CTAs - twice the CTAs a 128-row tile would give the narrow last layer;
-//   - no CTA pairs: the 256 x BN cluster tile with B multicast (cg = 2, gemm_tc.cuh) is the tile-configuration hook's,
-//     instantiated with the fp32 test epilogue only;
 //   - split-K (dW GEMMs, reduction over the batch): fill the machine but keep >= 8 k-blocks per split.
 GemmPlan plan_gemm(int M, int N, int K, int num_sms, bool allow_split) {
   const int total_kb = (K + 63) / 64;
@@ -92,7 +89,7 @@ GemmPlan plan_gemm(int M, int N, int K, int num_sms, bool allow_split) {
   }
   if (split > total_kb) split = total_kb;
   GemmPlan pl = {};
-  pl.cg = 1; pl.bn = bn;
+  pl.bn = bn;
   pl.kb_per_split = (total_kb + split - 1) / split;
   pl.split_k = (total_kb + pl.kb_per_split - 1) / pl.kb_per_split;
   const int work = tiles * pl.split_k;
@@ -344,10 +341,10 @@ int Net::enqueue_embed(int rows, bool scatter, float* grad, cudaStream_t st) {
     if (tc()) { p.dZ = dZ[0]; p.dZ_ps = A_ps[0]; p.ld_dZ = l0.ld_out; }
     else { p.dZ32 = dZf[0]; p.ld_dZ = l0.out; }
     p.gWe = grad + l0.w_off + static_cast<long long>(n_dense) * l0.out;
-    SB_TRY(launch(embed_scatter_kernel, dim3((rows + 7) / 8), dim3(256), 0, st, false, p));
+    SB_TRY(launch_kernel(embed_scatter_kernel, dim3((rows + 7) / 8), dim3(256), 0, st, false, p));
     mark("embed_scatter");
   } else {
-    SB_TRY(launch(embed_gather_kernel, dim3((rows + 7) / 8), dim3(256), 0, st, false, p));
+    SB_TRY(launch_kernel(embed_gather_kernel, dim3((rows + 7) / 8), dim3(256), 0, st, false, p));
     mark("embed_gather");
   }
   return SB_OK;
@@ -370,13 +367,13 @@ int Net::enqueue_load(int rows, float* zero_buf, long long zero_n) {
   if (blocks < 1) blocks = 1;
   // first kernel of the step: its stream predecessor is set_batch_kernel (a kernel), so PDL applies here too
   if (tc())
-    SB_TRY(launch(load_batch_kernel<true>, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, stream, use_pdl,
-                  static_cast<const BatchDesc*>(desc), rows, Fx, Xb, ldx, static_cast<float*>(nullptr), scal, zero_buf, zero_n,
-                  nparts, Xb_ps));
+    SB_TRY(launch_kernel(load_batch_kernel<true>, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, stream, use_pdl,
+                         static_cast<const BatchDesc*>(desc), rows, Fx, Xb, ldx, static_cast<float*>(nullptr), scal, zero_buf,
+                         zero_n, nparts, Xb_ps));
   else
-    SB_TRY(launch(load_batch_kernel<false>, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, stream, use_pdl,
-                  static_cast<const BatchDesc*>(desc), rows, Fx, static_cast<__nv_bfloat16*>(nullptr), ldx, Xf, scal, zero_buf, zero_n,
-                  1, 0ll));
+    SB_TRY(launch_kernel(load_batch_kernel<false>, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, stream, use_pdl,
+                         static_cast<const BatchDesc*>(desc), rows, Fx, static_cast<__nv_bfloat16*>(nullptr), ldx, Xf, scal,
+                         zero_buf, zero_n, 1, 0ll));
   mark("load_batch");
   if (sparse_step) SB_TRY(enqueue_embed(rows, false, nullptr, stream));
   return SB_OK;
@@ -482,16 +479,16 @@ int Net::enqueue_out(int rows, bool do_loss, bool do_bwd, float* yhat_dst, float
       rpb = ((rpb + 7) / 8) * 8;
       if (rpb < 8) rpb = 8;
       const dim3 g((rows + rpb - 1) / rpb);
-      if (hl.out <= 256) SB_TRY(launch(out_layer_rows_kernel<1>, g, dim3(256), 0, stream, use_pdl, p, rpb));
-      else if (hl.out <= 512) SB_TRY(launch(out_layer_rows_kernel<2>, g, dim3(256), 0, stream, use_pdl, p, rpb));
-      else SB_TRY(launch(out_layer_rows_kernel<4>, g, dim3(256), 0, stream, use_pdl, p, rpb));
+      if (hl.out <= 256) SB_TRY(launch_kernel(out_layer_rows_kernel<1>, g, dim3(256), 0, stream, use_pdl, p, rpb));
+      else if (hl.out <= 512) SB_TRY(launch_kernel(out_layer_rows_kernel<2>, g, dim3(256), 0, stream, use_pdl, p, rpb));
+      else SB_TRY(launch_kernel(out_layer_rows_kernel<4>, g, dim3(256), 0, stream, use_pdl, p, rpb));
     } else {
-      SB_TRY(launch(out_layer_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, stream, use_pdl, p));
+      SB_TRY(launch_kernel(out_layer_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, stream, use_pdl, p));
     }
   } else {
     p.A = Af[L - 1]; p.ldA = hl.out;
     if (do_bwd) { p.dZ = dZf[L - 1]; p.ld_dZ = hl.out; }
-    SB_TRY(launch(out_layer_kernel<float>, dim3(grid), dim3(256), 0, stream, use_pdl, p));
+    SB_TRY(launch_kernel(out_layer_kernel<float>, dim3(grid), dim3(256), 0, stream, use_pdl, p));
   }
   SB_CUDA(cudaGetLastError());
   mark("out_layer");
@@ -523,9 +520,8 @@ int Net::enqueue_backward(int rows, float* grad) {
       const GemmPlan b1 = plan_gemm(layers[1].in, layers[1].out, kx, gemm_sms / 3, true);
       const GemmPlan b0 = plan_gemm(layers[0].in, layers[0].out, kx, gemm_sms - b1.grid, true);
       auto waves = [&](const GemmPlan& pl, int M, int N, int sms) {   // k-blocks one CTA works through
-        const int tiles = ((M + 128 * pl.cg - 1) / (128 * pl.cg)) * ((N + pl.bn - 1) / pl.bn) * pl.split_k;
-        const int slots = sms / pl.cg;
-        return ((tiles + slots - 1) / slots) * pl.kb_per_split;
+        const int tiles = ((M + 127) / 128) * ((N + pl.bn - 1) / pl.bn) * pl.split_k;
+        return ((tiles + sms - 1) / sms) * pl.kb_per_split;
       };
       const int t_nat = waves(n0, layers[0].in, layers[0].out, gemm_sms) + waves(n1, layers[1].in, layers[1].out, gemm_sms);
       const int t0 = waves(b0, layers[0].in, layers[0].out, gemm_sms - b1.grid);
@@ -623,7 +619,7 @@ int Net::enqueue_backward(int rows, float* grad) {
           const GemmPlan gp = plan_gemm(rows, ly.in, round_up(ly.out, 64) * pairs_of(nparts), gemm_sms, false);
           TmapSet tm;
           SB_TRY(make_tmaps_bf16(tm.a, dZ[l], A_ps[l], nparts, rows, ly.out, ly.ld_out, 128));
-          SB_TRY(make_tmaps_bf16(tm.b, ly.Wn, Wn_ps[l], nparts, ly.in, ly.out, ly.ld_out, plan_box_rows_b(gp)));
+          SB_TRY(make_tmaps_bf16(tm.b, ly.Wn, Wn_ps[l], nparts, ly.in, ly.out, ly.ld_out, gp.bn));
           SB_TRY((launch_gemm_tc<EPI_DA, false, false>(gp, tm, p, stream, use_pdl)));
         }
         mark("gemm_da");

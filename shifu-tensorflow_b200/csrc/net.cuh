@@ -140,18 +140,6 @@ struct Net {
   }
 
   std::vector<void*> allocs;
-  // cudaLaunchKernelEx wrapper: optional programmatic-stream-serialization attribute
-  template <typename... KArgs, typename... Args>
-  int launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, Args... args) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
-    SB_CUDA(cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...));
-    return SB_OK;
-  }
   template <typename T> int dalloc(T** p, size_t n) {
     void* q = nullptr;
     SB_CUDA(cudaMalloc(&q, n * sizeof(T) + 256));

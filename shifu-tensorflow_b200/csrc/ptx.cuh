@@ -90,7 +90,7 @@ __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sy
 #define SB_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
 template <int N, int TA, int TB>
 __device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
-  static_assert(N == 32 || N == 64 || N == 128 || N == 256, "wgmma N");
+  static_assert(N == 32 || N == 64 || N == 128, "wgmma N");
   if constexpr (N == 32) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
@@ -121,47 +121,9 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t desc_a, u
         : SB_F8(0), SB_F8(8), SB_F8(16), SB_F8(24), SB_F8(32), SB_F8(40), SB_F8(48), SB_F8(56)
         : "l"(desc_a), "l"(desc_b), "r"(scale_d), "n"(TA), "n"(TB));
   }
-  if constexpr (N == 256) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %130, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
-        "%128, %129, p, 1, 1, %131, %132;\n\t}"
-        : SB_F8(0), SB_F8(8), SB_F8(16), SB_F8(24), SB_F8(32), SB_F8(40), SB_F8(48), SB_F8(56), SB_F8(64), SB_F8(72), SB_F8(80), SB_F8(88), SB_F8(96), SB_F8(104), SB_F8(112), SB_F8(120)
-        : "l"(desc_a), "l"(desc_b), "r"(scale_d), "n"(TA), "n"(TB));
-  }
 }
 
 #undef SB_F8
-
-// ---------------------------------------------------------------- CTA pairs (cluster of 2)
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the mbarrier at the same smem offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_local, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(bar_local), "r"(cta)
-      : "memory");
-}
-// The same load, multicast: the box lands at this smem offset in every CTA of the cluster named in cta_mask, and each of
-// them gets the bytes signalled on its mbarrier at offset `bar`.
-__device__ __forceinline__ void tma_load_2d_mc(uint32_t dst_smem, const void* tmap, uint32_t bar, int c0, int c1, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(dst_smem), "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask)
-      : "memory");
-}
 
 // ---------------------------------------------------------------- descriptors
 // Shared-memory matrix descriptor for a K-major bf16 operand tile staged by TMA with 128-byte swizzle:

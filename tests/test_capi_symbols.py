@@ -57,3 +57,6 @@ def test_argument_validation_is_host_side(sb):
     with pytest.raises(sb.ShifuB200Error) as e:
         sb.Model.load("", "in", "out")
     assert e.value.code == sb.capi.SB_ERR_INVALID and "Model path is null" in str(e.value)
+    with pytest.raises(sb.ShifuB200Error) as e:   # cfg_cg = 2 (the removed CTA-pair tile) is not a tile configuration
+        sb.capi.debug_gemm_bf16(np.zeros((256, 64), np.float32), np.zeros((128, 64), np.float32), cg=2, bn=128)
+    assert e.value.code == sb.capi.SB_ERR_INVALID and "not instantiated" in str(e.value)

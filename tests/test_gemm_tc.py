@@ -42,7 +42,7 @@ def test_gemm_bf16_matches_fp64(sb, M, N, K, split_k, layout):
     assert err <= 2e-5 * scale * 4, "max abs err %g (K=%d)" % (err, K)
 
 
-TILES = [(1, 64), (1, 128), (2, 128), (2, 256)]   # (CTAs per tile, BN)
+TILES = [(1, 64), (1, 128)]   # (cfg_cg = 1: the tile is forced, BN)
 
 
 @pytest.mark.gpu
@@ -50,8 +50,8 @@ TILES = [(1, 64), (1, 128), (2, 128), (2, 256)]   # (CTAs per tile, BN)
 @pytest.mark.parametrize("layout", sorted(LAYOUTS))
 @pytest.mark.parametrize("M,N,K,split_k", [(300, 200, 136, 1), (1000, 512, 1024, 2), (2048, 1024, 512, 1)])
 def test_gemm_every_tile_configuration(sb, M, N, K, split_k, layout, cg, bn):
-    """each instantiated tile shape (single CTA 128xBN, CTA pair 256xBN: a cluster of two sharing B by TMA multicast) on
-    ragged and multi-wave problems, forced through the debug hook (the planner would not pick every one of them here)"""
+    """each instantiated tile shape (128xBN) on ragged and multi-wave problems, forced through the debug hook (the planner
+    would not pick every one of them here)"""
     if bn == 64 and N > 64:
         N = 64
     a_mn, b_mn = LAYOUTS[layout]
