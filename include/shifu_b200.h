@@ -196,13 +196,6 @@ void* sb_trainer_stream(sb_trainer_t* t);
 /* number of this library's kernels launched by one step at this batch size (bench.py's gpu_launches) */
 int sb_trainer_kernels_per_step(sb_trainer_t* t, int32_t rows);
 
-/* measurement hook: runs ONE training step over resident rows outside the CUDA graph with a CUDA event after
- * every kernel launch on the trainer's stream; ms[i] is the device time of launch i, names is a '\n'-joined list
- * (load_batch, gemm_fwd, out_layer, gemm_dw, gemm_da, [allreduce], optimizer).  The step is a real step
- * (parameters are updated). */
-int sb_trainer_profile_step(sb_trainer_t* t, int64_t row_offset, int32_t rows, char* names, int32_t names_cap,
-                            float* ms, int32_t cap, int32_t* n_out);
-
 /* validation pass: sess.run([loss, global_step]) on the valid set (ssgd_monitor.py:281-284);
  * forward + loss only, any number of rows (processed in max_batch chunks with the reduction of
  * ONE big batch: sum w*(..)^2 over all rows / count of non-zero weights over all rows). */

@@ -116,7 +116,6 @@ PROTOTYPES = {
     "sb_trainer_sync": (C.c_int, [_vp]),
     "sb_trainer_stream": (C.c_void_p, [_vp]),
     "sb_trainer_kernels_per_step": (C.c_int, [_vp, C.c_int32]),
-    "sb_trainer_profile_step": (C.c_int, [_vp, C.c_int64, C.c_int32, C.c_char_p, C.c_int32, _f32p, C.c_int32, _P(C.c_int32)]),
     "sb_trainer_eval_loss": (C.c_int, [_vp, _f32p, _f32p, _f32p, C.c_int64, _f32p]),
     "sb_trainer_predict": (C.c_int, [_vp, _f32p, C.c_int64, _f32p]),
     "sb_trainer_save_checkpoint": (C.c_int, [_vp, _cp]),
@@ -444,15 +443,6 @@ class Trainer:
         if n < 0:
             check(n)
         return n
-
-    def profile_step(self, row_offset: int, rows: int):
-        """-> [(kernel name, milliseconds)] for one real (un-graphed) step over resident rows"""
-        names = C.create_string_buffer(4096)
-        ms = (C.c_float * 256)()
-        n = C.c_int32(0)
-        check(lib().sb_trainer_profile_step(self._h, row_offset, rows, names, 4096, ms, 256, C.byref(n)))
-        nm = names.value.decode().split("\n") if n.value else []
-        return [(nm[i], float(ms[i])) for i in range(n.value)]
 
     def eval_loss(self, X, y, w=None) -> float:
         X, y, w, rows = self._xyw(X, y, w)

@@ -52,7 +52,7 @@ struct sb_trainer {
   P2PPeers* d_peers = nullptr;     // device table of every rank's arena
   std::vector<void*> peer_bases;   // opened IPC mappings (to close)
   bool p2p_ready = false;
-  bool peers_share_device = false; // in-process replicas on this device (tests): see XchgParams::early_dependents
+  bool peers_share_device = false; // in-process replicas on this device (tests): see enqueue_xchg and enqueue_step_body
   bool grad_sharded = false;       // the reduced gradient of the last step lives in slices on its owners (sb_trainer_get_grads gathers)
   bool master_stale = false;       // sharded updates ran since the fp32 master / state were last gathered from their owners
   unsigned int epoch = 0;
@@ -69,7 +69,6 @@ struct sb_trainer {
   bool ll_ready = false;           // the LL exchange (xchg_ll_kernel) is usable: plain bf16, world > 1, buffers in the arena
   long long llg_off = 0, lls_off = 0;
   int x_sent = 0;                  // (while enqueueing a step) slots whose exchange the dW_0 chunk hook has launched
-  bool pending_xA = false;         // (while capturing) slot 0's exchange of the previous step has not been joined yet
   // pipelined host-buffer steps (sb_trainer_step_async): second staging slot + copy stream, so the H2D of batch i+1
   // overlaps the compute of batch i
   cudaStream_t copy_stream = nullptr;
@@ -103,14 +102,12 @@ static float lr_for_step(const sb_trainer* t, long long step /*1-based*/) {
   return t->lr;
 }
 
-static int enqueue_allreduce(sb_trainer* t, float* buf, long long off = 0, long long count = -1, cudaStream_t st = nullptr) {
+static int enqueue_allreduce(sb_trainer* t, float* buf) {
   if (t->world <= 1) return SB_OK;
   NcclApi* api = nccl_api();
   SB_CHECK(api && t->comm, SB_ERR_NCCL, "no gradient exchange configured: world = %d but neither an NCCL communicator (nccl_id) nor a "
            "peer table (sb_trainer_set_peer_handles / _pointers) exists", t->world);
-  if (count < 0) count = t->net.n_params;
-  if (!st) st = t->net.stream;
-  int r = api->AllReduce(buf + off, buf + off, static_cast<size_t>(count), NCCL_FLOAT32, NCCL_SUM, t->comm, st);
+  int r = api->AllReduce(buf, buf, static_cast<size_t>(t->net.n_params), NCCL_FLOAT32, NCCL_SUM, t->comm, t->net.stream);
   SB_CHECK(r == 0, SB_ERR_NCCL, "ncclAllReduce failed: %s", api->GetErrorString(r));
   return SB_OK;
 }
@@ -148,22 +145,16 @@ static XchgParams xchg_params(sb_trainer* t) {
   p.hyper = t->hyper;
   p.host_err = t->d_herr;
   p.timeout_ns = t->xchg_timeout_ns;
-  p.early_dependents = 0;
   static const bool fence_sys = getenv("SB_XCHG_FENCE_SYS") != nullptr;
   p.fence_gpu = fence_sys ? 0 : 1;
   return p;
 }
 
 // reduce-scatter -> owner update -> all-gather of the operands for the given segments (xchg_p2p.cuh); `g` must be t->grad
-// release_early: the launch lets its programmatic dependents start as soon as it has started itself (only for a launch whose
-// dependents need nothing it produces, see the deferred slot 0 in enqueue_step_body) - every other launch completes first,
-// also for dependents that were given the programmatic attribute
-static int enqueue_xchg(sb_trainer* t, int slot_mask, cudaStream_t st, bool publish_scalars, bool pdl, bool release_early = false,
-                        bool alone = false) {
+static int enqueue_xchg(sb_trainer* t, int slot_mask, cudaStream_t st, bool publish_scalars, bool pdl, bool alone = false) {
   Net& n = t->net;
   XchgParams p = xchg_params(t);
   p.slot_mask = slot_mask;
-  p.early_dependents = (release_early && !t->peers_share_device) ? 1 : 0;
   p.scal = publish_scalars ? n.scal : nullptr;
   p.host_scal = publish_scalars ? t->d_hscal : nullptr;
   char nm[24];
@@ -189,15 +180,8 @@ static int enqueue_xchg(sb_trainer* t, int slot_mask, cudaStream_t st, bool publ
   if (grid > want) grid = want;
   if (grid < 1) grid = 1;
   const dim3 g(static_cast<unsigned>(grid)), b(256);
-  // SB_XCHG_LL = all (default) | last | none: which launches use the LL protocol (flags inside the data).  An LL launch needs
-  // fewer round trips than the flag-and-pull kernel, at the price of polling and doubled store traffic beside the GEMM it
-  // runs with; "last" keeps it for the launch nothing runs beside.
-  static const int ll_mode = [] {
-    const char* e = getenv("SB_XCHG_LL");
-    if (e == nullptr) return 2;
-    return strcmp(e, "last") == 0 ? 1 : (strcmp(e, "none") == 0 ? 0 : 2);
-  }();
-  if (t->ll_ready && (ll_mode == 2 || (ll_mode == 1 && alone))) {
+  // plain bf16: the LL protocol (flags inside the data) needs fewer fabric round trips than the flag-and-pull kernel
+  if (t->ll_ready) {
     LLParams lp;
     lp.x = p; lp.llg_off = t->llg_off; lp.lls_off = t->lls_off; lp.n4 = t->xch_n4;
     if (t->world <= 2) SB_TRY(launch_kernel(xchg_ll_kernel<2>, g, b, 0, st, pdl, lp));
@@ -228,63 +212,39 @@ static int gather_master(sb_trainer* t) {
   return SB_OK;
 }
 
-// SB_PIPELINE_AR=1 (opt-in): per-layer exchange + update on the comm stream; then no single tail kernel exists and the
-// step scalars are read back with a copy instead
-static bool step_is_pipelined(const sb_trainer* t, int kind) {
-  static const bool want_pipeline = getenv("SB_PIPELINE_AR") != nullptr;
-  const Net& n = t->net;
-  return want_pipeline && kind == G_STEP && n.concurrent_bwd && !n.profiling && n.side != nullptr &&
-         n.tc();
-}
-
 // the body of one step as a sequence of stream operations (captured into a CUDA graph)
-static int enqueue_step_body(sb_trainer* t, int rows, int kind, bool resident = false, bool sparse = false, bool last_in_graph = true) {
+static int enqueue_step_body(sb_trainer* t, int rows, int kind, bool resident = false, bool sparse = false) {
   Net& n = t->net;
   struct Scope {
     Net& n;
     ~Scope() {
-      n.from_resident = false; n.zero_buf = nullptr; n.dw0_on_main = n.defer_join = false; n.sparse_step = false;
-      n.dw0_chunks = 1; n.dw1_last = false; n.on_dw0_chunk = nullptr; n.before_layer1 = nullptr; n.zero_layer = 0;
+      n.from_resident = false; n.zero_buf = nullptr; n.defer_join = false; n.sparse_step = false;
+      n.dw0_chunks = 1; n.dw1_last = false; n.on_dw0_chunk = nullptr;
       n.dw1_first = false; n.after_dw1 = nullptr; n.dw1_serial_auto = false;
-      n.beside_prev_xchg = false;
     }
   } scope{n};
   n.from_resident = resident;
   n.sparse_step = sparse;
   n.trace_k = 0;
-  // ---- schedule of the step's tail (decided first: the peer-exchange schedule also changes the forward pass) ----
-  const bool pipelined = step_is_pipelined(t, kind);
+  // ---- schedule of the step's tail ----
   // Single GPU, one update per mini-batch: no exchange, so nothing needs ALL gradients at once.  dW_0 runs on the main
   // stream behind the last dA GEMM and is followed (PDL) by the optimizer of layer 0 alone; the side stream updates the
   // other layers right after their dW GEMMs; the two streams only join at the end of the graph.
-  static const bool old_sched = getenv("SB_OLD_SCHED") != nullptr;
-  static const bool one_xchg = getenv("SB_XCHG_ONE") != nullptr;    // experiment: one exchange launch for everything after a join
-  const bool split_tail = !old_sched && kind == G_STEP && (t->world == 1 || (t->p2p_ready && !one_xchg)) && !pipelined &&
-                          n.concurrent_bwd && !n.profiling && n.side != nullptr && n.tc() && n.L > 1;
+  const bool split_tail = kind == G_STEP && (t->world == 1 || t->p2p_ready) && n.side != nullptr && n.tc() && n.L > 1;
   // Peer exchange (world > 1): one exchange launch costs several fabric round trips however little data it moves (xchg_p2p.cuh)
-  // - hidden when a GEMM follows it, exposed in full behind the last GEMM.  Default order ("first"):
+  // - hidden when a GEMM follows it, exposed in full behind the last GEMM:
   //   main:  ... dA_1 -> dW_1 -> dW_0 chunk 0 -> dW_0 chunk 1 | wait A, B0, B1 | next step
   //   side:  ... dW_2 ...     A ------------->
   //   comm:                             B0 ---------------->    B1 ------>
-  // A (every layer but hidden layer 0) and B0 run beside dW_0's chunks, only B1 - half of layer 0 - is exposed.
-  // Order "last" (SB_XCHG_ORDER=last, and replicas that share a device): dW_1 BEHIND dW_0 as cover for B1, and A beside the
-  // NEXT step's layer-0 forward GEMM, which reads nothing slot A writes: layer 1's forward waits for A, and - because peers
-  // may read this rank's gradient buffer until then - the buffer is cleared by layer 1's forward GEMM instead of layer 0's.
+  // A (every layer but hidden layer 0) and B0 run beside dW_0's chunks, only B1 - half of layer 0 - is exposed, on an
+  // otherwise idle GPU, where an exchange kernel is faster than beside a GEMM.
+  // Replicas that share ONE device (tests) put dW_1 BEHIND dW_0 instead, as cover for B1, and launch A on the side stream
+  // behind it: with three exchange launches of both replicas waiting beside each other's persistent GEMMs, dW_1 in front
+  // stopped making progress within the exchange timeout.
+  // Every exchange launch of the step is joined into the main stream before the step ends.  A rank's exchange only ends
+  // once every peer has read the gradient runs it owns of this rank (xchg_p2p.cuh), so the next step's layer-0 forward
+  // GEMM may clear the gradient buffer.
   const bool xsched = split_tail && t->world > 1;
-  // SB_XCHG_ORDER: "first" (default) = dW_1 in front of dW_0: slot A and chunk 0 hide behind dW_0's chunks, the LAST chunk's
-  // exchange runs on an otherwise idle GPU, where an exchange kernel is faster than beside a GEMM;
-  // "last" = dW_1 behind dW_0 as cover for the last chunk, slot A beside the next step's layer-0 forward.
-  static const bool order_last_env = getenv("SB_XCHG_ORDER") != nullptr && strcmp(getenv("SB_XCHG_ORDER"), "last") == 0;
-  // (replicas that share ONE device - tests - keep the "last" order: with three exchange launches of both replicas waiting
-  // beside each other's persistent GEMMs the "first" order stopped making progress within the exchange timeout)
-  const bool order_last = order_last_env || t->peers_share_device;
-  static const bool no_defer = getenv("SB_XCHG_NO_DEFER") != nullptr;
-  const bool defer_A = xsched && order_last && resident && n.L >= 3 && !no_defer;
-  if (xsched) {
-    n.zero_layer = defer_A ? 1 : 0;
-    n.beside_prev_xchg = t->pending_xA;     // slot A's exchange of the previous step is the kernel in front of this step
-    t->pending_xA = false;
-  }
   if (resident) {
     // no load kernel: the batch is read by TMA from the bf16 resident set; set_batch_kernel already published n_nz.
     // The gradient buffer is first written by the last forward layer's epilogue, so with more than one hidden layer the
@@ -302,44 +262,13 @@ static int enqueue_step_body(sb_trainer* t, int rows, int kind, bool resident = 
   bool fused_out = false;
   SB_TRY(n.enqueue_hidden_forward(rows, t->grad, &fused_out));
   if (!fused_out) SB_TRY(n.enqueue_out(rows, true, true, nullptr, t->grad));
-  // Gradient exchange pipelined behind the backward pass: as soon as layer l's dW GEMM is enqueued (side stream), its
-  // flat segment [W_l, b_l] (+ the output layer for l = L-1) is all-reduced and its optimizer update applied on the
-  // comm stream while the remaining dA / dW GEMMs still run - the role SyncReplicasOptimizer's accumulator + apply
-  // play in the reference (res/ssgd_monitor.py:136-142), without the parameter server.
-  // With NCCL as the exchange, the default is ONE all-reduce of the whole flat gradient after the backward pass: each NCCL
-  // launch has a fixed cost and its CTAs evict persistent GEMM CTAs, so the pipelined variant is opt-in (SB_PIPELINE_AR=1).
-  if (pipelined) {
-    n.on_layer_grads = [t](int l, cudaStream_t cs, int phase, long long e0, long long e1) -> int {
-      Net& nn = t->net;
-      const Layer& ly = nn.layers[l];
-      const int last = (l == nn.L - 1) ? nn.L : l;
-      const bool completes = e1 == static_cast<long long>(ly.in) * ly.out;  // this chunk also carries b_l (+ output layer)
-      if (phase == 0) {
-        const long long off = ly.w_off + e0;
-        const long long end = completes ? nn.layers[last].b_off + nn.layers[last].out : ly.w_off + e1;
-        return enqueue_allreduce(t, t->grad, off, end - off, cs);
-      }
-      // work-table runs are 1024 parameters each, chunk boundaries are multiples of 1024 (128 rows x out % 8 == 0)
-      const int w0 = nn.work_begin[l] + static_cast<int>(e0 / 1024);
-      const int w1 = completes ? nn.work_end[last] : nn.work_begin[l] + static_cast<int>(e1 / 1024);
-      return enqueue_optimizer(t, t->grad, w0, w1, cs);
-    };
-  } else {
-    n.on_layer_grads = nullptr;
-  }
-  // (dW_0 on the main stream also when an exchange or the accumulate kernel follows: it is then joined with the side
-  // stream as before)
-  n.dw0_on_main = !old_sched && !pipelined && n.concurrent_bwd && !n.profiling && n.side != nullptr &&
-                  n.tc() && n.L > 1;
   n.defer_join = split_tail;
   cudaStream_t comms[2] = {n.comm2, n.comm};
   if (xsched) {
-    // dW_1 leaves the side stream: in front of dW_0 ("first") or behind it ("last").  (SB_XCHG_BESIDE=1 keeps it beside dW_0
-    // like the single-GPU schedule, where the chunks of dW_0 share the SMs with dW_1.)
-    static const bool beside = getenv("SB_XCHG_BESIDE") != nullptr;
+    // dW_1 leaves the side stream: in front of dW_0, or behind it when the replicas share a device
     n.dw0_chunks = t->x_chunks;
-    n.dw1_last = !beside && order_last;
-    n.dw1_first = !beside && !order_last;
+    n.dw1_last = t->peers_share_device;
+    n.dw1_first = !t->peers_share_device;
     t->x_sent = 0;
     if (n.dw1_first) {
       n.after_dw1 = [t]() -> int {       // slot A on the side stream, behind dW_1 (main) and the other layers' dW GEMMs (side)
@@ -358,15 +287,14 @@ static int enqueue_step_body(sb_trainer* t, int rows, int kind, bool resident = 
       SB_CUDA(cudaEventRecord(t->ev_c[1 + c], nn.stream));
       SB_CUDA(cudaStreamWaitEvent(cs, t->ev_c[1 + c], 0));
       const bool last = c == t->x_chunks - 1;
-      SB_TRY(enqueue_xchg(t, 1 << (1 + c), cs, last, false, false, last && !nn.dw1_last));   // (the last chunk publishes the step scalars;
-                                                                                              //  no GEMM follows it unless dW_1 does)
+      SB_TRY(enqueue_xchg(t, 1 << (1 + c), cs, last, false, last && !nn.dw1_last));   // (the last chunk publishes the step scalars;
+                                                                                       //  no GEMM follows it unless dW_1 does)
       SB_CUDA(cudaEventRecord(t->ev_x[1 + c], cs));
       t->x_sent |= 1 << (1 + c);
       return SB_OK;
     };
   }
-  static const bool dw1_beside_n1 = getenv("SB_DW1_BESIDE") != nullptr;
-  if (split_tail && !xsched && !dw1_beside_n1) {
+  if (split_tail && !xsched) {
     // one GPU: dW_1 may move in front of dW_0 (Net::dw1_serial_auto); the side stream's optimizer launch then waits for it
     n.dw1_serial_auto = true;
     n.after_dw1 = [t]() -> int {
@@ -376,33 +304,13 @@ static int enqueue_step_body(sb_trainer* t, int rows, int kind, bool resident = 
       return SB_OK;
     };
   }
-  int bs = n.enqueue_backward(rows, t->grad);
-  n.on_layer_grads = nullptr;
-  SB_TRY(bs);
+  SB_TRY(n.enqueue_backward(rows, t->grad));
   if (xsched) {
     // slot A: every gradient but hidden layer 0's - complete behind dW_1 (main stream), the other layers' dW GEMMs (side
-    // stream) and the last dA GEMM (the last reader of their weight shadows).
-    // Deferred (multi-step graphs): the launch goes ON the main stream, as dW_1's programmatic dependent.  It releases ITS
-    // dependents at its start, the next step's layer-0 forward GEMM skips its dependency wait (all it needs - B0, B1 - are
-    // full dependencies) and so runs beside the exchange; layer 1's forward is a plain in-stream launch behind both.
-    // (As a node on another stream that nothing on the main chain waited for, the graph executor started the exchange well
-    // after B1 had ENDED - whichever stream carried it, with or without a waited-for marker kernel in front.)
-    const bool a_on_main = defer_A && n.dw1_last && !t->peers_share_device;
-    if (t->x_sent & XSEG_A) {
-      // (dW_1 first: launched by after_dw1)
-    } else if (a_on_main) {
-      if (n.L > 2) {
-        SB_CUDA(cudaEventRecord(n.ev_join, n.side));
-        SB_CUDA(cudaStreamWaitEvent(n.stream, n.ev_join, 0));
-      }
-      SB_TRY(enqueue_xchg(t, XSEG_A, n.stream, false, n.use_pdl, !last_in_graph));
-    } else {
-      if (n.dw1_last) {
-        SB_CUDA(cudaEventRecord(t->ev_c[0], n.stream));
-        SB_CUDA(cudaStreamWaitEvent(n.side, t->ev_c[0], 0));
-      } else {
-        SB_CUDA(cudaStreamWaitEvent(n.side, n.ev_da_done, 0));
-      }
+    // stream) and the last dA GEMM (the last reader of their weight shadows).  (dW_1 in front of dW_0: after_dw1 launched it.)
+    if (n.dw1_last) {
+      SB_CUDA(cudaEventRecord(t->ev_c[0], n.stream));
+      SB_CUDA(cudaStreamWaitEvent(n.side, t->ev_c[0], 0));
       SB_TRY(enqueue_xchg(t, XSEG_A, n.side, false, false));
       SB_CUDA(cudaEventRecord(t->ev_x[0], n.side));
     }
@@ -412,12 +320,11 @@ static int enqueue_step_body(sb_trainer* t, int rows, int kind, bool resident = 
     // (a layer-0 dW that was not cut into the trainer's chunks - wide+deep steps - is exchanged here, behind everything)
     const int missing = (xseg_all(t) & ~XSEG_A) & ~t->x_sent;
     if (missing) SB_TRY(enqueue_xchg(t, missing, n.stream, true, false));
-    if (a_on_main) t->pending_xA = !last_in_graph;      // (the last step of a graph: whatever follows is ordered behind it)
-    else SB_CUDA(cudaStreamWaitEvent(n.stream, t->ev_x[0], 0));
+    SB_CUDA(cudaStreamWaitEvent(n.stream, t->ev_x[0], 0));
     return SB_OK;
   }
   if (split_tail) {
-    SB_TRY(enqueue_optimizer(t, t->grad, n.work_begin[0], n.work_end[0], n.stream, true, n.use_pdl));
+    SB_TRY(enqueue_optimizer(t, t->grad, n.work_begin[0], n.work_end[0], n.stream, true, true));
     // the other layers' shadows are read by the dA GEMMs on the main stream: update them only after the last one
     SB_CUDA(cudaStreamWaitEvent(n.side, n.ev_da_done, 0));
     SB_TRY(enqueue_optimizer(t, t->grad, n.work_end[0], n.n_work, n.side));
@@ -426,13 +333,11 @@ static int enqueue_step_body(sb_trainer* t, int rows, int kind, bool resident = 
     return SB_OK;
   }
   if (kind == G_STEP) {
-    if (pipelined) return SB_OK;
     if (t->world > 1 && t->p2p_ready) {
-      // (fp32 mode, one hidden layer, profiling, SB_XCHG_ONE: no split tail) one launch handles both segments
+      // (fp32 mode or one hidden layer: no split tail) one launch handles both segments
       SB_TRY(enqueue_xchg(t, xseg_all(t), n.stream, true, false));
     } else {
       SB_TRY(enqueue_allreduce(t, t->grad));
-      if (t->world > 1 && n.profiling) { n.mark("allreduce"); --n.launches; }
       SB_TRY(enqueue_optimizer(t, t->grad, 0, -1, nullptr, true, false));
     }
   } else {
@@ -471,16 +376,14 @@ static int run_step(sb_trainer* t, const float* X, const float* y, const float* 
   Net& n = t->net;
   SB_CHECK(rows > 0 && rows <= n.max_batch, SB_ERR_INVALID, "rows=%d outside (0, max_batch=%d]", rows, n.max_batch);
   SB_CUDA(cudaSetDevice(n.device));
-  static const bool no_graph = getenv("SB_NO_GRAPH") != nullptr;
   const bool resident = resident_row0 >= 0 && t->dsXb != nullptr;
   // descriptor / scalar pair of this step: resident graph steps alternate, everything else uses pair 0
-  static const bool want_prep = !(getenv("SB_PREP") && getenv("SB_PREP")[0] == '0');
-  const bool prep = want_prep && resident && !no_graph && t->prep != nullptr;
+  const bool prep = resident && t->prep != nullptr;
   const int pair = prep ? static_cast<int>(t->prep_steps & 1) : 0;
   n.desc = t->descs[pair];
   n.scal = t->scals[pair];
   cudaGraphExec_t ge = nullptr;
-  if (!no_graph) SB_TRY(get_graph(t, rows, kind, resident, pair, &ge, sparse));
+  SB_TRY(get_graph(t, rows, kind, resident, pair, &ge, sparse));
   float lr_t = t->lr, gscale = 1.f / static_cast<float>(t->world);
   if (kind == G_STEP) {
     ++t->global_step;
@@ -511,11 +414,8 @@ static int run_step(sb_trainer* t, const float* X, const float* y, const float* 
                                                kind == G_STEP ? t->hist_slot(t->global_step) : nullptr);
   }
   SB_CUDA(cudaGetLastError());
-  if (no_graph) SB_TRY(enqueue_step_body(t, rows, kind, resident, sparse));
-  else SB_CUDA(cudaGraphLaunch(ge, n.stream));
+  SB_CUDA(cudaGraphLaunch(ge, n.stream));
   // the step's tail kernel (optimizer / accumulate) wrote (loss sum, n_nz) into h_scal; visible after a stream sync
-  if (step_is_pipelined(t, kind))
-    SB_CUDA(cudaMemcpyAsync(t->h_scal, n.scal, sizeof(float) * SCAL_COUNT, cudaMemcpyDeviceToHost, n.stream));
   if (kind == G_ACC) ++t->n_acc;
   t->grad_out_scale = (kind == G_STEP) ? gscale : 1.f;
   return SB_OK;
@@ -631,19 +531,17 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
     t->xch_n4 = (np + 3) / 4;
     t->net.arena_extra_bytes = static_cast<size_t>(t->xch_n4) * 16 + sizeof(P2PFlags);
     // LL exchange buffers (xchg_p2p.cuh): gbuf = world regions, sbuf = one, of n4 entries x 32 bytes
-    static const bool no_ll = getenv("SB_XCHG_PULL") != nullptr;
-    if (world > 1 && desc->precision == SB_PREC_BF16 && !no_ll) {
+    if (world > 1 && desc->precision == SB_PREC_BF16) {
       t->ll_ready = true;
       t->net.arena_extra_bytes += 256 + static_cast<size_t>(world + 1) * static_cast<size_t>(t->xch_n4) * 32;
     }
   }
   int s = t->net.init(desc, device, true);
   if (s != SB_OK) { t->net.destroy(); return s; }
-  if (!getenv("SB_NO_CARVEOUT")) {   // see Net::init: no L1 / shared-memory re-partition between the kernels of a step
-    cudaFuncSetAttribute(set_batch_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(optimizer_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(axpy_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  }
+  // see Net::init: no L1 / shared-memory re-partition between the kernels of a step
+  cudaFuncSetAttribute(set_batch_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  cudaFuncSetAttribute(optimizer_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  cudaFuncSetAttribute(axpy_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   Net& n = t->net;
   // gradient + exchange flags behind the parameters, in the arena a single IPC handle exports
   t->xch = n.arena;
@@ -674,10 +572,8 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
     // exchange slots: hidden layer 0 in row chunks of W_0 (128-row multiples; runs are 1024 parameters, so chunk borders fall
     // on run borders when out % 8 == 0), the last chunk also carries b_0; everything else is slot 0
     int chunks = 2;
-    if (const char* e = getenv("SB_XCHG_CHUNKS")) chunks = atoi(e);
-    if (chunks > SB_XCHG_SLOTS - 2) chunks = SB_XCHG_SLOTS - 2;   // (ev_c[SLOTS - 1] is the touch event)
     const Layer& l0 = n.layers[0];
-    if (chunks < 1 || !n.tc() || (l0.out % 8) != 0 || l0.in < 256 * chunks) chunks = 1;
+    if (!n.tc() || (l0.out % 8) != 0 || l0.in < 256 * chunks) chunks = 1;
     n.dw0_chunks = chunks;
     const int cr = n.dw0_chunk_rows();
     chunks = (l0.in + cr - 1) / cr;           // (rounding to 128 rows may need fewer chunks)
@@ -725,21 +621,6 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
     return set_error(SB_ERR_CUDA, "cudaHostGetDevicePointer failed");
   }
   if (world > 1 && nccl_id != nullptr) {
-    // The GEMMs are persistent (one CTA per SM, ~200 KB smem each): an NCCL CTA that lands on an SM evicts a GEMM CTA
-    // into a second wave.  Keep NCCL to a few CTAs and leave those SMs out of the GEMM grids.
-    // (only when the exchange is pipelined behind the backward pass, SB_PIPELINE_AR=1)
-    if (getenv("SB_PIPELINE_AR")) {
-      int nccl_ctas = 8;
-      if (const char* e = getenv("SB_NCCL_CTAS")) nccl_ctas = atoi(e);
-      if (nccl_ctas < 1) nccl_ctas = 1;
-      if (nccl_ctas > 32) nccl_ctas = 32;
-      char buf[16];
-      snprintf(buf, sizeof(buf), "%d", nccl_ctas);
-      setenv("NCCL_MAX_CTAS", buf, 0);
-      n.gemm_sms = n.num_sms - nccl_ctas;
-      n.dw_chunk_bytes = 2500000;
-      if (const char* e = getenv("SB_DW_CHUNK_BYTES")) n.dw_chunk_bytes = atoll(e);
-    }
     NcclApi* api = nccl_api();
     if (!api) { n.destroy(); return set_error(SB_ERR_NCCL, "libnccl.so.2 could not be loaded"); }
     NcclUniqueId id;
@@ -1203,17 +1084,15 @@ static int get_run_graph(sb_trainer* t, int rows, int set, cudaGraphExec_t* out)
   cudaGraph_t g = nullptr;
   SB_CUDA(cudaStreamBeginCapture(n.stream, cudaStreamCaptureModeThreadLocal));
   int s = SB_OK;
-  t->pending_xA = false;
   for (int k = 0; k < sb_trainer::RUN_S && s == SB_OK; ++k) {
     n.desc = t->run_descs[set][k];
     n.scal = t->run_scals[set][k];
-    // (SB_STEP_TRACE: an interior step is the one traced - with the peer exchange, the last step of a graph joins the
-    // exchange of slot A at its end instead of hiding it behind the next step's layer-0 forward)
+    // (SB_STEP_TRACE: an interior step is the one traced - it starts behind the previous step's tail, as most steps of a
+    // run do)
     n.trace_on = (k == 1);
-    s = enqueue_step_body(t, rows, G_STEP, true, false, k == sb_trainer::RUN_S - 1);
+    s = enqueue_step_body(t, rows, G_STEP, true, false);
   }
   n.trace_on = true;
-  t->pending_xA = false;
   n.desc = d0; n.scal = s0;
   cudaError_t e = cudaStreamEndCapture(n.stream, &g);
   if (s != SB_OK) { if (g) cudaGraphDestroy(g); return s; }
@@ -1237,10 +1116,8 @@ int sb_trainer_run_resident(sb_trainer_t* t, const int64_t* row_offsets, int32_t
              "step %d: rows [%lld, %lld) outside the resident set of %lld rows", i, (long long)row_offsets[i],
              (long long)(row_offsets[i] + rows), (long long)t->ds_rows);
   constexpr int S = sb_trainer::RUN_S;
-  static const bool no_graph = getenv("SB_NO_GRAPH") != nullptr;
-  static const bool no_multi = getenv("SB_NO_MULTI_STEP") != nullptr;
   int i = 0;
-  if (t->dsXb != nullptr && t->prep != nullptr && !no_graph && !no_multi) {
+  if (t->dsXb != nullptr && t->prep != nullptr) {
     SB_CUDA(cudaSetDevice(n.device));
     if (t->run_descs[0][0] == nullptr) {
       for (int set = 0; set < 2; ++set) {
@@ -1388,72 +1265,6 @@ int sb_trainer_kernels_per_step(sb_trainer_t* t, int32_t rows) {
   n.desc = d0; n.scal = s0;
   SB_TRY(s);
   return t->kernels_per_step[rows];
-}
-
-// One un-captured step over resident rows with a CUDA event after every launch.
-// ms[i] = device time between the end of launch i-1 (or the start marker) and the end of launch i.
-int sb_trainer_profile_step(sb_trainer_t* t, int64_t row_offset, int32_t rows, char* names, int32_t names_cap, float* ms,
-                            int32_t cap, int32_t* n_out) {
-  SB_CHECK(t && ms && n_out, SB_ERR_INVALID, "null argument");
-  SB_CHECK(t->ds_rows > 0, SB_ERR_STATE, "no resident dataset loaded");
-  SB_CHECK(row_offset >= 0 && rows > 0 && rows <= t->net.max_batch && row_offset + rows <= t->ds_rows, SB_ERR_INVALID, "bad row range");
-  Net& n = t->net;
-  SB_CUDA(cudaSetDevice(n.device));
-  ++t->global_step;
-  const float gscale = 1.f / static_cast<float>(t->world);
-  ++t->epoch;
-  const bool resident = t->dsXb != nullptr;
-  if (resident)
-    set_batch_kernel<<<1, 1, 0, n.stream>>>(n.desc, nullptr, t->dsY + row_offset, t->dsW + row_offset, lr_for_step(t, t->global_step),
-                                             gscale, t->epoch, static_cast<int>(row_offset), t->dsP, rows, n.scal);
-  else
-    set_batch_kernel<<<1, 1, 0, n.stream>>>(n.desc, t->dsX + row_offset * n.F, t->dsY + row_offset, t->dsW + row_offset,
-                                             lr_for_step(t, t->global_step), gscale, t->epoch);
-  n.profiling = true;
-  n.prof_events.clear(); n.prof_names.clear();
-  n.launches = 0;
-  // the two memsets of the step body run before the start marker so they are not charged to load_batch
-  int s = SB_OK;
-  {
-    n.from_resident = resident;
-    if (resident) s = (cudaMemsetAsync(t->grad, 0, sizeof(float) * n.n_params, n.stream) == cudaSuccess) ? SB_OK : SB_ERR_CUDA;
-    n.mark("start"); --n.launches;
-    if (!resident) s = n.enqueue_load(rows, t->grad, n.n_params);
-    bool fused_out = false;
-    if (s == SB_OK) s = n.enqueue_hidden_forward(rows, t->grad, &fused_out);
-    if (s == SB_OK && !fused_out) s = n.enqueue_out(rows, true, true, nullptr, t->grad);
-    if (s == SB_OK) s = n.enqueue_backward(rows, t->grad);
-    if (t->world > 1 && t->p2p_ready) {
-      if (s == SB_OK) s = enqueue_xchg(t, xseg_all(t), n.stream, false, false);
-    } else {
-      if (s == SB_OK) s = enqueue_allreduce(t, t->grad);
-      if (s == SB_OK && t->world > 1) { n.mark("allreduce"); --n.launches; }
-      if (s == SB_OK) s = enqueue_optimizer(t, t->grad);
-    }
-  }
-  n.profiling = false;
-  n.from_resident = false;
-  cudaError_t e = cudaStreamSynchronize(n.stream);
-  int cnt = 0;
-  std::string joined;
-  if (s == SB_OK && e == cudaSuccess) {
-    for (size_t i = 1; i < n.prof_events.size(); ++i) {
-      float v = 0.f;
-      cudaEventElapsedTime(&v, n.prof_events[i - 1], n.prof_events[i]);
-      if (cnt < cap) ms[cnt] = v;
-      if (!joined.empty()) joined += "\n";
-      joined += n.prof_names[i];
-      ++cnt;
-    }
-  }
-  for (cudaEvent_t ev : n.prof_events) cudaEventDestroy(ev);
-  n.prof_events.clear(); n.prof_names.clear();
-  SB_TRY(s);
-  SB_CHECK(e == cudaSuccess, SB_ERR_CUDA, "profile step failed: %s", cudaGetErrorString(e));
-  t->grad_out_scale = gscale;
-  *n_out = cnt;
-  if (names && names_cap > 0) { strncpy(names, joined.c_str(), names_cap - 1); names[names_cap - 1] = 0; }
-  return SB_OK;
 }
 
 // forward (+ optional loss) over any number of host rows, in max_batch chunks
@@ -1789,11 +1600,10 @@ static int debug_gemm_impl(const float* A, const float* B, float* D, int32_t M, 
         if (s == SB_OK) s = make_tmap_bf16(&pt.o, d_out, M, N, ldn, pp.bm_wg);
         if (s == SB_OK) s = make_tmap_bf16(&pt.x, d_aux, M, N, ldn, pp.bm_wg);
       }
-      const bool bench_pdl = getenv("SB_BENCH_PDL") != nullptr;
       auto real = [&]() -> int {
-        if (!a_mn && !b_mn) return launch_gemm_pp<EPI_DA>(pp, pt, q, 0, bench_pdl);
-        if (!a_mn) return launch_gemm_pp<EPI_FWD>(pp, pt, q, 0, bench_pdl);
-        return launch_gemm_tc<EPI_DW, true, true>(pl, tms, q, 0, bench_pdl);
+        if (!a_mn && !b_mn) return launch_gemm_pp<EPI_DA>(pp, pt, q, 0, false);
+        if (!a_mn) return launch_gemm_pp<EPI_FWD>(pp, pt, q, 0, false);
+        return launch_gemm_tc<EPI_DW, true, true>(pl, tms, q, 0, false);
       };
       if (s == SB_OK) s = a_mn ? set_gemm_tc_attrs<EPI_DW, true, true>() : set_gemm_pp_attrs();
       cudaEvent_t e0, e1;

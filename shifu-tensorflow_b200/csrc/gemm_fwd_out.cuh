@@ -31,6 +31,9 @@ struct FwdOutTmaps {
   CUtensorMap o[3];   // dZ_L [rows, N]: box 64 columns x 64 rows (store)
 };
 
+// widest tile: the widest last hidden layer whose GEMM also runs the output layer
+constexpr int FWD_OUT_MAX_N = 256;
+
 // besides the ring: align slack, barriers, bias + w_o, the two column-sum arrays per warp of a group, z partials
 // [tile parity][group][64], loss / db_o per warp of group 0, dZ_L staging tiles (X_BYTES)
 template <int BN>
@@ -278,7 +281,7 @@ gemm_fwd_out_kernel(const __grid_constant__ FwdOutTmaps tms, const GemmTcParams 
 // f(integral_constant BN): the narrowest tile that holds a whole row of A_L (N <= 256); one CTA per SM and 64-row tile
 template <typename F>
 static int with_fwd_out_bn(int N, F&& f) {
-  SB_CHECK(N <= 256, SB_ERR_INVALID, "fused output layer: last hidden layer %d wider than 256", N);
+  SB_CHECK(N <= FWD_OUT_MAX_N, SB_ERR_INVALID, "fused output layer: last hidden layer %d wider than %d", N, FWD_OUT_MAX_N);
   if (N <= 64) return f(std::integral_constant<int, 64>());
   if (N <= 128) return f(std::integral_constant<int, 128>());
   return f(std::integral_constant<int, 256>());

@@ -28,8 +28,6 @@ struct GemmTcParams {
   int M, N, K;
   int kb_per_split;  // k-blocks (of 64) per split
   int split_k;       // number of splits actually used (all non-empty)
-  int no_dep_wait;   // 1: do not wait for the programmatic primary (an exchange kernel this GEMM may run beside, capi.cu);
-                     // every real dependency of the launch is then a full one
   // EPI_FWD
   const float* bias;  // [N]
   int act;            // FWD: activation applied; DA: activation whose derivative is applied
@@ -150,7 +148,7 @@ __device__ __forceinline__ bool ring_enter(const Ring<Cfg>& ring, uint32_t empty
   }
   __syncthreads();
   if (threadIdx.x == 0) ring_stamp(p, tracing, 1);
-  if (!p.no_dep_wait) pdl_wait();
+  pdl_wait();
   pdl_launch_dependents();
   if (threadIdx.x == 0) ring_stamp(p, tracing, 2);
   return tracing;

@@ -72,10 +72,6 @@ struct XchgParams {
   unsigned int* host_err;                 // mapped pinned: [0] = 0 ok | 1 + 16 * slot + missing rank
   unsigned long long timeout_ns;          // 0 = wait forever
   int fence_gpu;                          // 1 (default): gpu-scope fence before the `updated` flag; SB_XCHG_FENCE_SYS=1 -> 0
-  int early_dependents;                   // 1: let the next kernel of the stream (PDL) become resident while this one still
-                                          // waits for its peers.  0 when the peers share this device (in-process replicas):
-                                          // the next step's persistent GEMM CTAs would take every SM's shared memory while
-                                          // they wait for this kernel, and the replica this kernel waits for could never run
   unsigned long long* trace;              // slots: 0 entry, 2 dependencies resolved, 3 every peer arrived (block 0), 4 last block's
                                           // runs done, 5 `updated` published, 6 every peer updated (block 0), 10 exit (gathered)
 };
@@ -148,7 +144,6 @@ xchg_update_kernel(const XchgParams p) {
   if (threadIdx.x == 0) sh_fail = 0u;
   trace_begin(p.trace, true);
   pdl_wait();                 // the gradient of these slots is complete (stream order / programmatic dependency)
-  if (p.early_dependents) pdl_launch_dependents();
   trace_begin(p.trace, false);
   __syncthreads();
   const unsigned int epoch = p.desc->epoch;
@@ -482,7 +477,6 @@ xchg_ll_kernel(const LLParams lp) {
   if (threadIdx.x == 0) sh_fail = 0u;
   trace_begin(p.trace, true);
   pdl_wait();
-  if (p.early_dependents) pdl_launch_dependents();
   trace_begin(p.trace, false);
   __syncthreads();
   const unsigned int ep = p.desc->epoch;

@@ -102,7 +102,7 @@ def _resident_rank_main(rank, world, port, out_dir, precision):
 def test_two_gpu_resident_run_matches_oracle(sb, tmp_path, precision):
     """sb_trainer_run_resident on two REAL GPUs over CUDA-IPC peer memory (no NCCL communicator at all): multi-step graphs
     with three hidden layers, i.e. the schedule bench.py times - dW_0 in chunks with their exchanges beside the next GEMMs,
-    slot 0's exchange beside the NEXT step's layer-0 forward (bf16: the LL kernel; fp32_tc: the flag-and-pull kernel)."""
+    slot 0's exchange on the side stream behind dW_1 (bf16: the LL kernel; fp32_tc: the flag-and-pull kernel)."""
     if sb.capi.device_count() < 2:
         pytest.skip("needs 2 GPUs")
     import torch.multiprocessing as mp
