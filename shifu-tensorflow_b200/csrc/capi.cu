@@ -41,7 +41,7 @@ struct sb_trainer {
   __nv_bfloat16* dsXb = nullptr;                           // bf16 mode: the set in GEMM-operand form [ds_rows, ldF]
   int* dsP = nullptr;                                      // prefix counts of non-zero weights [ds_rows + 1]
   long long ds_rows = 0;
-  std::map<std::pair<int, int>, cudaGraphExec_t> graphs;  // (rows, kind * 2 + from_resident) -> captured step
+  std::map<std::pair<int, int>, cudaGraphExec_t> graphs;  // (rows, kind * 8 + sparse * 4 + resident * 2 + pair) -> captured step
   std::map<int, int> kernels_per_step;
   // peer-memory exchange (xchg_p2p.cuh): the net's parameter arena [theta | s1 | s2 | shadows | gradient | P2PFlags] is
   // ONE exported allocation; `xch` aliases it
@@ -52,7 +52,7 @@ struct sb_trainer {
   P2PPeers* d_peers = nullptr;     // device table of every rank's arena
   std::vector<void*> peer_bases;   // opened IPC mappings (to close)
   bool p2p_ready = false;
-  bool peers_share_device = false; // in-process replicas on this device (tests): see enqueue_xchg and enqueue_step_body
+  bool peers_share_device = false; // in-process replicas on this device (tests): see enqueue_xchg and plan_dw1
   bool grad_sharded = false;       // the reduced gradient of the last step lives in slices on its owners (sb_trainer_get_grads gathers)
   bool master_stale = false;       // sharded updates ran since the fp32 master / state were last gathered from their owners
   unsigned int epoch = 0;
@@ -63,12 +63,18 @@ struct sb_trainer {
   // slot table of the exchange (fixed for the trainer's life: it defines who owns which run): slot 0 = every layer but
   // hidden layer 0, slots 1..x_chunks = row chunks of hidden layer 0 (the last one also carries b_0)
   int x_chunks = 1, x_slots = 2;
+  int x_chunk_rows = 0;            // rows of W_0 per slot chunk (128-row multiple; the last chunk may be shorter)
   int x_begin[SB_XCHG_SLOTS] = {}, x_end[SB_XCHG_SLOTS] = {};
   cudaEvent_t ev_x[SB_XCHG_SLOTS] = {};   // exchange of slot s complete (recorded on its comm stream)
   cudaEvent_t ev_c[SB_XCHG_SLOTS] = {};   // dW_0 chunk c complete on the main stream / tail of the main stream
   bool ll_ready = false;           // the LL exchange (xchg_ll_kernel) is usable: plain bf16, world > 1, buffers in the arena
   long long llg_off = 0, lls_off = 0;
-  int x_sent = 0;                  // (while enqueueing a step) slots whose exchange the dW_0 chunk hook has launched
+  // streams and events of the step schedule (enqueue_step_backward)
+  cudaStream_t side = nullptr;               // dW GEMMs run here, concurrently with the dA chain on the net's stream
+  cudaStream_t xstream[2] = {};              // the exchange launches behind dW_0's row chunks alternate between these
+  std::vector<cudaEvent_t> ev_dz;            // ev_dz[l]: dZ_l is complete on the net's stream
+  cudaEvent_t ev_join = nullptr;
+  cudaEvent_t ev_da_done = nullptr;          // the last dA GEMM (last reader of the bf16 weight shadows) is complete
   // pipelined host-buffer steps (sb_trainer_step_async): second staging slot + copy stream, so the H2D of batch i+1
   // overlaps the compute of batch i
   cudaStream_t copy_stream = nullptr;
@@ -83,6 +89,7 @@ struct sb_trainer {
   cudaEvent_t ev_prep[2] = {nullptr, nullptr}, ev_pos[2] = {nullptr, nullptr};
   unsigned long long prep_steps = 0;
   bool have_pos = false;   // ev_pos[] of the previous step is valid (no other user of the descriptors in between)
+  int last_pair = 0;       // the pair the last step used
   // sb_trainer_run_resident: RUN_S steps per captured graph (kernel -> kernel edges instead of a graph turn-around
   // between steps), two alternating descriptor sets so that the descriptors of chunk i+1 are written while chunk i runs
   enum { RUN_S = 4 };
@@ -112,15 +119,15 @@ static int enqueue_allreduce(sb_trainer* t, float* buf) {
   return SB_OK;
 }
 
-static int enqueue_optimizer(sb_trainer* t, const float* g, int w0 = 0, int w1 = -1, cudaStream_t st = nullptr,
+static int enqueue_optimizer(sb_trainer* t, const StepIn& in, const float* g, int w0 = 0, int w1 = -1, cudaStream_t st = nullptr,
                              bool publish_scalars = false, bool pdl = false) {
   Net& n = t->net;
   if (w1 < 0) w1 = n.n_work;
   if (!st) st = n.stream;
   if (w1 <= w0) return SB_OK;
   // pdl = false: plain dependency (runs after a stream join / on the comm stream)
-  SB_TRY(launch_kernel(optimizer_kernel, dim3(static_cast<unsigned>(w1 - w0)), dim3(256), 0, st, pdl, n.work + w0, n.desc, t->hyper,
-                       n.theta, g, n.s1, n.s2, n.scal, publish_scalars ? t->d_hscal : static_cast<float*>(nullptr),
+  SB_TRY(launch_kernel(optimizer_kernel, dim3(static_cast<unsigned>(w1 - w0)), dim3(256), 0, st, pdl, n.work + w0, in.desc, t->hyper,
+                       n.theta, g, n.s1, n.s2, in.scal, publish_scalars ? t->d_hscal : static_cast<float*>(nullptr),
                        n.next_trace(st == n.stream ? "opt" : "opt_side")));
   n.mark("optimizer");
   return SB_OK;
@@ -130,7 +137,7 @@ static int enqueue_optimizer(sb_trainer* t, const float* g, int w0 = 0, int w1 =
 enum { XSEG_A = 1 };
 static int xseg_all(const sb_trainer* t) { return (1 << t->x_slots) - 1; }
 
-static XchgParams xchg_params(sb_trainer* t) {
+static XchgParams xchg_params(sb_trainer* t, const BatchDesc* desc) {
   Net& n = t->net;
   XchgParams p;
   memset(&p, 0, sizeof(p));
@@ -141,7 +148,7 @@ static XchgParams xchg_params(sb_trainer* t) {
   p.work = n.work;
   p.n_slots = t->x_slots;
   for (int sl = 0; sl < t->x_slots; ++sl) { p.slot_begin[sl] = t->x_begin[sl]; p.slot_end[sl] = t->x_end[sl]; }
-  p.desc = n.desc;
+  p.desc = desc;
   p.hyper = t->hyper;
   p.host_err = t->d_herr;
   p.timeout_ns = t->xchg_timeout_ns;
@@ -151,11 +158,12 @@ static XchgParams xchg_params(sb_trainer* t) {
 }
 
 // reduce-scatter -> owner update -> all-gather of the operands for the given segments (xchg_p2p.cuh); `g` must be t->grad
-static int enqueue_xchg(sb_trainer* t, int slot_mask, cudaStream_t st, bool publish_scalars, bool pdl, bool alone = false) {
+static int enqueue_xchg(sb_trainer* t, const StepIn& in, int slot_mask, cudaStream_t st, bool publish_scalars, bool pdl,
+                        bool alone = false) {
   Net& n = t->net;
-  XchgParams p = xchg_params(t);
+  XchgParams p = xchg_params(t, in.desc);
   p.slot_mask = slot_mask;
-  p.scal = publish_scalars ? n.scal : nullptr;
+  p.scal = publish_scalars ? in.scal : nullptr;
   p.host_scal = publish_scalars ? t->d_hscal : nullptr;
   char nm[24];
   if (slot_mask == XSEG_A) snprintf(nm, sizeof(nm), "xchg_A");
@@ -204,7 +212,7 @@ static int gather_master(sb_trainer* t) {
   if (!t->p2p_ready || !t->master_stale || t->world <= 1) return SB_OK;
   Net& n = t->net;
   SB_CUDA(cudaStreamSynchronize(n.stream));     // my last exchange kernel has seen every peer's done flag
-  XchgParams p = xchg_params(t);
+  XchgParams p = xchg_params(t, n.desc);
   gather_master_kernel<<<n.n_work, 256, 0, n.stream>>>(p, 0);
   SB_CUDA(cudaGetLastError());
   SB_CUDA(cudaStreamSynchronize(n.stream));
@@ -212,152 +220,212 @@ static int gather_master(sb_trainer* t) {
   return SB_OK;
 }
 
-// the body of one step as a sequence of stream operations (captured into a CUDA graph)
-static int enqueue_step_body(sb_trainer* t, int rows, int kind, bool resident = false, bool sparse = false) {
+// `to` waits for everything enqueued on `from` so far
+static int join_streams(cudaStream_t to, cudaStream_t from, cudaEvent_t e) {
+  SB_CUDA(cudaEventRecord(e, from));
+  SB_CUDA(cudaStreamWaitEvent(to, e, 0));
+  return SB_OK;
+}
+
+// Where dW_1 runs, and the SM budget (grid cap) of dW_0 / dW_1, in a tensor-core step with more than one hidden layer:
+//   BESIDE  on the side stream, at the same time as dW_0 on the main stream;
+//   FRONT   on the main stream in front of dW_0;
+//   BEHIND  on the main stream behind dW_0.
+enum Dw1At { DW1_BESIDE, DW1_FRONT, DW1_BEHIND };
+struct Dw1Plan {
+  Dw1At at;
+  int sms[2];
+};
+
+static Dw1Plan plan_dw1(const sb_trainer* t, int rows, bool split_tail, bool xsched) {
+  const Net& n = t->net;
+  const int S = n.num_sms;
+  Dw1Plan d = {DW1_BESIDE, {S, S}};
+  // peer exchange: in front of dW_0, so that slot A's exchange hides behind dW_0's chunks; replicas that share a device
+  // put it behind, as cover for the last chunk's exchange
+  if (xsched) {
+    d.at = t->peers_share_device ? DW1_BEHIND : DW1_FRONT;
+    return d;
+  }
+  // dW_1 (side stream) and dW_0 (main stream) run at the same time, one CTA per SM each.  If their natural grids do not
+  // fit the machine together, dW_1's second wave only starts when dW_0's CTAs exit.
+  const Layer& l0 = n.layers[0];
+  const Layer& l1 = n.layers[1];
+  const int kx = round_up(rows, 64) * pairs_of(n.nparts);
+  const GemmPlan n0 = plan_gemm(l0.in, l0.out, kx, S, true);
+  const GemmPlan n1 = plan_gemm(l1.in, l1.out, kx, S, true);
+  if (n0.grid + n1.grid <= S) return d;
+  // single-GPU tail: dW_1 runs IN FRONT of dW_0 on the main stream instead of beside it - side by side the two persistent
+  // grids take turns on the SMs; small layers (cfg1) stay side by side.  Only when dW_0 alone fills every SM: on one H100,
+  // cfg2 (dW_0 = 128 tiles on 132 SMs, budget split below) measured within 1 % of both dW_1 in front and the natural
+  // grids, while moving dW_1 in front once dW_0 fills >= 90 % of the SMs made cfg1 4 % slower
+  if (split_tail && n0.grid == S) {
+    d.at = DW1_FRONT;
+    return d;
+  }
+  // compare, in k-blocks per CTA, "natural grids, dW_1 finishing after dW_0" against "dW_1 on a third of the SMs, dW_0
+  // on the rest" and take the shorter
+  const GemmPlan b1 = plan_gemm(l1.in, l1.out, kx, S / 3, true);
+  const GemmPlan b0 = plan_gemm(l0.in, l0.out, kx, S - b1.grid, true);
+  auto waves = [&](const GemmPlan& pl, const Layer& ly, int sms) {   // k-blocks one CTA works through
+    const int tiles = ((ly.in + 127) / 128) * ((ly.out + pl.bn - 1) / pl.bn) * pl.split_k;
+    return ((tiles + sms - 1) / sms) * pl.kb_per_split;
+  };
+  const int t_nat = waves(n0, l0, S) + waves(n1, l1, S);
+  const int t0 = waves(b0, l0, S - b1.grid);
+  const int t1 = waves(b1, l1, S / 3);
+  if ((t0 > t1 ? t0 : t1) < t_nat) { d.sms[1] = S / 3; d.sms[0] = S - b1.grid; }
+  return d;
+}
+
+// The step's backward pass and tail, in launch order.
+static int enqueue_step_backward(sb_trainer* t, const StepIn& in, int rows, int kind) {
   Net& n = t->net;
-  struct Scope {
-    Net& n;
-    ~Scope() {
-      n.from_resident = false; n.zero_buf = nullptr; n.defer_join = false; n.sparse_step = false;
-      n.dw0_chunks = 1; n.dw1_last = false; n.on_dw0_chunk = nullptr;
-      n.dw1_first = false; n.after_dw1 = nullptr; n.dw1_serial_auto = false;
-    }
-  } scope{n};
-  n.from_resident = resident;
-  n.sparse_step = sparse;
-  n.trace_k = 0;
-  // ---- schedule of the step's tail ----
-  // Single GPU, one update per mini-batch: no exchange, so nothing needs ALL gradients at once.  dW_0 runs on the main
-  // stream behind the last dA GEMM and is followed (PDL) by the optimizer of layer 0 alone; the side stream updates the
-  // other layers right after their dW GEMMs; the two streams only join at the end of the graph.
-  const bool split_tail = kind == G_STEP && (t->world == 1 || t->p2p_ready) && n.side != nullptr && n.tc() && n.L > 1;
-  // Peer exchange (world > 1): one exchange launch costs several fabric round trips however little data it moves (xchg_p2p.cuh)
-  // - hidden when a GEMM follows it, exposed in full behind the last GEMM:
-  //   main:  ... dA_1 -> dW_1 -> dW_0 chunk 0 -> dW_0 chunk 1 | wait A, B0, B1 | next step
-  //   side:  ... dW_2 ...     A ------------->
-  //   comm:                             B0 ---------------->    B1 ------>
-  // A (every layer but hidden layer 0) and B0 run beside dW_0's chunks, only B1 - half of layer 0 - is exposed, on an
-  // otherwise idle GPU, where an exchange kernel is faster than beside a GEMM.
-  // Replicas that share ONE device (tests) put dW_1 BEHIND dW_0 instead, as cover for B1, and launch A on the side stream
-  // behind it: with three exchange launches of both replicas waiting beside each other's persistent GEMMs, dW_1 in front
-  // stopped making progress within the exchange timeout.
-  // Every exchange launch of the step is joined into the main stream before the step ends.  A rank's exchange only ends
-  // once every peer has read the gradient runs it owns of this rank (xchg_p2p.cuh), so the next step's layer-0 forward
-  // GEMM may clear the gradient buffer.
-  const bool xsched = split_tail && t->world > 1;
-  if (resident) {
-    // no load kernel: the batch is read by TMA from the bf16 resident set; set_batch_kernel already published n_nz.
-    // The gradient buffer is first written by the last forward layer's epilogue, so with more than one hidden layer the
-    // layer-0 forward GEMM clears it (its producer warpgroup's idle warps, beside the main loop) instead of a memset node
-    // at the head of the chain.
-    if (n.L > 1) {
-      n.zero_buf = reinterpret_cast<float4*>(t->grad);   // cudaMalloc'ed, padded to xch_n4 float4
-      n.zero_n4 = t->xch_n4;
-    } else {
-      SB_CUDA(cudaMemsetAsync(t->grad, 0, sizeof(float) * n.n_params, n.stream));
+  float* g = t->grad;
+  const int L = n.L, S = n.num_sms;
+  if (!n.tc()) {
+    for (int l = L - 1; l >= 0; --l) {            // fp32: one stream
+      SB_TRY(n.enqueue_dw(in, l, rows, g, n.stream, false, S));
+      if (l > 0) SB_TRY(n.enqueue_da(l, rows, g));
     }
   } else {
-    SB_TRY(n.enqueue_load(rows, t->grad, n.n_params));   // also clears the gradient buffer and the step scalars
-  }
-  bool fused_out = false;
-  SB_TRY(n.enqueue_hidden_forward(rows, t->grad, &fused_out));
-  if (!fused_out) SB_TRY(n.enqueue_out(rows, true, true, nullptr, t->grad));
-  n.defer_join = split_tail;
-  cudaStream_t comms[2] = {n.comm2, n.comm};
-  if (xsched) {
-    // dW_1 leaves the side stream: in front of dW_0, or behind it when the replicas share a device
-    n.dw0_chunks = t->x_chunks;
-    n.dw1_last = t->peers_share_device;
-    n.dw1_first = !t->peers_share_device;
-    t->x_sent = 0;
-    if (n.dw1_first) {
-      n.after_dw1 = [t]() -> int {       // slot A on the side stream, behind dW_1 (main) and the other layers' dW GEMMs (side)
-        Net& nn = t->net;
-        SB_CUDA(cudaEventRecord(t->ev_c[0], nn.stream));
-        SB_CUDA(cudaStreamWaitEvent(nn.side, t->ev_c[0], 0));
-        SB_TRY(enqueue_xchg(t, XSEG_A, nn.side, false, false));
-        SB_CUDA(cudaEventRecord(t->ev_x[0], nn.side));
-        t->x_sent |= XSEG_A;
-        return SB_OK;
-      };
+    // Single GPU, one update per mini-batch: no exchange, so nothing needs ALL gradients at once.  dW_0 runs on the main
+    // stream behind the last dA GEMM and is followed (PDL) by the optimizer of layer 0 alone; the side stream updates the
+    // other layers right after their dW GEMMs; the two streams only join at the end of the graph.
+    const bool split_tail = kind == G_STEP && (t->world == 1 || t->p2p_ready) && L > 1;
+    // Peer exchange (world > 1): one exchange launch costs several fabric round trips however little data it moves
+    // (xchg_p2p.cuh) - hidden when a GEMM follows it, exposed in full behind the last GEMM:
+    //   main:  ... dA_1 -> dW_1 -> dW_0 chunk 0 -> dW_0 chunk 1 | wait A, B0, B1 | next step
+    //   side:  ... dW_2 ...     A ------------->
+    //   comm:                             B0 ---------------->    B1 ------>
+    // A (every layer but hidden layer 0) and B0 run beside dW_0's chunks, only B1 - half of layer 0 - is exposed, on an
+    // otherwise idle GPU, where an exchange kernel is faster than beside a GEMM.
+    // Replicas that share ONE device (tests) put dW_1 BEHIND dW_0 instead, as cover for B1, and launch A on the side
+    // stream behind it: with three exchange launches of both replicas waiting beside each other's persistent GEMMs, dW_1
+    // in front stopped making progress within the exchange timeout.
+    // Every exchange launch of the step is joined into the main stream before the step ends.  A rank's exchange only ends
+    // once every peer has read the gradient runs it owns of this rank (xchg_p2p.cuh), so the next step's layer-0 forward
+    // GEMM may clear the gradient buffer.
+    const bool xsched = split_tail && t->world > 1;
+    const Dw1Plan d1 = L > 1 ? plan_dw1(t, rows, split_tail, xsched) : Dw1Plan{DW1_BESIDE, {S, S}};
+    // dW_l and dA_l both consume dZ_l and are independent of each other: the dW GEMMs go to the side stream and overlap
+    // the dA chain
+    for (int l = L - 1; l >= 1; --l) {
+      if (l > 1 || d1.at == DW1_BESIDE) {
+        SB_TRY(join_streams(t->side, n.stream, t->ev_dz[l]));
+        SB_TRY(n.enqueue_dw(in, l, rows, g, t->side, false, l == 1 ? d1.sms[1] : S));
+      }
+      SB_TRY(n.enqueue_da(l, rows, g));
     }
-    n.on_dw0_chunk = [t, comms](int c) -> int {
-      Net& nn = t->net;
-      cudaStream_t cs = comms[c & 1];
-      SB_CUDA(cudaEventRecord(t->ev_c[1 + c], nn.stream));
-      SB_CUDA(cudaStreamWaitEvent(cs, t->ev_c[1 + c], 0));
-      const bool last = c == t->x_chunks - 1;
-      SB_TRY(enqueue_xchg(t, 1 << (1 + c), cs, last, false, last && !nn.dw1_last));   // (the last chunk publishes the step scalars;
-                                                                                       //  no GEMM follows it unless dW_1 does)
-      SB_CUDA(cudaEventRecord(t->ev_x[1 + c], cs));
-      t->x_sent |= 1 << (1 + c);
-      return SB_OK;
-    };
-  }
-  if (split_tail && !xsched) {
-    // one GPU: dW_1 may move in front of dW_0 (Net::dw1_serial_auto); the side stream's optimizer launch then waits for it
-    n.dw1_serial_auto = true;
-    n.after_dw1 = [t]() -> int {
-      Net& nn = t->net;
-      SB_CUDA(cudaEventRecord(t->ev_c[0], nn.stream));
-      SB_CUDA(cudaStreamWaitEvent(nn.side, t->ev_c[0], 0));
-      return SB_OK;
-    };
-  }
-  SB_TRY(n.enqueue_backward(rows, t->grad));
-  if (xsched) {
-    // slot A: every gradient but hidden layer 0's - complete behind dW_1 (main stream), the other layers' dW GEMMs (side
-    // stream) and the last dA GEMM (the last reader of their weight shadows).  (dW_1 in front of dW_0: after_dw1 launched it.)
-    if (n.dw1_last) {
-      SB_CUDA(cudaEventRecord(t->ev_c[0], n.stream));
-      SB_CUDA(cudaStreamWaitEvent(n.side, t->ev_c[0], 0));
-      SB_TRY(enqueue_xchg(t, XSEG_A, n.side, false, false));
-      SB_CUDA(cudaEventRecord(t->ev_x[0], n.side));
+    if (split_tail) SB_CUDA(cudaEventRecord(t->ev_da_done, n.stream));
+    if (L == 1) {
+      SB_TRY(join_streams(t->side, n.stream, t->ev_dz[0]));
+      SB_TRY(n.enqueue_dw(in, 0, rows, g, t->side, false, S));
+    } else {
+      if (d1.at == DW1_FRONT) {
+        // dW_0's last exchange then runs on an idle GPU; the side stream's next launch (slot A's exchange, or the
+        // optimizer of the other layers) waits for dW_1
+        SB_TRY(n.enqueue_dw(in, 1, rows, g, n.stream, true, d1.sms[1]));
+        SB_TRY(join_streams(t->side, n.stream, t->ev_c[0]));
+        if (xsched) {
+          SB_TRY(enqueue_xchg(t, in, XSEG_A, t->side, false, false));
+          SB_CUDA(cudaEventRecord(t->ev_x[0], t->side));
+        }
+      }
+      // dW_0 has nothing to overlap with (no dA_0): PDL-chained on the main stream right behind the last GEMM it starts
+      // earlier than as a cross-stream launch.  With the peer exchange it is cut into the slot chunks (each a contiguous
+      // slice of the flat gradient) and each chunk's exchange overlaps the GEMMs that follow it.
+      if (xsched && !in.sparse) {
+        for (int c = 0; c < t->x_chunks; ++c) {
+          const int r0 = c * t->x_chunk_rows, r1 = std::min(r0 + t->x_chunk_rows, n.layers[0].in);
+          SB_TRY(n.enqueue_dw(in, 0, rows, g, n.stream, true, d1.sms[0], r0, r1, t->x_chunks > 1 ? c : -1));
+          cudaStream_t cs = t->xstream[c & 1];
+          SB_TRY(join_streams(cs, n.stream, t->ev_c[1 + c]));
+          // the last chunk publishes the step scalars; no GEMM follows it unless dW_1 does
+          const bool last = c == t->x_chunks - 1;
+          SB_TRY(enqueue_xchg(t, in, 1 << (1 + c), cs, last, false, last && d1.at != DW1_BEHIND));
+          SB_CUDA(cudaEventRecord(t->ev_x[1 + c], cs));
+        }
+      } else {
+        SB_TRY(n.enqueue_dw(in, 0, rows, g, n.stream, true, d1.sms[0]));
+      }
+      if (d1.at == DW1_BEHIND) {
+        SB_TRY(n.enqueue_dw(in, 1, rows, g, n.stream, true, d1.sms[1]));
+        SB_TRY(join_streams(t->side, n.stream, t->ev_c[0]));
+        SB_TRY(enqueue_xchg(t, in, XSEG_A, t->side, false, false));
+        SB_CUDA(cudaEventRecord(t->ev_x[0], t->side));
+      }
     }
-    // whatever follows on the main stream (the next step's layer-0 forward, or the end of the graph) needs hidden layer 0
-    for (int c = 0; c < t->x_chunks; ++c)
-      if ((t->x_sent >> (1 + c)) & 1) SB_CUDA(cudaStreamWaitEvent(n.stream, t->ev_x[1 + c], 0));
-    // (a layer-0 dW that was not cut into the trainer's chunks - wide+deep steps - is exchanged here, behind everything)
-    const int missing = (xseg_all(t) & ~XSEG_A) & ~t->x_sent;
-    if (missing) SB_TRY(enqueue_xchg(t, missing, n.stream, true, false));
-    SB_CUDA(cudaStreamWaitEvent(n.stream, t->ev_x[0], 0));
-    return SB_OK;
-  }
-  if (split_tail) {
-    SB_TRY(enqueue_optimizer(t, t->grad, n.work_begin[0], n.work_end[0], n.stream, true, true));
-    // the other layers' shadows are read by the dA GEMMs on the main stream: update them only after the last one
-    SB_CUDA(cudaStreamWaitEvent(n.side, n.ev_da_done, 0));
-    SB_TRY(enqueue_optimizer(t, t->grad, n.work_end[0], n.n_work, n.side));
-    SB_CUDA(cudaEventRecord(n.ev_join, n.side));
-    SB_CUDA(cudaStreamWaitEvent(n.stream, n.ev_join, 0));
-    return SB_OK;
+    if (xsched) {
+      // whatever follows on the main stream (the next step's layer-0 forward, or the end of the graph) needs hidden
+      // layer 0.  A wide+deep step's layer-0 dW is not cut into the slot chunks: it is exchanged here, behind everything.
+      if (in.sparse) SB_TRY(enqueue_xchg(t, in, xseg_all(t) & ~XSEG_A, n.stream, true, false));
+      else
+        for (int c = 0; c < t->x_chunks; ++c) SB_CUDA(cudaStreamWaitEvent(n.stream, t->ev_x[1 + c], 0));
+      SB_CUDA(cudaStreamWaitEvent(n.stream, t->ev_x[0], 0));
+      return SB_OK;
+    }
+    if (split_tail) {
+      SB_TRY(enqueue_optimizer(t, in, g, n.work_begin[0], n.work_end[0], n.stream, true, true));
+      // the other layers' shadows are read by the dA GEMMs on the main stream: update them only after the last one
+      SB_CUDA(cudaStreamWaitEvent(t->side, t->ev_da_done, 0));
+      SB_TRY(enqueue_optimizer(t, in, g, n.work_end[0], n.n_work, t->side));
+      return join_streams(n.stream, t->side, t->ev_join);
+    }
+    SB_TRY(join_streams(n.stream, t->side, t->ev_join));
   }
   if (kind == G_STEP) {
     if (t->world > 1 && t->p2p_ready) {
       // (fp32 mode or one hidden layer: no split tail) one launch handles both segments
-      SB_TRY(enqueue_xchg(t, xseg_all(t), n.stream, true, false));
+      SB_TRY(enqueue_xchg(t, in, xseg_all(t), n.stream, true, false));
     } else {
-      SB_TRY(enqueue_allreduce(t, t->grad));
-      SB_TRY(enqueue_optimizer(t, t->grad, 0, -1, nullptr, true, false));
+      SB_TRY(enqueue_allreduce(t, g));
+      SB_TRY(enqueue_optimizer(t, in, g, 0, -1, nullptr, true, false));
     }
   } else {
     const long long np = n.n_params;
-    axpy_kernel<<<static_cast<unsigned>((np + 255) / 256), 256, 0, n.stream>>>(t->acc, t->grad, np, n.scal, t->d_hscal);
+    axpy_kernel<<<static_cast<unsigned>((np + 255) / 256), 256, 0, n.stream>>>(t->acc, g, np, in.scal, t->d_hscal);
     SB_CUDA(cudaGetLastError());
     n.mark("accumulate");
   }
   return SB_OK;
 }
 
-static int get_graph(sb_trainer* t, int rows, int kind, bool resident, int pair, cudaGraphExec_t* out, bool sparse = false) {
-  auto key = std::make_pair(rows, kind * 8 + (sparse ? 4 : 0) + (resident ? 2 : 0) + pair);
+// the body of one step as a sequence of stream operations (captured into a CUDA graph)
+static int enqueue_step_body(sb_trainer* t, const StepIn& in, int rows, int kind) {
+  Net& n = t->net;
+  n.trace_k = 0;
+  float4* clear = nullptr;
+  long long clear_n4 = 0;
+  if (in.resident) {
+    // no load kernel: the batch is read by TMA from the bf16 resident set; set_batch_kernel already published n_nz.
+    // The gradient buffer is first written by the last forward layer's epilogue, so with more than one hidden layer the
+    // layer-0 forward GEMM clears it (its producer warpgroup's idle warps, beside the main loop) instead of a memset node
+    // at the head of the chain.
+    if (n.L > 1) {
+      clear = reinterpret_cast<float4*>(t->grad);   // cudaMalloc'ed, padded to xch_n4 float4
+      clear_n4 = t->xch_n4;
+    } else {
+      SB_CUDA(cudaMemsetAsync(t->grad, 0, sizeof(float) * n.n_params, n.stream));
+    }
+  } else {
+    SB_TRY(n.enqueue_load(in, rows, t->grad, n.n_params));   // also clears the gradient buffer and the step scalars
+  }
+  bool fused_out = false;
+  SB_TRY(n.enqueue_hidden_forward(in, rows, t->grad, &fused_out, clear, clear_n4));
+  if (!fused_out) SB_TRY(n.enqueue_out(in, rows, true, true, nullptr, t->grad));
+  return enqueue_step_backward(t, in, rows, kind);
+}
+
+static int get_graph(sb_trainer* t, const StepIn& in, int rows, int kind, int pair, cudaGraphExec_t* out) {
+  auto key = std::make_pair(rows, kind * 8 + (in.sparse ? 4 : 0) + (in.resident ? 2 : 0) + pair);
   auto it = t->graphs.find(key);
   if (it != t->graphs.end()) { *out = it->second; return SB_OK; }
   Net& n = t->net;
   n.launches = 0;
   cudaGraph_t g = nullptr;
   SB_CUDA(cudaStreamBeginCapture(n.stream, cudaStreamCaptureModeThreadLocal));
-  int s = enqueue_step_body(t, rows, kind, resident, sparse);
+  int s = enqueue_step_body(t, in, rows, kind);
   cudaError_t e = cudaStreamEndCapture(n.stream, &g);
   if (s != SB_OK) { if (g) cudaGraphDestroy(g); return s; }
   SB_CHECK(e == cudaSuccess, SB_ERR_CUDA, "cudaStreamEndCapture failed: %s", cudaGetErrorString(e));
@@ -365,7 +433,7 @@ static int get_graph(sb_trainer* t, int rows, int kind, bool resident, int pair,
   SB_CUDA(cudaGraphInstantiate(&ge, g, 0));
   cudaGraphDestroy(g);
   t->graphs[key] = ge;
-  if (kind == G_STEP && !sparse && (resident || !t->dsXb)) t->kernels_per_step[rows] = n.launches + 1;  // + set_batch_kernel
+  if (kind == G_STEP && !in.sparse && (in.resident || !t->dsXb)) t->kernels_per_step[rows] = n.launches + 1;  // + set_batch_kernel
   *out = ge;
   return SB_OK;
 }
@@ -380,10 +448,10 @@ static int run_step(sb_trainer* t, const float* X, const float* y, const float* 
   // descriptor / scalar pair of this step: resident graph steps alternate, everything else uses pair 0
   const bool prep = resident && t->prep != nullptr;
   const int pair = prep ? static_cast<int>(t->prep_steps & 1) : 0;
-  n.desc = t->descs[pair];
-  n.scal = t->scals[pair];
+  const StepIn in{t->descs[pair], t->scals[pair], resident, sparse};
+  t->last_pair = pair;
   cudaGraphExec_t ge = nullptr;
-  SB_TRY(get_graph(t, rows, kind, resident, pair, &ge, sparse));
+  SB_TRY(get_graph(t, in, rows, kind, pair, &ge));
   float lr_t = t->lr, gscale = 1.f / static_cast<float>(t->world);
   if (kind == G_STEP) {
     ++t->global_step;
@@ -396,7 +464,7 @@ static int run_step(sb_trainer* t, const float* X, const float* y, const float* 
     // main stream's current position.
     if (!t->have_pos) SB_CUDA(cudaEventRecord(t->ev_pos[pair ^ 1], n.stream));
     SB_CUDA(cudaStreamWaitEvent(t->prep, t->ev_pos[pair ^ 1], 0));
-    set_batch_kernel<<<1, 1, 0, t->prep>>>(n.desc, nullptr, y, w, lr_t, gscale, t->epoch, static_cast<int>(resident_row0), t->dsP, rows, n.scal,
+    set_batch_kernel<<<1, 1, 0, t->prep>>>(in.desc, nullptr, y, w, lr_t, gscale, t->epoch, static_cast<int>(resident_row0), t->dsP, rows, in.scal,
                                            kind == G_STEP ? t->hist_slot(t->global_step) : nullptr);
     SB_CUDA(cudaGetLastError());
     SB_CUDA(cudaEventRecord(t->ev_prep[pair], t->prep));
@@ -407,10 +475,10 @@ static int run_step(sb_trainer* t, const float* X, const float* y, const float* 
   } else {
     t->have_pos = false;
     if (resident)
-      set_batch_kernel<<<1, 1, 0, n.stream>>>(n.desc, nullptr, y, w, lr_t, gscale, t->epoch, static_cast<int>(resident_row0), t->dsP, rows, n.scal,
+      set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, nullptr, y, w, lr_t, gscale, t->epoch, static_cast<int>(resident_row0), t->dsP, rows, in.scal,
                                                kind == G_STEP ? t->hist_slot(t->global_step) : nullptr);
     else
-      set_batch_kernel<<<1, 1, 0, n.stream>>>(n.desc, X, y, w ? w : n.ones, lr_t, gscale, t->epoch, 0, nullptr, 0, nullptr,
+      set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, X, y, w ? w : n.ones, lr_t, gscale, t->epoch, 0, nullptr, 0, nullptr,
                                                kind == G_STEP ? t->hist_slot(t->global_step) : nullptr);
   }
   SB_CUDA(cudaGetLastError());
@@ -543,6 +611,21 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
   cudaFuncSetAttribute(optimizer_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   cudaFuncSetAttribute(axpy_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   Net& n = t->net;
+  {
+    // streams and events of the step schedule; the side stream's CTAs are scheduled behind the main chain's
+    int prio_least = 0, prio_greatest = 0;
+    bool ok = cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest) == cudaSuccess &&
+              cudaStreamCreateWithPriority(&t->side, cudaStreamNonBlocking, prio_least) == cudaSuccess;
+    t->ev_dz.assign(n.L, nullptr);
+    for (auto& e : t->ev_dz) ok = ok && cudaEventCreateWithFlags(&e, cudaEventDisableTiming) == cudaSuccess;
+    ok = ok && cudaEventCreateWithFlags(&t->ev_join, cudaEventDisableTiming) == cudaSuccess &&
+         cudaEventCreateWithFlags(&t->ev_da_done, cudaEventDisableTiming) == cudaSuccess;
+    for (auto& x : t->xstream) ok = ok && cudaStreamCreateWithFlags(&x, cudaStreamNonBlocking) == cudaSuccess;
+    if (!ok) {
+      n.destroy();
+      return set_error(SB_ERR_CUDA, "cudaStreamCreate / cudaEventCreate failed");
+    }
+  }
   // gradient + exchange flags behind the parameters, in the arena a single IPC handle exports
   t->xch = n.arena;
   t->grad_off = static_cast<long long>(n.extra_off);
@@ -574,10 +657,9 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
     int chunks = 2;
     const Layer& l0 = n.layers[0];
     if (!n.tc() || (l0.out % 8) != 0 || l0.in < 256 * chunks) chunks = 1;
-    n.dw0_chunks = chunks;
-    const int cr = n.dw0_chunk_rows();
+    const int cr = round_up((l0.in + chunks - 1) / chunks, 128);
     chunks = (l0.in + cr - 1) / cr;           // (rounding to 128 rows may need fewer chunks)
-    n.dw0_chunks = 1;                          // the GEMM is only cut while a step with the peer exchange is enqueued
+    t->x_chunk_rows = cr;
     t->x_chunks = chunks;
     t->x_slots = 1 + chunks;
     t->x_begin[0] = n.work_end[0]; t->x_end[0] = n.n_work;
@@ -781,6 +863,11 @@ int sb_trainer_destroy(sb_trainer_t* t) {
   }
   for (void* p : t->peer_bases) cudaIpcCloseMemHandle(p);
   if (t->d_peers) cudaFree(t->d_peers);
+  for (cudaEvent_t e : t->ev_dz) if (e) cudaEventDestroy(e);
+  if (t->ev_join) cudaEventDestroy(t->ev_join);
+  if (t->ev_da_done) cudaEventDestroy(t->ev_da_done);
+  for (cudaStream_t x : t->xstream) if (x) cudaStreamDestroy(x);
+  if (t->side) cudaStreamDestroy(t->side);
   t->net.destroy();      // frees the arena (= xch)
   delete t;
   return SB_OK;
@@ -830,7 +917,7 @@ int sb_trainer_get_grads(sb_trainer_t* t, float* flat, int64_t n) {
     // sharded exchange: every owner kept the reduced gradient of its runs; collect them (overwrites this rank's own
     // contributions, which the next step clears anyway)
     SB_CUDA(cudaStreamSynchronize(t->net.stream));
-    gather_master_kernel<<<t->net.n_work, 256, 0, t->net.stream>>>(xchg_params(t), 1);
+    gather_master_kernel<<<t->net.n_work, 256, 0, t->net.stream>>>(xchg_params(t, t->net.desc), 1);
     SB_CUDA(cudaGetLastError());
   }
   SB_CUDA(cudaMemcpyAsync(flat, t->grad, sizeof(float) * n, cudaMemcpyDeviceToHost, t->net.stream));
@@ -878,20 +965,18 @@ int sb_trainer_step_sparse(sb_trainer_t* t, const float* Xd, const int32_t* idx,
 // forward (+ loss) over any number of sparse rows in max_batch chunks; out / loss accumulators nullable
 static int forward_chunks_sparse(Net& n, const float* Xd, const int32_t* idx, const float* y, const float* w, int64_t rows, float* out,
                                  double* loss_sum, double* nnz) {
-  struct Scope { Net& n; ~Scope() { n.sparse_step = false; } } scope{n};
+  const StepIn in{n.desc, n.scal, false, true};      // (the trainer's pair 0, see forward_chunks)
   const bool do_loss = loss_sum != nullptr;
   float h[SCAL_COUNT];
   for (int64_t r0 = 0; r0 < rows; r0 += n.max_batch) {
     const int c = static_cast<int>(rows - r0 < n.max_batch ? rows - r0 : n.max_batch);
     SB_TRY(stage_sparse_batch(n, Xd + r0 * n.n_dense, idx + r0 * n.n_cat, do_loss ? y + r0 : nullptr, (do_loss && w) ? w + r0 : nullptr, c));
-    set_batch_kernel<<<1, 1, 0, n.stream>>>(n.desc, n.stX, n.stY, (do_loss && w) ? n.stW : n.ones, 0.f, 1.f);
-    n.sparse_step = true;
-    SB_TRY(n.enqueue_load(c));
-    SB_TRY(n.enqueue_hidden_forward(c));
-    n.sparse_step = false;
-    SB_TRY(n.enqueue_out(c, do_loss, false, n.yhat, nullptr));
+    set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, n.stX, n.stY, (do_loss && w) ? n.stW : n.ones, 0.f, 1.f);
+    SB_TRY(n.enqueue_load(in, c));
+    SB_TRY(n.enqueue_hidden_forward(in, c));
+    SB_TRY(n.enqueue_out(in, c, do_loss, false, n.yhat, nullptr));
     if (out) SB_CUDA(cudaMemcpyAsync(out + r0, n.yhat, sizeof(float) * c, cudaMemcpyDeviceToHost, n.stream));
-    if (do_loss) SB_CUDA(cudaMemcpyAsync(h, n.scal, sizeof(h), cudaMemcpyDeviceToHost, n.stream));
+    if (do_loss) SB_CUDA(cudaMemcpyAsync(h, in.scal, sizeof(h), cudaMemcpyDeviceToHost, n.stream));
     SB_CUDA(cudaStreamSynchronize(n.stream));
     if (do_loss) { *loss_sum += h[SCAL_LOSS_SUM]; *nnz += h[SCAL_NNZ]; }
   }
@@ -972,18 +1057,20 @@ static int apply_accumulated_impl(sb_trainer_t* t, int64_t total_pushes) {
   ++t->global_step;
   const float gscale = 1.f / static_cast<float>(total_pushes);
   ++t->epoch;
-  set_batch_kernel<<<1, 1, 0, n.stream>>>(n.desc, nullptr, nullptr, nullptr, lr_for_step(t, t->global_step), gscale, t->epoch);
+  // the last step's pair: the next resident step's descriptor prefetch may write the other one while this update runs
+  const StepIn in{t->descs[t->last_pair], t->scals[t->last_pair]};
+  set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, nullptr, nullptr, nullptr, lr_for_step(t, t->global_step), gscale, t->epoch);
   SB_CUDA(cudaGetLastError());
   // exchange + apply through the (IPC-exported) gradient buffer; it then holds the applied mean for sb_trainer_get_grads
   SB_CUDA(cudaMemcpyAsync(t->grad, t->acc, sizeof(float) * n.n_params, cudaMemcpyDeviceToDevice, n.stream));
   if (t->world > 1 && t->p2p_ready) {
-    SB_TRY(enqueue_xchg(t, xseg_all(t), n.stream, false, false));
+    SB_TRY(enqueue_xchg(t, in, xseg_all(t), n.stream, false, false));
   } else {
     SB_TRY(enqueue_allreduce(t, t->grad));
-    SB_TRY(enqueue_optimizer(t, t->grad));
+    SB_TRY(enqueue_optimizer(t, in, t->grad));
   }
   const long long np = n.n_params;
-  scale_kernel<<<static_cast<unsigned>((np + 255) / 256), 256, 0, n.stream>>>(t->grad, n.desc, np);
+  scale_kernel<<<static_cast<unsigned>((np + 255) / 256), 256, 0, n.stream>>>(t->grad, in.desc, np);
   SB_CUDA(cudaGetLastError());
   t->grad_out_scale = 1.f;  // scale_kernel already applied 1/(world * n_acc)
   zero_f32_kernel<<<static_cast<unsigned>((np + 255) / 256), 256, 0, n.stream>>>(t->acc, np);   // (a preloaded kernel, see preload_exchange_kernels)
@@ -1080,20 +1167,17 @@ static int get_run_graph(sb_trainer* t, int rows, int set, cudaGraphExec_t* out)
   auto it = t->run_graphs.find(key);
   if (it != t->run_graphs.end()) { *out = it->second; return SB_OK; }
   Net& n = t->net;
-  BatchDesc* d0 = n.desc; float* s0 = n.scal;
   cudaGraph_t g = nullptr;
   SB_CUDA(cudaStreamBeginCapture(n.stream, cudaStreamCaptureModeThreadLocal));
   int s = SB_OK;
   for (int k = 0; k < sb_trainer::RUN_S && s == SB_OK; ++k) {
-    n.desc = t->run_descs[set][k];
-    n.scal = t->run_scals[set][k];
+    const StepIn in{t->run_descs[set][k], t->run_scals[set][k], true, false};
     // (SB_STEP_TRACE: an interior step is the one traced - it starts behind the previous step's tail, as most steps of a
     // run do)
     n.trace_on = (k == 1);
-    s = enqueue_step_body(t, rows, G_STEP, true, false);
+    s = enqueue_step_body(t, in, rows, G_STEP);
   }
   n.trace_on = true;
-  n.desc = d0; n.scal = s0;
   cudaError_t e = cudaStreamEndCapture(n.stream, &g);
   if (s != SB_OK) { if (g) cudaGraphDestroy(g); return s; }
   SB_CHECK(e == cudaSuccess, SB_ERR_CUDA, "cudaStreamEndCapture failed: %s", cudaGetErrorString(e));
@@ -1179,24 +1263,21 @@ int sb_trainer_loss_resident(sb_trainer_t* t, int64_t row_offset, int32_t rows, 
            "rows [%lld, %lld) outside the resident set of %lld rows", (long long)row_offset, (long long)(row_offset + rows),
            (long long)t->ds_rows);
   SB_CUDA(cudaSetDevice(n.device));
-  n.desc = t->descs[0];
-  n.scal = t->scals[0];
   t->have_pos = false;
   const bool resident = t->dsXb != nullptr;
+  const StepIn in{t->descs[0], t->scals[0], resident, false};      // (see forward_chunks)
   if (resident)
-    set_batch_kernel<<<1, 1, 0, n.stream>>>(n.desc, nullptr, t->dsY + row_offset, t->dsW + row_offset, 0.f, 1.f, t->epoch,
-                                             static_cast<int>(row_offset), t->dsP, rows, n.scal);
+    set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, nullptr, t->dsY + row_offset, t->dsW + row_offset, 0.f, 1.f, t->epoch,
+                                             static_cast<int>(row_offset), t->dsP, rows, in.scal);
   else
-    set_batch_kernel<<<1, 1, 0, n.stream>>>(n.desc, t->dsX + row_offset * n.F, t->dsY + row_offset, t->dsW + row_offset, 0.f, 1.f,
+    set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, t->dsX + row_offset * n.F, t->dsY + row_offset, t->dsW + row_offset, 0.f, 1.f,
                                              t->epoch);
   SB_CUDA(cudaGetLastError());
-  struct Scope { Net& n; ~Scope() { n.from_resident = false; } } scope{n};
-  n.from_resident = resident;
-  if (!resident) SB_TRY(n.enqueue_load(rows));
-  SB_TRY(n.enqueue_hidden_forward(rows));
-  SB_TRY(n.enqueue_out(rows, true, false, nullptr, nullptr));
+  if (!resident) SB_TRY(n.enqueue_load(in, rows));
+  SB_TRY(n.enqueue_hidden_forward(in, rows));
+  SB_TRY(n.enqueue_out(in, rows, true, false, nullptr, nullptr));
   float h[SCAL_COUNT];
-  SB_CUDA(cudaMemcpyAsync(h, n.scal, sizeof(h), cudaMemcpyDeviceToHost, n.stream));
+  SB_CUDA(cudaMemcpyAsync(h, in.scal, sizeof(h), cudaMemcpyDeviceToHost, n.stream));
   SB_CUDA(cudaStreamSynchronize(n.stream));
   *loss_out = h[SCAL_NNZ] > 0.f ? h[SCAL_LOSS_SUM] / h[SCAL_NNZ] : 0.f;
   return SB_OK;
@@ -1258,19 +1339,19 @@ void* sb_trainer_stream(sb_trainer_t* t) { return t ? reinterpret_cast<void*>(t-
 int sb_trainer_kernels_per_step(sb_trainer_t* t, int32_t rows) {
   SB_CHECK(t, SB_ERR_INVALID, "null trainer");
   cudaGraphExec_t ge;
-  Net& n = t->net;
-  BatchDesc* d0 = n.desc; float* s0 = n.scal;
-  n.desc = t->descs[0]; n.scal = t->scals[0];      // the graph bakes the pair's pointers
-  const int s = get_graph(t, rows, G_STEP, t->dsXb != nullptr, 0, &ge);
-  n.desc = d0; n.scal = s0;
-  SB_TRY(s);
+  const StepIn in{t->descs[0], t->scals[0], t->dsXb != nullptr, false};
+  SB_TRY(get_graph(t, in, rows, G_STEP, 0, &ge));
   return t->kernels_per_step[rows];
 }
 
 // forward (+ optional loss) over any number of host rows, in max_batch chunks
+// (a trainer's pair 0: these host-driven paths are not captured.  A step queues its descriptor writes ahead of its graph
+// on the main stream, and every forward path synchronises that stream before it returns, so no step's descriptor prefetch
+// overlaps them.)
 static int forward_chunks(Net& n, const float* X, const float* y, const float* w, int64_t rows, bool do_loss,
                           float* out, double* loss_sum, double* nnz) {
   SB_CUDA(cudaSetDevice(n.device));
+  const StepIn in{n.desc, n.scal};
   float h[SCAL_COUNT];
   for (int64_t r0 = 0; r0 < rows; r0 += n.max_batch) {
     const int c = static_cast<int>(rows - r0 < n.max_batch ? rows - r0 : n.max_batch);
@@ -1279,12 +1360,12 @@ static int forward_chunks(Net& n, const float* X, const float* y, const float* w
       SB_CUDA(cudaMemcpyAsync(n.stY, y + r0, sizeof(float) * c, cudaMemcpyDefault, n.stream));
       if (w) SB_CUDA(cudaMemcpyAsync(n.stW, w + r0, sizeof(float) * c, cudaMemcpyDefault, n.stream));
     }
-    set_batch_kernel<<<1, 1, 0, n.stream>>>(n.desc, n.stX, n.stY, (do_loss && w) ? n.stW : n.ones, 0.f, 1.f);
-    SB_TRY(n.enqueue_load(c));
-    SB_TRY(n.enqueue_hidden_forward(c));
-    SB_TRY(n.enqueue_out(c, do_loss, false, n.yhat, nullptr));
+    set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, n.stX, n.stY, (do_loss && w) ? n.stW : n.ones, 0.f, 1.f);
+    SB_TRY(n.enqueue_load(in, c));
+    SB_TRY(n.enqueue_hidden_forward(in, c));
+    SB_TRY(n.enqueue_out(in, c, do_loss, false, n.yhat, nullptr));
     if (out) SB_CUDA(cudaMemcpyAsync(out + r0, n.yhat, sizeof(float) * c, cudaMemcpyDefault, n.stream));
-    if (do_loss) SB_CUDA(cudaMemcpyAsync(h, n.scal, sizeof(h), cudaMemcpyDeviceToHost, n.stream));
+    if (do_loss) SB_CUDA(cudaMemcpyAsync(h, in.scal, sizeof(h), cudaMemcpyDeviceToHost, n.stream));
     SB_CUDA(cudaStreamSynchronize(n.stream));
     if (do_loss) { *loss_sum += h[SCAL_LOSS_SUM]; *nnz += h[SCAL_NNZ]; }
   }
@@ -1469,12 +1550,13 @@ int sb_model_score_device(sb_model_t* m, const float* dX, int64_t rows, float* d
   std::lock_guard<std::mutex> lk(m->mu);
   Net& n = m->net;
   SB_CUDA(cudaSetDevice(n.device));
+  const StepIn in{n.desc, n.scal};
   for (int64_t r0 = 0; r0 < rows; r0 += n.max_batch) {
     const int c = static_cast<int>(rows - r0 < n.max_batch ? rows - r0 : n.max_batch);
-    set_batch_kernel<<<1, 1, 0, n.stream>>>(n.desc, dX + r0 * n.F, nullptr, n.ones, 0.f, 1.f);
-    SB_TRY(n.enqueue_load(c));
-    SB_TRY(n.enqueue_hidden_forward(c));
-    SB_TRY(n.enqueue_out(c, false, false, dOut + r0, nullptr));
+    set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, dX + r0 * n.F, nullptr, n.ones, 0.f, 1.f);
+    SB_TRY(n.enqueue_load(in, c));
+    SB_TRY(n.enqueue_hidden_forward(in, c));
+    SB_TRY(n.enqueue_out(in, c, false, false, dOut + r0, nullptr));
   }
   return SB_OK;
 }

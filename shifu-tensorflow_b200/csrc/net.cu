@@ -97,8 +97,6 @@ GemmPlan plan_gemm(int M, int N, int K, int num_sms, bool allow_split) {
   return pl;
 }
 
-static inline int pairs_of(int np) { return np == 3 ? 6 : (np == 2 ? 3 : 1); }
-
 int validate_desc(const sb_net_desc* d) {
   SB_CHECK(d != nullptr, SB_ERR_INVALID, "net desc is null");
   SB_CHECK(d->n_features > 0, SB_ERR_INVALID, "n_features must be > 0 (got %d)", d->n_features);
@@ -136,19 +134,11 @@ int Net::init(const sb_net_desc* d, int device_, bool training_) {
   training = training_;
   const bool want_trace = getenv("SB_STEP_TRACE") != nullptr;
   SB_CUDA(cudaSetDevice(device));
-  // the main chain is the critical path: its CTAs are scheduled ahead of the side stream's (dW GEMMs, second optimizer)
+  // the main chain is the critical path: its CTAs are scheduled ahead of the trainer's side stream's (dW GEMMs, second
+  // optimizer)
   int prio_least = 0, prio_greatest = 0;
   SB_CUDA(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));
   SB_CUDA(cudaStreamCreateWithPriority(&stream, cudaStreamNonBlocking, prio_greatest));
-  if (training_) {
-    SB_CUDA(cudaStreamCreateWithPriority(&side, cudaStreamNonBlocking, prio_least));
-    ev_dz.resize(d->n_hidden);
-    for (auto& e : ev_dz) SB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    SB_CUDA(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
-    SB_CUDA(cudaEventCreateWithFlags(&ev_da_done, cudaEventDisableTiming));
-    SB_CUDA(cudaStreamCreateWithFlags(&comm, cudaStreamNonBlocking));
-    SB_CUDA(cudaStreamCreateWithFlags(&comm2, cudaStreamNonBlocking));
-  }
   F = d->n_features;
   L = d->n_hidden;
   precision = d->precision;
@@ -280,18 +270,6 @@ void Net::destroy() {
   if (stream) cudaStreamSynchronize(stream);
   for (void* p : allocs) cudaFree(p);
   allocs.clear();
-  for (cudaEvent_t e : ev_dz) cudaEventDestroy(e);
-  ev_dz.clear();
-  if (ev_join) cudaEventDestroy(ev_join);
-  ev_join = nullptr;
-  if (ev_da_done) cudaEventDestroy(ev_da_done);
-  ev_da_done = nullptr;
-  if (comm) cudaStreamDestroy(comm);
-  comm = nullptr;
-  if (comm2) cudaStreamDestroy(comm2);
-  comm2 = nullptr;
-  if (side) cudaStreamDestroy(side);
-  side = nullptr;
   if (stream) cudaStreamDestroy(stream);
   stream = nullptr;
 }
@@ -338,9 +316,9 @@ int Net::refresh_shadows() {
   return SB_OK;
 }
 
-int Net::enqueue_load(int rows, float* zero_buf, long long zero_n) {
-  const int Fx = sparse_step ? n_dense : F;        // a sparse step stages only the dense block
-  const int ldx = sparse_step ? ldD : ldF;
+int Net::enqueue_load(const StepIn& in, int rows, float* clear, long long clear_n) {
+  const int Fx = in.sparse ? n_dense : F;        // a sparse step stages only the dense block
+  const int ldx = in.sparse ? ldD : ldF;
   const long long units = static_cast<long long>(rows) * (ldx / 8);
   long long blocks = (units + 255) / 256;
   const long long cap = static_cast<long long>(num_sms) * 16;
@@ -349,28 +327,28 @@ int Net::enqueue_load(int rows, float* zero_buf, long long zero_n) {
   // first kernel of the step: its stream predecessor is set_batch_kernel (a kernel), so PDL applies here too
   if (tc())
     SB_TRY(launch_kernel(load_batch_kernel<true>, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, stream, true,
-                         static_cast<const BatchDesc*>(desc), rows, Fx, Xb, ldx, static_cast<float*>(nullptr), scal, zero_buf,
-                         zero_n, nparts, Xb_ps));
+                         static_cast<const BatchDesc*>(in.desc), rows, Fx, Xb, ldx, static_cast<float*>(nullptr), in.scal, clear,
+                         clear_n, nparts, Xb_ps));
   else
     SB_TRY(launch_kernel(load_batch_kernel<false>, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, stream, true,
-                         static_cast<const BatchDesc*>(desc), rows, Fx, static_cast<__nv_bfloat16*>(nullptr), ldx, Xf, scal,
-                         zero_buf, zero_n, 1, 0ll));
+                         static_cast<const BatchDesc*>(in.desc), rows, Fx, static_cast<__nv_bfloat16*>(nullptr), ldx, Xf, in.scal,
+                         clear, clear_n, 1, 0ll));
   mark("load_batch");
-  if (sparse_step) SB_TRY(enqueue_embed(rows, false, nullptr, stream));
+  if (in.sparse) SB_TRY(enqueue_embed(rows, false, nullptr, stream));
   return SB_OK;
 }
 
-int Net::enqueue_hidden_forward(int rows, float* grad, bool* fused_out) {
+int Net::enqueue_hidden_forward(const StepIn& in, int rows, float* grad, bool* fused_out, float4* clear, long long clear_n4) {
   if (fused_out) *fused_out = false;
   for (int l = 0; l < L; ++l) {
     Layer& ly = layers[l];
-    const bool sp0 = (l == 0) && sparse_step;       // wide+deep: contract the dense columns only, add the embedding sums
+    const bool sp0 = (l == 0) && in.sparse;       // wide+deep: contract the dense columns only, add the embedding sums
     const int k_in = sp0 ? n_dense : ly.in;
     const int ld_k = sp0 ? ldD : ly.ld_in;
     if (tc()) {
       // Z = A_{l-1}[rows,in] (K-major) x W_l[in,out] (MN-major B operand: n contiguous)
       TmapSet tm;
-      const bool res0 = (l == 0) && from_resident;
+      const bool res0 = (l == 0) && in.resident;
       const __nv_bfloat16* src = (l == 0) ? (res0 ? resident_Xb : Xb) : A[l - 1];
       const long long src_ps = (l == 0) ? (res0 ? resident_ps : Xb_ps) : A_ps[l - 1];
       const int src_rows = res0 ? static_cast<int>(resident_rows) : rows;
@@ -381,7 +359,7 @@ int Net::enqueue_hidden_forward(int rows, float* grad, bool* fused_out) {
       if (sp0) { p.addend = E; p.ld_add = ly.ld_out; }
       p.bias = theta + ly.b_off; p.act = ly.act;
       p.out = A[l]; p.ld_out = ly.ld_out; p.out_ps = A_ps[l];
-      p.a_rows = res0 ? desc : nullptr;
+      p.a_rows = res0 ? in.desc : nullptr;
       if (l == L - 1 && grad != nullptr && training && ly.out <= FWD_OUT_MAX_N && p.addend == nullptr) {
         // K2 + K3 + K4 + output backward in one kernel (gemm_fwd_out.cuh): 64-row tiles of whole rows of A_L
         FwdOutTmaps ft;
@@ -392,7 +370,7 @@ int Net::enqueue_hidden_forward(int rows, float* grad, bool* fused_out) {
         const int grid = tiles < num_sms ? tiles : num_sms;
         Layer& ol = layers[L];
         p.wo = theta + ol.w_off; p.bo = theta + ol.b_off;
-        p.desc = desc; p.scal = scal; p.loss = loss;
+        p.desc = in.desc; p.scal = in.scal; p.loss = loss;
         p.g_wo = grad + ol.w_off; p.g_bo = grad + ol.b_off; p.g_bL = grad + ly.b_off;
         p.trace = next_trace("fwd_out", l, rows, ly.out, k_in);
         SB_TRY(launch_gemm_fwd_out(grid, ft, p, stream, true));
@@ -400,10 +378,7 @@ int Net::enqueue_hidden_forward(int rows, float* grad, bool* fused_out) {
         mark("gemm_fwd_out");
         continue;
       }
-      if (l == 0 && zero_buf != nullptr) {
-        p.zero_buf = zero_buf; p.zero_n4 = zero_n4;
-        zero_buf = nullptr;
-      }
+      if (l == 0) { p.zero_buf = clear; p.zero_n4 = clear_n4; }
       p.trace = next_trace("fwd", l, rows, ly.out, k_in);
       if (nparts == 1 && p.addend == nullptr) {    // plain bf16: the ping-pong kernel
         const PpPlan pp = plan_gemm_pp(rows, ly.out, k_in, num_sms);
@@ -432,13 +407,13 @@ int Net::enqueue_hidden_forward(int rows, float* grad, bool* fused_out) {
   return SB_OK;
 }
 
-int Net::enqueue_out(int rows, bool do_loss, bool do_bwd, float* yhat_dst, float* grad) {
+int Net::enqueue_out(const StepIn& in, int rows, bool do_loss, bool do_bwd, float* yhat_dst, float* grad) {
   Layer& hl = layers[L - 1];
   Layer& ol = layers[L];
   OutLayerParams p = {};
   p.rows = rows; p.H = hl.out;
   p.wo = theta + ol.w_off; p.bo = theta + ol.b_off;
-  p.desc = desc; p.scal = scal; p.loss = loss; p.act = hl.act;
+  p.desc = in.desc; p.scal = in.scal; p.loss = loss; p.act = hl.act;
   p.do_bwd = do_bwd ? 1 : 0; p.do_loss = do_loss ? 1 : 0;
   p.yhat = yhat_dst;
   p.trace = next_trace("out_layer");
@@ -472,159 +447,90 @@ int Net::enqueue_out(int rows, bool do_loss, bool do_bwd, float* yhat_dst, float
   return SB_OK;
 }
 
-int Net::enqueue_backward(int rows, float* grad) {
-  // dW_l and dA_l both consume dZ_l and are independent of each other: the dW GEMMs go to the side stream and
-  // overlap the dA chain (they are each well under one wave at cfg1 sizes).
-  const bool fork = side != nullptr && tc();
-  // dW_1 (side stream) and dW_0 (main stream) run at the same time, one CTA per SM each.  If their natural grids do not
-  // fit the machine together, dW_1's second wave only starts when dW_0's CTAs exit.  Compare, in k-blocks per CTA, "natural grids, dW_1
-  // finishing after dW_0" against "dW_1 on a third of the SMs, dW_0 on the rest" and take the shorter.
-  int dw_sms[2] = {num_sms, num_sms};
-  // dw1_serial_auto (single-GPU tail): when the natural grids of dW_0 and dW_1 do not fit the machine together, dW_1 runs IN
-  // FRONT of dW_0 on the main stream instead of beside it - side by side the two persistent grids take turns on the SMs;
-  // small layers (cfg1) stay side by side.  Only when dW_0 alone fills every SM: on one H100, cfg2 (dW_0 = 128 tiles on 132
-  // SMs, budget split below) measured within 1 % of both dW_1 in front and the natural grids, while moving dW_1 in front
-  // once dW_0 fills >= 90 % of the SMs made cfg1 4 % slower
-  bool dw1_front = dw1_first;
-  if (fork && L > 1 && !dw1_last && !dw1_first) {
-    const int kx = round_up(rows, 64) * pairs_of(nparts);
-    const GemmPlan n0 = plan_gemm(layers[0].in, layers[0].out, kx, num_sms, true);
-    const GemmPlan n1 = plan_gemm(layers[1].in, layers[1].out, kx, num_sms, true);
-    if (n0.grid + n1.grid > num_sms && dw1_serial_auto && n0.grid == num_sms) {      // (dW_0 alone fills the machine)
-      dw1_front = true;
-    } else if (n0.grid + n1.grid > num_sms) {
-      const GemmPlan b1 = plan_gemm(layers[1].in, layers[1].out, kx, num_sms / 3, true);
-      const GemmPlan b0 = plan_gemm(layers[0].in, layers[0].out, kx, num_sms - b1.grid, true);
-      auto waves = [&](const GemmPlan& pl, int M, int N, int sms) {   // k-blocks one CTA works through
-        const int tiles = ((M + 127) / 128) * ((N + pl.bn - 1) / pl.bn) * pl.split_k;
-        return ((tiles + sms - 1) / sms) * pl.kb_per_split;
-      };
-      const int t_nat = waves(n0, layers[0].in, layers[0].out, num_sms) + waves(n1, layers[1].in, layers[1].out, num_sms);
-      const int t0 = waves(b0, layers[0].in, layers[0].out, num_sms - b1.grid);
-      const int t1 = waves(b1, layers[1].in, layers[1].out, num_sms / 3);
-      if ((t0 > t1 ? t0 : t1) < t_nat) { dw_sms[1] = num_sms / 3; dw_sms[0] = num_sms - b1.grid; }
-    }
+int Net::enqueue_dw(const StepIn& in, int l, int rows, float* grad, cudaStream_t st, bool pdl, int sms, int r0, int r1, int chunk) {
+  Layer& ly = layers[l];
+  const bool sp0 = (l == 0) && in.sparse;         // wide+deep: dW of the dense rows by GEMM, of the embedding rows by scatter-add
+  const int in_rows = sp0 ? n_dense : ly.in;
+  if (r1 < 0) r1 = in_rows;
+  if (sp0) SB_TRY(enqueue_embed(rows, true, grad, st));
+  if (!tc()) {
+    GemmF32Params p = {};
+    p.M = in_rows; p.N = ly.out; p.K = rows;
+    p.A = (l == 0) ? Xf : Af[l - 1]; p.sAm = 1; p.sAk = in_rows;
+    p.B = dZf[l]; p.sBk = ly.out; p.sBn = 1;
+    p.accum = grad + ly.w_off; p.ld_acc = ly.out;
+    const int tiles = ((p.M + 63) / 64) * ((p.N + 63) / 64);
+    int split = (2 * num_sms) / (tiles > 0 ? tiles : 1);
+    const int cap = (rows + 63) / 64;
+    if (split > cap) split = cap;
+    SB_TRY(launch_gemm_f32<EPI_DW>(p, split, st));
+    mark("gemm_dw");
+    return SB_OK;
   }
-  auto emit_dw_tc = [&](int l, bool force_main) -> int {
-        Layer& ly = layers[l];
-        const bool xchg_chunks = l == 0 && dw0_chunks >= 1 && on_dw0_chunk && (ly.out % 8 == 0 || dw0_chunks == 1) && !sparse_step;
-        const int n_chunks = xchg_chunks ? dw0_chunks : 1;
-        int chunk_rows = xchg_chunks ? dw0_chunk_rows() : round_up(ly.in, 128);
-        // dW_0 has nothing to overlap with (no dA_0): PDL-chained on the main stream right behind the last dA GEMM it
-        // starts earlier than as a cross-stream launch
-        const bool on_main = !fork || (l == 0 && L > 1) || force_main;
-        if (!on_main) {
-          SB_CUDA(cudaEventRecord(ev_dz[l], stream));
-          SB_CUDA(cudaStreamWaitEvent(side, ev_dz[l], 0));
-        }
-        const bool res0 = (l == 0) && from_resident;
-        const bool sp0 = (l == 0) && sparse_step;     // wide+deep: dW of the dense rows by GEMM, of the embedding rows by scatter-add
-        const int in_rows = sp0 ? n_dense : ly.in;
-        const int ld_k = sp0 ? ldD : ly.ld_in;
-        if (sp0) chunk_rows = round_up(in_rows, 128);
-        const __nv_bfloat16* ap = (l == 0) ? (res0 ? resident_Xb : Xb) : A[l - 1];
-        const long long ap_ps = (l == 0) ? (res0 ? resident_ps : Xb_ps) : A_ps[l - 1];
-        if (sp0) SB_TRY(enqueue_embed(rows, true, grad, on_main ? stream : side));
-        for (int r0 = 0; r0 < in_rows; r0 += chunk_rows) {
-          const int r1 = (r0 + chunk_rows < in_rows) ? r0 + chunk_rows : in_rows;
-          const GemmPlan pl = plan_gemm(r1 - r0, ly.out, round_up(rows, 64) * pairs_of(nparts), l < 2 ? dw_sms[l] : num_sms, true);
-          TmapSet tm;
-          // resident set: rows past the batch end are real rows of other batches; the B operand (dZ_l, extent = rows) is
-          // zero-filled there, so they contribute nothing
-          SB_TRY(make_tmaps_bf16(tm.a, ap + r0, ap_ps, nparts, res0 ? static_cast<int>(resident_rows) : rows, r1 - r0, ld_k, 64));
-          SB_TRY(make_tmaps_bf16(tm.b, dZ[l], A_ps[l], nparts, rows, ly.out, ly.ld_out, 64));
-          GemmTcParams p = {};
-          set_part_pairs(&p, nparts);
-          p.M = r1 - r0; p.N = ly.out; p.K = rows;
-          p.a_rows = res0 ? desc : nullptr;
-          p.accum = grad + ly.w_off + static_cast<long long>(r0) * ly.out; p.ld_acc = ly.out;
-          p.acc_vec4 = (ly.out % 4 == 0 && ly.w_off % 4 == 0) ? 1 : 0;
-          p.trace = next_trace("dW", l, r1 - r0, ly.out, rows, n_chunks > 1 ? r0 / chunk_rows : -1);
-          SB_TRY((launch_gemm_tc<EPI_DW, true, true>(pl, tm, p, on_main ? stream : side, on_main)));
-          mark("gemm_dw");
-          if (xchg_chunks) SB_TRY(on_dw0_chunk(r0 / chunk_rows));
-        }
-        return SB_OK;
-  };
-  for (int l = L - 1; l >= 0; --l) {
-    Layer& ly = layers[l];
-    if (tc()) {
-      // dW_l[in,out] += sum_rows A_{l-1}[rows,in] (MN-major A) * dZ_l[rows,out] (MN-major B), split-K over rows.
-      // With the peer exchange behind it, dW_0 is cut into row chunks of W_0 (each a contiguous slice of the flat
-      // gradient) so that the exchange of chunk c overlaps the GEMM of chunk c+1.
-      const bool dw1_moved = (dw1_last || dw1_front) && L > 1;
-      if (dw1_front && l == 0 && L > 1) {         // in front of dW_0 on the main stream: dW_0's last exchange then runs on an idle GPU
-        SB_TRY(emit_dw_tc(1, true));
-        if (after_dw1) SB_TRY(after_dw1());
-      }
-      if (!(dw1_moved && l == 1)) SB_TRY(emit_dw_tc(l, false));
-      if (dw1_last && !dw1_front && l == 0 && L > 1) SB_TRY(emit_dw_tc(1, true));   // behind dW_0 on the main stream (covers its last exchange)
-      if (l > 0) {
-        // dZ_{l-1}[rows,in] = (dZ_l[rows,out] (K-major) x W_l[in,out] (K-major B: k = out contiguous)) .* act'(A_{l-1})
-        Layer& pl = layers[l - 1];
-        GemmTcParams p = {};
-        set_part_pairs(&p, nparts);
-        p.M = rows; p.N = ly.in; p.K = ly.out;
-        p.act = pl.act;
-        p.aux = A[l - 1]; p.ld_aux = pl.ld_out; p.aux_ps = A_ps[l - 1];
-        p.out = dZ[l - 1]; p.ld_out = pl.ld_out; p.out_ps = A_ps[l - 1];
-        p.colsum = grad + pl.b_off;
-        p.trace = next_trace("dA", l, rows, ly.in, ly.out);
-        if (nparts == 1) {                           // plain bf16: the ping-pong kernel
-          const PpPlan pp = plan_gemm_pp(rows, ly.in, ly.out, num_sms);
-          PpTmaps pt;
-          SB_TRY(make_tmap_bf16(&pt.a, dZ[l], rows, ly.out, ly.ld_out, pp.bm_wg));
-          SB_TRY(make_tmap_bf16(&pt.b, ly.Wn, ly.in, ly.out, ly.ld_out, pp.bn));
-          SB_TRY(make_tmap_bf16(&pt.o, dZ[l - 1], rows, ly.in, pl.ld_out, pp.bm_wg));
-          SB_TRY(make_tmap_bf16(&pt.x, A[l - 1], rows, ly.in, pl.ld_out, pp.bm_wg));
-          SB_TRY(launch_gemm_pp<EPI_DA>(pp, pt, p, stream, true));
-        } else {
-          const GemmPlan gp = plan_gemm(rows, ly.in, round_up(ly.out, 64) * pairs_of(nparts), num_sms, false);
-          TmapSet tm;
-          SB_TRY(make_tmaps_bf16(tm.a, dZ[l], A_ps[l], nparts, rows, ly.out, ly.ld_out, 128));
-          SB_TRY(make_tmaps_bf16(tm.b, ly.Wn, Wn_ps[l], nparts, ly.in, ly.out, ly.ld_out, gp.bn));
-          SB_TRY((launch_gemm_tc<EPI_DA, false, false>(gp, tm, p, stream, true)));
-        }
-        mark("gemm_da");
-        if (l == 1 && fork && defer_join) SB_CUDA(cudaEventRecord(ev_da_done, stream));
-      }
-    } else {
-      {
-        const bool sp0 = (l == 0) && sparse_step;
-        const int in_rows = sp0 ? n_dense : ly.in;
-        if (sp0) SB_TRY(enqueue_embed(rows, true, grad, stream));
-        GemmF32Params p = {};
-        p.M = in_rows; p.N = ly.out; p.K = rows;
-        p.A = (l == 0) ? Xf : Af[l - 1]; p.sAm = 1; p.sAk = in_rows;
-        p.B = dZf[l]; p.sBk = ly.out; p.sBn = 1;
-        p.accum = grad + ly.w_off; p.ld_acc = ly.out;
-        const int tiles = ((p.M + 63) / 64) * ((p.N + 63) / 64);
-        int split = (2 * num_sms) / (tiles > 0 ? tiles : 1);
-        const int cap = (rows + 63) / 64;
-        if (split > cap) split = cap;
-        SB_TRY(launch_gemm_f32<EPI_DW>(p, split, stream));
-        mark("gemm_dw");
-      }
-      if (l > 0) {
-        Layer& pl = layers[l - 1];
-        GemmF32Params p = {};
-        p.M = rows; p.N = ly.in; p.K = ly.out;
-        p.A = dZf[l]; p.sAm = ly.out; p.sAk = 1;
-        p.B = theta + ly.w_off; p.sBk = 1; p.sBn = ly.out;
-        p.act = pl.act;
-        p.aux = Af[l - 1]; p.ld_aux = pl.out;
-        p.out = dZf[l - 1]; p.ld_out = pl.out;
-        p.colsum = grad + pl.b_off;
-        SB_TRY(launch_gemm_f32<EPI_DA>(p, 1, stream));
-        mark("gemm_da");
-      }
-    }
-  }
-  if (fork && !defer_join) {
-    SB_CUDA(cudaEventRecord(ev_join, side));
-    SB_CUDA(cudaStreamWaitEvent(stream, ev_join, 0));
-  }
+  // dW_l[in,out] += sum_rows A_{l-1}[rows,in] (MN-major A) * dZ_l[rows,out] (MN-major B), split-K over rows
+  const bool res0 = (l == 0) && in.resident;
+  const int ld_k = sp0 ? ldD : ly.ld_in;
+  const __nv_bfloat16* ap = (l == 0) ? (res0 ? resident_Xb : Xb) : A[l - 1];
+  const long long ap_ps = (l == 0) ? (res0 ? resident_ps : Xb_ps) : A_ps[l - 1];
+  const GemmPlan pl = plan_gemm(r1 - r0, ly.out, round_up(rows, 64) * pairs_of(nparts), sms, true);
+  TmapSet tm;
+  // resident set: rows past the batch end are real rows of other batches; the B operand (dZ_l, extent = rows) is
+  // zero-filled there, so they contribute nothing
+  SB_TRY(make_tmaps_bf16(tm.a, ap + r0, ap_ps, nparts, res0 ? static_cast<int>(resident_rows) : rows, r1 - r0, ld_k, 64));
+  SB_TRY(make_tmaps_bf16(tm.b, dZ[l], A_ps[l], nparts, rows, ly.out, ly.ld_out, 64));
+  GemmTcParams p = {};
+  set_part_pairs(&p, nparts);
+  p.M = r1 - r0; p.N = ly.out; p.K = rows;
+  p.a_rows = res0 ? in.desc : nullptr;
+  p.accum = grad + ly.w_off + static_cast<long long>(r0) * ly.out; p.ld_acc = ly.out;
+  p.acc_vec4 = (ly.out % 4 == 0 && ly.w_off % 4 == 0) ? 1 : 0;
+  p.trace = next_trace("dW", l, r1 - r0, ly.out, rows, chunk);
+  SB_TRY((launch_gemm_tc<EPI_DW, true, true>(pl, tm, p, st, pdl)));
+  mark("gemm_dw");
   return SB_OK;
 }
 
+int Net::enqueue_da(int l, int rows, float* grad) {
+  Layer& ly = layers[l];
+  Layer& pl = layers[l - 1];
+  if (!tc()) {
+    GemmF32Params p = {};
+    p.M = rows; p.N = ly.in; p.K = ly.out;
+    p.A = dZf[l]; p.sAm = ly.out; p.sAk = 1;
+    p.B = theta + ly.w_off; p.sBk = 1; p.sBn = ly.out;
+    p.act = pl.act;
+    p.aux = Af[l - 1]; p.ld_aux = pl.out;
+    p.out = dZf[l - 1]; p.ld_out = pl.out;
+    p.colsum = grad + pl.b_off;
+    SB_TRY(launch_gemm_f32<EPI_DA>(p, 1, stream));
+    mark("gemm_da");
+    return SB_OK;
+  }
+  // dZ_{l-1}[rows,in] = (dZ_l[rows,out] (K-major) x W_l[in,out] (K-major B: k = out contiguous)) .* act'(A_{l-1})
+  GemmTcParams p = {};
+  set_part_pairs(&p, nparts);
+  p.M = rows; p.N = ly.in; p.K = ly.out;
+  p.act = pl.act;
+  p.aux = A[l - 1]; p.ld_aux = pl.ld_out; p.aux_ps = A_ps[l - 1];
+  p.out = dZ[l - 1]; p.ld_out = pl.ld_out; p.out_ps = A_ps[l - 1];
+  p.colsum = grad + pl.b_off;
+  p.trace = next_trace("dA", l, rows, ly.in, ly.out);
+  if (nparts == 1) {                           // plain bf16: the ping-pong kernel
+    const PpPlan pp = plan_gemm_pp(rows, ly.in, ly.out, num_sms);
+    PpTmaps pt;
+    SB_TRY(make_tmap_bf16(&pt.a, dZ[l], rows, ly.out, ly.ld_out, pp.bm_wg));
+    SB_TRY(make_tmap_bf16(&pt.b, ly.Wn, ly.in, ly.out, ly.ld_out, pp.bn));
+    SB_TRY(make_tmap_bf16(&pt.o, dZ[l - 1], rows, ly.in, pl.ld_out, pp.bm_wg));
+    SB_TRY(make_tmap_bf16(&pt.x, A[l - 1], rows, ly.in, pl.ld_out, pp.bm_wg));
+    SB_TRY(launch_gemm_pp<EPI_DA>(pp, pt, p, stream, true));
+  } else {
+    const GemmPlan gp = plan_gemm(rows, ly.in, round_up(ly.out, 64) * pairs_of(nparts), num_sms, false);
+    TmapSet tm;
+    SB_TRY(make_tmaps_bf16(tm.a, dZ[l], A_ps[l], nparts, rows, ly.out, ly.ld_out, 128));
+    SB_TRY(make_tmaps_bf16(tm.b, ly.Wn, Wn_ps[l], nparts, ly.in, ly.out, ly.ld_out, gp.bn));
+    SB_TRY((launch_gemm_tc<EPI_DA, false, false>(gp, tm, p, stream, true)));
+  }
+  mark("gemm_da");
+  return SB_OK;
+}
 }  // namespace sb

@@ -4,7 +4,6 @@
 #include <vector>
 #include <map>
 #include <mutex>
-#include <functional>
 #include "common.cuh"
 #include "gemm_tc.cuh"
 #include "gemm_f32.cuh"
@@ -20,36 +19,20 @@ struct Layer {
   int ld_in = 0, ld_out = 0;
 };
 
+// What one step's launches read: its descriptor / scalar pair, whether layer 0 reads the HBM-resident set, whether the
+// step is a sparse (wide+deep) one.  The trainer alternates descriptor pairs between captured steps.
+struct StepIn {
+  BatchDesc* desc = nullptr;
+  float* scal = nullptr;
+  bool resident = false;   // layer 0's GEMMs read their A operand by TMA from resident_Xb at row offset desc->row0
+  bool sparse = false;     // wide+deep step: dense block + index matrix, hidden layer 0's one-hot block via the embedding
+};
+
+inline int pairs_of(int np) { return np == 3 ? 6 : (np == 2 ? 3 : 1); }
+
 struct Net {
   int device = 0, num_sms = 132;
   cudaStream_t stream = nullptr;
-  cudaStream_t side = nullptr;               // dW GEMMs run here, concurrently with the dA chain on `stream`
-  std::vector<cudaEvent_t> ev_dz;            // ev_dz[l]: dZ_l is complete on `stream`
-  cudaEvent_t ev_join = nullptr;
-  cudaStream_t comm = nullptr;               // the exchange launches behind dW_0's row chunks alternate between comm and comm2
-  cudaStream_t comm2 = nullptr;
-  // Peer-exchange schedule (world > 1, set by the trainer around enqueue_backward): dW_0 runs on the main stream in
-  // `dw0_chunks` row chunks of W_0 and on_dw0_chunk(c) is called behind each (its exchange goes to a comm stream and
-  // overlaps the GEMMs that follow).  dW_1 moves from the side stream to the main stream: in front of dW_0 (dw1_first,
-  // after_dw1 is called behind it), or behind dW_0 as cover for the last chunk's exchange (dw1_last, replicas that share
-  // a device).
-  int dw0_chunks = 1;
-  bool dw1_last = false;
-  bool dw1_first = false;
-  std::function<int()> after_dw1;
-  bool dw1_serial_auto = false;              // let enqueue_backward move dW_1 in front of dW_0 when their grids do not fit together
-  std::function<int(int /*chunk*/)> on_dw0_chunk;
-  int dw0_chunk_rows() const {
-    const int c = dw0_chunks > 1 ? dw0_chunks : 1;
-    return ((layers[0].in + c - 1) / c + 127) / 128 * 128;
-  }
-  // resident steps: the layer-0 forward GEMM's epilogue warps clear this buffer (the step's gradient) while they wait for
-  // their first accumulator; consumed (and reset) by enqueue_hidden_forward
-  float4* zero_buf = nullptr;
-  long long zero_n4 = 0;
-  // single-GPU step tail: the caller enqueues the optimizer per stream instead of joining first
-  bool defer_join = false;
-  cudaEvent_t ev_da_done = nullptr;          // the last dA GEMM (last reader of the bf16 weight shadows) is complete
   std::vector<int> work_begin, work_end;     // optimizer work-table range of layer l (0..L)
   int F = 0, L = 0;             // features, hidden layers
   std::vector<Layer> layers;    // L hidden + 1 output (out = 1)
@@ -79,8 +62,9 @@ struct Net {
   // fp32 workspace
   float* Xf = nullptr;
   std::vector<float*> Af, dZf;
-  float *yhat = nullptr, *scal = nullptr, *ones = nullptr;
-  BatchDesc* desc = nullptr;
+  float *yhat = nullptr, *ones = nullptr;
+  BatchDesc* desc = nullptr;               // the net's own descriptor / scalar pair (the trainer's pair 0)
+  float* scal = nullptr;
   float *stX = nullptr, *stY = nullptr, *stW = nullptr;  // H2D staging (device)
   OptWork* work = nullptr;
   int n_work = 0;
@@ -118,27 +102,32 @@ struct Net {
   int init(const sb_net_desc* d, int device_, bool training_);
   void destroy();
   int refresh_shadows();
-  // forward through the hidden layers (A_0 = current batch -> A_L)
-  int enqueue_load(int rows, float* zero_buf = nullptr, long long zero_n = 0);
+  // forward through the hidden layers (A_0 = current batch -> A_L).  The load kernel clears clear[0, clear_n) on the way.
+  int enqueue_load(const StepIn& in, int rows, float* clear = nullptr, long long clear_n = 0);
   // grad != nullptr (training step): the last hidden layer's GEMM also runs the output layer, the loss and the output
-  // backward in its epilogue when h_L <= 128; *fused_out tells the caller whether enqueue_out is still needed
-  int enqueue_hidden_forward(int rows, float* grad = nullptr, bool* fused_out = nullptr);
+  // backward in its epilogue when h_L <= 128; *fused_out tells the caller whether enqueue_out is still needed.  clear
+  // (resident steps): the layer-0 GEMM's idle producer warps clear clear[0, clear_n4) beside its main loop.
+  int enqueue_hidden_forward(const StepIn& in, int rows, float* grad = nullptr, bool* fused_out = nullptr, float4* clear = nullptr,
+                             long long clear_n4 = 0);
   // wide+deep first layer (oracle/wide_deep.py): hidden layer 0 = [n_dense numeric columns | n_onehot one-hot columns of
   // n_cat categorical columns]; a SPARSE step feeds (dense block, index matrix) and evaluates the one-hot block as an
   // embedding gather / scatter-add.  F = n_dense + n_onehot, the parameters are those of the dense net.
   int n_dense = 0, n_onehot = 0, n_cat = 0, ldD = 0;
   int* idx = nullptr;                        // [max_batch, n_cat] staged indices
   float* E = nullptr;                        // [max_batch, ld_out_0] embedding sums
-  bool sparse_step = false;                  // set while a sparse step is being enqueued
   int set_sparse(int n_dense_, int n_onehot_, int n_cat_);
   int enqueue_embed(int rows, bool scatter, float* grad, cudaStream_t st);
-  // bf16 HBM-resident training set (trainer): when `from_resident` is set while enqueueing, layer 0's GEMMs read their A
-  // operand from it by TMA at row offset desc->row0 and no load_batch kernel runs
+  // bf16 HBM-resident training set (trainer), read by steps with StepIn::resident
   const __nv_bfloat16* resident_Xb = nullptr;
   long long resident_rows = 0;
-  bool from_resident = false;
-  int enqueue_out(int rows, bool do_loss, bool do_bwd, float* yhat_dst, float* grad);
-  int enqueue_backward(int rows, float* grad);
+  int enqueue_out(const StepIn& in, int rows, bool do_loss, bool do_bwd, float* yhat_dst, float* grad);
+  // Backward pass, one GEMM per call; the trainer's step schedule (enqueue_step_backward, capi.cu) puts them on streams.
+  // dW_l[r0, r1) rows of W_l (r1 < 0: all) += A_{l-1}^T dZ_l on `st`, its grid capped at `sms` (tensor-core modes; `pdl`:
+  // launched with programmatic dependent launch); layer 0 of a sparse step also scatter-adds the embedding rows' gradient.
+  int enqueue_dw(const StepIn& in, int l, int rows, float* grad, cudaStream_t st, bool pdl, int sms, int r0 = 0, int r1 = -1,
+                 int chunk = -1);
+  // dZ_{l-1} = (dZ_l W_l^T) .* act'(A_{l-1}) and the bias gradient of layer l-1, on the main stream
+  int enqueue_da(int l, int rows, float* grad);
 };
 
 int validate_desc(const sb_net_desc* d);

@@ -27,7 +27,7 @@
 //              shadow (biases, output layer, fp32 mode), fp32 theta.  A peer's `updated` also says it no longer reads my
 //              gradient: on exit all my operands are final and my gradient buffer is free.
 //
-//   The schedule that hides the launches behind GEMMs lives in capi.cu (enqueue_step_body).
+//   The schedule that hides the launches behind GEMMs lives in capi.cu (enqueue_step_backward).
 //
 // A rank only reads other ranks' gradients of ITS runs and only writes ITS runs of other ranks' operands; the writes
 // happen after every rank has arrived, i.e. after every rank's last reader of those operands in this step (the launch is

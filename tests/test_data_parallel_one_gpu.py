@@ -3,7 +3,7 @@
     sb_trainer_load_dataset + sb_trainer_run_resident + the peer-memory exchange kernels of csrc/xchg_p2p.cuh (bf16: the LL
     kernel - gradients pushed to their owners with the flag inside the data, optimizer on the owned runs, new operands pushed
     back; fp32 / split modes: arrive flag -> P2P loads -> update -> `updated` flag -> all-gather by P2P loads), launched per
-    slot from the multi-step graphs.  (Replicas that share a device keep the serial launch order, see enqueue_step_body; the
+    slot from the multi-step graphs.  (Replicas that share a device keep the serial launch order, see enqueue_step_backward; the
     schedule bench.py times runs on two real GPUs in tests/test_multi_gpu.py::test_two_gpu_resident_run_matches_oracle.)
 
 W replicas (ranks) live in this process on the SAME device, each with its own streams and its own parameter arena; the
