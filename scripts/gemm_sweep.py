@@ -1,6 +1,6 @@
 """Sweep tile configurations over the GEMM shapes of cfg1 / cfg2 (run on the GPU box). Prints us and TFLOP/s.
 Forward and dA GEMMs run on the ping-pong kernel with their real epilogues (relu), once per warpgroup tile height
-(bm_wg 64 / 128; "plan" marks the planner's choice); dW GEMMs over tile width and split-K."""
+(bm_wg 64 / 128; "plan" marks the planner's choice); dW GEMMs (gemm_dw.cuh) over tile width (64 / 128 / 256) and split-K."""
 import sys, os, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -38,8 +38,8 @@ for cfgname, (B, F, h) in {"cfg1": (4096, 1000, [512, 256, 128]), "cfg2": (8192,
                 print("%s %-5s M=%5d N=%5d K=%5d bm_wg=%3d  %8.2f us  %7.1f TF %s" % (cfgname, name, M, N, K, bm, ms * 1e3, tf, tag), flush=True)
                 res.append(dict(cfg=cfgname, name=name, M=M, N=N, K=K, bm_wg=bm, us=ms * 1e3, tflops=tf))
             continue
-        for cg, bn in [(1, 64), (1, 128)]:
-            if bn == 64 and N > 64: continue
+        for cg, bn in [(1, 64), (1, 128), (1, 256)]:
+            if (bn == 64 and N > 64) or (bn == 256 and N <= 128): continue
             for sk in splits:
                 try:
                     ms = sb.capi.debug_gemm_bench(M, N, K, split_k=sk, a_mn=amn, b_mn=bmn, cg=cg, bn=bn, iters=30)

@@ -7,6 +7,7 @@
 #include <memory>
 #include <random>
 #include "net.cuh"
+#include "gemm_dw.cuh"
 #include "gemm_pp.cuh"
 #include "savedmodel.h"
 #include "xchg_p2p.cuh"
@@ -258,8 +259,11 @@ static Dw1Plan plan_dw1(const sb_trainer* t, int rows, bool split_tail, bool xsc
   // single-GPU tail: dW_1 runs IN FRONT of dW_0 on the main stream instead of beside it - side by side the two persistent
   // grids take turns on the SMs; small layers (cfg1) stay side by side.  Only when dW_0 alone fills every SM: on one H100,
   // cfg2 (dW_0 = 128 tiles on 132 SMs, budget split below) measured within 1 % of both dW_1 in front and the natural
-  // grids, while moving dW_1 in front once dW_0 fills >= 90 % of the SMs made cfg1 4 % slower
-  if (split_tail && n0.grid == S) {
+  // grids, while moving dW_1 in front once dW_0 fills >= 90 % of the SMs made cfg1 4 % slower.  A dW_0 on 128 x 256 tiles
+  // (plan_gemm; cfg2) also takes dW_1 in front: beside it, dW_1's CTAs only get SMs as dW_0 ends and then hold them while
+  // layer 0's optimizer runs (one H100 SXM, 700 W: the optimizer took 32 us sharing the SMs, 13 us after dW_1 in front;
+  // cfg2 +0.9 %)
+  if (split_tail && (n0.grid == S || n0.bn == 256)) {
     d.at = DW1_FRONT;
     return d;
   }
@@ -1604,8 +1608,8 @@ int sb_debug_gemm_bench(const float* A, const float* B, float* D, int32_t M, int
 
 static int debug_gemm_impl(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K, int32_t split_k,
                            int32_t a_mn, int32_t b_mn, int32_t cfg_cg, int32_t cfg_bn, int device, int iters, float* ms_out) {
-  SB_CHECK(cfg_cg == 0 || (cfg_cg == 1 && (cfg_bn == 64 || cfg_bn == 128)), SB_ERR_INVALID,
-           "tile configuration cg=%d bn=%d not instantiated", cfg_cg, cfg_bn);
+  SB_CHECK(cfg_cg == 0 || (cfg_cg == 1 && (cfg_bn == 64 || cfg_bn == 128 || (cfg_bn == 256 && a_mn && b_mn))), SB_ERR_INVALID,
+           "tile configuration cg=%d bn=%d not instantiated for this layout (bn=256: MM only)", cfg_cg, cfg_bn);
   SB_CHECK(A && B && D && M > 0 && N > 0 && K > 0, SB_ERR_INVALID, "bad argument");
   SB_CHECK((a_mn == 0 && b_mn == 0) || (a_mn == 0 && b_mn == 1) || (a_mn == 1 && b_mn == 1), SB_ERR_INVALID,
            "layout combination not instantiated (use KK, KM or MM)");
@@ -1650,12 +1654,16 @@ static int debug_gemm_impl(const float* A, const float* B, float* D, int32_t M, 
     GemmTcParams p = {};
     p.M = M; p.N = N; p.K = K;
     p.accum = dD; p.ld_acc = N;
+    p.acc_vec4 = (N % 4 == 0) ? 1 : 0;
+    // 256-wide tiles (MM, the dW layout, only): the dW kernel, whose red.add into the zeroed D is the product
     auto launch = [&]() -> int {
+      if (pl.bn == 256) return launch_gemm_dw(pl, tms, p, 0);
       if (!a_mn && !b_mn) return launch_gemm_tc<EPI_F32, false, false>(pl, tms, p, 0);
       if (!a_mn) return launch_gemm_tc<EPI_F32, false, true>(pl, tms, p, 0);
       return launch_gemm_tc<EPI_F32, true, true>(pl, tms, p, 0);
     };
-    if (!a_mn && !b_mn) s = set_gemm_tc_attrs<EPI_F32, false, false>();
+    if (pl.bn == 256) s = set_gemm_dw_attrs();
+    else if (!a_mn && !b_mn) s = set_gemm_tc_attrs<EPI_F32, false, false>();
     else if (!a_mn) s = set_gemm_tc_attrs<EPI_F32, false, true>();
     else s = set_gemm_tc_attrs<EPI_F32, true, true>();
     if (s == SB_OK) s = launch();
@@ -1685,6 +1693,7 @@ static int debug_gemm_impl(const float* A, const float* B, float* D, int32_t M, 
       auto real = [&]() -> int {
         if (!a_mn && !b_mn) return launch_gemm_pp<EPI_DA>(pp, pt, q, 0, false);
         if (!a_mn) return launch_gemm_pp<EPI_FWD>(pp, pt, q, 0, false);
+        if (pl.bn == 256) return launch_gemm_dw(pl, tms, q, 0, false);
         return launch_gemm_tc<EPI_DW, true, true>(pl, tms, q, 0, false);
       };
       if (s == SB_OK) s = a_mn ? set_gemm_tc_attrs<EPI_DW, true, true>() : set_gemm_pp_attrs();

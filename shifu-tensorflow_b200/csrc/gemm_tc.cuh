@@ -12,7 +12,7 @@
 //   EPI_DA  : dA = dZ_l W_l^T        A K-major [rows,out], B = W_l [in,out] K-major; *act'(A_{l-1}) -> dZ_{l-1},
 //                                    column sums -> db_{l-1}
 //   EPI_DW  : dW_l = A_{l-1}^T dZ_l  A = A_{l-1} [rows,in] MN-major, B = dZ_l [rows,out] MN-major; split-K over the
-//                                    batch, fp32 red.add into the flat gradient
+//                                    batch, fp32 red.add into the flat gradient (128 x 256 tiles: gemm_dw.cuh)
 //   EPI_F32 : plain fp32 store (kernel-level parity test hook)
 // Here EPI_FWD / EPI_DA are the split-precision parts and the wide+deep addend (GENERIC); the plain-bf16 forward and dA
 // GEMMs are gemm_pp.cuh, the last hidden GEMM of a training step with the output layer fused into its epilogue is
@@ -473,7 +473,7 @@ void set_part_pairs(GemmTcParams* p, int np);
 
 // Tile configuration chosen per problem.
 struct GemmPlan {
-  int bn;            // 64 / 128
+  int bn;            // 64 / 128; 256 for dW GEMMs only (gemm_dw.cuh)
   int split_k, kb_per_split;
   int grid;          // CTAs to launch
 };

@@ -5,6 +5,7 @@
 #include <string.h>
 #include <algorithm>
 #include "net.cuh"
+#include "gemm_dw.cuh"
 #include "gemm_fwd_out.cuh"
 #include "gemm_pp.cuh"
 
@@ -70,30 +71,46 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rows, int cols, int l
 
 // Tile configuration (persistent grid, one CTA per SM, 128 x BN tiles):
 //   - BN = 128 (64 for a layer at most 64 wide).  The plain-bf16 forward and dA GEMMs are planned apart (plan_gemm_pp,
-//     gemm_pp.cuh): two warpgroups per CTA with whole tiles each, 128 or 64 rows.  A 128 x 256 tile would fetch fewer operand bytes per flop, but its
-//     128-register accumulator plus the epilogue does not fit the consumer threads' registers without spills.  The fused
-//     output layer (gemm_fwd_out.cuh) is planned apart: it needs whole rows of A_L in one CTA, so it takes 64 x h_L tiles
-//     (h_L <= 256, the two consumer warpgroups split the columns: 64 accumulator registers per thread) and
-//     ceil(rows / 64) CTAs - twice the CTAs a 128-row tile would give the narrow last layer;
-//   - split-K (dW GEMMs, reduction over the batch): fill the machine but keep >= 8 k-blocks per split.
+//     gemm_pp.cuh): two warpgroups per CTA with whole tiles each, 128 or 64 rows.  The fused output layer
+//     (gemm_fwd_out.cuh) is planned apart: it needs whole rows of A_L in one CTA, so it takes 64 x h_L tiles (h_L <= 256,
+//     the two consumer warpgroups split the columns: 64 accumulator registers per thread) and ceil(rows / 64) CTAs -
+//     twice the CTAs a 128-row tile would give the narrow last layer;
+//   - split-K (dW GEMMs, reduction over the batch; allow_split): fill the machine but keep >= 8 k-blocks per split;
+//   - dW GEMMs take 128 x 256 tiles (gemm_dw.cuh) where that costs nothing in parallelism: the same grid as the 128-wide
+//     plan, no more k-blocks x tile width per CTA, and >= 32 k-blocks per split.  The wider tile reads fewer shared-memory
+//     operand bytes per flop, but needs twice the split-K factor for the same grid - twice the red.global traffic into
+//     the gradient - and a split of few k-blocks is mostly the ring's fill and drain.
 GemmPlan plan_gemm(int M, int N, int K, int num_sms, bool allow_split) {
   const int total_kb = (K + 63) / 64;
-  const int bn = N <= 64 ? 64 : 128;
-  const int tiles = ((M + 127) / 128) * ((N + bn - 1) / bn);
-  int split = 1;
-  if (allow_split) {
-    split = num_sms / tiles;
-    const int cap = total_kb / 8;
-    if (split > cap) split = cap;
-    if (split < 1) split = 1;
+  auto tiles_of = [&](int bn) { return ((M + 127) / 128) * ((N + bn - 1) / bn); };
+  auto plan = [&](int bn) {
+    const int tiles = tiles_of(bn);
+    int split = 1;
+    if (allow_split) {
+      split = num_sms / tiles;
+      const int cap = total_kb / 8;
+      if (split > cap) split = cap;
+      if (split < 1) split = 1;
+    }
+    if (split > total_kb) split = total_kb;
+    GemmPlan pl = {};
+    pl.bn = bn;
+    pl.kb_per_split = (total_kb + split - 1) / split;
+    pl.split_k = (total_kb + pl.kb_per_split - 1) / pl.kb_per_split;
+    const int work = tiles * pl.split_k;
+    pl.grid = work < num_sms ? work : num_sms;
+    return pl;
+  };
+  // k-blocks x tile width one CTA works through (whole waves of work items)
+  auto cost = [&](const GemmPlan& pl) {
+    const long long work = static_cast<long long>(tiles_of(pl.bn)) * pl.split_k;
+    return (work + pl.grid - 1) / pl.grid * pl.kb_per_split * pl.bn;
+  };
+  const GemmPlan pl = plan(N <= 64 ? 64 : 128);
+  if (allow_split && N > 128) {
+    const GemmPlan wide = plan(256);
+    if (wide.grid == pl.grid && cost(wide) <= cost(pl) && wide.kb_per_split >= 32) return wide;
   }
-  if (split > total_kb) split = total_kb;
-  GemmPlan pl = {};
-  pl.bn = bn;
-  pl.kb_per_split = (total_kb + split - 1) / split;
-  pl.split_k = (total_kb + pl.kb_per_split - 1) / pl.kb_per_split;
-  const int work = tiles * pl.split_k;
-  pl.grid = work < num_sms ? work : num_sms;
   return pl;
 }
 
@@ -257,6 +274,7 @@ int Net::init(const sb_net_desc* d, int device_, bool training_) {
     SB_TRY(set_gemm_pp_attrs());
     SB_TRY((set_gemm_tc_attrs<EPI_DA, false, false>()));
     SB_TRY((set_gemm_tc_attrs<EPI_DW, true, true>()));
+    SB_TRY(set_gemm_dw_attrs());
     // keep the SMs in the GEMMs' shared-memory carve-out for every kernel of the step, so that no launch in the chain
     // has to re-partition L1 / shared memory
     const int co = cudaSharedmemCarveoutMaxShared;
@@ -485,7 +503,8 @@ int Net::enqueue_dw(const StepIn& in, int l, int rows, float* grad, cudaStream_t
   p.accum = grad + ly.w_off + static_cast<long long>(r0) * ly.out; p.ld_acc = ly.out;
   p.acc_vec4 = (ly.out % 4 == 0 && ly.w_off % 4 == 0) ? 1 : 0;
   p.trace = next_trace("dW", l, r1 - r0, ly.out, rows, chunk);
-  SB_TRY((launch_gemm_tc<EPI_DW, true, true>(pl, tm, p, st, pdl)));
+  if (pl.bn == 256) SB_TRY(launch_gemm_dw(pl, tm, p, st, pdl));
+  else SB_TRY((launch_gemm_tc<EPI_DW, true, true>(pl, tm, p, st, pdl)));
   mark("gemm_dw");
   return SB_OK;
 }

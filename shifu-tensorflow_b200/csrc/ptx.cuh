@@ -90,7 +90,7 @@ __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sy
 #define SB_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
 template <int N, int TA, int TB>
 __device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
-  static_assert(N == 32 || N == 64 || N == 128, "wgmma N");
+  static_assert(N == 32 || N == 64 || N == 128 || N == 256, "wgmma N");
   if constexpr (N == 32) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
@@ -119,6 +119,20 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t desc_a, u
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
         "%64, %65, p, 1, 1, %67, %68;\n\t}"
         : SB_F8(0), SB_F8(8), SB_F8(16), SB_F8(24), SB_F8(32), SB_F8(40), SB_F8(48), SB_F8(56)
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d), "n"(TA), "n"(TB));
+  }
+  if constexpr (N == 256) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+        "%128, %129, p, 1, 1, %131, %132;\n\t}"
+        : SB_F8(0), SB_F8(8), SB_F8(16), SB_F8(24), SB_F8(32), SB_F8(40), SB_F8(48), SB_F8(56),
+          SB_F8(64), SB_F8(72), SB_F8(80), SB_F8(88), SB_F8(96), SB_F8(104), SB_F8(112), SB_F8(120)
         : "l"(desc_a), "l"(desc_b), "r"(scale_d), "n"(TA), "n"(TB));
   }
 }
