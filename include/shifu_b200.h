@@ -312,8 +312,8 @@ int sb_debug_gemm_bench(const float* A, const float* B, float* D, int32_t M, int
  *   forward: out = bf16(act(A W + bias))               A [M,K], W [K,N], bias [N]
  *   dA     : out = bf16((A W^T) * act'(aux)),          A [M,K], W [N,K], aux [M,N] (an activation output);
  *            colsum[N] = column sums of the fp32 product before rounding (nullable)
- * out [M,N] receives the bf16 results widened to fp32.  bm_wg = 0 lets the planner choose the rows of a warpgroup tile,
- * 64 or 128 forces them.  iters > 0: afterwards, average device milliseconds per launch over `iters` back-to-back
+ * out [M,N] receives the bf16 results widened to fp32.  bm_wg = 0 lets the planner choose the tile, 64 or 128 forces
+ * the rows of a ping-pong warpgroup tile, 256 the forward GEMM's 128 x 256 tile (invalid for dA).  iters > 0: afterwards, average device milliseconds per launch over `iters` back-to-back
  * launches into *ms_out. */
 int sb_debug_gemm_epilogue(const float* A, const float* W, const float* bias, const float* aux, float* out, float* colsum,
                            int32_t M, int32_t N, int32_t K, int32_t da, int32_t act, int32_t bm_wg, int device,

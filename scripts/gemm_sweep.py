@@ -1,6 +1,7 @@
 """Sweep tile configurations over the GEMM shapes of cfg1 / cfg2 (run on the GPU box). Prints us and TFLOP/s.
-Forward and dA GEMMs run on the ping-pong kernel with their real epilogues (relu), once per warpgroup tile height
-(bm_wg 64 / 128; "plan" marks the planner's choice); dW GEMMs (gemm_dw.cuh) over tile width (64 / 128 / 256) and split-K."""
+Forward and dA GEMMs run with their real epilogues (relu): on the ping-pong kernel once per warpgroup tile height
+(bm_wg 64 / 128), forward GEMMs also on the 128 x 256 tile of gemm_wide.cuh (bm_wg 256); "plan" marks the planner's
+choice.  dW GEMMs (gemm_dw.cuh) over tile width (64 / 128 / 256) and split-K."""
 import sys, os, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -17,10 +18,14 @@ def shapes(B, F, h):
             out.append(("dA%d" % (l + 1), B, dims[l], dims[l + 1], False, False, [1]))
     return out
 
-def planned_bm_wg(M, N, K, sms=132):   # plan_gemm_pp (gemm_pp.cuh)
+def planned_bm_wg(M, N, K, fwd, sms=132):   # plan_gemm_pp (gemm_pp.cuh)
+    tm, kb = (M + 127) // 128, (K + 63) // 64
+    wide, narrow = tm * ((N + 255) // 256), tm * ((N + 127) // 128)
+    if fwd and N > 128 and 8 * wide >= 7 * sms and kb >= 16 and 2 * -(-wide // sms) <= -(-narrow // sms):
+        return 256
     bn = 64 if N <= 64 else 128
-    t = ((M + 127) // 128) * ((N + bn - 1) // bn)
-    return 128 if t > sms or (8 * t >= 7 * sms and (K + 63) // 64 >= 8) else 64
+    t = tm * ((N + bn - 1) // bn)
+    return 128 if t > sms or (8 * t >= 7 * sms and kb >= 8) else 64
 
 res = []
 rng = np.random.default_rng(0)
@@ -31,10 +36,10 @@ for cfgname, (B, F, h) in {"cfg1": (4096, 1000, [512, 256, 128]), "cfg2": (8192,
             A = rng.standard_normal((M, K), dtype=np.float32)
             W = rng.standard_normal((N, K) if da else (K, N), dtype=np.float32)
             kw = dict(aux=rng.uniform(0, 1, (M, N)).astype(np.float32)) if da else dict(bias=np.zeros(N, np.float32))
-            for bm in (64, 128):
+            for bm in (64, 128) if da else (64, 128, 256):
                 _, _, ms = sb.capi.debug_gemm_epilogue(A, W, sb.capi.ACT_RELU, bm_wg=bm, iters=30, **kw)
                 tf = 2.0 * M * N * K / (ms * 1e-3) / 1e12
-                tag = "plan" if bm == planned_bm_wg(M, N, K) else ""
+                tag = "plan" if bm == planned_bm_wg(M, N, K, not da) else ""
                 print("%s %-5s M=%5d N=%5d K=%5d bm_wg=%3d  %8.2f us  %7.1f TF %s" % (cfgname, name, M, N, K, bm, ms * 1e3, tf, tag), flush=True)
                 res.append(dict(cfg=cfgname, name=name, M=M, N=N, K=K, bm_wg=bm, us=ms * 1e3, tflops=tf))
             continue

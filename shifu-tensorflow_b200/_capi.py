@@ -607,7 +607,9 @@ def debug_gemm_bench(M: int, N: int, K: int, split_k: int = 1, a_mn: bool = Fals
 def debug_gemm_epilogue(A: np.ndarray, W: np.ndarray, act: int, bias: Optional[np.ndarray] = None,
                         aux: Optional[np.ndarray] = None, bm_wg: int = 0, iters: int = 0, device: int = 0):
     """One plain-bf16 forward (aux None: act(A W + bias), W [K,N]) or dA (aux given: (A W^T) * act'(aux), W [N,K]) GEMM
-    with its fused epilogue -> (out [M,N] fp32 of the bf16 results, column sums [N] or None, ms per launch or None)"""
+    with its fused epilogue -> (out [M,N] fp32 of the bf16 results, column sums [N] or None, ms per launch or None).
+    bm_wg: 0 = the planner's tile, 64 / 128 = the ping-pong kernel's warpgroup tile rows, 256 = the forward GEMM's
+    128 x 256 tile"""
     A, W = _f32(A), _f32(W)
     M, K = A.shape
     da = aux is not None

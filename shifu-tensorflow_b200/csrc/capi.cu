@@ -9,6 +9,7 @@
 #include "net.cuh"
 #include "gemm_dw.cuh"
 #include "gemm_pp.cuh"
+#include "gemm_wide.cuh"
 #include "savedmodel.h"
 #include "xchg_p2p.cuh"
 
@@ -1681,8 +1682,8 @@ static int debug_gemm_impl(const float* A, const float* B, float* D, int32_t M, 
       GemmTcParams q = p;
       q.bias = d_bias; q.act = SB_ACT_RELU; q.out = d_out; q.ld_out = ldn; q.aux = d_aux; q.ld_aux = ldn; q.colsum = d_colsum;
       q.acc_vec4 = (N % 4 == 0) ? 1 : 0;
-      // KM / KK: the ping-pong kernel the step plans for the shape
-      const PpPlan pp = plan_gemm_pp(M, N, K, prop.multiProcessorCount);
+      // KM / KK: the kernel the step plans for the shape
+      const PpPlan pp = plan_gemm_pp(M, N, K, prop.multiProcessorCount, !a_mn && b_mn);
       PpTmaps pt;
       if (!a_mn) {
         if (s == SB_OK) s = make_tmap_bf16(&pt.a, dA, a_rows, a_cols, lda, pp.bm_wg);
@@ -1692,11 +1693,12 @@ static int debug_gemm_impl(const float* A, const float* B, float* D, int32_t M, 
       }
       auto real = [&]() -> int {
         if (!a_mn && !b_mn) return launch_gemm_pp<EPI_DA>(pp, pt, q, 0, false);
-        if (!a_mn) return launch_gemm_pp<EPI_FWD>(pp, pt, q, 0, false);
+        if (!a_mn) return pp.bn == 256 ? launch_gemm_wide(pp, pt, q, 0, false) : launch_gemm_pp<EPI_FWD>(pp, pt, q, 0, false);
         if (pl.bn == 256) return launch_gemm_dw(pl, tms, q, 0, false);
         return launch_gemm_tc<EPI_DW, true, true>(pl, tms, q, 0, false);
       };
       if (s == SB_OK) s = a_mn ? set_gemm_tc_attrs<EPI_DW, true, true>() : set_gemm_pp_attrs();
+      if (s == SB_OK && pp.bn == 256) s = set_gemm_wide_attrs();
       cudaEvent_t e0, e1;
       cudaEventCreate(&e0); cudaEventCreate(&e1);
       for (int i = 0; i < 3 && s == SB_OK; ++i) s = real();
@@ -1811,7 +1813,9 @@ int sb_debug_gemm_epilogue(const float* A, const float* W, const float* bias, co
   SB_CHECK(A && W && out && M > 0 && N > 0 && K > 0 && (da == 0 || da == 1), SB_ERR_INVALID, "bad argument");
   SB_CHECK(da ? aux != nullptr : bias != nullptr, SB_ERR_INVALID, "the forward GEMM needs a bias, the dA GEMM an aux matrix");
   SB_CHECK(act >= SB_ACT_NONE && act <= SB_ACT_LEAKYRELU, SB_ERR_INVALID, "act invalid");
-  SB_CHECK(bm_wg == 0 || bm_wg == 64 || bm_wg == 128, SB_ERR_INVALID, "bm_wg must be 0, 64 or 128 (got %d)", bm_wg);
+  SB_CHECK(bm_wg == 0 || bm_wg == 64 || bm_wg == 128 || bm_wg == PP_TILE_WIDE, SB_ERR_INVALID,
+           "bm_wg must be 0, 64, 128 or %d (got %d)", PP_TILE_WIDE, bm_wg);
+  SB_CHECK(!(da && bm_wg == PP_TILE_WIDE), SB_ERR_INVALID, "the %d-wide tile is for the forward GEMM only", PP_TILE_WIDE);
   SB_CHECK(iters >= 0 && (iters == 0 || ms_out != nullptr), SB_ERR_INVALID, "iters / ms_out");
   int n_dev = 0;
   SB_CHECK(cudaGetDeviceCount(&n_dev) == cudaSuccess && n_dev > 0, SB_ERR_CUDA, "no CUDA device available");
@@ -1849,7 +1853,7 @@ int sb_debug_gemm_epilogue(const float* A, const float* W, const float* bias, co
     SB_CUDA(cudaMemcpy(dX32, aux, sizeof(float) * mn, cudaMemcpyHostToDevice));
     cast_bf16_kernel<<<static_cast<unsigned>((mn + 255) / 256), 256>>>(dX32, M, N, d_aux, ldn);
   }
-  const PpPlan pp = plan_gemm_pp(M, N, K, prop.multiProcessorCount, bm_wg);
+  const PpPlan pp = plan_gemm_pp(M, N, K, prop.multiProcessorCount, da == 0, bm_wg);
   PpTmaps pt;
   int s = make_tmap_bf16(&pt.a, dA, M, K, lda, pp.bm_wg);
   if (s == SB_OK) s = make_tmap_bf16(&pt.b, dW, w_rows, w_cols, ldw, da ? pp.bn : 64);
@@ -1858,12 +1862,15 @@ int sb_debug_gemm_epilogue(const float* A, const float* W, const float* bias, co
   GemmTcParams p = {};
   p.M = M; p.N = N; p.K = K;
   p.act = act; p.bias = d_bias; p.colsum = colsum ? d_col : nullptr;
-  auto launch = [&]() { return da ? launch_gemm_pp<EPI_DA>(pp, pt, p, 0, false) : launch_gemm_pp<EPI_FWD>(pp, pt, p, 0, false); };
-  if (s == SB_OK) s = set_gemm_pp_attrs();
+  auto launch = [&]() {
+    if (da) return launch_gemm_pp<EPI_DA>(pp, pt, p, 0, false);
+    return pp.bn == 256 ? launch_gemm_wide(pp, pt, p, 0, false) : launch_gemm_pp<EPI_FWD>(pp, pt, p, 0, false);
+  };
+  if (s == SB_OK) s = pp.bn == 256 ? set_gemm_wide_attrs() : set_gemm_pp_attrs();
   if (s == SB_OK) s = launch();
   if (s == SB_OK) {
     cudaError_t e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) s = set_error(SB_ERR_CUDA, "gemm_pp_kernel failed: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) s = set_error(SB_ERR_CUDA, "%s failed: %s", pp.bn == 256 ? "gemm_wide_kernel" : "gemm_pp_kernel", cudaGetErrorString(e));
   }
   if (s == SB_OK) {
     std::vector<uint16_t> h(static_cast<size_t>(M) * ldn);

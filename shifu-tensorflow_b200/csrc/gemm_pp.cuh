@@ -227,23 +227,45 @@ gemm_pp_kernel(const __grid_constant__ PpTmaps tms, const GemmTcParams p) {
 
 // ------------------------------------------------------------------ host side
 struct PpPlan {
-  int bm_wg;   // rows of one warpgroup's tile: 128, or 64 when 128-row tiles would leave warpgroups without a tile
-  int bn;      // 64 / 128
+  int bm_wg;   // rows of one warpgroup's tile: 128, or 64 when 128-row tiles would leave warpgroups without a tile;
+               // 128 = the CTA's rows for the 128 x 256 forward tile (bn = 256)
+  int bn;      // 64 / 128: gemm_pp_kernel; 256: gemm_wide_kernel (gemm_wide.cuh, forward only)
   int grid;
 };
 
-// bm_wg = 0: chosen from the tile count.  A CTA needs two tiles for both of its warpgroups to have work, so with no more
-// 128-row tiles than SMs 64-row tiles give each CTA two to four.  Except when 128-row tiles still cover nearly every SM
-// and the main loop is long (>= 8 k-blocks): there the taller tile's operand reuse wins over the overlapped epilogue
-// (one H100 SXM, 132 SMs: 4096 x 512 x 1000 takes 11.7 us with 128-row tiles, 13.2 us with 64; 8192 x 256 x 512 7.6 vs
-// 9.1 us; 4096 x 512 x 256, 4 k-blocks, 7.8 vs 7.4 us).
-static inline PpPlan plan_gemm_pp(int M, int N, int K, int num_sms, int bm_wg = 0) {
+// PP_TILE_WIDE as the forced tile: the 128 x 256 forward tile of gemm_wide.cuh
+constexpr int PP_TILE_WIDE = 256;
+
+// tile = 0: chosen from the shape; 64 / 128 force the ping-pong kernel's warpgroup tile rows, PP_TILE_WIDE the 128 x 256
+// forward tile (the caller rejects it for dA).
+// Forward GEMMs go on 128 x 256 tiles when N > 128 (a narrower layer would fill half the tile with zeros), there are at
+// least 7/8 as many such tiles as SMs, no more waves of them than of 128 x 128 tiles (each counted twice: a 256-wide
+// tile is two 128-wide ones), and the main loop is long (>= 16 k-blocks), so that the exposed epilogue is a small share of
+// a tile.  cfg2's forward 0 and 1 qualify (256 and 128 tiles on 132 SMs; one H100 SXM at 400 W, relu: 8192 x 1024 x 2000
+// 71.0 -> 64.3 us, 8192 x 512 x 1024 18.0 -> 17.2 us), cfg1's largest does not (4096 x 512 x 1000, 64 tiles: 11.9 us on
+// ping-pong, 15.1 us wide), nor cfg2's forward 2 (8192 x 256 x 512, 64 tiles: 7.8 vs 10.5 us).
+// Otherwise (ping-pong) a CTA needs two tiles for both of its warpgroups to have work, so with no more 128-row tiles than
+// SMs 64-row tiles give each CTA two to four.  Except when 128-row tiles still cover nearly every SM and the main loop is
+// long (>= 8 k-blocks): there the taller tile's operand reuse wins over the overlapped epilogue (one H100 SXM, 132 SMs:
+// 4096 x 512 x 1000 takes 11.7 us with 128-row tiles, 13.2 us with 64; 8192 x 256 x 512 7.6 vs 9.1 us; 4096 x 512 x 256,
+// 4 k-blocks, 7.8 vs 7.4 us).
+static inline PpPlan plan_gemm_pp(int M, int N, int K, int num_sms, bool fwd, int tile = 0) {
   PpPlan pl = {};
+  const int tiles_m = (M + 127) / 128, kb = (K + 63) / 64;
+  const int wide_tiles = tiles_m * ((N + 255) / 256), narrow_tiles = tiles_m * ((N + 127) / 128);
+  const bool wide = fwd && N > 128 && 8 * wide_tiles >= 7 * num_sms && kb >= 16 &&
+                    2 * ((wide_tiles + num_sms - 1) / num_sms) <= (narrow_tiles + num_sms - 1) / num_sms;
+  if (tile == PP_TILE_WIDE || (tile == 0 && wide)) {
+    pl.bm_wg = 128;
+    pl.bn = 256;
+    pl.grid = wide_tiles < num_sms ? wide_tiles : num_sms;
+    return pl;
+  }
   pl.bn = N <= 64 ? 64 : 128;
   const int tiles_n = (N + pl.bn - 1) / pl.bn;
-  const int tiles128 = ((M + 127) / 128) * tiles_n;
-  const bool tall = tiles128 > num_sms || (8 * tiles128 >= 7 * num_sms && (K + 63) / 64 >= 8);
-  pl.bm_wg = bm_wg > 0 ? bm_wg : (tall ? 128 : 64);
+  const int tiles128 = tiles_m * tiles_n;
+  const bool tall = tiles128 > num_sms || (8 * tiles128 >= 7 * num_sms && kb >= 8);
+  pl.bm_wg = tile > 0 ? tile : (tall ? 128 : 64);
   const int tiles = ((M + pl.bm_wg - 1) / pl.bm_wg) * tiles_n;
   pl.grid = tiles < num_sms ? tiles : num_sms;
   return pl;

@@ -1,6 +1,6 @@
-// The skeleton shared by the wgmma GEMM kernels (gemm_tc.cuh, gemm_pp.cuh, gemm_fwd_out.cuh): the TMA producer, the
-// shared-memory operand ring, the consumers' k-block loop, kernel entry and exit.  The kernels add their tile enumeration,
-// the boxes they load per k-block and their epilogues.
+// The skeleton shared by the wgmma GEMM kernels (gemm_tc.cuh, gemm_pp.cuh, gemm_wide.cuh, gemm_dw.cuh, gemm_fwd_out.cuh):
+// the TMA producer, the shared-memory operand ring, the consumers' k-block loop, kernel entry and exit.  The kernels add
+// their tile enumeration, the boxes they load per k-block and their epilogues.
 //
 // Persistent, one CTA per SM, 384 threads = three warpgroups:
 //   warps 8..11: the producer warpgroup.  One thread fills a STAGES-deep ring of 128-byte-swizzled TMA boxes, one k-block

@@ -8,6 +8,7 @@
 #include "gemm_dw.cuh"
 #include "gemm_fwd_out.cuh"
 #include "gemm_pp.cuh"
+#include "gemm_wide.cuh"
 
 namespace sb {
 
@@ -272,6 +273,7 @@ int Net::init(const sb_net_desc* d, int device_, bool training_) {
     SB_TRY((set_gemm_tc_attrs<EPI_FWD, false, true>()));
     SB_TRY(set_gemm_fwd_out_attrs());
     SB_TRY(set_gemm_pp_attrs());
+    SB_TRY(set_gemm_wide_attrs());
     SB_TRY((set_gemm_tc_attrs<EPI_DA, false, false>()));
     SB_TRY((set_gemm_tc_attrs<EPI_DW, true, true>()));
     SB_TRY(set_gemm_dw_attrs());
@@ -399,12 +401,13 @@ int Net::enqueue_hidden_forward(const StepIn& in, int rows, float* grad, bool* f
       if (l == 0) { p.zero_buf = clear; p.zero_n4 = clear_n4; }
       p.trace = next_trace("fwd", l, rows, ly.out, k_in);
       if (nparts == 1 && p.addend == nullptr) {    // plain bf16: the ping-pong kernel
-        const PpPlan pp = plan_gemm_pp(rows, ly.out, k_in, num_sms);
+        const PpPlan pp = plan_gemm_pp(rows, ly.out, k_in, num_sms, true);
         PpTmaps pt;
         SB_TRY(make_tmap_bf16(&pt.a, src, src_rows, k_in, ld_k, pp.bm_wg));
         pt.b = tm.b[0];
         SB_TRY(make_tmap_bf16(&pt.o, A[l], rows, ly.out, ly.ld_out, pp.bm_wg));
-        SB_TRY(launch_gemm_pp<EPI_FWD>(pp, pt, p, stream, true));
+        if (pp.bn == 256) SB_TRY(launch_gemm_wide(pp, pt, p, stream, true));
+        else SB_TRY(launch_gemm_pp<EPI_FWD>(pp, pt, p, stream, true));
       } else {
         const GemmPlan pl = plan_gemm(rows, ly.out, round_up(k_in, 64) * pairs_of(nparts), num_sms, false);
         SB_TRY(make_tmaps_bf16(tm.a, src, src_ps, nparts, src_rows, k_in, ld_k, 128));
@@ -535,7 +538,7 @@ int Net::enqueue_da(int l, int rows, float* grad) {
   p.colsum = grad + pl.b_off;
   p.trace = next_trace("dA", l, rows, ly.in, ly.out);
   if (nparts == 1) {                           // plain bf16: the ping-pong kernel
-    const PpPlan pp = plan_gemm_pp(rows, ly.in, ly.out, num_sms);
+    const PpPlan pp = plan_gemm_pp(rows, ly.in, ly.out, num_sms, false);
     PpTmaps pt;
     SB_TRY(make_tmap_bf16(&pt.a, dZ[l], rows, ly.out, ly.ld_out, pp.bm_wg));
     SB_TRY(make_tmap_bf16(&pt.b, ly.Wn, ly.in, ly.out, ly.ld_out, pp.bn));
