@@ -319,6 +319,24 @@ int sb_debug_gemm_epilogue(const float* A, const float* W, const float* bias, co
                            int32_t M, int32_t N, int32_t K, int32_t da, int32_t act, int32_t bm_wg, int device,
                            int32_t iters, float* ms_out);
 
+/* The last hidden layer of a training step with the output layer fused into its GEMM (gemm_fwd_out_kernel, N <= 256),
+ * launched the way the step launches it:
+ *   a = act(A W + bias) (fp32),  z = a . wo + bo,  y_hat = sigmoid(z),  loss term and dz (SUM_BY_NONZERO_WEIGHTS),
+ *   dZ = dz * wo * act'(a) as np bf16 parts,  db_L += sum_r dZ,  dw_o += sum_r dz a,  db_o += sum_r dz,
+ *   loss_sum += sum_r loss term.
+ * A [a_rows, K] fp32; the batch is rows row0 .. row0 + M - 1, read at a row offset as a step reads the HBM-resident set.
+ * W [K, N], bias [N], wo [N] fp32.  A and W are split into np bf16 parts on the device (np = 1: plain bf16).
+ * y, w [M]; n_nz is the count of non-zero w.  g_bL [N], g_wo [N], g_bo [1] and loss_sum [1] are in/out: the kernel
+ * adds into the values passed in.  dZ [np, M, N] receives each part's bf16 widened to fp32.  Before the launch every
+ * part's pad columns N .. round_up(N, 8) - 1 and 64 rows past M are filled with a sentinel; *guard returns how many of
+ * them changed, except that a pad column of a batch row may hold +-0 (the tile is 0 beyond N and the bulk tensor store
+ * writes a row's last 16-byte piece whole).  grid = 0: the step's grid (one CTA per 64-row tile, at most one per SM);
+ * 1 .. SMs: that many CTAs, each running several tiles.  No PDL, no trace. */
+int sb_debug_gemm_fwd_out(const float* A, const float* W, const float* bias, const float* wo, float bo, const float* y,
+                          const float* w, float* dZ, float* g_bL, float* g_wo, float* g_bo, float* loss_sum, int32_t* guard,
+                          int32_t M, int32_t N, int32_t K, int32_t a_rows, int32_t row0, int32_t act, int32_t loss,
+                          int32_t np, int32_t grid, int device);
+
 #ifdef __cplusplus
 }
 #endif

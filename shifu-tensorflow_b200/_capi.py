@@ -155,6 +155,9 @@ PROTOTYPES = {
                                          C.c_int32, C.c_int32, C.c_int]),
     "sb_debug_gemm_epilogue": (C.c_int, [_f32p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                          C.c_int32, C.c_int32, C.c_int, C.c_int32, _f32p]),
+    "sb_debug_gemm_fwd_out": (C.c_int, [_f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p,
+                                        _P(C.c_int32), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                        C.c_int32, C.c_int32, C.c_int32, C.c_int]),
 }
 
 
@@ -624,6 +627,31 @@ def debug_gemm_epilogue(A: np.ndarray, W: np.ndarray, act: int, bias: Optional[n
                                        _ptr(aux) if da else None, _ptr(out), _ptr(cs) if da else None, M, N, K, int(da),
                                        act, bm_wg, device, iters, C.byref(ms)))
     return out, cs, (float(ms.value) if iters > 0 else None)
+
+
+def debug_gemm_fwd_out(A: np.ndarray, W: np.ndarray, bias: np.ndarray, wo: np.ndarray, bo: float, y: np.ndarray,
+                       w: np.ndarray, act: int, loss: int, np_parts: int = 1, row0: int = 0, M: Optional[int] = None,
+                       grid: int = 0, g_bL: Optional[np.ndarray] = None, g_wo: Optional[np.ndarray] = None, g_bo: float = 0.0,
+                       loss_sum: float = 0.0, device: int = 0):
+    """The fused output-layer GEMM of a training step (last hidden layer N <= 256) on rows row0 .. row0 + M - 1 of
+    A [a_rows, K] (M defaults to the rest of A), W [K, N], y / w [M].  g_bL, g_wo [N], g_bo and loss_sum are the initial
+    values the kernel adds into (zeros by default).  -> (dZ [np_parts, M, N] fp32 of the bf16 parts, g_bL, g_wo, g_bo,
+    loss_sum, number of changed sentinel elements around dZ)"""
+    A, W, bias, wo = _f32(A), _f32(W), _f32(bias), _f32(wo)
+    a_rows, K = A.shape
+    K2, N = W.shape
+    assert K == K2
+    M = a_rows - row0 if M is None else M
+    y, w = _f32(y).reshape(-1), _f32(w).reshape(-1)
+    assert y.size == M and w.size == M
+    g_bL = _f32(g_bL).copy() if g_bL is not None else np.zeros(N, np.float32)
+    g_wo = _f32(g_wo).copy() if g_wo is not None else np.zeros(N, np.float32)
+    gbo, ls, guard = C.c_float(g_bo), C.c_float(loss_sum), C.c_int32(-1)
+    dZ = np.zeros((max(np_parts, 1), max(M, 0), N), np.float32)
+    check(lib().sb_debug_gemm_fwd_out(_ptr(A), _ptr(W), _ptr(bias), _ptr(wo), float(bo), _ptr(y), _ptr(w), _ptr(dZ),
+                                      _ptr(g_bL), _ptr(g_wo), C.byref(gbo), C.byref(ls), C.byref(guard), M, N, K, a_rows, row0,
+                                      act, loss, np_parts, grid, device))
+    return dZ, g_bL, g_wo, float(gbo.value), float(ls.value), int(guard.value)
 
 
 def text_parse_device(text: bytes, col_map: Sequence[int], n_feat: int, delim: str = "|", device: int = 0, flag_cap: int = 65536):

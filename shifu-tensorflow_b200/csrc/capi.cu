@@ -8,6 +8,7 @@
 #include <random>
 #include "net.cuh"
 #include "gemm_dw.cuh"
+#include "gemm_fwd_out.cuh"
 #include "gemm_pp.cuh"
 #include "gemm_wide.cuh"
 #include "savedmodel.h"
@@ -1900,6 +1901,125 @@ int sb_debug_gemm_epilogue(const float* A, const float* W, const float* bias, co
   }
   cudaFree(dA32); cudaFree(dW32); cudaFree(dX32); cudaFree(d_bias); cudaFree(d_col);
   cudaFree(dA); cudaFree(dW); cudaFree(d_out); cudaFree(d_aux);
+  return s;
+}
+
+int sb_debug_gemm_fwd_out(const float* A, const float* W, const float* bias, const float* wo, float bo, const float* y,
+                          const float* w, float* dZ, float* g_bL, float* g_wo, float* g_bo, float* loss_sum, int32_t* guard,
+                          int32_t M, int32_t N, int32_t K, int32_t a_rows, int32_t row0, int32_t act, int32_t loss,
+                          int32_t np, int32_t grid, int device) {
+  SB_CHECK(A && W && bias && wo && y && w && dZ && g_bL && g_wo && g_bo && loss_sum && guard, SB_ERR_INVALID, "null argument");
+  SB_CHECK(M > 0 && K > 0 && N >= 1 && N <= FWD_OUT_MAX_N, SB_ERR_INVALID, "M=%d K=%d N=%d (N must be 1..%d)", M, K, N,
+           FWD_OUT_MAX_N);
+  SB_CHECK(np >= 1 && np <= 3, SB_ERR_INVALID, "np=%d outside 1..3", np);
+  SB_CHECK(loss == SB_LOSS_MSE || loss == SB_LOSS_SIGMOID_CE, SB_ERR_INVALID, "loss invalid");
+  SB_CHECK(act >= SB_ACT_NONE && act <= SB_ACT_LEAKYRELU, SB_ERR_INVALID, "act invalid");
+  SB_CHECK(grid >= 0, SB_ERR_INVALID, "grid=%d", grid);
+  SB_CHECK(row0 >= 0 && static_cast<long long>(row0) + M <= a_rows, SB_ERR_INVALID, "rows %d..%d outside the %d rows of A", row0,
+           row0 + M - 1, a_rows);
+  int n_dev = 0;
+  SB_CHECK(cudaGetDeviceCount(&n_dev) == cudaSuccess && n_dev > 0, SB_ERR_CUDA, "no CUDA device available");
+  cudaDeviceProp prop;
+  SB_CUDA(cudaGetDeviceProperties(&prop, device));
+  SB_CHECK(prop.major == 9 && prop.minor == 0, SB_ERR_CUDA, "device is sm_%d%d, need sm_90", prop.major, prop.minor);
+  SB_CHECK(grid <= prop.multiProcessorCount, SB_ERR_INVALID, "grid=%d above the %d SMs", grid, prop.multiProcessorCount);
+  SB_CUDA(cudaSetDevice(device));
+  // the step's layout: parts one after the other, rows of ld = round_up(cols, 8) elements; dZ has 64 guard rows per part
+  const int lda = round_up(K, 8), ldn = round_up(N, 8), dz_rows = M + 64;
+  const long long a_ps = static_cast<long long>(a_rows) * lda, w_ps = static_cast<long long>(K) * ldn;
+  const long long dz_ps = static_cast<long long>(dz_rows) * ldn;
+  const long long a_n = static_cast<long long>(a_rows) * K, w_n = static_cast<long long>(K) * N;
+  float *dA32 = nullptr, *dW32 = nullptr, *d_vec = nullptr, *d_yw = nullptr;
+  __nv_bfloat16 *dA = nullptr, *dW = nullptr, *d_dz = nullptr;
+  BatchDesc* d_desc = nullptr;
+  SB_CUDA(cudaMalloc(&dA32, sizeof(float) * a_n));
+  SB_CUDA(cudaMalloc(&dW32, sizeof(float) * w_n));
+  SB_CUDA(cudaMalloc(&dA, sizeof(__nv_bfloat16) * a_ps * np));
+  SB_CUDA(cudaMalloc(&dW, sizeof(__nv_bfloat16) * w_ps * np));
+  SB_CUDA(cudaMalloc(&d_dz, sizeof(__nv_bfloat16) * dz_ps * np));
+  // [bias N][w_o N][db_L N][dw_o N][b_o][db_o][scal SCAL_COUNT]
+  SB_CUDA(cudaMalloc(&d_vec, sizeof(float) * (4 * N + 2 + SCAL_COUNT)));
+  SB_CUDA(cudaMalloc(&d_yw, sizeof(float) * 2 * M));
+  SB_CUDA(cudaMalloc(&d_desc, sizeof(BatchDesc)));
+  float* d_bias = d_vec;
+  float* d_wo = d_vec + N;
+  float* d_gbL = d_vec + 2 * N;
+  float* d_gwo = d_vec + 3 * N;
+  float* d_bo = d_vec + 4 * N;
+  float* d_gbo = d_bo + 1;
+  float* d_scal = d_bo + 2;
+  SB_CUDA(cudaMemset(dA, 0, sizeof(__nv_bfloat16) * a_ps * np));
+  SB_CUDA(cudaMemset(dW, 0, sizeof(__nv_bfloat16) * w_ps * np));
+  SB_CUDA(cudaMemset(d_dz, 0x7f, sizeof(__nv_bfloat16) * dz_ps * np));   // every element the bf16 sentinel 0x7f7f
+  SB_CUDA(cudaMemcpy(dA32, A, sizeof(float) * a_n, cudaMemcpyHostToDevice));
+  SB_CUDA(cudaMemcpy(dW32, W, sizeof(float) * w_n, cudaMemcpyHostToDevice));
+  float nnz = 0.f;
+  for (int r = 0; r < M; ++r) nnz += (w[r] != 0.f) ? 1.f : 0.f;
+  std::vector<float> h_vec(4 * N + 2 + SCAL_COUNT, 0.f);
+  std::copy(bias, bias + N, h_vec.begin());
+  std::copy(wo, wo + N, h_vec.begin() + N);
+  std::copy(g_bL, g_bL + N, h_vec.begin() + 2 * N);
+  std::copy(g_wo, g_wo + N, h_vec.begin() + 3 * N);
+  h_vec[4 * N] = bo;
+  h_vec[4 * N + 1] = *g_bo;
+  h_vec[4 * N + 2 + SCAL_LOSS_SUM] = *loss_sum;
+  h_vec[4 * N + 2 + SCAL_NNZ] = nnz;
+  SB_CUDA(cudaMemcpy(d_vec, h_vec.data(), sizeof(float) * h_vec.size(), cudaMemcpyHostToDevice));
+  SB_CUDA(cudaMemcpy(d_yw, y, sizeof(float) * M, cudaMemcpyHostToDevice));
+  SB_CUDA(cudaMemcpy(d_yw + M, w, sizeof(float) * M, cudaMemcpyHostToDevice));
+  BatchDesc h_desc = {};
+  h_desc.y = d_yw; h_desc.w = d_yw + M; h_desc.gscale = 1.f; h_desc.row0 = row0;
+  SB_CUDA(cudaMemcpy(d_desc, &h_desc, sizeof(BatchDesc), cudaMemcpyHostToDevice));
+  cast_bf16_kernel<<<static_cast<unsigned>((a_n + 255) / 256), 256>>>(dA32, a_rows, K, dA, lda, np, a_ps);
+  cast_bf16_kernel<<<static_cast<unsigned>((w_n + 255) / 256), 256>>>(dW32, K, N, dW, ldn, np, w_ps);
+  // the launch of Net::enqueue_hidden_forward's fused branch
+  const bool resident = row0 != 0 || a_rows != M;
+  FwdOutTmaps ft;
+  int s = make_tmaps_bf16(ft.a, dA, a_ps, np, a_rows, K, lda, 64);
+  if (s == SB_OK) s = make_tmaps_bf16(ft.b, dW, w_ps, np, K, N, ldn, 64);
+  if (s == SB_OK) s = make_tmaps_bf16(ft.o, d_dz, dz_ps, np, M, N, ldn, 64);
+  GemmTcParams p = {};
+  set_part_pairs(&p, np);
+  p.M = M; p.N = N; p.K = K;
+  p.bias = d_bias; p.act = act;
+  p.a_rows = resident ? d_desc : nullptr;
+  p.wo = d_wo; p.bo = d_bo;
+  p.desc = d_desc; p.scal = d_scal; p.loss = loss;
+  p.g_wo = d_gwo; p.g_bo = d_gbo; p.g_bL = d_gbL;
+  const int tiles = (M + 63) / 64;
+  const int step_grid = tiles < prop.multiProcessorCount ? tiles : prop.multiProcessorCount;
+  if (s == SB_OK) s = set_gemm_fwd_out_attrs();
+  if (s == SB_OK) s = launch_gemm_fwd_out(grid > 0 ? grid : step_grid, ft, p, 0, false);
+  if (s == SB_OK) {
+    cudaError_t e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) s = set_error(SB_ERR_CUDA, "gemm_fwd_out_kernel failed: %s", cudaGetErrorString(e));
+  }
+  std::vector<uint16_t> h(static_cast<size_t>(dz_ps) * np);
+  if (s == SB_OK && (cudaMemcpy(h.data(), d_dz, sizeof(uint16_t) * h.size(), cudaMemcpyDeviceToHost) != cudaSuccess ||
+                     cudaMemcpy(h_vec.data(), d_vec, sizeof(float) * h_vec.size(), cudaMemcpyDeviceToHost) != cudaSuccess))
+    s = set_error(SB_ERR_CUDA, "D2H failed");
+  if (s == SB_OK) {
+    int32_t changed = 0;
+    for (int k = 0; k < np; ++k)
+      for (int r = 0; r < dz_rows; ++r)
+        for (int c = 0; c < ldn; ++c) {
+          const uint16_t v = h[static_cast<size_t>(k * dz_ps) + static_cast<size_t>(r) * ldn + c];
+          if (r < M && c < N) {
+            const uint32_t u = static_cast<uint32_t>(v) << 16;   // bf16 -> fp32, exact
+            memcpy(dZ + (static_cast<size_t>(k) * M + r) * N + c, &u, 4);
+          } else if (v != 0x7f7f && (r >= M || (v & 0x7fff) != 0)) {
+            // the bulk tensor store writes a row's last 16-byte piece whole, so the pad columns of a batch row may
+            // receive the tile's +-0 beyond N; anything else, or any write into the guard rows, is counted
+            ++changed;
+          }
+        }
+    *guard = changed;
+    std::copy(h_vec.begin() + 2 * N, h_vec.begin() + 3 * N, g_bL);
+    std::copy(h_vec.begin() + 3 * N, h_vec.begin() + 4 * N, g_wo);
+    *g_bo = h_vec[4 * N + 1];
+    *loss_sum = h_vec[4 * N + 2 + SCAL_LOSS_SUM];
+  }
+  cudaFree(dA32); cudaFree(dW32); cudaFree(dA); cudaFree(dW); cudaFree(d_dz); cudaFree(d_vec); cudaFree(d_yw); cudaFree(d_desc);
   return s;
 }
 

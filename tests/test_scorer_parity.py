@@ -12,11 +12,14 @@ GOLDEN_HEAD = os.path.join(os.path.dirname(__file__), "golden", "dummydl_head.np
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("hidden", [[100, 50], [64, 300], [64, 700], [64, 1100]], ids=["h50", "h300", "h700", "h1100"])
 @pytest.mark.parametrize("precision,tol", [(0, 1e-5), (2, 1e-5), (3, 1e-5), (1, 2e-2)])
-def test_model_score_matches_oracle(sb, precision, tol):
+def test_model_score_matches_oracle(sb, precision, tol, hidden):
     """1e-5 (north star) must hold in both parity modes: fp32 on the CUDA cores (0) and fp32-class on the tensor cores
-    (2 = three bf16 parts); the two-part mode (3) meets it as well on this net; plain bf16 (1) is the performance mode."""
-    net, params, cfg, desc = make_pair(sb, 200, [100, 50], [so.ACT_RELU, so.ACT_TANH], precision=precision)
+    (2 = three bf16 parts); the two-part mode (3) meets it as well on these nets; plain bf16 (1) is the performance mode.
+    A last hidden layer of 300 / 700 / 1100 scores through out_layer_rows_kernel<2> / <4> / out_layer_kernel<bf16> on
+    the tensor cores and through out_layer_kernel<float>'s column chunks on the CUDA cores."""
+    net, params, cfg, desc = make_pair(sb, 200, hidden, [so.ACT_RELU, so.ACT_TANH], precision=precision)
     X, _, _ = so.synth_batch(1000, 200, 3)
     m = sb.Model.create(desc, so.flatten_params(params))
     got = m.score(X)

@@ -79,6 +79,46 @@ def test_dense_step_launch_order(sb, monkeypatch, case):
     assert names == c["names"]
 
 
+# Which kernel runs the output layer: the fused output-layer GEMM (fwd_out, last hidden layer <= 256 wide and not a
+# wide+deep first layer) or the output-layer kernel of its own (out_layer).  Pins the route of the parity tests that exist
+# for one of them (test_trainer_parity.py, test_wide_deep_gpu.py): out_layer_rows_kernel<1 / 2 / 4> up to 256 / 512 /
+# 1024 columns, out_layer_kernel<bf16> beyond.
+ROUTES = {
+    # name: (hidden, precision, sparse, kernel)
+    "h256_bf16": ([96, 256], 1, False, "fwd_out"),
+    "h257_bf16": ([96, 257], 1, False, "out_layer"),
+    "h256_fp32tc": ([96, 256], 2, False, "fwd_out"),
+    "h300_bf16x2": ([96, 300], 3, False, "out_layer"),
+    "h700_bf16": ([96, 700], 1, False, "out_layer"),
+    "h700_fp32tc": ([96, 700], 2, False, "out_layer"),
+    "h1100_bf16": ([96, 1100], 1, False, "out_layer"),
+    "h1100_bf16x2": ([96, 1100], 3, False, "out_layer"),
+    "wide_deep_one_layer": ([48], 1, True, "out_layer"),
+}
+
+
+@pytest.mark.parametrize("case", sorted(ROUTES))
+def test_output_layer_route(sb, case):
+    hidden, prec, sparse, kernel = ROUTES[case]
+    rows, n_dense, vocab = 300, 21, [5, 9, 3, 17]
+    F = n_dense + sum(vocab) if sparse else 120
+    with sb.Trainer(_desc(sb, F, hidden, rows, prec)) as t:
+        if sparse:
+            Xd, idx, y, w = wd.synth_wide_deep_batch(rows, n_dense, vocab, 2)
+            t.init_xavier(1)
+            t.set_sparse(n_dense, sum(vocab), len(vocab))
+            assert np.isfinite(t.step_sparse(Xd, idx, y, w))
+        else:
+            t.kernels_per_step(rows)
+        names, _ = t.debug_step_trace()
+    fused = [n for n in names if n.startswith("fwd_out")]
+    own = [n for n in names if n == "out_layer"]
+    if kernel == "fwd_out":
+        assert fused == ["fwd_out%d@%dx%dx%d" % (len(hidden) - 1, rows, hidden[-1], hidden[-2])] and not own, names
+    else:
+        assert own == ["out_layer"] and not fused, names
+
+
 @pytest.mark.parametrize("case", sorted(SPARSE_CASES))
 def test_sparse_step_launch_order(sb, case):
     c = SPARSE_CASES[case]

@@ -101,24 +101,50 @@ def _bf16_case(sb, F, hidden, acts, rows, loss, weights, seed=3):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("cfg_name,F,hidden,rows", [("cfg0", 200, [100, 50], 100), ("cfg1", 1000, [512, 256, 128], 4096),
-                                                    ("cfg2", 2000, [1024, 512, 256], 8192)])
+                                                    ("cfg2", 2000, [1024, 512, 256], 8192),
+                                                    ("h700", 120, [96, 700], 300),      # out_layer_rows_kernel<4>
+                                                    ("h1100", 120, [96, 1100], 300)])   # out_layer_kernel<bf16>
 def test_bf16_step_against_bf16_oracle(sb, cfg_name, F, hidden, rows):
     """tensor-core path (bf16 operands, fp32 accumulation) against the oracle that rounds to bf16 at exactly the
     points the kernels do (oracle.loss_and_grads_bf16).  What is left is fp32-vs-fp64 accumulation order, so the
     bound is tight: 1e-5 absolute on the loss, 2e-3 of the gradient's max magnitude on gradients (an activation
-    sitting on a rounding boundary may flip one bf16 ulp).  The distance to the pure fp32 oracle is the bf16
-    quantisation itself and is only sanity-bounded here (it is reported in DESIGN.md)."""
+    sitting on a rounding boundary may flip one bf16 ulp).  The output layer's blocks (w_o, b_o and b_L) are small next
+    to the hidden layers' and are held to the same bound relative to their own max magnitude.  The distance to the pure
+    fp32 oracle is the bf16 quantisation itself and is only sanity-bounded here (it is reported in DESIGN.md)."""
     acts = [so.ACT_RELU] * len(hidden)
     net, L32, g32, Lb, gb, gl, gg = _bf16_case(sb, F, hidden, acts, rows, so.LOSS_MSE, "ones")
     assert abs(gl - Lb) <= 2e-5
     gmax = np.abs(gb).max()
     assert np.abs(gg - gb).max() <= 2e-3 * gmax, (np.abs(gg - gb).max(), gmax)
+    blocks_got, blocks_want = so.unflatten_params(net, gg), so.unflatten_params(net, gb)
+    for name, i in (("w_o", -2), ("b_o", -1), ("b_L", -3)):
+        a, b = blocks_got[i], blocks_want[i]
+        assert np.abs(a - b).max() <= 2e-3 * np.abs(b).max(), (name, np.abs(a - b).max(), np.abs(b).max())
     assert abs(gl - L32) <= 2e-3 * abs(L32)
     assert np.abs(gg - g32).max() <= 0.15 * np.abs(g32).max()
     for a, b in zip(so.unflatten_params(net, gg), so.unflatten_params(net, g32)):   # direction per block
         a = a.ravel().astype(np.float64); b = b.ravel().astype(np.float64)
         if np.linalg.norm(b) > 0:
             assert a @ b / (np.linalg.norm(a) * np.linalg.norm(b) + 1e-300) > 0.995
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("loss", [so.LOSS_MSE, so.LOSS_SIGMOID_CE])
+@pytest.mark.parametrize("prec", [0, 2, 3])    # sb.PREC_FP32, sb.PREC_FP32_TC, sb.PREC_BF16X2
+@pytest.mark.parametrize("h_last", [300, 700, 1100])
+def test_unfused_output_layer_fp32_class(sb, h_last, prec, loss):
+    """A last hidden layer wider than the fused output-layer GEMM takes (256): the output layer runs in its own kernel,
+    out_layer_rows_kernel<2 / 4> (h_L <= 512 / 1024) or out_layer_kernel<bf16> on the tensor-core modes, reading and
+    writing every bf16 part, and out_layer_kernel<float> in column chunks of 128 on the CUDA cores.  FP32 and FP32_TC
+    meet the north star's 1e-4; BF16X2 (~2^-17 per product) is held to 2e-3 of the largest gradient."""
+    rl, rg, _, gl, gg, _ = _one_step(sb, 120, [96, h_last], [so.ACT_TANH, so.ACT_RELU], 300, loss, so.OPT_SGD, prec,
+                                     weights="mixed")
+    if prec == 3:
+        assert abs(gl - rl) <= 2e-3 * max(1.0, abs(rl))
+        assert np.abs(gg - rg).max() <= 2e-3 * np.abs(rg).max()
+    else:
+        assert abs(gl - rl) <= 1e-4
+        assert np.abs(gg - rg).max() <= 1e-4
 
 
 @pytest.mark.gpu

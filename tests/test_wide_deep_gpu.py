@@ -23,12 +23,16 @@ def _setup(sb, n_dense, vocab, hidden, acts, rows, prec, opt=so.OPT_SGD, lr=0.1,
 
 
 @pytest.mark.parametrize("prec", [0, 2, 1])
-@pytest.mark.parametrize("shape", ["small", "cfg4"])
+@pytest.mark.parametrize("shape", ["small", "cfg4", "one_layer"])
 def test_sparse_step_matches_oracle_and_dense_step(sb, prec, shape):
     if shape == "small":
         n_dense, vocab, hidden, acts, rows = 21, [5, 9, 3, 17], [40, 24], [so.ACT_TANH, so.ACT_RELU], 130
-    else:       # BASELINE config 4: 500 dense + 5000 one-hot (50 categorical columns x 100 values), [1024, 512]
+    elif shape == "cfg4":   # BASELINE config 4: 500 dense + 5000 one-hot (50 categorical columns x 100 values), [1024, 512]
         n_dense, vocab, hidden, acts, rows = 500, [100] * 50, [1024, 512], [so.ACT_RELU, so.ACT_RELU], 2048
+    else:       # one hidden layer: its GEMM adds the embedding sums, so the output layer is not fused (out_layer_rows_kernel<1>)
+        n_dense, vocab, hidden, acts, rows = 21, [5, 9, 3, 17], [48], [so.ACT_RELU], 130
+    # the sparse step fuses the output layer into the last hidden GEMM only when that GEMM is not the first layer's
+    sparse_fused = hidden[-1] <= 256 and len(hidden) > 1
     net, params, desc, (Xd, idx, y, w), n_onehot = _setup(sb, n_dense, vocab, hidden, acts, rows, prec)
     Xfull = np.concatenate([Xd, wd.onehot_matrix(idx, n_onehot)], axis=1)
     L, g, yhat = wd.loss_and_grads_sparse(net, params, Xd, idx, y, w)
@@ -49,10 +53,15 @@ def test_sparse_step_matches_oracle_and_dense_step(sb, prec, shape):
         assert np.abs(pred - yhat.ravel()).max() <= 1e-5
         assert np.abs(grads - grads_d).max() <= 1e-5 + 1e-4 * gmax and abs(loss - loss_d) <= 1e-5
     else:                     # bf16: against the dense bf16-emulating oracle on the one-hot matrix (0/1 are exact in bf16)
-        Lb, gb, yb = so.loss_and_grads_bf16(net, params, Xfull, y, w, fused_out=hidden[-1] <= 256)
+        Lb, gb, yb = so.loss_and_grads_bf16(net, params, Xfull, y, w, fused_out=sparse_fused)
         gb = so.flatten_params(gb)
         assert abs(loss - Lb) <= 2e-5 and np.abs(grads - gb).max() <= 2e-3 * np.abs(gb).max()
-        assert abs(loss - loss_d) <= 2e-5 and np.abs(grads - grads_d).max() <= 2e-3 * gmax
+        if sparse_fused == (hidden[-1] <= 256):
+            assert abs(loss - loss_d) <= 2e-5 and np.abs(grads - grads_d).max() <= 2e-3 * gmax
+        else:   # the dense step keeps A_L in fp32 where the sparse one rounds it: each against the oracle of its own rounding
+            Ld, gd, _ = so.loss_and_grads_bf16(net, params, Xfull, y, w, fused_out=True)
+            gd = so.flatten_params(gd)
+            assert abs(loss_d - Ld) <= 2e-5 and np.abs(grads_d - gd).max() <= 2e-3 * np.abs(gd).max()
     assert np.abs(pred - pred_dense).max() <= (1e-6 if prec != 1 else 2e-3)
     assert np.abs(theta - theta_d).max() <= (1e-5 if prec != 1 else 2e-3)
     # rows of the embedding block nobody selected keep a zero gradient
