@@ -279,16 +279,11 @@ int sb_savedmodel_read(const char* saved_model_dir, const char* input_name, cons
                        int64_t* n_params);
 
 /* ---- kernel-level test hooks (parity tests of single kernels through the C ABI) ---- */
-/* D[M,N] = A[M,K] * B[N,K]^T on the wgmma path: A, B are fp32 host arrays that are rounded to
- * bf16 on the device; D fp32 host.  split_k >= 1. */
-int sb_debug_gemm_bf16(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K,
-                       int32_t split_k, int device);
-/* same with explicit operand layouts: a_mn = 0: A is [M,K] (K-major), 1: A is [K,M] (MN-major); b_mn likewise for
- * B ([N,K] or [K,N]).  Instantiated combinations: (0,0) dA GEMM, (0,1) forward GEMM, (1,1) dW GEMM. */
-int sb_debug_gemm_bf16_ex(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K,
-                          int32_t split_k, int32_t a_mn, int32_t b_mn, int device);
-/* same, forcing the tile configuration: cfg_cg = 1 forces a 128 x cfg_bn tile (cfg_bn 64|128); cfg_cg = 0 lets the
- * planner choose.  Any other cfg_cg is SB_ERR_INVALID. */
+/* D[M,N] = A * B^T on the wgmma path: A, B are fp32 host arrays that are rounded to bf16 on the device; D fp32 host.
+ * split_k >= 1.  Operand layouts: a_mn = 0: A is [M,K] (K-major), 1: A is [K,M] (MN-major); b_mn likewise for
+ * B ([N,K] or [K,N]).  Instantiated combinations: (0,0) dA GEMM, (0,1) forward GEMM, (1,1) dW GEMM.
+ * cfg_cg = 1 forces a 128 x cfg_bn tile (cfg_bn 64|128, or 256 for (1,1)); cfg_cg = 0 lets the planner choose.  Any
+ * other cfg_cg is SB_ERR_INVALID. */
 int sb_debug_gemm_bf16_cfg(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K,
                            int32_t split_k, int32_t a_mn, int32_t b_mn, int32_t cfg_cg, int32_t cfg_bn, int device);
 
@@ -296,13 +291,13 @@ int sb_debug_gemm_bf16_cfg(const float* A, const float* B, float* D, int32_t M, 
  * the tensor-core parity GEMM behind SB_PREC_FP32_TC / SB_PREC_BF16X2. */
 int sb_debug_gemm_split(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K, int32_t np, int device);
 
-/* micro-benchmark of one tile configuration: average device milliseconds per launch over `iters` back-to-back launches
- * (CUDA events on the launching stream, operands L2-warm) */
 /* Timeline of the last step (trainer created with SB_STEP_TRACE=1 in the environment): for each GEMM launch of the
  * step, 16 %globaltimer stamps (ns) of its CTA 0: [0] entry, [1] setup done, [2] dependencies resolved, [3] first TMA
  * issued, [4] first stage landed, [5] MMAs of the first tile issued, [6] first accumulator complete, [7] first
  * epilogue done, [8] exit.  names = comma-separated kernel roles.  Measurement aid; no reference counterpart. */
 int sb_debug_step_trace(sb_trainer_t* t, uint64_t* stamps, int32_t cap_kernels, char* names, int32_t names_cap, int32_t* n_kernels);
+/* micro-benchmark of one tile configuration: average device milliseconds per launch over `iters` back-to-back launches
+ * (CUDA events on the launching stream, operands L2-warm) */
 int sb_debug_gemm_bench(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K, int32_t split_k,
                         int32_t a_mn, int32_t b_mn, int32_t cfg_cg, int32_t cfg_bn, int device, int32_t iters,
                         float* ms_out);

@@ -146,8 +146,6 @@ PROTOTYPES = {
     "sb_savedmodel_write": (C.c_int, [_cp, _P(NetDesc), _f32p, C.c_int64]),
     "sb_savedmodel_read": (C.c_int, [_cp, _cp, _cp, _cp, _P(NetDesc), _P(C.c_int32), _f32p, C.c_int64, _P(C.c_int64)]),
     "sb_debug_gemm_split": (C.c_int, [_f32p, _f32p, _f32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int]),
-    "sb_debug_gemm_bf16": (C.c_int, [_f32p, _f32p, _f32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int]),
-    "sb_debug_gemm_bf16_ex": (C.c_int, [_f32p, _f32p, _f32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int]),
     "sb_debug_step_trace": (C.c_int, [_vp, C.POINTER(C.c_uint64), C.c_int32, C.c_char_p, C.c_int32, C.POINTER(C.c_int32)]),
     "sb_debug_gemm_bench": (C.c_int, [_f32p, _f32p, _f32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                       C.c_int32, C.c_int32, C.c_int, C.c_int32, _f32p]),

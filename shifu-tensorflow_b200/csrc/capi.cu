@@ -1,4 +1,5 @@
-// extern "C" surface of libshifu_b200.so: trainer, scorer, rendezvous, test hooks.
+// extern "C" surface of libshifu_b200.so: trainer, scorer, rendezvous, step-trace hook (the kernel-level test hooks are
+// in net.cu).
 // See include/shifu_b200.h for the contract and the reference call each entry point replaces.
 #include <math.h>
 #include <stdlib.h>
@@ -7,10 +8,6 @@
 #include <memory>
 #include <random>
 #include "net.cuh"
-#include "gemm_dw.cuh"
-#include "gemm_fwd_out.cuh"
-#include "gemm_pp.cuh"
-#include "gemm_wide.cuh"
 #include "savedmodel.h"
 #include "xchg_p2p.cuh"
 
@@ -83,6 +80,7 @@ struct sb_trainer {
   cudaStream_t copy_stream = nullptr;
   float *st2X = nullptr, *st2Y = nullptr, *st2W = nullptr;
   cudaEvent_t ev_copied[2] = {nullptr, nullptr}, ev_consumed[2] = {nullptr, nullptr};
+  bool copy_ready = false;   // every piece of the second slot exists
   unsigned long long async_steps = 0;
   // resident steps: the batch descriptor of step i+1 is written on `prep` while step i still runs (two descriptor /
   // scalar pairs, one captured graph per pair), so set_batch_kernel leaves the critical path
@@ -99,10 +97,60 @@ struct sb_trainer {
   BatchDesc* run_descs[2][RUN_S] = {};
   float* run_scals[2][RUN_S] = {};
   cudaEvent_t ev_run_prep[2] = {nullptr, nullptr}, ev_run_done[2] = {nullptr, nullptr};
+  bool run_ready = false;  // every descriptor, scalar block and event of both sets exists
   bool run_used[2] = {false, false};
   unsigned long long run_chunks = 0;
   std::map<int, cudaGraphExec_t> run_graphs;   // rows * 2 + set
+
+  // Releases what the trainer created.  Pointers into the net's allocations (descs, scals, grad, flags, xch, s1, s2, acc,
+  // st2*, run_descs, run_scals) are freed by `net`, the first member and so the last destroyed.
+  ~sb_trainer() {
+    drop_step_graphs();
+    auto destroy_event = [](cudaEvent_t e) { if (e) cudaEventDestroy(e); };
+    for (cudaEvent_t e : ev_dz) destroy_event(e);
+    destroy_event(ev_join);
+    destroy_event(ev_da_done);
+    for (int i = 0; i < SB_XCHG_SLOTS; ++i) { destroy_event(ev_x[i]); destroy_event(ev_c[i]); }
+    for (int i = 0; i < 2; ++i) {
+      destroy_event(ev_copied[i]); destroy_event(ev_consumed[i]);
+      destroy_event(ev_prep[i]); destroy_event(ev_pos[i]);
+      destroy_event(ev_run_prep[i]); destroy_event(ev_run_done[i]);
+    }
+    if (prep) cudaStreamSynchronize(prep);
+    for (cudaStream_t s : {xstream[0], xstream[1], side, prep, copy_stream}) if (s) cudaStreamDestroy(s);
+    if (h_scal) cudaFreeHost(h_scal);
+    if (h_err) cudaFreeHost(h_err);
+    if (h_hist) cudaFreeHost(h_hist);
+    close_peer_mappings();   // before the net frees the arena they were opened against
+    if (d_peers) cudaFree(d_peers);
+    free_dataset();
+    if (comm) { NcclApi* api = nccl_api(); if (api) api->CommDestroy(comm); }
+  }
+
+  void drop_step_graphs() {   // captured steps carry the exchange and the resident set they were captured with
+    for (auto& kv : graphs) cudaGraphExecDestroy(kv.second);
+    graphs.clear();
+    for (auto& kv : run_graphs) cudaGraphExecDestroy(kv.second);
+    run_graphs.clear();
+  }
+  void free_dataset() {
+    if (dsX) cudaFree(dsX);
+    if (dsXb) cudaFree(dsXb);
+    if (dsP) cudaFree(dsP);
+    if (dsY) cudaFree(dsY);
+    if (dsW) cudaFree(dsW);
+    dsX = dsY = dsW = nullptr; dsXb = nullptr; dsP = nullptr; ds_rows = 0;
+  }
+  void close_peer_mappings() {
+    for (void* p : peer_bases) cudaIpcCloseMemHandle(p);
+    peer_bases.clear();
+  }
 };
+
+static int create_event(cudaEvent_t* e) {   // (no-op if it exists: a retry after a failure creates what is missing)
+  if (!*e) SB_CUDA(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+  return SB_OK;
+}
 
 static float lr_for_step(const sb_trainer* t, long long step /*1-based*/) {
   if (t->hyper.kind == SB_OPT_ADAM) {
@@ -610,28 +658,22 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
       t->net.arena_extra_bytes += 256 + static_cast<size_t>(world + 1) * static_cast<size_t>(t->xch_n4) * 32;
     }
   }
-  int s = t->net.init(desc, device, true);
-  if (s != SB_OK) { t->net.destroy(); return s; }
+  // from here on, a failed step returns and `t` releases whatever exists
+  SB_TRY(t->net.init(desc, device, true));
   // see Net::init: no L1 / shared-memory re-partition between the kernels of a step
   cudaFuncSetAttribute(set_batch_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   cudaFuncSetAttribute(optimizer_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   cudaFuncSetAttribute(axpy_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   Net& n = t->net;
-  {
-    // streams and events of the step schedule; the side stream's CTAs are scheduled behind the main chain's
-    int prio_least = 0, prio_greatest = 0;
-    bool ok = cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest) == cudaSuccess &&
-              cudaStreamCreateWithPriority(&t->side, cudaStreamNonBlocking, prio_least) == cudaSuccess;
-    t->ev_dz.assign(n.L, nullptr);
-    for (auto& e : t->ev_dz) ok = ok && cudaEventCreateWithFlags(&e, cudaEventDisableTiming) == cudaSuccess;
-    ok = ok && cudaEventCreateWithFlags(&t->ev_join, cudaEventDisableTiming) == cudaSuccess &&
-         cudaEventCreateWithFlags(&t->ev_da_done, cudaEventDisableTiming) == cudaSuccess;
-    for (auto& x : t->xstream) ok = ok && cudaStreamCreateWithFlags(&x, cudaStreamNonBlocking) == cudaSuccess;
-    if (!ok) {
-      n.destroy();
-      return set_error(SB_ERR_CUDA, "cudaStreamCreate / cudaEventCreate failed");
-    }
-  }
+  // streams and events of the step schedule; the side stream's CTAs are scheduled behind the main chain's
+  int prio_least = 0, prio_greatest = 0;
+  SB_CUDA(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));
+  SB_CUDA(cudaStreamCreateWithPriority(&t->side, cudaStreamNonBlocking, prio_least));
+  t->ev_dz.assign(n.L, nullptr);
+  for (auto& e : t->ev_dz) SB_TRY(create_event(&e));
+  SB_TRY(create_event(&t->ev_join));
+  SB_TRY(create_event(&t->ev_da_done));
+  for (auto& x : t->xstream) SB_CUDA(cudaStreamCreateWithFlags(&x, cudaStreamNonBlocking));
   // gradient + exchange flags behind the parameters, in the arena a single IPC handle exports
   t->xch = n.arena;
   t->grad_off = static_cast<long long>(n.extra_off);
@@ -642,18 +684,12 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
     t->llg_off = (t->flags_off + static_cast<long long>(sizeof(P2PFlags)) + 255) / 256 * 256;
     t->lls_off = t->llg_off + static_cast<long long>(world) * t->xch_n4 * 32;
     // entries carry the epoch of the exchange that wrote them; epochs start at 1
-    if (cudaMemset(n.arena + t->llg_off, 0, static_cast<size_t>(world + 1) * static_cast<size_t>(t->xch_n4) * 32) != cudaSuccess) {
-      n.destroy();
-      return set_error(SB_ERR_CUDA, "cudaMemset(exchange buffers) failed");
-    }
+    SB_CUDA(cudaMemset(n.arena + t->llg_off, 0, static_cast<size_t>(world + 1) * static_cast<size_t>(t->xch_n4) * 32));
   }
   t->s1 = n.s1; t->s2 = n.s2;
-  if ((s = n.dalloc(&t->acc, n.n_params))) { n.destroy(); return s; }
-  if (cudaHostAlloc(reinterpret_cast<void**>(&t->h_err), sizeof(unsigned int) * 4, cudaHostAllocMapped) != cudaSuccess ||
-      cudaHostGetDevicePointer(reinterpret_cast<void**>(&t->d_herr), t->h_err, 0) != cudaSuccess) {
-    n.destroy();
-    return set_error(SB_ERR_CUDA, "cudaHostAlloc(exchange error word) failed");
-  }
+  SB_TRY(n.dalloc(&t->acc, n.n_params));
+  SB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&t->h_err), sizeof(unsigned int) * 4, cudaHostAllocMapped));
+  SB_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&t->d_herr), t->h_err, 0));
   memset(t->h_err, 0, sizeof(unsigned int) * 4);
   if (const char* e = getenv("SB_XCHG_TIMEOUT_S")) t->xchg_timeout_ns = static_cast<unsigned long long>(atof(e) * 1e9);
   if (const char* e = getenv("SB_XCHG_BLOCKS")) t->xchg_blocks = atoi(e);
@@ -675,46 +711,32 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
       t->x_end[1 + c] = (c == chunks - 1) ? n.work_end[0] : n.work_begin[0] + static_cast<int>(e1 / 1024);
     }
     for (int i = 0; i < SB_XCHG_SLOTS; ++i) {
-      if (cudaEventCreateWithFlags(&t->ev_x[i], cudaEventDisableTiming) != cudaSuccess ||
-          cudaEventCreateWithFlags(&t->ev_c[i], cudaEventDisableTiming) != cudaSuccess) {
-        n.destroy();
-        return set_error(SB_ERR_CUDA, "cudaEventCreate failed");
-      }
+      SB_TRY(create_event(&t->ev_x[i]));
+      SB_TRY(create_event(&t->ev_c[i]));
     }
   }
-  if (cudaHostAlloc(reinterpret_cast<void**>(&t->h_scal), sizeof(float) * SCAL_COUNT, cudaHostAllocMapped) != cudaSuccess) {
-    n.destroy();
-    return set_error(SB_ERR_CUDA, "cudaHostAlloc failed");
-  }
+  SB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&t->h_scal), sizeof(float) * SCAL_COUNT, cudaHostAllocMapped));
   memset(t->h_scal, 0, sizeof(float) * SCAL_COUNT);
-  if (cudaHostAlloc(reinterpret_cast<void**>(&t->h_hist), sizeof(float2) * sb_trainer::HIST, cudaHostAllocMapped) != cudaSuccess ||
-      cudaHostGetDevicePointer(reinterpret_cast<void**>(&t->d_hist), t->h_hist, 0) != cudaSuccess) {
-    n.destroy();
-    return set_error(SB_ERR_CUDA, "cudaHostAlloc(loss history) failed");
-  }
+  SB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&t->h_hist), sizeof(float2) * sb_trainer::HIST, cudaHostAllocMapped));
+  SB_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&t->d_hist), t->h_hist, 0));
   memset(t->h_hist, 0, sizeof(float2) * sb_trainer::HIST);
   t->descs[0] = n.desc;
   t->scals[0] = n.scal;
-  if ((s = n.dalloc(&t->descs[1], 1)) || (s = n.dalloc(&t->scals[1], SCAL_COUNT))) { n.destroy(); return s; }
-  if (cudaStreamCreateWithFlags(&t->prep, cudaStreamNonBlocking) != cudaSuccess) { n.destroy(); return set_error(SB_ERR_CUDA, "cudaStreamCreate failed"); }
+  SB_TRY(n.dalloc(&t->descs[1], 1));
+  SB_TRY(n.dalloc(&t->scals[1], SCAL_COUNT));
+  SB_CUDA(cudaStreamCreateWithFlags(&t->prep, cudaStreamNonBlocking));
   for (int i = 0; i < 2; ++i) {
-    if (cudaEventCreateWithFlags(&t->ev_prep[i], cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&t->ev_pos[i], cudaEventDisableTiming) != cudaSuccess) {
-      n.destroy();
-      return set_error(SB_ERR_CUDA, "cudaEventCreate failed");
-    }
+    SB_TRY(create_event(&t->ev_prep[i]));
+    SB_TRY(create_event(&t->ev_pos[i]));
   }
-  if (cudaHostGetDevicePointer(reinterpret_cast<void**>(&t->d_hscal), t->h_scal, 0) != cudaSuccess) {
-    t->net.destroy();
-    return set_error(SB_ERR_CUDA, "cudaHostGetDevicePointer failed");
-  }
+  SB_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&t->d_hscal), t->h_scal, 0));
   if (world > 1 && nccl_id != nullptr) {
     NcclApi* api = nccl_api();
-    if (!api) { n.destroy(); return set_error(SB_ERR_NCCL, "libnccl.so.2 could not be loaded"); }
+    SB_CHECK(api, SB_ERR_NCCL, "libnccl.so.2 could not be loaded");
     NcclUniqueId id;
     memcpy(&id, nccl_id, sizeof(id));
     int r = api->CommInitRank(&t->comm, world, id, rank);
-    if (r != 0) { n.destroy(); return set_error(SB_ERR_NCCL, "ncclCommInitRank failed: %s", api->GetErrorString(r)); }
+    SB_CHECK(r == 0, SB_ERR_NCCL, "ncclCommInitRank failed: %s", api->GetErrorString(r));
   }
   SB_CUDA(cudaStreamSynchronize(n.stream));
   *out = t.release();
@@ -729,18 +751,6 @@ int sb_trainer_ipc_handle(sb_trainer_t* t, void* out64) {
   SB_CUDA(cudaIpcGetMemHandle(&h, t->xch));
   memcpy(out64, &h, sizeof(h));
   return SB_OK;
-}
-
-static void drop_step_graphs(sb_trainer* t) {
-  for (auto& kv : t->graphs) cudaGraphExecDestroy(kv.second);   // captured steps carry the exchange they were captured with
-  t->graphs.clear();
-  for (auto& kv : t->run_graphs) cudaGraphExecDestroy(kv.second);
-  t->run_graphs.clear();
-}
-
-static void close_peer_mappings(sb_trainer* t) {
-  for (void* p : t->peer_bases) cudaIpcCloseMemHandle(p);
-  t->peer_bases.clear();
 }
 
 // CUDA loads kernels lazily, at their first launch, and that load may synchronise the device: behind an exchange kernel that
@@ -772,7 +782,7 @@ static int install_peer_table(sb_trainer* t, void* const* bases) {
   for (int q = 0; q < t->world; ++q) hp.base[q] = static_cast<char*>((q == t->rank) ? t->xch : bases[q]);
   if (!t->d_peers) SB_CUDA(cudaMalloc(&t->d_peers, sizeof(P2PPeers)));
   SB_CUDA(cudaMemcpy(t->d_peers, &hp, sizeof(hp), cudaMemcpyHostToDevice));
-  drop_step_graphs(t);
+  t->drop_step_graphs();
   t->p2p_ready = true;
   return SB_OK;
 }
@@ -783,7 +793,7 @@ int sb_trainer_set_peer_handles(sb_trainer_t* t, const void* handles, int32_t n_
            SB_MAX_RANKS, n_handles);
   SB_CUDA(cudaSetDevice(t->net.device));
   SB_CUDA(cudaStreamSynchronize(t->net.stream));
-  close_peer_mappings(t);
+  t->close_peer_mappings();
   t->p2p_ready = false;
   void* bases[SB_MAX_RANKS] = {};
   for (int q = 0; q < t->world; ++q) {
@@ -793,7 +803,7 @@ int sb_trainer_set_peer_handles(sb_trainer_t* t, const void* handles, int32_t n_
     cudaError_t e = cudaIpcOpenMemHandle(&bases[q], h, cudaIpcMemLazyEnablePeerAccess);
     if (e != cudaSuccess) {
       cudaGetLastError();
-      close_peer_mappings(t);   // all or nothing: a half-mapped table must never be used
+      t->close_peer_mappings();   // all or nothing: a half-mapped table must never be used
       return set_error(SB_ERR_CUDA, "cudaIpcOpenMemHandle(rank %d) failed: %s (no P2P path / separate IPC namespace?)", q,
                        cudaGetErrorString(e));
     }
@@ -806,8 +816,8 @@ int sb_trainer_clear_peer_handles(sb_trainer_t* t) {
   SB_CHECK(t, SB_ERR_INVALID, "null trainer");
   SB_CUDA(cudaSetDevice(t->net.device));
   SB_CUDA(cudaStreamSynchronize(t->net.stream));
-  close_peer_mappings(t);
-  if (t->p2p_ready) drop_step_graphs(t);
+  t->close_peer_mappings();
+  if (t->p2p_ready) t->drop_step_graphs();
   t->p2p_ready = false;
   return SB_OK;
 }
@@ -836,45 +846,14 @@ int sb_trainer_set_peer_pointers(sb_trainer_t* t, void* const* bases, int32_t n)
       cudaGetLastError();
     }
   }
-  close_peer_mappings(t);
+  t->close_peer_mappings();
   return install_peer_table(t, bases);
 }
 
 int sb_trainer_destroy(sb_trainer_t* t) {
   if (!t) return SB_OK;
   cudaSetDevice(t->net.device);
-  if (t->net.stream) cudaStreamSynchronize(t->net.stream);
-  for (auto& kv : t->graphs) cudaGraphExecDestroy(kv.second);
-  for (auto& kv : t->run_graphs) cudaGraphExecDestroy(kv.second);
-  for (int i = 0; i < 2; ++i) {
-    if (t->ev_run_prep[i]) cudaEventDestroy(t->ev_run_prep[i]);
-    if (t->ev_run_done[i]) cudaEventDestroy(t->ev_run_done[i]);
-  }
-  if (t->comm) { NcclApi* api = nccl_api(); if (api) api->CommDestroy(t->comm); }
-  if (t->dsX) cudaFree(t->dsX);
-  if (t->dsXb) cudaFree(t->dsXb);
-  if (t->dsP) cudaFree(t->dsP);
-  if (t->dsY) cudaFree(t->dsY);
-  if (t->dsW) cudaFree(t->dsW);
-  if (t->h_scal) cudaFreeHost(t->h_scal);
-  if (t->h_err) cudaFreeHost(t->h_err);
-  if (t->h_hist) cudaFreeHost(t->h_hist);
-  if (t->copy_stream) cudaStreamDestroy(t->copy_stream);
-  if (t->prep) { cudaStreamSynchronize(t->prep); cudaStreamDestroy(t->prep); }
-  for (int i = 0; i < 2; ++i) {
-    if (t->ev_prep[i]) cudaEventDestroy(t->ev_prep[i]);
-    if (t->ev_pos[i]) cudaEventDestroy(t->ev_pos[i]);
-    if (t->ev_copied[i]) cudaEventDestroy(t->ev_copied[i]);
-    if (t->ev_consumed[i]) cudaEventDestroy(t->ev_consumed[i]);
-  }
-  for (void* p : t->peer_bases) cudaIpcCloseMemHandle(p);
-  if (t->d_peers) cudaFree(t->d_peers);
-  for (cudaEvent_t e : t->ev_dz) if (e) cudaEventDestroy(e);
-  if (t->ev_join) cudaEventDestroy(t->ev_join);
-  if (t->ev_da_done) cudaEventDestroy(t->ev_da_done);
-  for (cudaStream_t x : t->xstream) if (x) cudaStreamDestroy(x);
-  if (t->side) cudaStreamDestroy(t->side);
-  t->net.destroy();      // frees the arena (= xch)
+  cudaStreamSynchronize(t->net.stream);
   delete t;
   return SB_OK;
 }
@@ -1008,16 +987,17 @@ int sb_trainer_step_async(sb_trainer_t* t, const float* X, const float* y, const
   Net& n = t->net;
   SB_CHECK(rows > 0 && rows <= n.max_batch, SB_ERR_INVALID, "rows=%d outside (0, max_batch=%d]", rows, n.max_batch);
   SB_CUDA(cudaSetDevice(n.device));
-  if (!t->copy_stream) {
-    SB_CUDA(cudaStreamCreateWithFlags(&t->copy_stream, cudaStreamNonBlocking));
-    SB_TRY(n.dalloc(&t->st2X, static_cast<size_t>(n.max_batch) * n.F));
-    SB_TRY(n.dalloc(&t->st2Y, n.max_batch));
-    SB_TRY(n.dalloc(&t->st2W, n.max_batch));
+  if (!t->copy_ready) {
+    if (!t->copy_stream) SB_CUDA(cudaStreamCreateWithFlags(&t->copy_stream, cudaStreamNonBlocking));
+    if (!t->st2X) SB_TRY(n.dalloc(&t->st2X, static_cast<size_t>(n.max_batch) * n.F));
+    if (!t->st2Y) SB_TRY(n.dalloc(&t->st2Y, n.max_batch));
+    if (!t->st2W) SB_TRY(n.dalloc(&t->st2W, n.max_batch));
     for (int i = 0; i < 2; ++i) {
-      SB_CUDA(cudaEventCreateWithFlags(&t->ev_copied[i], cudaEventDisableTiming));
-      SB_CUDA(cudaEventCreateWithFlags(&t->ev_consumed[i], cudaEventDisableTiming));
+      SB_TRY(create_event(&t->ev_copied[i]));
+      SB_TRY(create_event(&t->ev_consumed[i]));
     }
     SB_CUDA(cudaStreamSynchronize(n.stream));   // the zero-fill of the new staging buffers ran on the main stream
+    t->copy_ready = true;
   }
   const int slot = static_cast<int>(t->async_steps & 1);
   float* sx = slot ? t->st2X : n.stX;
@@ -1093,16 +1073,8 @@ int sb_trainer_load_dataset(sb_trainer_t* t, const float* X, const float* y, con
   Net& n = t->net;
   SB_CUDA(cudaSetDevice(n.device));
   SB_CUDA(cudaStreamSynchronize(n.stream));
-  for (auto& kv : t->graphs) cudaGraphExecDestroy(kv.second);   // captured steps carry tensor maps of the old set
-  t->graphs.clear();
-  for (auto& kv : t->run_graphs) cudaGraphExecDestroy(kv.second);
-  t->run_graphs.clear();
-  if (t->dsX) cudaFree(t->dsX);
-  if (t->dsXb) cudaFree(t->dsXb);
-  if (t->dsY) cudaFree(t->dsY);
-  if (t->dsW) cudaFree(t->dsW);
-  if (t->dsP) cudaFree(t->dsP);
-  t->dsX = t->dsY = t->dsW = nullptr; t->dsXb = nullptr; t->dsP = nullptr; t->ds_rows = 0;
+  t->drop_step_graphs();   // captured steps carry tensor maps of the old set
+  t->free_dataset();
   SB_CUDA(cudaMalloc(&t->dsY, sizeof(float) * n_rows));
   SB_CUDA(cudaMalloc(&t->dsW, sizeof(float) * n_rows));
   SB_CUDA(cudaMemcpyAsync(t->dsY, y, sizeof(float) * n_rows, cudaMemcpyDefault, n.stream));
@@ -1121,18 +1093,17 @@ int sb_trainer_load_dataset(sb_trainer_t* t, const float* X, const float* y, con
     SB_CUDA(cudaMemsetAsync(t->dsXb, 0, sizeof(__nv_bfloat16) * part_elems * n.nparts, n.stream));
     n.resident_ps = static_cast<long long>(part_elems);
     const int64_t win = 32768;
-    float* tmp = nullptr;
-    SB_CUDA(cudaMalloc(&tmp, sizeof(float) * static_cast<size_t>(win < n_rows ? win : n_rows) * n.F));
+    DevBuf<float> tmp;
+    SB_TRY(tmp.alloc(static_cast<size_t>(win < n_rows ? win : n_rows) * n.F));
     for (int64_t r0 = 0; r0 < n_rows; r0 += win) {
       const int64_t c = n_rows - r0 < win ? n_rows - r0 : win;
-      SB_CUDA(cudaMemcpyAsync(tmp, X + r0 * n.F, sizeof(float) * c * n.F, cudaMemcpyDefault, n.stream));
-      cast_bf16_kernel<<<static_cast<unsigned>((c * n.F + 255) / 256), 256, 0, n.stream>>>(tmp, static_cast<int>(c), n.F,
+      SB_CUDA(cudaMemcpyAsync(tmp.p, X + r0 * n.F, sizeof(float) * c * n.F, cudaMemcpyDefault, n.stream));
+      cast_bf16_kernel<<<static_cast<unsigned>((c * n.F + 255) / 256), 256, 0, n.stream>>>(tmp.p, static_cast<int>(c), n.F,
                                                                                            t->dsXb + r0 * n.ldF, n.ldF, n.nparts,
                                                                                            n.resident_ps);
       SB_CUDA(cudaGetLastError());
       SB_CUDA(cudaStreamSynchronize(n.stream));   // X may be pageable: the window is reused
     }
-    cudaFree(tmp);
     std::vector<int> prefix(static_cast<size_t>(n_rows) + 1);
     prefix[0] = 0;
     std::vector<float> w_host;
@@ -1209,16 +1180,17 @@ int sb_trainer_run_resident(sb_trainer_t* t, const int64_t* row_offsets, int32_t
   int i = 0;
   if (t->dsXb != nullptr && t->prep != nullptr) {
     SB_CUDA(cudaSetDevice(n.device));
-    if (t->run_descs[0][0] == nullptr) {
+    if (!t->run_ready) {
       for (int set = 0; set < 2; ++set) {
         for (int k = 0; k < S; ++k) {
-          SB_TRY(n.dalloc(&t->run_descs[set][k], 1));
-          SB_TRY(n.dalloc(&t->run_scals[set][k], SCAL_COUNT));
+          if (!t->run_descs[set][k]) SB_TRY(n.dalloc(&t->run_descs[set][k], 1));
+          if (!t->run_scals[set][k]) SB_TRY(n.dalloc(&t->run_scals[set][k], SCAL_COUNT));
         }
-        SB_CUDA(cudaEventCreateWithFlags(&t->ev_run_prep[set], cudaEventDisableTiming));
-        SB_CUDA(cudaEventCreateWithFlags(&t->ev_run_done[set], cudaEventDisableTiming));
+        SB_TRY(create_event(&t->ev_run_prep[set]));
+        SB_TRY(create_event(&t->ev_run_done[set]));
       }
       SB_CUDA(cudaStreamSynchronize(n.stream));   // the zero-fill of the new descriptors ran on the main stream
+      t->run_ready = true;
     }
     const float gscale = 1.f / static_cast<float>(t->world);
     for (; i + S <= n_steps; i += S) {
@@ -1297,19 +1269,18 @@ int sb_trainer_broadcast_state(sb_trainer_t* t, int32_t root) {
   SB_CHECK(api && t->comm, SB_ERR_NCCL, "no NCCL communicator");
   Net& n = t->net;
   SB_CUDA(cudaSetDevice(n.device));
-  long long* d_step = nullptr;
-  SB_CUDA(cudaMalloc(&d_step, sizeof(long long)));
-  SB_CUDA(cudaMemcpyAsync(d_step, &t->global_step, sizeof(long long), cudaMemcpyHostToDevice, n.stream));
+  DevBuf<long long> d_step;
+  SB_TRY(d_step.alloc(1));
+  SB_CUDA(cudaMemcpyAsync(d_step.p, &t->global_step, sizeof(long long), cudaMemcpyHostToDevice, n.stream));
   int r = api->Broadcast(n.theta, n.theta, static_cast<size_t>(n.n_params), NCCL_FLOAT32, root, t->comm, n.stream);
   if (r == 0) r = api->Broadcast(t->s1, t->s1, static_cast<size_t>(n.n_params), NCCL_FLOAT32, root, t->comm, n.stream);
   if (r == 0) r = api->Broadcast(t->s2, t->s2, static_cast<size_t>(n.n_params), NCCL_FLOAT32, root, t->comm, n.stream);
-  if (r == 0) r = api->Broadcast(d_step, d_step, 1, NCCL_INT64, root, t->comm, n.stream);
-  if (r != 0) { cudaFree(d_step); return set_error(SB_ERR_NCCL, "ncclBroadcast failed: %s", api->GetErrorString(r)); }
+  if (r == 0) r = api->Broadcast(d_step.p, d_step.p, 1, NCCL_INT64, root, t->comm, n.stream);
+  SB_CHECK(r == 0, SB_ERR_NCCL, "ncclBroadcast failed: %s", api->GetErrorString(r));
   long long step = 0;
-  SB_CUDA(cudaMemcpyAsync(&step, d_step, sizeof(long long), cudaMemcpyDeviceToHost, n.stream));
+  SB_CUDA(cudaMemcpyAsync(&step, d_step.p, sizeof(long long), cudaMemcpyDeviceToHost, n.stream));
   SB_TRY(n.refresh_shadows());
   SB_CUDA(cudaStreamSynchronize(n.stream));
-  cudaFree(d_step);
   t->global_step = step;
   return poll_nccl(t);
 }
@@ -1471,13 +1442,9 @@ static int model_from_desc(sb_net_desc d, const float* flat, int64_t n, int devi
   d.max_batch = d.precision == SB_PREC_FP32 ? MODEL_CHUNK_ROWS : (d.precision == SB_PREC_BF16 ? MODEL_CHUNK_ROWS_BF16 : MODEL_CHUNK_ROWS_BF16 / 2);
   std::unique_ptr<sb_model> m(new sb_model());
   m->desc = d;
-  int s = m->net.init(&d, device, false);
-  if (s != SB_OK) { m->net.destroy(); return s; }
-  if (n != m->net.n_params) {
-    m->net.destroy();
-    return set_error(SB_ERR_INVALID, "expected %lld params, got %lld", (long long)m->net.n_params, (long long)n);
-  }
   Net& net = m->net;
+  SB_TRY(net.init(&d, device, false));
+  SB_CHECK(n == net.n_params, SB_ERR_INVALID, "expected %lld params, got %lld", (long long)net.n_params, (long long)n);
   SB_CUDA(cudaMemcpyAsync(net.theta, flat, sizeof(float) * n, cudaMemcpyHostToDevice, net.stream));
   SB_TRY(net.refresh_shadows());
   SB_CUDA(cudaStreamSynchronize(net.stream));
@@ -1519,9 +1486,6 @@ int sb_model_load(const char* saved_model_dir, const char* input_name, const cha
 }
 
 int sb_model_destroy(sb_model_t* m) {
-  if (!m) return SB_OK;
-  cudaSetDevice(m->net.device);
-  m->net.destroy();
   delete m;
   return SB_OK;
 }
@@ -1575,11 +1539,8 @@ int sb_model_sync(sb_model_t* m) {
 void* sb_model_stream(sb_model_t* m) { return m ? reinterpret_cast<void*>(m->net.stream) : nullptr; }
 
 // ================================================================================================
-// kernel-level test hook
+// step-timeline test hook (the kernel-level hooks are in net.cu, beside the step's GEMM launches)
 // ================================================================================================
-static int debug_gemm_impl(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K, int32_t split_k,
-                           int32_t a_mn, int32_t b_mn, int32_t cfg_cg, int32_t cfg_bn, int device, int iters, float* ms_out);
-
 int sb_debug_step_trace(sb_trainer_t* t, uint64_t* stamps, int32_t cap_kernels, char* names, int32_t names_cap, int32_t* n_kernels) {
   SB_CHECK(t && stamps && n_kernels, SB_ERR_INVALID, "null argument");
   Net& n = t->net;
@@ -1595,432 +1556,6 @@ int sb_debug_step_trace(sb_trainer_t* t, uint64_t* stamps, int32_t cap_kernels, 
     snprintf(names, names_cap, "%s", all.c_str());
   }
   return SB_OK;
-}
-
-int sb_debug_gemm_bf16_cfg(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K, int32_t split_k,
-                           int32_t a_mn, int32_t b_mn, int32_t cfg_cg, int32_t cfg_bn, int device) {
-  return debug_gemm_impl(A, B, D, M, N, K, split_k, a_mn, b_mn, cfg_cg, cfg_bn, device, 0, nullptr);
-}
-int sb_debug_gemm_bench(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K, int32_t split_k,
-                        int32_t a_mn, int32_t b_mn, int32_t cfg_cg, int32_t cfg_bn, int device, int32_t iters, float* ms_out) {
-  SB_CHECK(iters > 0 && ms_out, SB_ERR_INVALID, "iters / ms_out");
-  return debug_gemm_impl(A, B, D, M, N, K, split_k, a_mn, b_mn, cfg_cg, cfg_bn, device, iters, ms_out);
-}
-}  // extern "C"
-
-static int debug_gemm_impl(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K, int32_t split_k,
-                           int32_t a_mn, int32_t b_mn, int32_t cfg_cg, int32_t cfg_bn, int device, int iters, float* ms_out) {
-  SB_CHECK(cfg_cg == 0 || (cfg_cg == 1 && (cfg_bn == 64 || cfg_bn == 128 || (cfg_bn == 256 && a_mn && b_mn))), SB_ERR_INVALID,
-           "tile configuration cg=%d bn=%d not instantiated for this layout (bn=256: MM only)", cfg_cg, cfg_bn);
-  SB_CHECK(A && B && D && M > 0 && N > 0 && K > 0, SB_ERR_INVALID, "bad argument");
-  SB_CHECK((a_mn == 0 && b_mn == 0) || (a_mn == 0 && b_mn == 1) || (a_mn == 1 && b_mn == 1), SB_ERR_INVALID,
-           "layout combination not instantiated (use KK, KM or MM)");
-  int n_dev = 0;
-  SB_CHECK(cudaGetDeviceCount(&n_dev) == cudaSuccess && n_dev > 0, SB_ERR_CUDA, "no CUDA device available");
-  cudaDeviceProp prop;
-  SB_CUDA(cudaGetDeviceProperties(&prop, device));
-  SB_CHECK(prop.major == 9 && prop.minor == 0, SB_ERR_CUDA, "device is sm_%d%d, need sm_90", prop.major, prop.minor);
-  SB_CUDA(cudaSetDevice(device));
-  // stored shapes: K-major [R, K]; MN-major [K, R]
-  const int a_rows = a_mn ? K : M, a_cols = a_mn ? M : K;
-  const int b_rows = b_mn ? K : N, b_cols = b_mn ? N : K;
-  const int lda = round_up(a_cols, 8), ldb = round_up(b_cols, 8);
-  float *dA32 = nullptr, *dB32 = nullptr, *dD = nullptr;
-  __nv_bfloat16 *dA = nullptr, *dB = nullptr;
-  SB_CUDA(cudaMalloc(&dA32, sizeof(float) * M * K));
-  SB_CUDA(cudaMalloc(&dB32, sizeof(float) * N * K));
-  SB_CUDA(cudaMalloc(&dD, sizeof(float) * M * N));
-  SB_CUDA(cudaMalloc(&dA, sizeof(__nv_bfloat16) * a_rows * lda));
-  SB_CUDA(cudaMalloc(&dB, sizeof(__nv_bfloat16) * b_rows * ldb));
-  SB_CUDA(cudaMemset(dA, 0, sizeof(__nv_bfloat16) * a_rows * lda));
-  SB_CUDA(cudaMemset(dB, 0, sizeof(__nv_bfloat16) * b_rows * ldb));
-  SB_CUDA(cudaMemset(dD, 0, sizeof(float) * M * N));
-  SB_CUDA(cudaMemcpy(dA32, A, sizeof(float) * M * K, cudaMemcpyHostToDevice));
-  SB_CUDA(cudaMemcpy(dB32, B, sizeof(float) * N * K, cudaMemcpyHostToDevice));
-  cast_bf16_kernel<<<static_cast<unsigned>((static_cast<long long>(M) * K + 255) / 256), 256>>>(dA32, a_rows, a_cols, dA, lda);
-  cast_bf16_kernel<<<static_cast<unsigned>((static_cast<long long>(N) * K + 255) / 256), 256>>>(dB32, b_rows, b_cols, dB, ldb);
-  GemmPlan pl = plan_gemm(M, N, K, prop.multiProcessorCount, false);
-  if (cfg_cg > 0) pl.bn = cfg_bn;  // explicit tile configuration requested by the test
-  {
-    const int total_kb = (K + 63) / 64;
-    int want = split_k < 1 ? 1 : (split_k > total_kb ? total_kb : split_k);
-    pl.kb_per_split = (total_kb + want - 1) / want;
-    pl.split_k = (total_kb + pl.kb_per_split - 1) / pl.kb_per_split;
-    const int work = ((M + 127) / 128) * ((N + pl.bn - 1) / pl.bn) * pl.split_k;
-    pl.grid = work < prop.multiProcessorCount ? work : prop.multiProcessorCount;
-  }
-  TmapSet tms;
-  int s = make_tmap_bf16(&tms.a[0], dA, a_rows, a_cols, lda, a_mn ? 64 : 128);
-  if (s == SB_OK) s = make_tmap_bf16(&tms.b[0], dB, b_rows, b_cols, ldb, b_mn ? 64 : pl.bn);
-  if (s == SB_OK) {
-    GemmTcParams p = {};
-    p.M = M; p.N = N; p.K = K;
-    p.accum = dD; p.ld_acc = N;
-    p.acc_vec4 = (N % 4 == 0) ? 1 : 0;
-    // 256-wide tiles (MM, the dW layout, only): the dW kernel, whose red.add into the zeroed D is the product
-    auto launch = [&]() -> int {
-      if (pl.bn == 256) return launch_gemm_dw(pl, tms, p, 0);
-      if (!a_mn && !b_mn) return launch_gemm_tc<EPI_F32, false, false>(pl, tms, p, 0);
-      if (!a_mn) return launch_gemm_tc<EPI_F32, false, true>(pl, tms, p, 0);
-      return launch_gemm_tc<EPI_F32, true, true>(pl, tms, p, 0);
-    };
-    if (pl.bn == 256) s = set_gemm_dw_attrs();
-    else if (!a_mn && !b_mn) s = set_gemm_tc_attrs<EPI_F32, false, false>();
-    else if (!a_mn) s = set_gemm_tc_attrs<EPI_F32, false, true>();
-    else s = set_gemm_tc_attrs<EPI_F32, true, true>();
-    if (s == SB_OK) s = launch();
-    if (s == SB_OK && iters > 0) {
-      // benchmark with the REAL epilogue of the layout's use: KM -> forward (bias + relu -> bf16), KK -> dA
-      // (act' * , bf16 store, column sums), MM -> dW (fp32 red.add)
-      const int ldn = round_up(N, 8);
-      float *d_bias = nullptr, *d_colsum = nullptr;
-      __nv_bfloat16 *d_out = nullptr, *d_aux = nullptr;
-      cudaMalloc(&d_bias, sizeof(float) * N); cudaMemset(d_bias, 0, sizeof(float) * N);
-      cudaMalloc(&d_colsum, sizeof(float) * N); cudaMemset(d_colsum, 0, sizeof(float) * N);
-      cudaMalloc(&d_out, sizeof(__nv_bfloat16) * static_cast<size_t>(M) * ldn);
-      cudaMalloc(&d_aux, sizeof(__nv_bfloat16) * static_cast<size_t>(M) * ldn);
-      cudaMemset(d_aux, 0x3f, sizeof(__nv_bfloat16) * static_cast<size_t>(M) * ldn);
-      GemmTcParams q = p;
-      q.bias = d_bias; q.act = SB_ACT_RELU; q.out = d_out; q.ld_out = ldn; q.aux = d_aux; q.ld_aux = ldn; q.colsum = d_colsum;
-      q.acc_vec4 = (N % 4 == 0) ? 1 : 0;
-      // KM / KK: the kernel the step plans for the shape
-      const PpPlan pp = plan_gemm_pp(M, N, K, prop.multiProcessorCount, !a_mn && b_mn);
-      PpTmaps pt;
-      if (!a_mn) {
-        if (s == SB_OK) s = make_tmap_bf16(&pt.a, dA, a_rows, a_cols, lda, pp.bm_wg);
-        if (s == SB_OK) s = make_tmap_bf16(&pt.b, dB, b_rows, b_cols, ldb, b_mn ? 64 : pp.bn);
-        if (s == SB_OK) s = make_tmap_bf16(&pt.o, d_out, M, N, ldn, pp.bm_wg);
-        if (s == SB_OK) s = make_tmap_bf16(&pt.x, d_aux, M, N, ldn, pp.bm_wg);
-      }
-      auto real = [&]() -> int {
-        if (!a_mn && !b_mn) return launch_gemm_pp<EPI_DA>(pp, pt, q, 0, false);
-        if (!a_mn) return pp.bn == 256 ? launch_gemm_wide(pp, pt, q, 0, false) : launch_gemm_pp<EPI_FWD>(pp, pt, q, 0, false);
-        if (pl.bn == 256) return launch_gemm_dw(pl, tms, q, 0, false);
-        return launch_gemm_tc<EPI_DW, true, true>(pl, tms, q, 0, false);
-      };
-      if (s == SB_OK) s = a_mn ? set_gemm_tc_attrs<EPI_DW, true, true>() : set_gemm_pp_attrs();
-      if (s == SB_OK && pp.bn == 256) s = set_gemm_wide_attrs();
-      cudaEvent_t e0, e1;
-      cudaEventCreate(&e0); cudaEventCreate(&e1);
-      for (int i = 0; i < 3 && s == SB_OK; ++i) s = real();
-      cudaEventRecord(e0, 0);
-      for (int i = 0; i < iters && s == SB_OK; ++i) s = real();
-      cudaEventRecord(e1, 0);
-      cudaEventSynchronize(e1);
-      float ms = 0.f;
-      cudaEventElapsedTime(&ms, e0, e1);
-      *ms_out = ms / iters;
-      cudaEventDestroy(e0); cudaEventDestroy(e1);
-      if (getenv("SB_GEMM_TRACE")) {
-        // one more launch with %globaltimer stamps from CTA 0 (ns relative to kernel entry), and the host-visible
-        // launch-to-completion time of a single isolated launch
-        unsigned long long* d_tr = nullptr;
-        cudaMalloc(&d_tr, 16 * sizeof(unsigned long long));
-        cudaMemset(d_tr, 0, 16 * sizeof(unsigned long long));
-        q.trace = d_tr;
-        cudaDeviceSynchronize();
-        cudaEvent_t t0, t1;
-        cudaEventCreate(&t0); cudaEventCreate(&t1);
-        cudaEventRecord(t0, 0);
-        s = real();
-        cudaEventRecord(t1, 0);
-        cudaEventSynchronize(t1);
-        float one = 0.f;
-        cudaEventElapsedTime(&one, t0, t1);
-        unsigned long long h[16];
-        cudaMemcpy(h, d_tr, sizeof(h), cudaMemcpyDeviceToHost);
-        if (a_mn)
-          fprintf(stderr, "[trace] M=%d N=%d K=%d bn=%d split=%d single-launch %.2f us | ns since entry:", M, N, K, pl.bn, pl.split_k,
-                  one * 1e3f);
-        else
-          fprintf(stderr, "[trace] M=%d N=%d K=%d ping-pong bm_wg=%d bn=%d single-launch %.2f us | ns since entry:", M, N, K, pp.bm_wg,
-                  pp.bn, one * 1e3f);
-        const char* nm[9] = {"entry", "setup", "deps", "tma0", "land0", "mma_done", "acc_ready", "epi_done", "exit"};
-        for (int i = 1; i < 9; ++i) fprintf(stderr, " %s=%lld", nm[i], (long long)(h[i] - h[0]));
-        fprintf(stderr, "\n");
-        cudaEventDestroy(t0); cudaEventDestroy(t1);
-        cudaFree(d_tr);
-        q.trace = nullptr;
-      }
-      cudaFree(d_bias); cudaFree(d_colsum); cudaFree(d_out); cudaFree(d_aux);
-    }
-  }
-  if (s == SB_OK) {
-    cudaError_t e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) s = set_error(SB_ERR_CUDA, "gemm_tc_kernel failed: %s", cudaGetErrorString(e));
-    else if (cudaMemcpy(D, dD, sizeof(float) * M * N, cudaMemcpyDeviceToHost) != cudaSuccess) s = set_error(SB_ERR_CUDA, "D2H failed");
-  }
-  cudaFree(dA32); cudaFree(dB32); cudaFree(dD); cudaFree(dA); cudaFree(dB);
-  return s;
-}
-
-extern "C" {
-
-// D[M,N] = A[M,K] B[N,K]^T with every fp32 operand value split into `np` bf16 parts (np = 1: plain bf16)
-int sb_debug_gemm_split(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K, int32_t np, int device) {
-  SB_CHECK(A && B && D && M > 0 && N > 0 && K > 0 && np >= 1 && np <= 3, SB_ERR_INVALID, "bad argument");
-  int n_dev = 0;
-  SB_CHECK(cudaGetDeviceCount(&n_dev) == cudaSuccess && n_dev > 0, SB_ERR_CUDA, "no CUDA device available");
-  cudaDeviceProp prop;
-  SB_CUDA(cudaGetDeviceProperties(&prop, device));
-  SB_CHECK(prop.major == 9 && prop.minor == 0, SB_ERR_CUDA, "device is sm_%d%d, need sm_90", prop.major, prop.minor);
-  SB_CUDA(cudaSetDevice(device));
-  const int ld = round_up(K, 8);
-  const long long a_ps = static_cast<long long>(M) * ld, b_ps = static_cast<long long>(N) * ld;
-  float *dA32 = nullptr, *dB32 = nullptr, *dD = nullptr;
-  __nv_bfloat16 *dA = nullptr, *dB = nullptr;
-  SB_CUDA(cudaMalloc(&dA32, sizeof(float) * M * K));
-  SB_CUDA(cudaMalloc(&dB32, sizeof(float) * N * K));
-  SB_CUDA(cudaMalloc(&dD, sizeof(float) * M * N));
-  SB_CUDA(cudaMalloc(&dA, sizeof(__nv_bfloat16) * a_ps * np));
-  SB_CUDA(cudaMalloc(&dB, sizeof(__nv_bfloat16) * b_ps * np));
-  SB_CUDA(cudaMemset(dA, 0, sizeof(__nv_bfloat16) * a_ps * np));
-  SB_CUDA(cudaMemset(dB, 0, sizeof(__nv_bfloat16) * b_ps * np));
-  SB_CUDA(cudaMemset(dD, 0, sizeof(float) * M * N));
-  SB_CUDA(cudaMemcpy(dA32, A, sizeof(float) * M * K, cudaMemcpyHostToDevice));
-  SB_CUDA(cudaMemcpy(dB32, B, sizeof(float) * N * K, cudaMemcpyHostToDevice));
-  cast_bf16_kernel<<<static_cast<unsigned>((static_cast<long long>(M) * K + 255) / 256), 256>>>(dA32, M, K, dA, ld, np, a_ps);
-  cast_bf16_kernel<<<static_cast<unsigned>((static_cast<long long>(N) * K + 255) / 256), 256>>>(dB32, N, K, dB, ld, np, b_ps);
-  GemmTcParams p = {};
-  set_part_pairs(&p, np);
-  p.M = M; p.N = N; p.K = K;
-  p.accum = dD; p.ld_acc = N;
-  const GemmPlan pl = plan_gemm(M, N, round_up(K, 64) * p.n_pairs, prop.multiProcessorCount, false);
-  TmapSet tms;
-  int s = make_tmaps_bf16(tms.a, dA, a_ps, np, M, K, ld, 128);
-  if (s == SB_OK) s = make_tmaps_bf16(tms.b, dB, b_ps, np, N, K, ld, pl.bn);
-  if (s == SB_OK) s = set_gemm_tc_attrs<EPI_F32, false, false>();
-  if (s == SB_OK) s = launch_gemm_tc<EPI_F32, false, false>(pl, tms, p, 0);
-  if (s == SB_OK) {
-    cudaError_t e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) s = set_error(SB_ERR_CUDA, "gemm_tc_kernel (split) failed: %s", cudaGetErrorString(e));
-    else if (cudaMemcpy(D, dD, sizeof(float) * M * N, cudaMemcpyDeviceToHost) != cudaSuccess) s = set_error(SB_ERR_CUDA, "D2H failed");
-  }
-  cudaFree(dA32); cudaFree(dB32); cudaFree(dD); cudaFree(dA); cudaFree(dB);
-  return s;
-}
-
-int sb_debug_gemm_bf16_ex(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K, int32_t split_k,
-                          int32_t a_mn, int32_t b_mn, int device) {
-  return sb_debug_gemm_bf16_cfg(A, B, D, M, N, K, split_k, a_mn, b_mn, 0, 0, device);
-}
-int sb_debug_gemm_bf16(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K, int32_t split_k, int device) {
-  return sb_debug_gemm_bf16_cfg(A, B, D, M, N, K, split_k, 0, 0, 0, 0, device);
-}
-
-int sb_debug_gemm_epilogue(const float* A, const float* W, const float* bias, const float* aux, float* out, float* colsum,
-                           int32_t M, int32_t N, int32_t K, int32_t da, int32_t act, int32_t bm_wg, int device,
-                           int32_t iters, float* ms_out) {
-  SB_CHECK(A && W && out && M > 0 && N > 0 && K > 0 && (da == 0 || da == 1), SB_ERR_INVALID, "bad argument");
-  SB_CHECK(da ? aux != nullptr : bias != nullptr, SB_ERR_INVALID, "the forward GEMM needs a bias, the dA GEMM an aux matrix");
-  SB_CHECK(act >= SB_ACT_NONE && act <= SB_ACT_LEAKYRELU, SB_ERR_INVALID, "act invalid");
-  SB_CHECK(bm_wg == 0 || bm_wg == 64 || bm_wg == 128 || bm_wg == PP_TILE_WIDE, SB_ERR_INVALID,
-           "bm_wg must be 0, 64, 128 or %d (got %d)", PP_TILE_WIDE, bm_wg);
-  SB_CHECK(!(da && bm_wg == PP_TILE_WIDE), SB_ERR_INVALID, "the %d-wide tile is for the forward GEMM only", PP_TILE_WIDE);
-  SB_CHECK(iters >= 0 && (iters == 0 || ms_out != nullptr), SB_ERR_INVALID, "iters / ms_out");
-  int n_dev = 0;
-  SB_CHECK(cudaGetDeviceCount(&n_dev) == cudaSuccess && n_dev > 0, SB_ERR_CUDA, "no CUDA device available");
-  cudaDeviceProp prop;
-  SB_CUDA(cudaGetDeviceProperties(&prop, device));
-  SB_CHECK(prop.major == 9 && prop.minor == 0, SB_ERR_CUDA, "device is sm_%d%d, need sm_90", prop.major, prop.minor);
-  SB_CUDA(cudaSetDevice(device));
-  // stored shapes: A [M, K]; W [K, N] (forward, MN-major operand) or [N, K] (dA, K-major operand)
-  const int w_rows = da ? N : K, w_cols = da ? K : N;
-  const int lda = round_up(K, 8), ldw = round_up(w_cols, 8), ldn = round_up(N, 8);
-  const size_t mn = static_cast<size_t>(M) * N;
-  float *dA32 = nullptr, *dW32 = nullptr, *dX32 = nullptr, *d_bias = nullptr, *d_col = nullptr;
-  __nv_bfloat16 *dA = nullptr, *dW = nullptr, *d_out = nullptr, *d_aux = nullptr;
-  SB_CUDA(cudaMalloc(&dA32, sizeof(float) * M * K));
-  SB_CUDA(cudaMalloc(&dW32, sizeof(float) * N * K));
-  SB_CUDA(cudaMalloc(&dX32, sizeof(float) * mn));
-  SB_CUDA(cudaMalloc(&d_bias, sizeof(float) * N));
-  SB_CUDA(cudaMalloc(&d_col, sizeof(float) * N));
-  SB_CUDA(cudaMalloc(&dA, sizeof(__nv_bfloat16) * M * lda));
-  SB_CUDA(cudaMalloc(&dW, sizeof(__nv_bfloat16) * w_rows * ldw));
-  SB_CUDA(cudaMalloc(&d_out, sizeof(__nv_bfloat16) * M * ldn));
-  SB_CUDA(cudaMalloc(&d_aux, sizeof(__nv_bfloat16) * M * ldn));
-  SB_CUDA(cudaMemset(dA, 0, sizeof(__nv_bfloat16) * M * lda));
-  SB_CUDA(cudaMemset(dW, 0, sizeof(__nv_bfloat16) * w_rows * ldw));
-  SB_CUDA(cudaMemset(d_out, 0, sizeof(__nv_bfloat16) * M * ldn));
-  SB_CUDA(cudaMemset(d_aux, 0, sizeof(__nv_bfloat16) * M * ldn));
-  SB_CUDA(cudaMemset(d_bias, 0, sizeof(float) * N));
-  SB_CUDA(cudaMemset(d_col, 0, sizeof(float) * N));
-  SB_CUDA(cudaMemcpy(dA32, A, sizeof(float) * M * K, cudaMemcpyHostToDevice));
-  SB_CUDA(cudaMemcpy(dW32, W, sizeof(float) * N * K, cudaMemcpyHostToDevice));
-  if (bias) SB_CUDA(cudaMemcpy(d_bias, bias, sizeof(float) * N, cudaMemcpyHostToDevice));
-  cast_bf16_kernel<<<static_cast<unsigned>((static_cast<long long>(M) * K + 255) / 256), 256>>>(dA32, M, K, dA, lda);
-  cast_bf16_kernel<<<static_cast<unsigned>((static_cast<long long>(N) * K + 255) / 256), 256>>>(dW32, w_rows, w_cols, dW, ldw);
-  if (aux) {
-    SB_CUDA(cudaMemcpy(dX32, aux, sizeof(float) * mn, cudaMemcpyHostToDevice));
-    cast_bf16_kernel<<<static_cast<unsigned>((mn + 255) / 256), 256>>>(dX32, M, N, d_aux, ldn);
-  }
-  const PpPlan pp = plan_gemm_pp(M, N, K, prop.multiProcessorCount, da == 0, bm_wg);
-  PpTmaps pt;
-  int s = make_tmap_bf16(&pt.a, dA, M, K, lda, pp.bm_wg);
-  if (s == SB_OK) s = make_tmap_bf16(&pt.b, dW, w_rows, w_cols, ldw, da ? pp.bn : 64);
-  if (s == SB_OK) s = make_tmap_bf16(&pt.o, d_out, M, N, ldn, pp.bm_wg);
-  if (s == SB_OK) s = make_tmap_bf16(&pt.x, d_aux, M, N, ldn, pp.bm_wg);
-  GemmTcParams p = {};
-  p.M = M; p.N = N; p.K = K;
-  p.act = act; p.bias = d_bias; p.colsum = colsum ? d_col : nullptr;
-  auto launch = [&]() {
-    if (da) return launch_gemm_pp<EPI_DA>(pp, pt, p, 0, false);
-    return pp.bn == 256 ? launch_gemm_wide(pp, pt, p, 0, false) : launch_gemm_pp<EPI_FWD>(pp, pt, p, 0, false);
-  };
-  if (s == SB_OK) s = pp.bn == 256 ? set_gemm_wide_attrs() : set_gemm_pp_attrs();
-  if (s == SB_OK) s = launch();
-  if (s == SB_OK) {
-    cudaError_t e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) s = set_error(SB_ERR_CUDA, "%s failed: %s", pp.bn == 256 ? "gemm_wide_kernel" : "gemm_pp_kernel", cudaGetErrorString(e));
-  }
-  if (s == SB_OK) {
-    std::vector<uint16_t> h(static_cast<size_t>(M) * ldn);
-    if (cudaMemcpy(h.data(), d_out, sizeof(uint16_t) * h.size(), cudaMemcpyDeviceToHost) != cudaSuccess) s = set_error(SB_ERR_CUDA, "D2H failed");
-    for (int r = 0; r < M && s == SB_OK; ++r)
-      for (int c = 0; c < N; ++c) {
-        const uint32_t u = static_cast<uint32_t>(h[static_cast<size_t>(r) * ldn + c]) << 16;   // bf16 -> fp32, exact
-        memcpy(out + static_cast<size_t>(r) * N + c, &u, 4);
-      }
-    if (s == SB_OK && colsum && cudaMemcpy(colsum, d_col, sizeof(float) * N, cudaMemcpyDeviceToHost) != cudaSuccess)
-      s = set_error(SB_ERR_CUDA, "D2H failed");
-  }
-  if (s == SB_OK && iters > 0) {
-    cudaEvent_t e0, e1;
-    cudaEventCreate(&e0); cudaEventCreate(&e1);
-    for (int i = 0; i < 3 && s == SB_OK; ++i) s = launch();
-    cudaEventRecord(e0, 0);
-    for (int i = 0; i < iters && s == SB_OK; ++i) s = launch();
-    cudaEventRecord(e1, 0);
-    cudaEventSynchronize(e1);
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, e0, e1);
-    *ms_out = ms / iters;
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    cudaError_t e = cudaDeviceSynchronize();
-    if (s == SB_OK && e != cudaSuccess) s = set_error(SB_ERR_CUDA, "gemm_pp_kernel failed: %s", cudaGetErrorString(e));
-  }
-  cudaFree(dA32); cudaFree(dW32); cudaFree(dX32); cudaFree(d_bias); cudaFree(d_col);
-  cudaFree(dA); cudaFree(dW); cudaFree(d_out); cudaFree(d_aux);
-  return s;
-}
-
-int sb_debug_gemm_fwd_out(const float* A, const float* W, const float* bias, const float* wo, float bo, const float* y,
-                          const float* w, float* dZ, float* g_bL, float* g_wo, float* g_bo, float* loss_sum, int32_t* guard,
-                          int32_t M, int32_t N, int32_t K, int32_t a_rows, int32_t row0, int32_t act, int32_t loss,
-                          int32_t np, int32_t grid, int device) {
-  SB_CHECK(A && W && bias && wo && y && w && dZ && g_bL && g_wo && g_bo && loss_sum && guard, SB_ERR_INVALID, "null argument");
-  SB_CHECK(M > 0 && K > 0 && N >= 1 && N <= FWD_OUT_MAX_N, SB_ERR_INVALID, "M=%d K=%d N=%d (N must be 1..%d)", M, K, N,
-           FWD_OUT_MAX_N);
-  SB_CHECK(np >= 1 && np <= 3, SB_ERR_INVALID, "np=%d outside 1..3", np);
-  SB_CHECK(loss == SB_LOSS_MSE || loss == SB_LOSS_SIGMOID_CE, SB_ERR_INVALID, "loss invalid");
-  SB_CHECK(act >= SB_ACT_NONE && act <= SB_ACT_LEAKYRELU, SB_ERR_INVALID, "act invalid");
-  SB_CHECK(grid >= 0, SB_ERR_INVALID, "grid=%d", grid);
-  SB_CHECK(row0 >= 0 && static_cast<long long>(row0) + M <= a_rows, SB_ERR_INVALID, "rows %d..%d outside the %d rows of A", row0,
-           row0 + M - 1, a_rows);
-  int n_dev = 0;
-  SB_CHECK(cudaGetDeviceCount(&n_dev) == cudaSuccess && n_dev > 0, SB_ERR_CUDA, "no CUDA device available");
-  cudaDeviceProp prop;
-  SB_CUDA(cudaGetDeviceProperties(&prop, device));
-  SB_CHECK(prop.major == 9 && prop.minor == 0, SB_ERR_CUDA, "device is sm_%d%d, need sm_90", prop.major, prop.minor);
-  SB_CHECK(grid <= prop.multiProcessorCount, SB_ERR_INVALID, "grid=%d above the %d SMs", grid, prop.multiProcessorCount);
-  SB_CUDA(cudaSetDevice(device));
-  // the step's layout: parts one after the other, rows of ld = round_up(cols, 8) elements; dZ has 64 guard rows per part
-  const int lda = round_up(K, 8), ldn = round_up(N, 8), dz_rows = M + 64;
-  const long long a_ps = static_cast<long long>(a_rows) * lda, w_ps = static_cast<long long>(K) * ldn;
-  const long long dz_ps = static_cast<long long>(dz_rows) * ldn;
-  const long long a_n = static_cast<long long>(a_rows) * K, w_n = static_cast<long long>(K) * N;
-  float *dA32 = nullptr, *dW32 = nullptr, *d_vec = nullptr, *d_yw = nullptr;
-  __nv_bfloat16 *dA = nullptr, *dW = nullptr, *d_dz = nullptr;
-  BatchDesc* d_desc = nullptr;
-  SB_CUDA(cudaMalloc(&dA32, sizeof(float) * a_n));
-  SB_CUDA(cudaMalloc(&dW32, sizeof(float) * w_n));
-  SB_CUDA(cudaMalloc(&dA, sizeof(__nv_bfloat16) * a_ps * np));
-  SB_CUDA(cudaMalloc(&dW, sizeof(__nv_bfloat16) * w_ps * np));
-  SB_CUDA(cudaMalloc(&d_dz, sizeof(__nv_bfloat16) * dz_ps * np));
-  // [bias N][w_o N][db_L N][dw_o N][b_o][db_o][scal SCAL_COUNT]
-  SB_CUDA(cudaMalloc(&d_vec, sizeof(float) * (4 * N + 2 + SCAL_COUNT)));
-  SB_CUDA(cudaMalloc(&d_yw, sizeof(float) * 2 * M));
-  SB_CUDA(cudaMalloc(&d_desc, sizeof(BatchDesc)));
-  float* d_bias = d_vec;
-  float* d_wo = d_vec + N;
-  float* d_gbL = d_vec + 2 * N;
-  float* d_gwo = d_vec + 3 * N;
-  float* d_bo = d_vec + 4 * N;
-  float* d_gbo = d_bo + 1;
-  float* d_scal = d_bo + 2;
-  SB_CUDA(cudaMemset(dA, 0, sizeof(__nv_bfloat16) * a_ps * np));
-  SB_CUDA(cudaMemset(dW, 0, sizeof(__nv_bfloat16) * w_ps * np));
-  SB_CUDA(cudaMemset(d_dz, 0x7f, sizeof(__nv_bfloat16) * dz_ps * np));   // every element the bf16 sentinel 0x7f7f
-  SB_CUDA(cudaMemcpy(dA32, A, sizeof(float) * a_n, cudaMemcpyHostToDevice));
-  SB_CUDA(cudaMemcpy(dW32, W, sizeof(float) * w_n, cudaMemcpyHostToDevice));
-  float nnz = 0.f;
-  for (int r = 0; r < M; ++r) nnz += (w[r] != 0.f) ? 1.f : 0.f;
-  std::vector<float> h_vec(4 * N + 2 + SCAL_COUNT, 0.f);
-  std::copy(bias, bias + N, h_vec.begin());
-  std::copy(wo, wo + N, h_vec.begin() + N);
-  std::copy(g_bL, g_bL + N, h_vec.begin() + 2 * N);
-  std::copy(g_wo, g_wo + N, h_vec.begin() + 3 * N);
-  h_vec[4 * N] = bo;
-  h_vec[4 * N + 1] = *g_bo;
-  h_vec[4 * N + 2 + SCAL_LOSS_SUM] = *loss_sum;
-  h_vec[4 * N + 2 + SCAL_NNZ] = nnz;
-  SB_CUDA(cudaMemcpy(d_vec, h_vec.data(), sizeof(float) * h_vec.size(), cudaMemcpyHostToDevice));
-  SB_CUDA(cudaMemcpy(d_yw, y, sizeof(float) * M, cudaMemcpyHostToDevice));
-  SB_CUDA(cudaMemcpy(d_yw + M, w, sizeof(float) * M, cudaMemcpyHostToDevice));
-  BatchDesc h_desc = {};
-  h_desc.y = d_yw; h_desc.w = d_yw + M; h_desc.gscale = 1.f; h_desc.row0 = row0;
-  SB_CUDA(cudaMemcpy(d_desc, &h_desc, sizeof(BatchDesc), cudaMemcpyHostToDevice));
-  cast_bf16_kernel<<<static_cast<unsigned>((a_n + 255) / 256), 256>>>(dA32, a_rows, K, dA, lda, np, a_ps);
-  cast_bf16_kernel<<<static_cast<unsigned>((w_n + 255) / 256), 256>>>(dW32, K, N, dW, ldn, np, w_ps);
-  // the launch of Net::enqueue_hidden_forward's fused branch
-  const bool resident = row0 != 0 || a_rows != M;
-  FwdOutTmaps ft;
-  int s = make_tmaps_bf16(ft.a, dA, a_ps, np, a_rows, K, lda, 64);
-  if (s == SB_OK) s = make_tmaps_bf16(ft.b, dW, w_ps, np, K, N, ldn, 64);
-  if (s == SB_OK) s = make_tmaps_bf16(ft.o, d_dz, dz_ps, np, M, N, ldn, 64);
-  GemmTcParams p = {};
-  set_part_pairs(&p, np);
-  p.M = M; p.N = N; p.K = K;
-  p.bias = d_bias; p.act = act;
-  p.a_rows = resident ? d_desc : nullptr;
-  p.wo = d_wo; p.bo = d_bo;
-  p.desc = d_desc; p.scal = d_scal; p.loss = loss;
-  p.g_wo = d_gwo; p.g_bo = d_gbo; p.g_bL = d_gbL;
-  const int tiles = (M + 63) / 64;
-  const int step_grid = tiles < prop.multiProcessorCount ? tiles : prop.multiProcessorCount;
-  if (s == SB_OK) s = set_gemm_fwd_out_attrs();
-  if (s == SB_OK) s = launch_gemm_fwd_out(grid > 0 ? grid : step_grid, ft, p, 0, false);
-  if (s == SB_OK) {
-    cudaError_t e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) s = set_error(SB_ERR_CUDA, "gemm_fwd_out_kernel failed: %s", cudaGetErrorString(e));
-  }
-  std::vector<uint16_t> h(static_cast<size_t>(dz_ps) * np);
-  if (s == SB_OK && (cudaMemcpy(h.data(), d_dz, sizeof(uint16_t) * h.size(), cudaMemcpyDeviceToHost) != cudaSuccess ||
-                     cudaMemcpy(h_vec.data(), d_vec, sizeof(float) * h_vec.size(), cudaMemcpyDeviceToHost) != cudaSuccess))
-    s = set_error(SB_ERR_CUDA, "D2H failed");
-  if (s == SB_OK) {
-    int32_t changed = 0;
-    for (int k = 0; k < np; ++k)
-      for (int r = 0; r < dz_rows; ++r)
-        for (int c = 0; c < ldn; ++c) {
-          const uint16_t v = h[static_cast<size_t>(k * dz_ps) + static_cast<size_t>(r) * ldn + c];
-          if (r < M && c < N) {
-            const uint32_t u = static_cast<uint32_t>(v) << 16;   // bf16 -> fp32, exact
-            memcpy(dZ + (static_cast<size_t>(k) * M + r) * N + c, &u, 4);
-          } else if (v != 0x7f7f && (r >= M || (v & 0x7fff) != 0)) {
-            // the bulk tensor store writes a row's last 16-byte piece whole, so the pad columns of a batch row may
-            // receive the tile's +-0 beyond N; anything else, or any write into the guard rows, is counted
-            ++changed;
-          }
-        }
-    *guard = changed;
-    std::copy(h_vec.begin() + 2 * N, h_vec.begin() + 3 * N, g_bL);
-    std::copy(h_vec.begin() + 3 * N, h_vec.begin() + 4 * N, g_wo);
-    *g_bo = h_vec[4 * N + 1];
-    *loss_sum = h_vec[4 * N + 2 + SCAL_LOSS_SUM];
-  }
-  cudaFree(dA32); cudaFree(dW32); cudaFree(dA); cudaFree(dW); cudaFree(d_dz); cudaFree(d_vec); cudaFree(d_yw); cudaFree(d_desc);
-  return s;
 }
 
 }  // extern "C"

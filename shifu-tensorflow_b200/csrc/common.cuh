@@ -6,6 +6,7 @@
 #include <stdio.h>
 #include <string>
 #include <type_traits>
+#include <utility>
 
 #include "../../include/shifu_b200.h"
 
@@ -33,6 +34,25 @@ int set_error(int code, const char* fmt, ...);
     int _s = (expr);          \
     if (_s != SB_OK) return _s; \
   } while (0)
+
+// A device allocation of n T that is freed when its owner goes out of scope
+template <typename T>
+struct DevBuf {
+  T* p = nullptr;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  DevBuf(DevBuf&& o) noexcept : p(o.p) { o.p = nullptr; }
+  DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p, o.p); return *this; }
+  ~DevBuf() { if (p) cudaFree(p); }
+  int alloc(size_t n) {
+    SB_CHECK(p == nullptr, SB_ERR_STATE, "DevBuf allocated twice");
+    void* q = nullptr;
+    SB_CUDA(cudaMalloc(&q, n * sizeof(T)));
+    p = static_cast<T*>(q);
+    return SB_OK;
+  }
+};
 
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }

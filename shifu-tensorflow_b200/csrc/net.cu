@@ -1,5 +1,6 @@
 // Net: device state + kernel sequencing for the tabular-DNN forward / backward.
 // Mirrors generate_from_modelconf + model (res/ssgd_monitor.py:91-144) as a list of fused launches.
+// Also the kernel-level test hooks (sb_debug_gemm_*), so that every GEMM kernel is compiled in this one translation unit.
 #include <stdarg.h>
 #include <stdlib.h>
 #include <string.h>
@@ -131,6 +132,7 @@ int validate_desc(const sb_net_desc* d) {
   return SB_OK;
 }
 
+// makes `device` current if it is an sm_90 device
 static int check_device(int device, int* num_sms) {
   int n = 0;
   cudaError_t e = cudaGetDeviceCount(&n);
@@ -142,6 +144,7 @@ static int check_device(int device, int* num_sms) {
   SB_CHECK(prop.major == 9 && prop.minor == 0, SB_ERR_CUDA, "device %d is sm_%d%d; this library is built for sm_90a only",
            device, prop.major, prop.minor);
   *num_sms = prop.multiProcessorCount;
+  SB_CUDA(cudaSetDevice(device));
   return SB_OK;
 }
 
@@ -151,7 +154,6 @@ int Net::init(const sb_net_desc* d, int device_, bool training_) {
   device = device_;
   training = training_;
   const bool want_trace = getenv("SB_STEP_TRACE") != nullptr;
-  SB_CUDA(cudaSetDevice(device));
   // the main chain is the critical path: its CTAs are scheduled ahead of the trainer's side stream's (dW GEMMs, second
   // optimizer)
   int prio_least = 0, prio_greatest = 0;
@@ -286,12 +288,12 @@ int Net::init(const sb_net_desc* d, int device_, bool training_) {
   return SB_OK;
 }
 
-void Net::destroy() {
+Net::~Net() {
+  if (!stream && allocs.empty()) return;    // init never got to the device
+  cudaSetDevice(device);
   if (stream) cudaStreamSynchronize(stream);
   for (void* p : allocs) cudaFree(p);
-  allocs.clear();
   if (stream) cudaStreamDestroy(stream);
-  stream = nullptr;
 }
 
 int Net::set_sparse(int n_dense_, int n_onehot_, int n_cat_) {
@@ -555,4 +557,363 @@ int Net::enqueue_da(int l, int rows, float* grad) {
   mark("gemm_da");
   return SB_OK;
 }
+
+// ================================================================================================
+// kernel-level test hooks: one GEMM of the step on fp32 host operands, through the launches above
+// ================================================================================================
+template <typename T>
+static int alloc_filled(DevBuf<T>* b, size_t n, int byte = 0) {
+  SB_TRY(b->alloc(n));
+  SB_CUDA(cudaMemset(b->p, byte, sizeof(T) * n));
+  return SB_OK;
+}
+
+// fp32 host [rows, cols] -> np bf16 parts on the device, each [rows, round_up(cols, 8)] with zero padding, one behind the other
+static int upload_bf16(DevBuf<__nv_bfloat16>* dst, const float* src, int rows, int cols, int np = 1) {
+  const int ld = round_up(cols, 8);
+  const long long ps = static_cast<long long>(rows) * ld, n = static_cast<long long>(rows) * cols;
+  SB_TRY(alloc_filled(dst, static_cast<size_t>(ps) * np));
+  DevBuf<float> f32;
+  SB_TRY(f32.alloc(n));
+  SB_CUDA(cudaMemcpy(f32.p, src, sizeof(float) * n, cudaMemcpyHostToDevice));
+  cast_bf16_kernel<<<static_cast<unsigned>((n + 255) / 256), 256>>>(f32.p, rows, cols, dst->p, ld, np, ps);
+  SB_CUDA(cudaGetLastError());
+  return SB_OK;
+}
+
+// np bf16 parts of part_stride elements on the device, rows of round_up(cols, 8) -> fp32 host [np, rows, cols] (widening
+// is exact); raw keeps every part's bits, padding included
+static int download_bf16(float* dst, const __nv_bfloat16* src, int rows, int cols, int np, long long part_stride,
+                         std::vector<uint16_t>& raw) {
+  const int ld = round_up(cols, 8);
+  raw.resize(static_cast<size_t>(part_stride) * np);
+  SB_CUDA(cudaMemcpy(raw.data(), src, sizeof(uint16_t) * raw.size(), cudaMemcpyDeviceToHost));
+  for (int k = 0; k < np; ++k)
+    for (int r = 0; r < rows; ++r)
+      for (int c = 0; c < cols; ++c) {
+        const uint32_t u = static_cast<uint32_t>(raw[static_cast<size_t>(k * part_stride) + static_cast<size_t>(r) * ld + c]) << 16;
+        memcpy(dst + (static_cast<size_t>(k) * rows + r) * cols + c, &u, 4);
+      }
+  return SB_OK;
+}
+
+static int sync_hook(const char* kernel) {
+  const cudaError_t e = cudaDeviceSynchronize();
+  SB_CHECK(e == cudaSuccess, SB_ERR_CUDA, "%s failed: %s", kernel, cudaGetErrorString(e));
+  return SB_OK;
+}
+
+// average device milliseconds per launch over `iters` back-to-back launches after `warmup` ones (CUDA events on the
+// legacy stream)
+template <typename Launch>
+static int time_launches(Launch&& launch, int warmup, int iters, float* ms_out) {
+  struct Events {
+    cudaEvent_t e[2] = {};
+    ~Events() { for (cudaEvent_t x : e) if (x) cudaEventDestroy(x); }
+  } ev;
+  SB_CUDA(cudaEventCreate(&ev.e[0]));
+  SB_CUDA(cudaEventCreate(&ev.e[1]));
+  for (int i = 0; i < warmup; ++i) SB_TRY(launch());
+  SB_CUDA(cudaEventRecord(ev.e[0], 0));
+  for (int i = 0; i < iters; ++i) SB_TRY(launch());
+  SB_CUDA(cudaEventRecord(ev.e[1], 0));
+  SB_CUDA(cudaEventSynchronize(ev.e[1]));
+  float ms = 0.f;
+  SB_CUDA(cudaEventElapsedTime(&ms, ev.e[0], ev.e[1]));
+  *ms_out = ms / iters;
+  return SB_OK;
+}
+
+static int debug_gemm_impl(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K, int32_t split_k,
+                           int32_t a_mn, int32_t b_mn, int32_t cfg_cg, int32_t cfg_bn, int device, int iters, float* ms_out) {
+  SB_CHECK(cfg_cg == 0 || (cfg_cg == 1 && (cfg_bn == 64 || cfg_bn == 128 || (cfg_bn == 256 && a_mn && b_mn))), SB_ERR_INVALID,
+           "tile configuration cg=%d bn=%d not instantiated for this layout (bn=256: MM only)", cfg_cg, cfg_bn);
+  SB_CHECK(A && B && D && M > 0 && N > 0 && K > 0, SB_ERR_INVALID, "bad argument");
+  SB_CHECK((a_mn == 0 && b_mn == 0) || (a_mn == 0 && b_mn == 1) || (a_mn == 1 && b_mn == 1), SB_ERR_INVALID,
+           "layout combination not instantiated (use KK, KM or MM)");
+  int sms = 0;
+  SB_TRY(check_device(device, &sms));
+  // stored shapes: K-major [R, K]; MN-major [K, R]
+  const int a_rows = a_mn ? K : M, a_cols = a_mn ? M : K;
+  const int b_rows = b_mn ? K : N, b_cols = b_mn ? N : K;
+  const int lda = round_up(a_cols, 8), ldb = round_up(b_cols, 8);
+  DevBuf<__nv_bfloat16> dA, dB;
+  DevBuf<float> dD;
+  SB_TRY(upload_bf16(&dA, A, a_rows, a_cols));
+  SB_TRY(upload_bf16(&dB, B, b_rows, b_cols));
+  SB_TRY(alloc_filled(&dD, static_cast<size_t>(M) * N));
+  GemmPlan pl = plan_gemm(M, N, K, sms, false);
+  if (cfg_cg > 0) pl.bn = cfg_bn;  // explicit tile configuration requested by the test
+  {
+    const int total_kb = (K + 63) / 64;
+    int want = split_k < 1 ? 1 : (split_k > total_kb ? total_kb : split_k);
+    pl.kb_per_split = (total_kb + want - 1) / want;
+    pl.split_k = (total_kb + pl.kb_per_split - 1) / pl.kb_per_split;
+    const int work = ((M + 127) / 128) * ((N + pl.bn - 1) / pl.bn) * pl.split_k;
+    pl.grid = work < sms ? work : sms;
+  }
+  TmapSet tms;
+  SB_TRY(make_tmap_bf16(&tms.a[0], dA.p, a_rows, a_cols, lda, a_mn ? 64 : 128));
+  SB_TRY(make_tmap_bf16(&tms.b[0], dB.p, b_rows, b_cols, ldb, b_mn ? 64 : pl.bn));
+  GemmTcParams p = {};
+  p.M = M; p.N = N; p.K = K;
+  p.accum = dD.p; p.ld_acc = N;
+  p.acc_vec4 = (N % 4 == 0) ? 1 : 0;
+  // 256-wide tiles (MM, the dW layout, only): the dW kernel, whose red.add into the zeroed D is the product
+  if (pl.bn == 256) {
+    SB_TRY(set_gemm_dw_attrs());
+    SB_TRY(launch_gemm_dw(pl, tms, p, 0));
+  } else if (!a_mn && !b_mn) {
+    SB_TRY((set_gemm_tc_attrs<EPI_F32, false, false>()));
+    SB_TRY((launch_gemm_tc<EPI_F32, false, false>(pl, tms, p, 0)));
+  } else if (!a_mn) {
+    SB_TRY((set_gemm_tc_attrs<EPI_F32, false, true>()));
+    SB_TRY((launch_gemm_tc<EPI_F32, false, true>(pl, tms, p, 0)));
+  } else {
+    SB_TRY((set_gemm_tc_attrs<EPI_F32, true, true>()));
+    SB_TRY((launch_gemm_tc<EPI_F32, true, true>(pl, tms, p, 0)));
+  }
+  if (iters > 0) {
+    // benchmark with the REAL epilogue of the layout's use: KM -> forward (bias + relu -> bf16), KK -> dA
+    // (act' * , bf16 store, column sums), MM -> dW (fp32 red.add)
+    const int ldn = round_up(N, 8);
+    DevBuf<float> d_bias, d_colsum;
+    DevBuf<__nv_bfloat16> d_out, d_aux;
+    SB_TRY(alloc_filled(&d_bias, N));
+    SB_TRY(alloc_filled(&d_colsum, N));
+    SB_TRY(d_out.alloc(static_cast<size_t>(M) * ldn));
+    SB_TRY(alloc_filled(&d_aux, static_cast<size_t>(M) * ldn, 0x3f));
+    GemmTcParams q = p;
+    q.bias = d_bias.p; q.act = SB_ACT_RELU; q.out = d_out.p; q.ld_out = ldn; q.aux = d_aux.p; q.ld_aux = ldn; q.colsum = d_colsum.p;
+    // KM / KK: the kernel the step plans for the shape
+    const PpPlan pp = plan_gemm_pp(M, N, K, sms, !a_mn && b_mn);
+    PpTmaps pt;
+    if (!a_mn) {
+      SB_TRY(make_tmap_bf16(&pt.a, dA.p, a_rows, a_cols, lda, pp.bm_wg));
+      SB_TRY(make_tmap_bf16(&pt.b, dB.p, b_rows, b_cols, ldb, b_mn ? 64 : pp.bn));
+      SB_TRY(make_tmap_bf16(&pt.o, d_out.p, M, N, ldn, pp.bm_wg));
+      SB_TRY(make_tmap_bf16(&pt.x, d_aux.p, M, N, ldn, pp.bm_wg));
+    }
+    auto real = [&]() -> int {
+      if (!a_mn && !b_mn) return launch_gemm_pp<EPI_DA>(pp, pt, q, 0, false);
+      if (!a_mn) return pp.bn == 256 ? launch_gemm_wide(pp, pt, q, 0, false) : launch_gemm_pp<EPI_FWD>(pp, pt, q, 0, false);
+      if (pl.bn == 256) return launch_gemm_dw(pl, tms, q, 0, false);
+      return launch_gemm_tc<EPI_DW, true, true>(pl, tms, q, 0, false);
+    };
+    SB_TRY((a_mn ? set_gemm_tc_attrs<EPI_DW, true, true>() : set_gemm_pp_attrs()));
+    if (pp.bn == 256) SB_TRY(set_gemm_wide_attrs());
+    SB_TRY(time_launches(real, 3, iters, ms_out));
+    if (getenv("SB_GEMM_TRACE")) {
+      // one more launch with %globaltimer stamps from CTA 0 (ns relative to kernel entry), and the host-visible
+      // launch-to-completion time of a single isolated launch
+      DevBuf<unsigned long long> d_tr;
+      SB_TRY(alloc_filled(&d_tr, 16));
+      q.trace = d_tr.p;
+      SB_CUDA(cudaDeviceSynchronize());
+      float one = 0.f;
+      SB_TRY(time_launches(real, 0, 1, &one));
+      unsigned long long h[16];
+      SB_CUDA(cudaMemcpy(h, d_tr.p, sizeof(h), cudaMemcpyDeviceToHost));
+      if (a_mn)
+        fprintf(stderr, "[trace] M=%d N=%d K=%d bn=%d split=%d single-launch %.2f us | ns since entry:", M, N, K, pl.bn, pl.split_k,
+                one * 1e3f);
+      else
+        fprintf(stderr, "[trace] M=%d N=%d K=%d ping-pong bm_wg=%d bn=%d single-launch %.2f us | ns since entry:", M, N, K, pp.bm_wg,
+                pp.bn, one * 1e3f);
+      const char* nm[9] = {"entry", "setup", "deps", "tma0", "land0", "mma_done", "acc_ready", "epi_done", "exit"};
+      for (int i = 1; i < 9; ++i) fprintf(stderr, " %s=%lld", nm[i], (long long)(h[i] - h[0]));
+      fprintf(stderr, "\n");
+    }
+  }
+  SB_TRY(sync_hook("gemm_tc_kernel"));
+  SB_CUDA(cudaMemcpy(D, dD.p, sizeof(float) * M * N, cudaMemcpyDeviceToHost));
+  return SB_OK;
+}
 }  // namespace sb
+
+using namespace sb;
+
+extern "C" {
+
+int sb_debug_gemm_bf16_cfg(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K, int32_t split_k,
+                           int32_t a_mn, int32_t b_mn, int32_t cfg_cg, int32_t cfg_bn, int device) {
+  return debug_gemm_impl(A, B, D, M, N, K, split_k, a_mn, b_mn, cfg_cg, cfg_bn, device, 0, nullptr);
+}
+int sb_debug_gemm_bench(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K, int32_t split_k,
+                        int32_t a_mn, int32_t b_mn, int32_t cfg_cg, int32_t cfg_bn, int device, int32_t iters, float* ms_out) {
+  SB_CHECK(iters > 0 && ms_out, SB_ERR_INVALID, "iters / ms_out");
+  return debug_gemm_impl(A, B, D, M, N, K, split_k, a_mn, b_mn, cfg_cg, cfg_bn, device, iters, ms_out);
+}
+
+// D[M,N] = A[M,K] B[N,K]^T with every fp32 operand value split into `np` bf16 parts (np = 1: plain bf16)
+int sb_debug_gemm_split(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K, int32_t np, int device) {
+  SB_CHECK(A && B && D && M > 0 && N > 0 && K > 0 && np >= 1 && np <= 3, SB_ERR_INVALID, "bad argument");
+  int sms = 0;
+  SB_TRY(check_device(device, &sms));
+  const int ld = round_up(K, 8);
+  const long long a_ps = static_cast<long long>(M) * ld, b_ps = static_cast<long long>(N) * ld;
+  DevBuf<__nv_bfloat16> dA, dB;
+  DevBuf<float> dD;
+  SB_TRY(upload_bf16(&dA, A, M, K, np));
+  SB_TRY(upload_bf16(&dB, B, N, K, np));
+  SB_TRY(alloc_filled(&dD, static_cast<size_t>(M) * N));
+  GemmTcParams p = {};
+  set_part_pairs(&p, np);
+  p.M = M; p.N = N; p.K = K;
+  p.accum = dD.p; p.ld_acc = N;
+  const GemmPlan pl = plan_gemm(M, N, round_up(K, 64) * p.n_pairs, sms, false);
+  TmapSet tms;
+  SB_TRY(make_tmaps_bf16(tms.a, dA.p, a_ps, np, M, K, ld, 128));
+  SB_TRY(make_tmaps_bf16(tms.b, dB.p, b_ps, np, N, K, ld, pl.bn));
+  SB_TRY((set_gemm_tc_attrs<EPI_F32, false, false>()));
+  SB_TRY((launch_gemm_tc<EPI_F32, false, false>(pl, tms, p, 0)));
+  SB_TRY(sync_hook("gemm_tc_kernel (split)"));
+  SB_CUDA(cudaMemcpy(D, dD.p, sizeof(float) * M * N, cudaMemcpyDeviceToHost));
+  return SB_OK;
+}
+
+int sb_debug_gemm_epilogue(const float* A, const float* W, const float* bias, const float* aux, float* out, float* colsum,
+                           int32_t M, int32_t N, int32_t K, int32_t da, int32_t act, int32_t bm_wg, int device,
+                           int32_t iters, float* ms_out) {
+  SB_CHECK(A && W && out && M > 0 && N > 0 && K > 0 && (da == 0 || da == 1), SB_ERR_INVALID, "bad argument");
+  SB_CHECK(da ? aux != nullptr : bias != nullptr, SB_ERR_INVALID, "the forward GEMM needs a bias, the dA GEMM an aux matrix");
+  SB_CHECK(act >= SB_ACT_NONE && act <= SB_ACT_LEAKYRELU, SB_ERR_INVALID, "act invalid");
+  SB_CHECK(bm_wg == 0 || bm_wg == 64 || bm_wg == 128 || bm_wg == PP_TILE_WIDE, SB_ERR_INVALID,
+           "bm_wg must be 0, 64, 128 or %d (got %d)", PP_TILE_WIDE, bm_wg);
+  SB_CHECK(!(da && bm_wg == PP_TILE_WIDE), SB_ERR_INVALID, "the %d-wide tile is for the forward GEMM only", PP_TILE_WIDE);
+  SB_CHECK(iters >= 0 && (iters == 0 || ms_out != nullptr), SB_ERR_INVALID, "iters / ms_out");
+  int sms = 0;
+  SB_TRY(check_device(device, &sms));
+  // stored shapes: A [M, K]; W [K, N] (forward, MN-major operand) or [N, K] (dA, K-major operand)
+  const int w_rows = da ? N : K, w_cols = da ? K : N;
+  const int lda = round_up(K, 8), ldw = round_up(w_cols, 8), ldn = round_up(N, 8);
+  DevBuf<__nv_bfloat16> dA, dW, d_out, d_aux;
+  DevBuf<float> d_bias, d_col;
+  SB_TRY(upload_bf16(&dA, A, M, K));
+  SB_TRY(upload_bf16(&dW, W, w_rows, w_cols));
+  SB_TRY(alloc_filled(&d_out, static_cast<size_t>(M) * ldn));
+  SB_TRY(aux ? upload_bf16(&d_aux, aux, M, N) : alloc_filled(&d_aux, static_cast<size_t>(M) * ldn));
+  SB_TRY(alloc_filled(&d_bias, N));
+  SB_TRY(alloc_filled(&d_col, N));
+  if (bias) SB_CUDA(cudaMemcpy(d_bias.p, bias, sizeof(float) * N, cudaMemcpyHostToDevice));
+  const PpPlan pp = plan_gemm_pp(M, N, K, sms, da == 0, bm_wg);
+  PpTmaps pt;
+  SB_TRY(make_tmap_bf16(&pt.a, dA.p, M, K, lda, pp.bm_wg));
+  SB_TRY(make_tmap_bf16(&pt.b, dW.p, w_rows, w_cols, ldw, da ? pp.bn : 64));
+  SB_TRY(make_tmap_bf16(&pt.o, d_out.p, M, N, ldn, pp.bm_wg));
+  SB_TRY(make_tmap_bf16(&pt.x, d_aux.p, M, N, ldn, pp.bm_wg));
+  GemmTcParams p = {};
+  p.M = M; p.N = N; p.K = K;
+  p.act = act; p.bias = d_bias.p; p.colsum = colsum ? d_col.p : nullptr;
+  auto launch = [&]() {
+    if (da) return launch_gemm_pp<EPI_DA>(pp, pt, p, 0, false);
+    return pp.bn == 256 ? launch_gemm_wide(pp, pt, p, 0, false) : launch_gemm_pp<EPI_FWD>(pp, pt, p, 0, false);
+  };
+  const char* kernel = pp.bn == 256 ? "gemm_wide_kernel" : "gemm_pp_kernel";
+  SB_TRY(pp.bn == 256 ? set_gemm_wide_attrs() : set_gemm_pp_attrs());
+  SB_TRY(launch());
+  SB_TRY(sync_hook(kernel));
+  std::vector<uint16_t> h;
+  SB_TRY(download_bf16(out, d_out.p, M, N, 1, static_cast<long long>(M) * ldn, h));
+  if (colsum) SB_CUDA(cudaMemcpy(colsum, d_col.p, sizeof(float) * N, cudaMemcpyDeviceToHost));
+  if (iters > 0) {
+    SB_TRY(time_launches(launch, 3, iters, ms_out));
+    SB_TRY(sync_hook(kernel));
+  }
+  return SB_OK;
+}
+
+int sb_debug_gemm_fwd_out(const float* A, const float* W, const float* bias, const float* wo, float bo, const float* y,
+                          const float* w, float* dZ, float* g_bL, float* g_wo, float* g_bo, float* loss_sum, int32_t* guard,
+                          int32_t M, int32_t N, int32_t K, int32_t a_rows, int32_t row0, int32_t act, int32_t loss,
+                          int32_t np, int32_t grid, int device) {
+  SB_CHECK(A && W && bias && wo && y && w && dZ && g_bL && g_wo && g_bo && loss_sum && guard, SB_ERR_INVALID, "null argument");
+  SB_CHECK(M > 0 && K > 0 && N >= 1 && N <= FWD_OUT_MAX_N, SB_ERR_INVALID, "M=%d K=%d N=%d (N must be 1..%d)", M, K, N,
+           FWD_OUT_MAX_N);
+  SB_CHECK(np >= 1 && np <= 3, SB_ERR_INVALID, "np=%d outside 1..3", np);
+  SB_CHECK(loss == SB_LOSS_MSE || loss == SB_LOSS_SIGMOID_CE, SB_ERR_INVALID, "loss invalid");
+  SB_CHECK(act >= SB_ACT_NONE && act <= SB_ACT_LEAKYRELU, SB_ERR_INVALID, "act invalid");
+  SB_CHECK(grid >= 0, SB_ERR_INVALID, "grid=%d", grid);
+  SB_CHECK(row0 >= 0 && static_cast<long long>(row0) + M <= a_rows, SB_ERR_INVALID, "rows %d..%d outside the %d rows of A", row0,
+           row0 + M - 1, a_rows);
+  int sms = 0;
+  SB_TRY(check_device(device, &sms));
+  SB_CHECK(grid <= sms, SB_ERR_INVALID, "grid=%d above the %d SMs", grid, sms);
+  // the step's layout: parts one after the other, rows of ld = round_up(cols, 8) elements; dZ has 64 guard rows per part
+  const int lda = round_up(K, 8), ldn = round_up(N, 8), dz_rows = M + 64;
+  const long long a_ps = static_cast<long long>(a_rows) * lda, w_ps = static_cast<long long>(K) * ldn;
+  const long long dz_ps = static_cast<long long>(dz_rows) * ldn;
+  DevBuf<__nv_bfloat16> dA, dW, d_dz;
+  DevBuf<float> d_vec, d_yw;
+  DevBuf<BatchDesc> d_desc;
+  SB_TRY(upload_bf16(&dA, A, a_rows, K, np));
+  SB_TRY(upload_bf16(&dW, W, K, N, np));
+  SB_TRY(alloc_filled(&d_dz, static_cast<size_t>(dz_ps) * np, 0x7f));   // every element the bf16 sentinel 0x7f7f
+  // [bias N][w_o N][db_L N][dw_o N][b_o][db_o][scal SCAL_COUNT]
+  float nnz = 0.f;
+  for (int r = 0; r < M; ++r) nnz += (w[r] != 0.f) ? 1.f : 0.f;
+  std::vector<float> h_vec(4 * N + 2 + SCAL_COUNT, 0.f);
+  std::copy(bias, bias + N, h_vec.begin());
+  std::copy(wo, wo + N, h_vec.begin() + N);
+  std::copy(g_bL, g_bL + N, h_vec.begin() + 2 * N);
+  std::copy(g_wo, g_wo + N, h_vec.begin() + 3 * N);
+  h_vec[4 * N] = bo;
+  h_vec[4 * N + 1] = *g_bo;
+  h_vec[4 * N + 2 + SCAL_LOSS_SUM] = *loss_sum;
+  h_vec[4 * N + 2 + SCAL_NNZ] = nnz;
+  SB_TRY(d_vec.alloc(h_vec.size()));
+  SB_CUDA(cudaMemcpy(d_vec.p, h_vec.data(), sizeof(float) * h_vec.size(), cudaMemcpyHostToDevice));
+  float* d_bias = d_vec.p;
+  float* d_wo = d_vec.p + N;
+  float* d_gbL = d_vec.p + 2 * N;
+  float* d_gwo = d_vec.p + 3 * N;
+  float* d_bo = d_vec.p + 4 * N;
+  float* d_gbo = d_bo + 1;
+  float* d_scal = d_bo + 2;
+  SB_TRY(d_yw.alloc(2 * static_cast<size_t>(M)));
+  SB_CUDA(cudaMemcpy(d_yw.p, y, sizeof(float) * M, cudaMemcpyHostToDevice));
+  SB_CUDA(cudaMemcpy(d_yw.p + M, w, sizeof(float) * M, cudaMemcpyHostToDevice));
+  BatchDesc h_desc = {};
+  h_desc.y = d_yw.p; h_desc.w = d_yw.p + M; h_desc.gscale = 1.f; h_desc.row0 = row0;
+  SB_TRY(d_desc.alloc(1));
+  SB_CUDA(cudaMemcpy(d_desc.p, &h_desc, sizeof(BatchDesc), cudaMemcpyHostToDevice));
+  // the launch of Net::enqueue_hidden_forward's fused branch
+  const bool resident = row0 != 0 || a_rows != M;
+  FwdOutTmaps ft;
+  SB_TRY(make_tmaps_bf16(ft.a, dA.p, a_ps, np, a_rows, K, lda, 64));
+  SB_TRY(make_tmaps_bf16(ft.b, dW.p, w_ps, np, K, N, ldn, 64));
+  SB_TRY(make_tmaps_bf16(ft.o, d_dz.p, dz_ps, np, M, N, ldn, 64));
+  GemmTcParams p = {};
+  set_part_pairs(&p, np);
+  p.M = M; p.N = N; p.K = K;
+  p.bias = d_bias; p.act = act;
+  p.a_rows = resident ? d_desc.p : nullptr;
+  p.wo = d_wo; p.bo = d_bo;
+  p.desc = d_desc.p; p.scal = d_scal; p.loss = loss;
+  p.g_wo = d_gwo; p.g_bo = d_gbo; p.g_bL = d_gbL;
+  const int tiles = (M + 63) / 64;
+  const int step_grid = tiles < sms ? tiles : sms;
+  SB_TRY(set_gemm_fwd_out_attrs());
+  SB_TRY(launch_gemm_fwd_out(grid > 0 ? grid : step_grid, ft, p, 0, false));
+  SB_TRY(sync_hook("gemm_fwd_out_kernel"));
+  std::vector<uint16_t> h;
+  SB_TRY(download_bf16(dZ, d_dz.p, M, N, np, dz_ps, h));
+  SB_CUDA(cudaMemcpy(h_vec.data(), d_vec.p, sizeof(float) * h_vec.size(), cudaMemcpyDeviceToHost));
+  int32_t changed = 0;
+  for (int k = 0; k < np; ++k)
+    for (int r = 0; r < dz_rows; ++r)
+      for (int c = 0; c < ldn; ++c) {
+        const uint16_t v = h[static_cast<size_t>(k * dz_ps) + static_cast<size_t>(r) * ldn + c];
+        // the bulk tensor store writes a row's last 16-byte piece whole, so the pad columns of a batch row may receive
+        // the tile's +-0 beyond N; anything else, or any write into the guard rows, is counted
+        if ((r >= M || c >= N) && v != 0x7f7f && (r >= M || (v & 0x7fff) != 0)) ++changed;
+      }
+  *guard = changed;
+  std::copy(h_vec.begin() + 2 * N, h_vec.begin() + 3 * N, g_bL);
+  std::copy(h_vec.begin() + 3 * N, h_vec.begin() + 4 * N, g_wo);
+  *g_bo = h_vec[4 * N + 1];
+  *loss_sum = h_vec[4 * N + 2 + SCAL_LOSS_SUM];
+  return SB_OK;
+}
+
+}  // extern "C"

@@ -93,14 +93,17 @@ struct Net {
   template <typename T> int dalloc(T** p, size_t n) {
     void* q = nullptr;
     SB_CUDA(cudaMalloc(&q, n * sizeof(T) + 256));
-    SB_CUDA(cudaMemsetAsync(q, 0, n * sizeof(T) + 256, stream));
     allocs.push_back(q);
+    SB_CUDA(cudaMemsetAsync(q, 0, n * sizeof(T) + 256, stream));
     *p = reinterpret_cast<T*>(q);
     return SB_OK;
   }
 
+  Net() = default;
+  Net(const Net&) = delete;
+  Net& operator=(const Net&) = delete;
+  ~Net();   // waits for the stream, frees every allocation and the stream
   int init(const sb_net_desc* d, int device_, bool training_);
-  void destroy();
   int refresh_shadows();
   // forward through the hidden layers (A_0 = current batch -> A_L).  The load kernel clears clear[0, clear_n) on the way.
   int enqueue_load(const StepIn& in, int rows, float* clear = nullptr, long long clear_n = 0);
