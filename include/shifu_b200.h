@@ -287,9 +287,33 @@ int sb_savedmodel_read(const char* saved_model_dir, const char* input_name, cons
 int sb_debug_gemm_bf16_cfg(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K,
                            int32_t split_k, int32_t a_mn, int32_t b_mn, int32_t cfg_cg, int32_t cfg_bn, int device);
 
-/* D = A B^T with every fp32 operand value held as np bf16 parts (np = 2: three part products, 3: six; see sb_precision):
- * the tensor-core parity GEMM behind SB_PREC_FP32_TC / SB_PREC_BF16X2. */
-int sb_debug_gemm_split(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K, int32_t np, int device);
+/* One forward (kind 0), dA (kind 1) or dW (kind 2) GEMM of a training step at `precision` (sb_precision), launched by the
+ * step's own per-layer launch code on a network built so that the GEMM is one of its layers: the step's planning, tensor
+ * maps, part pairs and kernel instantiations.  All matrices are fp32 row-major on the host; the tensor-core modes store
+ * them as np bf16 parts (np = 1 BF16, 2 BF16X2, 3 FP32_TC) split as the step splits them.  out receives [np, M, N]: each
+ * part's bf16 widened to fp32 (FP32: the fp32 values, one part).
+ *   kind 0: out = the parts of act(A[row0 .. row0 + M - 1] W + addend + bias).  A [a_rows, K], W [K, N], bias [N].
+ *           a_rows > M or row0 > 0: the batch is read at a row offset, as a step on the HBM-resident set reads it (tensor-
+ *           core modes).  addend [M, N] (nullable): a wide+deep step, whose layer 0 adds the embedding sums.
+ *           clear_n4 > 0 (tensor-core modes): the GEMM's idle producer warps clear a buffer of clear_n4 float4, as on a
+ *           resident step.
+ *   kind 1: out = the parts of (A W^T) * act'(aux), colsum[N] += its column sums.  A = dZ_l [M, K], W = W_l [N, K],
+ *           aux = A_{l-1} [M, N] (stored as np parts).
+ *   kind 2: grad[M, N] += A^T dZ over the K batch rows, rows r0 .. r1 - 1 only (an exchange chunk; r0 a multiple of 8,
+ *           FP32: the whole matrix).  A [a_rows, M] with the batch at row0 (resident as for kind 0), dZ passed in W [K, N].
+ * sms: the grid cap (the SMs a dW GEMM may take, or the Net's SM count for the forward and dA plans; a small value puts
+ * several tiles on each CTA); 0 = every SM.  route (nullable, route_cap bytes) receives the kernel and tile launched, e.g.
+ * "gemm_tc<128,DW>", "gemm_dw", "gemm_tc<64,FWD,GENERIC>", "gemm_pp<DA>", "gemm_wide", "gemm_f32<DA>".
+ * Before the launch the 64 rows past M of every output part and its pad columns N .. round_up(N, 8) - 1, the gradient
+ * outside its in/out region (kind 1: the column sums; kind 2: rows r0 .. r1 - 1) and 256 floats behind it, and the cleared
+ * buffer with 256 floats behind it are filled with a sentinel.  *guard returns how many of these changed, and how many
+ * floats of the cleared range are not +0, except that a pad column of a batch row may hold what the kernels store beyond N:
+ * kind 0 the parts of act(0) (the tile is 0 there), kind 1 +-0.  Every argument is checked before any device work; a bad
+ * one is SB_ERR_INVALID. */
+int sb_debug_gemm_layer(int32_t kind, int32_t precision, const float* A, const float* W, const float* bias, const float* aux,
+                        const float* addend, float* out, float* colsum, float* grad, int32_t* guard, char* route,
+                        int32_t route_cap, int32_t M, int32_t N, int32_t K, int32_t a_rows, int32_t row0, int32_t act,
+                        int32_t r0, int32_t r1, int32_t sms, int64_t clear_n4, int device);
 
 /* Timeline of the last step (trainer created with SB_STEP_TRACE=1 in the environment): for each GEMM launch of the
  * step, 16 %globaltimer stamps (ns) of its CTA 0: [0] entry, [1] setup done, [2] dependencies resolved, [3] first TMA

@@ -145,7 +145,9 @@ PROTOTYPES = {
                                            C.c_int64, _P(C.c_int64), _P(CellFlag), C.c_int64, _P(C.c_int64)]),
     "sb_savedmodel_write": (C.c_int, [_cp, _P(NetDesc), _f32p, C.c_int64]),
     "sb_savedmodel_read": (C.c_int, [_cp, _cp, _cp, _cp, _P(NetDesc), _P(C.c_int32), _f32p, C.c_int64, _P(C.c_int64)]),
-    "sb_debug_gemm_split": (C.c_int, [_f32p, _f32p, _f32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int]),
+    "sb_debug_gemm_layer": (C.c_int, [C.c_int32, C.c_int32, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _P(C.c_int32),
+                                      C.c_char_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                      C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_int]),
     "sb_debug_step_trace": (C.c_int, [_vp, C.POINTER(C.c_uint64), C.c_int32, C.c_char_p, C.c_int32, C.POINTER(C.c_int32)]),
     "sb_debug_gemm_bench": (C.c_int, [_f32p, _f32p, _f32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                       C.c_int32, C.c_int32, C.c_int, C.c_int32, _f32p]),
@@ -581,15 +583,66 @@ def debug_gemm_bf16(A: np.ndarray, B: np.ndarray, split_k: int = 1, device: int 
     return D
 
 
+GEMM_FWD, GEMM_DA, GEMM_DW = 0, 1, 2
+PARTS = {PREC_FP32: 1, PREC_BF16: 1, PREC_FP32_TC: 3, PREC_BF16X2: 2}
+
+
+def debug_gemm_layer(kind: int, precision: int, A: np.ndarray, W: np.ndarray, act: int = ACT_NONE,
+                     bias: Optional[np.ndarray] = None, aux: Optional[np.ndarray] = None, addend: Optional[np.ndarray] = None,
+                     colsum: Optional[np.ndarray] = None, grad: Optional[np.ndarray] = None, M: Optional[int] = None,
+                     row0: int = 0, r0: int = 0, r1: Optional[int] = None, sms: int = 0, clear_n4: int = 0, device: int = 0):
+    """One forward / dA / dW GEMM of a training step through the step's own launch code (sb_debug_gemm_layer):
+      GEMM_FWD: A [a_rows, K] (batch = rows row0 .. row0 + M - 1, M defaults to the rest), W [K, N], bias [N], addend [M, N]
+      GEMM_DA : A = dZ_l [M, K], W = W_l [N, K], aux = A_{l-1} [M, N], colsum [N] (in/out, zeros by default)
+      GEMM_DW : A [a_rows, M] (batch = rows row0 .. row0 + K - 1), W = dZ [K, N], grad [M, N] (in/out, zeros by default),
+                rows r0 .. r1 - 1 (r1 defaults to M)
+    -> (out [np, M, N] or None, colsum or None, grad or None, guard count, route name)"""
+    A, W = _f32(A), _f32(W)
+    nparts = PARTS[precision]
+    out = cs = g = None
+    if kind == GEMM_DW:
+        a_rows, Mx = A.shape
+        K, N = W.shape
+        if row0 + K > a_rows:
+            raise ValueError("the batch of K = %d rows at row0 = %d runs past A" % (K, row0))
+        g = np.zeros((Mx, N), np.float32) if grad is None else _f32(grad).copy()
+        a_rows_arg, M = a_rows, Mx
+    elif kind == GEMM_DA:
+        M, K = A.shape
+        N = W.shape[0]
+        assert W.shape == (N, K) and np.shape(aux) == (M, N)
+        cs = np.zeros(N, np.float32) if colsum is None else _f32(colsum).copy()
+        a_rows_arg = M
+    else:
+        a_rows_arg, K = A.shape
+        N = W.shape[1]
+        M = a_rows_arg - row0 if M is None else M
+    if kind != GEMM_DW:
+        out = np.zeros((nparts, M, N), np.float32)
+    bias = None if bias is None else _f32(bias)
+    aux = None if aux is None else _f32(aux)
+    addend = None if addend is None else _f32(addend)
+    guard = C.c_int32(-1)
+    route = C.create_string_buffer(64)
+    check(lib().sb_debug_gemm_layer(kind, precision, _ptr(A), _ptr(W), _ptr(bias), _ptr(aux), _ptr(addend), _ptr(out), _ptr(cs),
+                                    _ptr(g), C.byref(guard), route, 64, M, N, K, a_rows_arg, row0, act, r0,
+                                    M if r1 is None else r1, sms, clear_n4, device))
+    return out, cs, g, int(guard.value), route.value.decode()
+
+
 def debug_gemm_split(A: np.ndarray, B: np.ndarray, np_parts: int, device: int = 0) -> np.ndarray:
-    """D[M,N] = A[M,K] B[N,K]^T on the wgmma path with every fp32 value split into np_parts bf16 parts"""
+    """D[M,N] = A[M,K] B[N,K]^T with every fp32 value split into np_parts bf16 parts (1 = plain bf16): the forward GEMM of
+    a step in that precision (debug_gemm_layer, act none, zero bias), its stored parts summed in float64"""
+    prec = {1: PREC_BF16, 2: PREC_BF16X2, 3: PREC_FP32_TC}.get(np_parts)
+    if prec is None:
+        raise ShifuB200Error(SB_ERR_INVALID, "np_parts=%r outside 1..3" % (np_parts,))
     A, B = _f32(A), _f32(B)
-    M, K = A.shape
-    N, K2 = B.shape
-    assert K == K2
-    D = np.zeros((M, N), np.float32)
-    check(lib().sb_debug_gemm_split(_ptr(A), _ptr(B), _ptr(D), M, N, K, np_parts, device))
-    return D
+    assert A.shape[1] == B.shape[1]
+    out, _, _, guard, _ = debug_gemm_layer(GEMM_FWD, prec, A, B.T.copy(), ACT_NONE, bias=np.zeros(B.shape[0], np.float32),
+                                           device=device)
+    if guard != 0:
+        raise ShifuB200Error(SB_ERR_STATE, "%d sentinel elements around the output changed" % guard)
+    return out.astype(np.float64).sum(axis=0)
 
 
 def debug_gemm_bench(M: int, N: int, K: int, split_k: int = 1, a_mn: bool = False, b_mn: bool = False, cg: int = 0,

@@ -408,12 +408,18 @@ int Net::enqueue_hidden_forward(const StepIn& in, int rows, float* grad, bool* f
         SB_TRY(make_tmap_bf16(&pt.a, src, src_rows, k_in, ld_k, pp.bm_wg));
         pt.b = tm.b[0];
         SB_TRY(make_tmap_bf16(&pt.o, A[l], rows, ly.out, ly.ld_out, pp.bm_wg));
-        if (pp.bn == 256) SB_TRY(launch_gemm_wide(pp, pt, p, stream, true));
-        else SB_TRY(launch_gemm_pp<EPI_FWD>(pp, pt, p, stream, true));
+        if (pp.bn == 256) {
+          SB_TRY(launch_gemm_wide(pp, pt, p, stream, true));
+          mark("gemm_wide");
+        } else {
+          SB_TRY(launch_gemm_pp<EPI_FWD>(pp, pt, p, stream, true));
+          mark("gemm_pp<FWD>");
+        }
       } else {
         const GemmPlan pl = plan_gemm(rows, ly.out, round_up(k_in, 64) * pairs_of(nparts), num_sms, false);
         SB_TRY(make_tmaps_bf16(tm.a, src, src_ps, nparts, src_rows, k_in, ld_k, 128));
         SB_TRY((launch_gemm_tc<EPI_FWD, false, true>(pl, tm, p, stream, true)));
+        mark(pl.bn == 64 ? "gemm_tc<64,FWD,GENERIC>" : "gemm_tc<128,FWD,GENERIC>");
       }
     } else {
       GemmF32Params p = {};
@@ -424,8 +430,8 @@ int Net::enqueue_hidden_forward(const StepIn& in, int rows, float* grad, bool* f
       p.bias = theta + ly.b_off; p.act = ly.act;
       p.out = Af[l]; p.ld_out = ly.out;
       SB_TRY(launch_gemm_f32<EPI_FWD>(p, 1, stream));
+      mark("gemm_f32<FWD>");
     }
-    mark("gemm_fwd");
   }
   return SB_OK;
 }
@@ -487,7 +493,7 @@ int Net::enqueue_dw(const StepIn& in, int l, int rows, float* grad, cudaStream_t
     const int cap = (rows + 63) / 64;
     if (split > cap) split = cap;
     SB_TRY(launch_gemm_f32<EPI_DW>(p, split, st));
-    mark("gemm_dw");
+    mark("gemm_f32<DW>");
     return SB_OK;
   }
   // dW_l[in,out] += sum_rows A_{l-1}[rows,in] (MN-major A) * dZ_l[rows,out] (MN-major B), split-K over rows
@@ -508,9 +514,13 @@ int Net::enqueue_dw(const StepIn& in, int l, int rows, float* grad, cudaStream_t
   p.accum = grad + ly.w_off + static_cast<long long>(r0) * ly.out; p.ld_acc = ly.out;
   p.acc_vec4 = (ly.out % 4 == 0 && ly.w_off % 4 == 0) ? 1 : 0;
   p.trace = next_trace("dW", l, r1 - r0, ly.out, rows, chunk);
-  if (pl.bn == 256) SB_TRY(launch_gemm_dw(pl, tm, p, st, pdl));
-  else SB_TRY((launch_gemm_tc<EPI_DW, true, true>(pl, tm, p, st, pdl)));
-  mark("gemm_dw");
+  if (pl.bn == 256) {
+    SB_TRY(launch_gemm_dw(pl, tm, p, st, pdl));
+    mark("gemm_dw");
+  } else {
+    SB_TRY((launch_gemm_tc<EPI_DW, true, true>(pl, tm, p, st, pdl)));
+    mark(pl.bn == 64 ? "gemm_tc<64,DW>" : "gemm_tc<128,DW>");
+  }
   return SB_OK;
 }
 
@@ -527,7 +537,7 @@ int Net::enqueue_da(int l, int rows, float* grad) {
     p.out = dZf[l - 1]; p.ld_out = pl.out;
     p.colsum = grad + pl.b_off;
     SB_TRY(launch_gemm_f32<EPI_DA>(p, 1, stream));
-    mark("gemm_da");
+    mark("gemm_f32<DA>");
     return SB_OK;
   }
   // dZ_{l-1}[rows,in] = (dZ_l[rows,out] (K-major) x W_l[in,out] (K-major B: k = out contiguous)) .* act'(A_{l-1})
@@ -547,14 +557,15 @@ int Net::enqueue_da(int l, int rows, float* grad) {
     SB_TRY(make_tmap_bf16(&pt.o, dZ[l - 1], rows, ly.in, pl.ld_out, pp.bm_wg));
     SB_TRY(make_tmap_bf16(&pt.x, A[l - 1], rows, ly.in, pl.ld_out, pp.bm_wg));
     SB_TRY(launch_gemm_pp<EPI_DA>(pp, pt, p, stream, true));
+    mark("gemm_pp<DA>");
   } else {
     const GemmPlan gp = plan_gemm(rows, ly.in, round_up(ly.out, 64) * pairs_of(nparts), num_sms, false);
     TmapSet tm;
     SB_TRY(make_tmaps_bf16(tm.a, dZ[l], A_ps[l], nparts, rows, ly.out, ly.ld_out, 128));
     SB_TRY(make_tmaps_bf16(tm.b, ly.Wn, Wn_ps[l], nparts, ly.in, ly.out, ly.ld_out, gp.bn));
     SB_TRY((launch_gemm_tc<EPI_DA, false, false>(gp, tm, p, stream, true)));
+    mark(gp.bn == 64 ? "gemm_tc<64,DA,GENERIC>" : "gemm_tc<128,DA,GENERIC>");
   }
-  mark("gemm_da");
   return SB_OK;
 }
 
@@ -568,17 +579,24 @@ static int alloc_filled(DevBuf<T>* b, size_t n, int byte = 0) {
   return SB_OK;
 }
 
-// fp32 host [rows, cols] -> np bf16 parts on the device, each [rows, round_up(cols, 8)] with zero padding, one behind the other
-static int upload_bf16(DevBuf<__nv_bfloat16>* dst, const float* src, int rows, int cols, int np = 1) {
-  const int ld = round_up(cols, 8);
-  const long long ps = static_cast<long long>(rows) * ld, n = static_cast<long long>(rows) * cols;
-  SB_TRY(alloc_filled(dst, static_cast<size_t>(ps) * np));
+// fp32 host [rows, cols] -> np bf16 parts (bf16_residual, the step's split) into a device buffer: rows of ld elements, parts
+// ps elements apart; the pad columns are left as they are
+static int upload_parts(__nv_bfloat16* dst, const float* src, int rows, int cols, int ld, int np, long long ps) {
+  const long long n = static_cast<long long>(rows) * cols;
   DevBuf<float> f32;
   SB_TRY(f32.alloc(n));
   SB_CUDA(cudaMemcpy(f32.p, src, sizeof(float) * n, cudaMemcpyHostToDevice));
-  cast_bf16_kernel<<<static_cast<unsigned>((n + 255) / 256), 256>>>(f32.p, rows, cols, dst->p, ld, np, ps);
+  cast_bf16_kernel<<<static_cast<unsigned>((n + 255) / 256), 256>>>(f32.p, rows, cols, dst, ld, np, ps);
   SB_CUDA(cudaGetLastError());
   return SB_OK;
+}
+
+// fp32 host [rows, cols] -> np bf16 parts on the device, each [rows, round_up(cols, 8)] with zero padding, one behind the other
+static int upload_bf16(DevBuf<__nv_bfloat16>* dst, const float* src, int rows, int cols, int np = 1) {
+  const int ld = round_up(cols, 8);
+  const long long ps = static_cast<long long>(rows) * ld;
+  SB_TRY(alloc_filled(dst, static_cast<size_t>(ps) * np));
+  return upload_parts(dst->p, src, rows, cols, ld, np, ps);
 }
 
 // np bf16 parts of part_stride elements on the device, rows of round_up(cols, 8) -> fp32 host [np, rows, cols] (widening
@@ -745,30 +763,189 @@ int sb_debug_gemm_bench(const float* A, const float* B, float* D, int32_t M, int
   return debug_gemm_impl(A, B, D, M, N, K, split_k, a_mn, b_mn, cfg_cg, cfg_bn, device, iters, ms_out);
 }
 
-// D[M,N] = A[M,K] B[N,K]^T with every fp32 operand value split into `np` bf16 parts (np = 1: plain bf16)
-int sb_debug_gemm_split(const float* A, const float* B, float* D, int32_t M, int32_t N, int32_t K, int32_t np, int device) {
-  SB_CHECK(A && B && D && M > 0 && N > 0 && K > 0 && np >= 1 && np <= 3, SB_ERR_INVALID, "bad argument");
-  int sms = 0;
-  SB_TRY(check_device(device, &sms));
-  const int ld = round_up(K, 8);
-  const long long a_ps = static_cast<long long>(M) * ld, b_ps = static_cast<long long>(N) * ld;
-  DevBuf<__nv_bfloat16> dA, dB;
-  DevBuf<float> dD;
-  SB_TRY(upload_bf16(&dA, A, M, K, np));
-  SB_TRY(upload_bf16(&dB, B, N, K, np));
-  SB_TRY(alloc_filled(&dD, static_cast<size_t>(M) * N));
-  GemmTcParams p = {};
-  set_part_pairs(&p, np);
-  p.M = M; p.N = N; p.K = K;
-  p.accum = dD.p; p.ld_acc = N;
-  const GemmPlan pl = plan_gemm(M, N, round_up(K, 64) * p.n_pairs, sms, false);
-  TmapSet tms;
-  SB_TRY(make_tmaps_bf16(tms.a, dA.p, a_ps, np, M, K, ld, 128));
-  SB_TRY(make_tmaps_bf16(tms.b, dB.p, b_ps, np, N, K, ld, pl.bn));
-  SB_TRY((set_gemm_tc_attrs<EPI_F32, false, false>()));
-  SB_TRY((launch_gemm_tc<EPI_F32, false, false>(pl, tms, p, 0)));
-  SB_TRY(sync_hook("gemm_tc_kernel (split)"));
-  SB_CUDA(cudaMemcpy(D, dD.p, sizeof(float) * M * N, cudaMemcpyDeviceToHost));
+// One forward, dA or dW GEMM of a training step, launched by the step's own Net::enqueue_* code on a Net built so that the
+// GEMM is one of its layers (see shifu_b200.h)
+int sb_debug_gemm_layer(int32_t kind, int32_t precision, const float* A, const float* W, const float* bias, const float* aux,
+                        const float* addend, float* out, float* colsum, float* grad, int32_t* guard, char* route,
+                        int32_t route_cap, int32_t M, int32_t N, int32_t K, int32_t a_rows, int32_t row0, int32_t act,
+                        int32_t r0, int32_t r1, int32_t sms, int64_t clear_n4, int device) {
+  enum { FWD = 0, DA = 1, DW = 2 };
+  SB_CHECK(kind >= FWD && kind <= DW, SB_ERR_INVALID, "kind=%d (0 forward, 1 dA, 2 dW)", kind);
+  SB_CHECK(precision >= SB_PREC_FP32 && precision <= SB_PREC_BF16X2, SB_ERR_INVALID, "precision=%d invalid", precision);
+  SB_CHECK(act >= SB_ACT_NONE && act <= SB_ACT_LEAKYRELU, SB_ERR_INVALID, "act=%d invalid", act);
+  SB_CHECK(M > 0 && N > 0 && K > 0, SB_ERR_INVALID, "M=%d N=%d K=%d", M, N, K);
+  SB_CHECK(A && W && guard && (route == nullptr || route_cap > 0), SB_ERR_INVALID, "null argument");
+  SB_CHECK(kind != FWD || (bias && out), SB_ERR_INVALID, "the forward GEMM needs bias and out");
+  SB_CHECK(kind != DA || (aux && out && colsum), SB_ERR_INVALID, "the dA GEMM needs aux, out and colsum");
+  SB_CHECK(kind != DW || grad, SB_ERR_INVALID, "the dW GEMM needs grad");
+  SB_CHECK(addend == nullptr || kind == FWD, SB_ERR_INVALID, "an addend belongs to the forward GEMM only");
+  const bool tc = precision != SB_PREC_FP32;
+  const int rows = kind == DW ? K : M;                  // batch rows
+  SB_CHECK(row0 >= 0 && static_cast<long long>(row0) + rows <= a_rows, SB_ERR_INVALID, "rows %d..%d outside the %d rows of A",
+           row0, row0 + rows - 1, a_rows);
+  const bool resident = row0 != 0 || a_rows != rows;
+  SB_CHECK(!resident || (tc && kind != DA && addend == nullptr), SB_ERR_INVALID,
+           "a resident batch is read by the layer-0 forward / dW GEMMs of a dense tensor-core step only");
+  if (kind == DW) {
+    SB_CHECK(r0 >= 0 && r0 < r1 && r1 <= M && r0 % 8 == 0, SB_ERR_INVALID, "rows r0=%d .. r1=%d of the %d-row gradient "
+             "(r0 a multiple of 8)", r0, r1, M);
+    SB_CHECK(tc || (r0 == 0 && r1 == M), SB_ERR_INVALID, "the fp32 dW GEMM has no row chunks");
+  }
+  SB_CHECK(clear_n4 >= 0 && (clear_n4 == 0 || (kind == FWD && tc)), SB_ERR_INVALID,
+           "clear_n4=%lld: the tensor-core forward GEMM only", static_cast<long long>(clear_n4));
+  SB_CHECK(sms >= 0, SB_ERR_INVALID, "sms=%d", sms);
+  int dev_sms = 0;
+  SB_TRY(check_device(device, &dev_sms));
+  SB_CHECK(sms <= dev_sms, SB_ERR_INVALID, "sms=%d above the %d SMs", sms, dev_sms);
+
+  // the net: forward = layer 0 (F = K, hidden [N]; a sparse step contracts the K dense columns of F = K + 1), dA = layer 1
+  // (hidden [N, K]), dW = layer 0 (F = M, hidden [N]).  64 rows past the batch in every activation part are guard rows.
+  sb_net_desc d = {};
+  d.n_features = kind == FWD ? (addend ? K + 1 : K) : (kind == DA ? 8 : M);
+  d.n_hidden = kind == DA ? 2 : 1;
+  d.hidden[0] = N; d.acts[0] = kind == DW ? SB_ACT_NONE : act;
+  d.hidden[1] = K; d.acts[1] = SB_ACT_NONE;
+  d.loss = SB_LOSS_MSE; d.optimizer = SB_OPT_SGD;
+  d.max_batch = kind == DW ? K : M + 64;
+  d.precision = precision;
+  constexpr int GUARD = 256;                            // floats behind the gradient / the cleared buffer
+  const uint32_t S32 = 0x7f7f7f7fu;                     // sentinels: fp32 3.4e38, bf16 3.4e38
+  const uint16_t S16 = 0x7f7f;
+  DevBuf<__nv_bfloat16> res;
+  DevBuf<float> g, clr;
+  Net net;                                              // (destroyed first: waits for its stream)
+  SB_TRY(net.init(&d, device, true));
+  if (sms > 0) net.num_sms = sms;
+  const int np = net.nparts;
+  if (addend) SB_TRY(net.set_sparse(K, 1, 1));
+  const Layer& l0 = net.layers[0];
+  // parameters: W and bias into theta, the bf16 shadows from there (set_params)
+  std::vector<float> theta(static_cast<size_t>(net.n_params), 0.f);
+  if (kind == FWD) {
+    std::copy(W, W + static_cast<size_t>(K) * N, theta.begin() + l0.w_off);
+    std::copy(bias, bias + N, theta.begin() + l0.b_off);
+  } else if (kind == DA) {
+    std::copy(W, W + static_cast<size_t>(N) * K, theta.begin() + net.layers[1].w_off);
+  }
+  SB_CUDA(cudaMemcpy(net.theta, theta.data(), sizeof(float) * theta.size(), cudaMemcpyHostToDevice));
+  BatchDesc hd = {};
+  hd.row0 = row0;
+  SB_CUDA(cudaMemcpy(net.desc, &hd, sizeof(hd), cudaMemcpyHostToDevice));
+  // the batch operand of layer 0: the staged batch, or the resident set
+  if (kind != DA) {
+    const int cols = kind == FWD ? K : M;
+    if (resident) {
+      net.resident_ps = static_cast<long long>(a_rows) * net.ldF;
+      net.resident_rows = a_rows;
+      SB_TRY(alloc_filled(&res, static_cast<size_t>(net.resident_ps) * np));
+      SB_TRY(upload_parts(res.p, A, a_rows, cols, net.ldF, np, net.resident_ps));
+      net.resident_Xb = res.p;
+    } else if (tc) {
+      SB_TRY(upload_parts(net.Xb, A, rows, cols, addend ? net.ldD : net.ldF, np, net.Xb_ps));
+    } else {
+      SB_CUDA(cudaMemcpy(net.Xf, A, sizeof(float) * rows * cols, cudaMemcpyHostToDevice));
+    }
+  }
+  if (addend)
+    SB_CUDA(cudaMemcpy2D(net.E, sizeof(float) * l0.ld_out, addend, sizeof(float) * N, sizeof(float) * N, M, cudaMemcpyHostToDevice));
+  if (kind == DA) {     // dZ_1 [M, K], A_0 [M, N]
+    if (tc) {
+      SB_TRY(upload_parts(net.dZ[1], A, M, K, net.layers[1].ld_out, np, net.A_ps[1]));
+      SB_TRY(upload_parts(net.A[0], aux, M, N, l0.ld_out, np, net.A_ps[0]));
+    } else {
+      SB_CUDA(cudaMemcpy(net.dZf[1], A, sizeof(float) * M * K, cudaMemcpyHostToDevice));
+      SB_CUDA(cudaMemcpy(net.Af[0], aux, sizeof(float) * M * N, cudaMemcpyHostToDevice));
+    }
+  }
+  if (kind == DW) {     // dZ_0 [K, N]
+    if (tc) SB_TRY(upload_parts(net.dZ[0], W, K, N, l0.ld_out, np, net.A_ps[0]));
+    else SB_CUDA(cudaMemcpy(net.dZf[0], W, sizeof(float) * K * N, cudaMemcpyHostToDevice));
+  }
+  // the output, with its guard rows and pad columns, filled with the sentinel
+  void* outp = nullptr;
+  size_t out_bytes = 0;
+  if (kind != DW) {
+    outp = tc ? static_cast<void*>(kind == FWD ? net.A[0] : net.dZ[0]) : static_cast<void*>(kind == FWD ? net.Af[0] : net.dZf[0]);
+    out_bytes = tc ? sizeof(__nv_bfloat16) * net.A_ps[0] * np : sizeof(float) * static_cast<size_t>(net.max_batch) * N;
+    SB_CUDA(cudaMemset(outp, 0x7f, out_bytes));
+  }
+  // the gradient: the in/out region (dA: the column sums = layer 0's bias slot; dW: rows r0 .. r1 - 1 of W_0's slot) holds
+  // the caller's values, everything else and GUARD floats behind it the sentinel
+  const size_t g_n = static_cast<size_t>(net.n_params) + GUARD;
+  std::vector<float> hg(g_n);
+  {
+    float s;
+    memcpy(&s, &S32, 4);
+    std::fill(hg.begin(), hg.end(), s);
+  }
+  auto in_region = [&](size_t i) {
+    if (kind == DA) return i >= static_cast<size_t>(l0.b_off) && i < static_cast<size_t>(l0.b_off) + N;
+    return i >= static_cast<size_t>(r0) * N && i < static_cast<size_t>(r1) * N;    // W_0 at offset 0
+  };
+  if (kind == DA) std::copy(colsum, colsum + N, hg.begin() + l0.b_off);
+  if (kind == DW) std::copy(grad + static_cast<size_t>(r0) * N, grad + static_cast<size_t>(r1) * N, hg.begin() + static_cast<size_t>(r0) * N);
+  if (kind != FWD) {
+    SB_TRY(g.alloc(g_n));
+    SB_CUDA(cudaMemcpy(g.p, hg.data(), sizeof(float) * g_n, cudaMemcpyHostToDevice));
+  }
+  const size_t clr_n = clear_n4 > 0 ? static_cast<size_t>(clear_n4) * 4 + GUARD : 0;
+  if (clear_n4 > 0) SB_TRY(alloc_filled(&clr, clr_n, 0x7f));
+  SB_CUDA(cudaDeviceSynchronize());     // the uploads above ran on the legacy stream, the net launches on its own
+
+  StepIn in;
+  in.desc = net.desc; in.scal = net.scal; in.resident = resident; in.sparse = addend != nullptr;
+  SB_TRY(net.refresh_shadows());
+  net.launches = 0;
+  if (kind == FWD) SB_TRY(net.enqueue_hidden_forward(in, M, nullptr, nullptr, reinterpret_cast<float4*>(clr.p), clear_n4));
+  else if (kind == DA) SB_TRY(net.enqueue_da(1, M, g.p));
+  else SB_TRY(net.enqueue_dw(in, 0, K, g.p, net.stream, false, sms > 0 ? sms : dev_sms, r0, r1));
+  SB_CHECK(net.launches == 1 && net.last_kernel != nullptr, SB_ERR_STATE, "%d GEMM launches", net.launches);
+  SB_TRY(sync_hook(net.last_kernel));
+  if (route) {
+    strncpy(route, net.last_kernel, static_cast<size_t>(route_cap) - 1);
+    route[route_cap - 1] = '\0';
+  }
+
+  int32_t changed = 0;
+  if (kind != DW) {
+    if (tc) {
+      std::vector<uint16_t> h;
+      SB_TRY(download_bf16(out, static_cast<const __nv_bfloat16*>(outp), M, N, np, net.A_ps[0], h));
+      // pad columns of a batch row may hold what the kernels store beyond N: forward the parts of act(0) (the tile is 0
+      // there), dA +-0
+      const uint16_t a0 = kind == FWD && act == SB_ACT_SIGMOID ? 0x3f00 : 0;     // bf16(0.5)
+      const int ld = l0.ld_out;
+      for (int k = 0; k < np; ++k)
+        for (int r = 0; r < M + 64; ++r)
+          for (int c = (r < M ? N : 0); c < ld; ++c) {
+            const uint16_t v = h[static_cast<size_t>(k * net.A_ps[0]) + static_cast<size_t>(r) * ld + c];
+            const uint16_t want = k == 0 ? a0 : 0;
+            const bool legit = r < M && (v == want || (want == 0 && v == 0x8000));
+            if (v != S16 && !legit) ++changed;
+          }
+    } else {
+      std::vector<uint32_t> h(static_cast<size_t>(M + 64) * N);
+      SB_CUDA(cudaMemcpy(h.data(), outp, sizeof(uint32_t) * h.size(), cudaMemcpyDeviceToHost));
+      memcpy(out, h.data(), sizeof(float) * M * N);
+      for (size_t i = static_cast<size_t>(M) * N; i < h.size(); ++i) changed += h[i] != S32;
+    }
+  }
+  if (kind != FWD) {
+    SB_CUDA(cudaMemcpy(hg.data(), g.p, sizeof(float) * g_n, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < g_n; ++i) {
+      uint32_t u;
+      memcpy(&u, &hg[i], 4);
+      if (!in_region(i) && u != S32) ++changed;
+    }
+    if (kind == DA) std::copy(hg.begin() + l0.b_off, hg.begin() + l0.b_off + N, colsum);
+    else std::copy(hg.begin() + static_cast<size_t>(r0) * N, hg.begin() + static_cast<size_t>(r1) * N, grad + static_cast<size_t>(r0) * N);
+  }
+  if (clear_n4 > 0) {
+    std::vector<uint32_t> h(clr_n);
+    SB_CUDA(cudaMemcpy(h.data(), clr.p, sizeof(uint32_t) * clr_n, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < clr_n; ++i) changed += i < clr_n - GUARD ? h[i] != 0u : h[i] != S32;
+  }
+  *guard = changed;
   return SB_OK;
 }
 

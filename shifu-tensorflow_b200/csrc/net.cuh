@@ -87,7 +87,9 @@ struct Net {
     trace_n = trace_k + 1;
     return step_trace + 16 * (trace_k++);
   }
-  void mark(const char* /*kernel*/) { ++launches; }
+  // every launch of an enqueue_* routine: `kernel` names the kernel and tile it launched (sb_debug_gemm_layer reports it)
+  const char* last_kernel = nullptr;
+  void mark(const char* kernel) { ++launches; last_kernel = kernel; }
 
   std::vector<void*> allocs;
   template <typename T> int dalloc(T** p, size_t n) {
