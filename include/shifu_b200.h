@@ -356,6 +356,36 @@ int sb_debug_gemm_fwd_out(const float* A, const float* W, const float* bias, con
                           int32_t M, int32_t N, int32_t K, int32_t a_rows, int32_t row0, int32_t act, int32_t loss,
                           int32_t np, int32_t grid, int device);
 
+/* ---- test hooks of the peer-memory gradient exchange (csrc/xchg_p2p.cuh), on a trainer with a peer table ---- */
+/* Read (write = 0) or write (1) one raw buffer of this rank's parameter arena, after waiting for the trainer's stream:
+ * which = SB_DEBUG_BUF_THETA / _S1 / _S2 / _GRAD: float[n_params] (no gather from the run owners: a non-owner's stale
+ * master and state stay visible); SB_DEBUG_BUF_SHADOW + l: the bf16 shadow of hidden layer l as uint16 bits
+ * [np, in, ld_out], pad columns out .. ld_out - 1 included (tensor-core modes only, else SB_ERR_STATE).  Writing theta
+ * leaves the shadows alone; write = 2 (theta only) also refreshes them.  A wrong length is SB_ERR_INVALID. */
+#define SB_DEBUG_BUF_THETA 0
+#define SB_DEBUG_BUF_S1 1
+#define SB_DEBUG_BUF_S2 2
+#define SB_DEBUG_BUF_GRAD 3
+#define SB_DEBUG_BUF_SHADOW 4
+int sb_debug_trainer_buffer(sb_trainer_t* t, int32_t which, void* host, int64_t n, int32_t write);
+/* Queue one exchange of the slots in slot_mask exactly as a step does, and return without waiting: the descriptor of
+ * the next update (global step + 1 and its lr_t, gradient scale `gscale` (0: 1 / world), epoch + 1), then the step's
+ * exchange launch on the trainer's stream - its slot and work tables, grid rule (alone: as the last launch of a step)
+ * and kernel choice.  grid > 0 replaces the grid rule.  Every rank of the peer table must queue the same exchange before
+ * any of them is waited for (sb_trainer_sync, which also reports a peer that never arrived).  *lr_t_out, *grid_out
+ * (nullable) receive the lr_t and grid used, route (route_cap bytes) the kernel launched, e.g. "xchg_ll<4>",
+ * "xchg_update<16>".  A mask outside the trainer's slots is SB_ERR_INVALID, no peer table SB_ERR_STATE; both are found
+ * before any device work. */
+int sb_debug_exchange(sb_trainer_t* t, int32_t slot_mask, float gscale, int32_t grid, int32_t alone, float* lr_t_out,
+                      int32_t* grid_out, char* route, int32_t route_cap);
+/* The exchange's ownership tables.  info[SB_DEBUG_XINFO_WORDS] = {slots, SMs, LL protocol, replicas share the device,
+ * rank, world, np, 0, slot_begin[8], slot_end[8]}.  work (nullable: query *n_work) receives SB_DEBUG_XWORK_WORDS int64
+ * per run of the optimizer's work table: {off, count, out_dim, mat_off, ld_out, np, hidden layer whose shadow the run
+ * refreshes or -1, part_stride}.  The runs of slot s are [slot_begin[s], slot_end[s]). */
+#define SB_DEBUG_XINFO_WORDS 24
+#define SB_DEBUG_XWORK_WORDS 8
+int sb_debug_exchange_layout(sb_trainer_t* t, int32_t* info, int32_t info_cap, int64_t* work, int64_t work_cap, int32_t* n_work);
+
 #ifdef __cplusplus
 }
 #endif

@@ -158,7 +158,14 @@ PROTOTYPES = {
     "sb_debug_gemm_fwd_out": (C.c_int, [_f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p,
                                         _P(C.c_int32), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                         C.c_int32, C.c_int32, C.c_int32, C.c_int]),
+    "sb_debug_trainer_buffer": (C.c_int, [_vp, C.c_int32, _vp, C.c_int64, C.c_int32]),
+    "sb_debug_exchange": (C.c_int, [_vp, C.c_int32, C.c_float, C.c_int32, C.c_int32, _f32p, _P(C.c_int32), C.c_char_p,
+                                    C.c_int32]),
+    "sb_debug_exchange_layout": (C.c_int, [_vp, _P(C.c_int32), C.c_int32, _P(C.c_int64), C.c_int64, _P(C.c_int32)]),
 }
+
+DEBUG_BUF_THETA, DEBUG_BUF_S1, DEBUG_BUF_S2, DEBUG_BUF_GRAD, DEBUG_BUF_SHADOW = 0, 1, 2, 3, 4
+DEBUG_XINFO_WORDS, DEBUG_XWORK_WORDS = 24, 8
 
 
 def lib():
@@ -466,6 +473,42 @@ class Trainer:
         k = C.c_int32()
         check(lib().sb_debug_step_trace(self._h, buf.ctypes.data_as(C.POINTER(C.c_uint64)), 32, names, 4096, C.byref(k)))
         return names.value.decode().split(","), buf[:k.value].copy()
+
+    # ---- exchange test hooks (sb_debug_trainer_buffer / sb_debug_exchange / sb_debug_exchange_layout) ----
+    def debug_buffer(self, which: int, value: Optional[np.ndarray] = None, n: Optional[int] = None,
+                     refresh_shadows: bool = False) -> Optional[np.ndarray]:
+        """value None: -> a copy of one raw arena buffer (which < DEBUG_BUF_SHADOW: float32 [n_params]; DEBUG_BUF_SHADOW + l:
+        the uint16 bits of hidden layer l's shadow, n values = np * in * ld_out).  Otherwise write `value` (float32 or
+        uint16 as read), refreshing the shadows from theta if asked."""
+        dtype = np.float32 if which < DEBUG_BUF_SHADOW else np.uint16
+        if value is None:
+            out = np.empty(self.n_params if n is None else n, dtype)
+            check(lib().sb_debug_trainer_buffer(self._h, which, out.ctypes.data_as(_vp), out.size, 0))
+            return out
+        value = np.ascontiguousarray(value, dtype=dtype).reshape(-1)
+        check(lib().sb_debug_trainer_buffer(self._h, which, value.ctypes.data_as(_vp), value.size, 2 if refresh_shadows else 1))
+        return None
+
+    def debug_exchange(self, slot_mask: int, gscale: float = 0.0, grid: int = 0, alone: bool = False):
+        """queue one exchange of the slots in slot_mask as a step does, without waiting -> (lr_t, grid, kernel name)"""
+        lr_t, g = C.c_float(), C.c_int32()
+        route = C.create_string_buffer(64)
+        check(lib().sb_debug_exchange(self._h, int(slot_mask), float(gscale), int(grid), int(alone), C.byref(lr_t), C.byref(g),
+                                      route, 64))
+        return float(lr_t.value), int(g.value), route.value.decode()
+
+    def debug_exchange_layout(self) -> dict:
+        info = (C.c_int32 * DEBUG_XINFO_WORDS)()
+        n = C.c_int32()
+        check(lib().sb_debug_exchange_layout(self._h, info, DEBUG_XINFO_WORDS, None, 0, C.byref(n)))
+        work = np.zeros((n.value, DEBUG_XWORK_WORDS), np.int64)
+        check(lib().sb_debug_exchange_layout(self._h, info, DEBUG_XINFO_WORDS, work.ctypes.data_as(_P(C.c_int64)), work.size,
+                                             C.byref(n)))
+        s = info[0]
+        return dict(slots=s, sms=info[1], ll=bool(info[2]), share_device=bool(info[3]), rank=info[4], world=info[5], np=info[6],
+                    begin=list(info[8:8 + s]), end=list(info[16:16 + s]),
+                    work=[dict(zip(("off", "count", "out_dim", "mat_off", "ld_out", "np", "layer", "part_stride"),
+                                   (int(v) for v in row))) for row in work])
 
     @property
     def global_step(self) -> int:

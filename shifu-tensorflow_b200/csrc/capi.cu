@@ -3,6 +3,7 @@
 // See include/shifu_b200.h for the contract and the reference call each entry point replaces.
 #include <math.h>
 #include <stdlib.h>
+#include <cmath>
 #include <string.h>
 #include <algorithm>
 #include <memory>
@@ -208,9 +209,32 @@ static XchgParams xchg_params(sb_trainer* t, const BatchDesc* desc) {
   return p;
 }
 
-// reduce-scatter -> owner update -> all-gather of the operands for the given segments (xchg_p2p.cuh); `g` must be t->grad
+// grid of an exchange launch over the slots of `slot_mask`
+static int xchg_grid(const sb_trainer* t, int slot_mask, bool alone) {
+  int runs = 0, all_runs = 0;      // owned runs of the launch (the largest share) / runs of the launch
+  for (int sl = 0; sl < t->x_slots; ++sl)
+    if ((slot_mask >> sl) & 1) {
+      runs += (t->x_end[sl] - t->x_begin[sl] + t->world - 1) / t->world;
+      all_runs += t->x_end[sl] - t->x_begin[sl];
+    }
+  const int U = t->world <= 2 ? 2 : 1;      // runs per block iteration of the update phase (xchg_update_kernel)
+  const int want = std::max((runs + U - 1) / U, (all_runs - runs + 3) / 4);   // ... and 4 per iteration of the gather phase
+  // one block per SM and launch.  A GEMM CTA takes a whole SM (registers and shared memory, gemm_tc.cuh), so exchange
+  // blocks run only on SMs no GEMM CTA holds and otherwise wait for GEMM CTAs to leave - those never wait for an exchange,
+  // so this cannot deadlock, only be slow.  The schedule below was tuned where an exchange block fitted beside a GEMM CTA;
+  // on H100 it has not been measured with more than one GPU.
+  // (alone: nothing but other exchange launches runs beside this one - two blocks per SM, all loads of a phase in one round)
+  int grid = t->xchg_blocks > 0 ? t->xchg_blocks : (alone ? 2 : 1) * t->net.num_sms;
+  if (t->peers_share_device && grid > 32) grid = 32;    // replicas on ONE device: leave registers to the replica being waited for
+  if (grid > want) grid = want;
+  if (grid < 1) grid = 1;
+  return grid;
+}
+
+// reduce-scatter -> owner update -> all-gather of the operands for the given segments (xchg_p2p.cuh); `g` must be t->grad.
+// grid > 0 replaces the grid rule (sb_debug_exchange).
 static int enqueue_xchg(sb_trainer* t, const StepIn& in, int slot_mask, cudaStream_t st, bool publish_scalars, bool pdl,
-                        bool alone = false) {
+                        bool alone = false, int grid = 0) {
   Net& n = t->net;
   XchgParams p = xchg_params(t, in.desc);
   p.slot_mask = slot_mask;
@@ -221,38 +245,23 @@ static int enqueue_xchg(sb_trainer* t, const StepIn& in, int slot_mask, cudaStre
   else if ((slot_mask & (slot_mask - 1)) == 0) snprintf(nm, sizeof(nm), "xchg_B%d", __builtin_ctz(slot_mask) - 1);
   else snprintf(nm, sizeof(nm), "xchg");
   p.trace = n.next_trace(nm);
-  int runs = 0, all_runs = 0;      // owned runs of the launch (the largest share) / runs of the launch
-  for (int sl = 0; sl < t->x_slots; ++sl)
-    if ((slot_mask >> sl) & 1) {
-      runs += (p.slot_end[sl] - p.slot_begin[sl] + t->world - 1) / t->world;
-      all_runs += p.slot_end[sl] - p.slot_begin[sl];
-    }
-  const int U = t->world <= 2 ? 2 : 1;      // runs per block iteration of the update phase (xchg_update_kernel)
-  const int want = std::max((runs + U - 1) / U, (all_runs - runs + 3) / 4);   // ... and 4 per iteration of the gather phase
-  // one block per SM and launch.  A GEMM CTA takes a whole SM (registers and shared memory, gemm_tc.cuh), so exchange
-  // blocks run only on SMs no GEMM CTA holds and otherwise wait for GEMM CTAs to leave - those never wait for an exchange,
-  // so this cannot deadlock, only be slow.  The schedule below was tuned where an exchange block fitted beside a GEMM CTA;
-  // on H100 it has not been measured with more than one GPU.
-  // (alone: nothing but other exchange launches runs beside this one - two blocks per SM, all loads of a phase in one round)
-  int grid = t->xchg_blocks > 0 ? t->xchg_blocks : (alone ? 2 : 1) * n.num_sms;
-  if (t->peers_share_device && grid > 32) grid = 32;    // replicas on ONE device: leave registers to the replica being waited for
-  if (grid > want) grid = want;
-  if (grid < 1) grid = 1;
+  if (grid <= 0) grid = xchg_grid(t, slot_mask, alone);
   const dim3 g(static_cast<unsigned>(grid)), b(256);
   // plain bf16: the LL protocol (flags inside the data) needs fewer fabric round trips than the flag-and-pull kernel
+  const char* kernel;
   if (t->ll_ready) {
     LLParams lp;
     lp.x = p; lp.llg_off = t->llg_off; lp.lls_off = t->lls_off; lp.n4 = t->xch_n4;
-    if (t->world <= 2) SB_TRY(launch_kernel(xchg_ll_kernel<2>, g, b, 0, st, pdl, lp));
-    else if (t->world <= 4) SB_TRY(launch_kernel(xchg_ll_kernel<4>, g, b, 0, st, pdl, lp));
-    else if (t->world <= 8) SB_TRY(launch_kernel(xchg_ll_kernel<8>, g, b, 0, st, pdl, lp));
-    else SB_TRY(launch_kernel(xchg_ll_kernel<16>, g, b, 0, st, pdl, lp));
+    if (t->world <= 2) { SB_TRY(launch_kernel(xchg_ll_kernel<2>, g, b, 0, st, pdl, lp)); kernel = "xchg_ll<2>"; }
+    else if (t->world <= 4) { SB_TRY(launch_kernel(xchg_ll_kernel<4>, g, b, 0, st, pdl, lp)); kernel = "xchg_ll<4>"; }
+    else if (t->world <= 8) { SB_TRY(launch_kernel(xchg_ll_kernel<8>, g, b, 0, st, pdl, lp)); kernel = "xchg_ll<8>"; }
+    else { SB_TRY(launch_kernel(xchg_ll_kernel<16>, g, b, 0, st, pdl, lp)); kernel = "xchg_ll<16>"; }
   } else
-  if (t->world <= 2) SB_TRY(launch_kernel(xchg_update_kernel<2>, g, b, 0, st, pdl, p));
-  else if (t->world <= 4) SB_TRY(launch_kernel(xchg_update_kernel<4>, g, b, 0, st, pdl, p));
-  else if (t->world <= 8) SB_TRY(launch_kernel(xchg_update_kernel<8>, g, b, 0, st, pdl, p));
-  else SB_TRY(launch_kernel(xchg_update_kernel<16>, g, b, 0, st, pdl, p));
-  n.mark("xchg_update");
+  if (t->world <= 2) { SB_TRY(launch_kernel(xchg_update_kernel<2>, g, b, 0, st, pdl, p)); kernel = "xchg_update<2>"; }
+  else if (t->world <= 4) { SB_TRY(launch_kernel(xchg_update_kernel<4>, g, b, 0, st, pdl, p)); kernel = "xchg_update<4>"; }
+  else if (t->world <= 8) { SB_TRY(launch_kernel(xchg_update_kernel<8>, g, b, 0, st, pdl, p)); kernel = "xchg_update<8>"; }
+  else { SB_TRY(launch_kernel(xchg_update_kernel<16>, g, b, 0, st, pdl, p)); kernel = "xchg_update<16>"; }
+  n.mark(kernel);
   t->master_stale = true;
   t->grad_sharded = true;
   return SB_OK;
@@ -1554,6 +1563,100 @@ int sb_debug_step_trace(sb_trainer_t* t, uint64_t* stamps, int32_t cap_kernels, 
     std::string all;
     for (int i = 0; i < k; ++i) { if (i) all += ','; all += n.trace_names[i]; }
     snprintf(names, names_cap, "%s", all.c_str());
+  }
+  return SB_OK;
+}
+
+// ================================================================================================
+// exchange test hooks: a rank's raw arena buffers, one exchange launch as a step queues it, the ownership tables
+// ================================================================================================
+int sb_debug_trainer_buffer(sb_trainer_t* t, int32_t which, void* host, int64_t n, int32_t write) {
+  SB_CHECK(t && host, SB_ERR_INVALID, "null argument");
+  Net& net = t->net;
+  SB_CHECK(which >= SB_DEBUG_BUF_THETA && which < SB_DEBUG_BUF_SHADOW + net.L, SB_ERR_INVALID,
+           "buffer %d outside [0, %d)", which, SB_DEBUG_BUF_SHADOW + net.L);
+  SB_CHECK(write >= 0 && write <= 2 && (write != 2 || which == SB_DEBUG_BUF_THETA), SB_ERR_INVALID,
+           "write = %d: 0 reads, 1 writes, 2 writes theta and refreshes the shadows", write);
+  if (which < SB_DEBUG_BUF_SHADOW) {
+    SB_CHECK(n == net.n_params, SB_ERR_INVALID, "expected %lld floats, got %lld", (long long)net.n_params, (long long)n);
+    float* dev = which == SB_DEBUG_BUF_THETA ? net.theta : which == SB_DEBUG_BUF_S1 ? net.s1 : which == SB_DEBUG_BUF_S2 ? net.s2 : t->grad;
+    SB_CUDA(cudaSetDevice(net.device));
+    SB_CUDA(cudaStreamSynchronize(net.stream));
+    if (write) SB_CUDA(cudaMemcpyAsync(dev, host, sizeof(float) * n, cudaMemcpyHostToDevice, net.stream));
+    else SB_CUDA(cudaMemcpyAsync(host, dev, sizeof(float) * n, cudaMemcpyDeviceToHost, net.stream));
+    if (write == 2) SB_TRY(net.refresh_shadows());
+  } else {
+    const int l = which - SB_DEBUG_BUF_SHADOW;
+    SB_CHECK(net.tc(), SB_ERR_STATE, "layer %d has no bf16 shadow in fp32 mode", l);
+    const Layer& ly = net.layers[l];
+    const long long part = static_cast<long long>(ly.in) * ly.ld_out;
+    SB_CHECK(n == part * net.nparts, SB_ERR_INVALID, "expected %d x %d x %d bf16 values, got %lld", net.nparts, ly.in, ly.ld_out,
+             (long long)n);
+    SB_CUDA(cudaSetDevice(net.device));
+    SB_CUDA(cudaStreamSynchronize(net.stream));
+    for (int k = 0; k < net.nparts; ++k) {
+      uint16_t* h = static_cast<uint16_t*>(host) + k * part;
+      __nv_bfloat16* d = ly.Wn + k * net.Wn_ps[l];
+      if (write) SB_CUDA(cudaMemcpyAsync(d, h, sizeof(uint16_t) * part, cudaMemcpyHostToDevice, net.stream));
+      else SB_CUDA(cudaMemcpyAsync(h, d, sizeof(uint16_t) * part, cudaMemcpyDeviceToHost, net.stream));
+    }
+  }
+  SB_CUDA(cudaStreamSynchronize(net.stream));
+  return SB_OK;
+}
+
+int sb_debug_exchange(sb_trainer_t* t, int32_t slot_mask, float gscale, int32_t grid, int32_t alone, float* lr_t_out,
+                      int32_t* grid_out, char* route, int32_t route_cap) {
+  SB_CHECK(t, SB_ERR_INVALID, "null trainer");
+  SB_CHECK(t->world > 1 && t->p2p_ready, SB_ERR_STATE, "no peers configured (world = %d): set the peer table first", t->world);
+  SB_CHECK(slot_mask > 0 && (slot_mask & ~xseg_all(t)) == 0, SB_ERR_INVALID, "slot mask 0x%x outside 0x%x (%d slots)", slot_mask,
+           xseg_all(t), t->x_slots);
+  SB_CHECK(std::isfinite(gscale) && gscale >= 0.f, SB_ERR_INVALID, "gscale %g is not a finite value >= 0", gscale);
+  SB_CHECK(grid >= 0 && grid <= 65535, SB_ERR_INVALID, "grid %d outside [0, 65535]", grid);
+  SB_CHECK(route_cap >= 0 && (route != nullptr || route_cap == 0), SB_ERR_INVALID, "route_cap %d without a buffer", route_cap);
+  Net& n = t->net;
+  SB_CUDA(cudaSetDevice(n.device));
+  // as a step: the descriptor of this update (step count, lr_t, gradient scale, epoch), then the exchange on the main stream.
+  // Nothing here waits for the device - the peers' launches are still to be queued by the same host thread.
+  ++t->global_step;
+  const float lr_t = lr_for_step(t, t->global_step);
+  const float gs = gscale > 0.f ? gscale : 1.f / static_cast<float>(t->world);
+  ++t->epoch;
+  const StepIn in{t->descs[t->last_pair], t->scals[t->last_pair]};
+  set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, nullptr, nullptr, nullptr, lr_t, gs, t->epoch);
+  SB_CUDA(cudaGetLastError());
+  if (grid <= 0) grid = xchg_grid(t, slot_mask, alone != 0);
+  n.last_kernel = nullptr;
+  SB_TRY(enqueue_xchg(t, in, slot_mask, n.stream, false, false, alone != 0, grid));
+  t->grad_out_scale = gs;
+  if (lr_t_out) *lr_t_out = lr_t;
+  if (grid_out) *grid_out = grid;
+  if (route_cap > 0) snprintf(route, static_cast<size_t>(route_cap), "%s", n.last_kernel ? n.last_kernel : "");
+  return SB_OK;
+}
+
+int sb_debug_exchange_layout(sb_trainer_t* t, int32_t* info, int32_t info_cap, int64_t* work, int64_t work_cap, int32_t* n_work) {
+  SB_CHECK(t && info && n_work, SB_ERR_INVALID, "null argument");
+  SB_CHECK(info_cap >= SB_DEBUG_XINFO_WORDS, SB_ERR_INVALID, "info needs %d words, got %d", SB_DEBUG_XINFO_WORDS, info_cap);
+  Net& n = t->net;
+  SB_CHECK(work == nullptr || work_cap >= static_cast<int64_t>(n.n_work) * SB_DEBUG_XWORK_WORDS, SB_ERR_INVALID,
+           "work needs %lld words, got %lld", static_cast<long long>(n.n_work) * SB_DEBUG_XWORK_WORDS, (long long)work_cap);
+  *n_work = n.n_work;
+  memset(info, 0, sizeof(int32_t) * SB_DEBUG_XINFO_WORDS);
+  info[0] = t->x_slots; info[1] = n.num_sms; info[2] = t->ll_ready; info[3] = t->peers_share_device;
+  info[4] = t->rank; info[5] = t->world; info[6] = n.nparts;
+  for (int s = 0; s < SB_XCHG_SLOTS; ++s) { info[8 + s] = t->x_begin[s]; info[16 + s] = t->x_end[s]; }
+  if (work == nullptr) return SB_OK;
+  std::vector<OptWork> wk(static_cast<size_t>(n.n_work));
+  SB_CUDA(cudaSetDevice(n.device));
+  SB_CUDA(cudaStreamSynchronize(n.stream));
+  SB_CUDA(cudaMemcpy(wk.data(), n.work, sizeof(OptWork) * wk.size(), cudaMemcpyDeviceToHost));
+  for (int i = 0; i < n.n_work; ++i) {
+    int64_t* o = work + static_cast<size_t>(i) * SB_DEBUG_XWORK_WORDS;
+    int layer = -1;
+    for (int l = 0; l < n.L; ++l) if (wk[i].Wn != nullptr && wk[i].Wn == n.layers[l].Wn) layer = l;
+    o[0] = wk[i].off; o[1] = wk[i].count; o[2] = wk[i].out_dim; o[3] = wk[i].mat_off;
+    o[4] = wk[i].ld_out; o[5] = wk[i].np; o[6] = layer; o[7] = wk[i].part_stride;
   }
   return SB_OK;
 }
