@@ -226,13 +226,24 @@ int32_t sb_model_n_features(const sb_model_t* m);
 int32_t sb_model_n_layers(const sb_model_t* m);
 /* batched compute(): X [rows, n_features] fp32 host -> out [rows] fp32 host */
 int sb_model_score(sb_model_t* m, const float* X, int64_t rows, float* out);
-/* compute(MLData): one row of doubles -> double (double->float cast at TensorflowModel.java:64-68) */
+/* compute(MLData): one row of doubles -> double (double->float cast at TensorflowModel.java:64-68).
+ * Concurrent calls on one handle share device batches of up to 128 rows; a lone call is scored at once.  A row's
+ * score is the same whichever rows share its batch. */
 int sb_model_score_row_f64(sb_model_t* m, const double* row, int32_t n, double* out);
 /* device-resident scoring (X, out are DEVICE pointers on the model's device), asynchronous on the
  * model's stream; sb_model_sync waits. */
 int sb_model_score_device(sb_model_t* m, const float* dX, int64_t rows, float* dOut);
 int sb_model_sync(sb_model_t* m);
 void* sb_model_stream(sb_model_t* m);
+/* Test hooks of the scorer.  stats[SB_DEBUG_MSTAT_WORDS] since creation = {compute() batches run, rows they scored,
+ * the largest batch, batches run by the one-launch fp32 kernel, batches run by the captured tensor-core graph,
+ * one-launch fp32 forwards of any entry point}. */
+#define SB_DEBUG_MSTAT_WORDS 6
+enum { SB_DEBUG_MSTAT_BATCHES = 0, SB_DEBUG_MSTAT_ROWS = 1, SB_DEBUG_MSTAT_MAX_FILL = 2, SB_DEBUG_MSTAT_SMALL = 3,
+       SB_DEBUG_MSTAT_GRAPH = 4, SB_DEBUG_MSTAT_SMALL_LAUNCHES = 5 };
+int sb_debug_model_batch_stats(sb_model_t* m, int64_t* stats, int32_t n_stats);
+/* The next compute() batch waits until k rows are queued or timeout_ms have passed (k = 0: no wait). */
+int sb_debug_model_hold(sb_model_t* m, int32_t k, int32_t timeout_ms);
 
 /* ---- text ingest: the per-cell float() loop of load_data (ssgd_monitor.py:387-419) on the GPU ----
  * text: the gunzipped, delim-separated lines (must end with '\n'), HOST memory.  col_map[c] gives the role of text

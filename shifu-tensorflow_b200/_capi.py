@@ -132,6 +132,8 @@ PROTOTYPES = {
     "sb_model_score_device": (C.c_int, [_vp, _vp, C.c_int64, _vp]),
     "sb_model_sync": (C.c_int, [_vp]),
     "sb_model_stream": (C.c_void_p, [_vp]),
+    "sb_debug_model_batch_stats": (C.c_int, [_vp, _P(C.c_int64), C.c_int32]),
+    "sb_debug_model_hold": (C.c_int, [_vp, C.c_int32, C.c_int32]),
     "sb_text_parse": (C.c_int, [_cp, C.c_int64, C.c_char, _P(C.c_int32), C.c_int32, C.c_int32, _f32p, _f32p, _f32p, C.c_int64,
                                 _P(C.c_int64), _P(CellFlag), C.c_int64, _P(C.c_int64), C.c_int]),
     "sb_text_parse_device": (C.c_int, [_cp, C.c_int64, C.c_char, _P(C.c_int32), C.c_int32, C.c_int32, _P(_f32p), _P(_f32p), _P(_f32p),
@@ -166,6 +168,8 @@ PROTOTYPES = {
 
 DEBUG_BUF_THETA, DEBUG_BUF_S1, DEBUG_BUF_S2, DEBUG_BUF_GRAD, DEBUG_BUF_SHADOW = 0, 1, 2, 3, 4
 DEBUG_XINFO_WORDS, DEBUG_XWORK_WORDS = 24, 8
+DEBUG_MSTAT_WORDS = 6
+SMALL_ROWS = 128        # score_rows.cuh: an fp32 model scores batches of up to this many rows in one launch
 
 
 def lib():
@@ -583,6 +587,17 @@ class Model:
     @property
     def stream(self) -> int:
         return int(lib().sb_model_stream(self._h) or 0)
+
+    def batch_stats(self) -> dict:
+        """counters since creation (sb_debug_model_batch_stats): compute() batches, their rows, the largest batch, batches
+        run by the one-launch fp32 kernel / by the captured tensor-core graph, and one-launch fp32 forwards of any entry point"""
+        st = np.zeros(DEBUG_MSTAT_WORDS, np.int64)
+        check(lib().sb_debug_model_batch_stats(self._h, st.ctypes.data_as(_P(C.c_int64)), st.size))
+        return dict(zip(("batches", "rows", "max_fill", "small", "graph", "small_launches"), (int(v) for v in st)))
+
+    def hold(self, k: int, timeout_ms: int):
+        """the next compute() batch waits until k rows are queued or timeout_ms have passed (sb_debug_model_hold)"""
+        check(lib().sb_debug_model_hold(self._h, int(k), int(timeout_ms)))
 
 
 def nccl_unique_id() -> bytes:

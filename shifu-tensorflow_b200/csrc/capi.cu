@@ -6,10 +6,14 @@
 #include <cmath>
 #include <string.h>
 #include <algorithm>
+#include <atomic>
+#include <chrono>
+#include <condition_variable>
 #include <memory>
 #include <random>
 #include "net.cuh"
 #include "savedmodel.h"
+#include "score_rows.cuh"
 #include "xchg_p2p.cuh"
 
 using namespace sb;
@@ -1438,10 +1442,50 @@ int sb_trainer_export_savedmodel(sb_trainer_t* t, const char* export_dir) {
 // ================================================================================================
 }  // extern "C"
 
+// compute() (sb_model_score_row_f64) callers on one handle share device batches of up to MB_ROWS rows: the tensor-core
+// kernels' tile height.  plan_gemm / plan_gemm_pp depend on M only through ceil(M / 128) and the grid size, so every GEMM
+// plan of <= 128 rows is the one-row plan, and rows never interact in the forward GEMMs, the load or the output kernels:
+// a row's score does not depend on which rows shared its batch.
+static const int MB_ROWS = 128;
+static_assert(SMALL_ROWS >= MB_ROWS, "an fp32 micro-batch is one score_rows_kernel launch");
+
+struct RowWaiter {            // one compute() call, on its caller's stack
+  float value = 0.f;
+  int status = SB_OK;
+  std::string err;            // the leader's error text, re-raised in the caller's thread
+  bool done = false;
+};
+
 struct sb_model {
   Net net;
   sb_net_desc desc;
-  std::mutex mu;
+  std::mutex mu;              // device work on the model's stream
+  DevBuf<float> sr_act;       // fp32: score_rows_kernel's two activation buffers [SMALL_ROWS, sr_ld]
+  int sr_ld = 0;
+  // compute() queue (guarded by q_mu).  No thread of its own: the first caller that finds no batch in flight leads,
+  // running every queued row in batches until the queue is empty; the others wait for their result.
+  std::mutex q_mu;
+  std::condition_variable q_cv;
+  float* stage[2] = {nullptr, nullptr};       // pinned [MB_ROWS, F]: one buffer fills while the other's batch runs
+  float* res[2] = {nullptr, nullptr};         // pinned [MB_ROWS] scores
+  RowWaiter* waiters[2][MB_ROWS] = {};
+  int fill[2] = {0, 0};       // rows queued in a buffer
+  int writers[2] = {0, 0};    // callers still converting their row into it
+  int cur = 0;                // the buffer that takes new rows
+  bool leading = false;
+  int hold_k = 0, hold_ms = 0;                // sb_debug_model_hold
+  cudaGraphExec_t mb_graph = nullptr;         // tensor-core modes: the forward of MB_ROWS staged rows
+  std::atomic<long long> st[SB_DEBUG_MSTAT_WORDS] = {};
+  ~sb_model() {
+    if (!net.stream) return;
+    cudaSetDevice(net.device);
+    cudaStreamSynchronize(net.stream);
+    if (mb_graph) cudaGraphExecDestroy(mb_graph);
+    for (int b = 0; b < 2; ++b) {
+      if (stage[b]) cudaFreeHost(stage[b]);
+      if (res[b]) cudaFreeHost(res[b]);
+    }
+  }
 };
 
 static const int MODEL_CHUNK_ROWS = 16384;        // fp32 parity mode
@@ -1456,9 +1500,117 @@ static int model_from_desc(sb_net_desc d, const float* flat, int64_t n, int devi
   SB_CHECK(n == net.n_params, SB_ERR_INVALID, "expected %lld params, got %lld", (long long)net.n_params, (long long)n);
   SB_CUDA(cudaMemcpyAsync(net.theta, flat, sizeof(float) * n, cudaMemcpyHostToDevice, net.stream));
   SB_TRY(net.refresh_shadows());
+  if (!net.tc()) {
+    int widest = 1;
+    for (int l = 0; l < net.L; ++l) widest = std::max(widest, net.layers[l].out);
+    m->sr_ld = round_up(widest, 4);
+    SB_TRY(m->sr_act.alloc(static_cast<size_t>(2) * SMALL_ROWS * m->sr_ld));
+    SB_TRY(set_max_smem(score_rows_kernel, SR_SMEM));
+  }
+  for (int b = 0; b < 2; ++b) {
+    SB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&m->stage[b]), sizeof(float) * MB_ROWS * net.F, cudaHostAllocDefault));
+    SB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&m->res[b]), sizeof(float) * MB_ROWS, cudaHostAllocDefault));
+  }
   SB_CUDA(cudaStreamSynchronize(net.stream));
   *out = m.release();
   return SB_OK;
+}
+
+// The forward of `rows` (<= max_batch) device rows dX -> scores dOut (device), queued on the model's stream: every scoring
+// path of a model comes through here.  An fp32 batch of <= SMALL_ROWS rows is one score_rows_kernel launch; any other
+// batch runs the layer-by-layer launches.  Both give the same bits.  Called with m->mu held.
+static int model_forward(sb_model* m, const float* dX, int rows, float* dOut) {
+  Net& n = m->net;
+  if (!n.tc() && rows <= SMALL_ROWS) {
+    ScoreRowsParams p = {};
+    p.rows = rows; p.F = n.F; p.L = n.L;
+    p.X = dX; p.theta = n.theta;
+    p.act[0] = m->sr_act.p; p.act[1] = m->sr_act.p + static_cast<size_t>(SMALL_ROWS) * m->sr_ld; p.ld_act = m->sr_ld;
+    p.yhat = dOut;
+    for (int l = 0; l < n.L; ++l) { p.out[l] = n.layers[l].out; p.act_fn[l] = n.layers[l].act; }
+    for (int l = 0; l <= n.L; ++l) { p.w_off[l] = n.layers[l].w_off; p.b_off[l] = n.layers[l].b_off; }
+    const int clusters = (rows + SR_ROWS - 1) / SR_ROWS;
+    score_rows_kernel<<<clusters * SR_CLUSTER, SR_THREADS, SR_SMEM, n.stream>>>(p);
+    SB_CUDA(cudaGetLastError());
+    ++m->st[SB_DEBUG_MSTAT_SMALL_LAUNCHES];
+    return SB_OK;
+  }
+  const StepIn in{n.desc, n.scal};
+  set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, dX, nullptr, n.ones, 0.f, 1.f);
+  SB_TRY(n.enqueue_load(in, rows));
+  SB_TRY(n.enqueue_hidden_forward(in, rows));
+  return n.enqueue_out(in, rows, false, false, dOut, nullptr);
+}
+
+// tensor-core modes: model_forward of MB_ROWS rows of the staging area, captured once, so a micro-batch is one launch
+static int capture_micro_batch(sb_model* m) {
+  Net& n = m->net;
+  cudaGraph_t g = nullptr;
+  SB_CUDA(cudaStreamBeginCapture(n.stream, cudaStreamCaptureModeThreadLocal));
+  const int s = model_forward(m, n.stX, MB_ROWS, n.yhat);
+  const cudaError_t e = cudaStreamEndCapture(n.stream, &g);
+  if (s != SB_OK) { if (g) cudaGraphDestroy(g); return s; }
+  SB_CHECK(e == cudaSuccess, SB_ERR_CUDA, "cudaStreamEndCapture failed: %s", cudaGetErrorString(e));
+  const cudaError_t ei = cudaGraphInstantiate(&m->mb_graph, g, 0);
+  cudaGraphDestroy(g);
+  SB_CHECK(ei == cudaSuccess, SB_ERR_CUDA, "cudaGraphInstantiate failed: %s", cudaGetErrorString(ei));
+  return SB_OK;
+}
+
+// one compute() batch: rows of staging buffer b -> m->res[b].  A tensor-core batch runs at MB_ROWS rows, its pad rows
+// zero-filled; only the real rows are copied back.
+static int run_micro_batch(sb_model* m, int b, int rows) {
+  std::lock_guard<std::mutex> lk(m->mu);
+  Net& n = m->net;
+  SB_CUDA(cudaSetDevice(n.device));
+  if (n.tc() && !m->mb_graph) SB_TRY(capture_micro_batch(m));
+  const size_t row_bytes = sizeof(float) * n.F;
+  SB_CUDA(cudaMemcpyAsync(n.stX, m->stage[b], row_bytes * rows, cudaMemcpyHostToDevice, n.stream));
+  if (n.tc()) {
+    if (rows < MB_ROWS) SB_CUDA(cudaMemsetAsync(n.stX + static_cast<size_t>(rows) * n.F, 0, row_bytes * (MB_ROWS - rows), n.stream));
+    SB_CUDA(cudaGraphLaunch(m->mb_graph, n.stream));
+    ++m->st[SB_DEBUG_MSTAT_GRAPH];
+  } else {
+    SB_TRY(model_forward(m, n.stX, rows, n.yhat));
+    ++m->st[SB_DEBUG_MSTAT_SMALL];
+  }
+  SB_CUDA(cudaMemcpyAsync(m->res[b], n.yhat, sizeof(float) * rows, cudaMemcpyDeviceToHost, n.stream));
+  SB_CUDA(cudaStreamSynchronize(n.stream));
+  return SB_OK;
+}
+
+// The leader (q_mu held through lk): runs the queued rows in batches until the queue is empty, and publishes each
+// caller's result and status.
+static void lead_batches(sb_model* m, std::unique_lock<std::mutex>& lk) {
+  while (m->fill[m->cur] > 0) {
+    if (m->hold_k > 0) {      // sb_debug_model_hold: this batch waits for hold_k rows or the timeout
+      const int k = m->hold_k;
+      m->hold_k = 0;
+      m->q_cv.wait_until(lk, std::chrono::steady_clock::now() + std::chrono::milliseconds(m->hold_ms),
+                         [&] { return m->fill[m->cur] >= k; });
+    }
+    const int b = m->cur;
+    m->q_cv.wait(lk, [&] { return m->writers[b] == 0; });
+    const int rows = m->fill[b];
+    m->cur ^= 1;              // new rows go to the other buffer (empty: its batch was published before this one began)
+    m->q_cv.notify_all();
+    lk.unlock();
+    const int s = run_micro_batch(m, b, rows);
+    const std::string err = s == SB_OK ? std::string() : last_error_ref();
+    lk.lock();
+    for (int i = 0; i < rows; ++i) {
+      RowWaiter* w = m->waiters[b][i];
+      w->status = s;
+      if (s == SB_OK) w->value = m->res[b][i];
+      else w->err = err;
+      w->done = true;
+    }
+    m->fill[b] = 0;
+    ++m->st[SB_DEBUG_MSTAT_BATCHES];
+    m->st[SB_DEBUG_MSTAT_ROWS] += rows;
+    if (rows > m->st[SB_DEBUG_MSTAT_MAX_FILL]) m->st[SB_DEBUG_MSTAT_MAX_FILL] = rows;
+    m->q_cv.notify_all();
+  }
 }
 
 extern "C" {
@@ -1507,19 +1659,46 @@ int sb_model_score(sb_model_t* m, const float* X, int64_t rows, float* out) {
   SB_CHECK(X && out, SB_ERR_INVALID, "null argument");
   if (rows <= 0) return SB_OK;
   std::lock_guard<std::mutex> lk(m->mu);
-  double a = 0, b = 0;
-  return forward_chunks(m->net, X, nullptr, nullptr, rows, false, out, &a, &b);
+  Net& n = m->net;
+  SB_CUDA(cudaSetDevice(n.device));
+  for (int64_t r0 = 0; r0 < rows; r0 += n.max_batch) {
+    const int c = static_cast<int>(rows - r0 < n.max_batch ? rows - r0 : n.max_batch);
+    SB_CUDA(cudaMemcpyAsync(n.stX, X + r0 * n.F, sizeof(float) * c * static_cast<size_t>(n.F), cudaMemcpyDefault, n.stream));
+    SB_TRY(model_forward(m, n.stX, c, n.yhat));
+    SB_CUDA(cudaMemcpyAsync(out + r0, n.yhat, sizeof(float) * c, cudaMemcpyDefault, n.stream));
+    SB_CUDA(cudaStreamSynchronize(n.stream));
+  }
+  return SB_OK;
 }
 
 int sb_model_score_row_f64(sb_model_t* m, const double* row, int32_t n, double* out) {
   SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
   SB_CHECK(row && out, SB_ERR_INVALID, "null argument");
   SB_CHECK(n == m->net.F, SB_ERR_INVALID, "expected %d features, got %d", m->net.F, n);
-  std::vector<float> f(static_cast<size_t>(n));
+  RowWaiter me;
+  std::unique_lock<std::mutex> lk(m->q_mu);
+  m->q_cv.wait(lk, [&] { return m->fill[m->cur] < MB_ROWS; });
+  const int b = m->cur, slot = m->fill[b]++;
+  m->waiters[b][slot] = &me;
+  ++m->writers[b];
+  lk.unlock();
+  float* f = m->stage[b] + static_cast<size_t>(slot) * n;
   for (int i = 0; i < n; ++i) f[i] = static_cast<float>(row[i]);  // TensorflowModel.java:64-68
-  float r = 0.f;
-  SB_TRY(sb_model_score(m, f.data(), 1, &r));
-  *out = static_cast<double>(r);
+  lk.lock();
+  if (--m->writers[b] == 0) m->q_cv.notify_all();
+  while (!me.done) {
+    if (!m->leading) {        // no batch in flight: lead (a lone caller is scored at once)
+      m->leading = true;
+      lead_batches(m, lk);
+      m->leading = false;
+      m->q_cv.notify_all();
+    } else {
+      m->q_cv.wait(lk);
+    }
+  }
+  lk.unlock();
+  if (me.status != SB_OK) return set_error(me.status, "%s", me.err.c_str());
+  *out = static_cast<double>(me.value);
   return SB_OK;
 }
 
@@ -1529,13 +1708,9 @@ int sb_model_score_device(sb_model_t* m, const float* dX, int64_t rows, float* d
   std::lock_guard<std::mutex> lk(m->mu);
   Net& n = m->net;
   SB_CUDA(cudaSetDevice(n.device));
-  const StepIn in{n.desc, n.scal};
   for (int64_t r0 = 0; r0 < rows; r0 += n.max_batch) {
     const int c = static_cast<int>(rows - r0 < n.max_batch ? rows - r0 : n.max_batch);
-    set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, dX + r0 * n.F, nullptr, n.ones, 0.f, 1.f);
-    SB_TRY(n.enqueue_load(in, c));
-    SB_TRY(n.enqueue_hidden_forward(in, c));
-    SB_TRY(n.enqueue_out(in, c, false, false, dOut + r0, nullptr));
+    SB_TRY(model_forward(m, dX + r0 * n.F, c, dOut + r0));
   }
   return SB_OK;
 }
@@ -1546,6 +1721,23 @@ int sb_model_sync(sb_model_t* m) {
   return SB_OK;
 }
 void* sb_model_stream(sb_model_t* m) { return m ? reinterpret_cast<void*>(m->net.stream) : nullptr; }
+
+int sb_debug_model_batch_stats(sb_model_t* m, int64_t* stats, int32_t n_stats) {
+  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
+  SB_CHECK(stats && n_stats >= SB_DEBUG_MSTAT_WORDS, SB_ERR_INVALID, "stats needs %d words, got %d", SB_DEBUG_MSTAT_WORDS, n_stats);
+  for (int i = 0; i < SB_DEBUG_MSTAT_WORDS; ++i) stats[i] = m->st[i].load();
+  return SB_OK;
+}
+
+int sb_debug_model_hold(sb_model_t* m, int32_t k, int32_t timeout_ms) {
+  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
+  SB_CHECK(k >= 0 && k <= MB_ROWS && timeout_ms >= 0, SB_ERR_INVALID, "k = %d outside [0, %d] or timeout_ms = %d < 0", k, MB_ROWS,
+           timeout_ms);
+  std::lock_guard<std::mutex> lk(m->q_mu);
+  m->hold_k = k;
+  m->hold_ms = timeout_ms;
+  return SB_OK;
+}
 
 // ================================================================================================
 // step-timeline test hook (the kernel-level hooks are in net.cu, beside the step's GEMM launches)
