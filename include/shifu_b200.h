@@ -123,6 +123,14 @@ int sb_trainer_get_params(sb_trainer_t* t, float* flat, int64_t n);
 int sb_trainer_init_xavier(sb_trainer_t* t, uint64_t seed);
 /* parity hook: the (all-reduced, mean over ranks) gradient the last step applied */
 int sb_trainer_get_grads(sb_trainer_t* t, float* flat, int64_t n);
+/* Deterministic training (on = 1; default 0): every reduction over CTAs of a training step is added in a fixed order,
+ * so two runs with the same build, GPU model and SM count, descriptor, inputs, seed, world size and sequence of calls
+ * give bit-identical parameters, optimizer state, gradients, losses and checkpoint / SavedModel files.  Call it right
+ * after sb_trainer_create: SB_ERR_STATE after the first step or graph capture, after the peer exchange was set up, on a
+ * wide+deep trainer (sb_trainer_set_sparse is refused on a deterministic one).  All four precisions.  A
+ * deterministic trainer with world > 1 needs a peer table (sb_trainer_set_peer_handles / _pointers): without one its
+ * first step returns SB_ERR_STATE (NCCL's all-reduce fixes no summation order). */
+int sb_trainer_set_deterministic(sb_trainer_t* t, int32_t on);
 
 /* one sess.run([train_step, loss, global_step], feed_dict) (ssgd_monitor.py:272-276) in the
  * "clean" schedule: forward, loss, backward, gradient mean over ranks, one optimizer update.

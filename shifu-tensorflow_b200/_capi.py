@@ -97,6 +97,7 @@ PROTOTYPES = {
     "sb_trainer_get_grads": (C.c_int, [_vp, _f32p, C.c_int64]),
     "sb_trainer_step": (C.c_int, [_vp, _f32p, _f32p, _f32p, C.c_int32, _f32p]),
     "sb_trainer_set_sparse": (C.c_int, [_vp, C.c_int32, C.c_int32, C.c_int32]),
+    "sb_trainer_set_deterministic": (C.c_int, [_vp, C.c_int32]),
     "sb_trainer_step_sparse": (C.c_int, [_vp, _f32p, _P(C.c_int32), _f32p, _f32p, C.c_int32, _f32p]),
     "sb_trainer_predict_sparse": (C.c_int, [_vp, _f32p, _P(C.c_int32), C.c_int64, _f32p]),
     "sb_trainer_eval_loss_sparse": (C.c_int, [_vp, _f32p, _P(C.c_int32), _f32p, _f32p, C.c_int64, _f32p]),
@@ -258,7 +259,8 @@ class DeviceArray:
 class Trainer:
     """Owns one sb_trainer_t.  X is [rows, n_features] float32, y / w are [rows] (or [rows,1])."""
 
-    def __init__(self, desc: NetDesc, device: int = 0, nccl_id: Optional[bytes] = None, rank: int = 0, world: int = 1):
+    def __init__(self, desc: NetDesc, device: int = 0, nccl_id: Optional[bytes] = None, rank: int = 0, world: int = 1,
+                 deterministic: bool = False):
         self._h = C.c_void_p()
         self.desc = desc
         idbuf = None
@@ -270,6 +272,12 @@ class Trainer:
                                       rank, world, C.byref(self._h)))
         self.n_params = int(lib().sb_trainer_param_count(self._h))
         self.n_features = int(desc.n_features)
+        if deterministic:
+            self.set_deterministic(True)
+
+    def set_deterministic(self, on: bool = True):
+        """fixed-order reductions in every training kernel (sb_trainer_set_deterministic); before the first step"""
+        check(lib().sb_trainer_set_deterministic(self._h, 1 if on else 0))
 
     def close(self):
         if getattr(self, "_h", None) is not None and self._h:

@@ -94,6 +94,7 @@ struct sb_trainer {
   cudaStream_t prep = nullptr;
   cudaEvent_t ev_prep[2] = {nullptr, nullptr}, ev_pos[2] = {nullptr, nullptr};
   unsigned long long prep_steps = 0;
+  bool started = false;    // a step ran or was captured: sb_trainer_set_deterministic is refused from here on
   bool have_pos = false;   // ev_pos[] of the previous step is valid (no other user of the descriptors in between)
   int last_pair = 0;       // the pair the last step used
   // sb_trainer_run_resident: RUN_S steps per captured graph (kernel -> kernel edges instead of a graph turn-around
@@ -316,8 +317,9 @@ static Dw1Plan plan_dw1(const sb_trainer* t, int rows, bool split_tail, bool xsc
   const Layer& l0 = n.layers[0];
   const Layer& l1 = n.layers[1];
   const int kx = round_up(rows, 64) * pairs_of(n.nparts);
-  const GemmPlan n0 = plan_gemm(l0.in, l0.out, kx, S, true);
-  const GemmPlan n1 = plan_gemm(l1.in, l1.out, kx, S, true);
+  const int ms = n.dw_max_split();
+  const GemmPlan n0 = plan_gemm(l0.in, l0.out, kx, S, true, ms);
+  const GemmPlan n1 = plan_gemm(l1.in, l1.out, kx, S, true, ms);
   if (n0.grid + n1.grid <= S) return d;
   // single-GPU tail: dW_1 runs IN FRONT of dW_0 on the main stream instead of beside it - side by side the two persistent
   // grids take turns on the SMs; small layers (cfg1) stay side by side.  Only when dW_0 alone fills every SM: on one H100,
@@ -332,8 +334,8 @@ static Dw1Plan plan_dw1(const sb_trainer* t, int rows, bool split_tail, bool xsc
   }
   // compare, in k-blocks per CTA, "natural grids, dW_1 finishing after dW_0" against "dW_1 on a third of the SMs, dW_0
   // on the rest" and take the shorter
-  const GemmPlan b1 = plan_gemm(l1.in, l1.out, kx, S / 3, true);
-  const GemmPlan b0 = plan_gemm(l0.in, l0.out, kx, S - b1.grid, true);
+  const GemmPlan b1 = plan_gemm(l1.in, l1.out, kx, S / 3, true, ms);
+  const GemmPlan b0 = plan_gemm(l0.in, l0.out, kx, S - b1.grid, true, ms);
   auto waves = [&](const GemmPlan& pl, const Layer& ly, int sms) {   // k-blocks one CTA works through
     const int tiles = ((ly.in + 127) / 128) * ((ly.out + pl.bn - 1) / pl.bn) * pl.split_k;
     return ((tiles + sms - 1) / sms) * pl.kb_per_split;
@@ -489,6 +491,7 @@ static int get_graph(sb_trainer* t, const StepIn& in, int rows, int kind, int pa
   auto it = t->graphs.find(key);
   if (it != t->graphs.end()) { *out = it->second; return SB_OK; }
   Net& n = t->net;
+  t->started = true;
   n.launches = 0;
   cudaGraph_t g = nullptr;
   SB_CUDA(cudaStreamBeginCapture(n.stream, cudaStreamCaptureModeThreadLocal));
@@ -506,9 +509,20 @@ static int get_graph(sb_trainer* t, const StepIn& in, int rows, int kind, int pa
 }
 
 // X, y, w are DEVICE pointers here
+// A deterministic trainer with more than one rank needs the peer-memory exchange, which adds the ranks' gradients in rank
+// order; NCCL's all-reduce promises no summation order.
+static int check_det_exchange(const sb_trainer* t) {
+  SB_CHECK(!t->net.det || t->world == 1 || t->p2p_ready, SB_ERR_STATE,
+           "deterministic trainer (rank %d of %d) has no peer table: the NCCL all-reduce does not fix its summation order, so "
+           "deterministic training across ranks needs sb_trainer_set_peer_handles / _pointers", t->rank, t->world);
+  return SB_OK;
+}
+
 static int run_step(sb_trainer* t, const float* X, const float* y, const float* w, int rows, int kind, long long resident_row0 = -1,
                     bool sparse = false) {
   Net& n = t->net;
+  SB_TRY(check_det_exchange(t));
+  t->started = true;
   SB_CHECK(rows > 0 && rows <= n.max_batch, SB_ERR_INVALID, "rows=%d outside (0, max_batch=%d]", rows, n.max_batch);
   SB_CUDA(cudaSetDevice(n.device));
   const bool resident = resident_row0 >= 0 && t->dsXb != nullptr;
@@ -935,7 +949,22 @@ int sb_trainer_step(sb_trainer_t* t, const float* X, const float* y, const float
 // ---- wide+deep (BASELINE config 4): hidden layer 0 = [dense | one-hot]; the step feeds (dense block, index matrix) ----
 int sb_trainer_set_sparse(sb_trainer_t* t, int32_t n_dense, int32_t n_onehot, int32_t n_cat) {
   SB_CHECK(t, SB_ERR_INVALID, "null trainer");
+  SB_CHECK(!t->net.det, SB_ERR_STATE, "wide+deep on a deterministic trainer: the embedding gradient is scatter-added with "
+           "red.global (embed_scatter_kernel), whose summation order is not fixed");
   return t->net.set_sparse(n_dense, n_onehot, n_cat);
+}
+
+int sb_trainer_set_deterministic(sb_trainer_t* t, int32_t on) {
+  SB_CHECK(t, SB_ERR_INVALID, "null trainer");
+  Net& n = t->net;
+  if ((on != 0) == n.det) return SB_OK;
+  SB_CHECK(!t->started && t->n_acc == 0 && t->global_step == 0, SB_ERR_STATE,
+           "sb_trainer_set_deterministic after the first step or graph capture: set it right after sb_trainer_create");
+  SB_CHECK(!t->p2p_ready, SB_ERR_STATE, "sb_trainer_set_deterministic after the peer exchange was set up: set it first");
+  if (!on) { n.det = false; return SB_OK; }
+  SB_CHECK(n.n_cat == 0, SB_ERR_STATE, "deterministic training of a wide+deep trainer: the embedding gradient is scatter-added "
+           "with red.global (embed_scatter_kernel), whose summation order is not fixed");
+  return n.enable_det();
 }
 
 static int stage_sparse_batch(Net& n, const float* Xd, const int32_t* idx, const float* y, const float* w, int rows) {
@@ -1191,6 +1220,7 @@ int sb_trainer_run_resident(sb_trainer_t* t, const int64_t* row_offsets, int32_t
              (long long)(row_offsets[i] + rows), (long long)t->ds_rows);
   constexpr int S = sb_trainer::RUN_S;
   int i = 0;
+  SB_TRY(check_det_exchange(t));
   if (t->dsXb != nullptr && t->prep != nullptr) {
     SB_CUDA(cudaSetDevice(n.device));
     if (!t->run_ready) {

@@ -162,4 +162,74 @@ __device__ __forceinline__ void colsum_row_groups(float (&v)[N_], int lane) {
   colsum_halve<N_ / 8>(v, lane, 4);
 }
 
+// element j (0..7) of 8 bf16 packed in a uint4, as fp32, from the words themselves (j a compile-time constant after
+// unrolling): no byte view of the vector, so it stays in registers
+__device__ __forceinline__ float bf16_of_u4(const uint4& v, int j) {
+  const uint32_t w = (j >> 1) == 0 ? v.x : (j >> 1) == 1 ? v.y : (j >> 1) == 2 ? v.z : v.w;
+  return __uint_as_float((j & 1) ? (w & 0xFFFF0000u) : (w << 16));
+}
+
+// ---- deterministic epilogues (DET = true instantiations, sb_trainer_set_deterministic) ----
+// A reduction over the CTAs of a launch: each CTA stores its partial sums with plain stores into its own slots of the
+// launch's workspace; the CTA that takes the last ticket adds the slots in ascending slot order and writes the result.
+// The order of the adds is fixed by slot index, never by arrival.
+//
+// det_last_cta is called by the `nthreads` threads of the CTA that stored slots (named barrier `bar`; `leader` is one of
+// them) after their slot stores.  It returns true in all of them in the last of the launch's `n_ctas` CTAs; that CTA has
+// already put the ticket back to 0, so the next launch (or graph replay) needs no memset.
+__device__ __forceinline__ bool det_last_cta(unsigned int* ticket, unsigned int n_ctas, int bar, int nthreads, bool leader) {
+  __threadfence();   // this thread's slot stores are visible device-wide before the CTA takes its ticket
+  asm volatile("bar.sync %0, %1;" ::"r"(bar), "r"(nthreads) : "memory");
+  int mine = 0, last = 0;
+  if (leader) mine = atomicAdd(ticket, 1u) == n_ctas - 1u ? 1 : 0;
+  asm volatile(
+      "{\n .reg .pred p, q;\n setp.ne.s32 p, %1, 0;\n bar.red.or.pred q, %2, %3, p;\n selp.s32 %0, 1, 0, q;\n}"
+      : "=r"(last) : "r"(mine), "r"(bar), "r"(nthreads) : "memory");
+  if (last) {
+    if (leader) *ticket = 0u;   // every CTA of this launch has taken its ticket
+    __threadfence();            // the other CTAs' slots are read after this (with ld.global.cg: not through L1)
+  }
+  return last != 0;
+}
+
+// det_last_cta + det_colsum_finish for the wgmma GEMMs' dA epilogues, called once after the tile loop.  Not inlined: the
+// ordered sum's loop would otherwise be scheduled into a kernel whose registers the accumulator already fills.
+static __device__ __noinline__ void det_colsum_tail(unsigned int* ticket, const float* slots, int n_slots, int N, float* dst, int bar,
+                                             int nthreads, int tid);
+
+// Ordered sum of column slots [n_slots][N] into dst[0, N) (dst[c] += sum over s of slots[s][c], s ascending)
+__device__ __forceinline__ void det_colsum_finish(const float* slots, int n_slots, int N, float* dst, int tid, int nthreads) {
+  for (int c = tid; c < N; c += nthreads) {
+    float s = 0.f;
+    for (int k = 0; k < n_slots; ++k) s += __ldcg(slots + static_cast<size_t>(k) * N + c);
+    dst[c] += s;
+  }
+}
+
+// Output layer's slots, per CTA: [loss sum, db_o, db_L[halves][H], dw_o[halves][H]] (halves = partial sums per column and
+// CTA).  Ordered sum over CTAs, then halves, into the step scalar and the flat gradient; loss / bwd select the outputs.
+__device__ __forceinline__ size_t det_out_stride(int H, int halves) { return 2 + 2 * static_cast<size_t>(halves) * H; }
+__device__ __forceinline__ void det_out_finish(const float* ws, int n_ctas, int H, int halves, bool loss, bool bwd, float* loss_dst,
+                                               float* g_bo, float* g_bL, float* g_wo, int tid, int nthreads) {
+  const size_t stride = det_out_stride(H, halves);
+  for (int j = tid; j < 2 + 2 * H; j += nthreads) {
+    if (j == 0 ? !loss : !bwd) continue;
+    size_t off;
+    float* dst;
+    int nh = halves;
+    if (j < 2) { off = j; dst = j == 0 ? loss_dst : g_bo; nh = 1; }
+    else if (j < 2 + H) { off = 2 + (j - 2); dst = g_bL + (j - 2); }
+    else { off = 2 + static_cast<size_t>(halves) * H + (j - 2 - H); dst = g_wo + (j - 2 - H); }
+    float s = 0.f;
+    for (int b = 0; b < n_ctas; ++b)
+      for (int h = 0; h < nh; ++h) s += __ldcg(ws + b * stride + off + static_cast<size_t>(h) * H);
+    *dst += s;
+  }
+}
+
+static __device__ __noinline__ void det_colsum_tail(unsigned int* ticket, const float* slots, int n_slots, int N, float* dst, int bar,
+                                             int nthreads, int tid) {
+  if (det_last_cta(ticket, gridDim.x, bar, nthreads, tid == 0)) det_colsum_finish(slots, n_slots, N, dst, tid, nthreads);
+}
+
 }  // namespace sb

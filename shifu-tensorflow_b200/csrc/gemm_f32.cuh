@@ -19,11 +19,14 @@ struct GemmF32Params {
   float* colsum;
   float* accum; int ld_acc;
   const float* addend; int ld_add;   // EPI_FWD, nullable: added to the pre-activation (wide+deep: the embedding sum)
+  float* det_ws; unsigned int* det_ticket;   // EPI_DA with DET: column-sum slots [row tile][N] and the launch's ticket
 };
 
-template <int EPI>
+// DET (EPI_DA only): the column sums go to slot blockIdx.y (the row tile) and the last CTA adds the row tiles in order
+template <int EPI, bool DET = false>
 __global__ void __launch_bounds__(256)
 gemm_f32_kernel(const GemmF32Params p) {
+  static_assert(!DET || EPI == EPI_DA, "DET: dA column sums only");
   constexpr int BM = 64, BN = 64, BK = 16;
   __shared__ float As[BK][BM + 4];
   __shared__ float Bs[BK][BN + 4];
@@ -113,13 +116,21 @@ gemm_f32_kernel(const GemmF32Params p) {
         float s = 0.f;
 #pragma unroll
         for (int r = 0; r < 16; ++r) s += red[r][tid];
-        if (n0 + tid < p.N) atomicAdd(p.colsum + n0 + tid, s);
+        if constexpr (DET) {
+          if (n0 + tid < p.N) p.det_ws[static_cast<size_t>(blockIdx.y) * p.N + n0 + tid] = s;
+        } else {
+          if (n0 + tid < p.N) atomicAdd(p.colsum + n0 + tid, s);
+        }
+      }
+      if constexpr (DET) {
+        if (det_last_cta(p.det_ticket, gridDim.x * gridDim.y * gridDim.z, 0, 256, tid == 0))
+          det_colsum_finish(p.det_ws, static_cast<int>(gridDim.y), p.N, p.colsum, tid, 256);
       }
     }
   }
 }
 
-template <int EPI>
+template <int EPI, bool DET = false>
 int launch_gemm_f32(GemmF32Params p, int split_k, cudaStream_t st) {
   const int total_kb = (p.K + 15) / 16;
   if (split_k < 1) split_k = 1;
@@ -128,7 +139,7 @@ int launch_gemm_f32(GemmF32Params p, int split_k, cudaStream_t st) {
   split_k = kb_per > 0 ? (total_kb + kb_per - 1) / kb_per : 1;
   p.k_per_split = kb_per * 16;
   dim3 grid((p.N + 63) / 64, (p.M + 63) / 64, split_k);
-  gemm_f32_kernel<EPI><<<grid, 256, 0, st>>>(p);
+  gemm_f32_kernel<EPI, DET><<<grid, 256, 0, st>>>(p);
   SB_CUDA(cudaGetLastError());
   return SB_OK;
 }

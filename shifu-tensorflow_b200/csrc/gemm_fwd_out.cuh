@@ -46,7 +46,9 @@ struct FwdOutCfg : RingCfg<64 * 64 * 2, BN * 64 * 2, 1024 + 256 + 2 * BN * 4 + 4
   static constexpr int EPI_THREADS = 256;           // the two consumer warpgroups
 };
 
-template <int BN, int ACT>
+// DET: the CTA's loss sum, db_o, db_L and dw_o go to its slots of p.det_ws (common.cuh, det_out_finish with halves = 1)
+// and the CTA that arrives last adds the CTAs in ascending order
+template <int BN, int ACT, bool DET = false>
 __global__ void __launch_bounds__(FwdOutCfg<BN>::THREADS, 1)
 gemm_fwd_out_kernel(const __grid_constant__ FwdOutTmaps tms, const GemmTcParams p) {
   using Cfg = FwdOutCfg<BN>;
@@ -260,8 +262,14 @@ gemm_fwd_out_kernel(const __grid_constant__ FwdOutTmaps tms, const GemmTcParams 
     if (et == 0) {
       float ls = 0.f, ds = 0.f;
       for (int w = 0; w < 4; ++w) { ls += lds(sm_lw + w * 8u); ds += lds(sm_lw + w * 8u + 4u); }
-      atomicAdd(p.scal + SCAL_LOSS_SUM, ls);
-      atomicAdd(p.g_bo, ds);
+      if constexpr (DET) {
+        float* slots = p.det_ws + blockIdx.x * det_out_stride(p.N, 1);
+        slots[0] = ls;
+        slots[1] = ds;
+      } else {
+        atomicAdd(p.scal + SCAL_LOSS_SUM, ls);
+        atomicAdd(p.g_bo, ds);
+      }
     }
     for (int j = et; j < BN && j < p.N; j += Cfg::EPI_THREADS) {
       float db = 0.f, dw = 0.f;
@@ -269,8 +277,19 @@ gemm_fwd_out_kernel(const __grid_constant__ FwdOutTmaps tms, const GemmTcParams 
         db += lds(sm_col + static_cast<uint32_t>(w * 2 * BN + j) * 4u);
         dw += lds(sm_col + static_cast<uint32_t>(w * 2 * BN + BN + j) * 4u);
       }
-      if (db != 0.f) red_add_f32(p.g_bL + j, db);
-      if (dw != 0.f) red_add_f32(p.g_wo + j, dw);
+      if constexpr (DET) {
+        float* slots = p.det_ws + blockIdx.x * det_out_stride(p.N, 1);
+        slots[2 + j] = db;
+        slots[2 + p.N + j] = dw;
+      } else {
+        if (db != 0.f) red_add_f32(p.g_bL + j, db);
+        if (dw != 0.f) red_add_f32(p.g_wo + j, dw);
+      }
+    }
+    if constexpr (DET) {
+      if (det_last_cta(p.det_ticket, gridDim.x, 1, Cfg::EPI_THREADS, et == 0))
+        det_out_finish(p.det_ws, static_cast<int>(gridDim.x), p.N, 1, true, true, p.scal + SCAL_LOSS_SUM, p.g_bo, p.g_bL, p.g_wo, et,
+                       Cfg::EPI_THREADS);
     }
     if (xthread) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // the last tiles are in global memory
   }
@@ -290,6 +309,8 @@ static int with_fwd_out_bn(int N, F&& f) {
 static int launch_gemm_fwd_out(int grid, const FwdOutTmaps& tms, const GemmTcParams& p, cudaStream_t st, bool pdl) {
   return with_fwd_out_bn(p.N, [&](auto BN) {
     return with_act(p.act, [&](auto ACT) {
+      if (p.det_ws != nullptr)   // DET: p.det_ws holds grid x (2 + 2 N) floats
+        return launch_kernel(gemm_fwd_out_kernel<BN, ACT, true>, grid, FwdOutCfg<BN>::THREADS, FwdOutCfg<BN>::SMEM_BYTES, st, pdl, tms, p);
       return launch_kernel(gemm_fwd_out_kernel<BN, ACT>, grid, FwdOutCfg<BN>::THREADS, FwdOutCfg<BN>::SMEM_BYTES, st, pdl, tms, p);
     });
   });
@@ -300,7 +321,10 @@ static int set_gemm_fwd_out_attrs() {
   for (int n : {64, 128, 256})
     for (int act = SB_ACT_NONE; act <= SB_ACT_LEAKYRELU; ++act)
       SB_TRY(with_fwd_out_bn(n, [&](auto BN) {
-        return with_act(act, [&](auto ACT) { return set_max_smem(gemm_fwd_out_kernel<BN, ACT>, FwdOutCfg<BN>::SMEM_BYTES); });
+        return with_act(act, [&](auto ACT) {
+          SB_TRY(set_max_smem(gemm_fwd_out_kernel<BN, ACT, true>, FwdOutCfg<BN>::SMEM_BYTES));
+          return set_max_smem(gemm_fwd_out_kernel<BN, ACT>, FwdOutCfg<BN>::SMEM_BYTES);
+        });
       }));
   return SB_OK;
 }

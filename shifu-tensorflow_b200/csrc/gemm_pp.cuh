@@ -46,10 +46,13 @@ struct GemmPpCfg : RingCfg<BM_WG * 64 * 2, BN * 64 * 2, 1024 + 256 + 2 * BN * 4 
   static constexpr int X_BYTES = X_TILE * (BN / 64);       // one group's epilogue buffer
 };
 
-template <int BM_WG, int BN, int EPI, int ACT>
+// DET (dA only): a tile's column sums are stored into slot m0 / BM_WG (its row tile) of p.det_ws [row tile][N] instead of
+// red.global, and the CTA that arrives last adds the row tiles in ascending order into p.colsum (common.cuh, det_last_cta)
+template <int BM_WG, int BN, int EPI, int ACT, bool DET = false>
 __global__ void __launch_bounds__(GemmPpCfg<BM_WG, BN>::THREADS, 1)
 gemm_pp_kernel(const __grid_constant__ PpTmaps tms, const GemmTcParams p) {
   static_assert(EPI == EPI_FWD || EPI == EPI_DA, "forward or dA");
+  static_assert(!DET || EPI == EPI_DA, "DET: dA column sums only");
   using Cfg = GemmPpCfg<BM_WG, BN>;
   constexpr int BK = Cfg::BK, MI = BM_WG / 64;
   constexpr bool B_MN = EPI == EPI_FWD;
@@ -215,10 +218,20 @@ gemm_pp_kernel(const __grid_constant__ PpTmaps tms, const GemmTcParams p) {
             asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(cb + (w * BN + j) * 4u) : "memory");
             v += x;
           }
-          if (n0 + j < p.N && v != 0.f) red_add_f32(p.colsum + n0 + j, v);
+          if constexpr (DET) {
+            if (n0 + j < p.N) p.det_ws[(t / tiles_n) * p.N + n0 + j] = v;   // row tile t / tiles_n (< 2^31 slots)
+          } else {
+            if (n0 + j < p.N && v != 0.f) red_add_f32(p.colsum + n0 + j, v);
+          }
         }
       }
       if (lt == 0 && threadIdx.x == 0) ring_stamp(p, tracing, 7);  // first tile's epilogue done
+    }
+    if constexpr (DET) {
+      // both consumer groups (named barrier 1, unused by the main loop) have stored the slots of all their tiles
+      // (nothing of the tile loop stays live for this: the predicate and the slot count come from the parameters)
+      if (p.colsum != nullptr)
+        det_colsum_tail(p.det_ticket, p.det_ws, (p.M + BM_WG - 1) / BM_WG, p.N, p.colsum, 1, 256, static_cast<int>(threadIdx.x));
     }
     if (xthread) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // the last tiles are in global memory
   }
@@ -282,12 +295,16 @@ static int with_pp_shape(int bm_wg, int bn, F&& f) {
   return set_error(SB_ERR_INVALID, "no gemm_pp instantiation for bm_wg=%d bn=%d", bm_wg, bn);
 }
 
-// tensor maps (pl.bm_wg-row boxes) must have been made for the same plan
+// tensor maps (pl.bm_wg-row boxes) must have been made for the same plan.  A dA launch with p.det_ws set runs the DET
+// instantiation (p.det_ws: [ceil(M / bm_wg)][N] floats).
 template <int EPI>
 static int launch_gemm_pp(const PpPlan& pl, const PpTmaps& tms, const GemmTcParams& p, cudaStream_t st, bool pdl) {
   return with_pp_shape(pl.bm_wg, pl.bn, [&](auto BM_WG, auto BN) {
     return with_act(p.act, [&](auto ACT) {
       using Cfg = GemmPpCfg<BM_WG, BN>;
+      if constexpr (EPI == EPI_DA)
+        if (p.det_ws != nullptr)
+          return launch_kernel(gemm_pp_kernel<BM_WG, BN, EPI, ACT, true>, pl.grid, Cfg::THREADS, Cfg::SMEM_BYTES, st, pdl, tms, p);
       return launch_kernel(gemm_pp_kernel<BM_WG, BN, EPI, ACT>, pl.grid, Cfg::THREADS, Cfg::SMEM_BYTES, st, pdl, tms, p);
     });
   });
@@ -302,6 +319,7 @@ static int set_gemm_pp_attrs() {
           return with_act(act, [&](auto ACT) {
             const int bytes = GemmPpCfg<BM_WG, BN>::SMEM_BYTES;
             SB_TRY(set_max_smem(gemm_pp_kernel<BM_WG, BN, EPI_FWD, ACT>, bytes));
+            SB_TRY(set_max_smem(gemm_pp_kernel<BM_WG, BN, EPI_DA, ACT, true>, bytes));
             return set_max_smem(gemm_pp_kernel<BM_WG, BN, EPI_DA, ACT>, bytes);
           });
         }));

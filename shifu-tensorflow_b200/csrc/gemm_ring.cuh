@@ -69,6 +69,9 @@ struct GemmTcParams {
   // gather (oracle/wide_deep.py) while this GEMM contracts only the dense columns.
   const float* addend;
   int ld_add;
+  // DET instantiations only (common.cuh, det_last_cta): the launch's slot workspace and ticket
+  float* det_ws;
+  unsigned int* det_ticket;
 };
 
 // Geometry of a ring GEMM: stages of A_BYTES + B_BYTES (one k-block) in the 227 KB of dynamic shared memory a block may

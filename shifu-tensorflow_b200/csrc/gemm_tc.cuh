@@ -65,9 +65,13 @@ __device__ __forceinline__ void epi_da_chunk(float (&v)[32], const __nv_bfloat16
 
 // GENERIC = true adds the cold features at compile time: split-precision part stores / loads (np > 1) and the fp32 addend
 // of the wide+deep first layer.  EPI_FWD / EPI_DA are instantiated with it only.
-template <int BN, int EPI, bool A_MN, bool B_MN, bool GENERIC = false>
+// DET (dA only, deterministic training): each epilogue warp stores its column sums into its own shared-memory slot
+// (plain st.shared instead of red.shared), the 4 warps of a column are added in warp order, the tile's sums go to row
+// tile tm of p.det_ws [tiles_m][N], and the CTA that arrives last adds the row tiles in order (common.cuh, det_last_cta).
+template <int BN, int EPI, bool A_MN, bool B_MN, bool GENERIC = false, bool DET = false>
 __global__ void __launch_bounds__(GemmTcCfg<BN>::THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
+  static_assert(!DET || EPI == EPI_DA, "DET: dA column sums only");
   using Cfg = GemmTcCfg<BN>;
   const int act_sel = p.act;
   constexpr int BM = Cfg::BM, BK = Cfg::BK;
@@ -145,15 +149,32 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
     // Column sums (bias gradients) are accumulated per CTA in shared memory and flushed to the flat gradient ONCE per tile
     // and column: one red.global per column per 128 rows instead of one per 32 rows (with one red per warp and chunk, the
     // wide dA GEMMs wait on the L2 atomic units).
-    // layout: [buffer (tile parity)][BN] floats
+    // layout: [buffer (tile parity)][BN] floats; DET: [buffer][quarter][BN] (8 BN floats = the 4096 bytes at BN = 128)
     const uint32_t sm_col = sm_vec + 2048u + static_cast<uint32_t>(Cfg::TR_BYTES);
+    static_assert(!DET || 8 * BN * 4 <= 4096, "DET column-sum slots");
     const int rt = quarter * 32 + lane;                                   // row of this thread inside the CTA's 128 rows
     auto col_slot = [&](int buf, int j) { return sm_col + static_cast<uint32_t>((buf * BN + j) * 4); };
     auto red_shared = [](uint32_t a, float v) { asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(a), "f"(v) : "memory"); };
-    if constexpr (EPI == EPI_DA) {
+    if constexpr (EPI == EPI_DA && !DET) {
       for (int j = et; j < 2 * BN; j += ET) asm volatile("st.shared.f32 [%0], %1;" ::"r"(sm_col + static_cast<uint32_t>(j) * 4u), "f"(0.f) : "memory");
       bar_all();
     }
+    // DET: after every epilogue warp has stored its sums of tile `it`: the 4 quarters in order, one slot store per column
+    // into row tile tm_ of p.det_ws (every column < N of the tile is written by all 4 quarters, so no clearing is needed)
+    auto flush_cols_det = [&](int it_, int tm_, int tn_) {
+      bar_all();
+      for (int j = et; j < BN; j += ET) {
+        const int col = tn_ * BN + j;
+        float vsum = 0.f;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          float x;
+          asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(sm_col + static_cast<uint32_t>(((it_ & 1) * 4 + q) * BN + j) * 4u) : "memory");
+          vsum += x;
+        }
+        if (col < p.N) p.det_ws[static_cast<size_t>(tm_) * p.N + col] = vsum;
+      }
+    };
     // after every epilogue warp has added its sums of tile `it`: one thread per column flushes and clears buffer it & 1
     auto flush_cols = [&](int it_, int tn_, float* dst) {
       bar_all();
@@ -402,7 +423,11 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
             if (p.colsum != nullptr) {
               // bias gradient: per-column sum over this warp's 32 rows, accumulated per CTA in shared memory
               const float s = warp_colsum_32x32(v, lane);
-              red_shared(col_slot(it & 1, c * 32 + lane), s);     // columns beyond N / rows beyond M were zeroed above
+              if constexpr (DET)   // this warp's own slot: one writer per address
+                asm volatile("st.shared.f32 [%0], %1;" ::"r"(sm_col + static_cast<uint32_t>(((it & 1) * 4 + quarter) * BN + c * 32 + lane) * 4u),
+                             "f"(s) : "memory");
+              else
+                red_shared(col_slot(it & 1, c * 32 + lane), s);     // columns beyond N / rows beyond M were zeroed above
             }
           }
         } else if constexpr (EPI == EPI_DW) {
@@ -446,10 +471,16 @@ gemm_tc_kernel(const __grid_constant__ TmapSet tms, const GemmTcParams p) {
           }
         }
       }
-      if constexpr (EPI == EPI_DA) {
+      if constexpr (DET) {
+        if (p.colsum != nullptr) flush_cols_det(it, tm, tn);
+      } else if constexpr (EPI == EPI_DA) {
         if (p.colsum != nullptr) flush_cols(it, tn, p.colsum);
       }
       if (w == w_first && threadIdx.x == 0) ring_stamp(p, tracing, 7);  // first tile's epilogue done
+    }
+    if constexpr (DET) {
+      // (named barrier 1 = every consumer warp; dA runs without split-K, so the work items are the tiles)
+      if (p.colsum != nullptr) det_colsum_tail(p.det_ticket, p.det_ws, (p.M + BM - 1) / BM, p.N, p.colsum, 1, ET, et);
     }
   }
   ring_exit(p, tracing);
@@ -477,7 +508,8 @@ struct GemmPlan {
   int split_k, kb_per_split;
   int grid;          // CTAs to launch
 };
-GemmPlan plan_gemm(int M, int N, int K, int num_sms, bool allow_split);
+// max_split > 0 caps the split-K factor (deterministic training: 2, see Net::enqueue_dw)
+GemmPlan plan_gemm(int M, int N, int K, int num_sms, bool allow_split, int max_split = 0);
 
 template <int EPI, bool A_MN, bool B_MN>
 int launch_gemm_tc(const GemmPlan& pl, const TmapSet& tms, GemmTcParams p, cudaStream_t st, bool pdl = false) {
@@ -487,6 +519,17 @@ int launch_gemm_tc(const GemmPlan& pl, const TmapSet& tms, GemmTcParams p, cudaS
   p.kb_per_split = pl.kb_per_split;
   // forward / dA: split-precision parts or an fp32 addend, the GENERIC instantiations (plain bf16 is gemm_pp.cuh)
   constexpr bool GENERIC = EPI == EPI_FWD || EPI == EPI_DA;
+  if constexpr (EPI == EPI_DA) {
+    if (p.det_ws != nullptr) {   // deterministic training: p.det_ws holds [ceil(M / 128)][N] floats
+      if (pl.bn == 64)
+        return launch_kernel(gemm_tc_kernel<64, EPI, A_MN, B_MN, true, true>, pl.grid, GemmTcCfg<64>::THREADS,
+                             GemmTcCfg<64>::SMEM_BYTES, st, pdl, tms, p);
+      if (pl.bn == 128)
+        return launch_kernel(gemm_tc_kernel<128, EPI, A_MN, B_MN, true, true>, pl.grid, GemmTcCfg<128>::THREADS,
+                             GemmTcCfg<128>::SMEM_BYTES, st, pdl, tms, p);
+      return set_error(SB_ERR_INVALID, "no gemm_tc instantiation for bn=%d", pl.bn);
+    }
+  }
   if (pl.bn == 64)
     return launch_kernel(gemm_tc_kernel<64, EPI, A_MN, B_MN, GENERIC>, pl.grid, GemmTcCfg<64>::THREADS, GemmTcCfg<64>::SMEM_BYTES,
                          st, pdl, tms, p);
@@ -500,6 +543,10 @@ int launch_gemm_tc(const GemmPlan& pl, const TmapSet& tms, GemmTcParams p, cudaS
 template <int EPI, bool A_MN, bool B_MN>
 int set_gemm_tc_attrs() {
   constexpr bool GENERIC = EPI == EPI_FWD || EPI == EPI_DA;
+  if constexpr (EPI == EPI_DA) {
+    SB_TRY((set_max_smem(gemm_tc_kernel<64, EPI, A_MN, B_MN, true, true>, GemmTcCfg<64>::SMEM_BYTES)));
+    SB_TRY((set_max_smem(gemm_tc_kernel<128, EPI, A_MN, B_MN, true, true>, GemmTcCfg<128>::SMEM_BYTES)));
+  }
   SB_TRY(set_max_smem(gemm_tc_kernel<64, EPI, A_MN, B_MN, GENERIC>, GemmTcCfg<64>::SMEM_BYTES));
   return set_max_smem(gemm_tc_kernel<128, EPI, A_MN, B_MN, GENERIC>, GemmTcCfg<128>::SMEM_BYTES);
 }

@@ -135,6 +135,8 @@ struct OutLayerParams {
   unsigned long long* trace;              // debug timeline (nullable): [0] entry, [2] deps resolved (block 0), [10] last exit
   int np;                                 // bf16 parts per value of A / dZ (split-precision modes; 0 or 1 = plain)
   long long a_ps, dz_ps;                  // element stride between parts
+  float* det_ws;                          // DET instantiations only (common.cuh, det_last_cta): slots and ticket
+  unsigned int* det_ticket;
 };
 
 // in-graph kernel span for the step timeline: begin = block 0's stamp after griddepcontrol.wait, end = atomicMax over blocks
@@ -152,7 +154,8 @@ template <typename T> __device__ __forceinline__ void st_from_float(T* p, float 
 template <> __device__ __forceinline__ void st_from_float<float>(float* p, float v) { *p = v; }
 template <> __device__ __forceinline__ void st_from_float<__nv_bfloat16>(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
 
-template <typename T>
+// DET: the per-block loss sum, db_o and the two row halves' dw_o / db_L go to the block's slots (det_out_finish, halves = 2)
+template <typename T, bool DET = false>
 __global__ void __launch_bounds__(256)
 out_layer_kernel(const OutLayerParams p) {
   trace_begin(p.trace, true);
@@ -208,17 +211,31 @@ out_layer_kernel(const OutLayerParams p) {
     if (tid == 0) {
       float s = 0.f;
       for (int i = 0; i < 8; ++i) s += blk_red[i];
-      atomicAdd(p.scal + SCAL_LOSS_SUM, s);
+      if constexpr (DET) p.det_ws[blockIdx.x * det_out_stride(p.H, 2)] = s;
+      else atomicAdd(p.scal + SCAL_LOSS_SUM, s);
     }
   }
-  if (!p.do_bwd) { trace_end(p.trace); return; }
+  float* const slots = DET ? p.det_ws + blockIdx.x * det_out_stride(p.H, 2) : nullptr;
+  auto det_finish = [&]() {
+    if (det_last_cta(p.det_ticket, gridDim.x, 0, 256, tid == 0))
+      det_out_finish(p.det_ws, static_cast<int>(gridDim.x), p.H, 2, p.do_loss != 0, p.do_bwd != 0, p.scal + SCAL_LOSS_SUM, p.g_bo,
+                     p.g_bL, p.g_wo, tid, 256);
+  };
+  if (!p.do_bwd) {
+    if constexpr (DET) det_finish();
+    trace_end(p.trace);
+    return;
+  }
   __syncthreads();
 
   // ---- phase 2: rank-1 backward over column chunks of 128 ----
   float dbo = 0.f;
   if (tid < 32) {
     dbo = warp_sum(dz_row[tid]);
-    if (tid == 0) atomicAdd(p.g_bo, dbo);
+    if (tid == 0) {
+      if constexpr (DET) slots[1] = dbo;
+      else atomicAdd(p.g_bo, dbo);
+    }
   }
   T* __restrict__ dZ = reinterpret_cast<T*>(p.dZ);
   for (int c0 = 0; c0 < p.H; c0 += 128) {
@@ -242,10 +259,16 @@ out_layer_kernel(const OutLayerParams p) {
       }
     }
     if (j < p.H) {
-      atomicAdd(p.g_wo + j, s_dw);
-      atomicAdd(p.g_bL + j, s_db);
+      if constexpr (DET) {
+        slots[2 + rh * p.H + j] = s_db;
+        slots[2 + (2 + rh) * p.H + j] = s_dw;
+      } else {
+        atomicAdd(p.g_wo + j, s_dw);
+        atomicAdd(p.g_bL + j, s_db);
+      }
     }
   }
+  if constexpr (DET) det_finish();
   trace_end(p.trace);
 }
 
@@ -255,7 +278,8 @@ out_layer_kernel(const OutLayerParams p) {
 // reduction and the dw_o / db_L column sums stay in registers over all rows of the warp; a block reduces them through
 // shared memory and issues ONE atomic per column (the 32-rows-per-block kernel above reads A_L twice with 2-byte
 // accesses).
-template <int NCH>
+// DET: the block's sums go to its slots (det_out_finish, halves = 1) instead of one atomic per column
+template <int NCH, bool DET = false>
 __global__ void __launch_bounds__(256)
 out_layer_rows_kernel(const OutLayerParams p, int rows_per_block) {
   trace_begin(p.trace, true);
@@ -290,15 +314,19 @@ out_layer_rows_kernel(const OutLayerParams p, int rows_per_block) {
       const int col0 = c * 256 + lane * 8;
       uint4 raw = make_uint4(0, 0, 0, 0);
       if (col0 < p.ldA && col0 < p.H) raw = *reinterpret_cast<const uint4*>(A + static_cast<size_t>(r) * p.ldA + col0);
-      const __nv_bfloat16* h = reinterpret_cast<const __nv_bfloat16*>(&raw);
 #pragma unroll
-      for (int k = 0; k < 8; ++k) a[c][k] = (col0 + k < p.H) ? __bfloat162float(h[k]) : 0.f;   // pad columns of A_L hold act(0), not 0
+      for (int k = 0; k < 8; ++k) {   // pad columns of A_L hold act(0), not 0
+        if constexpr (DET) a[c][k] = (col0 + k < p.H) ? bf16_of_u4(raw, k) : 0.f;   // no byte view of raw: registers only
+        else a[c][k] = (col0 + k < p.H) ? __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(&raw)[k]) : 0.f;
+      }
       for (int part = 1; part < p.np; ++part) {       // split-precision modes: add the lower parts
         uint4 lo = make_uint4(0, 0, 0, 0);
         if (col0 < p.ldA && col0 < p.H) lo = *reinterpret_cast<const uint4*>(A + part * p.a_ps + static_cast<size_t>(r) * p.ldA + col0);
-        const __nv_bfloat16* hl = reinterpret_cast<const __nv_bfloat16*>(&lo);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) a[c][k] += (col0 + k < p.H) ? __bfloat162float(hl[k]) : 0.f;
+        for (int k = 0; k < 8; ++k) {
+          if constexpr (DET) a[c][k] += (col0 + k < p.H) ? bf16_of_u4(lo, k) : 0.f;
+          else a[c][k] += (col0 + k < p.H) ? __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(&lo)[k]) : 0.f;
+        }
       }
 #pragma unroll
       for (int k = 0; k < 8; ++k) z = fmaf(a[c][k], wo[c][k], z);
@@ -352,10 +380,25 @@ out_layer_rows_kernel(const OutLayerParams p, int rows_per_block) {
   if (tid == 0) {
     float l = 0.f, d = 0.f;
     for (int i = 0; i < 8; ++i) { l += red_s[0][i]; d += red_s[1][i]; }
-    if (p.do_loss) atomicAdd(p.scal + SCAL_LOSS_SUM, l);
-    if (p.do_bwd) atomicAdd(p.g_bo, d);
+    if constexpr (DET) {
+      float* slots = p.det_ws + blockIdx.x * det_out_stride(p.H, 1);
+      slots[0] = l;
+      slots[1] = d;
+    } else {
+      if (p.do_loss) atomicAdd(p.scal + SCAL_LOSS_SUM, l);
+      if (p.do_bwd) atomicAdd(p.g_bo, d);
+    }
   }
-  if (!p.do_bwd) { trace_end(p.trace); return; }
+  auto det_finish = [&]() {
+    if (det_last_cta(p.det_ticket, gridDim.x, 0, 256, tid == 0))
+      det_out_finish(p.det_ws, static_cast<int>(gridDim.x), p.H, 1, p.do_loss != 0, p.do_bwd != 0, p.scal + SCAL_LOSS_SUM, p.g_bo,
+                     p.g_bL, p.g_wo, tid, 256);
+  };
+  if (!p.do_bwd) {
+    if constexpr (DET) det_finish();
+    trace_end(p.trace);
+    return;
+  }
 #pragma unroll
   for (int c = 0; c < NCH; ++c) {
     if (c * 256 >= p.H) break;
@@ -368,10 +411,17 @@ out_layer_rows_kernel(const OutLayerParams p, int rows_per_block) {
       float dw = 0.f, db = 0.f;
 #pragma unroll
       for (int i = 0; i < 8; ++i) { dw += red[0][i][tid]; db += red[1][i][tid]; }
-      atomicAdd(p.g_wo + j, dw);
-      atomicAdd(p.g_bL + j, db);
+      if constexpr (DET) {
+        float* slots = p.det_ws + blockIdx.x * det_out_stride(p.H, 1);
+        slots[2 + j] = db;
+        slots[2 + p.H + j] = dw;
+      } else {
+        atomicAdd(p.g_wo + j, dw);
+        atomicAdd(p.g_bL + j, db);
+      }
     }
   }
+  if constexpr (DET) det_finish();
   trace_end(p.trace);
 }
 

@@ -82,7 +82,7 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rows, int cols, int l
 //     plan, no more k-blocks x tile width per CTA, and >= 32 k-blocks per split.  The wider tile reads fewer shared-memory
 //     operand bytes per flop, but needs twice the split-K factor for the same grid - twice the red.global traffic into
 //     the gradient - and a split of few k-blocks is mostly the ring's fill and drain.
-GemmPlan plan_gemm(int M, int N, int K, int num_sms, bool allow_split) {
+GemmPlan plan_gemm(int M, int N, int K, int num_sms, bool allow_split, int max_split) {
   const int total_kb = (K + 63) / 64;
   auto tiles_of = [&](int bn) { return ((M + 127) / 128) * ((N + bn - 1) / bn); };
   auto plan = [&](int bn) {
@@ -92,6 +92,7 @@ GemmPlan plan_gemm(int M, int N, int K, int num_sms, bool allow_split) {
       split = num_sms / tiles;
       const int cap = total_kb / 8;
       if (split > cap) split = cap;
+      if (max_split > 0 && split > max_split) split = max_split;
       if (split < 1) split = 1;
     }
     if (split > total_kb) split = total_kb;
@@ -284,6 +285,7 @@ int Net::init(const sb_net_desc* d, int device_, bool training_) {
     const int co = cudaSharedmemCarveoutMaxShared;
     cudaFuncSetAttribute(load_batch_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, co);
     cudaFuncSetAttribute(out_layer_kernel<__nv_bfloat16>, cudaFuncAttributePreferredSharedMemoryCarveout, co);
+    cudaFuncSetAttribute(out_layer_kernel<__nv_bfloat16, true>, cudaFuncAttributePreferredSharedMemoryCarveout, co);
   }
   return SB_OK;
 }
@@ -306,6 +308,34 @@ int Net::set_sparse(int n_dense_, int n_onehot_, int n_cat_) {
   if (!idx) SB_TRY(dalloc(&idx, static_cast<size_t>(max_batch) * n_cat));
   if (!E) SB_TRY(dalloc(&E, static_cast<size_t>(max_batch) * layers[0].ld_out));
   SB_CUDA(cudaStreamSynchronize(stream));
+  return SB_OK;
+}
+
+// Slot workspaces of the deterministic epilogues, one per launch site, sized for max_batch rows: the output layer has at
+// most max(2 SMs + 2, max_batch / 32) CTAs (fused: one per SM; out_layer_rows_kernel: ~2 per SM; out_layer_kernel: 32
+// rows each) of 2 + 4 h_L slots; dA_l has one slot row per 64-row tile (the smallest dA tile) and column of in_l.
+// Reuse: a site's slots and ticket are written and read only by that site's launch, and all of a site's launches go to
+// the net's main stream, where two of them are always separated by complete kernels:
+//   - PDL: griddepcontrol.launch_dependents lets the next kernel START early, but every kernel of the chain executes
+//     griddepcontrol.wait before its first global access, and that returns only once the preceding grid has completed
+//     and flushed its memory - the last CTA's ordered sum included.  So the next launch of the same site cannot store
+//     into the slots while the last CTA still reads them.
+//   - The dW side stream runs beside the dA chain, but the dW GEMMs use no workspace (red.global with split-K <= 2).
+//   - set_batch_kernel on the prep stream writes the next step's descriptor and scalars, never a slot or a ticket.
+//   - eval_loss / loss_resident use the output layer's site on the same main stream, behind or ahead of whole steps.
+// The ticket is put back to 0 by the last CTA of each launch, so a graph replay starts from 0 without a memset node.
+int Net::enable_det() {
+  if (det_tickets) { det = true; return SB_OK; }
+  SB_CUDA(cudaSetDevice(device));
+  const Layer& hl = layers[L - 1];
+  const long long ctas = std::max<long long>(2LL * num_sms + 2, (max_batch + 31) / 32);
+  SB_TRY(dalloc(&det_out_ws, static_cast<size_t>(ctas) * (2 + 4 * static_cast<size_t>(hl.out))));
+  det_col_ws.assign(L, nullptr);
+  for (int l = 1; l < L; ++l)
+    SB_TRY(dalloc(&det_col_ws[l], static_cast<size_t>((max_batch + 63) / 64) * layers[l - 1].out));
+  SB_TRY(dalloc(&det_tickets, static_cast<size_t>(L)));
+  SB_CUDA(cudaStreamSynchronize(stream));
+  det = true;
   return SB_OK;
 }
 
@@ -394,6 +424,7 @@ int Net::enqueue_hidden_forward(const StepIn& in, int rows, float* grad, bool* f
         p.wo = theta + ol.w_off; p.bo = theta + ol.b_off;
         p.desc = in.desc; p.scal = in.scal; p.loss = loss;
         p.g_wo = grad + ol.w_off; p.g_bo = grad + ol.b_off; p.g_bL = grad + ly.b_off;
+        if (det) { p.det_ws = det_out_ws; p.det_ticket = det_tickets; }
         p.trace = next_trace("fwd_out", l, rows, ly.out, k_in);
         SB_TRY(launch_gemm_fwd_out(grid, ft, p, stream, true));
         if (fused_out) *fused_out = true;
@@ -449,6 +480,8 @@ int Net::enqueue_out(const StepIn& in, int rows, bool do_loss, bool do_bwd, floa
   if (do_bwd) {
     p.g_wo = grad + ol.w_off; p.g_bo = grad + ol.b_off; p.g_bL = grad + hl.b_off;
   }
+  const bool d = det && (do_loss || do_bwd);   // the DET instantiations (slots + last-CTA sum) when anything is summed
+  if (d) { p.det_ws = det_out_ws; p.det_ticket = det_tickets; }
   const int grid = (rows + 31) / 32;
   if (tc()) {
     p.A = A[L - 1]; p.ldA = hl.ld_out;
@@ -460,16 +493,23 @@ int Net::enqueue_out(const StepIn& in, int rows, bool do_loss, bool do_bwd, floa
       rpb = ((rpb + 7) / 8) * 8;
       if (rpb < 8) rpb = 8;
       const dim3 g((rows + rpb - 1) / rpb);
-      if (hl.out <= 256) SB_TRY(launch_kernel(out_layer_rows_kernel<1>, g, dim3(256), 0, stream, true, p, rpb));
+      if (d) {
+        if (hl.out <= 256) SB_TRY(launch_kernel(out_layer_rows_kernel<1, true>, g, dim3(256), 0, stream, true, p, rpb));
+        else if (hl.out <= 512) SB_TRY(launch_kernel(out_layer_rows_kernel<2, true>, g, dim3(256), 0, stream, true, p, rpb));
+        else SB_TRY(launch_kernel(out_layer_rows_kernel<4, true>, g, dim3(256), 0, stream, true, p, rpb));
+      } else if (hl.out <= 256) SB_TRY(launch_kernel(out_layer_rows_kernel<1>, g, dim3(256), 0, stream, true, p, rpb));
       else if (hl.out <= 512) SB_TRY(launch_kernel(out_layer_rows_kernel<2>, g, dim3(256), 0, stream, true, p, rpb));
       else SB_TRY(launch_kernel(out_layer_rows_kernel<4>, g, dim3(256), 0, stream, true, p, rpb));
+    } else if (d) {
+      SB_TRY(launch_kernel(out_layer_kernel<__nv_bfloat16, true>, dim3(grid), dim3(256), 0, stream, true, p));
     } else {
       SB_TRY(launch_kernel(out_layer_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, stream, true, p));
     }
   } else {
     p.A = Af[L - 1]; p.ldA = hl.out;
     if (do_bwd) { p.dZ = dZf[L - 1]; p.ld_dZ = hl.out; }
-    SB_TRY(launch_kernel(out_layer_kernel<float>, dim3(grid), dim3(256), 0, stream, true, p));
+    if (d) SB_TRY(launch_kernel(out_layer_kernel<float, true>, dim3(grid), dim3(256), 0, stream, true, p));
+    else SB_TRY(launch_kernel(out_layer_kernel<float>, dim3(grid), dim3(256), 0, stream, true, p));
   }
   SB_CUDA(cudaGetLastError());
   mark("out_layer");
@@ -492,6 +532,7 @@ int Net::enqueue_dw(const StepIn& in, int l, int rows, float* grad, cudaStream_t
     int split = (2 * num_sms) / (tiles > 0 ? tiles : 1);
     const int cap = (rows + 63) / 64;
     if (split > cap) split = cap;
+    if (det && split > 2) split = 2;   // at most two atomic addends per element (see dw_max_split)
     SB_TRY(launch_gemm_f32<EPI_DW>(p, split, st));
     mark("gemm_f32<DW>");
     return SB_OK;
@@ -501,7 +542,7 @@ int Net::enqueue_dw(const StepIn& in, int l, int rows, float* grad, cudaStream_t
   const int ld_k = sp0 ? ldD : ly.ld_in;
   const __nv_bfloat16* ap = (l == 0) ? (res0 ? resident_Xb : Xb) : A[l - 1];
   const long long ap_ps = (l == 0) ? (res0 ? resident_ps : Xb_ps) : A_ps[l - 1];
-  const GemmPlan pl = plan_gemm(r1 - r0, ly.out, round_up(rows, 64) * pairs_of(nparts), sms, true);
+  const GemmPlan pl = plan_gemm(r1 - r0, ly.out, round_up(rows, 64) * pairs_of(nparts), sms, true, dw_max_split());
   TmapSet tm;
   // resident set: rows past the batch end are real rows of other batches; the B operand (dZ_l, extent = rows) is
   // zero-filled there, so they contribute nothing
@@ -536,7 +577,12 @@ int Net::enqueue_da(int l, int rows, float* grad) {
     p.aux = Af[l - 1]; p.ld_aux = pl.out;
     p.out = dZf[l - 1]; p.ld_out = pl.out;
     p.colsum = grad + pl.b_off;
-    SB_TRY(launch_gemm_f32<EPI_DA>(p, 1, stream));
+    if (det) {
+      p.det_ws = det_col_ws[l]; p.det_ticket = det_tickets + l;
+      SB_TRY((launch_gemm_f32<EPI_DA, true>(p, 1, stream)));
+    } else {
+      SB_TRY(launch_gemm_f32<EPI_DA>(p, 1, stream));
+    }
     mark("gemm_f32<DA>");
     return SB_OK;
   }
@@ -549,6 +595,7 @@ int Net::enqueue_da(int l, int rows, float* grad) {
   p.out = dZ[l - 1]; p.ld_out = pl.ld_out; p.out_ps = A_ps[l - 1];
   p.colsum = grad + pl.b_off;
   p.trace = next_trace("dA", l, rows, ly.in, ly.out);
+  if (det) { p.det_ws = det_col_ws[l]; p.det_ticket = det_tickets + l; }
   if (nparts == 1) {                           // plain bf16: the ping-pong kernel
     const PpPlan pp = plan_gemm_pp(rows, ly.in, ly.out, num_sms, false);
     PpTmaps pt;

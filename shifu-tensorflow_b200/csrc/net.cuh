@@ -133,6 +133,16 @@ struct Net {
                  int chunk = -1);
   // dZ_{l-1} = (dZ_l W_l^T) .* act'(A_{l-1}) and the bias gradient of layer l-1, on the main stream
   int enqueue_da(int l, int rows, float* grad);
+
+  // Deterministic training (sb_trainer_set_deterministic, DESIGN §6b).  Every launch that sums over CTAs runs its DET
+  // instantiation: partials into the launch site's own slots, the last CTA adds them in slot order.  dW GEMMs keep their
+  // red.global epilogue with split-K capped at 2 (two addends onto a zeroed element: 0 + a + b == 0 + b + a).
+  bool det = false;
+  float* det_out_ws = nullptr;            // output layer (fused or not): [CTA][2 + 4 h_L]
+  std::vector<float*> det_col_ws;         // det_col_ws[l], dA_l (l >= 1): column-sum slots [64-row tile][in_l]
+  unsigned int* det_tickets = nullptr;    // [L]: 0 = output layer, l = dA_l
+  int enable_det();                       // allocates the workspaces for max_batch rows (once)
+  int dw_max_split() const { return det ? 2 : 0; }
 };
 
 int validate_desc(const sb_net_desc* d);

@@ -28,6 +28,10 @@ Optional ModelConfig train.params the reference does not have (defaults = refere
              local step is dropped, after R = replicas_to_aggregate accepted pushes their MEAN is applied as ONE update
              (class SyncReplicasSchedule below restates the token / accumulator bookkeeping on the host)
              | "batch" (one update per mini-batch, the north-star wording)
+  Deterministic  true | false (default): every reduction of a training step is added in a fixed order
+             (sb_trainer_set_deterministic), so a run with the same data, SB_SEED, configuration, build, GPU model and
+             worker count reproduces its model bit for bit.  Every Precision; not with wide+deep columns; several
+             workers need the peer-memory exchange (all ranks on one host)
 
 File paths (TRAINING_DATA_PATH, TMP_MODEL_PATH, FINAL_MODEL_PATH) may carry a scheme.  The stock AM hands out fully
 qualified HDFS URIs (TrainingDataSet.java:74) which the reference reads through tf.gfile; here `hdfs://`, `viewfs://`,
@@ -91,6 +95,16 @@ def generate_from_modelconf(model_conf: dict):
     num_hidden_nodes = [int(s) for s in train_params['NumHiddenNodes']]
     activation_func = [get_activation_fun(s) for s in train_params['ActivationFunc']]
     return num_hidden_nodes[:num_hidden_layer], activation_func[:num_hidden_layer]
+
+
+def deterministic_requested(params: dict) -> bool:
+    """train.params.Deterministic: a JSON bool, or the strings true / false"""
+    v = params.get('Deterministic', False)
+    if isinstance(v, str):
+        if v.strip().lower() not in ('true', 'false'):
+            raise ValueError("train.params.Deterministic must be true or false, got %r" % v)
+        return v.strip().lower() == 'true'
+    return bool(v)
 
 
 def model(feature_count: int, model_conf: Optional[dict], max_batch: int) -> capi.NetDesc:
@@ -547,6 +561,10 @@ def main(_=None, env=None, rng=random) -> int:
     if schedule not in ('sync_replicas', 'epoch', 'batch'):
         raise ValueError("train.params.Schedule must be sync_replicas (alias epoch) or batch, got %r" % schedule)
     per_batch_update = schedule == 'batch'
+    deterministic = deterministic_requested(params)
+    if deterministic and wide_deep:
+        raise ValueError("train.params.Deterministic with wide+deep columns: the embedding gradient is scatter-added in no "
+                         "fixed order; train the dense model (SELECTED_COLUMN_NUMS) or drop Deterministic")
 
     device = int(env.get("SB_DEVICE", env.get("LOCAL_RANK", "0")))
     if env.get("SB_HOST_LOADER", "0") == "1":
@@ -622,9 +640,16 @@ def main(_=None, env=None, rng=random) -> int:
     rdv = Rendezvous(cluster_spec, task_index, n_workers)
     nccl_id = exchange_nccl_id(rdv)
     trainer = capi.Trainer(desc, device=device, nccl_id=nccl_id, rank=task_index, world=n_workers)
+    if deterministic:
+        trainer.set_deterministic(True)   # before the peer exchange is set up and before the first step
+    peer = False
     if n_workers > 1 and env.get("SB_EXCHANGE", "p2p") != "nccl":
-        if enable_peer_exchange(trainer, rdv):
+        peer = enable_peer_exchange(trainer, rdv)
+        if peer:
             logging.info("gradient exchange: peer-memory kernels (all %d ranks on this host)" % n_workers)
+    if deterministic and n_workers > 1 and not peer:
+        raise ValueError("train.params.Deterministic with %d workers needs the peer-memory exchange (all ranks on one host), "
+                         "which could not be enabled; NCCL's all-reduce adds in no fixed order" % n_workers)
     # The reference has ONE copy of the variables (on the parameter servers); the chief alone initialises or restores it
     # (MonitoredTrainingSession(is_chief=...), ssgd_monitor.py:251-257).  Replicas: worker 0 initialises / restores, then
     # parameters, optimizer state and global_step are broadcast, so every rank starts from the same state and runs the
