@@ -187,6 +187,16 @@ int sb_trainer_accumulate_resident(sb_trainer_t* t, int64_t row_offset, int32_t 
 /* forward + loss only over resident rows, no gradient, no update: what a sess.run whose push the accumulator drops as stale
  * still reports (its loss), ssgd_monitor.py:276 */
 int sb_trainer_loss_resident(sb_trainer_t* t, int64_t row_offset, int32_t rows, float* loss_out);
+/* Read the resident set through a row order: after this call, the resident entry points (step_resident[_async],
+ * run_resident, accumulate_resident, loss_resident) address logical row r as row rows[r] of the set loaded by
+ * sb_trainer_load_dataset, and check their offsets against n instead of the set's length.  Any list of in-range rows
+ * (1 <= n < 2^31; repeats allowed), HOST memory; it is copied (4 bytes per row on the device), and checked on the host
+ * before any device work (SB_ERR_INVALID).  rows == NULL with n == 0 goes back to the physical order.  SB_ERR_STATE
+ * without a resident set.  Loading a new set drops the order.  Waits for the queued steps; captured step graphs are
+ * reused.  eval_loss, predict, host-batch and sparse steps are unaffected.  An ordered step gathers its batch into the
+ * step's batch buffer first (gather_batch_kernel) - every epoch can draw new mini-batches without a second copy of the
+ * set. */
+int sb_trainer_set_row_order(sb_trainer_t* t, const int64_t* rows, int64_t n);
 int sb_trainer_last_loss(sb_trainer_t* t, float* loss_out);
 /* the loss curve: mini-batch loss of update steps first_step .. first_step + n - 1 (1-based global_step values; the last
  * 8192 steps are kept).  Every step's tail kernel posts its (loss sum, n_nz) into pinned host memory, so asynchronous

@@ -112,6 +112,7 @@ PROTOTYPES = {
     "sb_trainer_step_resident_async": (C.c_int, [_vp, C.c_int64, C.c_int32]),
     "sb_trainer_run_resident": (C.c_int, [_vp, C.POINTER(C.c_int64), C.c_int32, C.c_int32]),
     "sb_trainer_accumulate_resident": (C.c_int, [_vp, C.c_int64, C.c_int32, _f32p]),
+    "sb_trainer_set_row_order": (C.c_int, [_vp, C.POINTER(C.c_int64), C.c_int64]),
     "sb_trainer_last_loss": (C.c_int, [_vp, _f32p]),
     "sb_trainer_loss_history": (C.c_int, [_vp, C.c_int64, C.c_int32, _f32p]),
     "sb_trainer_sync": (C.c_int, [_vp]),
@@ -441,6 +442,15 @@ class Trainer:
         loss = C.c_float()
         check(lib().sb_trainer_accumulate_resident(self._h, row_offset, rows, C.byref(loss)))
         return float(loss.value)
+
+    def set_row_order(self, rows=None):
+        """the resident steps read logical row r as row rows[r] of the loaded set (sb_trainer_set_row_order); None: the
+        physical order"""
+        if rows is None:
+            check(lib().sb_trainer_set_row_order(self._h, None, 0))
+            return
+        order = np.ascontiguousarray(rows, dtype=np.int64).reshape(-1)
+        check(lib().sb_trainer_set_row_order(self._h, order.ctypes.data_as(C.POINTER(C.c_int64)), order.size))
 
     def last_loss(self) -> float:
         loss = C.c_float()

@@ -46,8 +46,14 @@ struct sb_trainer {
   __nv_bfloat16* dsXb = nullptr;                           // bf16 mode: the set in GEMM-operand form [ds_rows, ldF]
   int* dsP = nullptr;                                      // prefix counts of non-zero weights [ds_rows + 1]
   long long ds_rows = 0;
-  std::map<std::pair<int, int>, cudaGraphExec_t> graphs;  // (rows, kind * 8 + sparse * 4 + resident * 2 + pair) -> captured step
-  std::map<int, int> kernels_per_step;
+  // row order of the resident set (sb_trainer_set_row_order): the resident entry points address logical row r as row
+  // ord[r] (int32 on the device, the only per-row memory an order costs); ord_n == 0: physical order
+  int* ord = nullptr;
+  long long ord_n = 0, ord_cap = 0;
+  float *ordY = nullptr, *ordW = nullptr;   // [max_batch] labels / weights of an ordered step's batch (gather_batch_kernel)
+  // (rows, ordered * 16 + kind * 8 + sparse * 4 + resident * 2 + pair) -> captured step
+  std::map<std::pair<int, int>, cudaGraphExec_t> graphs;
+  std::map<int, int> kernels_per_step;   // rows * 2 + ordered
   // peer-memory exchange (xchg_p2p.cuh): the net's parameter arena [theta | s1 | s2 | shadows | gradient | P2PFlags] is
   // ONE exported allocation; `xch` aliases it
   void* xch = nullptr;
@@ -106,7 +112,7 @@ struct sb_trainer {
   bool run_ready = false;  // every descriptor, scalar block and event of both sets exists
   bool run_used[2] = {false, false};
   unsigned long long run_chunks = 0;
-  std::map<int, cudaGraphExec_t> run_graphs;   // rows * 2 + set
+  std::map<int, cudaGraphExec_t> run_graphs;   // (rows * 2 + set) * 2 + ordered
 
   // Releases what the trainer created.  Pointers into the net's allocations (descs, scals, grad, flags, xch, s1, s2, acc,
   // st2*, run_descs, run_scals) are freed by `net`, the first member and so the last destroyed.
@@ -146,7 +152,14 @@ struct sb_trainer {
     if (dsY) cudaFree(dsY);
     if (dsW) cudaFree(dsW);
     dsX = dsY = dsW = nullptr; dsXb = nullptr; dsP = nullptr; ds_rows = 0;
+    drop_row_order();
   }
+  void drop_row_order() {
+    if (ord) cudaFree(ord);
+    ord = nullptr;
+    ord_n = ord_cap = 0;
+  }
+  long long resident_len() const { return ord_n > 0 ? ord_n : ds_rows; }   // what resident offsets are checked against
   void close_peer_mappings() {
     for (void* p : peer_bases) cudaIpcCloseMemHandle(p);
     peer_bases.clear();
@@ -460,6 +473,28 @@ static int enqueue_step_backward(sb_trainer* t, const StepIn& in, int rows, int 
   return SB_OK;
 }
 
+// first kernel of an ordered step, in load_batch_kernel's place: the batch's rows of the resident set through the order
+// slice in.desc->order into Xb / Xf, ordY / ordW and the step scalars; clears clear[0, clear_n) on the way
+static int enqueue_gather(sb_trainer* t, const StepIn& in, int rows, float* clear, long long clear_n) {
+  Net& n = t->net;
+  GatherParams p = {};
+  p.desc = in.desc;
+  p.rows = rows; p.F = n.F; p.ldF = n.ldF; p.np = n.nparts;
+  p.src_b = t->dsXb; p.src_ps = n.resident_ps; p.Xb = n.Xb; p.Xb_ps = n.Xb_ps;
+  p.src_f = t->dsX; p.Xf = n.Xf;
+  p.src_y = t->dsY; p.src_w = t->dsW; p.y = t->ordY; p.w = t->ordW;
+  p.scal = in.scal;
+  p.zero_buf = clear; p.zero_n = clear_n;
+  p.trace = n.next_trace("gather_batch");
+  const long long units = static_cast<long long>(rows) * (n.tc() ? n.ldF / 8 : (n.F + 3) / 4);
+  const long long blocks = std::max(1LL, std::min((units + 255) / 256, static_cast<long long>(n.num_sms) * 16));
+  const dim3 g(static_cast<unsigned>(blocks));
+  if (n.tc()) SB_TRY(launch_kernel(gather_batch_kernel<true>, g, dim3(256), 0, n.stream, true, p));
+  else SB_TRY(launch_kernel(gather_batch_kernel<false>, g, dim3(256), 0, n.stream, true, p));
+  n.mark("gather_batch");
+  return SB_OK;
+}
+
 // the body of one step as a sequence of stream operations (captured into a CUDA graph)
 static int enqueue_step_body(sb_trainer* t, const StepIn& in, int rows, int kind) {
   Net& n = t->net;
@@ -477,6 +512,8 @@ static int enqueue_step_body(sb_trainer* t, const StepIn& in, int rows, int kind
     } else {
       SB_CUDA(cudaMemsetAsync(t->grad, 0, sizeof(float) * n.n_params, n.stream));
     }
+  } else if (in.ordered) {
+    SB_TRY(enqueue_gather(t, in, rows, t->grad, n.n_params));
   } else {
     SB_TRY(n.enqueue_load(in, rows, t->grad, n.n_params));   // also clears the gradient buffer and the step scalars
   }
@@ -487,7 +524,7 @@ static int enqueue_step_body(sb_trainer* t, const StepIn& in, int rows, int kind
 }
 
 static int get_graph(sb_trainer* t, const StepIn& in, int rows, int kind, int pair, cudaGraphExec_t* out) {
-  auto key = std::make_pair(rows, kind * 8 + (in.sparse ? 4 : 0) + (in.resident ? 2 : 0) + pair);
+  auto key = std::make_pair(rows, (in.ordered ? 16 : 0) + kind * 8 + (in.sparse ? 4 : 0) + (in.resident ? 2 : 0) + pair);
   auto it = t->graphs.find(key);
   if (it != t->graphs.end()) { *out = it->second; return SB_OK; }
   Net& n = t->net;
@@ -503,7 +540,8 @@ static int get_graph(sb_trainer* t, const StepIn& in, int rows, int kind, int pa
   SB_CUDA(cudaGraphInstantiate(&ge, g, 0));
   cudaGraphDestroy(g);
   t->graphs[key] = ge;
-  if (kind == G_STEP && !in.sparse && (in.resident || !t->dsXb)) t->kernels_per_step[rows] = n.launches + 1;  // + set_batch_kernel
+  if (kind == G_STEP && !in.sparse && (in.resident || in.ordered || !t->dsXb))
+    t->kernels_per_step[rows * 2 + (in.ordered ? 1 : 0)] = n.launches + 1;  // + set_batch_kernel
   *out = ge;
   return SB_OK;
 }
@@ -525,11 +563,16 @@ static int run_step(sb_trainer* t, const float* X, const float* y, const float* 
   t->started = true;
   SB_CHECK(rows > 0 && rows <= n.max_batch, SB_ERR_INVALID, "rows=%d outside (0, max_batch=%d]", rows, n.max_batch);
   SB_CUDA(cudaSetDevice(n.device));
-  const bool resident = resident_row0 >= 0 && t->dsXb != nullptr;
+  // ordered: resident_row0 is a position in the row order, y / w are ordY / ordW (resident_step)
+  const bool ordered = resident_row0 >= 0 && t->ord_n > 0;
+  const bool resident = resident_row0 >= 0 && t->dsXb != nullptr && !ordered;
+  const int* order = ordered ? t->ord + resident_row0 : nullptr;
+  const int row0 = ordered ? 0 : static_cast<int>(resident_row0);
+  const int* nz_prefix = ordered ? nullptr : t->dsP;   // an ordered step's n_nz is counted by gather_batch_kernel
   // descriptor / scalar pair of this step: resident graph steps alternate, everything else uses pair 0
-  const bool prep = resident && t->prep != nullptr;
+  const bool prep = (resident || ordered) && t->prep != nullptr;
   const int pair = prep ? static_cast<int>(t->prep_steps & 1) : 0;
-  const StepIn in{t->descs[pair], t->scals[pair], resident, sparse};
+  const StepIn in{t->descs[pair], t->scals[pair], resident, sparse, ordered};
   t->last_pair = pair;
   cudaGraphExec_t ge = nullptr;
   SB_TRY(get_graph(t, in, rows, kind, pair, &ge));
@@ -545,8 +588,8 @@ static int run_step(sb_trainer* t, const float* X, const float* y, const float* 
     // main stream's current position.
     if (!t->have_pos) SB_CUDA(cudaEventRecord(t->ev_pos[pair ^ 1], n.stream));
     SB_CUDA(cudaStreamWaitEvent(t->prep, t->ev_pos[pair ^ 1], 0));
-    set_batch_kernel<<<1, 1, 0, t->prep>>>(in.desc, nullptr, y, w, lr_t, gscale, t->epoch, static_cast<int>(resident_row0), t->dsP, rows, in.scal,
-                                           kind == G_STEP ? t->hist_slot(t->global_step) : nullptr);
+    set_batch_kernel<<<1, 1, 0, t->prep>>>(in.desc, nullptr, y, w, lr_t, gscale, t->epoch, row0, nz_prefix, rows, in.scal,
+                                           kind == G_STEP ? t->hist_slot(t->global_step) : nullptr, order);
     SB_CUDA(cudaGetLastError());
     SB_CUDA(cudaEventRecord(t->ev_prep[pair], t->prep));
     SB_CUDA(cudaEventRecord(t->ev_pos[pair], n.stream));
@@ -555,9 +598,9 @@ static int run_step(sb_trainer* t, const float* X, const float* y, const float* 
     ++t->prep_steps;
   } else {
     t->have_pos = false;
-    if (resident)
-      set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, nullptr, y, w, lr_t, gscale, t->epoch, static_cast<int>(resident_row0), t->dsP, rows, in.scal,
-                                               kind == G_STEP ? t->hist_slot(t->global_step) : nullptr);
+    if (resident || ordered)
+      set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, nullptr, y, w, lr_t, gscale, t->epoch, row0, nz_prefix, rows, in.scal,
+                                               kind == G_STEP ? t->hist_slot(t->global_step) : nullptr, order);
     else
       set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, X, y, w ? w : n.ones, lr_t, gscale, t->epoch, 0, nullptr, 0, nullptr,
                                                kind == G_STEP ? t->hist_slot(t->global_step) : nullptr);
@@ -1173,16 +1216,17 @@ int sb_trainer_load_dataset(sb_trainer_t* t, const float* X, const float* y, con
 static int resident_step(sb_trainer_t* t, int64_t row_offset, int32_t rows, int kind) {
   SB_CHECK(t, SB_ERR_INVALID, "null trainer");
   SB_CHECK(t->ds_rows > 0, SB_ERR_STATE, "no resident dataset loaded");
-  SB_CHECK(row_offset >= 0 && rows > 0 && row_offset + rows <= t->ds_rows, SB_ERR_INVALID,
-           "rows [%lld, %lld) outside the resident set of %lld rows", (long long)row_offset, (long long)(row_offset + rows),
-           (long long)t->ds_rows);
+  SB_CHECK(row_offset >= 0 && rows > 0 && row_offset + rows <= t->resident_len(), SB_ERR_INVALID,
+           "rows [%lld, %lld) outside the resident set of %lld %s", (long long)row_offset, (long long)(row_offset + rows),
+           (long long)t->resident_len(), t->ord_n > 0 ? "rows of the row order" : "rows");
+  if (t->ord_n > 0) return run_step(t, nullptr, t->ordY, t->ordW, rows, kind, row_offset);
   return run_step(t, t->dsX ? t->dsX + row_offset * t->net.F : nullptr, t->dsY + row_offset, t->dsW + row_offset, rows, kind,
                   row_offset);
 }
 
-// RUN_S consecutive steps as ONE graph over descriptor set `set`
-static int get_run_graph(sb_trainer* t, int rows, int set, cudaGraphExec_t* out) {
-  const int key = rows * 2 + set;
+// RUN_S consecutive steps as ONE graph over descriptor set `set` (ordered: through the row order)
+static int get_run_graph(sb_trainer* t, int rows, int set, bool ordered, cudaGraphExec_t* out) {
+  const int key = (rows * 2 + set) * 2 + (ordered ? 1 : 0);
   auto it = t->run_graphs.find(key);
   if (it != t->run_graphs.end()) { *out = it->second; return SB_OK; }
   Net& n = t->net;
@@ -1190,7 +1234,7 @@ static int get_run_graph(sb_trainer* t, int rows, int set, cudaGraphExec_t* out)
   SB_CUDA(cudaStreamBeginCapture(n.stream, cudaStreamCaptureModeThreadLocal));
   int s = SB_OK;
   for (int k = 0; k < sb_trainer::RUN_S && s == SB_OK; ++k) {
-    const StepIn in{t->run_descs[set][k], t->run_scals[set][k], true, false};
+    const StepIn in{t->run_descs[set][k], t->run_scals[set][k], !ordered, false, ordered};
     // (SB_STEP_TRACE: an interior step is the one traced - it starts behind the previous step's tail, as most steps of a
     // run do)
     n.trace_on = (k == 1);
@@ -1214,14 +1258,16 @@ int sb_trainer_run_resident(sb_trainer_t* t, const int64_t* row_offsets, int32_t
   SB_CHECK(t->ds_rows > 0, SB_ERR_STATE, "no resident dataset loaded");
   Net& n = t->net;
   SB_CHECK(rows > 0 && rows <= n.max_batch, SB_ERR_INVALID, "rows=%d outside (0, max_batch=%d]", rows, n.max_batch);
+  const long long len = t->resident_len();
   for (int i = 0; i < n_steps; ++i)
-    SB_CHECK(row_offsets[i] >= 0 && row_offsets[i] + rows <= t->ds_rows, SB_ERR_INVALID,
-             "step %d: rows [%lld, %lld) outside the resident set of %lld rows", i, (long long)row_offsets[i],
-             (long long)(row_offsets[i] + rows), (long long)t->ds_rows);
+    SB_CHECK(row_offsets[i] >= 0 && row_offsets[i] + rows <= len, SB_ERR_INVALID,
+             "step %d: rows [%lld, %lld) outside the resident set of %lld %s", i, (long long)row_offsets[i],
+             (long long)(row_offsets[i] + rows), len, t->ord_n > 0 ? "rows of the row order" : "rows");
   constexpr int S = sb_trainer::RUN_S;
   int i = 0;
   SB_TRY(check_det_exchange(t));
-  if (t->dsXb != nullptr && t->prep != nullptr) {
+  const bool ordered = t->ord_n > 0;
+  if ((t->dsXb != nullptr || ordered) && t->prep != nullptr) {
     SB_CUDA(cudaSetDevice(n.device));
     if (!t->run_ready) {
       for (int set = 0; set < 2; ++set) {
@@ -1239,16 +1285,21 @@ int sb_trainer_run_resident(sb_trainer_t* t, const int64_t* row_offsets, int32_t
     for (; i + S <= n_steps; i += S) {
       const int set = static_cast<int>(t->run_chunks & 1);
       cudaGraphExec_t ge = nullptr;
-      SB_TRY(get_run_graph(t, rows, set, &ge));
+      SB_TRY(get_run_graph(t, rows, set, ordered, &ge));
       // this set was last read by the chunk two launches back
       if (t->run_used[set]) SB_CUDA(cudaStreamWaitEvent(t->prep, t->ev_run_done[set], 0));
       for (int k = 0; k < S; ++k) {
         const long long off = row_offsets[i + k];
         ++t->global_step;
         ++t->epoch;
-        set_batch_kernel<<<1, 1, 0, t->prep>>>(t->run_descs[set][k], nullptr, t->dsY + off, t->dsW + off,
-                                               lr_for_step(t, t->global_step), gscale, t->epoch, static_cast<int>(off), t->dsP,
-                                               rows, t->run_scals[set][k], t->hist_slot(t->global_step));
+        if (ordered)
+          set_batch_kernel<<<1, 1, 0, t->prep>>>(t->run_descs[set][k], nullptr, t->ordY, t->ordW, lr_for_step(t, t->global_step),
+                                                 gscale, t->epoch, 0, nullptr, rows, t->run_scals[set][k],
+                                                 t->hist_slot(t->global_step), t->ord + off);
+        else
+          set_batch_kernel<<<1, 1, 0, t->prep>>>(t->run_descs[set][k], nullptr, t->dsY + off, t->dsW + off,
+                                                 lr_for_step(t, t->global_step), gscale, t->epoch, static_cast<int>(off), t->dsP,
+                                                 rows, t->run_scals[set][k], t->hist_slot(t->global_step));
       }
       SB_CUDA(cudaGetLastError());
       SB_CUDA(cudaEventRecord(t->ev_run_prep[set], t->prep));
@@ -1280,21 +1331,26 @@ int sb_trainer_loss_resident(sb_trainer_t* t, int64_t row_offset, int32_t rows, 
   SB_CHECK(t && loss_out, SB_ERR_INVALID, "null argument");
   SB_CHECK(t->ds_rows > 0, SB_ERR_STATE, "no resident dataset loaded");
   Net& n = t->net;
-  SB_CHECK(row_offset >= 0 && rows > 0 && rows <= n.max_batch && row_offset + rows <= t->ds_rows, SB_ERR_INVALID,
-           "rows [%lld, %lld) outside the resident set of %lld rows", (long long)row_offset, (long long)(row_offset + rows),
-           (long long)t->ds_rows);
+  SB_CHECK(row_offset >= 0 && rows > 0 && rows <= n.max_batch && row_offset + rows <= t->resident_len(), SB_ERR_INVALID,
+           "rows [%lld, %lld) outside the resident set of %lld %s", (long long)row_offset, (long long)(row_offset + rows),
+           (long long)t->resident_len(), t->ord_n > 0 ? "rows of the row order" : "rows");
   SB_CUDA(cudaSetDevice(n.device));
   t->have_pos = false;
-  const bool resident = t->dsXb != nullptr;
-  const StepIn in{t->descs[0], t->scals[0], resident, false};      // (see forward_chunks)
-  if (resident)
+  const bool ordered = t->ord_n > 0;
+  const bool resident = t->dsXb != nullptr && !ordered;
+  const StepIn in{t->descs[0], t->scals[0], resident, false, ordered};      // (see forward_chunks)
+  if (ordered)
+    set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, nullptr, t->ordY, t->ordW, 0.f, 1.f, t->epoch, 0, nullptr, rows, in.scal,
+                                             nullptr, t->ord + row_offset);
+  else if (resident)
     set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, nullptr, t->dsY + row_offset, t->dsW + row_offset, 0.f, 1.f, t->epoch,
                                              static_cast<int>(row_offset), t->dsP, rows, in.scal);
   else
     set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, t->dsX + row_offset * n.F, t->dsY + row_offset, t->dsW + row_offset, 0.f, 1.f,
                                              t->epoch);
   SB_CUDA(cudaGetLastError());
-  if (!resident) SB_TRY(n.enqueue_load(in, rows));
+  if (ordered) SB_TRY(enqueue_gather(t, in, rows, nullptr, 0));
+  else if (!resident) SB_TRY(n.enqueue_load(in, rows));
   SB_TRY(n.enqueue_hidden_forward(in, rows));
   SB_TRY(n.enqueue_out(in, rows, true, false, nullptr, nullptr));
   float h[SCAL_COUNT];
@@ -1359,9 +1415,41 @@ void* sb_trainer_stream(sb_trainer_t* t) { return t ? reinterpret_cast<void*>(t-
 int sb_trainer_kernels_per_step(sb_trainer_t* t, int32_t rows) {
   SB_CHECK(t, SB_ERR_INVALID, "null trainer");
   cudaGraphExec_t ge;
-  const StepIn in{t->descs[0], t->scals[0], t->dsXb != nullptr, false};
+  const bool ordered = t->ord_n > 0;   // the path resident steps take now
+  const StepIn in{t->descs[0], t->scals[0], t->dsXb != nullptr && !ordered, false, ordered};
   SB_TRY(get_graph(t, in, rows, G_STEP, 0, &ge));
-  return t->kernels_per_step[rows];
+  return t->kernels_per_step[rows * 2 + (ordered ? 1 : 0)];
+}
+
+int sb_trainer_set_row_order(sb_trainer_t* t, const int64_t* rows, int64_t n) {
+  SB_CHECK(t, SB_ERR_INVALID, "null trainer");
+  SB_CHECK((rows == nullptr && n == 0) || (rows != nullptr && n >= 1 && n < (1ll << 31)), SB_ERR_INVALID,
+           "row order of %lld rows (%s list): give 1 <= n < 2^31 rows, or NULL and 0 for the physical order", (long long)n,
+           rows ? "non-null" : "null");
+  SB_CHECK(t->ds_rows > 0, SB_ERR_STATE, "no resident dataset loaded");
+  std::vector<int> h(static_cast<size_t>(n));
+  for (int64_t i = 0; i < n; ++i) {
+    SB_CHECK(rows[i] >= 0 && rows[i] < t->ds_rows, SB_ERR_INVALID, "row order entry %lld = %lld outside the resident set of %lld rows",
+             (long long)i, (long long)rows[i], (long long)t->ds_rows);
+    h[static_cast<size_t>(i)] = static_cast<int>(rows[i]);
+  }
+  Net& net = t->net;
+  SB_CUDA(cudaSetDevice(net.device));
+  // steps already queued read the current order (and ordY / ordW) when they run; the graphs read the order through the
+  // descriptor, so neither a new buffer nor new contents need a new capture
+  SB_CUDA(cudaStreamSynchronize(net.stream));
+  if (n == 0) { t->drop_row_order(); return SB_OK; }
+  if (!t->ordY) SB_TRY(net.dalloc(&t->ordY, net.max_batch));
+  if (!t->ordW) SB_TRY(net.dalloc(&t->ordW, net.max_batch));
+  if (n > t->ord_cap) {
+    t->drop_row_order();
+    SB_CUDA(cudaMalloc(&t->ord, sizeof(int) * n));
+    t->ord_cap = n;
+  }
+  SB_CUDA(cudaMemcpyAsync(t->ord, h.data(), sizeof(int) * n, cudaMemcpyHostToDevice, net.stream));
+  SB_CUDA(cudaStreamSynchronize(net.stream));
+  t->ord_n = n;
+  return SB_OK;
 }
 
 // forward (+ optional loss) over any number of host rows, in max_batch chunks

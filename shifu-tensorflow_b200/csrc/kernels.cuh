@@ -18,6 +18,7 @@ struct BatchDesc {
   unsigned int epoch;  // exchange round (flag value of the peer-memory all-reduce)
   int row0;            // first row of the batch inside the bf16 HBM-resident set (TMA row-coordinate offset)
   float2* hist;        // nullable: slot of this step in the pinned-host loss history (loss sum, n_nz), written by the step's tail
+  const int* order;    // ordered resident steps (gather_batch_kernel): the batch's slice of the row order, row r = order[r]
 };
 
 // nz_prefix != nullptr (bf16 resident set): the batch is consumed by TMA straight from the resident set, there is no
@@ -25,8 +26,9 @@ struct BatchDesc {
 // and clears the loss accumulator.
 static __global__ void set_batch_kernel(BatchDesc* d, const float* X, const float* y, const float* w, float lr_t, float gscale,
                                         unsigned int epoch = 0, int row0 = 0, const int* nz_prefix = nullptr, int rows = 0,
-                                        float* scal = nullptr, float2* hist = nullptr) {
+                                        float* scal = nullptr, float2* hist = nullptr, const int* order = nullptr) {
   d->X = X; d->y = y; d->w = w; d->lr_t = lr_t; d->gscale = gscale; d->epoch = epoch; d->row0 = row0; d->hist = hist;
+  d->order = order;
   if (nz_prefix != nullptr) {
     scal[1] = static_cast<float>(nz_prefix[row0 + rows] - nz_prefix[row0]);  // SCAL_NNZ
     scal[0] = 0.f;                                                           // SCAL_LOSS_SUM
@@ -145,6 +147,79 @@ __device__ __forceinline__ void trace_begin(unsigned long long* trace, bool entr
 }
 __device__ __forceinline__ void trace_end(unsigned long long* trace) {
   if (trace != nullptr && threadIdx.x == 0) atomicMax(trace + 10, static_cast<unsigned long long>(globaltimer_ns()));
+}
+
+// ------------------------------------------------------------------------------------------------
+// Ordered resident steps (sb_trainer_set_row_order): the first kernel of the step, in load_batch_kernel's place and with
+// its duties (clear the gradient buffer, publish n_nz and the cleared loss sum).  Row r of the batch is row
+// desc->order[r] of the resident set.  Tensor-core modes copy that row's np bf16 parts, pad columns included, into Xb as
+// they are, so Xb holds what load_batch_kernel writes for the same rows; fp32 mode copies the fp32 row into Xf.  y and w
+// are gathered into the batch buffers the descriptor points the loss at.  HBM-bound: 16-byte vectors; block 0 counts the
+// non-zero weights in load_batch_kernel's order.
+// ------------------------------------------------------------------------------------------------
+struct GatherParams {
+  const BatchDesc* desc;
+  int rows, F, ldF, np;
+  const __nv_bfloat16* src_b; long long src_ps;   // tensor-core modes: the resident set [n, ldF], np parts src_ps apart
+  __nv_bfloat16* Xb; long long Xb_ps;             // -> [rows, ldF] parts
+  const float* src_f; float* Xf;                  // fp32 mode: the resident set [n, F] -> [rows, F]
+  const float* src_y; const float* src_w;         // labels / weights of the resident set [n]
+  float* y; float* w;                             // -> [rows]
+  float* scal;
+  float* zero_buf; long long zero_n;
+  unsigned long long* trace;
+};
+
+template <bool BF16>
+__global__ void __launch_bounds__(256)
+gather_batch_kernel(const GatherParams p) {
+  trace_begin(p.trace, true);
+  pdl_wait();
+  pdl_launch_dependents();
+  trace_begin(p.trace, false);
+  const long long stride = gridDim.x * 256ll, tid0 = blockIdx.x * 256ll + threadIdx.x;
+  for (long long i = tid0; i < p.zero_n; i += stride) p.zero_buf[i] = 0.f;
+  const int* __restrict__ order = p.desc->order;
+  if constexpr (BF16) {
+    const int groups = p.ldF >> 3;   // 8-element vectors per row (ldF is a multiple of 8)
+    const long long total = static_cast<long long>(p.rows) * groups;
+    for (long long u = tid0; u < total; u += stride) {
+      const int r = static_cast<int>(u / groups), c = static_cast<int>(u % groups) * 8;
+      const size_t s = static_cast<size_t>(__ldg(order + r)) * p.ldF + c, d = static_cast<size_t>(r) * p.ldF + c;
+      for (int part = 0; part < p.np; ++part)
+        *reinterpret_cast<uint4*>(p.Xb + part * p.Xb_ps + d) = __ldg(reinterpret_cast<const uint4*>(p.src_b + part * p.src_ps + s));
+    }
+  } else {
+    const bool vec = ((p.F & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.src_f) & 15) == 0);
+    const int groups = vec ? (p.F >> 2) : p.F;   // 4-float vectors (or single floats) per row
+    const long long total = static_cast<long long>(p.rows) * groups;
+    for (long long u = tid0; u < total; u += stride) {
+      const int r = static_cast<int>(u / groups), c = static_cast<int>(u % groups);
+      const size_t s = static_cast<size_t>(__ldg(order + r)) * p.F, d = static_cast<size_t>(r) * p.F;
+      if (vec) reinterpret_cast<float4*>(p.Xf + d)[c] = __ldg(reinterpret_cast<const float4*>(p.src_f + s) + c);
+      else p.Xf[d + c] = __ldg(p.src_f + s + c);
+    }
+  }
+  for (long long r = tid0; r < p.rows; r += stride) {
+    const int s = __ldg(order + r);
+    p.y[r] = __ldg(p.src_y + s);
+    p.w[r] = __ldg(p.src_w + s);
+  }
+  if (blockIdx.x == 0) {
+    float cnt = 0.f;
+    for (int i = threadIdx.x; i < p.rows; i += 256) cnt += (__ldg(p.src_w + __ldg(order + i)) != 0.f) ? 1.f : 0.f;
+    cnt = warp_sum(cnt);
+    __shared__ float part[8];
+    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = cnt;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float t = 0.f;
+      for (int i = 0; i < 8; ++i) t += part[i];
+      p.scal[SCAL_NNZ] = t;
+      p.scal[SCAL_LOSS_SUM] = 0.f;
+    }
+  }
+  trace_end(p.trace);
 }
 
 template <typename T> __device__ __forceinline__ float ld_as_float(const T* p);

@@ -284,6 +284,7 @@ int Net::init(const sb_net_desc* d, int device_, bool training_) {
     // has to re-partition L1 / shared memory
     const int co = cudaSharedmemCarveoutMaxShared;
     cudaFuncSetAttribute(load_batch_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, co);
+    cudaFuncSetAttribute(gather_batch_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, co);
     cudaFuncSetAttribute(out_layer_kernel<__nv_bfloat16>, cudaFuncAttributePreferredSharedMemoryCarveout, co);
     cudaFuncSetAttribute(out_layer_kernel<__nv_bfloat16, true>, cudaFuncAttributePreferredSharedMemoryCarveout, co);
   }

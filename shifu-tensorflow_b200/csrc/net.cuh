@@ -26,6 +26,7 @@ struct StepIn {
   float* scal = nullptr;
   bool resident = false;   // layer 0's GEMMs read their A operand by TMA from resident_Xb at row offset desc->row0
   bool sparse = false;     // wide+deep step: dense block + index matrix, hidden layer 0's one-hot block via the embedding
+  bool ordered = false;    // resident step through the row order: gather_batch_kernel fills Xb / Xf, layer 0 reads them
 };
 
 inline int pairs_of(int np) { return np == 3 ? 6 : (np == 2 ? 3 : 1); }

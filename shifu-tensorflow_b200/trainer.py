@@ -32,6 +32,10 @@ Optional ModelConfig train.params the reference does not have (defaults = refere
              (sb_trainer_set_deterministic), so a run with the same data, SB_SEED, configuration, build, GPU model and
              worker count reproduces its model bit for bit.  Every Precision; not with wide+deep columns; several
              workers need the peer-memory exchange (all ranks on one host)
+  Shuffle    true | false (default): before every pass over its training rows, each worker draws a new permutation of
+             them (keyed by SB_SEED, or a logged random seed, the worker index and global_step) and trains on
+             mini-batches cut from that order (sb_trainer_set_row_order; wide+deep: the host arrays are permuted).  The
+             validation set keeps its order
 
 File paths (TRAINING_DATA_PATH, TMP_MODEL_PATH, FINAL_MODEL_PATH) may carry a scheme.  The stock AM hands out fully
 qualified HDFS URIs (TrainingDataSet.java:74) which the reference reads through tf.gfile; here `hdfs://`, `viewfs://`,
@@ -97,14 +101,30 @@ def generate_from_modelconf(model_conf: dict):
     return num_hidden_nodes[:num_hidden_layer], activation_func[:num_hidden_layer]
 
 
-def deterministic_requested(params: dict) -> bool:
-    """train.params.Deterministic: a JSON bool, or the strings true / false"""
-    v = params.get('Deterministic', False)
+def _bool_param(params: dict, key: str) -> bool:
+    """train.params.<key>: a JSON bool, or the strings true / false; absent = false"""
+    v = params.get(key, False)
     if isinstance(v, str):
         if v.strip().lower() not in ('true', 'false'):
-            raise ValueError("train.params.Deterministic must be true or false, got %r" % v)
+            raise ValueError("train.params.%s must be true or false, got %r" % (key, v))
         return v.strip().lower() == 'true'
     return bool(v)
+
+
+def deterministic_requested(params: dict) -> bool:
+    """train.params.Deterministic: a JSON bool, or the strings true / false"""
+    return _bool_param(params, 'Deterministic')
+
+
+def shuffle_requested(params: dict) -> bool:
+    """train.params.Shuffle: a JSON bool, or the strings true / false"""
+    return _bool_param(params, 'Shuffle')
+
+
+def pass_order(seed: int, task_index: int, global_step: int, n_rows: int) -> np.ndarray:
+    """Shuffle: the order of this rank's training rows for the pass that starts at `global_step`.  Keyed by the step, so a
+    run resumed from a checkpoint draws the orders an uninterrupted run draws."""
+    return np.random.default_rng((seed, task_index, global_step)).permutation(n_rows)
 
 
 def model(feature_count: int, model_conf: Optional[dict], max_batch: int) -> capi.NetDesc:
@@ -562,6 +582,7 @@ def main(_=None, env=None, rng=random) -> int:
         raise ValueError("train.params.Schedule must be sync_replicas (alias epoch) or batch, got %r" % schedule)
     per_batch_update = schedule == 'batch'
     deterministic = deterministic_requested(params)
+    shuffle = shuffle_requested(params)
     if deterministic and wide_deep:
         raise ValueError("train.params.Deterministic with wide+deep columns: the embedding gradient is scatter-added in no "
                          "fixed order; train the dense model (SELECTED_COLUMN_NUMS) or drop Deterministic")
@@ -682,14 +703,27 @@ def main(_=None, env=None, rng=random) -> int:
     sched.local_step = [sched.global_step] * n_workers
     sched.tokens = [sched.global_step] * sched.R
 
+    shuffle_seed = 0
+    if shuffle:
+        shuffle_seed = int(env.get("SB_SEED", "0")) or random.SystemRandom().randrange(1, 2 ** 63)
+        logging.info("Shuffle: a new order of the training rows every pass, seed %d" % shuffle_seed)
+    sparse_rows = (train_x, train_idx, train_y, train_w) if wide_deep else None
+
     logging.info('Starting training on worker %d' % task_index)
     while trainer.global_step < epochs:           # StopAtStepHook(num_steps=EPOCH) (ssgd_monitor.py:235)
         start = time.time()
         l = 0.0
+        if shuffle:
+            perm = pass_order(shuffle_seed, task_index, trainer.global_step, len(train_x))
+            if wide_deep:
+                sparse_rows = (train_x[perm], train_idx[perm], train_y[perm], train_w[perm])
+            else:
+                trainer.set_row_order(perm)
         if wide_deep:
+            sx, si, sy, sw = sparse_rows
             for i in range(total_batch):
                 a, b = int(bounds[i]), int(bounds[i + 1])
-                l = trainer.step_sparse(train_x[a:b], train_idx[a:b], train_y[a:b], train_w[a:b])
+                l = trainer.step_sparse(sx[a:b], si[a:b], sy[a:b], sw[a:b])
                 if trainer.global_step >= epochs:
                     break
         elif per_batch_update:
