@@ -49,8 +49,18 @@ typedef enum { SB_ACT_SIGMOID = 0, SB_ACT_TANH = 1, SB_ACT_RELU = 2, SB_ACT_LEAK
 /* SB_LOSS_MSE = tf.losses.mean_squared_error on the sigmoid output, SUM_BY_NONZERO_WEIGHTS
  * (ssgd_monitor.py:129) - the reference's loss.  SB_LOSS_SIGMOID_CE = BASELINE.json's wording. */
 typedef enum { SB_LOSS_MSE = 0, SB_LOSS_SIGMOID_CE = 1 } sb_loss;
-/* ADADELTA: ssgd_monitor.py:138; ADAM: ssgd.py:57; SGD: ssgd_monitor_bk.py:81; MOMENTUM: north star */
-typedef enum { SB_OPT_ADADELTA = 0, SB_OPT_ADAM = 1, SB_OPT_SGD = 2, SB_OPT_MOMENTUM = 3 } sb_optimizer;
+/* ADADELTA: ssgd_monitor.py:138; ADAM: ssgd.py:57; SGD: ssgd_monitor_bk.py:81; MOMENTUM: north star.
+ * ADAGRAD, RMSPROP, FTRL: the other TF 1.x optimizers in their training_ops.cc kernel forms (ApplyAdagrad; ApplyRMSProp,
+ * not centered; ApplyFtrl with lr_power = -0.5 and no l2 shrinkage).  Every update is element-wise in fp32 with correctly
+ * rounded square roots and divisions.  Optimizer state (s1 / s2) per parameter and its start value, written when the
+ * trainer is created (sb_trainer_set_params and sb_trainer_init_xavier leave the state as it is, for every optimizer):
+ *   ADADELTA  accum = 0, accum_update = 0     ADAM     m = 0, v = 0         SGD   -
+ *   MOMENTUM  accum = 0                       ADAGRAD  accum = initial_accumulator
+ *   RMSPROP   ms = 1 (TF's ones initializer), mom = 0                     FTRL  accum = initial_accumulator, linear = 0
+ * FTRL sets a parameter to exactly 0 while |linear| <= l1 (also with l1 = 0 and linear = 0, e.g. a zero gradient from
+ * the start), as TF does. */
+typedef enum { SB_OPT_ADADELTA = 0, SB_OPT_ADAM = 1, SB_OPT_SGD = 2, SB_OPT_MOMENTUM = 3, SB_OPT_ADAGRAD = 4,
+               SB_OPT_RMSPROP = 5, SB_OPT_FTRL = 6 } sb_optimizer;
 /* SB_PREC_FP32: fp32 operands and fp32 accumulation end to end (what TF-CPU computes) - parity mode (CUDA cores).
  * SB_PREC_BF16: bf16 operands on the tensor cores (wgmma), fp32 accumulation, fp32 master
  *               weights and optimizer state - performance mode.
@@ -69,13 +79,19 @@ typedef struct {
   int32_t loss;                    /* sb_loss                                                          */
   int32_t optimizer;               /* sb_optimizer                                                     */
   float learning_rate;             /* train.params.LearningRate, ssgd_monitor.py:133                   */
-  float rho;                       /* Adadelta rho (TF default 0.95)                                   */
-  float epsilon;                   /* Adadelta / Adam epsilon (TF default 1e-8)                        */
+  float rho;                       /* Adadelta rho (TF default 0.95); RMSProp decay (TF default 0.9)   */
+  float epsilon;                   /* Adadelta / Adam epsilon (TF default 1e-8); RMSProp (1e-10)       */
   float beta1, beta2;              /* Adam (TF defaults 0.9 / 0.999)                                   */
-  float momentum;                  /* Momentum                                                         */
+  float momentum;                  /* Momentum; RMSProp momentum (TF default 0.0)                      */
   int32_t max_batch;               /* largest mini-batch (rows) a step will be given                   */
   int32_t precision;               /* sb_precision                                                     */
 } sb_net_desc;
+/* Optimizer fields each optimizer reads (the others are ignored, whatever they hold):
+ *   ADADELTA rho, epsilon    ADAM beta1, beta2, epsilon    SGD -    MOMENTUM momentum
+ *   RMSPROP  rho (decay, in [0, 1]), momentum (>= 0), epsilon (>= 0); a value out of range is SB_ERR_INVALID, found
+ *            before any device work
+ *   ADAGRAD  initial_accumulator, FTRL initial_accumulator, l1, l2: sb_trainer_set_optimizer_params (TF's defaults
+ *            0.1, 0, 0 until it is called).  The descriptor's layout is unchanged, so callers built against it keep working. */
 
 typedef struct sb_trainer sb_trainer_t;
 typedef struct sb_model sb_model_t;
@@ -131,6 +147,11 @@ int sb_trainer_get_grads(sb_trainer_t* t, float* flat, int64_t n);
  * deterministic trainer with world > 1 needs a peer table (sb_trainer_set_peer_handles / _pointers): without one its
  * first step returns SB_ERR_STATE (NCCL's all-reduce fixes no summation order). */
 int sb_trainer_set_deterministic(sb_trainer_t* t, int32_t on);
+/* Adagrad / FTRL hyperparameters the descriptor has no field for: accum's start value initial_accumulator (> 0; TF default
+ * 0.1) and FTRL's l1 / l2 regularization strengths (>= 0; TF defaults 0).  Writes initial_accumulator into the state at
+ * once (a device fill).  Call it right after sb_trainer_create: SB_ERR_STATE after the first step or graph capture,
+ * SB_ERR_INVALID for an optimizer that reads none of them or a value out of range (both before any device work). */
+int sb_trainer_set_optimizer_params(sb_trainer_t* t, float initial_accumulator, float l1, float l2);
 
 /* one sess.run([train_step, loss, global_step], feed_dict) (ssgd_monitor.py:272-276) in the
  * "clean" schedule: forward, loss, backward, gradient mean over ranks, one optimizer update.

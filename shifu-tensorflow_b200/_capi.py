@@ -23,7 +23,12 @@ SB_MAX_HIDDEN = 32
 SB_NCCL_ID_BYTES = 128
 ACT_SIGMOID, ACT_TANH, ACT_RELU, ACT_LEAKYRELU, ACT_NONE = 0, 1, 2, 3, -1
 LOSS_MSE, LOSS_SIGMOID_CE = 0, 1
-OPT_ADADELTA, OPT_ADAM, OPT_SGD, OPT_MOMENTUM = 0, 1, 2, 3
+OPT_ADADELTA, OPT_ADAM, OPT_SGD, OPT_MOMENTUM, OPT_ADAGRAD, OPT_RMSPROP, OPT_FTRL = 0, 1, 2, 3, 4, 5, 6
+# TF 1.x defaults of the hyperparameters make_desc fills in when the caller passes none: RMSPropOptimizer's (decay,
+# epsilon, momentum) differ from the values every other optimizer gets
+_RMSPROP_DEFAULTS = dict(rho=0.9, epsilon=1e-10, momentum=0.0)
+_OTHER_DEFAULTS = dict(rho=0.95, epsilon=1e-8, momentum=0.9)
+INITIAL_ACCUMULATOR, L1, L2 = 0.1, 0.0, 0.0     # Adagrad / FTRL (Trainer(initial_accumulator=, l1=, l2=))
 PREC_FP32, PREC_BF16, PREC_FP32_TC, PREC_BF16X2 = 0, 1, 2, 3
 SB_OK, SB_ERR_INVALID, SB_ERR_CUDA, SB_ERR_NCCL, SB_ERR_IO, SB_ERR_STATE, SB_ERR_FORMAT = 0, -1, -2, -3, -4, -5, -6
 
@@ -40,9 +45,15 @@ class NetDesc(C.Structure):
 
 
 def make_desc(n_features: int, hidden: Sequence[int], acts: Sequence[int], loss: int = LOSS_MSE,
-              optimizer: int = OPT_ADADELTA, learning_rate: float = 0.001, rho: float = 0.95, epsilon: float = 1e-8,
-              beta1: float = 0.9, beta2: float = 0.999, momentum: float = 0.9, max_batch: int = 128,
-              precision: int = PREC_FP32) -> NetDesc:
+              optimizer: int = OPT_ADADELTA, learning_rate: float = 0.001, rho: Optional[float] = None,
+              epsilon: Optional[float] = None, beta1: float = 0.9, beta2: float = 0.999, momentum: Optional[float] = None,
+              max_batch: int = 128, precision: int = PREC_FP32) -> NetDesc:
+    """rho / epsilon / momentum left at None take the TF 1.x default of `optimizer`: RMSProp decay 0.9, epsilon 1e-10,
+    momentum 0.0; every other optimizer rho 0.95, epsilon 1e-8, momentum 0.9."""
+    dflt = _RMSPROP_DEFAULTS if optimizer == OPT_RMSPROP else _OTHER_DEFAULTS
+    rho = dflt["rho"] if rho is None else rho
+    epsilon = dflt["epsilon"] if epsilon is None else epsilon
+    momentum = dflt["momentum"] if momentum is None else momentum
     if len(hidden) != len(acts):
         raise ValueError("hidden and acts must have the same length")
     if len(hidden) > SB_MAX_HIDDEN:
@@ -98,6 +109,7 @@ PROTOTYPES = {
     "sb_trainer_step": (C.c_int, [_vp, _f32p, _f32p, _f32p, C.c_int32, _f32p]),
     "sb_trainer_set_sparse": (C.c_int, [_vp, C.c_int32, C.c_int32, C.c_int32]),
     "sb_trainer_set_deterministic": (C.c_int, [_vp, C.c_int32]),
+    "sb_trainer_set_optimizer_params": (C.c_int, [_vp, C.c_float, C.c_float, C.c_float]),
     "sb_trainer_step_sparse": (C.c_int, [_vp, _f32p, _P(C.c_int32), _f32p, _f32p, C.c_int32, _f32p]),
     "sb_trainer_predict_sparse": (C.c_int, [_vp, _f32p, _P(C.c_int32), C.c_int64, _f32p]),
     "sb_trainer_eval_loss_sparse": (C.c_int, [_vp, _f32p, _P(C.c_int32), _f32p, _f32p, C.c_int64, _f32p]),
@@ -261,7 +273,9 @@ class Trainer:
     """Owns one sb_trainer_t.  X is [rows, n_features] float32, y / w are [rows] (or [rows,1])."""
 
     def __init__(self, desc: NetDesc, device: int = 0, nccl_id: Optional[bytes] = None, rank: int = 0, world: int = 1,
-                 deterministic: bool = False):
+                 deterministic: bool = False, initial_accumulator: Optional[float] = None, l1: Optional[float] = None,
+                 l2: Optional[float] = None):
+        """initial_accumulator / l1 / l2 (Adagrad, FTRL; None = TF's default): see set_optimizer_params"""
         self._h = C.c_void_p()
         self.desc = desc
         idbuf = None
@@ -275,10 +289,18 @@ class Trainer:
         self.n_features = int(desc.n_features)
         if deterministic:
             self.set_deterministic(True)
+        if (initial_accumulator, l1, l2) != (None, None, None):
+            self.set_optimizer_params(INITIAL_ACCUMULATOR if initial_accumulator is None else initial_accumulator,
+                                      L1 if l1 is None else l1, L2 if l2 is None else l2)
 
     def set_deterministic(self, on: bool = True):
         """fixed-order reductions in every training kernel (sb_trainer_set_deterministic); before the first step"""
         check(lib().sb_trainer_set_deterministic(self._h, 1 if on else 0))
+
+    def set_optimizer_params(self, initial_accumulator: float = INITIAL_ACCUMULATOR, l1: float = L1, l2: float = L2):
+        """Adagrad / FTRL: accum's start value (> 0) and FTRL's l1 / l2 strengths (>= 0) (sb_trainer_set_optimizer_params);
+        before the first step"""
+        check(lib().sb_trainer_set_optimizer_params(self._h, float(initial_accumulator), float(l1), float(l2)))
 
     def close(self):
         if getattr(self, "_h", None) is not None and self._h:

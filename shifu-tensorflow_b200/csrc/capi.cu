@@ -28,6 +28,7 @@ struct sb_trainer {
   sb_net_desc desc;
   OptHyper hyper;
   float lr = 0.f;
+  float initial_accumulator = 0.1f;   // Adagrad / FTRL: start value of s1 (sb_trainer_set_optimizer_params)
   int rank = 0, world = 1;
   NcclComm comm = nullptr;
   float *grad = nullptr, *s1 = nullptr, *s2 = nullptr, *acc = nullptr;
@@ -196,7 +197,7 @@ static int enqueue_optimizer(sb_trainer* t, const StepIn& in, const float* g, in
   if (!st) st = n.stream;
   if (w1 <= w0) return SB_OK;
   // pdl = false: plain dependency (runs after a stream join / on the comm stream)
-  SB_TRY(launch_kernel(optimizer_kernel, dim3(static_cast<unsigned>(w1 - w0)), dim3(256), 0, st, pdl, n.work + w0, in.desc, t->hyper,
+  SB_TRY(launch_kernel(opt_ext(t->hyper.kind) ? optimizer_kernel<true> : optimizer_kernel<false>, dim3(static_cast<unsigned>(w1 - w0)), dim3(256), 0, st, pdl, n.work + w0, in.desc, t->hyper,
                        n.theta, g, n.s1, n.s2, in.scal, publish_scalars ? t->d_hscal : static_cast<float*>(nullptr),
                        n.next_trace(st == n.stream ? "opt" : "opt_side")));
   n.mark("optimizer");
@@ -249,6 +250,25 @@ static int xchg_grid(const sb_trainer* t, int slot_mask, bool alone) {
   return grid;
 }
 
+// the exchange kernel of the world size and optimizer group (opt_ext); *kernel names it (the same name for both groups)
+template <bool EXT>
+static int launch_xchg(sb_trainer* t, const XchgParams& p, dim3 g, dim3 b, cudaStream_t st, bool pdl, const char** kernel) {
+  // plain bf16: the LL protocol (flags inside the data) needs fewer fabric round trips than the flag-and-pull kernel
+  if (t->ll_ready) {
+    LLParams lp;
+    lp.x = p; lp.llg_off = t->llg_off; lp.lls_off = t->lls_off; lp.n4 = t->xch_n4;
+    if (t->world <= 2) { SB_TRY(launch_kernel(xchg_ll_kernel<2, EXT>, g, b, 0, st, pdl, lp)); *kernel = "xchg_ll<2>"; }
+    else if (t->world <= 4) { SB_TRY(launch_kernel(xchg_ll_kernel<4, EXT>, g, b, 0, st, pdl, lp)); *kernel = "xchg_ll<4>"; }
+    else if (t->world <= 8) { SB_TRY(launch_kernel(xchg_ll_kernel<8, EXT>, g, b, 0, st, pdl, lp)); *kernel = "xchg_ll<8>"; }
+    else { SB_TRY(launch_kernel(xchg_ll_kernel<16, EXT>, g, b, 0, st, pdl, lp)); *kernel = "xchg_ll<16>"; }
+  } else
+  if (t->world <= 2) { SB_TRY(launch_kernel(xchg_update_kernel<2, EXT>, g, b, 0, st, pdl, p)); *kernel = "xchg_update<2>"; }
+  else if (t->world <= 4) { SB_TRY(launch_kernel(xchg_update_kernel<4, EXT>, g, b, 0, st, pdl, p)); *kernel = "xchg_update<4>"; }
+  else if (t->world <= 8) { SB_TRY(launch_kernel(xchg_update_kernel<8, EXT>, g, b, 0, st, pdl, p)); *kernel = "xchg_update<8>"; }
+  else { SB_TRY(launch_kernel(xchg_update_kernel<16, EXT>, g, b, 0, st, pdl, p)); *kernel = "xchg_update<16>"; }
+  return SB_OK;
+}
+
 // reduce-scatter -> owner update -> all-gather of the operands for the given segments (xchg_p2p.cuh); `g` must be t->grad.
 // grid > 0 replaces the grid rule (sb_debug_exchange).
 static int enqueue_xchg(sb_trainer* t, const StepIn& in, int slot_mask, cudaStream_t st, bool publish_scalars, bool pdl,
@@ -265,20 +285,9 @@ static int enqueue_xchg(sb_trainer* t, const StepIn& in, int slot_mask, cudaStre
   p.trace = n.next_trace(nm);
   if (grid <= 0) grid = xchg_grid(t, slot_mask, alone);
   const dim3 g(static_cast<unsigned>(grid)), b(256);
-  // plain bf16: the LL protocol (flags inside the data) needs fewer fabric round trips than the flag-and-pull kernel
   const char* kernel;
-  if (t->ll_ready) {
-    LLParams lp;
-    lp.x = p; lp.llg_off = t->llg_off; lp.lls_off = t->lls_off; lp.n4 = t->xch_n4;
-    if (t->world <= 2) { SB_TRY(launch_kernel(xchg_ll_kernel<2>, g, b, 0, st, pdl, lp)); kernel = "xchg_ll<2>"; }
-    else if (t->world <= 4) { SB_TRY(launch_kernel(xchg_ll_kernel<4>, g, b, 0, st, pdl, lp)); kernel = "xchg_ll<4>"; }
-    else if (t->world <= 8) { SB_TRY(launch_kernel(xchg_ll_kernel<8>, g, b, 0, st, pdl, lp)); kernel = "xchg_ll<8>"; }
-    else { SB_TRY(launch_kernel(xchg_ll_kernel<16>, g, b, 0, st, pdl, lp)); kernel = "xchg_ll<16>"; }
-  } else
-  if (t->world <= 2) { SB_TRY(launch_kernel(xchg_update_kernel<2>, g, b, 0, st, pdl, p)); kernel = "xchg_update<2>"; }
-  else if (t->world <= 4) { SB_TRY(launch_kernel(xchg_update_kernel<4>, g, b, 0, st, pdl, p)); kernel = "xchg_update<4>"; }
-  else if (t->world <= 8) { SB_TRY(launch_kernel(xchg_update_kernel<8>, g, b, 0, st, pdl, p)); kernel = "xchg_update<8>"; }
-  else { SB_TRY(launch_kernel(xchg_update_kernel<16>, g, b, 0, st, pdl, p)); kernel = "xchg_update<16>"; }
+  if (opt_ext(t->hyper.kind)) SB_TRY(launch_xchg<true>(t, p, g, b, st, pdl, &kernel));
+  else SB_TRY(launch_xchg<false>(t, p, g, b, st, pdl, &kernel));
   n.mark(kernel);
   t->master_stale = true;
   t->grad_sharded = true;
@@ -703,6 +712,19 @@ int sb_nccl_unique_id(void* out128) {
   return SB_OK;
 }
 
+// Optimizer state that does not start at 0 (the arena's value): Adagrad's and FTRL's accum start at initial_accumulator,
+// RMSProp's ms at 1 (TF's RMSPropOptimizer creates its `rms` slot with a ones initializer).  Every rank fills its whole
+// state, so the runs a rank owns in the peer exchange start there as well.
+static int fill_initial_state(sb_trainer* t) {
+  Net& n = t->net;
+  const int k = t->hyper.kind;
+  if (k != SB_OPT_ADAGRAD && k != SB_OPT_FTRL && k != SB_OPT_RMSPROP) return SB_OK;
+  const float v = k == SB_OPT_RMSPROP ? 1.f : t->initial_accumulator;
+  fill_kernel<<<static_cast<unsigned>((n.n_params + 255) / 256), 256, 0, n.stream>>>(n.s1, v, n.n_params);
+  SB_CUDA(cudaGetLastError());
+  return SB_OK;
+}
+
 int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, int rank, int world, sb_trainer_t** out) {
   SB_CHECK(out, SB_ERR_INVALID, "out is null");
   *out = nullptr;
@@ -716,6 +738,7 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
   t->hyper.kind = desc->optimizer;
   t->hyper.rho = desc->rho; t->hyper.eps = desc->epsilon;
   t->hyper.beta1 = desc->beta1; t->hyper.beta2 = desc->beta2; t->hyper.momentum = desc->momentum;
+  t->hyper.l1 = 0.f; t->hyper.l2 = 0.f;
   {
     // parameter count is needed for the size of the gradient buffer that lives behind the parameters in the arena
     long long np = 0; int prev = desc->n_features;
@@ -732,7 +755,8 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
   SB_TRY(t->net.init(desc, device, true));
   // see Net::init: no L1 / shared-memory re-partition between the kernels of a step
   cudaFuncSetAttribute(set_batch_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  cudaFuncSetAttribute(optimizer_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  cudaFuncSetAttribute(optimizer_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  cudaFuncSetAttribute(optimizer_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   cudaFuncSetAttribute(axpy_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   Net& n = t->net;
   // streams and events of the step schedule; the side stream's CTAs are scheduled behind the main chain's
@@ -757,6 +781,7 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
     SB_CUDA(cudaMemset(n.arena + t->llg_off, 0, static_cast<size_t>(world + 1) * static_cast<size_t>(t->xch_n4) * 32));
   }
   t->s1 = n.s1; t->s2 = n.s2;
+  SB_TRY(fill_initial_state(t.get()));
   SB_TRY(n.dalloc(&t->acc, n.n_params));
   SB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&t->h_err), sizeof(unsigned int) * 4, cudaHostAllocMapped));
   SB_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&t->d_herr), t->h_err, 0));
@@ -828,14 +853,22 @@ int sb_trainer_ipc_handle(sb_trainer_t* t, void* out64) {
 // with it the thread - would never return.  Everything a non-captured path launches around an exchange is loaded up front.
 static int preload_exchange_kernels() {
   cudaFuncAttributes a;
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<2>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<4>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<8>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<16>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<2>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<4>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<8>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<16>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<2, false>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<4, false>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<8, false>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<16, false>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<2, false>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<4, false>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<8, false>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<16, false>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<2, true>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<4, true>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<8, true>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<16, true>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<2, true>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<4, true>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<8, true>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<16, true>));
   SB_CUDA(cudaFuncGetAttributes(&a, gather_master_kernel));
   SB_CUDA(cudaFuncGetAttributes(&a, set_batch_kernel));
   SB_CUDA(cudaFuncGetAttributes(&a, scale_kernel));
@@ -1008,6 +1041,26 @@ int sb_trainer_set_deterministic(sb_trainer_t* t, int32_t on) {
   SB_CHECK(n.n_cat == 0, SB_ERR_STATE, "deterministic training of a wide+deep trainer: the embedding gradient is scatter-added "
            "with red.global (embed_scatter_kernel), whose summation order is not fixed");
   return n.enable_det();
+}
+
+int sb_trainer_set_optimizer_params(sb_trainer_t* t, float initial_accumulator, float l1, float l2) {
+  SB_CHECK(t, SB_ERR_INVALID, "null trainer");
+  const int k = t->hyper.kind;
+  SB_CHECK(k == SB_OPT_ADAGRAD || k == SB_OPT_FTRL, SB_ERR_INVALID,
+           "optimizer %d reads none of initial_accumulator, l1, l2 (Adagrad and FTRL do)", k);
+  SB_CHECK(initial_accumulator > 0.f && std::isfinite(initial_accumulator), SB_ERR_INVALID,
+           "initial_accumulator must be > 0 (got %g)", initial_accumulator);
+  SB_CHECK(l1 >= 0.f && l2 >= 0.f && std::isfinite(l1) && std::isfinite(l2), SB_ERR_INVALID,
+           "l1 and l2 must be >= 0 (got %g, %g)", l1, l2);
+  SB_CHECK(k == SB_OPT_FTRL || (l1 == 0.f && l2 == 0.f), SB_ERR_INVALID, "Adagrad has no l1 / l2 (got %g, %g)", l1, l2);
+  SB_CHECK(!t->started && t->n_acc == 0 && t->global_step == 0, SB_ERR_STATE,
+           "sb_trainer_set_optimizer_params after the first step or graph capture: set it right after sb_trainer_create");
+  SB_CUDA(cudaSetDevice(t->net.device));
+  t->initial_accumulator = initial_accumulator;
+  t->hyper.l1 = l1; t->hyper.l2 = l2;
+  SB_TRY(fill_initial_state(t));
+  SB_CUDA(cudaStreamSynchronize(t->net.stream));
+  return SB_OK;
 }
 
 static int stage_sparse_batch(Net& n, const float* Xd, const int32_t* idx, const float* y, const float* w, int rows) {

@@ -503,15 +503,51 @@ out_layer_rows_kernel(const OutLayerParams p, int rows_per_block) {
 // ------------------------------------------------------------------------------------------------
 // K7 fused multi-tensor optimizer over the flat parameter vector (TF 1.x kernel forms: ApplyAdadelta
 // res/ssgd_monitor.py:138, ApplyAdam res/ssgd.py:57, ApplyGradientDescent res/ssgd_monitor_bk.py:81,
-// ApplyMomentum).  Reads the (all-reduced) gradient once, updates fp32 master weights + state, and in
-// bf16 mode refreshes the bf16 shadow of every hidden-layer weight matrix in the same pass.
+// ApplyMomentum, ApplyAdagrad, ApplyRMSProp, ApplyFtrl).  Reads the (all-reduced) gradient once, updates fp32 master
+// weights + state, and in bf16 mode refreshes the bf16 shadow of every hidden-layer weight matrix in the same pass.
 // ------------------------------------------------------------------------------------------------
 struct OptHyper {
   int kind;
-  float rho, eps, beta1, beta2, momentum;
+  float rho, eps, beta1, beta2, momentum;   // rho = RMSProp decay as well
+  float l1, l2;                             // FTRL
 };
 
+// EXT: Adagrad, RMSProp or FTRL.  Every kernel that applies the update is instantiated once per group and launched for the
+// optimizer's group, so the reference's four run without the three later cases in their switch: with one switch of all
+// seven, the larger update cost the peer exchange kernels spills (ptxas -v, DESIGN.md section 5).
+__host__ __device__ __forceinline__ bool opt_ext(int kind) { return kind >= SB_OPT_ADAGRAD; }
+
+// the state streams each optimizer has (HBM-bound passes touch only those): SGD none, Momentum and Adagrad s1, the others
+// s1 + s2
+template <bool EXT>
+__device__ __forceinline__ bool opt_uses_s1(int kind) { return EXT || kind != SB_OPT_SGD; }
+template <bool EXT>
+__device__ __forceinline__ bool opt_uses_s2(int kind) {
+  return EXT ? kind != SB_OPT_ADAGRAD : (kind == SB_OPT_ADAM || kind == SB_OPT_ADADELTA);
+}
+
+// correctly rounded sqrtf and true divisions throughout (no rsqrtf, no fast-math): the fp32 oracle bounds stay tight
+template <bool EXT>
 __device__ __forceinline__ float opt_update(const OptHyper& h, float lr_t, float theta, float g, float& s1, float& s2) {
+  if constexpr (EXT) {
+    switch (h.kind) {
+      case SB_OPT_ADAGRAD:   // s1 = accum
+        s1 = s1 + g * g;
+        return theta - lr_t * g / sqrtf(s1);
+      case SB_OPT_RMSPROP:   // s1 = ms, s2 = mom (not centered)
+        s1 = s1 + (g * g - s1) * (1.f - h.rho);
+        s2 = h.momentum * s2 + lr_t * g / sqrtf(s1 + h.eps);
+        return theta - s2;
+      default: {             // SB_OPT_FTRL: s1 = accum, s2 = linear (lr_power = -0.5, no l2 shrinkage)
+        const float a = s1 + g * g;
+        const float sa = sqrtf(a);
+        s2 = s2 + (g - (sa - sqrtf(s1)) / lr_t * theta);
+        s1 = a;
+        const float q = sa / lr_t + 2.f * h.l2;
+        return fabsf(s2) > h.l1 ? (copysignf(h.l1, s2) - s2) / q : 0.f;
+      }
+    }
+  }
   switch (h.kind) {
     case SB_OPT_SGD:
       return theta - lr_t * g;
@@ -558,6 +594,7 @@ __device__ __forceinline__ void shadow_store1(const OptWork& wk, long long at, f
   for (int part = 0; part < wk.np; ++part) wk.Wn[part * wk.part_stride + at] = __float2bfloat16_rn(bf16_residual(t, part));
 }
 
+template <bool EXT>
 static __global__ void __launch_bounds__(256)
 optimizer_kernel(const OptWork* __restrict__ work, const BatchDesc* __restrict__ desc, OptHyper h,
                  float* __restrict__ theta, const float* __restrict__ grad, float* __restrict__ s1, float* __restrict__ s2,
@@ -576,9 +613,9 @@ optimizer_kernel(const OptWork* __restrict__ work, const BatchDesc* __restrict__
   }
   const OptWork wk = work[blockIdx.x];
   const float lr_t = desc->lr_t, gs = desc->gscale;
-  // HBM-bound: only touch the state streams the optimizer actually has (SGD: none, Momentum: s1, Adam/Adadelta: s1+s2)
-  const bool use_s1 = h.kind != SB_OPT_SGD;
-  const bool use_s2 = h.kind == SB_OPT_ADAM || h.kind == SB_OPT_ADADELTA;
+  // HBM-bound: only touch the state streams the optimizer actually has
+  const bool use_s1 = opt_uses_s1<EXT>(h.kind);
+  const bool use_s2 = opt_uses_s2<EXT>(h.kind);
   if ((wk.off & 3) == 0 && (wk.count & 3) == 0 && (wk.Wn == nullptr || ((wk.out_dim & 3) == 0 && ((wk.off - wk.mat_off) & 3) == 0))) {
     // 16-byte path: one thread = 4 consecutive parameters (a full 1024-run = 256 threads x float4)
     const int e = threadIdx.x * 4;
@@ -589,10 +626,10 @@ optimizer_kernel(const OptWork* __restrict__ work, const BatchDesc* __restrict__
       float4 a = use_s1 ? *reinterpret_cast<const float4*>(s1 + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
       float4 b = use_s2 ? *reinterpret_cast<const float4*>(s2 + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
       float4 t;
-      t.x = opt_update(h, lr_t, th.x, g.x * gs, a.x, b.x);
-      t.y = opt_update(h, lr_t, th.y, g.y * gs, a.y, b.y);
-      t.z = opt_update(h, lr_t, th.z, g.z * gs, a.z, b.z);
-      t.w = opt_update(h, lr_t, th.w, g.w * gs, a.w, b.w);
+      t.x = opt_update<EXT>(h, lr_t, th.x, g.x * gs, a.x, b.x);
+      t.y = opt_update<EXT>(h, lr_t, th.y, g.y * gs, a.y, b.y);
+      t.z = opt_update<EXT>(h, lr_t, th.z, g.z * gs, a.z, b.z);
+      t.w = opt_update<EXT>(h, lr_t, th.w, g.w * gs, a.w, b.w);
       *reinterpret_cast<float4*>(theta + idx) = t;
       if (use_s1) *reinterpret_cast<float4*>(s1 + idx) = a;
       if (use_s2) *reinterpret_cast<float4*>(s2 + idx) = b;
@@ -611,7 +648,7 @@ optimizer_kernel(const OptWork* __restrict__ work, const BatchDesc* __restrict__
     if (e < wk.count) {
       const long long idx = wk.off + e;
       float a = use_s1 ? s1[idx] : 0.f, b = use_s2 ? s2[idx] : 0.f;
-      const float t = opt_update(h, lr_t, theta[idx], grad[idx] * gs, a, b);
+      const float t = opt_update<EXT>(h, lr_t, theta[idx], grad[idx] * gs, a, b);
       theta[idx] = t;
       if (use_s1) s1[idx] = a;
       if (use_s2) s2[idx] = b;

@@ -18,7 +18,9 @@ processes simply idle (the stock AM insists on >= 1 PS, SURVEY.md 8b).  The refe
 periods and the 5 s sleep per epoch are not reproduced.
 
 Optional ModelConfig train.params the reference does not have (defaults = reference behaviour):
-  Optimizer  "adadelta" (default) | "adam" | "sgd" | "momentum"
+  Optimizer  "adadelta" (default) | "adam" | "sgd" | "momentum" | "adagrad" | "rmsprop" | "ftrl", each with the TF 1.x
+             defaults of its other hyperparameters (Adagrad initial_accumulator 0.1; RMSProp decay 0.9, momentum 0,
+             epsilon 1e-10, not centered; FTRL learning_rate_power -0.5, initial_accumulator 0.1, l1 = l2 = 0)
   Loss       "squared" (default: MSE on the sigmoid output, ssgd_monitor.py:129) | "log" (sigmoid cross-entropy)
   Precision  "bf16" (default) | "fp32" (CUDA-core parity mode) | "fp32_tc" (fp32-class accuracy on the tensor cores:
              three bf16 parts per value) | "bf16x2" (two parts)
@@ -71,7 +73,8 @@ REPLICAS_TO_AGGREGATE_RATIO = 1
 DELIMITER = '|'
 BATCH_SIZE = 100
 
-_OPT = {"adadelta": capi.OPT_ADADELTA, "adam": capi.OPT_ADAM, "sgd": capi.OPT_SGD, "momentum": capi.OPT_MOMENTUM}
+_OPT = {"adadelta": capi.OPT_ADADELTA, "adam": capi.OPT_ADAM, "sgd": capi.OPT_SGD, "momentum": capi.OPT_MOMENTUM,
+        "adagrad": capi.OPT_ADAGRAD, "rmsprop": capi.OPT_RMSPROP, "ftrl": capi.OPT_FTRL}
 _LOSS = {"squared": capi.LOSS_MSE, "log": capi.LOSS_SIGMOID_CE}
 
 
