@@ -23,6 +23,27 @@ using namespace sb;
 // ================================================================================================
 enum { G_STEP = 0, G_ACC = 1, G_KINDS = 2 };
 
+// A captured graph: `steps` consecutive steps (1, or RUN_S for sb_trainer_run_resident) of `kind` over `rows`-row batches
+// of feed `feed`, reading the descriptor slots of ring set `set`
+struct GraphKey {
+  int rows, kind;
+  Feed feed;
+  int steps, set;
+  bool operator<(const GraphKey& o) const {
+    return std::tie(rows, kind, feed, steps, set) < std::tie(o.rows, o.kind, o.feed, o.steps, o.set);
+  }
+};
+
+// One step's batch: everything set_batch_kernel reads besides the update's scalars (write_desc)
+struct Batch {
+  Feed feed = Feed::HOST;
+  const float *X = nullptr, *y = nullptr, *w = nullptr;
+  int row0 = 0;                     // RESIDENT: first row in the resident set
+  const int* nz_prefix = nullptr;   // RESIDENT: n_nz is published from the set's prefix counts
+  const int* order = nullptr;       // ORDERED: the batch's slice of the row order
+  int rows = 0;
+};
+
 struct sb_trainer {
   Net net;
   sb_net_desc desc;
@@ -52,9 +73,8 @@ struct sb_trainer {
   int* ord = nullptr;
   long long ord_n = 0, ord_cap = 0;
   float *ordY = nullptr, *ordW = nullptr;   // [max_batch] labels / weights of an ordered step's batch (gather_batch_kernel)
-  // (rows, ordered * 16 + kind * 8 + sparse * 4 + resident * 2 + pair) -> captured step
-  std::map<std::pair<int, int>, cudaGraphExec_t> graphs;
-  std::map<int, int> kernels_per_step;   // rows * 2 + ordered
+  std::map<GraphKey, cudaGraphExec_t> graphs;
+  std::map<std::pair<int, Feed>, int> kernels_per_step;   // (rows, feed) of a captured single G_STEP step
   // peer-memory exchange (xchg_p2p.cuh): the net's parameter arena [theta | s1 | s2 | shadows | gradient | P2PFlags] is
   // ONE exported allocation; `xch` aliases it
   void* xch = nullptr;
@@ -94,29 +114,24 @@ struct sb_trainer {
   cudaEvent_t ev_copied[2] = {nullptr, nullptr}, ev_consumed[2] = {nullptr, nullptr};
   bool copy_ready = false;   // every piece of the second slot exists
   unsigned long long async_steps = 0;
-  // resident steps: the batch descriptor of step i+1 is written on `prep` while step i still runs (two descriptor /
-  // scalar pairs, one captured graph per pair), so set_batch_kernel leaves the critical path
-  BatchDesc* descs[2] = {nullptr, nullptr};
-  float* scals[2] = {nullptr, nullptr};
+  // Descriptor ring: two sets of RUN_S (descriptor, scalar) slots; set 0 slot 0 is the net's own.  sb_trainer_run_resident
+  // captures RUN_S steps per graph (kernel -> kernel edges instead of a graph turn-around between steps).  Prefetched
+  // launches (bf16-resident and ordered steps) alternate between the sets: the descriptors of launch i+1 are written on
+  // `prep` while launch i still runs, so set_batch_kernel leaves the critical path.  Every other user of a slot writes
+  // set 0 (host-batch steps, forward paths) or the last prefetched set (update-only launches) on the main stream.
+  enum { RUN_S = 4 };
+  BatchDesc* ring_desc[2][RUN_S] = {};
+  float* ring_scal[2][RUN_S] = {};
   cudaStream_t prep = nullptr;
   cudaEvent_t ev_prep[2] = {nullptr, nullptr}, ev_pos[2] = {nullptr, nullptr};
-  unsigned long long prep_steps = 0;
+  unsigned long long prefetches = 0;   // prefetched launches so far: launch i uses set i & 1
   bool started = false;    // a step ran or was captured: sb_trainer_set_deterministic is refused from here on
-  bool have_pos = false;   // ev_pos[] of the previous step is valid (no other user of the descriptors in between)
-  int last_pair = 0;       // the pair the last step used
-  // sb_trainer_run_resident: RUN_S steps per captured graph (kernel -> kernel edges instead of a graph turn-around
-  // between steps), two alternating descriptor sets so that the descriptors of chunk i+1 are written while chunk i runs
-  enum { RUN_S = 4 };
-  BatchDesc* run_descs[2][RUN_S] = {};
-  float* run_scals[2][RUN_S] = {};
-  cudaEvent_t ev_run_prep[2] = {nullptr, nullptr}, ev_run_done[2] = {nullptr, nullptr};
-  bool run_ready = false;  // every descriptor, scalar block and event of both sets exists
-  bool run_used[2] = {false, false};
-  unsigned long long run_chunks = 0;
-  std::map<int, cudaGraphExec_t> run_graphs;   // (rows * 2 + set) * 2 + ordered
+  bool have_pos = false;   // ev_pos[] of the previous prefetched launch is valid (no step on set 0 since)
+  int last_set = 0;        // the set of the last prefetched launch
+  StepIn slot(int set, int k, Feed feed = Feed::HOST) const { return StepIn{ring_desc[set][k], ring_scal[set][k], feed}; }
 
-  // Releases what the trainer created.  Pointers into the net's allocations (descs, scals, grad, flags, xch, s1, s2, acc,
-  // st2*, run_descs, run_scals) are freed by `net`, the first member and so the last destroyed.
+  // Releases what the trainer created.  Pointers into the net's allocations (ring_desc, ring_scal, grad, flags, xch, s1,
+  // s2, acc, st2*) are freed by `net`, the first member and so the last destroyed.
   ~sb_trainer() {
     drop_step_graphs();
     auto destroy_event = [](cudaEvent_t e) { if (e) cudaEventDestroy(e); };
@@ -127,7 +142,6 @@ struct sb_trainer {
     for (int i = 0; i < 2; ++i) {
       destroy_event(ev_copied[i]); destroy_event(ev_consumed[i]);
       destroy_event(ev_prep[i]); destroy_event(ev_pos[i]);
-      destroy_event(ev_run_prep[i]); destroy_event(ev_run_done[i]);
     }
     if (prep) cudaStreamSynchronize(prep);
     for (cudaStream_t s : {xstream[0], xstream[1], side, prep, copy_stream}) if (s) cudaStreamDestroy(s);
@@ -143,8 +157,6 @@ struct sb_trainer {
   void drop_step_graphs() {   // captured steps carry the exchange and the resident set they were captured with
     for (auto& kv : graphs) cudaGraphExecDestroy(kv.second);
     graphs.clear();
-    for (auto& kv : run_graphs) cudaGraphExecDestroy(kv.second);
-    run_graphs.clear();
   }
   void free_dataset() {
     if (dsX) cudaFree(dsX);
@@ -161,6 +173,8 @@ struct sb_trainer {
     ord_n = ord_cap = 0;
   }
   long long resident_len() const { return ord_n > 0 ? ord_n : ds_rows; }   // what resident offsets are checked against
+  // the feed of a resident step: the fp32 set is read in place through the host-batch graph
+  Feed resident_feed() const { return ord_n > 0 ? Feed::ORDERED : dsXb ? Feed::RESIDENT : Feed::HOST; }
   void close_peer_mappings() {
     for (void* p : peer_bases) cudaIpcCloseMemHandle(p);
     peer_bases.clear();
@@ -178,6 +192,62 @@ static float lr_for_step(const sb_trainer* t, long long step /*1-based*/) {
     return static_cast<float>(t->lr * sqrt(1.0 - pow(b2, static_cast<double>(step))) / (1.0 - pow(b1, static_cast<double>(step))));
   }
   return t->lr;
+}
+
+// an update: advances the step count and the exchange round; -> the update's learning rate
+static float begin_update(sb_trainer* t) {
+  ++t->global_step;
+  ++t->epoch;
+  return lr_for_step(t, t->global_step);
+}
+
+// The only writer of a step descriptor: batch `b` (nullptr: an update without a batch), the update's scalars and the
+// step's slot in the loss history, into slot `in` on stream `st`
+static int write_desc(cudaStream_t st, const StepIn& in, const Batch* b, float lr_t, float gscale, unsigned int epoch,
+                      float2* hist) {
+  static const Batch none{};
+  const Batch& x = b ? *b : none;
+  return launch_kernel(set_batch_kernel, dim3(1), dim3(1), 0, st, false, in.desc, x.X, x.y, x.w, lr_t, gscale, epoch, x.row0,
+                       x.nz_prefix, x.rows, in.scal, hist, x.order);
+}
+
+// a batch of fp32 rows on the device (the staging area, or the fp32 resident set); w == nullptr weighs every row 1
+static Batch host_batch(const Net& n, const float* X, const float* y, const float* w, int rows, Feed feed = Feed::HOST) {
+  Batch b;
+  b.feed = feed;
+  b.X = X; b.y = y; b.w = w ? w : n.ones;
+  b.rows = rows;
+  return b;
+}
+
+// rows [off, off + rows) of the resident set, through the row order if one is set.  step >= 0 names the step of a run
+// in the error message.
+static int resident_batch(const sb_trainer* t, long long off, int rows, int step, Batch* b) {
+  SB_CHECK(t->ds_rows > 0, SB_ERR_STATE, "no resident dataset loaded");
+  const long long len = t->resident_len();
+  if (off < 0 || rows <= 0 || off + rows > len) {
+    char at[32] = "";
+    if (step >= 0) snprintf(at, sizeof(at), "step %d: ", step);
+    return set_error(SB_ERR_INVALID, "%srows [%lld, %lld) outside the resident set of %lld %s", at, off, off + rows, len,
+                     t->ord_n > 0 ? "rows of the row order" : "rows");
+  }
+  SB_CHECK(rows <= t->net.max_batch, SB_ERR_INVALID, "rows=%d outside (0, max_batch=%d]", rows, t->net.max_batch);
+  *b = Batch{};
+  b->feed = t->resident_feed();
+  b->rows = rows;
+  if (b->feed == Feed::ORDERED) {   // gather_batch_kernel counts n_nz and fills ordY / ordW
+    b->y = t->ordY; b->w = t->ordW;
+    b->order = t->ord + off;
+    return SB_OK;
+  }
+  b->y = t->dsY + off; b->w = t->dsW + off;
+  if (b->feed == Feed::RESIDENT) {
+    b->row0 = static_cast<int>(off);
+    b->nz_prefix = t->dsP;
+  } else {
+    b->X = t->dsX + off * t->net.F;
+  }
+  return SB_OK;
 }
 
 static int enqueue_allreduce(sb_trainer* t, float* buf) {
@@ -426,7 +496,7 @@ static int enqueue_step_backward(sb_trainer* t, const StepIn& in, int rows, int 
       // dW_0 has nothing to overlap with (no dA_0): PDL-chained on the main stream right behind the last GEMM it starts
       // earlier than as a cross-stream launch.  With the peer exchange it is cut into the slot chunks (each a contiguous
       // slice of the flat gradient) and each chunk's exchange overlaps the GEMMs that follow it.
-      if (xsched && !in.sparse) {
+      if (xsched && in.feed != Feed::SPARSE) {
         for (int c = 0; c < t->x_chunks; ++c) {
           const int r0 = c * t->x_chunk_rows, r1 = std::min(r0 + t->x_chunk_rows, n.layers[0].in);
           SB_TRY(n.enqueue_dw(in, 0, rows, g, n.stream, true, d1.sms[0], r0, r1, t->x_chunks > 1 ? c : -1));
@@ -450,7 +520,7 @@ static int enqueue_step_backward(sb_trainer* t, const StepIn& in, int rows, int 
     if (xsched) {
       // whatever follows on the main stream (the next step's layer-0 forward, or the end of the graph) needs hidden
       // layer 0.  A wide+deep step's layer-0 dW is not cut into the slot chunks: it is exchanged here, behind everything.
-      if (in.sparse) SB_TRY(enqueue_xchg(t, in, xseg_all(t) & ~XSEG_A, n.stream, true, false));
+      if (in.feed == Feed::SPARSE) SB_TRY(enqueue_xchg(t, in, xseg_all(t) & ~XSEG_A, n.stream, true, false));
       else
         for (int c = 0; c < t->x_chunks; ++c) SB_CUDA(cudaStreamWaitEvent(n.stream, t->ev_x[1 + c], 0));
       SB_CUDA(cudaStreamWaitEvent(n.stream, t->ev_x[0], 0));
@@ -504,36 +574,40 @@ static int enqueue_gather(sb_trainer* t, const StepIn& in, int rows, float* clea
   return SB_OK;
 }
 
+// The first kernel of a step or forward, by feed: HOST / SPARSE load_batch_kernel, ORDERED gather_batch_kernel (t: its
+// trainer), RESIDENT none (layer 0 reads the set by TMA; set_batch_kernel already published n_nz).  Clears
+// clear[0, clear_n) on the way.
+static int enqueue_first(Net& n, sb_trainer* t, const StepIn& in, int rows, float* clear, long long clear_n) {
+  if (in.feed == Feed::RESIDENT) return SB_OK;
+  if (in.feed == Feed::ORDERED) return enqueue_gather(t, in, rows, clear, clear_n);
+  return n.enqueue_load(in, rows, clear, clear_n);
+}
+
 // the body of one step as a sequence of stream operations (captured into a CUDA graph)
 static int enqueue_step_body(sb_trainer* t, const StepIn& in, int rows, int kind) {
   Net& n = t->net;
   n.trace_k = 0;
   float4* clear = nullptr;
   long long clear_n4 = 0;
-  if (in.resident) {
-    // no load kernel: the batch is read by TMA from the bf16 resident set; set_batch_kernel already published n_nz.
-    // The gradient buffer is first written by the last forward layer's epilogue, so with more than one hidden layer the
-    // layer-0 forward GEMM clears it (its producer warpgroup's idle warps, beside the main loop) instead of a memset node
-    // at the head of the chain.
+  if (in.feed == Feed::RESIDENT) {
+    // no first kernel to clear the gradient buffer.  It is first written by the last forward layer's epilogue, so with
+    // more than one hidden layer the layer-0 forward GEMM clears it (its producer warpgroup's idle warps, beside the main
+    // loop) instead of a memset node at the head of the chain.
     if (n.L > 1) {
       clear = reinterpret_cast<float4*>(t->grad);   // cudaMalloc'ed, padded to xch_n4 float4
       clear_n4 = t->xch_n4;
     } else {
       SB_CUDA(cudaMemsetAsync(t->grad, 0, sizeof(float) * n.n_params, n.stream));
     }
-  } else if (in.ordered) {
-    SB_TRY(enqueue_gather(t, in, rows, t->grad, n.n_params));
-  } else {
-    SB_TRY(n.enqueue_load(in, rows, t->grad, n.n_params));   // also clears the gradient buffer and the step scalars
   }
+  SB_TRY(enqueue_first(n, t, in, rows, t->grad, n.n_params));   // also clears the step scalars
   bool fused_out = false;
   SB_TRY(n.enqueue_hidden_forward(in, rows, t->grad, &fused_out, clear, clear_n4));
   if (!fused_out) SB_TRY(n.enqueue_out(in, rows, true, true, nullptr, t->grad));
   return enqueue_step_backward(t, in, rows, kind);
 }
 
-static int get_graph(sb_trainer* t, const StepIn& in, int rows, int kind, int pair, cudaGraphExec_t* out) {
-  auto key = std::make_pair(rows, (in.ordered ? 16 : 0) + kind * 8 + (in.sparse ? 4 : 0) + (in.resident ? 2 : 0) + pair);
+static int get_graph(sb_trainer* t, const GraphKey& key, cudaGraphExec_t* out) {
   auto it = t->graphs.find(key);
   if (it != t->graphs.end()) { *out = it->second; return SB_OK; }
   Net& n = t->net;
@@ -541,7 +615,14 @@ static int get_graph(sb_trainer* t, const StepIn& in, int rows, int kind, int pa
   n.launches = 0;
   cudaGraph_t g = nullptr;
   SB_CUDA(cudaStreamBeginCapture(n.stream, cudaStreamCaptureModeThreadLocal));
-  int s = enqueue_step_body(t, in, rows, kind);
+  int s = SB_OK;
+  for (int k = 0; k < key.steps && s == SB_OK; ++k) {
+    // (SB_STEP_TRACE: of a run, an interior step is the one traced - it starts behind the previous step's tail, as most
+    // steps of a run do)
+    n.trace_on = key.steps == 1 || k == 1;
+    s = enqueue_step_body(t, t->slot(key.set, k, key.feed), key.rows, key.kind);
+  }
+  n.trace_on = true;
   cudaError_t e = cudaStreamEndCapture(n.stream, &g);
   if (s != SB_OK) { if (g) cudaGraphDestroy(g); return s; }
   SB_CHECK(e == cudaSuccess, SB_ERR_CUDA, "cudaStreamEndCapture failed: %s", cudaGetErrorString(e));
@@ -549,13 +630,34 @@ static int get_graph(sb_trainer* t, const StepIn& in, int rows, int kind, int pa
   SB_CUDA(cudaGraphInstantiate(&ge, g, 0));
   cudaGraphDestroy(g);
   t->graphs[key] = ge;
-  if (kind == G_STEP && !in.sparse && (in.resident || in.ordered || !t->dsXb))
-    t->kernels_per_step[rows * 2 + (in.ordered ? 1 : 0)] = n.launches + 1;  // + set_batch_kernel
+  if (key.steps == 1 && key.kind == G_STEP && key.feed != Feed::SPARSE)
+    t->kernels_per_step[{key.rows, key.feed}] = n.launches + 1;  // + set_batch_kernel
   *out = ge;
   return SB_OK;
 }
 
-// X, y, w are DEVICE pointers here
+// A prefetched launch writes the descriptors of ring set `set` = prefetches & 1 on `prep`:
+//   prefetch_begin(t, set);  write_desc(t->prep, t->slot(set, k), ...) ...;  prefetch_end(t, set);  graph launch
+// Set s was last read by the prefetched launch two back and by whatever followed it on the main stream before the previous
+// prefetched launch (update-only launches write the last set there): ev_pos[s ^ 1], recorded right before that launch,
+// covers both.  Without one (have_pos false: the first prefetched launch, or a step on set 0 since), join the main stream's
+// current position.
+static int prefetch_begin(sb_trainer* t, int set) {
+  if (!t->have_pos) SB_CUDA(cudaEventRecord(t->ev_pos[set ^ 1], t->net.stream));
+  SB_CUDA(cudaStreamWaitEvent(t->prep, t->ev_pos[set ^ 1], 0));
+  return SB_OK;
+}
+
+static int prefetch_end(sb_trainer* t, int set) {
+  SB_CUDA(cudaEventRecord(t->ev_prep[set], t->prep));
+  SB_CUDA(cudaEventRecord(t->ev_pos[set], t->net.stream));
+  SB_CUDA(cudaStreamWaitEvent(t->net.stream, t->ev_prep[set], 0));
+  t->have_pos = true;
+  t->last_set = set;
+  ++t->prefetches;
+  return SB_OK;
+}
+
 // A deterministic trainer with more than one rank needs the peer-memory exchange, which adds the ranks' gradients in rank
 // order; NCCL's all-reduce promises no summation order.
 static int check_det_exchange(const sb_trainer* t) {
@@ -565,60 +667,65 @@ static int check_det_exchange(const sb_trainer* t) {
   return SB_OK;
 }
 
-static int run_step(sb_trainer* t, const float* X, const float* y, const float* w, int rows, int kind, long long resident_row0 = -1,
-                    bool sparse = false) {
+// One step over batch `b`: bf16-resident and ordered steps are prefetched, every other step writes set 0 on the main stream
+static int run_step(sb_trainer* t, const Batch& b, int kind) {
   Net& n = t->net;
   SB_TRY(check_det_exchange(t));
   t->started = true;
-  SB_CHECK(rows > 0 && rows <= n.max_batch, SB_ERR_INVALID, "rows=%d outside (0, max_batch=%d]", rows, n.max_batch);
+  SB_CHECK(b.rows > 0 && b.rows <= n.max_batch, SB_ERR_INVALID, "rows=%d outside (0, max_batch=%d]", b.rows, n.max_batch);
   SB_CUDA(cudaSetDevice(n.device));
-  // ordered: resident_row0 is a position in the row order, y / w are ordY / ordW (resident_step)
-  const bool ordered = resident_row0 >= 0 && t->ord_n > 0;
-  const bool resident = resident_row0 >= 0 && t->dsXb != nullptr && !ordered;
-  const int* order = ordered ? t->ord + resident_row0 : nullptr;
-  const int row0 = ordered ? 0 : static_cast<int>(resident_row0);
-  const int* nz_prefix = ordered ? nullptr : t->dsP;   // an ordered step's n_nz is counted by gather_batch_kernel
-  // descriptor / scalar pair of this step: resident graph steps alternate, everything else uses pair 0
-  const bool prep = (resident || ordered) && t->prep != nullptr;
-  const int pair = prep ? static_cast<int>(t->prep_steps & 1) : 0;
-  const StepIn in{t->descs[pair], t->scals[pair], resident, sparse, ordered};
-  t->last_pair = pair;
+  const bool prefetch = b.feed == Feed::RESIDENT || b.feed == Feed::ORDERED;
+  const int set = prefetch ? static_cast<int>(t->prefetches & 1) : 0;
   cudaGraphExec_t ge = nullptr;
-  SB_TRY(get_graph(t, in, rows, kind, pair, &ge));
-  float lr_t = t->lr, gscale = 1.f / static_cast<float>(t->world);
-  if (kind == G_STEP) {
-    ++t->global_step;
-    lr_t = lr_for_step(t, t->global_step);
-  }
-  if (kind == G_STEP) ++t->epoch;
-  if (prep) {
-    // pair `pair` was last read by the step two back and by whatever followed it on the main stream before the previous
-    // step's graph: ev_pos[pair ^ 1] (recorded right before that graph) covers both.  First step of a run: join the
-    // main stream's current position.
-    if (!t->have_pos) SB_CUDA(cudaEventRecord(t->ev_pos[pair ^ 1], n.stream));
-    SB_CUDA(cudaStreamWaitEvent(t->prep, t->ev_pos[pair ^ 1], 0));
-    set_batch_kernel<<<1, 1, 0, t->prep>>>(in.desc, nullptr, y, w, lr_t, gscale, t->epoch, row0, nz_prefix, rows, in.scal,
-                                           kind == G_STEP ? t->hist_slot(t->global_step) : nullptr, order);
-    SB_CUDA(cudaGetLastError());
-    SB_CUDA(cudaEventRecord(t->ev_prep[pair], t->prep));
-    SB_CUDA(cudaEventRecord(t->ev_pos[pair], n.stream));
-    SB_CUDA(cudaStreamWaitEvent(n.stream, t->ev_prep[pair], 0));
-    t->have_pos = true;
-    ++t->prep_steps;
+  SB_TRY(get_graph(t, GraphKey{b.rows, kind, b.feed, 1, set}, &ge));
+  const float gscale = 1.f / static_cast<float>(t->world);
+  const float lr_t = kind == G_STEP ? begin_update(t) : t->lr;
+  float2* hist = kind == G_STEP ? t->hist_slot(t->global_step) : nullptr;
+  if (prefetch) {
+    SB_TRY(prefetch_begin(t, set));
+    SB_TRY(write_desc(t->prep, t->slot(set, 0), &b, lr_t, gscale, t->epoch, hist));
+    SB_TRY(prefetch_end(t, set));
   } else {
     t->have_pos = false;
-    if (resident || ordered)
-      set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, nullptr, y, w, lr_t, gscale, t->epoch, row0, nz_prefix, rows, in.scal,
-                                               kind == G_STEP ? t->hist_slot(t->global_step) : nullptr, order);
-    else
-      set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, X, y, w ? w : n.ones, lr_t, gscale, t->epoch, 0, nullptr, 0, nullptr,
-                                               kind == G_STEP ? t->hist_slot(t->global_step) : nullptr);
+    SB_TRY(write_desc(n.stream, t->slot(0, 0), &b, lr_t, gscale, t->epoch, hist));
   }
-  SB_CUDA(cudaGetLastError());
   SB_CUDA(cudaGraphLaunch(ge, n.stream));
   // the step's tail kernel (optimizer / accumulate) wrote (loss sum, n_nz) into h_scal; visible after a stream sync
   if (kind == G_ACC) ++t->n_acc;
   t->grad_out_scale = (kind == G_STEP) ? gscale : 1.f;
+  return SB_OK;
+}
+
+// The forward of one batch on the main stream: its descriptor into slot `in`, the feed's first kernel, the hidden layers and
+// the output layer (do_loss: + the loss sum into in.scal), scores to yhat_dst (nullable).  t: the trainer of an ORDERED
+// batch (the scorer has none).
+static int enqueue_forward(Net& n, sb_trainer* t, StepIn in, const Batch& b, unsigned int epoch, bool do_loss, float* yhat_dst) {
+  in.feed = b.feed;
+  SB_TRY(write_desc(n.stream, in, &b, 0.f, 1.f, epoch, nullptr));
+  SB_TRY(enqueue_first(n, t, in, b.rows, nullptr, 0));
+  SB_TRY(n.enqueue_hidden_forward(in, b.rows));
+  return n.enqueue_out(in, b.rows, do_loss, false, yhat_dst, nullptr);
+}
+
+// forward (+ loss if loss_sum != nullptr) over any number of rows in max_batch chunks: stage(r0, c, &b) stages rows
+// [r0, r0 + c) and describes them in b; out nullable.
+// (Slot set 0: these host-driven paths are not captured.  A step queues its descriptor writes ahead of its graph on the
+// main stream, and every forward path synchronises that stream before it returns, so no descriptor prefetch overlaps them.)
+template <typename Stage>
+static int forward_chunks(Net& n, int64_t rows, Stage stage, float* out, double* loss_sum, double* nnz) {
+  SB_CUDA(cudaSetDevice(n.device));
+  const StepIn in{n.desc, n.scal};
+  float h[SCAL_COUNT];
+  for (int64_t r0 = 0; r0 < rows; r0 += n.max_batch) {
+    const int c = static_cast<int>(rows - r0 < n.max_batch ? rows - r0 : n.max_batch);
+    Batch b;
+    SB_TRY(stage(r0, c, &b));
+    SB_TRY(enqueue_forward(n, nullptr, in, b, 0, loss_sum != nullptr, n.yhat));
+    if (out) SB_CUDA(cudaMemcpyAsync(out + r0, n.yhat, sizeof(float) * c, cudaMemcpyDefault, n.stream));
+    if (loss_sum) SB_CUDA(cudaMemcpyAsync(h, in.scal, sizeof(h), cudaMemcpyDeviceToHost, n.stream));
+    SB_CUDA(cudaStreamSynchronize(n.stream));
+    if (loss_sum) { *loss_sum += h[SCAL_LOSS_SUM]; *nnz += h[SCAL_NNZ]; }
+  }
   return SB_OK;
 }
 
@@ -815,15 +922,17 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
   SB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&t->h_hist), sizeof(float2) * sb_trainer::HIST, cudaHostAllocMapped));
   SB_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&t->d_hist), t->h_hist, 0));
   memset(t->h_hist, 0, sizeof(float2) * sb_trainer::HIST);
-  t->descs[0] = n.desc;
-  t->scals[0] = n.scal;
-  SB_TRY(n.dalloc(&t->descs[1], 1));
-  SB_TRY(n.dalloc(&t->scals[1], SCAL_COUNT));
-  SB_CUDA(cudaStreamCreateWithFlags(&t->prep, cudaStreamNonBlocking));
-  for (int i = 0; i < 2; ++i) {
-    SB_TRY(create_event(&t->ev_prep[i]));
-    SB_TRY(create_event(&t->ev_pos[i]));
+  t->ring_desc[0][0] = n.desc;
+  t->ring_scal[0][0] = n.scal;
+  for (int set = 0; set < 2; ++set) {
+    for (int k = set == 0 ? 1 : 0; k < sb_trainer::RUN_S; ++k) {
+      SB_TRY(n.dalloc(&t->ring_desc[set][k], 1));
+      SB_TRY(n.dalloc(&t->ring_scal[set][k], SCAL_COUNT));
+    }
+    SB_TRY(create_event(&t->ev_prep[set]));
+    SB_TRY(create_event(&t->ev_pos[set]));
   }
+  SB_CUDA(cudaStreamCreateWithFlags(&t->prep, cudaStreamNonBlocking));
   SB_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&t->d_hscal), t->h_scal, 0));
   if (world > 1 && nccl_id != nullptr) {
     NcclApi* api = nccl_api();
@@ -1018,7 +1127,7 @@ int sb_trainer_get_grads(sb_trainer_t* t, float* flat, int64_t n) {
 int sb_trainer_step(sb_trainer_t* t, const float* X, const float* y, const float* w, int32_t rows, float* loss_out) {
   SB_CHECK(t, SB_ERR_INVALID, "null trainer");
   SB_TRY(stage_host_batch(t, X, y, w, rows));
-  SB_TRY(run_step(t, t->net.stX, t->net.stY, w ? t->net.stW : nullptr, rows, G_STEP));
+  SB_TRY(run_step(t, host_batch(t->net, t->net.stX, t->net.stY, w ? t->net.stW : nullptr, rows), G_STEP));
   return finish_loss(t, loss_out);
 }
 
@@ -1081,41 +1190,30 @@ int sb_trainer_step_sparse(sb_trainer_t* t, const float* Xd, const int32_t* idx,
                            float* loss_out) {
   SB_CHECK(t && y, SB_ERR_INVALID, "null argument");
   SB_TRY(stage_sparse_batch(t->net, Xd, idx, y, w, rows));
-  SB_TRY(run_step(t, t->net.stX, t->net.stY, w ? t->net.stW : nullptr, rows, G_STEP, -1, true));
+  SB_TRY(run_step(t, host_batch(t->net, t->net.stX, t->net.stY, w ? t->net.stW : nullptr, rows, Feed::SPARSE), G_STEP));
   return finish_loss(t, loss_out);
 }
 
-// forward (+ loss) over any number of sparse rows in max_batch chunks; out / loss accumulators nullable
-static int forward_chunks_sparse(Net& n, const float* Xd, const int32_t* idx, const float* y, const float* w, int64_t rows, float* out,
-                                 double* loss_sum, double* nnz) {
-  const StepIn in{n.desc, n.scal, false, true};      // (the trainer's pair 0, see forward_chunks)
-  const bool do_loss = loss_sum != nullptr;
-  float h[SCAL_COUNT];
-  for (int64_t r0 = 0; r0 < rows; r0 += n.max_batch) {
-    const int c = static_cast<int>(rows - r0 < n.max_batch ? rows - r0 : n.max_batch);
-    SB_TRY(stage_sparse_batch(n, Xd + r0 * n.n_dense, idx + r0 * n.n_cat, do_loss ? y + r0 : nullptr, (do_loss && w) ? w + r0 : nullptr, c));
-    set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, n.stX, n.stY, (do_loss && w) ? n.stW : n.ones, 0.f, 1.f);
-    SB_TRY(n.enqueue_load(in, c));
-    SB_TRY(n.enqueue_hidden_forward(in, c));
-    SB_TRY(n.enqueue_out(in, c, do_loss, false, n.yhat, nullptr));
-    if (out) SB_CUDA(cudaMemcpyAsync(out + r0, n.yhat, sizeof(float) * c, cudaMemcpyDeviceToHost, n.stream));
-    if (do_loss) SB_CUDA(cudaMemcpyAsync(h, in.scal, sizeof(h), cudaMemcpyDeviceToHost, n.stream));
-    SB_CUDA(cudaStreamSynchronize(n.stream));
-    if (do_loss) { *loss_sum += h[SCAL_LOSS_SUM]; *nnz += h[SCAL_NNZ]; }
-  }
-  return SB_OK;
+// forward (+ loss: y != nullptr) over any number of sparse rows; out / loss accumulators nullable
+static int forward_sparse(Net& n, const float* Xd, const int32_t* idx, const float* y, const float* w, int64_t rows, float* out,
+                          double* loss_sum, double* nnz) {
+  return forward_chunks(n, rows, [&](int64_t r0, int c, Batch* b) -> int {
+    SB_TRY(stage_sparse_batch(n, Xd + r0 * n.n_dense, idx + r0 * n.n_cat, y ? y + r0 : nullptr, (y && w) ? w + r0 : nullptr, c));
+    *b = host_batch(n, n.stX, n.stY, (y && w) ? n.stW : nullptr, c, Feed::SPARSE);
+    return SB_OK;
+  }, out, loss_sum, nnz);
 }
 
 int sb_trainer_predict_sparse(sb_trainer_t* t, const float* Xd, const int32_t* idx, int64_t rows, float* out) {
   SB_CHECK(t && out, SB_ERR_INVALID, "null argument");
-  return forward_chunks_sparse(t->net, Xd, idx, nullptr, nullptr, rows, out, nullptr, nullptr);
+  return forward_sparse(t->net, Xd, idx, nullptr, nullptr, rows, out, nullptr, nullptr);
 }
 
 int sb_trainer_eval_loss_sparse(sb_trainer_t* t, const float* Xd, const int32_t* idx, const float* y, const float* w, int64_t rows,
                                 float* loss_out) {
   SB_CHECK(t && y && loss_out && rows > 0, SB_ERR_INVALID, "bad argument");
   double ls = 0, nz = 0;
-  SB_TRY(forward_chunks_sparse(t->net, Xd, idx, y, w, rows, nullptr, &ls, &nz));
+  SB_TRY(forward_sparse(t->net, Xd, idx, y, w, rows, nullptr, &ls, &nz));
   *loss_out = nz > 0 ? static_cast<float>(ls / nz) : 0.f;
   return SB_OK;
 }
@@ -1148,7 +1246,7 @@ int sb_trainer_step_async(sb_trainer_t* t, const float* X, const float* y, const
   if (w) SB_CUDA(cudaMemcpyAsync(sw, w, sizeof(float) * rows, cudaMemcpyHostToDevice, t->copy_stream));
   SB_CUDA(cudaEventRecord(t->ev_copied[slot], t->copy_stream));
   SB_CUDA(cudaStreamWaitEvent(n.stream, t->ev_copied[slot], 0));
-  SB_TRY(run_step(t, sx, sy, w ? sw : nullptr, rows, G_STEP));
+  SB_TRY(run_step(t, host_batch(n, sx, sy, w ? sw : nullptr, rows), G_STEP));
   SB_CUDA(cudaEventRecord(t->ev_consumed[slot], n.stream));
   ++t->async_steps;
   return SB_OK;
@@ -1157,7 +1255,7 @@ int sb_trainer_step_async(sb_trainer_t* t, const float* X, const float* y, const
 int sb_trainer_accumulate(sb_trainer_t* t, const float* X, const float* y, const float* w, int32_t rows, float* loss_out) {
   SB_CHECK(t, SB_ERR_INVALID, "null trainer");
   SB_TRY(stage_host_batch(t, X, y, w, rows));
-  SB_TRY(run_step(t, t->net.stX, t->net.stY, w ? t->net.stW : nullptr, rows, G_ACC));
+  SB_TRY(run_step(t, host_batch(t->net, t->net.stX, t->net.stY, w ? t->net.stW : nullptr, rows), G_ACC));
   return finish_loss(t, loss_out);
 }
 
@@ -1178,13 +1276,11 @@ int sb_trainer_apply_accumulated_mean(sb_trainer_t* t, int64_t total_pushes) {
 static int apply_accumulated_impl(sb_trainer_t* t, int64_t total_pushes) {
   Net& n = t->net;
   SB_CUDA(cudaSetDevice(n.device));
-  ++t->global_step;
   const float gscale = 1.f / static_cast<float>(total_pushes);
-  ++t->epoch;
-  // the last step's pair: the next resident step's descriptor prefetch may write the other one while this update runs
-  const StepIn in{t->descs[t->last_pair], t->scals[t->last_pair]};
-  set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, nullptr, nullptr, nullptr, lr_for_step(t, t->global_step), gscale, t->epoch);
-  SB_CUDA(cudaGetLastError());
+  const float lr_t = begin_update(t);
+  // the last prefetched set: the next descriptor prefetch writes the other one, possibly while this update runs
+  const StepIn in = t->slot(t->last_set, 0);
+  SB_TRY(write_desc(n.stream, in, nullptr, lr_t, gscale, t->epoch, nullptr));
   // exchange + apply through the (IPC-exported) gradient buffer; it then holds the applied mean for sb_trainer_get_grads
   SB_CUDA(cudaMemcpyAsync(t->grad, t->acc, sizeof(float) * n.n_params, cudaMemcpyDeviceToDevice, n.stream));
   if (t->world > 1 && t->p2p_ready) {
@@ -1268,41 +1364,9 @@ int sb_trainer_load_dataset(sb_trainer_t* t, const float* X, const float* y, con
 
 static int resident_step(sb_trainer_t* t, int64_t row_offset, int32_t rows, int kind) {
   SB_CHECK(t, SB_ERR_INVALID, "null trainer");
-  SB_CHECK(t->ds_rows > 0, SB_ERR_STATE, "no resident dataset loaded");
-  SB_CHECK(row_offset >= 0 && rows > 0 && row_offset + rows <= t->resident_len(), SB_ERR_INVALID,
-           "rows [%lld, %lld) outside the resident set of %lld %s", (long long)row_offset, (long long)(row_offset + rows),
-           (long long)t->resident_len(), t->ord_n > 0 ? "rows of the row order" : "rows");
-  if (t->ord_n > 0) return run_step(t, nullptr, t->ordY, t->ordW, rows, kind, row_offset);
-  return run_step(t, t->dsX ? t->dsX + row_offset * t->net.F : nullptr, t->dsY + row_offset, t->dsW + row_offset, rows, kind,
-                  row_offset);
-}
-
-// RUN_S consecutive steps as ONE graph over descriptor set `set` (ordered: through the row order)
-static int get_run_graph(sb_trainer* t, int rows, int set, bool ordered, cudaGraphExec_t* out) {
-  const int key = (rows * 2 + set) * 2 + (ordered ? 1 : 0);
-  auto it = t->run_graphs.find(key);
-  if (it != t->run_graphs.end()) { *out = it->second; return SB_OK; }
-  Net& n = t->net;
-  cudaGraph_t g = nullptr;
-  SB_CUDA(cudaStreamBeginCapture(n.stream, cudaStreamCaptureModeThreadLocal));
-  int s = SB_OK;
-  for (int k = 0; k < sb_trainer::RUN_S && s == SB_OK; ++k) {
-    const StepIn in{t->run_descs[set][k], t->run_scals[set][k], !ordered, false, ordered};
-    // (SB_STEP_TRACE: an interior step is the one traced - it starts behind the previous step's tail, as most steps of a
-    // run do)
-    n.trace_on = (k == 1);
-    s = enqueue_step_body(t, in, rows, G_STEP);
-  }
-  n.trace_on = true;
-  cudaError_t e = cudaStreamEndCapture(n.stream, &g);
-  if (s != SB_OK) { if (g) cudaGraphDestroy(g); return s; }
-  SB_CHECK(e == cudaSuccess, SB_ERR_CUDA, "cudaStreamEndCapture failed: %s", cudaGetErrorString(e));
-  cudaGraphExec_t ge = nullptr;
-  SB_CUDA(cudaGraphInstantiate(&ge, g, 0));
-  cudaGraphDestroy(g);
-  t->run_graphs[key] = ge;
-  *out = ge;
-  return SB_OK;
+  Batch b;
+  SB_TRY(resident_batch(t, row_offset, rows, -1, &b));
+  return run_step(t, b, kind);
 }
 
 int sb_trainer_run_resident(sb_trainer_t* t, const int64_t* row_offsets, int32_t n_steps, int32_t rows) {
@@ -1311,57 +1375,27 @@ int sb_trainer_run_resident(sb_trainer_t* t, const int64_t* row_offsets, int32_t
   SB_CHECK(t->ds_rows > 0, SB_ERR_STATE, "no resident dataset loaded");
   Net& n = t->net;
   SB_CHECK(rows > 0 && rows <= n.max_batch, SB_ERR_INVALID, "rows=%d outside (0, max_batch=%d]", rows, n.max_batch);
-  const long long len = t->resident_len();
-  for (int i = 0; i < n_steps; ++i)
-    SB_CHECK(row_offsets[i] >= 0 && row_offsets[i] + rows <= len, SB_ERR_INVALID,
-             "step %d: rows [%lld, %lld) outside the resident set of %lld %s", i, (long long)row_offsets[i],
-             (long long)(row_offsets[i] + rows), len, t->ord_n > 0 ? "rows of the row order" : "rows");
+  Batch b;
+  for (int i = 0; i < n_steps; ++i) SB_TRY(resident_batch(t, row_offsets[i], rows, i, &b));
   constexpr int S = sb_trainer::RUN_S;
   int i = 0;
   SB_TRY(check_det_exchange(t));
-  const bool ordered = t->ord_n > 0;
-  if ((t->dsXb != nullptr || ordered) && t->prep != nullptr) {
+  const Feed feed = t->resident_feed();
+  if (feed != Feed::HOST) {      // (the fp32 set without an order runs one host-batch graph per step, not prefetched)
     SB_CUDA(cudaSetDevice(n.device));
-    if (!t->run_ready) {
-      for (int set = 0; set < 2; ++set) {
-        for (int k = 0; k < S; ++k) {
-          if (!t->run_descs[set][k]) SB_TRY(n.dalloc(&t->run_descs[set][k], 1));
-          if (!t->run_scals[set][k]) SB_TRY(n.dalloc(&t->run_scals[set][k], SCAL_COUNT));
-        }
-        SB_TRY(create_event(&t->ev_run_prep[set]));
-        SB_TRY(create_event(&t->ev_run_done[set]));
-      }
-      SB_CUDA(cudaStreamSynchronize(n.stream));   // the zero-fill of the new descriptors ran on the main stream
-      t->run_ready = true;
-    }
     const float gscale = 1.f / static_cast<float>(t->world);
     for (; i + S <= n_steps; i += S) {
-      const int set = static_cast<int>(t->run_chunks & 1);
+      const int set = static_cast<int>(t->prefetches & 1);
       cudaGraphExec_t ge = nullptr;
-      SB_TRY(get_run_graph(t, rows, set, ordered, &ge));
-      // this set was last read by the chunk two launches back
-      if (t->run_used[set]) SB_CUDA(cudaStreamWaitEvent(t->prep, t->ev_run_done[set], 0));
+      SB_TRY(get_graph(t, GraphKey{rows, G_STEP, feed, S, set}, &ge));
+      SB_TRY(prefetch_begin(t, set));
       for (int k = 0; k < S; ++k) {
-        const long long off = row_offsets[i + k];
-        ++t->global_step;
-        ++t->epoch;
-        if (ordered)
-          set_batch_kernel<<<1, 1, 0, t->prep>>>(t->run_descs[set][k], nullptr, t->ordY, t->ordW, lr_for_step(t, t->global_step),
-                                                 gscale, t->epoch, 0, nullptr, rows, t->run_scals[set][k],
-                                                 t->hist_slot(t->global_step), t->ord + off);
-        else
-          set_batch_kernel<<<1, 1, 0, t->prep>>>(t->run_descs[set][k], nullptr, t->dsY + off, t->dsW + off,
-                                                 lr_for_step(t, t->global_step), gscale, t->epoch, static_cast<int>(off), t->dsP,
-                                                 rows, t->run_scals[set][k], t->hist_slot(t->global_step));
+        SB_TRY(resident_batch(t, row_offsets[i + k], rows, i + k, &b));
+        const float lr_t = begin_update(t);
+        SB_TRY(write_desc(t->prep, t->slot(set, k), &b, lr_t, gscale, t->epoch, t->hist_slot(t->global_step)));
       }
-      SB_CUDA(cudaGetLastError());
-      SB_CUDA(cudaEventRecord(t->ev_run_prep[set], t->prep));
-      SB_CUDA(cudaStreamWaitEvent(n.stream, t->ev_run_prep[set], 0));
+      SB_TRY(prefetch_end(t, set));
       SB_CUDA(cudaGraphLaunch(ge, n.stream));
-      SB_CUDA(cudaEventRecord(t->ev_run_done[set], n.stream));
-      t->run_used[set] = true;
-      ++t->run_chunks;
-      t->have_pos = false;          // the single-step descriptor prefetch re-joins the main stream
       t->grad_out_scale = gscale;
     }
   }
@@ -1382,30 +1416,13 @@ int sb_trainer_accumulate_resident(sb_trainer_t* t, int64_t row_offset, int32_t 
 }
 int sb_trainer_loss_resident(sb_trainer_t* t, int64_t row_offset, int32_t rows, float* loss_out) {
   SB_CHECK(t && loss_out, SB_ERR_INVALID, "null argument");
-  SB_CHECK(t->ds_rows > 0, SB_ERR_STATE, "no resident dataset loaded");
+  Batch b;
+  SB_TRY(resident_batch(t, row_offset, rows, -1, &b));
   Net& n = t->net;
-  SB_CHECK(row_offset >= 0 && rows > 0 && rows <= n.max_batch && row_offset + rows <= t->resident_len(), SB_ERR_INVALID,
-           "rows [%lld, %lld) outside the resident set of %lld %s", (long long)row_offset, (long long)(row_offset + rows),
-           (long long)t->resident_len(), t->ord_n > 0 ? "rows of the row order" : "rows");
   SB_CUDA(cudaSetDevice(n.device));
   t->have_pos = false;
-  const bool ordered = t->ord_n > 0;
-  const bool resident = t->dsXb != nullptr && !ordered;
-  const StepIn in{t->descs[0], t->scals[0], resident, false, ordered};      // (see forward_chunks)
-  if (ordered)
-    set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, nullptr, t->ordY, t->ordW, 0.f, 1.f, t->epoch, 0, nullptr, rows, in.scal,
-                                             nullptr, t->ord + row_offset);
-  else if (resident)
-    set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, nullptr, t->dsY + row_offset, t->dsW + row_offset, 0.f, 1.f, t->epoch,
-                                             static_cast<int>(row_offset), t->dsP, rows, in.scal);
-  else
-    set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, t->dsX + row_offset * n.F, t->dsY + row_offset, t->dsW + row_offset, 0.f, 1.f,
-                                             t->epoch);
-  SB_CUDA(cudaGetLastError());
-  if (ordered) SB_TRY(enqueue_gather(t, in, rows, nullptr, 0));
-  else if (!resident) SB_TRY(n.enqueue_load(in, rows));
-  SB_TRY(n.enqueue_hidden_forward(in, rows));
-  SB_TRY(n.enqueue_out(in, rows, true, false, nullptr, nullptr));
+  const StepIn in = t->slot(0, 0);      // (see forward_chunks)
+  SB_TRY(enqueue_forward(n, t, in, b, t->epoch, true, nullptr));
   float h[SCAL_COUNT];
   SB_CUDA(cudaMemcpyAsync(h, in.scal, sizeof(h), cudaMemcpyDeviceToHost, n.stream));
   SB_CUDA(cudaStreamSynchronize(n.stream));
@@ -1468,10 +1485,9 @@ void* sb_trainer_stream(sb_trainer_t* t) { return t ? reinterpret_cast<void*>(t-
 int sb_trainer_kernels_per_step(sb_trainer_t* t, int32_t rows) {
   SB_CHECK(t, SB_ERR_INVALID, "null trainer");
   cudaGraphExec_t ge;
-  const bool ordered = t->ord_n > 0;   // the path resident steps take now
-  const StepIn in{t->descs[0], t->scals[0], t->dsXb != nullptr && !ordered, false, ordered};
-  SB_TRY(get_graph(t, in, rows, G_STEP, 0, &ge));
-  return t->kernels_per_step[rows * 2 + (ordered ? 1 : 0)];
+  const Feed feed = t->resident_feed();   // the path resident steps take now (no set loaded: host-batch steps)
+  SB_TRY(get_graph(t, GraphKey{rows, G_STEP, feed, 1, 0}, &ge));
+  return t->kernels_per_step[{rows, feed}];
 }
 
 int sb_trainer_set_row_order(sb_trainer_t* t, const int64_t* rows, int64_t n) {
@@ -1505,39 +1521,25 @@ int sb_trainer_set_row_order(sb_trainer_t* t, const int64_t* rows, int64_t n) {
   return SB_OK;
 }
 
-// forward (+ optional loss) over any number of host rows, in max_batch chunks
-// (a trainer's pair 0: these host-driven paths are not captured.  A step queues its descriptor writes ahead of its graph
-// on the main stream, and every forward path synchronises that stream before it returns, so no step's descriptor prefetch
-// overlaps them.)
-static int forward_chunks(Net& n, const float* X, const float* y, const float* w, int64_t rows, bool do_loss,
-                          float* out, double* loss_sum, double* nnz) {
-  SB_CUDA(cudaSetDevice(n.device));
-  const StepIn in{n.desc, n.scal};
-  float h[SCAL_COUNT];
-  for (int64_t r0 = 0; r0 < rows; r0 += n.max_batch) {
-    const int c = static_cast<int>(rows - r0 < n.max_batch ? rows - r0 : n.max_batch);
+// forward (+ loss: y != nullptr) over any number of host or device rows; out / loss accumulators nullable
+static int forward_rows(Net& n, const float* X, const float* y, const float* w, int64_t rows, float* out, double* loss_sum,
+                        double* nnz) {
+  return forward_chunks(n, rows, [&](int64_t r0, int c, Batch* b) -> int {
     SB_CUDA(cudaMemcpyAsync(n.stX, X + r0 * n.F, sizeof(float) * c * static_cast<size_t>(n.F), cudaMemcpyDefault, n.stream));
-    if (do_loss) {
+    if (y) {
       SB_CUDA(cudaMemcpyAsync(n.stY, y + r0, sizeof(float) * c, cudaMemcpyDefault, n.stream));
       if (w) SB_CUDA(cudaMemcpyAsync(n.stW, w + r0, sizeof(float) * c, cudaMemcpyDefault, n.stream));
     }
-    set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, n.stX, n.stY, (do_loss && w) ? n.stW : n.ones, 0.f, 1.f);
-    SB_TRY(n.enqueue_load(in, c));
-    SB_TRY(n.enqueue_hidden_forward(in, c));
-    SB_TRY(n.enqueue_out(in, c, do_loss, false, n.yhat, nullptr));
-    if (out) SB_CUDA(cudaMemcpyAsync(out + r0, n.yhat, sizeof(float) * c, cudaMemcpyDefault, n.stream));
-    if (do_loss) SB_CUDA(cudaMemcpyAsync(h, in.scal, sizeof(h), cudaMemcpyDeviceToHost, n.stream));
-    SB_CUDA(cudaStreamSynchronize(n.stream));
-    if (do_loss) { *loss_sum += h[SCAL_LOSS_SUM]; *nnz += h[SCAL_NNZ]; }
-  }
-  return SB_OK;
+    *b = host_batch(n, n.stX, n.stY, (y && w) ? n.stW : nullptr, c);
+    return SB_OK;
+  }, out, loss_sum, nnz);
 }
 
 int sb_trainer_eval_loss(sb_trainer_t* t, const float* X, const float* y, const float* w, int64_t rows, float* loss_out) {
   SB_CHECK(t && X && y && loss_out, SB_ERR_INVALID, "null argument");
   SB_CHECK(rows > 0, SB_ERR_INVALID, "rows must be > 0");
   double ls = 0, nz = 0;
-  SB_TRY(forward_chunks(t->net, X, y, w, rows, true, nullptr, &ls, &nz));
+  SB_TRY(forward_rows(t->net, X, y, w, rows, nullptr, &ls, &nz));
   *loss_out = nz > 0 ? static_cast<float>(ls / nz) : 0.f;
   return SB_OK;
 }
@@ -1545,8 +1547,7 @@ int sb_trainer_eval_loss(sb_trainer_t* t, const float* X, const float* y, const 
 int sb_trainer_predict(sb_trainer_t* t, const float* X, int64_t rows, float* out) {
   SB_CHECK(t && X && out, SB_ERR_INVALID, "null argument");
   SB_CHECK(rows > 0, SB_ERR_INVALID, "rows must be > 0");
-  double ls = 0, nz = 0;
-  return forward_chunks(t->net, X, nullptr, nullptr, rows, false, out, &ls, &nz);
+  return forward_rows(t->net, X, nullptr, nullptr, rows, out, nullptr, nullptr);
 }
 
 // ---- checkpoint: flat blob {magic, version, n_params, global_step, optimizer, theta, s1, s2} ----
@@ -1706,11 +1707,7 @@ static int model_forward(sb_model* m, const float* dX, int rows, float* dOut) {
     ++m->st[SB_DEBUG_MSTAT_SMALL_LAUNCHES];
     return SB_OK;
   }
-  const StepIn in{n.desc, n.scal};
-  set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, dX, nullptr, n.ones, 0.f, 1.f);
-  SB_TRY(n.enqueue_load(in, rows));
-  SB_TRY(n.enqueue_hidden_forward(in, rows));
-  return n.enqueue_out(in, rows, false, false, dOut, nullptr);
+  return enqueue_forward(n, nullptr, StepIn{n.desc, n.scal}, host_batch(n, dX, nullptr, nullptr, rows), 0, false, dOut);
 }
 
 // tensor-core modes: model_forward of MB_ROWS rows of the staging area, captured once, so a micro-batch is one launch
@@ -1981,13 +1978,10 @@ int sb_debug_exchange(sb_trainer_t* t, int32_t slot_mask, float gscale, int32_t 
   SB_CUDA(cudaSetDevice(n.device));
   // as a step: the descriptor of this update (step count, lr_t, gradient scale, epoch), then the exchange on the main stream.
   // Nothing here waits for the device - the peers' launches are still to be queued by the same host thread.
-  ++t->global_step;
-  const float lr_t = lr_for_step(t, t->global_step);
+  const float lr_t = begin_update(t);
   const float gs = gscale > 0.f ? gscale : 1.f / static_cast<float>(t->world);
-  ++t->epoch;
-  const StepIn in{t->descs[t->last_pair], t->scals[t->last_pair]};
-  set_batch_kernel<<<1, 1, 0, n.stream>>>(in.desc, nullptr, nullptr, nullptr, lr_t, gs, t->epoch);
-  SB_CUDA(cudaGetLastError());
+  const StepIn in = t->slot(t->last_set, 0);    // (as apply_accumulated)
+  SB_TRY(write_desc(n.stream, in, nullptr, lr_t, gs, t->epoch, nullptr));
   if (grid <= 0) grid = xchg_grid(t, slot_mask, alone != 0);
   n.last_kernel = nullptr;
   SB_TRY(enqueue_xchg(t, in, slot_mask, n.stream, false, false, alone != 0, grid));

@@ -375,8 +375,8 @@ int Net::refresh_shadows() {
 }
 
 int Net::enqueue_load(const StepIn& in, int rows, float* clear, long long clear_n) {
-  const int Fx = in.sparse ? n_dense : F;        // a sparse step stages only the dense block
-  const int ldx = in.sparse ? ldD : ldF;
+  const int Fx = in.feed == Feed::SPARSE ? n_dense : F;        // a sparse step stages only the dense block
+  const int ldx = in.feed == Feed::SPARSE ? ldD : ldF;
   const long long units = static_cast<long long>(rows) * (ldx / 8);
   long long blocks = (units + 255) / 256;
   const long long cap = static_cast<long long>(num_sms) * 16;
@@ -392,7 +392,7 @@ int Net::enqueue_load(const StepIn& in, int rows, float* clear, long long clear_
                          static_cast<const BatchDesc*>(in.desc), rows, Fx, static_cast<__nv_bfloat16*>(nullptr), ldx, Xf, in.scal,
                          clear, clear_n, 1, 0ll));
   mark("load_batch");
-  if (in.sparse) SB_TRY(enqueue_embed(rows, false, nullptr, stream));
+  if (in.feed == Feed::SPARSE) SB_TRY(enqueue_embed(rows, false, nullptr, stream));
   return SB_OK;
 }
 
@@ -400,13 +400,13 @@ int Net::enqueue_hidden_forward(const StepIn& in, int rows, float* grad, bool* f
   if (fused_out) *fused_out = false;
   for (int l = 0; l < L; ++l) {
     Layer& ly = layers[l];
-    const bool sp0 = (l == 0) && in.sparse;       // wide+deep: contract the dense columns only, add the embedding sums
+    const bool sp0 = (l == 0) && in.feed == Feed::SPARSE;       // wide+deep: contract the dense columns only, add the embedding sums
     const int k_in = sp0 ? n_dense : ly.in;
     const int ld_k = sp0 ? ldD : ly.ld_in;
     if (tc()) {
       // Z = A_{l-1}[rows,in] (K-major) x W_l[in,out] (MN-major B operand: n contiguous)
       TmapSet tm;
-      const bool res0 = (l == 0) && in.resident;
+      const bool res0 = (l == 0) && in.feed == Feed::RESIDENT;
       const __nv_bfloat16* src = (l == 0) ? (res0 ? resident_Xb : Xb) : A[l - 1];
       const long long src_ps = (l == 0) ? (res0 ? resident_ps : Xb_ps) : A_ps[l - 1];
       const int src_rows = res0 ? static_cast<int>(resident_rows) : rows;
@@ -524,7 +524,7 @@ int Net::enqueue_out(const StepIn& in, int rows, bool do_loss, bool do_bwd, floa
 
 int Net::enqueue_dw(const StepIn& in, int l, int rows, float* grad, cudaStream_t st, bool pdl, int sms, int r0, int r1, int chunk) {
   Layer& ly = layers[l];
-  const bool sp0 = (l == 0) && in.sparse;         // wide+deep: dW of the dense rows by GEMM, of the embedding rows by scatter-add
+  const bool sp0 = (l == 0) && in.feed == Feed::SPARSE;         // wide+deep: dW of the dense rows by GEMM, of the embedding rows by scatter-add
   const int in_rows = sp0 ? n_dense : ly.in;
   if (r1 < 0) r1 = in_rows;
   if (sp0) SB_TRY(enqueue_embed(rows, true, grad, st));
@@ -544,7 +544,7 @@ int Net::enqueue_dw(const StepIn& in, int l, int rows, float* grad, cudaStream_t
     return SB_OK;
   }
   // dW_l[in,out] += sum_rows A_{l-1}[rows,in] (MN-major A) * dZ_l[rows,out] (MN-major B), split-K over rows
-  const bool res0 = (l == 0) && in.resident;
+  const bool res0 = (l == 0) && in.feed == Feed::RESIDENT;
   const int ld_k = sp0 ? ldD : ly.ld_in;
   const __nv_bfloat16* ap = (l == 0) ? (res0 ? resident_Xb : Xb) : A[l - 1];
   const long long ap_ps = (l == 0) ? (res0 ? resident_ps : Xb_ps) : A_ps[l - 1];
@@ -946,7 +946,7 @@ int sb_debug_gemm_layer(int32_t kind, int32_t precision, const float* A, const f
   SB_CUDA(cudaDeviceSynchronize());     // the uploads above ran on the legacy stream, the net launches on its own
 
   StepIn in;
-  in.desc = net.desc; in.scal = net.scal; in.resident = resident; in.sparse = addend != nullptr;
+  in.desc = net.desc; in.scal = net.scal; in.feed = resident ? Feed::RESIDENT : addend ? Feed::SPARSE : Feed::HOST;
   SB_TRY(net.refresh_shadows());
   net.launches = 0;
   if (kind == FWD) SB_TRY(net.enqueue_hidden_forward(in, M, nullptr, nullptr, reinterpret_cast<float4*>(clr.p), clear_n4));

@@ -19,14 +19,19 @@ struct Layer {
   int ld_in = 0, ld_out = 0;
 };
 
-// What one step's launches read: its descriptor / scalar pair, whether layer 0 reads the HBM-resident set, whether the
-// step is a sparse (wide+deep) one.  The trainer alternates descriptor pairs between captured steps.
+// Where layer 0 of a step gets its batch:
+//   HOST      fp32 rows at desc->X (the staging area, or the fp32 resident set): load_batch_kernel fills Xb / Xf
+//   SPARSE    wide+deep: dense block + index matrix, hidden layer 0's one-hot block via the embedding
+//   RESIDENT  layer 0's GEMMs read their A operand by TMA from resident_Xb at row offset desc->row0
+//   ORDERED   resident rows through the row order: gather_batch_kernel fills Xb / Xf, layer 0 reads them
+enum class Feed { HOST, SPARSE, RESIDENT, ORDERED };
+
+// What one step's launches read: its descriptor / scalar slot and its feed.  The trainer takes the slots of its captured
+// steps from a ring of descriptor sets (capi.cu).
 struct StepIn {
   BatchDesc* desc = nullptr;
   float* scal = nullptr;
-  bool resident = false;   // layer 0's GEMMs read their A operand by TMA from resident_Xb at row offset desc->row0
-  bool sparse = false;     // wide+deep step: dense block + index matrix, hidden layer 0's one-hot block via the embedding
-  bool ordered = false;    // resident step through the row order: gather_batch_kernel fills Xb / Xf, layer 0 reads them
+  Feed feed = Feed::HOST;
 };
 
 inline int pairs_of(int np) { return np == 3 ? 6 : (np == 2 ? 3 : 1); }
@@ -64,7 +69,7 @@ struct Net {
   float* Xf = nullptr;
   std::vector<float*> Af, dZf;
   float *yhat = nullptr, *ones = nullptr;
-  BatchDesc* desc = nullptr;               // the net's own descriptor / scalar pair (the trainer's pair 0)
+  BatchDesc* desc = nullptr;               // the net's own descriptor / scalar slot (set 0, slot 0 of a trainer's ring)
   float* scal = nullptr;
   float *stX = nullptr, *stY = nullptr, *stW = nullptr;  // H2D staging (device)
   OptWork* work = nullptr;
@@ -123,7 +128,7 @@ struct Net {
   float* E = nullptr;                        // [max_batch, ld_out_0] embedding sums
   int set_sparse(int n_dense_, int n_onehot_, int n_cat_);
   int enqueue_embed(int rows, bool scatter, float* grad, cudaStream_t st);
-  // bf16 HBM-resident training set (trainer), read by steps with StepIn::resident
+  // bf16 HBM-resident training set (trainer), read by steps with Feed::RESIDENT
   const __nv_bfloat16* resident_Xb = nullptr;
   long long resident_rows = 0;
   int enqueue_out(const StepIn& in, int rows, bool do_loss, bool do_bwd, float* yhat_dst, float* grad);
