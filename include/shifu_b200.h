@@ -406,6 +406,46 @@ int sb_debug_gemm_fwd_out(const float* A, const float* W, const float* bias, con
                           int32_t M, int32_t N, int32_t K, int32_t a_rows, int32_t row0, int32_t act, int32_t loss,
                           int32_t np, int32_t grid, int device);
 
+/* The output layer of a step at `precision` (sb_precision) on its own (out_layer_rows_kernel / out_layer_kernel), launched
+ * by the step's own launch code on a network whose last hidden layer (width H, activation act) holds A_L:
+ *   z = A_L . wo + bo,  y_hat = sigmoid(z),  loss term and dz (SUM_BY_NONZERO_WEIGHTS, n_nz = the count of non-zero w),
+ *   dZ = dz * wo * act'(A_L),  db_L += sum_r dZ,  dw_o += sum_r dz A_L,  db_o += sum_r dz,  loss_sum += sum_r loss term.
+ * A [M, H] fp32 host, stored as the step stores A_L: np bf16 parts split as the step splits them (np = 1 BF16, 2 BF16X2,
+ * 3 FP32_TC) or fp32.  wo [H]; y, w [M] (do_loss = 1).  (do_loss, do_bwd) = (1, 1): a training step; (1, 0): an
+ * evaluation (y_hat and the loss); (0, 0): a score (y_hat only; y and w may be null).  yhat [M] (nullable unless
+ * do_loss = 0) receives y_hat; dZ [np, M, H] each part's bf16 widened to fp32 (FP32: one part); g_bL [H], g_wo [H], g_bo
+ * and loss_sum are in/out: the kernel adds into the values passed in.  det = 1: the deterministic instantiation,
+ * launched twice on the same network from the same initial values; the results are the second launch's and
+ * *repeat_same (nullable) is 1 if every output bit, guards included, equals the first launch's (-1 for det = 0).
+ * sms: the SM count the launch code plans for (0 = every SM).  route (nullable, route_cap bytes) receives the kernel
+ * instantiation launched, e.g. "out_layer_rows<2,DET>", "out_layer<bf16>", "out_layer<float>".
+ * Before the launch, A_L's pad columns and the 64 rows past M of every part hold NaN, and so do y and w past M (all of
+ * them for a score) and n_nz for a score.  The 64 rows past M of dZ and y_hat, dZ's pad columns, the flat gradient
+ * outside the g_bL / g_wo / g_bo slots (all of it unless do_bwd) and 256 floats behind it, and the step-scalar words
+ * other than the loss sum (and that one too unless do_loss) are filled with a sentinel or the input value; *guard returns
+ * how many of them changed, except that a pad column of a batch row may hold +-0 on a backward (the 16-byte pieces of
+ * dZ reach into it).  On a score or an evaluation dZ must stay the sentinel too.  Every argument is checked before any
+ * device work (do_bwd needs do_loss; M, H >= 1; sms up to the device's SM count); a bad one is SB_ERR_INVALID. */
+int sb_debug_out_layer(int32_t precision, int32_t det, int32_t do_loss, int32_t do_bwd, const float* A, const float* wo, float bo,
+                       const float* y, const float* w, float* yhat, float* dZ, float* g_bL, float* g_wo, float* g_bo,
+                       float* loss_sum, int32_t* guard, int32_t* repeat_same, char* route, int32_t route_cap, int32_t M, int32_t H,
+                       int32_t act, int32_t loss, int32_t sms, int device);
+
+/* The wide+deep first layer's embedding kernels (embed_gather_kernel, embed_scatter_kernel), launched by the step's own
+ * launch code on a network with 3 dense columns and n_onehot one-hot columns of n_cat categorical columns, hidden [H].
+ * W_e [n_onehot, H] fp32 is put into the parameters and stored as the step stores it (np bf16 shadow parts, or fp32);
+ * idx [rows, n_cat] holds one-hot columns in [0, n_onehot) or -1 (missing), checked as the sparse entry points check it.
+ *   scatter = 0: out [rows, H] = E, E[r] = sum over c with idx[r, c] >= 0 of W_e[idx[r, c]] (every part).
+ *   scatter = 1: out [n_onehot, H] is in/out, W_e's rows of the flat gradient: row j gains the sum over every (r, c) with
+ *                idx[r, c] = j of dZ_0[r], where dZ [rows, H] fp32 is stored as the step stores dZ_0 (np parts or fp32).
+ *                We may be null.
+ * W_e's dense neighbours, b_0 and the output layer hold NaN, and so do dZ_0's pad columns and 64 rows past the batch.
+ * Before the launch E's pad columns and its 64 rows past the batch (gather), or the flat gradient outside W_e's rows and
+ * 256 floats behind it (scatter-add), are filled with a sentinel; *guard returns how many of them changed.  Every argument
+ * is checked before any device work; a bad one is SB_ERR_INVALID. */
+int sb_debug_embed(int32_t precision, int32_t scatter, const float* We, const int32_t* idx, const float* dZ, float* out,
+                   int32_t* guard, int32_t rows, int32_t H, int32_t n_onehot, int32_t n_cat, int device);
+
 /* ---- test hooks of the peer-memory gradient exchange (csrc/xchg_p2p.cuh), on a trainer with a peer table ---- */
 /* Read (write = 0) or write (1) one raw buffer of this rank's parameter arena, after waiting for the trainer's stream:
  * which = SB_DEBUG_BUF_THETA / _S1 / _S2 / _GRAD: float[n_params] (no gather from the run owners: a non-owner's stale

@@ -174,6 +174,11 @@ PROTOTYPES = {
     "sb_debug_gemm_fwd_out": (C.c_int, [_f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p,
                                         _P(C.c_int32), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                         C.c_int32, C.c_int32, C.c_int32, C.c_int]),
+    "sb_debug_out_layer": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, _f32p, _f32p, C.c_float, _f32p, _f32p, _f32p,
+                                     _f32p, _f32p, _f32p, _f32p, _f32p, _P(C.c_int32), _P(C.c_int32), C.c_char_p, C.c_int32,
+                                     C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int]),
+    "sb_debug_embed": (C.c_int, [C.c_int32, C.c_int32, _f32p, _P(C.c_int32), _f32p, _f32p, _P(C.c_int32), C.c_int32, C.c_int32,
+                                 C.c_int32, C.c_int32, C.c_int]),
     "sb_debug_trainer_buffer": (C.c_int, [_vp, C.c_int32, _vp, C.c_int64, C.c_int32]),
     "sb_debug_exchange": (C.c_int, [_vp, C.c_int32, C.c_float, C.c_int32, C.c_int32, _f32p, _P(C.c_int32), C.c_char_p,
                                     C.c_int32]),
@@ -801,6 +806,51 @@ def debug_gemm_fwd_out(A: np.ndarray, W: np.ndarray, bias: np.ndarray, wo: np.nd
                                       _ptr(g_bL), _ptr(g_wo), C.byref(gbo), C.byref(ls), C.byref(guard), M, N, K, a_rows, row0,
                                       act, loss, np_parts, grid, device))
     return dZ, g_bL, g_wo, float(gbo.value), float(ls.value), int(guard.value)
+
+
+def debug_out_layer(precision: int, A: np.ndarray, wo: np.ndarray, bo: float, act: int, loss: int,
+                    y: Optional[np.ndarray] = None, w: Optional[np.ndarray] = None, do_loss: bool = True, do_bwd: bool = True,
+                    det: bool = False, g_bL: Optional[np.ndarray] = None, g_wo: Optional[np.ndarray] = None, g_bo: float = 0.0,
+                    loss_sum: float = 0.0, sms: int = 0, M: Optional[int] = None, H: Optional[int] = None, device: int = 0):
+    """The output layer of a step on its own (sb_debug_out_layer) through the step's launch code, on A_L = A [M, H]
+    (M, H default to A's shape), wo [H], y / w [M] (do_loss).  g_bL, g_wo [H], g_bo and loss_sum are the initial values the
+    kernel adds into (zeros by default).  -> dict with yhat [M], dZ [np, M, H] (fp32 of the stored parts), g_bL, g_wo,
+    g_bo, loss_sum, guard (changed sentinel elements), repeat_same (det: 1 if a second launch gave the same bits, else
+    -1) and route (the kernel instantiation)"""
+    A, wo = _f32(A), _f32(wo)
+    M = A.shape[0] if M is None else M
+    H = A.shape[1] if H is None else H
+    nparts = PARTS.get(precision, 1)
+    y = None if y is None else _f32(y).reshape(-1)
+    w = None if w is None else _f32(w).reshape(-1)
+    yhat = np.zeros(max(M, 0), np.float32)
+    dZ = np.zeros((nparts, max(M, 0), max(H, 0)), np.float32)
+    g_bL = _f32(g_bL).copy() if g_bL is not None else np.zeros(max(H, 0), np.float32)
+    g_wo = _f32(g_wo).copy() if g_wo is not None else np.zeros(max(H, 0), np.float32)
+    gbo, ls, guard, same = C.c_float(g_bo), C.c_float(loss_sum), C.c_int32(-1), C.c_int32(-1)
+    route = C.create_string_buffer(64)
+    check(lib().sb_debug_out_layer(precision, int(det), int(do_loss), int(do_bwd), _ptr(A), _ptr(wo), float(bo), _ptr(y), _ptr(w),
+                                   _ptr(yhat), _ptr(dZ), _ptr(g_bL), _ptr(g_wo), C.byref(gbo), C.byref(ls), C.byref(guard),
+                                   C.byref(same), route, 64, M, H, act, loss, sms, device))
+    return dict(yhat=yhat, dZ=dZ, g_bL=g_bL, g_wo=g_wo, g_bo=float(gbo.value), loss_sum=float(ls.value),
+                guard=int(guard.value), repeat_same=int(same.value), route=route.value.decode())
+
+
+def debug_embed(precision: int, idx: np.ndarray, n_onehot: int, H: int, We: Optional[np.ndarray] = None,
+                dZ: Optional[np.ndarray] = None, grad: Optional[np.ndarray] = None, device: int = 0):
+    """The wide+deep embedding kernels of a sparse step (sb_debug_embed) through the step's launch code, idx [rows, n_cat]:
+    dZ None: the gather of W_e [n_onehot, H] -> E [rows, H]; dZ [rows, H] given: the scatter-add into W_e's gradient
+    rows, grad [n_onehot, H] their initial value (zeros by default) -> the rows after it.  -> (result, guard count)"""
+    idx = np.ascontiguousarray(idx, dtype=np.int32)
+    rows, n_cat = idx.shape if idx.ndim == 2 else (0, 0)
+    scatter = dZ is not None
+    We = None if We is None else _f32(We)
+    dZ = None if dZ is None else _f32(dZ)
+    out = (np.zeros((n_onehot, H), np.float32) if grad is None else _f32(grad).copy()) if scatter else np.zeros((rows, H), np.float32)
+    guard = C.c_int32(-1)
+    check(lib().sb_debug_embed(precision, int(scatter), _ptr(We), idx.ctypes.data_as(_P(C.c_int32)), _ptr(dZ), _ptr(out),
+                               C.byref(guard), rows, H, n_onehot, n_cat, device))
+    return out, int(guard.value)
 
 
 def text_parse_device(text: bytes, col_map: Sequence[int], n_feat: int, delim: str = "|", device: int = 0, flag_cap: int = 65536):

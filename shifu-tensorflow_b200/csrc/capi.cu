@@ -1176,8 +1176,7 @@ static int stage_sparse_batch(Net& n, const float* Xd, const int32_t* idx, const
   SB_CHECK(n.n_cat > 0, SB_ERR_STATE, "sb_trainer_set_sparse has not been called");
   SB_CHECK(Xd && idx, SB_ERR_INVALID, "Xd and idx must not be null");
   SB_CHECK(rows > 0 && rows <= n.max_batch, SB_ERR_INVALID, "rows=%d outside (0, max_batch=%d]", rows, n.max_batch);
-  for (long long i = 0; i < static_cast<long long>(rows) * n.n_cat; ++i)
-    SB_CHECK(idx[i] < n.n_onehot, SB_ERR_INVALID, "idx[%lld] = %d outside [-1, n_onehot=%d)", i, idx[i], n.n_onehot);
+  SB_TRY(check_sparse_idx(idx, static_cast<long long>(rows) * n.n_cat, n.n_onehot));
   SB_CUDA(cudaSetDevice(n.device));
   SB_CUDA(cudaMemcpyAsync(n.stX, Xd, sizeof(float) * rows * static_cast<size_t>(n.n_dense), cudaMemcpyHostToDevice, n.stream));
   SB_CUDA(cudaMemcpyAsync(n.idx, idx, sizeof(int32_t) * rows * static_cast<size_t>(n.n_cat), cudaMemcpyHostToDevice, n.stream));

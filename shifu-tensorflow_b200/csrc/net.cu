@@ -1,10 +1,12 @@
 // Net: device state + kernel sequencing for the tabular-DNN forward / backward.
 // Mirrors generate_from_modelconf + model (res/ssgd_monitor.py:91-144) as a list of fused launches.
-// Also the kernel-level test hooks (sb_debug_gemm_*), so that every GEMM kernel is compiled in this one translation unit.
+// Also the kernel-level test hooks (sb_debug_gemm_*, sb_debug_out_layer, sb_debug_embed), so that every GEMM kernel is
+// compiled in this one translation unit.
 #include <stdarg.h>
 #include <stdlib.h>
 #include <string.h>
 #include <algorithm>
+#include <limits>
 #include "net.cuh"
 #include "gemm_dw.cuh"
 #include "gemm_fwd_out.cuh"
@@ -304,6 +306,12 @@ Net::~Net() {
   if (stream) cudaStreamDestroy(stream);
 }
 
+int check_sparse_idx(const int32_t* idx, long long n, int n_onehot) {
+  for (long long i = 0; i < n; ++i)
+    SB_CHECK(idx[i] >= -1 && idx[i] < n_onehot, SB_ERR_INVALID, "idx[%lld] = %d outside [-1, n_onehot=%d)", i, idx[i], n_onehot);
+  return SB_OK;
+}
+
 int Net::set_sparse(int n_dense_, int n_onehot_, int n_cat_) {
   SB_CHECK(n_dense_ >= 1 && n_onehot_ >= 1 && n_cat_ >= 1, SB_ERR_INVALID, "wide+deep needs >= 1 dense, one-hot and categorical column");
   SB_CHECK(n_dense_ + n_onehot_ == F, SB_ERR_INVALID, "n_dense (%d) + n_onehot (%d) must equal n_features (%d): the sparse path evaluates "
@@ -489,6 +497,7 @@ int Net::enqueue_out(const StepIn& in, int rows, bool do_loss, bool do_bwd, floa
   const bool d = det && (do_loss || do_bwd);   // the DET instantiations (slots + last-CTA sum) when anything is summed
   if (d) { p.det_ws = det_out_ws; p.det_ticket = det_tickets; }
   const int grid = (rows + 31) / 32;
+  const char* kernel;
   if (tc()) {
     p.A = A[L - 1]; p.ldA = hl.ld_out;
     p.np = nparts; p.a_ps = A_ps[L - 1]; p.dz_ps = A_ps[L - 1];
@@ -499,26 +508,33 @@ int Net::enqueue_out(const StepIn& in, int rows, bool do_loss, bool do_bwd, floa
       rpb = ((rpb + 7) / 8) * 8;
       if (rpb < 8) rpb = 8;
       const dim3 g((rows + rpb - 1) / rpb);
+      static const char* const names[2][3] = {{"out_layer_rows<1>", "out_layer_rows<2>", "out_layer_rows<4>"},
+                                              {"out_layer_rows<1,DET>", "out_layer_rows<2,DET>", "out_layer_rows<4,DET>"}};
+      const int nch = hl.out <= 256 ? 0 : (hl.out <= 512 ? 1 : 2);
+      kernel = names[d ? 1 : 0][nch];
       if (d) {
-        if (hl.out <= 256) SB_TRY(launch_kernel(out_layer_rows_kernel<1, true>, g, dim3(256), 0, stream, true, p, rpb));
-        else if (hl.out <= 512) SB_TRY(launch_kernel(out_layer_rows_kernel<2, true>, g, dim3(256), 0, stream, true, p, rpb));
+        if (nch == 0) SB_TRY(launch_kernel(out_layer_rows_kernel<1, true>, g, dim3(256), 0, stream, true, p, rpb));
+        else if (nch == 1) SB_TRY(launch_kernel(out_layer_rows_kernel<2, true>, g, dim3(256), 0, stream, true, p, rpb));
         else SB_TRY(launch_kernel(out_layer_rows_kernel<4, true>, g, dim3(256), 0, stream, true, p, rpb));
-      } else if (hl.out <= 256) SB_TRY(launch_kernel(out_layer_rows_kernel<1>, g, dim3(256), 0, stream, true, p, rpb));
-      else if (hl.out <= 512) SB_TRY(launch_kernel(out_layer_rows_kernel<2>, g, dim3(256), 0, stream, true, p, rpb));
+      } else if (nch == 0) SB_TRY(launch_kernel(out_layer_rows_kernel<1>, g, dim3(256), 0, stream, true, p, rpb));
+      else if (nch == 1) SB_TRY(launch_kernel(out_layer_rows_kernel<2>, g, dim3(256), 0, stream, true, p, rpb));
       else SB_TRY(launch_kernel(out_layer_rows_kernel<4>, g, dim3(256), 0, stream, true, p, rpb));
     } else if (d) {
       SB_TRY(launch_kernel(out_layer_kernel<__nv_bfloat16, true>, dim3(grid), dim3(256), 0, stream, true, p));
+      kernel = "out_layer<bf16,DET>";
     } else {
       SB_TRY(launch_kernel(out_layer_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, stream, true, p));
+      kernel = "out_layer<bf16>";
     }
   } else {
     p.A = Af[L - 1]; p.ldA = hl.out;
     if (do_bwd) { p.dZ = dZf[L - 1]; p.ld_dZ = hl.out; }
     if (d) SB_TRY(launch_kernel(out_layer_kernel<float, true>, dim3(grid), dim3(256), 0, stream, true, p));
     else SB_TRY(launch_kernel(out_layer_kernel<float>, dim3(grid), dim3(256), 0, stream, true, p));
+    kernel = d ? "out_layer<float,DET>" : "out_layer<float>";
   }
   SB_CUDA(cudaGetLastError());
-  mark("out_layer");
+  mark(kernel);
   return SB_OK;
 }
 
@@ -1143,6 +1159,264 @@ int sb_debug_gemm_fwd_out(const float* A, const float* W, const float* bias, con
   std::copy(h_vec.begin() + 3 * N, h_vec.begin() + 4 * N, g_wo);
   *g_bo = h_vec[4 * N + 1];
   *loss_sum = h_vec[4 * N + 2 + SCAL_LOSS_SUM];
+  return SB_OK;
+}
+
+// The output layer of a step launched by Net::enqueue_out on a Net whose last hidden layer holds A_L (see shifu_b200.h)
+int sb_debug_out_layer(int32_t precision, int32_t det, int32_t do_loss, int32_t do_bwd, const float* A, const float* wo, float bo,
+                       const float* y, const float* w, float* yhat, float* dZ, float* g_bL, float* g_wo, float* g_bo,
+                       float* loss_sum, int32_t* guard, int32_t* repeat_same, char* route, int32_t route_cap, int32_t M, int32_t H,
+                       int32_t act, int32_t loss, int32_t sms, int device) {
+  SB_CHECK(precision >= SB_PREC_FP32 && precision <= SB_PREC_BF16X2, SB_ERR_INVALID, "precision=%d invalid", precision);
+  SB_CHECK((det == 0 || det == 1) && (do_loss == 0 || do_loss == 1) && (do_bwd == 0 || do_bwd == 1), SB_ERR_INVALID,
+           "det=%d do_loss=%d do_bwd=%d (each 0 or 1)", det, do_loss, do_bwd);
+  SB_CHECK(do_loss || !do_bwd, SB_ERR_INVALID, "do_bwd needs do_loss: the backward starts from the loss gradient");
+  SB_CHECK(M >= 1 && M <= (1 << 30) && H >= 1 && H <= (1 << 20), SB_ERR_INVALID, "M=%d H=%d", M, H);
+  SB_CHECK(act >= SB_ACT_NONE && act <= SB_ACT_LEAKYRELU, SB_ERR_INVALID, "act=%d invalid", act);
+  SB_CHECK(loss == SB_LOSS_MSE || loss == SB_LOSS_SIGMOID_CE, SB_ERR_INVALID, "loss=%d invalid", loss);
+  SB_CHECK(A && wo && guard && (route == nullptr || route_cap > 0), SB_ERR_INVALID, "null argument");
+  SB_CHECK(!do_loss || (y && w && loss_sum), SB_ERR_INVALID, "the loss needs y, w and loss_sum");
+  SB_CHECK(!do_bwd || (dZ && g_bL && g_wo && g_bo), SB_ERR_INVALID, "the backward needs dZ, g_bL, g_wo and g_bo");
+  SB_CHECK(do_loss || yhat, SB_ERR_INVALID, "a score (do_loss = 0) needs yhat");
+  SB_CHECK(sms >= 0, SB_ERR_INVALID, "sms=%d", sms);
+  int dev_sms = 0;
+  SB_TRY(check_device(device, &dev_sms));
+  SB_CHECK(sms <= dev_sms, SB_ERR_INVALID, "sms=%d above the %d SMs", sms, dev_sms);
+
+  // the net: F = 8, hidden [H] with A_L = A_0; 64 rows past the batch in every activation part are guard rows
+  sb_net_desc d = {};
+  d.n_features = 8; d.n_hidden = 1;
+  d.hidden[0] = H; d.acts[0] = act;
+  d.loss = loss; d.optimizer = SB_OPT_SGD;
+  d.max_batch = M + 64;
+  d.precision = precision;
+  constexpr int GUARD = 256;                            // floats behind the gradient
+  const uint32_t S32 = 0x7f7f7f7fu;                     // sentinels: fp32 3.4e38, bf16 3.4e38
+  const uint16_t S16 = 0x7f7f;
+  const float qnan = std::numeric_limits<float>::quiet_NaN();
+  float s32;
+  memcpy(&s32, &S32, 4);
+  DevBuf<float> g, d_yh, d_yw;
+  Net net;                                              // (destroyed first: waits for its stream)
+  SB_TRY(net.init(&d, device, true));
+  if (det) SB_TRY(net.enable_det());
+  if (sms > 0) net.num_sms = sms;
+  const bool tc = net.tc();
+  const int np = net.nparts;
+  const Layer& hl = net.layers[0];
+  const Layer& ol = net.layers[1];
+  const int rows_all = M + 64, ld = tc ? hl.ld_out : H;
+  std::vector<float> theta(static_cast<size_t>(net.n_params), 0.f);
+  std::copy(wo, wo + H, theta.begin() + ol.w_off);
+  theta[static_cast<size_t>(ol.b_off)] = bo;
+  SB_CUDA(cudaMemcpy(net.theta, theta.data(), sizeof(float) * theta.size(), cudaMemcpyHostToDevice));
+  // A_L: every part's pad columns and the 64 rows past M hold NaN, which a result can only show if the kernel reads them
+  if (tc) {
+    SB_CUDA(cudaMemset(net.A[0], 0xff, sizeof(__nv_bfloat16) * static_cast<size_t>(net.A_ps[0]) * np));
+    SB_TRY(upload_parts(net.A[0], A, M, H, ld, np, net.A_ps[0]));
+  } else {
+    SB_CUDA(cudaMemset(net.Af[0], 0xff, sizeof(float) * static_cast<size_t>(rows_all) * H));
+    SB_CUDA(cudaMemcpy(net.Af[0], A, sizeof(float) * static_cast<size_t>(M) * H, cudaMemcpyHostToDevice));
+  }
+  // y / w: the caller's rows, NaN behind them; all NaN for a score, which must not read them
+  std::vector<float> hyw(2 * static_cast<size_t>(rows_all), qnan);
+  float nnz = 0.f;
+  if (do_loss) {
+    std::copy(y, y + M, hyw.begin());
+    std::copy(w, w + M, hyw.begin() + rows_all);
+    for (int r = 0; r < M; ++r) nnz += w[r] != 0.f ? 1.f : 0.f;
+  }
+  SB_TRY(d_yw.alloc(hyw.size()));
+  SB_CUDA(cudaMemcpy(d_yw.p, hyw.data(), sizeof(float) * hyw.size(), cudaMemcpyHostToDevice));
+  BatchDesc hd = {};
+  hd.y = d_yw.p; hd.w = d_yw.p + rows_all; hd.gscale = 1.f;
+  SB_CUDA(cudaMemcpy(net.desc, &hd, sizeof(hd), cudaMemcpyHostToDevice));
+  // the step scalars: the loss sum in/out and n_nz; the other words (and both, for a score) must keep what they hold
+  float hscal[SCAL_COUNT];
+  std::fill(hscal, hscal + SCAL_COUNT, s32);
+  hscal[SCAL_NNZ] = do_loss ? nnz : qnan;
+  if (do_loss) hscal[SCAL_LOSS_SUM] = *loss_sum;
+  // the flat gradient: the g_bL, g_wo, g_bo slots (contiguous: b_0, w_o, b_o) in/out on a backward, the rest and GUARD
+  // floats behind it the sentinel
+  const size_t g_n = static_cast<size_t>(net.n_params) + GUARD;
+  const size_t io0 = static_cast<size_t>(hl.b_off), io1 = static_cast<size_t>(ol.b_off) + 1;
+  std::vector<float> hg(g_n, s32);
+  if (do_bwd) {
+    std::copy(g_bL, g_bL + H, hg.begin() + hl.b_off);
+    std::copy(g_wo, g_wo + H, hg.begin() + ol.w_off);
+    hg[static_cast<size_t>(ol.b_off)] = *g_bo;
+  }
+  SB_TRY(g.alloc(g_n));
+  SB_TRY(d_yh.alloc(rows_all));
+  void* dz_dev = tc ? static_cast<void*>(net.dZ[0]) : static_cast<void*>(net.dZf[0]);
+  const size_t dz_bytes = tc ? sizeof(__nv_bfloat16) * static_cast<size_t>(net.A_ps[0]) * np : sizeof(float) * static_cast<size_t>(rows_all) * H;
+  // one launch from the initial values -> the raw bits of [gradient | scalars | yhat | dZ]
+  const size_t o_scal = g_n * 4, o_yh = o_scal + sizeof(hscal), o_dz = o_yh + sizeof(float) * rows_all;
+  std::vector<char> res, first;
+  StepIn in;
+  in.desc = net.desc; in.scal = net.scal;
+  auto launch = [&](std::vector<char>& out) -> int {
+    SB_CUDA(cudaMemcpy(g.p, hg.data(), sizeof(float) * g_n, cudaMemcpyHostToDevice));
+    SB_CUDA(cudaMemcpy(net.scal, hscal, sizeof(hscal), cudaMemcpyHostToDevice));
+    SB_CUDA(cudaMemset(d_yh.p, 0x7f, sizeof(float) * rows_all));
+    SB_CUDA(cudaMemset(dz_dev, 0x7f, dz_bytes));
+    SB_CUDA(cudaDeviceSynchronize());     // the uploads ran on the legacy stream, the net launches on its own
+    net.launches = 0;
+    SB_TRY(net.enqueue_out(in, M, do_loss != 0, do_bwd != 0, yhat ? d_yh.p : nullptr, g.p));
+    SB_CHECK(net.launches == 1 && net.last_kernel != nullptr, SB_ERR_STATE, "%d output-layer launches", net.launches);
+    SB_TRY(sync_hook(net.last_kernel));
+    out.resize(o_dz + dz_bytes);
+    SB_CUDA(cudaMemcpy(out.data(), g.p, sizeof(float) * g_n, cudaMemcpyDeviceToHost));
+    SB_CUDA(cudaMemcpy(out.data() + o_scal, net.scal, sizeof(hscal), cudaMemcpyDeviceToHost));
+    SB_CUDA(cudaMemcpy(out.data() + o_yh, d_yh.p, sizeof(float) * rows_all, cudaMemcpyDeviceToHost));
+    SB_CUDA(cudaMemcpy(out.data() + o_dz, dz_dev, dz_bytes, cudaMemcpyDeviceToHost));
+    return SB_OK;
+  };
+  // DET: a second launch on the same net (its slots and ticket as the first one left them) from the same initial values
+  SB_TRY(launch(res));
+  if (det) {
+    first.swap(res);
+    SB_TRY(launch(res));
+  }
+  if (repeat_same) *repeat_same = det ? (res == first ? 1 : 0) : -1;
+  if (route) {
+    strncpy(route, net.last_kernel, static_cast<size_t>(route_cap) - 1);
+    route[route_cap - 1] = '\0';
+  }
+
+  int32_t changed = 0;
+  auto u32_at = [&](size_t byte) { uint32_t u; memcpy(&u, res.data() + byte, 4); return u; };
+  for (size_t i = 0; i < g_n; ++i)
+    if (!(do_bwd && i >= io0 && i < io1) && u32_at(4 * i) != S32) ++changed;
+  for (int i = 0; i < SCAL_COUNT; ++i) {
+    uint32_t want;
+    memcpy(&want, hscal + i, 4);
+    if (!(do_loss && i == SCAL_LOSS_SUM) && u32_at(o_scal + 4 * i) != want) ++changed;
+  }
+  for (int r = M; r < rows_all; ++r) changed += u32_at(o_yh + 4 * static_cast<size_t>(r)) != S32;
+  if (yhat) memcpy(yhat, res.data() + o_yh, sizeof(float) * M);
+  if (do_bwd) {
+    memcpy(g_bL, res.data() + 4 * hl.b_off, sizeof(float) * H);
+    memcpy(g_wo, res.data() + 4 * ol.w_off, sizeof(float) * H);
+    memcpy(g_bo, res.data() + 4 * ol.b_off, sizeof(float));
+  }
+  if (do_loss) memcpy(loss_sum, res.data() + o_scal + 4 * SCAL_LOSS_SUM, sizeof(float));
+  // dZ: a backward writes the batch rows' H columns; a batch row's pad columns may hold the sentinel or the +-0 of the
+  // 16-byte piece that reaches into them; nothing else changes (a score or an eval: nothing at all)
+  if (tc) {
+    const uint16_t* h = reinterpret_cast<const uint16_t*>(res.data() + o_dz);
+    for (int k = 0; k < np; ++k)
+      for (int r = 0; r < rows_all; ++r)
+        for (int c = 0; c < ld; ++c) {
+          const uint16_t v = h[static_cast<size_t>(k * net.A_ps[0]) + static_cast<size_t>(r) * ld + c];
+          if (do_bwd && r < M && c < H) {
+            const uint32_t u = static_cast<uint32_t>(v) << 16;
+            memcpy(dZ + (static_cast<size_t>(k) * M + r) * H + c, &u, 4);
+          } else if (v != S16 && !(do_bwd && r < M && (v & 0x7fff) == 0)) {
+            ++changed;
+          }
+        }
+  } else {
+    for (size_t i = 0; i < static_cast<size_t>(rows_all) * H; ++i)
+      if (do_bwd && i < static_cast<size_t>(M) * H) memcpy(dZ + i, res.data() + o_dz + 4 * i, 4);
+      else changed += u32_at(o_dz + 4 * i) != S32;
+  }
+  *guard = changed;
+  return SB_OK;
+}
+
+// The wide+deep embedding gather / scatter-add of a sparse step launched by Net::enqueue_embed (see shifu_b200.h)
+int sb_debug_embed(int32_t precision, int32_t scatter, const float* We, const int32_t* idx, const float* dZ, float* out,
+                   int32_t* guard, int32_t rows, int32_t H, int32_t n_onehot, int32_t n_cat, int device) {
+  SB_CHECK(precision >= SB_PREC_FP32 && precision <= SB_PREC_BF16X2, SB_ERR_INVALID, "precision=%d invalid", precision);
+  SB_CHECK(scatter == 0 || scatter == 1, SB_ERR_INVALID, "scatter=%d (0 gather, 1 scatter-add)", scatter);
+  SB_CHECK(rows >= 1 && rows <= (1 << 24) && H >= 1 && H <= (1 << 16) && n_onehot >= 1 && n_onehot <= (1 << 24) && n_cat >= 1 &&
+           n_cat <= 4096, SB_ERR_INVALID, "rows=%d H=%d n_onehot=%d n_cat=%d", rows, H, n_onehot, n_cat);
+  SB_CHECK(idx && out && guard, SB_ERR_INVALID, "null argument");
+  SB_CHECK(scatter ? dZ != nullptr : We != nullptr, SB_ERR_INVALID, "the gather needs We, the scatter-add dZ");
+  SB_TRY(check_sparse_idx(idx, static_cast<long long>(rows) * n_cat, n_onehot));
+  SB_CHECK(static_cast<long long>(3 + n_onehot) * H < (1LL << 31), SB_ERR_INVALID, "W_0 of %d x %d elements", 3 + n_onehot, H);
+  int dev_sms = 0;
+  SB_TRY(check_device(device, &dev_sms));
+
+  // the net: n_dense = 3 dense columns ahead of the n_onehot embedding rows of W_0, hidden [H]; 64 guard rows past the batch
+  constexpr int N_DENSE = 3, GUARD = 256;
+  sb_net_desc d = {};
+  d.n_features = N_DENSE + n_onehot; d.n_hidden = 1;
+  d.hidden[0] = H; d.acts[0] = SB_ACT_NONE;
+  d.loss = SB_LOSS_MSE; d.optimizer = SB_OPT_SGD;
+  d.max_batch = rows + 64;
+  d.precision = precision;
+  const uint32_t S32 = 0x7f7f7f7fu;
+  const float qnan = std::numeric_limits<float>::quiet_NaN();
+  float s32;
+  memcpy(&s32, &S32, 4);
+  DevBuf<float> g;
+  Net net;                                              // (destroyed first: waits for its stream)
+  SB_TRY(net.init(&d, device, true));
+  SB_TRY(net.set_sparse(N_DENSE, n_onehot, n_cat));
+  const bool tc = net.tc();
+  const int np = net.nparts;
+  const Layer& l0 = net.layers[0];
+  const int rows_all = rows + 64;
+  const size_t e0 = static_cast<size_t>(l0.w_off) + static_cast<size_t>(N_DENSE) * H, e1 = e0 + static_cast<size_t>(n_onehot) * H;
+  // theta: W_e's rows; W_d's rows, b_0 and the output layer NaN, so that a gather reading outside W_e shows it.  The bf16
+  // shadow parts from there, as set_params makes them.
+  std::vector<float> theta(static_cast<size_t>(net.n_params), qnan);
+  if (We) std::copy(We, We + (e1 - e0), theta.begin() + e0);
+  else std::fill(theta.begin() + e0, theta.begin() + e1, 0.f);
+  SB_CUDA(cudaMemcpy(net.theta, theta.data(), sizeof(float) * theta.size(), cudaMemcpyHostToDevice));
+  SB_CUDA(cudaDeviceSynchronize());     // a pageable copy may still be landing when cudaMemcpy returns; the refresh runs
+  SB_TRY(net.refresh_shadows());        // on the net's own stream
+  SB_CUDA(cudaMemcpy(net.idx, idx, sizeof(int32_t) * static_cast<size_t>(rows) * n_cat, cudaMemcpyHostToDevice));
+  int32_t changed = 0;
+  if (!scatter) {
+    // E [rows_all, ld_out]: the sentinel everywhere; the gather writes the batch rows' H columns only
+    const int ldE = l0.ld_out;
+    const size_t e_n = static_cast<size_t>(rows_all) * ldE;
+    SB_CUDA(cudaMemset(net.E, 0x7f, sizeof(float) * e_n));
+    SB_CUDA(cudaDeviceSynchronize());
+    net.launches = 0;
+    SB_TRY(net.enqueue_embed(rows, false, nullptr, net.stream));
+    SB_CHECK(net.launches == 1, SB_ERR_STATE, "%d embedding launches", net.launches);
+    SB_TRY(sync_hook(net.last_kernel));
+    std::vector<uint32_t> h(e_n);
+    SB_CUDA(cudaMemcpy(h.data(), net.E, sizeof(float) * e_n, cudaMemcpyDeviceToHost));
+    for (int r = 0; r < rows_all; ++r)
+      for (int c = 0; c < ldE; ++c) {
+        const uint32_t v = h[static_cast<size_t>(r) * ldE + c];
+        if (r < rows && c < H) memcpy(out + static_cast<size_t>(r) * H + c, &v, 4);
+        else changed += v != S32;
+      }
+  } else {
+    // dZ_0: the caller's rows as the step stores them (np bf16 parts, or fp32); pad columns and guard rows NaN
+    if (tc) {
+      SB_CUDA(cudaMemset(net.dZ[0], 0xff, sizeof(__nv_bfloat16) * static_cast<size_t>(net.A_ps[0]) * np));
+      SB_TRY(upload_parts(net.dZ[0], dZ, rows, H, l0.ld_out, np, net.A_ps[0]));
+    } else {
+      SB_CUDA(cudaMemset(net.dZf[0], 0xff, sizeof(float) * static_cast<size_t>(rows_all) * H));
+      SB_CUDA(cudaMemcpy(net.dZf[0], dZ, sizeof(float) * static_cast<size_t>(rows) * H, cudaMemcpyHostToDevice));
+    }
+    // the flat gradient: W_e's rows in/out, W_d's rows, b_0, the output layer and GUARD floats behind the sentinel
+    const size_t g_n = static_cast<size_t>(net.n_params) + GUARD;
+    std::vector<float> hg(g_n, s32);
+    std::copy(out, out + (e1 - e0), hg.begin() + e0);
+    SB_TRY(g.alloc(g_n));
+    SB_CUDA(cudaMemcpy(g.p, hg.data(), sizeof(float) * g_n, cudaMemcpyHostToDevice));
+    SB_CUDA(cudaDeviceSynchronize());
+    net.launches = 0;
+    SB_TRY(net.enqueue_embed(rows, true, g.p, net.stream));
+    SB_CHECK(net.launches == 1, SB_ERR_STATE, "%d embedding launches", net.launches);
+    SB_TRY(sync_hook(net.last_kernel));
+    SB_CUDA(cudaMemcpy(hg.data(), g.p, sizeof(float) * g_n, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < g_n; ++i) {
+      uint32_t u;
+      memcpy(&u, &hg[i], 4);
+      if ((i < e0 || i >= e1) && u != S32) ++changed;
+    }
+    std::copy(hg.begin() + e0, hg.begin() + e1, out);
+  }
+  *guard = changed;
   return SB_OK;
 }
 

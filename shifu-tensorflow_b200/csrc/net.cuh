@@ -152,5 +152,8 @@ struct Net {
 };
 
 int validate_desc(const sb_net_desc* d);
+// a wide+deep index matrix of n entries: each a one-hot column in [0, n_onehot) or -1 (missing); anything else is
+// SB_ERR_INVALID (a negative index other than -1 is not "missing", and a numpy caller would read it as a row from the end)
+int check_sparse_idx(const int32_t* idx, long long n, int n_onehot);
 
 }  // namespace sb

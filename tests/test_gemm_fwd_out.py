@@ -6,7 +6,7 @@ Oracle: float64 of the same operation, z = act(A W + b) . w_o + b_o, y_hat = sig
 loss = sum_r loss term.  np = 1 takes A and W rounded to bf16 (the kernel then multiplies exactly and accumulates in
 fp32); np = 2 / 3 takes the fp32 inputs (the kernel splits them into bf16 parts).
 
-Tolerances follow the arithmetic, with u = 2^-24:
+Tolerances follow the arithmetic, with u = 2^-24 (the output-layer half is out_layer_ref.output_layer):
   pre-activation  e_pre = c_np * (|A| |W| + |b|): the fp32-class bound of the tensor-core contraction that
                   test_gemm_split.py holds the split GEMM to (c = 3e-6 for np = 1 and 3, 2e-5 for np = 2)
   a = act(pre)    e_a = e_pre + 4u (|a| + 1)                         (|act'| <= 1, a few ulp of tanhf / expf)
@@ -27,13 +27,10 @@ import numpy as np
 import pytest
 
 from conftest import bf16_round
+from out_layer_ref import ACTS, CE, LOSSES, MSE, U, output_layer
+from out_layer_ref import activation as _act
 
-ACTS = {"sigmoid": 0, "tanh": 1, "relu": 2, "leakyrelu": 3, "none": -1}
-MSE, CE = 0, 1
-LOSSES = {"mse": MSE, "ce": CE}
-U = 2.0 ** -24
 ACC = {1: 3e-6, 2: 2e-5, 3: 3e-6}
-ALPHA = 0.2
 OUTS = ("dZ", "db_L", "dw_o", "db_o", "loss")
 
 _worst = {}
@@ -70,76 +67,19 @@ def _operands(M, N, K, seed, a_rows=None, row0=0):
     return _cache[key]
 
 
-def _act(z, act):
-    if act == ACTS["sigmoid"]:
-        return 1.0 / (1.0 + np.exp(-z))
-    if act == ACTS["tanh"]:
-        return np.tanh(z)
-    if act == ACTS["relu"]:
-        return np.maximum(z, 0.0)
-    if act == ACTS["leakyrelu"]:
-        return np.where(z > 0, z, ALPHA * z)
-    return z
-
-
-def _act_grad(a, act):
-    if act == ACTS["sigmoid"]:
-        return a * (1.0 - a)
-    if act == ACTS["tanh"]:
-        return 1.0 - a * a
-    if act == ACTS["relu"]:
-        return (a > 0).astype(np.float64)
-    if act == ACTS["leakyrelu"]:
-        return np.where(a > 0, 1.0, ALPHA)
-    return np.ones_like(a)
-
-
 def _reference(A, W, bias, wo, bo, y, w, act, loss, np_parts, row0, M):
     """float64 values and bounds (module docstring) of every output"""
     f64 = np.float64
     Ab, Wb = A[row0:row0 + M], W
     if np_parts == 1:
         Ab, Wb = bf16_round(Ab), bf16_round(Wb)
-    A64, W64, b64, wo64 = Ab.astype(f64), Wb.astype(f64), bias.astype(f64), wo.astype(f64)
-    N = W.shape[1]
+    A64, W64, b64 = Ab.astype(f64), Wb.astype(f64), bias.astype(f64)
     pre = A64 @ W64 + b64
     e_pre = ACC[np_parts] * (np.abs(A64) @ np.abs(W64) + np.abs(b64))
     a = _act(pre, act)
     e_a = e_pre + 4 * U * (np.abs(a) + 1)
-    aw = a * wo64
-    z = aw.sum(axis=1) + f64(bo)
-    e_z = e_a @ np.abs(wo64) + (N + 4) * U * (np.abs(aw).sum(axis=1) + abs(f64(bo)))
-    yh = 1.0 / (1.0 + np.exp(-z))
-    y64, w64 = y.astype(f64), w.astype(f64)
-    nnz = np.count_nonzero(w)
-    inv = 1.0 / nnz if nnz else 0.0
-    if loss == MSE:
-        per = w64 * (yh - y64) ** 2
-        dz = 2 * w64 * (yh - y64) * yh * (1 - yh) * inv
-    else:
-        per = w64 * (np.maximum(z, 0) - z * y64 + np.log1p(np.exp(-np.abs(z))))
-        dz = w64 * (yh - y64) * inv
-    e_per = np.abs(w64) * (e_z + 8 * U * (np.abs(z) + 1))
-    e_dz = np.abs(w64) * inv * (0.625 * e_z + 16 * U) + 8 * U * np.abs(dz)
-    dzw = np.abs(dz)[:, None] * np.abs(wo64)[None, :]
-    g = dz[:, None] * wo64[None, :] * _act_grad(a, act)
-    e_g = 2 * dzw * e_a + np.abs(wo64)[None, :] * e_dz[:, None] + 4 * U * np.abs(g)
-    if act in (ACTS["relu"], ACTS["leakyrelu"]):
-        kink = np.abs(pre) <= e_pre
-        flip = np.where(kink, dzw * (1.0 - (ALPHA if act == ACTS["leakyrelu"] else 0.0)), 0.0)
-    else:
-        kink = np.zeros(pre.shape, bool)
-        flip = 0.0
-    d = (M + 63) // 64 + 20
-    dza = dz[:, None] * a
-    ref = {"g": g, "e_g": e_g, "kink": kink,
-           "db_L": (g.sum(axis=0), (e_g + flip).sum(axis=0) + d * U * np.abs(g).sum(axis=0)),
-           "dw_o": (dza.sum(axis=0), (np.abs(dz)[:, None] * e_a + np.abs(a) * e_dz[:, None]).sum(axis=0)
-                    + d * U * np.abs(dza).sum(axis=0)),
-           "db_o": (dz.sum(), e_dz.sum() + d * U * np.abs(dz).sum()),
-           "loss": (per.sum(), e_per.sum() + d * U * np.abs(per).sum()),
-           "d": d}
-    return ref
+    kink = np.abs(pre) <= e_pre if act in (ACTS["relu"], ACTS["leakyrelu"]) else None
+    return output_layer(a, e_a, wo, bo, y, w, act, loss, (M + 63) // 64 + 20, kink)
 
 
 def _note(name, err, tol):

@@ -80,3 +80,11 @@ def test_sparse_argument_checks(sb):
         bad = idx.copy(); bad[0, 0] = n_onehot
         with pytest.raises(sb.ShifuB200Error):
             t.step_sparse(Xd, bad, y, w)
+        # -1 is the only "missing" index: any other negative one is refused by every sparse entry point
+        for j in (-2, -2 ** 31):
+            bad = idx.copy(); bad[-1, 1] = j
+            for call in (lambda: t.step_sparse(Xd, bad, y, w), lambda: t.predict_sparse(Xd, bad),
+                         lambda: t.eval_loss_sparse(Xd, bad, y, w)):
+                with pytest.raises(sb.ShifuB200Error) as e:
+                    call()
+                assert e.value.code == sb.capi.SB_ERR_INVALID and "outside [-1," in str(e.value)
