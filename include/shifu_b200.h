@@ -152,6 +152,18 @@ int sb_trainer_set_deterministic(sb_trainer_t* t, int32_t on);
  * once (a device fill).  Call it right after sb_trainer_create: SB_ERR_STATE after the first step or graph capture,
  * SB_ERR_INVALID for an optimizer that reads none of them or a value out of range (both before any device work). */
 int sb_trainer_set_optimizer_params(sb_trainer_t* t, float initial_accumulator, float l1, float l2);
+/* Fine-tuning with frozen layers (ModelConfig train.params FixedLayers / FixedBias).  Layers are numbered from 1: hidden
+ * layers 1..n_hidden, the output layer n_hidden + 1.  The weights of every listed layer, and its bias when fix_bias != 0,
+ * are fixed: a step never changes their values, their optimizer state or their bf16 shadows (bit for bit, whatever the
+ * optimizer - Adam, Momentum, RMSProp and FTRL would move a parameter with a zero gradient), sb_trainer_get_grads reports
+ * 0 for them, and the peer exchange neither moves nor updates them.  A step skips the dW GEMM of every frozen weight
+ * matrix and the dA GEMMs that nothing at or below them needs; every parameter that trains gets the gradient it gets
+ * without frozen layers.  layers == NULL with n == 0 freezes nothing (the default).  SB_ERR_INVALID, before any device
+ * work: a layer outside [1, n_hidden + 1], a layer listed twice, or every parameter fixed.  SB_ERR_STATE after the first
+ * step or graph capture, or after the peer exchange was set up.  Every rank must fix the same parameters:
+ * sb_trainer_set_peer_handles / _pointers refuse a peer that does not (SB_ERR_INVALID), so call this on every rank
+ * before the exchange handles are shared. */
+int sb_trainer_set_fixed_layers(sb_trainer_t* t, const int32_t* layers, int32_t n, int32_t fix_bias);
 
 /* one sess.run([train_step, loss, global_step], feed_dict) (ssgd_monitor.py:272-276) in the
  * "clean" schedule: forward, loss, backward, gradient mean over ranks, one optimizer update.

@@ -110,6 +110,7 @@ PROTOTYPES = {
     "sb_trainer_set_sparse": (C.c_int, [_vp, C.c_int32, C.c_int32, C.c_int32]),
     "sb_trainer_set_deterministic": (C.c_int, [_vp, C.c_int32]),
     "sb_trainer_set_optimizer_params": (C.c_int, [_vp, C.c_float, C.c_float, C.c_float]),
+    "sb_trainer_set_fixed_layers": (C.c_int, [_vp, _P(C.c_int32), C.c_int32, C.c_int32]),
     "sb_trainer_step_sparse": (C.c_int, [_vp, _f32p, _P(C.c_int32), _f32p, _f32p, C.c_int32, _f32p]),
     "sb_trainer_predict_sparse": (C.c_int, [_vp, _f32p, _P(C.c_int32), C.c_int64, _f32p]),
     "sb_trainer_eval_loss_sparse": (C.c_int, [_vp, _f32p, _P(C.c_int32), _f32p, _f32p, C.c_int64, _f32p]),
@@ -279,8 +280,9 @@ class Trainer:
 
     def __init__(self, desc: NetDesc, device: int = 0, nccl_id: Optional[bytes] = None, rank: int = 0, world: int = 1,
                  deterministic: bool = False, initial_accumulator: Optional[float] = None, l1: Optional[float] = None,
-                 l2: Optional[float] = None):
-        """initial_accumulator / l1 / l2 (Adagrad, FTRL; None = TF's default): see set_optimizer_params"""
+                 l2: Optional[float] = None, fixed_layers: Sequence[int] = (), fixed_bias: bool = True):
+        """initial_accumulator / l1 / l2 (Adagrad, FTRL; None = TF's default): see set_optimizer_params;
+        fixed_layers / fixed_bias: see set_fixed_layers"""
         self._h = C.c_void_p()
         self.desc = desc
         idbuf = None
@@ -297,6 +299,17 @@ class Trainer:
         if (initial_accumulator, l1, l2) != (None, None, None):
             self.set_optimizer_params(INITIAL_ACCUMULATOR if initial_accumulator is None else initial_accumulator,
                                       L1 if l1 is None else l1, L2 if l2 is None else l2)
+        if len(fixed_layers) > 0:
+            self.set_fixed_layers(fixed_layers, fixed_bias)
+
+    def set_fixed_layers(self, layers: Sequence[int], fix_bias: bool = True):
+        """Fine-tuning: never change the weights of these layers, nor their biases when fix_bias (Shifu's FixedLayers /
+        FixedBias; sb_trainer_set_fixed_layers).  Layers are numbered from 1: hidden layers 1..n_hidden, the output layer
+        n_hidden + 1.  Their values, optimizer state and bf16 shadows keep their bits, get_grads reports 0 for them, and a
+        step skips the GEMMs only they need.  Before the first step and before the peer exchange is set up, on every rank."""
+        arr = np.ascontiguousarray([int(x) for x in layers], dtype=np.int32)
+        ptr = arr.ctypes.data_as(_P(C.c_int32)) if arr.size else None
+        check(lib().sb_trainer_set_fixed_layers(self._h, ptr, int(arr.size), 1 if fix_bias else 0))
 
     def set_deterministic(self, on: bool = True):
         """fixed-order reductions in every training kernel (sb_trainer_set_deterministic); before the first step"""

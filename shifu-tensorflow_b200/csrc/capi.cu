@@ -125,6 +125,12 @@ struct sb_trainer {
   cudaStream_t prep = nullptr;
   cudaEvent_t ev_prep[2] = {nullptr, nullptr}, ev_pos[2] = {nullptr, nullptr};
   unsigned long long prefetches = 0;   // prefetched launches so far: launch i uses set i & 1
+  // Fine-tuning (sb_trainer_set_fixed_layers): whether W_l / b_l of layer l = 0..L train, and the same as bit masks of the
+  // frozen ones (what the peers compare).  dA_l (l >= 1) runs only for l > l_min, the lowest hidden layer with a parameter
+  // that trains (L: none), since it exists to make dZ_{l-1} for dW and bias gradients at or below layer l - 1.
+  std::vector<char> w_trains, b_trains;
+  int l_min = 0;
+  unsigned long long frozen_w = 0, frozen_b = 0;
   bool started = false;    // a step ran or was captured: sb_trainer_set_deterministic is refused from here on
   bool have_pos = false;   // ev_pos[] of the previous prefetched launch is valid (no step on set 0 since)
   int last_set = 0;        // the set of the last prefetched launch
@@ -444,10 +450,14 @@ static int enqueue_step_backward(sb_trainer* t, const StepIn& in, int rows, int 
   Net& n = t->net;
   float* g = t->grad;
   const int L = n.L, S = n.num_sms;
+  // frozen layers (sb_trainer_set_fixed_layers): dW_l only where W_l trains, dA_l only where something at or below layer
+  // l - 1 needs dZ_{l-1}.  With nothing frozen both are always true.
+  auto dw = [&](int l) { return t->w_trains[static_cast<size_t>(l)] != 0; };
+  auto da = [&](int l) { return l > t->l_min; };
   if (!n.tc()) {
     for (int l = L - 1; l >= 0; --l) {            // fp32: one stream
-      SB_TRY(n.enqueue_dw(in, l, rows, g, n.stream, false, S));
-      if (l > 0) SB_TRY(n.enqueue_da(l, rows, g));
+      if (dw(l)) SB_TRY(n.enqueue_dw(in, l, rows, g, n.stream, false, S));
+      if (l > 0 && da(l)) SB_TRY(n.enqueue_da(l, rows, g));
     }
   } else {
     // Single GPU, one update per mini-batch: no exchange, so nothing needs ALL gradients at once.  dW_0 runs on the main
@@ -468,28 +478,42 @@ static int enqueue_step_backward(sb_trainer* t, const StepIn& in, int rows, int 
     // once every peer has read the gradient runs it owns of this rank (xchg_p2p.cuh), so the next step's layer-0 forward
     // GEMM may clear the gradient buffer.
     const bool xsched = split_tail && t->world > 1;
-    const Dw1Plan d1 = L > 1 ? plan_dw1(t, rows, split_tail, xsched) : Dw1Plan{DW1_BESIDE, {S, S}};
+    Dw1Plan d1 = L > 1 ? plan_dw1(t, rows, split_tail, xsched) : Dw1Plan{DW1_BESIDE, {S, S}};
+    if (L > 1 && !(dw(0) && dw(1))) {
+      // dW_0 or dW_1 frozen: the other one has the SMs to itself.  Without dW_0 (and without the exchange, which keeps its
+      // plan) dW_1 is the last GEMM: in front, PDL-chained on the main stream.
+      d1.sms[0] = d1.sms[1] = S;
+      if (!xsched && !dw(0)) d1.at = DW1_FRONT;
+    }
+    // the exchange's slot A publishes the step scalars when there are no layer-0 chunks (W_0 frozen)
+    const bool a_publishes = t->x_chunks == 0;
+    bool side_used = false;     // a launch went to the side stream (which the end of the step then joins)
     // dW_l and dA_l both consume dZ_l and are independent of each other: the dW GEMMs go to the side stream and overlap
     // the dA chain
     for (int l = L - 1; l >= 1; --l) {
-      if (l > 1 || d1.at == DW1_BESIDE) {
+      if ((l > 1 || d1.at == DW1_BESIDE) && dw(l)) {
         SB_TRY(join_streams(t->side, n.stream, t->ev_dz[l]));
         SB_TRY(n.enqueue_dw(in, l, rows, g, t->side, false, l == 1 ? d1.sms[1] : S));
+        side_used = true;
       }
-      SB_TRY(n.enqueue_da(l, rows, g));
+      if (da(l)) SB_TRY(n.enqueue_da(l, rows, g));
     }
     if (split_tail) SB_CUDA(cudaEventRecord(t->ev_da_done, n.stream));
     if (L == 1) {
-      SB_TRY(join_streams(t->side, n.stream, t->ev_dz[0]));
-      SB_TRY(n.enqueue_dw(in, 0, rows, g, t->side, false, S));
+      if (dw(0)) {
+        SB_TRY(join_streams(t->side, n.stream, t->ev_dz[0]));
+        SB_TRY(n.enqueue_dw(in, 0, rows, g, t->side, false, S));
+        side_used = true;
+      }
     } else {
       if (d1.at == DW1_FRONT) {
         // dW_0's last exchange then runs on an idle GPU; the side stream's next launch (slot A's exchange, or the
         // optimizer of the other layers) waits for dW_1
-        SB_TRY(n.enqueue_dw(in, 1, rows, g, n.stream, true, d1.sms[1]));
+        if (dw(1)) SB_TRY(n.enqueue_dw(in, 1, rows, g, n.stream, true, d1.sms[1]));
         SB_TRY(join_streams(t->side, n.stream, t->ev_c[0]));
+        side_used = true;
         if (xsched) {
-          SB_TRY(enqueue_xchg(t, in, XSEG_A, t->side, false, false));
+          SB_TRY(enqueue_xchg(t, in, XSEG_A, t->side, a_publishes, false));
           SB_CUDA(cudaEventRecord(t->ev_x[0], t->side));
         }
       }
@@ -507,33 +531,38 @@ static int enqueue_step_backward(sb_trainer* t, const StepIn& in, int rows, int 
           SB_TRY(enqueue_xchg(t, in, 1 << (1 + c), cs, last, false, last && d1.at != DW1_BEHIND));
           SB_CUDA(cudaEventRecord(t->ev_x[1 + c], cs));
         }
-      } else {
+      } else if (dw(0)) {
         SB_TRY(n.enqueue_dw(in, 0, rows, g, n.stream, true, d1.sms[0]));
       }
       if (d1.at == DW1_BEHIND) {
-        SB_TRY(n.enqueue_dw(in, 1, rows, g, n.stream, true, d1.sms[1]));
+        if (dw(1)) SB_TRY(n.enqueue_dw(in, 1, rows, g, n.stream, true, d1.sms[1]));
         SB_TRY(join_streams(t->side, n.stream, t->ev_c[0]));
-        SB_TRY(enqueue_xchg(t, in, XSEG_A, t->side, false, false));
+        side_used = true;
+        SB_TRY(enqueue_xchg(t, in, XSEG_A, t->side, a_publishes, false));
         SB_CUDA(cudaEventRecord(t->ev_x[0], t->side));
       }
     }
     if (xsched) {
       // whatever follows on the main stream (the next step's layer-0 forward, or the end of the graph) needs hidden
       // layer 0.  A wide+deep step's layer-0 dW is not cut into the slot chunks: it is exchanged here, behind everything.
-      if (in.feed == Feed::SPARSE) SB_TRY(enqueue_xchg(t, in, xseg_all(t) & ~XSEG_A, n.stream, true, false));
-      else
+      if (in.feed == Feed::SPARSE) {
+        if (t->x_chunks > 0) SB_TRY(enqueue_xchg(t, in, xseg_all(t) & ~XSEG_A, n.stream, true, false));
+      } else {
         for (int c = 0; c < t->x_chunks; ++c) SB_CUDA(cudaStreamWaitEvent(n.stream, t->ev_x[1 + c], 0));
+      }
       SB_CUDA(cudaStreamWaitEvent(n.stream, t->ev_x[0], 0));
       return SB_OK;
     }
     if (split_tail) {
+      // the layer-0 optimizer publishes the step scalars, or the other layers' one when layer 0 has nothing that trains
+      const bool l0_runs = n.work_end[0] > n.work_begin[0];
       SB_TRY(enqueue_optimizer(t, in, g, n.work_begin[0], n.work_end[0], n.stream, true, true));
       // the other layers' shadows are read by the dA GEMMs on the main stream: update them only after the last one
       SB_CUDA(cudaStreamWaitEvent(t->side, t->ev_da_done, 0));
-      SB_TRY(enqueue_optimizer(t, in, g, n.work_end[0], n.n_work, t->side));
+      SB_TRY(enqueue_optimizer(t, in, g, n.work_end[0], n.n_work, t->side, !l0_runs));
       return join_streams(n.stream, t->side, t->ev_join);
     }
-    SB_TRY(join_streams(n.stream, t->side, t->ev_join));
+    if (side_used) SB_TRY(join_streams(n.stream, t->side, t->ev_join));
   }
   if (kind == G_STEP) {
     if (t->world > 1 && t->p2p_ready) {
@@ -832,6 +861,34 @@ static int fill_initial_state(sb_trainer* t) {
   return SB_OK;
 }
 
+// Exchange slots over the work table: hidden layer 0 in row chunks of W_0 (128-row multiples; runs are 1024 parameters, so
+// chunk borders fall on run borders when out % 8 == 0), the last chunk also carries b_0; everything else is slot 0.  With
+// W_0 frozen there are no chunks, and slot 0 also carries b_0 if it trains.
+static void set_exchange_slots(sb_trainer* t) {
+  const Net& n = t->net;
+  const Layer& l0 = n.layers[0];
+  if (!t->w_trains[0]) {
+    t->x_chunk_rows = 0;
+    t->x_chunks = 0;
+    t->x_slots = 1;
+    t->x_begin[0] = n.work_begin[0]; t->x_end[0] = n.n_work;
+    return;
+  }
+  int chunks = 2;
+  if (!n.tc() || (l0.out % 8) != 0 || l0.in < 256 * chunks) chunks = 1;
+  const int cr = round_up((l0.in + chunks - 1) / chunks, 128);
+  chunks = (l0.in + cr - 1) / cr;           // (rounding to 128 rows may need fewer chunks)
+  t->x_chunk_rows = cr;
+  t->x_chunks = chunks;
+  t->x_slots = 1 + chunks;
+  t->x_begin[0] = n.work_end[0]; t->x_end[0] = n.n_work;
+  for (int c = 0; c < chunks; ++c) {
+    const long long e0 = static_cast<long long>(c) * cr * l0.out, e1 = static_cast<long long>(c + 1) * cr * l0.out;
+    t->x_begin[1 + c] = n.work_begin[0] + static_cast<int>(e0 / 1024);
+    t->x_end[1 + c] = (c == chunks - 1) ? n.work_end[0] : n.work_begin[0] + static_cast<int>(e1 / 1024);
+  }
+}
+
 int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, int rank, int world, sb_trainer_t** out) {
   SB_CHECK(out, SB_ERR_INVALID, "out is null");
   *out = nullptr;
@@ -895,27 +952,12 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
   memset(t->h_err, 0, sizeof(unsigned int) * 4);
   if (const char* e = getenv("SB_XCHG_TIMEOUT_S")) t->xchg_timeout_ns = static_cast<unsigned long long>(atof(e) * 1e9);
   if (const char* e = getenv("SB_XCHG_BLOCKS")) t->xchg_blocks = atoi(e);
-  {
-    // exchange slots: hidden layer 0 in row chunks of W_0 (128-row multiples; runs are 1024 parameters, so chunk borders fall
-    // on run borders when out % 8 == 0), the last chunk also carries b_0; everything else is slot 0
-    int chunks = 2;
-    const Layer& l0 = n.layers[0];
-    if (!n.tc() || (l0.out % 8) != 0 || l0.in < 256 * chunks) chunks = 1;
-    const int cr = round_up((l0.in + chunks - 1) / chunks, 128);
-    chunks = (l0.in + cr - 1) / cr;           // (rounding to 128 rows may need fewer chunks)
-    t->x_chunk_rows = cr;
-    t->x_chunks = chunks;
-    t->x_slots = 1 + chunks;
-    t->x_begin[0] = n.work_end[0]; t->x_end[0] = n.n_work;
-    for (int c = 0; c < chunks; ++c) {
-      const long long e0 = static_cast<long long>(c) * cr * l0.out, e1 = static_cast<long long>(c + 1) * cr * l0.out;
-      t->x_begin[1 + c] = n.work_begin[0] + static_cast<int>(e0 / 1024);
-      t->x_end[1 + c] = (c == chunks - 1) ? n.work_end[0] : n.work_begin[0] + static_cast<int>(e1 / 1024);
-    }
-    for (int i = 0; i < SB_XCHG_SLOTS; ++i) {
-      SB_TRY(create_event(&t->ev_x[i]));
-      SB_TRY(create_event(&t->ev_c[i]));
-    }
+  t->w_trains.assign(static_cast<size_t>(n.L + 1), 1);
+  t->b_trains.assign(static_cast<size_t>(n.L + 1), 1);
+  set_exchange_slots(t.get());
+  for (int i = 0; i < SB_XCHG_SLOTS; ++i) {
+    SB_TRY(create_event(&t->ev_x[i]));
+    SB_TRY(create_event(&t->ev_c[i]));
   }
   SB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&t->h_scal), sizeof(float) * SCAL_COUNT, cudaHostAllocMapped));
   memset(t->h_scal, 0, sizeof(float) * SCAL_COUNT);
@@ -989,6 +1031,21 @@ static int preload_exchange_kernels() {
 // peers' exchange allocations -> device table; bases[rank] is ignored (own allocation)
 static int install_peer_table(sb_trainer* t, void* const* bases) {
   SB_TRY(preload_exchange_kernels());
+  // every rank must freeze the same parameters (sb_trainer_set_fixed_layers): the slot tables define who owns which run.
+  // Read each peer's masks from its flag block and refuse a mismatch instead of exchanging with it.
+  for (int q = 0; q < t->world; ++q) {
+    if (q == t->rank) continue;
+    unsigned long long theirs[2] = {};
+    const char* at = static_cast<const char*>(bases[q]) + t->flags_off + offsetof(P2PFlags, frozen);
+    SB_CUDA(cudaMemcpyAsync(theirs, at, sizeof(theirs), cudaMemcpyDefault, t->net.stream));
+    SB_CUDA(cudaStreamSynchronize(t->net.stream));
+    if (theirs[0] != t->frozen_w || theirs[1] != t->frozen_b) {
+      t->close_peer_mappings();
+      return set_error(SB_ERR_INVALID, "rank %d fixes other parameters than rank %d (frozen W / b layer masks %#llx / %#llx vs "
+                       "%#llx / %#llx): every rank needs the same sb_trainer_set_fixed_layers", q, t->rank, theirs[0], theirs[1],
+                       t->frozen_w, t->frozen_b);
+    }
+  }
   P2PPeers hp;
   memset(&hp, 0, sizeof(hp));
   for (int q = 0; q < t->world; ++q) hp.base[q] = static_cast<char*>((q == t->rank) ? t->xch : bases[q]);
@@ -1121,6 +1178,13 @@ int sb_trainer_get_grads(sb_trainer_t* t, float* flat, int64_t n) {
   SB_CUDA(cudaStreamSynchronize(t->net.stream));
   const float gs = t->grad_out_scale;
   if (gs != 1.f) for (int64_t i = 0; i < n; ++i) flat[i] *= gs;
+  // a frozen parameter's gradient is 0 (a dA or output-layer epilogue that runs for the layers below may have written the
+  // bias gradient of a frozen layer; no update reads it)
+  for (size_t l = 0; l < t->net.layers.size(); ++l) {
+    const Layer& ly = t->net.layers[l];
+    if (!t->w_trains[l]) std::fill(flat + ly.w_off, flat + ly.w_off + static_cast<long long>(ly.in) * ly.out, 0.f);
+    if (!t->b_trains[l]) std::fill(flat + ly.b_off, flat + ly.b_off + ly.out, 0.f);
+  }
   return SB_OK;
 }
 
@@ -1169,6 +1233,46 @@ int sb_trainer_set_optimizer_params(sb_trainer_t* t, float initial_accumulator, 
   t->hyper.l1 = l1; t->hyper.l2 = l2;
   SB_TRY(fill_initial_state(t));
   SB_CUDA(cudaStreamSynchronize(t->net.stream));
+  return SB_OK;
+}
+
+int sb_trainer_set_fixed_layers(sb_trainer_t* t, const int32_t* layers, int32_t n, int32_t fix_bias) {
+  SB_CHECK(t, SB_ERR_INVALID, "null trainer");
+  SB_CHECK(n >= 0, SB_ERR_INVALID, "n = %d must be >= 0", n);
+  SB_CHECK(n == 0 || layers, SB_ERR_INVALID, "layers is null");
+  Net& net = t->net;
+  const int nl = net.L + 1;                    // layers 1..L hidden, L + 1 the output layer
+  std::vector<char> w(static_cast<size_t>(nl), 1), b(static_cast<size_t>(nl), 1);
+  for (int i = 0; i < n; ++i) {
+    const int x = layers[i];
+    SB_CHECK(x >= 1 && x <= nl, SB_ERR_INVALID, "fixed layer %d outside [1, %d] (hidden layers 1..%d, output layer %d)", x, nl,
+             nl - 1, nl);
+    SB_CHECK(w[static_cast<size_t>(x - 1)], SB_ERR_INVALID, "fixed layer %d listed twice", x);
+    w[static_cast<size_t>(x - 1)] = 0;
+    if (fix_bias) b[static_cast<size_t>(x - 1)] = 0;
+  }
+  int l_min = net.L;
+  for (int l = net.L - 1; l >= 0; --l)
+    if (w[static_cast<size_t>(l)] || b[static_cast<size_t>(l)]) l_min = l;
+  const bool any = l_min < net.L || w[static_cast<size_t>(net.L)] || b[static_cast<size_t>(net.L)];
+  SB_CHECK(any, SB_ERR_INVALID, "every parameter is fixed: nothing would train");
+  SB_CHECK(!t->started && t->n_acc == 0 && t->global_step == 0, SB_ERR_STATE,
+           "sb_trainer_set_fixed_layers after the first step or graph capture: set it right after sb_trainer_create");
+  SB_CHECK(!t->p2p_ready, SB_ERR_STATE, "sb_trainer_set_fixed_layers after the peer exchange was set up: set it first");
+  SB_CUDA(cudaSetDevice(net.device));
+  SB_TRY(net.set_trainable(w, b));
+  t->w_trains = w; t->b_trains = b;
+  t->l_min = l_min;
+  t->frozen_w = t->frozen_b = 0;
+  for (int l = 0; l < nl; ++l) {
+    if (!w[static_cast<size_t>(l)]) t->frozen_w |= 1ull << l;
+    if (!b[static_cast<size_t>(l)]) t->frozen_b |= 1ull << l;
+  }
+  set_exchange_slots(t);
+  // the peers compare the masks when their tables are set (install_peer_table)
+  const unsigned long long masks[2] = {t->frozen_w, t->frozen_b};
+  SB_CUDA(cudaMemcpyAsync(t->flags->frozen, masks, sizeof(masks), cudaMemcpyHostToDevice, net.stream));
+  SB_CUDA(cudaStreamSynchronize(net.stream));
   return SB_OK;
 }
 

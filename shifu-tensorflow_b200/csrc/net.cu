@@ -248,35 +248,13 @@ int Net::init(const sb_net_desc* d, int device_, bool training_) {
   }
 
   // optimizer / shadow-refresh work table: runs of <= 1024 consecutive parameters
-  std::vector<OptWork> wk;
-  auto add_runs = [&](long long o, long long n, const Layer* mat) {
-    for (long long s = 0; s < n; s += 1024) {
-      OptWork w = {};
-      w.off = o + s; w.count = static_cast<int>(n - s < 1024 ? n - s : 1024);
-      w.np = 1;
-      if (mat) {
-        w.out_dim = mat->out; w.mat_off = mat->w_off; w.Wn = mat->Wn; w.ld_out = mat->ld_out;
-        w.np = nparts; w.part_stride = Wn_ps[static_cast<size_t>(mat - layers.data())];
-      }
-      wk.push_back(w);
-    }
-  };
-  work_begin.assign(L + 1, 0); work_end.assign(L + 1, 0);
-  for (int l = 0; l <= L; ++l) {
-    Layer& ly = layers[l];
-    work_begin[l] = static_cast<int>(wk.size());
-    if (bf && l < L) {
-      add_runs(ly.w_off, static_cast<long long>(ly.in) * ly.out, &ly);
-      add_runs(ly.b_off, ly.out, nullptr);
-    } else {
-      add_runs(ly.w_off, static_cast<long long>(ly.in) * ly.out + ly.out, nullptr);
-    }
-    work_end[l] = static_cast<int>(wk.size());
-  }
+  const std::vector<char> all(static_cast<size_t>(L + 1), 1);
+  const std::vector<OptWork> wk = build_work(all, all, &work_begin, &work_end);
   n_work = static_cast<int>(wk.size());
   SB_TRY(dalloc(&work, wk.size()));
   SB_CUDA(cudaMemcpyAsync(work, wk.data(), wk.size() * sizeof(OptWork), cudaMemcpyHostToDevice, stream));
   SB_CUDA(cudaStreamSynchronize(stream));
+  work_all = work; n_work_all = n_work;
 
   // opt in to > 48 KB dynamic shared memory once, outside of any stream capture
   if (bf) {
@@ -375,9 +353,63 @@ int Net::enqueue_embed(int rows, bool scatter, float* grad, cudaStream_t st) {
   return SB_OK;
 }
 
+// The runs of every parameter that trains (w_trains[l] / b_trains[l]: W_l / b_l of layer l = 0..L), layer by layer; the
+// range of layer l goes to [(*begin)[l], (*end)[l]).  A tensor-core net keeps W_l (shadow-backed) and b_l in separate
+// runs; fp32 mode puts W_l and b_l, which lie next to each other, into one stretch of runs when both train.
+std::vector<OptWork> Net::build_work(const std::vector<char>& w_trains, const std::vector<char>& b_trains, std::vector<int>* begin,
+                                     std::vector<int>* end) const {
+  std::vector<OptWork> wk;
+  auto add_runs = [&](long long o, long long n, const Layer* mat) {
+    for (long long s = 0; s < n; s += 1024) {
+      OptWork w = {};
+      w.off = o + s; w.count = static_cast<int>(n - s < 1024 ? n - s : 1024);
+      w.np = 1;
+      if (mat) {
+        w.out_dim = mat->out; w.mat_off = mat->w_off; w.Wn = mat->Wn; w.ld_out = mat->ld_out;
+        w.np = nparts; w.part_stride = Wn_ps[static_cast<size_t>(mat - layers.data())];
+      }
+      wk.push_back(w);
+    }
+  };
+  begin->assign(L + 1, 0); end->assign(L + 1, 0);
+  for (int l = 0; l <= L; ++l) {
+    const Layer& ly = layers[l];
+    const long long nw = static_cast<long long>(ly.in) * ly.out;
+    (*begin)[l] = static_cast<int>(wk.size());
+    if (tc() && l < L) {
+      if (w_trains[l]) add_runs(ly.w_off, nw, &ly);
+      if (b_trains[l]) add_runs(ly.b_off, ly.out, nullptr);
+    } else if (w_trains[l] && b_trains[l]) {
+      add_runs(ly.w_off, nw + ly.out, nullptr);
+    } else {
+      if (w_trains[l]) add_runs(ly.w_off, nw, nullptr);
+      if (b_trains[l]) add_runs(ly.b_off, ly.out, nullptr);
+    }
+    (*end)[l] = static_cast<int>(wk.size());
+  }
+  return wk;
+}
+
+int Net::set_trainable(const std::vector<char>& w_trains, const std::vector<char>& b_trains) {
+  SB_CUDA(cudaSetDevice(device));
+  const std::vector<OptWork> wk = build_work(w_trains, b_trains, &work_begin, &work_end);
+  n_work = static_cast<int>(wk.size());
+  const bool every = std::all_of(w_trains.begin(), w_trains.end(), [](char c) { return c != 0; }) &&
+                     std::all_of(b_trains.begin(), b_trains.end(), [](char c) { return c != 0; });
+  if (every) {                       // everything trains: the table init() built
+    work = work_all;
+    return SB_OK;
+  }
+  if (!work_part) SB_TRY(dalloc(&work_part, static_cast<size_t>(n_work_all)));
+  work = work_part;
+  if (n_work > 0) SB_CUDA(cudaMemcpyAsync(work, wk.data(), wk.size() * sizeof(OptWork), cudaMemcpyHostToDevice, stream));
+  SB_CUDA(cudaStreamSynchronize(stream));
+  return SB_OK;
+}
+
 int Net::refresh_shadows() {
   if (!tc()) return SB_OK;
-  shadow_refresh_kernel<<<n_work, 256, 0, stream>>>(work, theta);
+  shadow_refresh_kernel<<<n_work_all, 256, 0, stream>>>(work_all, theta);
   SB_CUDA(cudaGetLastError());
   return SB_OK;
 }

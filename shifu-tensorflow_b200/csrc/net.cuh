@@ -72,8 +72,19 @@ struct Net {
   BatchDesc* desc = nullptr;               // the net's own descriptor / scalar slot (set 0, slot 0 of a trainer's ring)
   float* scal = nullptr;
   float *stX = nullptr, *stY = nullptr, *stW = nullptr;  // H2D staging (device)
+  // The optimizer's work table: the runs of every parameter that trains (all of them unless set_trainable froze some).
+  // work_all / n_work_all: every run, which the shadow refresh walks.
   OptWork* work = nullptr;
   int n_work = 0;
+  OptWork* work_all = nullptr;
+  int n_work_all = 0;
+  OptWork* work_part = nullptr;            // the table's storage once set_trainable left parameters out
+  std::vector<OptWork> build_work(const std::vector<char>& w_trains, const std::vector<char>& b_trains, std::vector<int>* begin,
+                                  std::vector<int>* end) const;
+  // Freeze parameters (fine-tuning, sb_trainer_set_fixed_layers): the work table and work_begin / work_end keep only the runs
+  // of W_l where w_trains[l] and of b_l where b_trains[l] (l = 0..L).  Frozen runs are never updated or shadow-refreshed by
+  // a step.
+  int set_trainable(const std::vector<char>& w_trains, const std::vector<char>& b_trains);
   int launches = 0;  // kernels enqueued since last reset (for gpu_launches accounting)
   // SB_STEP_TRACE=1: every GEMM of a step stamps %globaltimer milestones of its CTA 0 into 16 slots (debug timeline)
   unsigned long long* step_trace = nullptr;

@@ -49,8 +49,11 @@ struct P2PFlags {                                     // at arena + flags_off on
   unsigned int arrive[SB_XCHG_SLOTS][SB_MAX_RANKS];   // arrive[slot][q] written by rank q
   unsigned int done[SB_XCHG_SLOTS][SB_MAX_RANKS];     // done[slot][q]   written by rank q
   unsigned int blocks_done[SB_XCHG_SLOTS];            // local: grid-wide completion counter per slot
-  unsigned int pad[24];
+  unsigned long long frozen[2];                       // frozen W / b layer masks (sb_trainer_set_fixed_layers), read by
+                                                      // every peer when its table is set: the slot tables must agree
+  unsigned int pad[20];
 };
+static_assert(sizeof(P2PFlags) == 1152, "P2PFlags layout");
 
 struct P2PPeers {                         // device-resident table, same order on every rank
   char* base[SB_MAX_RANKS];               // arena of every rank (own entry = own arena)

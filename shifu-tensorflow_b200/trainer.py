@@ -38,6 +38,14 @@ Optional ModelConfig train.params the reference does not have (defaults = refere
              them (keyed by SB_SEED, or a logged random seed, the worker index and global_step) and trains on
              mini-batches cut from that order (sb_trainer_set_row_order; wide+deep: the host arrays are permuted).  The
              validation set keeps its order
+  FixedLayers  list of layer numbers (ints, or strings that parse as ints; default none): fine-tuning - these layers'
+             weights are never changed (sb_trainer_set_fixed_layers).  Layers are numbered from 1 as in Shifu's NN
+             trainer: hidden layers 1..NumHiddenLayers, the output layer NumHiddenLayers + 1.  A fixed layer's values,
+             optimizer state and bf16 shadows keep their bits, and a step skips the GEMMs only they need
+  FixedBias  true (default) | false: whether the FixedLayers' biases are fixed as well
+  Start a fine-tuning run from an earlier model with SB_INIT_MODEL=<local SavedModel directory> (FINAL_MODEL_PATH of that
+  run): its weights must have the ModelConfig's topology; global_step starts at 0 and the optimizer state at its start
+  values.  A checkpoint in TMP_MODEL_PATH still takes precedence.
 
 File paths (TRAINING_DATA_PATH, TMP_MODEL_PATH, FINAL_MODEL_PATH) may carry a scheme.  The stock AM hands out fully
 qualified HDFS URIs (TrainingDataSet.java:74) which the reference reads through tf.gfile; here `hdfs://`, `viewfs://`,
@@ -122,6 +130,52 @@ def deterministic_requested(params: dict) -> bool:
 def shuffle_requested(params: dict) -> bool:
     """train.params.Shuffle: a JSON bool, or the strings true / false"""
     return _bool_param(params, 'Shuffle')
+
+
+def fixed_layers_requested(params: dict) -> tuple:
+    """train.params.FixedLayers (a JSON list of layer numbers, ints or strings that parse as ints; absent = none) and
+    FixedBias (a JSON bool or the strings true / false; absent = true) -> (sorted layer list, fix_bias).  Layers are
+    numbered from 1: hidden layers 1..NumHiddenLayers, the output layer NumHiddenLayers + 1.  Raises ValueError for a
+    layer out of range, a layer listed twice, or a list that freezes every parameter."""
+    raw = params.get('FixedLayers', [])
+    if raw is None:
+        raw = []
+    if not isinstance(raw, (list, tuple)):
+        raise ValueError("train.params.FixedLayers must be a list of layer numbers, got %r" % (raw,))
+    layers = []
+    for v in raw:
+        if isinstance(v, bool):
+            raise ValueError("train.params.FixedLayers: %r is not a layer number" % (v,))
+        try:
+            layers.append(int(v.strip()) if isinstance(v, str) else int(v))
+        except (TypeError, ValueError):
+            raise ValueError("train.params.FixedLayers: %r is not a layer number" % (v,)) from None
+        if isinstance(v, float) and v != layers[-1]:
+            raise ValueError("train.params.FixedLayers: %r is not a layer number" % (v,))
+    fix_bias = _bool_param(params, 'FixedBias') if 'FixedBias' in params else True
+    n_layers = int(params.get('NumHiddenLayers', 1)) + 1
+    for x in layers:
+        if not 1 <= x <= n_layers:
+            raise ValueError("train.params.FixedLayers: layer %d outside 1..%d (hidden layers 1..%d, output layer %d)"
+                             % (x, n_layers, n_layers - 1, n_layers))
+    if len(set(layers)) != len(layers):
+        raise ValueError("train.params.FixedLayers lists a layer twice: %r" % (layers,))
+    if fix_bias and len(layers) == n_layers:
+        raise ValueError("train.params.FixedLayers fixes every layer and FixedBias their biases: nothing would train")
+    return sorted(layers), fix_bias
+
+
+def read_init_model(saved_model_dir: str, desc: capi.NetDesc) -> np.ndarray:
+    """SB_INIT_MODEL: the flat parameters of a SavedModel this worker exported (FINAL_MODEL_PATH of an earlier run), checked
+    against the ModelConfig's topology.  Raises ValueError naming both when they differ."""
+    F, hidden, acts, out_act, flat = capi.savedmodel_read(saved_model_dir, "shifu_input_0", "shifu_output_0")
+    want_hidden = [int(desc.hidden[i]) for i in range(desc.n_hidden)]
+    want_acts = [int(desc.acts[i]) for i in range(desc.n_hidden)]
+    if (F, hidden, acts) != (int(desc.n_features), want_hidden, want_acts) or out_act != capi.ACT_SIGMOID:
+        raise ValueError("SB_INIT_MODEL %s has %d inputs, hidden layers %s, activations %s; the ModelConfig has %d inputs, "
+                         "hidden layers %s, activations %s" % (saved_model_dir, F, hidden, acts, int(desc.n_features),
+                                                               want_hidden, want_acts))
+    return flat
 
 
 def pass_order(seed: int, task_index: int, global_step: int, n_rows: int) -> np.ndarray:
@@ -586,6 +640,7 @@ def main(_=None, env=None, rng=random) -> int:
     per_batch_update = schedule == 'batch'
     deterministic = deterministic_requested(params)
     shuffle = shuffle_requested(params)
+    fixed_layers, fixed_bias = fixed_layers_requested(params)
     if deterministic and wide_deep:
         raise ValueError("train.params.Deterministic with wide+deep columns: the embedding gradient is scatter-added in no "
                          "fixed order; train the dense model (SELECTED_COLUMN_NUMS) or drop Deterministic")
@@ -661,11 +716,19 @@ def main(_=None, env=None, rng=random) -> int:
     max_rows = max(bounds[i + 1] - bounds[i] for i in range(total_batch))
 
     desc = model(feature_count, model_conf, max_rows)
+    # SB_INIT_MODEL: start from the weights of an earlier run's SavedModel (global_step 0, fresh optimizer state) - what a
+    # FixedLayers run fine-tunes.  A checkpoint in TMP_MODEL_PATH still wins (the restore below).
+    init_flat = None
+    if env.get("SB_INIT_MODEL") and (is_chief or n_workers == 1):
+        init_flat = read_init_model(_Fs.local(env["SB_INIT_MODEL"]), desc)
     rdv = Rendezvous(cluster_spec, task_index, n_workers)
     nccl_id = exchange_nccl_id(rdv)
     trainer = capi.Trainer(desc, device=device, nccl_id=nccl_id, rank=task_index, world=n_workers)
     if deterministic:
         trainer.set_deterministic(True)   # before the peer exchange is set up and before the first step
+    if fixed_layers:
+        trainer.set_fixed_layers(fixed_layers, fixed_bias)   # the same: every rank, before the peer exchange
+        logging.info("FixedLayers %s (FixedBias %s): these layers are not trained" % (fixed_layers, fixed_bias))
     peer = False
     if n_workers > 1 and env.get("SB_EXCHANGE", "p2p") != "nccl":
         peer = enable_peer_exchange(trainer, rdv)
@@ -686,6 +749,8 @@ def main(_=None, env=None, rng=random) -> int:
             _Fs.fetch(tmp_model_path.rstrip("/") + "/model.ckpt", ckpt)
         if os.path.exists(ckpt):                  # MonitoredTrainingSession restores the latest checkpoint (:251-257)
             trainer.load_checkpoint(ckpt)
+        elif init_flat is not None:
+            trainer.set_params(init_flat)
         else:
             trainer.init_xavier(int(env.get("SB_SEED", "0")) or random.SystemRandom().randrange(1, 2 ** 31))
     if n_workers > 1:
