@@ -487,6 +487,15 @@ int sb_debug_exchange(sb_trainer_t* t, int32_t slot_mask, float gscale, int32_t 
 #define SB_DEBUG_XINFO_WORDS 24
 #define SB_DEBUG_XWORK_WORDS 8
 int sb_debug_exchange_layout(sb_trainer_t* t, int32_t* info, int32_t info_cap, int64_t* work, int64_t work_cap, int32_t* n_work);
+/* Test hook of the single-GPU optimizer (csrc/kernels.cuh optimizer_kernel), on a world-1 trainer.  Queue one update
+ * without waiting: the descriptor of the next update (global step + 1 and its lr_t, gradient scale `gscale` (0: 1 / world),
+ * epoch + 1), then the optimizer over the raw gradient buffer - tail = 0: one launch over the whole work table, as
+ * sb_trainer_apply_accumulated and a step without the split tail queue it; tail = 1: the step's split tail (layer 0's
+ * runs on the main stream, the others on the side stream, then the join).  *lr_t_out (nullable) receives lr_t, route
+ * (route_cap bytes) the launches, "+"-joined, each as "optimizer<base|ext>@<main|side>[first run,end run)".  A bad
+ * gscale or tail, or tail = 1 with one hidden layer, is SB_ERR_INVALID; world > 1 is SB_ERR_STATE; both are found before
+ * any device work. */
+int sb_debug_optimizer(sb_trainer_t* t, float gscale, int32_t tail, float* lr_t_out, char* route, int32_t route_cap);
 
 #ifdef __cplusplus
 }

@@ -184,6 +184,7 @@ PROTOTYPES = {
     "sb_debug_exchange": (C.c_int, [_vp, C.c_int32, C.c_float, C.c_int32, C.c_int32, _f32p, _P(C.c_int32), C.c_char_p,
                                     C.c_int32]),
     "sb_debug_exchange_layout": (C.c_int, [_vp, _P(C.c_int32), C.c_int32, _P(C.c_int64), C.c_int64, _P(C.c_int32)]),
+    "sb_debug_optimizer": (C.c_int, [_vp, C.c_float, C.c_int32, _f32p, C.c_char_p, C.c_int32]),
 }
 
 DEBUG_BUF_THETA, DEBUG_BUF_S1, DEBUG_BUF_S2, DEBUG_BUF_GRAD, DEBUG_BUF_SHADOW = 0, 1, 2, 3, 4
@@ -558,6 +559,14 @@ class Trainer:
         check(lib().sb_debug_exchange(self._h, int(slot_mask), float(gscale), int(grid), int(alone), C.byref(lr_t), C.byref(g),
                                       route, 64))
         return float(lr_t.value), int(g.value), route.value.decode()
+
+    def debug_optimizer(self, gscale: float = 0.0, tail: int = 0):
+        """queue one single-GPU optimizer pass over the raw gradient buffer without waiting (tail = 1: the step's split
+        tail; sb_debug_optimizer) -> (lr_t, route)"""
+        lr_t = C.c_float()
+        route = C.create_string_buffer(256)
+        check(lib().sb_debug_optimizer(self._h, float(gscale), int(tail), C.byref(lr_t), route, 256))
+        return float(lr_t.value), route.value.decode()
 
     def debug_exchange_layout(self) -> dict:
         info = (C.c_int32 * DEBUG_XINFO_WORDS)()

@@ -266,17 +266,25 @@ static int enqueue_allreduce(sb_trainer* t, float* buf) {
   return SB_OK;
 }
 
+// route (nullable, sb_debug_optimizer): appends "+"-joined "optimizer<base|ext>@<main|side>[w0,w1)" for the launch
 static int enqueue_optimizer(sb_trainer* t, const StepIn& in, const float* g, int w0 = 0, int w1 = -1, cudaStream_t st = nullptr,
-                             bool publish_scalars = false, bool pdl = false) {
+                             bool publish_scalars = false, bool pdl = false, std::string* route = nullptr) {
   Net& n = t->net;
   if (w1 < 0) w1 = n.n_work;
   if (!st) st = n.stream;
   if (w1 <= w0) return SB_OK;
+  const bool ext = opt_ext(t->hyper.kind);
   // pdl = false: plain dependency (runs after a stream join / on the comm stream)
-  SB_TRY(launch_kernel(opt_ext(t->hyper.kind) ? optimizer_kernel<true> : optimizer_kernel<false>, dim3(static_cast<unsigned>(w1 - w0)), dim3(256), 0, st, pdl, n.work + w0, in.desc, t->hyper,
+  SB_TRY(launch_kernel(ext ? optimizer_kernel<true> : optimizer_kernel<false>, dim3(static_cast<unsigned>(w1 - w0)), dim3(256), 0, st, pdl, n.work + w0, in.desc, t->hyper,
                        n.theta, g, n.s1, n.s2, in.scal, publish_scalars ? t->d_hscal : static_cast<float*>(nullptr),
                        n.next_trace(st == n.stream ? "opt" : "opt_side")));
   n.mark("optimizer");
+  if (route) {
+    char r[64];
+    snprintf(r, sizeof(r), "%soptimizer<%s>@%s[%d,%d)", route->empty() ? "" : "+", ext ? "ext" : "base",
+             st == n.stream ? "main" : "side", w0, w1);
+    *route += r;
+  }
   return SB_OK;
 }
 
@@ -388,6 +396,20 @@ static int join_streams(cudaStream_t to, cudaStream_t from, cudaEvent_t e) {
   SB_CUDA(cudaEventRecord(e, from));
   SB_CUDA(cudaStreamWaitEvent(to, e, 0));
   return SB_OK;
+}
+
+// The single-GPU step's split tail: layer 0's runs on the main stream, PDL-chained behind dW_0 and publishing the step
+// scalars; the other runs on the side stream once the last dA GEMM (ev_da_done, recorded by the caller) no longer reads
+// their shadows; then the main stream joins the side stream.
+static int enqueue_split_tail(sb_trainer* t, const StepIn& in, const float* g, std::string* route = nullptr) {
+  Net& n = t->net;
+  // the layer-0 optimizer publishes the step scalars, or the other layers' one when layer 0 has nothing that trains
+  const bool l0_runs = n.work_end[0] > n.work_begin[0];
+  SB_TRY(enqueue_optimizer(t, in, g, n.work_begin[0], n.work_end[0], n.stream, true, true, route));
+  // the other layers' shadows are read by the dA GEMMs on the main stream: update them only after the last one
+  SB_CUDA(cudaStreamWaitEvent(t->side, t->ev_da_done, 0));
+  SB_TRY(enqueue_optimizer(t, in, g, n.work_end[0], n.n_work, t->side, !l0_runs, false, route));
+  return join_streams(n.stream, t->side, t->ev_join);
 }
 
 // Where dW_1 runs, and the SM budget (grid cap) of dW_0 / dW_1, in a tensor-core step with more than one hidden layer:
@@ -553,15 +575,7 @@ static int enqueue_step_backward(sb_trainer* t, const StepIn& in, int rows, int 
       SB_CUDA(cudaStreamWaitEvent(n.stream, t->ev_x[0], 0));
       return SB_OK;
     }
-    if (split_tail) {
-      // the layer-0 optimizer publishes the step scalars, or the other layers' one when layer 0 has nothing that trains
-      const bool l0_runs = n.work_end[0] > n.work_begin[0];
-      SB_TRY(enqueue_optimizer(t, in, g, n.work_begin[0], n.work_end[0], n.stream, true, true));
-      // the other layers' shadows are read by the dA GEMMs on the main stream: update them only after the last one
-      SB_CUDA(cudaStreamWaitEvent(t->side, t->ev_da_done, 0));
-      SB_TRY(enqueue_optimizer(t, in, g, n.work_end[0], n.n_work, t->side, !l0_runs));
-      return join_streams(n.stream, t->side, t->ev_join);
-    }
+    if (split_tail) return enqueue_split_tail(t, in, g);
     if (side_used) SB_TRY(join_streams(n.stream, t->side, t->ev_join));
   }
   if (kind == G_STEP) {
@@ -2092,6 +2106,35 @@ int sb_debug_exchange(sb_trainer_t* t, int32_t slot_mask, float gscale, int32_t 
   if (lr_t_out) *lr_t_out = lr_t;
   if (grid_out) *grid_out = grid;
   if (route_cap > 0) snprintf(route, static_cast<size_t>(route_cap), "%s", n.last_kernel ? n.last_kernel : "");
+  return SB_OK;
+}
+
+int sb_debug_optimizer(sb_trainer_t* t, float gscale, int32_t tail, float* lr_t_out, char* route, int32_t route_cap) {
+  SB_CHECK(t, SB_ERR_INVALID, "null trainer");
+  SB_CHECK(std::isfinite(gscale) && gscale >= 0.f, SB_ERR_INVALID, "gscale %g is not a finite value >= 0", gscale);
+  SB_CHECK(tail == 0 || tail == 1, SB_ERR_INVALID, "tail = %d: 0 runs one pass over the work table, 1 the split tail", tail);
+  SB_CHECK(tail == 0 || t->net.L > 1, SB_ERR_INVALID, "the split tail needs two hidden layers (the net has %d)", t->net.L);
+  SB_CHECK(route_cap >= 0 && (route != nullptr || route_cap == 0), SB_ERR_INVALID, "route_cap %d without a buffer", route_cap);
+  SB_CHECK(t->world == 1, SB_ERR_STATE, "world = %d: a peer update is sb_debug_exchange, an NCCL rank needs its communicator",
+           t->world);
+  Net& n = t->net;
+  SB_CUDA(cudaSetDevice(n.device));
+  // as a single-GPU update: the descriptor (step count, lr_t, gradient scale, epoch), then the optimizer as
+  // apply_accumulated and the non-split step queue it (tail = 0) or as the step's split tail (tail = 1)
+  const float lr_t = begin_update(t);
+  const float gs = gscale > 0.f ? gscale : 1.f / static_cast<float>(t->world);
+  const StepIn in = t->slot(t->last_set, 0);    // (as apply_accumulated)
+  SB_TRY(write_desc(n.stream, in, nullptr, lr_t, gs, t->epoch, nullptr));
+  std::string r;
+  if (tail) {
+    SB_CUDA(cudaEventRecord(t->ev_da_done, n.stream));     // no dA GEMM here to record it
+    SB_TRY(enqueue_split_tail(t, in, t->grad, &r));
+  } else {
+    SB_TRY(enqueue_optimizer(t, in, t->grad, 0, -1, nullptr, true, false, &r));
+  }
+  t->grad_out_scale = gs;
+  if (lr_t_out) *lr_t_out = lr_t;
+  if (route_cap > 0) snprintf(route, static_cast<size_t>(route_cap), "%s", r.c_str());
   return SB_OK;
 }
 

@@ -20,48 +20,27 @@ model built here from a Python restatement of xchg_share, not from anything the 
 After the three exchanges get_params() (which gathers the stale masters from the owners) is the owners' theta on every
 rank, and get_grads() the owners' raw gradients times gscale, bit-identical on all ranks.
 
-Bounds for the master and state.  u = 2^-24; every float32 operation rounds once (an FMA once for two), so an
-expression of k operations is within about k u of its terms' magnitudes, and an input error e of a later operand
-propagates with its coefficient.  With S the sum of the magnitudes of an expression's terms the check is
-|got - ref| <= C u S, C = 16 (at least twice the operation count of the longest chain below):
-  SGD        theta' = theta - lr g                               S_t = |theta| + lr |g|
-  Momentum   s1' = s1 m + g                                      S_1 = |s1| m + |g|
-             theta' = theta - lr s1'                             S_t = |theta| + lr S_1
-  Adam       s1' = s1 + (g - s1)(1 - b1)                         S_1 = |s1| + (1 - b1)(|g| + |s1|)
-             s2' = s2 + (g g - s2)(1 - b2)                       S_2 = s2 + (1 - b2)(g g + s2)  (<= 3 s2' / b2: no
-                                                                 cancellation, the terms are >= 0)
-             theta' = theta - lr s1' / (sqrt(s2') + eps)         S_t = |theta| + lr S_1 / D + |step| (1 + S_2 / (2 s2'))
-                                                                 (D = sqrt(s2') + eps; sqrt halves s2's relative error)
-  Adadelta   s1' = s1 rho + g g (1 - rho)                        S_1 = s1 rho + g g (1 - rho)
-             upd = sqrt(s2 + eps) / sqrt(s1' + eps) g            S_u = |upd| (1 + S_1 / (2 (s1' + eps)))
-             s2' = s2 rho + upd upd (1 - rho)                    S_2 = s2 rho + 3 upd upd (1 - rho)
-             theta' = theta - upd lr                             S_t = |theta| + lr S_u
-1 - beta is exact in float32 for beta in [1/2, 1] (Sterbenz), so the reference uses the same constants.  The exact case
-(SGD, lr = 2^-4, gscale = 1/4, dyadic theta and gradients with few bits) has no rounding anywhere and must match the
-float64 result bit for bit.
+Bounds for the master and state: tests/opt_ref.py derives them (|got - ref| <= C u S, S the sum of the magnitudes of an
+expression's terms) for every optimizer; FTRL's l1 branch is also checked apart from the bound.  The exact case (SGD,
+lr = 2^-4, gscale = 1/4, dyadic theta and gradients with few bits) has no rounding anywhere and must match the float64
+result bit for bit.
 
 Co-residency: every exchange block of every rank must be resident at once (they spin on each other), and nothing but
 exchange kernels runs here, so W x grid <= SM count is asserted before each launch; W >= 5 runs at most 8 blocks per
 rank.  The kernel each launch ran ("xchg_ll<4>", "xchg_update<16>", ...) is checked against the instantiation the world
-size selects, and the case matrix reaches both kernels at W = 2, 4, 8 and 16."""
+size selects, and the case matrix reaches both kernels at W = 2, 4, 8 and 16 with the reference's four rules
+(<W, false>) and at W = 2 and 3 (U = 2 and U = 1 update loops) with Adagrad, RMSProp and FTRL (<W, true>)."""
 import ctypes as C
-import math
 import zlib
 
 import numpy as np
 import pytest
 
-from conftest import bf16_round
-
-FP32, BF16, FP32_TC, BF16X2 = 0, 1, 2, 3
-PNAME = {FP32: "fp32", BF16: "bf16", FP32_TC: "fp32_tc", BF16X2: "bf16x2"}
-NPARTS = {FP32: 1, BF16: 1, FP32_TC: 3, BF16X2: 2}
-ADADELTA, ADAM, SGD, MOMENTUM = 0, 1, 2, 3
-ONAME = {ADADELTA: "adadelta", ADAM: "adam", SGD: "sgd", MOMENTUM: "momentum"}
-U = 2.0 ** -24
-C_BOUND = 16.0
-RHO, EPS, BETA1, BETA2, MOM = 0.95, 1e-8, 0.9, 0.999, 0.9
+from opt_ref import (ADADELTA, ADAGRAD, ADAM, BETA1, BETA2, BF16, BF16X2, C_BOUND, EPS, EXT, FP32, FP32_TC, FTRL, MOM,
+                     MOMENTUM, NPARTS, ONAME, PNAME, RHO, RMSPROP, SGD, U, _bits_equal, check_l1_branch, lr_t_of, reference,
+                     s1_start, shadow_bits, uses_s1, uses_s2)
 TIMEOUT_S = "5"
+FTRL_L1, FTRL_L2 = 0.5, 0.25
 
 # nets (features, hidden widths): the layouts of the work runs
 NETS = {
@@ -70,6 +49,8 @@ NETS = {
     "chunk": (600, [24, 40]),        # tensor-core modes: layer 0 in two row-chunk slots (in >= 512, out % 8 == 0)
     "tiny": (8, [8]),                # slot 0 = 1 run, slot 1 = 2 runs: most ranks own nothing
 }
+
+LR = {SGD: 0.05, MOMENTUM: 0.05, ADAM: 0.003, ADADELTA: 1.0, ADAGRAD: 0.05, RMSPROP: 0.003, FTRL: 0.05}
 
 _worst = {}
 
@@ -119,61 +100,6 @@ def predicted_grid(lay, W, mask, alone):
     return max(1, min(grid, want))
 
 
-def shadow_bits(theta, part):
-    """bf16 bits of bf16_residual(theta, part), round to nearest even"""
-    x = np.asarray(theta, np.float32).copy()
-    for _ in range(part):
-        x = (x - bf16_round(x)).astype(np.float32)
-    return (bf16_round(x).view(np.uint32) >> 16).astype(np.uint16)
-
-
-def reference(kind, lr, th, a, b, g):
-    """float64 opt_update on float32 inputs -> (theta', s1', s2', S_t, S_1, S_2)"""
-    th, a, b, g = (np.asarray(v, np.float64) for v in (th, a, b, g))
-    lr = float(lr)
-    f = lambda v: float(np.float32(v))
-    rho, eps, b1, b2, m = f(RHO), f(EPS), f(BETA1), f(BETA2), f(MOM)
-    zero = np.zeros_like(th)
-    if kind == SGD:
-        return th - lr * g, a, b, np.abs(th) + lr * np.abs(g), zero, zero
-    if kind == MOMENTUM:
-        a2 = a * m + g
-        S1 = np.abs(a) * m + np.abs(g)
-        return th - lr * a2, a2, b, np.abs(th) + lr * S1, S1, zero
-    if kind == ADAM:
-        a2 = a + (g - a) * (1 - b1)
-        b2_ = b + (g * g - b) * (1 - b2)
-        S1 = np.abs(a) + (1 - b1) * (np.abs(g) + np.abs(a))
-        S2 = b + (1 - b2) * (g * g + b)
-        D = np.sqrt(b2_) + eps
-        step = lr * a2 / D
-        rel2 = np.divide(S2, 2 * b2_, out=np.zeros_like(S2), where=b2_ > 0)
-        return th - step, a2, b2_, np.abs(th) + lr * S1 / D + np.abs(step) * (1 + rel2), S1, S2
-    a2 = a * rho + g * g * (1 - rho)
-    S1 = a * rho + g * g * (1 - rho)
-    upd = np.sqrt(b + eps) / np.sqrt(a2 + eps) * g
-    Su = np.abs(upd) * (1 + S1 / (2 * (a2 + eps)))
-    b2_ = b * rho + upd * upd * (1 - rho)
-    S2 = b * rho + 3 * upd * upd * (1 - rho)
-    return th - upd * lr, a2, b2_, np.abs(th) + lr * Su, S1, S2
-
-
-def lr_t_of(kind, lr, step):
-    if kind != ADAM:
-        return float(np.float32(lr))
-    b1, b2 = float(np.float32(BETA1)), float(np.float32(BETA2))
-    return float(np.float32(lr)) * math.sqrt(1 - b2 ** step) / (1 - b1 ** step)
-
-
-def _bits_equal(got, want, what):
-    g, w = np.asarray(got), np.asarray(want)
-    gv = g.view(np.uint32 if g.dtype == np.float32 else np.uint16)
-    wv = w.view(np.uint32 if w.dtype == np.float32 else np.uint16)
-    bad = np.flatnonzero(gv.reshape(-1) != wv.reshape(-1))
-    assert bad.size == 0, "%s: %d elements differ, first at %s: got %r want %r" % (
-        what, bad.size, bad[:8], g.reshape(-1)[bad[:8]], w.reshape(-1)[bad[:8]])
-
-
 class Replicas:
     """W trainers on device 0 joined by their peer tables, their raw buffers and the model of what they must hold"""
 
@@ -182,7 +108,11 @@ class Replicas:
         acts = [sb.ACT_RELU] * len(hidden)
         desc = sb.make_desc(F, hidden, acts, optimizer=kind, learning_rate=lr, rho=RHO, epsilon=EPS, beta1=BETA1, beta2=BETA2,
                             momentum=MOM, max_batch=8, precision=prec)
-        self.ts = [sb.Trainer(desc, device=0, nccl_id=None, rank=r, world=W) for r in range(W)]
+        # FTRL runs with both penalties on (and Adagrad / FTRL with a non-default start accumulator, which the raw s1
+        # written below replaces)
+        self.l1, self.l2 = (FTRL_L1, FTRL_L2) if kind == FTRL else (0.0, 0.0)
+        kw = dict(initial_accumulator=0.25, l1=self.l1, l2=self.l2) if kind in (ADAGRAD, FTRL) else {}
+        self.ts = [sb.Trainer(desc, device=0, nccl_id=None, rank=r, world=W, **kw) for r in range(W)]
         bases = [t.exchange_base for t in self.ts]
         for t in self.ts:
             t.set_peer_pointers(bases)
@@ -201,8 +131,7 @@ class Replicas:
         else:
             self.theta = [(rng.standard_normal(self.n) * 0.5).astype(np.float32) for _ in range(W)]
         sq = kind in (ADAM, ADADELTA)           # squared-gradient accumulators are >= 0
-        self.s1 = [(np.abs(v) if kind == ADADELTA else v).astype(np.float32)
-                   for v in (rng.standard_normal(self.n) * 0.1 for _ in range(W))]
+        self.s1 = [s1_start(kind, v) for v in (rng.standard_normal(self.n) * 0.1 for _ in range(W))]
         self.s2 = [(np.abs(rng.standard_normal(self.n)) * 0.01 if sq else rng.standard_normal(self.n)).astype(np.float32)
                    for _ in range(W)]
         self.shadow = [[np.full((self.np, i, -(-o // 8) * 8), 0x7FA0 + r, np.uint16) for (i, o) in self.dims] for r in range(W)]
@@ -258,7 +187,7 @@ class Replicas:
         exp_2 = [v.copy() for v in self.s2]
         exp_g = [v.copy() for v in self.grad]
         exp_sh = [[v.copy() for v in sh] for sh in self.shadow]
-        use1, use2 = self.kind != SGD, self.kind in (ADAM, ADADELTA)
+        use1, use2 = uses_s1(self.kind), uses_s2(self.kind)
         for s in range(self.lay["slots"]):
             if not (mask >> s) & 1:
                 continue
@@ -275,7 +204,8 @@ class Replicas:
                 _bits_equal(got[o][3][idx], acc, "reduced gradient of " + where)
                 exp_g[o][idx] = acc
                 g = (acc * gs).astype(np.float32)
-                rt, r1, r2, St, S1, S2 = reference(self.kind, lr_t, self.theta[o][idx], self.s1[o][idx], self.s2[o][idx], g)
+                rt, r1, r2, St, S1, S2 = reference(self.kind, lr_t, self.theta[o][idx], self.s1[o][idx], self.s2[o][idx], g,
+                                                   self.l1, self.l2)
                 gt, g1, g2 = got[o][0][idx], got[o][1][idx], got[o][2][idx]
                 if self.exact:
                     _bits_equal(gt, rt.astype(np.float32), "exact theta of " + where)
@@ -285,8 +215,9 @@ class Replicas:
                         continue
                     err = np.abs(gv.astype(np.float64) - rv)
                     tol = C_BOUND * U * S + 1e-45
-                    _note(name, err, tol)
+                    _note("%s %s" % (ONAME[self.kind], name), err, tol)
                     assert np.all(err <= tol), "%s of %s: worst error / bound %.3g" % (name, where, float(np.max(err / tol)))
+                check_l1_branch(self.kind, gt, r2, S2, self.l1, "theta of " + where)
                 exp_t[o][idx] = gt
                 if use1:
                     exp_1[o][idx] = g1
@@ -384,6 +315,10 @@ def _cases():
         out.append((16, prec, MOMENTUM, "tiny", "each", -2, 0.0, False))
     for W, prec, net in ((3, FP32, "odd"), (5, BF16, "m8"), (2, FP32_TC, "odd"), (16, BF16, "odd")):   # no rounding anywhere
         out.append((W, prec, SGD, net, "all", 0 if W <= 4 else -2, 0.25, True))
+    for opt in EXT:                                             # the <W, true> instantiations: U = 2 and U = 1, both protocols
+        for W, prec, net, plan in ((2, BF16, "m8", "all"), (3, BF16, "odd", "each"), (2, FP32, "odd", "each"),
+                                   (3, FP32, "m8", "all"), (3, FP32_TC, "odd", "all"), (2, BF16X2, "m8", "step")):
+            out.append((W, prec, opt, net, plan, 0, 0.0, False))
     return list(dict.fromkeys(out))
 
 
@@ -403,7 +338,7 @@ def test_exchange_against_float64(sb, monkeypatch, case):
     W, prec, opt, net, plan, grid, gscale, exact = case
     monkeypatch.setenv("SB_XCHG_TIMEOUT_S", TIMEOUT_S)
     monkeypatch.delenv("SB_XCHG_BLOCKS", raising=False)
-    lr = 2.0 ** -4 if exact else {SGD: 0.05, MOMENTUM: 0.05, ADAM: 0.003, ADADELTA: 1.0}[opt]
+    lr = 2.0 ** -4 if exact else LR[opt]
     reps = Replicas(sb, W, prec, net, opt, lr, seed=zlib.crc32(_id(case).encode()), exact=exact)
     try:
         lay = reps.lay
@@ -421,9 +356,12 @@ def test_exchange_against_float64(sb, monkeypatch, case):
 
 
 def test_case_matrix_reaches_every_instantiation():
-    routes = {kernel_name(c[0], c[1]) for c in CASES}
-    want = {"xchg_%s<%d>" % (k, w) for k in ("ll", "update") for w in (2, 4, 8, 16)}
+    # kernel_name names both optimizer groups alike: <W, false> for the reference's four rules, <W, true> for the others
+    routes = {(kernel_name(c[0], c[1]), c[2] in EXT) for c in CASES}
+    want = {("xchg_%s<%d>" % (k, w), False) for k in ("ll", "update") for w in (2, 4, 8, 16)}
+    want |= {("xchg_%s<%d>" % (k, w), True) for k in ("ll", "update") for w in (2, 4)}
     assert want <= routes, want - routes
+    assert {c[2] for c in CASES} == set(ONAME)
     # every kernel also meets uneven shares, and every split mode a W = 8 exchange
     assert {(c[0], c[1]) for c in CASES} >= {(3, FP32), (3, BF16), (5, FP32), (5, BF16), (8, FP32_TC), (8, BF16X2)}
 
