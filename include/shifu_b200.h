@@ -303,7 +303,9 @@ int sb_debug_model_hold(sb_model_t* m, int32_t k, int32_t timeout_ms);
  * weight column.  Every value is float32(float64(text)) exactly as numpy feeds the reference's fp32 placeholders.
  * Cells the exact fast path declines (> 15-19 significant digits, |exp| > 22, nan/inf, malformed) are NOT written:
  * they are listed in flags[0..min(n_flags, flag_cap)) for the caller to resolve with its own float(); slot -100 marks
- * a line whose number of feature cells / target cell is wrong. */
+ * a line whose number of feature cells / target cell is wrong.  col_map must name every feature index 0 .. n_feat - 1
+ * exactly once, the target exactly once and the weight at most once, with no entry outside [SB_COL_WEIGHT, n_feat);
+ * any other map is SB_ERR_INVALID before any device work (shared by sb_text_parse_device and the host hook). */
 #define SB_COL_SKIP (-1)
 #define SB_COL_TARGET (-2)
 #define SB_COL_WEIGHT (-3)
@@ -463,13 +465,42 @@ int sb_debug_embed(int32_t precision, int32_t scatter, const float* We, const in
  * which = SB_DEBUG_BUF_THETA / _S1 / _S2 / _GRAD: float[n_params] (no gather from the run owners: a non-owner's stale
  * master and state stay visible); SB_DEBUG_BUF_SHADOW + l: the bf16 shadow of hidden layer l as uint16 bits
  * [np, in, ld_out], pad columns out .. ld_out - 1 included (tensor-core modes only, else SB_ERR_STATE).  Writing theta
- * leaves the shadows alone; write = 2 (theta only) also refreshes them.  A wrong length is SB_ERR_INVALID. */
+ * leaves the shadows alone; write = 2 (theta only) also refreshes them.  A wrong length is SB_ERR_INVALID.
+ * The step's input stage (sb_debug_first_kernel), on any trainer:
+ *   SB_DEBUG_BUF_BATCH_X: layer 0's batch operand.  Tensor-core modes: Xb as uint16 bits [np, max_batch, ldx] with
+ *     ldx = round_up(F, 8), or round_up(n_dense, 8) once sb_trainer_set_sparse was called; fp32 mode: Xf [max_batch, F].
+ *   SB_DEBUG_BUF_BATCH_Y / _W: float[max_batch], the labels / weights a step's descriptor points at: ordY / ordW of
+ *     ordered steps while a row order is set, else the host staging buffers (a host step without w reads ones instead).
+ *   SB_DEBUG_BUF_SCAL: float[4], the step scalars of descriptor slot (0, 0) (loss sum, n_nz, 2 unused).
+ *   SB_DEBUG_BUF_DS_X: the resident set: uint16 bits [np, ds_rows, round_up(F, 8)] (tensor-core modes) or float
+ *     [ds_rows, F] (fp32 mode); _DS_Y / _DS_W: float[ds_rows]; _DS_P: int32[ds_rows + 1], the prefix counts of the
+ *     non-zero weights (tensor-core modes only, else SB_ERR_STATE).  Read-only; without a loaded set SB_ERR_STATE.
+ * A bad id, a write to a read-only id and a bad write mode are SB_ERR_INVALID before the trainer is looked at. */
 #define SB_DEBUG_BUF_THETA 0
 #define SB_DEBUG_BUF_S1 1
 #define SB_DEBUG_BUF_S2 2
 #define SB_DEBUG_BUF_GRAD 3
 #define SB_DEBUG_BUF_SHADOW 4
+#define SB_DEBUG_BUF_BATCH_X (SB_DEBUG_BUF_SHADOW + SB_MAX_HIDDEN)
+#define SB_DEBUG_BUF_BATCH_Y (SB_DEBUG_BUF_BATCH_X + 1)
+#define SB_DEBUG_BUF_BATCH_W (SB_DEBUG_BUF_BATCH_X + 2)
+#define SB_DEBUG_BUF_SCAL (SB_DEBUG_BUF_BATCH_X + 3)
+#define SB_DEBUG_BUF_DS_X (SB_DEBUG_BUF_BATCH_X + 4)
+#define SB_DEBUG_BUF_DS_Y (SB_DEBUG_BUF_BATCH_X + 5)
+#define SB_DEBUG_BUF_DS_W (SB_DEBUG_BUF_BATCH_X + 6)
+#define SB_DEBUG_BUF_DS_P (SB_DEBUG_BUF_BATCH_X + 7)
 int sb_debug_trainer_buffer(sb_trainer_t* t, int32_t which, void* host, int64_t n, int32_t write);
+/* Queue what a step queues before layer 0, and wait for it: the batch's descriptor into slot (0, 0), then the step's first
+ * kernel (enqueue_first), which clears the gradient buffer [0, n_params) when clear = 1.
+ *   X != NULL: host rows, staged as sb_trainer_step stages them (X [rows, F], y, w nullable), or on a sparse trainer as
+ *              sb_trainer_step_sparse does (X = the dense block [rows, n_dense], idx [rows, n_cat]);
+ *   X == NULL: rows [row_offset, row_offset + rows) of the resident set, as a resident step reads them (through the row
+ *              order if one is set); y, w and idx must be NULL.
+ * route (route_cap bytes) receives the kernels launched, "+"-joined: "load_batch<bf16>", "load_batch<fp32>",
+ * "gather_batch<bf16>", "gather_batch<fp32>" (a sparse step's load is followed by "+embed_gather"), or "none" for a
+ * bf16-resident batch, whose descriptor write publishes n_nz and layer 0 reads the set in place.  Changes neither the step count nor any captured step.  Read the results with sb_debug_trainer_buffer. */
+int sb_debug_first_kernel(sb_trainer_t* t, const float* X, const float* y, const float* w, const int32_t* idx, int64_t row_offset,
+                          int32_t rows, int32_t clear, char* route, int32_t route_cap);
 /* Queue one exchange of the slots in slot_mask exactly as a step does, and return without waiting: the descriptor of
  * the next update (global step + 1 and its lr_t, gradient scale `gscale` (0: 1 / world), epoch + 1), then the step's
  * exchange launch on the trainer's stream - its slot and work tables, grid rule (alone: as the last launch of a step)

@@ -181,6 +181,8 @@ PROTOTYPES = {
     "sb_debug_embed": (C.c_int, [C.c_int32, C.c_int32, _f32p, _P(C.c_int32), _f32p, _f32p, _P(C.c_int32), C.c_int32, C.c_int32,
                                  C.c_int32, C.c_int32, C.c_int]),
     "sb_debug_trainer_buffer": (C.c_int, [_vp, C.c_int32, _vp, C.c_int64, C.c_int32]),
+    "sb_debug_first_kernel": (C.c_int, [_vp, _f32p, _f32p, _f32p, _P(C.c_int32), C.c_int64, C.c_int32, C.c_int32, C.c_char_p,
+                                        C.c_int32]),
     "sb_debug_exchange": (C.c_int, [_vp, C.c_int32, C.c_float, C.c_int32, C.c_int32, _f32p, _P(C.c_int32), C.c_char_p,
                                     C.c_int32]),
     "sb_debug_exchange_layout": (C.c_int, [_vp, _P(C.c_int32), C.c_int32, _P(C.c_int64), C.c_int64, _P(C.c_int32)]),
@@ -188,6 +190,12 @@ PROTOTYPES = {
 }
 
 DEBUG_BUF_THETA, DEBUG_BUF_S1, DEBUG_BUF_S2, DEBUG_BUF_GRAD, DEBUG_BUF_SHADOW = 0, 1, 2, 3, 4
+# the step's input stage (sb_debug_first_kernel): batch operand, its y / w, slot (0, 0)'s scalars; the resident set (read-only)
+DEBUG_BUF_BATCH_X = DEBUG_BUF_SHADOW + SB_MAX_HIDDEN
+DEBUG_BUF_BATCH_Y, DEBUG_BUF_BATCH_W, DEBUG_BUF_SCAL = DEBUG_BUF_BATCH_X + 1, DEBUG_BUF_BATCH_X + 2, DEBUG_BUF_BATCH_X + 3
+DEBUG_BUF_DS_X, DEBUG_BUF_DS_Y, DEBUG_BUF_DS_W, DEBUG_BUF_DS_P = (DEBUG_BUF_BATCH_X + 4, DEBUG_BUF_BATCH_X + 5, DEBUG_BUF_BATCH_X + 6,
+                                                                  DEBUG_BUF_BATCH_X + 7)
+SCAL_LOSS_SUM, SCAL_NNZ, SCAL_COUNT = 0, 1, 4
 DEBUG_XINFO_WORDS, DEBUG_XWORK_WORDS = 24, 8
 DEBUG_MSTAT_WORDS = 6
 SMALL_ROWS = 128        # score_rows.cuh: an fp32 model scores batches of up to this many rows in one launch
@@ -538,12 +546,21 @@ class Trainer:
         return names.value.decode().split(","), buf[:k.value].copy()
 
     # ---- exchange test hooks (sb_debug_trainer_buffer / sb_debug_exchange / sb_debug_exchange_layout) ----
+    def debug_buffer_dtype(self, which: int):
+        """element type of buffer `which` of debug_buffer"""
+        if which in (DEBUG_BUF_BATCH_X, DEBUG_BUF_DS_X):
+            return np.float32 if self.desc.precision == PREC_FP32 else np.uint16
+        if which == DEBUG_BUF_DS_P:
+            return np.int32
+        return np.float32 if which < DEBUG_BUF_SHADOW or which >= DEBUG_BUF_BATCH_X else np.uint16
+
     def debug_buffer(self, which: int, value: Optional[np.ndarray] = None, n: Optional[int] = None,
                      refresh_shadows: bool = False) -> Optional[np.ndarray]:
         """value None: -> a copy of one raw arena buffer (which < DEBUG_BUF_SHADOW: float32 [n_params]; DEBUG_BUF_SHADOW + l:
-        the uint16 bits of hidden layer l's shadow, n values = np * in * ld_out).  Otherwise write `value` (float32 or
-        uint16 as read), refreshing the shadows from theta if asked."""
-        dtype = np.float32 if which < DEBUG_BUF_SHADOW else np.uint16
+        the uint16 bits of hidden layer l's shadow, n values = np * in * ld_out) or input-stage buffer (DEBUG_BUF_BATCH_X ..
+        DEBUG_BUF_DS_P, n values of debug_buffer_dtype; include/shifu_b200.h gives the shapes).  Otherwise write `value`
+        (of the type read), refreshing the shadows from theta if asked."""
+        dtype = self.debug_buffer_dtype(which)
         if value is None:
             out = np.empty(self.n_params if n is None else n, dtype)
             check(lib().sb_debug_trainer_buffer(self._h, which, out.ctypes.data_as(_vp), out.size, 0))
@@ -551,6 +568,27 @@ class Trainer:
         value = np.ascontiguousarray(value, dtype=dtype).reshape(-1)
         check(lib().sb_debug_trainer_buffer(self._h, which, value.ctypes.data_as(_vp), value.size, 2 if refresh_shadows else 1))
         return None
+
+    def debug_first_kernel(self, X=None, y=None, w=None, idx=None, row_offset: int = 0, rows: Optional[int] = None,
+                           clear: bool = False) -> str:
+        """what a step queues before layer 0, waited for (sb_debug_first_kernel): host rows X / y / w (idx: the dense block and
+        index matrix of a sparse trainer), or with X None rows [row_offset, row_offset + rows) of the resident set -> the
+        kernel launched ("none" for a bf16-resident batch)"""
+        route = C.create_string_buffer(64)
+        if X is None:
+            check(lib().sb_debug_first_kernel(self._h, None, None, None, None, int(row_offset), int(rows), int(clear), route, 64))
+            return route.value.decode()
+        X, y = _f32(X), _f32(y).reshape(-1)
+        w = None if w is None else _f32(w).reshape(-1)
+        idx_p = None
+        if idx is not None:
+            idx = np.ascontiguousarray(idx, dtype=np.int32)
+            idx_p = idx.ctypes.data_as(_P(C.c_int32))
+        n = X.shape[0] if rows is None else int(rows)
+        if y.size < n or (w is not None and w.size < n) or X.shape[0] < n:
+            raise ValueError("X, y, w hold fewer than rows = %d rows" % n)
+        check(lib().sb_debug_first_kernel(self._h, _ptr(X), _ptr(y), _ptr(w), idx_p, int(row_offset), n, int(clear), route, 64))
+        return route.value.decode()
 
     def debug_exchange(self, slot_mask: int, gscale: float = 0.0, grid: int = 0, alone: bool = False):
         """queue one exchange of the slots in slot_mask as a step does, without waiting -> (lr_t, grid, kernel name)"""

@@ -613,7 +613,7 @@ static int enqueue_gather(sb_trainer* t, const StepIn& in, int rows, float* clea
   const dim3 g(static_cast<unsigned>(blocks));
   if (n.tc()) SB_TRY(launch_kernel(gather_batch_kernel<true>, g, dim3(256), 0, n.stream, true, p));
   else SB_TRY(launch_kernel(gather_batch_kernel<false>, g, dim3(256), 0, n.stream, true, p));
-  n.mark("gather_batch");
+  n.mark(n.tc() ? "gather_batch<bf16>" : "gather_batch<fp32>");
   return SB_OK;
 }
 
@@ -2047,13 +2047,72 @@ int sb_debug_step_trace(sb_trainer_t* t, uint64_t* stamps, int32_t cap_kernels, 
 // ================================================================================================
 // exchange test hooks: a rank's raw arena buffers, one exchange launch as a step queues it, the ownership tables
 // ================================================================================================
+// The input-stage buffers of sb_debug_trainer_buffer (SB_DEBUG_BUF_BATCH_X .. _DS_P): one device range per part, laid
+// out one behind the other on the host
+static int input_buffer(sb_trainer* t, int which, void* host, int64_t count, bool write) {
+  Net& n = t->net;
+  struct Range { void* dev; long long elems; };
+  std::vector<Range> rs;
+  size_t esz = sizeof(float);
+  const bool bf = n.tc();
+  const bool resident = which >= SB_DEBUG_BUF_DS_X;
+  SB_CHECK(!resident || t->ds_rows > 0, SB_ERR_STATE, "buffer %d: no resident dataset loaded", which);
+  const long long ds = t->ds_rows;
+  switch (which) {
+    case SB_DEBUG_BUF_BATCH_X:
+      if (bf) {
+        const int ldx = n.n_cat > 0 ? n.ldD : n.ldF;
+        esz = sizeof(uint16_t);
+        for (int k = 0; k < n.nparts; ++k) rs.push_back({n.Xb + k * n.Xb_ps, static_cast<long long>(n.max_batch) * ldx});
+      } else {
+        rs.push_back({n.Xf, static_cast<long long>(n.max_batch) * n.F});
+      }
+      break;
+    case SB_DEBUG_BUF_BATCH_Y: rs.push_back({t->ord_n > 0 ? t->ordY : n.stY, n.max_batch}); break;
+    case SB_DEBUG_BUF_BATCH_W: rs.push_back({t->ord_n > 0 ? t->ordW : n.stW, n.max_batch}); break;
+    case SB_DEBUG_BUF_SCAL: rs.push_back({t->slot(0, 0).scal, SCAL_COUNT}); break;
+    case SB_DEBUG_BUF_DS_X:
+      if (bf) {
+        esz = sizeof(uint16_t);
+        for (int k = 0; k < n.nparts; ++k) rs.push_back({t->dsXb + k * n.resident_ps, ds * n.ldF});
+      } else {
+        rs.push_back({t->dsX, ds * n.F});
+      }
+      break;
+    case SB_DEBUG_BUF_DS_Y: rs.push_back({t->dsY, ds}); break;
+    case SB_DEBUG_BUF_DS_W: rs.push_back({t->dsW, ds}); break;
+    default:   // SB_DEBUG_BUF_DS_P
+      SB_CHECK(t->dsP, SB_ERR_STATE, "buffer %d: the fp32 resident set has no prefix counts", which);
+      esz = sizeof(int);
+      rs.push_back({t->dsP, ds + 1});
+  }
+  long long total = 0;
+  for (const Range& r : rs) total += r.elems;
+  SB_CHECK(count == total, SB_ERR_INVALID, "buffer %d: expected %lld values, got %lld", which, total, (long long)count);
+  SB_CUDA(cudaSetDevice(n.device));
+  SB_CUDA(cudaStreamSynchronize(n.stream));
+  char* h = static_cast<char*>(host);
+  for (const Range& r : rs) {
+    const size_t bytes = esz * static_cast<size_t>(r.elems);
+    if (write) SB_CUDA(cudaMemcpyAsync(r.dev, h, bytes, cudaMemcpyHostToDevice, n.stream));
+    else SB_CUDA(cudaMemcpyAsync(h, r.dev, bytes, cudaMemcpyDeviceToHost, n.stream));
+    h += bytes;
+  }
+  SB_CUDA(cudaStreamSynchronize(n.stream));
+  return SB_OK;
+}
+
 int sb_debug_trainer_buffer(sb_trainer_t* t, int32_t which, void* host, int64_t n, int32_t write) {
-  SB_CHECK(t && host, SB_ERR_INVALID, "null argument");
-  Net& net = t->net;
-  SB_CHECK(which >= SB_DEBUG_BUF_THETA && which < SB_DEBUG_BUF_SHADOW + net.L, SB_ERR_INVALID,
-           "buffer %d outside [0, %d)", which, SB_DEBUG_BUF_SHADOW + net.L);
+  const bool input = which >= SB_DEBUG_BUF_BATCH_X && which <= SB_DEBUG_BUF_DS_P;
+  SB_CHECK((which >= SB_DEBUG_BUF_THETA && which < SB_DEBUG_BUF_SHADOW + SB_MAX_HIDDEN) || input, SB_ERR_INVALID,
+           "buffer %d is not a buffer id", which);
   SB_CHECK(write >= 0 && write <= 2 && (write != 2 || which == SB_DEBUG_BUF_THETA), SB_ERR_INVALID,
            "write = %d: 0 reads, 1 writes, 2 writes theta and refreshes the shadows", write);
+  SB_CHECK(write == 0 || which < SB_DEBUG_BUF_DS_X, SB_ERR_INVALID, "buffer %d (the resident set) is read-only", which);
+  SB_CHECK(t && host, SB_ERR_INVALID, "null argument");
+  Net& net = t->net;
+  if (input) return input_buffer(t, which, host, n, write != 0);
+  SB_CHECK(which < SB_DEBUG_BUF_SHADOW + net.L, SB_ERR_INVALID, "buffer %d outside [0, %d)", which, SB_DEBUG_BUF_SHADOW + net.L);
   if (which < SB_DEBUG_BUF_SHADOW) {
     SB_CHECK(n == net.n_params, SB_ERR_INVALID, "expected %lld floats, got %lld", (long long)net.n_params, (long long)n);
     float* dev = which == SB_DEBUG_BUF_THETA ? net.theta : which == SB_DEBUG_BUF_S1 ? net.s1 : which == SB_DEBUG_BUF_S2 ? net.s2 : t->grad;
@@ -2079,6 +2138,42 @@ int sb_debug_trainer_buffer(sb_trainer_t* t, int32_t which, void* host, int64_t 
     }
   }
   SB_CUDA(cudaStreamSynchronize(net.stream));
+  return SB_OK;
+}
+
+int sb_debug_first_kernel(sb_trainer_t* t, const float* X, const float* y, const float* w, const int32_t* idx, int64_t row_offset,
+                          int32_t rows, int32_t clear, char* route, int32_t route_cap) {
+  SB_CHECK(clear == 0 || clear == 1, SB_ERR_INVALID, "clear = %d: 0 or 1", clear);
+  SB_CHECK(route_cap >= 0 && (route != nullptr || route_cap == 0), SB_ERR_INVALID, "route_cap %d without a buffer", route_cap);
+  SB_CHECK(X != nullptr || (y == nullptr && w == nullptr && idx == nullptr), SB_ERR_INVALID,
+           "resident rows (X null) take no y, w or idx");
+  SB_CHECK(X == nullptr || (y != nullptr && row_offset == 0), SB_ERR_INVALID, "host rows need y and take no row_offset");
+  SB_CHECK(t, SB_ERR_INVALID, "null trainer");
+  Net& n = t->net;
+  Batch b;
+  if (X == nullptr) {
+    SB_TRY(resident_batch(t, row_offset, rows, -1, &b));
+  } else if (n.n_cat > 0) {   // as sb_trainer_step_sparse
+    SB_TRY(stage_sparse_batch(n, X, idx, y, w, rows));
+    b = host_batch(n, n.stX, n.stY, w ? n.stW : nullptr, rows, Feed::SPARSE);
+  } else {                    // as sb_trainer_step
+    SB_CHECK(idx == nullptr, SB_ERR_INVALID, "idx on a trainer without sb_trainer_set_sparse");
+    SB_TRY(stage_host_batch(t, X, y, w, rows));
+    b = host_batch(n, n.stX, n.stY, w ? n.stW : nullptr, rows);
+  }
+  SB_CUDA(cudaSetDevice(n.device));
+  // as run_step for a batch it does not prefetch: set 0 written on the main stream, then what enqueue_step_body queues
+  // ahead of layer 0
+  const StepIn in = t->slot(0, 0, b.feed);
+  t->have_pos = false;
+  SB_TRY(write_desc(n.stream, in, &b, t->lr, 1.f / static_cast<float>(t->world), t->epoch, nullptr));
+  std::string r;
+  n.marks = &r;
+  const int s = enqueue_first(n, t, in, b.rows, clear ? t->grad : nullptr, clear ? n.n_params : 0);
+  n.marks = nullptr;
+  SB_TRY(s);
+  SB_CUDA(cudaStreamSynchronize(n.stream));
+  if (route_cap > 0) snprintf(route, static_cast<size_t>(route_cap), "%s", r.empty() ? "none" : r.c_str());
   return SB_OK;
 }
 

@@ -431,7 +431,7 @@ int Net::enqueue_load(const StepIn& in, int rows, float* clear, long long clear_
     SB_TRY(launch_kernel(load_batch_kernel<false>, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, stream, true,
                          static_cast<const BatchDesc*>(in.desc), rows, Fx, static_cast<__nv_bfloat16*>(nullptr), ldx, Xf, in.scal,
                          clear, clear_n, 1, 0ll));
-  mark("load_batch");
+  mark(tc() ? "load_batch<bf16>" : "load_batch<fp32>");
   if (in.feed == Feed::SPARSE) SB_TRY(enqueue_embed(rows, false, nullptr, stream));
   return SB_OK;
 }

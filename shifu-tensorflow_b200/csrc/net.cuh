@@ -106,7 +106,11 @@ struct Net {
   }
   // every launch of an enqueue_* routine: `kernel` names the kernel and tile it launched (sb_debug_gemm_layer reports it)
   const char* last_kernel = nullptr;
-  void mark(const char* kernel) { ++launches; last_kernel = kernel; }
+  std::string* marks = nullptr;   // non-null: every launch's name is appended, "+"-joined (sb_debug_first_kernel)
+  void mark(const char* kernel) {
+    ++launches; last_kernel = kernel;
+    if (marks) { if (!marks->empty()) *marks += '+'; *marks += kernel; }
+  }
 
   std::vector<void*> allocs;
   template <typename T> int dalloc(T** p, size_t n) {

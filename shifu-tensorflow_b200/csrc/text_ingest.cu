@@ -181,6 +181,28 @@ static int check_args(const char* text, int64_t n_bytes, const int32_t* col_map,
   SB_CHECK(text && col_map && X && y && w && n_rows_out && n_flags_out, SB_ERR_INVALID, "null argument");
   SB_CHECK(n_bytes > 0 && n_map > 0 && n_feat > 0, SB_ERR_INVALID, "empty input");
   SB_CHECK(text[n_bytes - 1] == '\n', SB_ERR_INVALID, "text must end with a newline");
+  // parse_line stores a feature cell at X[row * n_feat + role] unchecked: every role must name a column of X, and each
+  // column exactly once (a repeated index would leave another column silently 0 with no line flagged)
+  SB_CHECK(n_feat <= n_map, SB_ERR_INVALID, "col_map has %d entries, fewer than n_feat=%d features", n_map, n_feat);
+  std::vector<char> seen(static_cast<size_t>(n_feat), 0);
+  int n_seen = 0, n_target = 0, n_weight = 0;
+  for (int32_t c = 0; c < n_map; ++c) {
+    const int32_t r = col_map[c];
+    SB_CHECK(r >= SB_COL_WEIGHT && r < n_feat, SB_ERR_INVALID, "col_map[%d] = %d outside [%d, n_feat=%d)", c, r, SB_COL_WEIGHT,
+             n_feat);
+    if (r >= 0) {
+      SB_CHECK(!seen[static_cast<size_t>(r)], SB_ERR_INVALID, "col_map[%d]: feature %d is mapped twice", c, r);
+      seen[static_cast<size_t>(r)] = 1;
+      ++n_seen;
+    } else if (r == SB_COL_TARGET) {
+      ++n_target;
+    } else if (r == SB_COL_WEIGHT) {
+      ++n_weight;
+    }
+  }
+  SB_CHECK(n_seen == n_feat, SB_ERR_INVALID, "col_map maps %d of n_feat=%d features", n_seen, n_feat);
+  SB_CHECK(n_target == 1, SB_ERR_INVALID, "col_map has %d target columns, needs exactly one", n_target);
+  SB_CHECK(n_weight <= 1, SB_ERR_INVALID, "col_map has %d weight columns, at most one", n_weight);
   return SB_OK;
 }
 

@@ -327,9 +327,12 @@ def load_data_gpu(data_file: str, feature_column_nums: Optional[List[int]], targ
         col_map[sample_weight_column_num] = capi.COL_WEIGHT
     n_feat = len(feature_column_nums)
     X, y, w, flags, text, _kernel_ms = capi.text_parse_device(text, col_map, n_feat, DELIMITER, device=device)
+    # a line without the selected columns is reported by number before any of its cells is resolved (an empty line also
+    # flags its empty target cell, and the flags arrive in no fixed order)
+    bad = [row for row, slot, _, _ in flags if slot == -100]
+    if bad:
+        raise ValueError("line %d does not have the selected columns" % min(bad))
     for row, slot, off, ln in flags:
-        if slot == -100:
-            raise ValueError("line %d does not have the selected columns" % row)
         cell = text[off:off + ln].decode('utf-8')
         v = float(cell.strip('\n'))        # ValueError here = the cell the reference would log and skip
         if slot >= 0:

@@ -157,3 +157,236 @@ def test_device_resident_set_feeds_the_trainer_without_a_host_copy(sb):
             assert a.step_resident(k * 128, 128) == b.step_resident(k * 128, 128)
         # (the evaluation loss is summed with fp32 atomics across CTAs: equal up to the summation order)
         assert abs(a.eval_loss(Xh, yh, wh) - b.eval_loss(Xd, yd, wd)) <= 1e-6
+
+
+# ---------------------------------------------------------------------------------------------------- col_map validation
+# parse_line stores a feature cell at X[row * n_feat + role] without a check of its own, so every map is checked before
+# anything is parsed: on the host hook, sb_text_parse and sb_text_parse_device alike (a CPU-only machine reaches the check
+# before the device lookup).
+T, W, S = -2, -3, -1
+BAD_MAPS = {
+    "feature_past_n_feat": ([T, 0, 1, 3], 3, "outside"),
+    "feature_at_n_feat": ([T, 0, 1, 2, 3], 3, "outside"),
+    "below_weight": ([T, 0, 1, -4], 2, "outside"),
+    "repeated_feature": ([T, 0, 1, 1, 2], 3, "mapped twice"),
+    "fewer_features": ([T, 0, 1, S], 3, "maps 2 of n_feat=3"),
+    "map_shorter_than_n_feat": ([T, 0], 3, "fewer than n_feat"),
+    "no_target": ([0, 1, 2, W], 3, "0 target columns"),
+    "two_targets": ([T, 0, 1, 2, T], 3, "2 target columns"),
+    "two_weights": ([T, 0, 1, 2, W, W], 3, "2 weight columns"),
+}
+
+
+def _parse_raw(sb, text, col_map, n_feat, entry):
+    import ctypes as C
+    cm = (C.c_int32 * len(col_map))(*col_map)
+    X, y, w = (np.zeros(64, np.float32) for _ in range(3))
+    flags = (sb.capi.CellFlag * 4)()
+    n_rows, n_flags = C.c_int64(0), C.c_int64(0)
+    lib, p = sb.capi.lib(), sb.capi._ptr
+    if entry == "device":
+        dX, dy, dw = (sb.capi._f32p() for _ in range(3))
+        return lib.sb_text_parse_device(text, len(text), b"|", cm, len(col_map), n_feat, C.byref(dX), C.byref(dy), C.byref(dw),
+                                        C.byref(n_rows), flags, 4, C.byref(n_flags), 0, None)
+    args = [text, len(text), b"|", cm, len(col_map), n_feat, p(X), p(y), p(w), 4, C.byref(n_rows), flags, 4, C.byref(n_flags)]
+    return lib.sb_debug_text_parse_host(*args) if entry == "host" else lib.sb_text_parse(*args, 0)
+
+
+@pytest.mark.parametrize("entry", ["host", "parse", "device"])
+@pytest.mark.parametrize("case", sorted(BAD_MAPS))
+def test_col_map_is_rejected_before_any_parsing(sb, case, entry):
+    col_map, n_feat, msg = BAD_MAPS[case]
+    text = b"1|0.5|0.25|2|3|4|5\n"
+    assert _parse_raw(sb, text, col_map, n_feat, entry) == sb.capi.SB_ERR_INVALID
+    assert msg in sb.capi.lib().sb_last_error().decode()
+
+
+def test_valid_col_maps_still_parse(sb):
+    for col_map, n_feat in (([T, 2, S, 0, 1, W], 3), ([1, 0, T], 2), ([T, 0], 1)):
+        X, y, w, flags, _ = sb.capi.text_parse(b"1|0.5|0.25|2|3|4\n", col_map, n_feat, host_debug=True)
+        assert X.shape == (1, n_feat)
+
+
+# ---------------------------------------------------------------------------------------------------- GPU chunk edges
+CHUNK = 16384
+
+
+def _python_parse(text, col_map, n_feat):
+    """float() per cell: X, y, w and the rows whose feature / target cells are missing"""
+    lines = text.split(b"\n")
+    if lines and lines[-1] == b"":
+        lines = lines[:-1]
+    X = np.zeros((len(lines), n_feat), np.float32)
+    y = np.zeros(len(lines), np.float32)
+    w = np.ones(len(lines), np.float32)
+    bad = []
+    for r, ln in enumerate(lines):
+        cells = ln.split(b"|")
+        seen, tgt = 0, False
+        for c, role in enumerate(col_map):
+            if c >= len(cells) or role == COL_SKIP or cells[c] == b"":
+                continue
+            if role >= 0:
+                X[r, role] = float(cells[c]); seen += 1
+            elif role == COL_TARGET:
+                y[r] = float(cells[c]); tgt = True
+            else:
+                v = float(cells[c])
+                w[r] = 1.0 if v < 0.0 else v
+        if seen != n_feat or not tgt:
+            bad.append(r)
+    return X, y, w, bad
+
+
+COL_SKIP, COL_TARGET, COL_WEIGHT = -1, -2, -3
+
+
+def _resolve(X, y, w, flags, text):
+    X, y, w = X.copy(), y.copy(), w.copy()
+    bad = sorted(row for row, slot, _, _ in flags if slot == -100)
+    for row, slot, off, ln in flags:
+        if row in bad:
+            continue
+        v = float(text[off:off + ln])
+        if slot >= 0:
+            X[row, slot] = v
+        elif slot == COL_TARGET:
+            y[row] = v
+        else:
+            w[row] = 1.0 if v < 0.0 else v
+    return X, y, w, bad
+
+
+def _check_gpu_text(sb, text, col_map, n_feat, want_bad=()):
+    """GPU parse == host hook (bits and sorted flags) == float() per cell, flags resolved; -> the appended text"""
+    Xg, yg, wg, fg, tx = sb.capi.text_parse(text, col_map, n_feat)
+    Xh, yh, wh, fh, _ = sb.capi.text_parse(text, col_map, n_feat, host_debug=True)
+    np.testing.assert_array_equal(Xg.view(np.uint32), Xh.view(np.uint32))
+    np.testing.assert_array_equal(yg.view(np.uint32), yh.view(np.uint32))
+    np.testing.assert_array_equal(wg.view(np.uint32), wh.view(np.uint32))
+    assert sorted(fg) == sorted(fh)
+    X, y, w, bad = _resolve(Xg, yg, wg, fg, tx)
+    Xp, yp, wp, badp = _python_parse(tx, col_map, n_feat)
+    assert bad == badp == sorted(want_bad)
+    ok = np.setdiff1d(np.arange(len(y)), bad)
+    np.testing.assert_array_equal(X[ok].view(np.uint32), Xp[ok].view(np.uint32))
+    np.testing.assert_array_equal(y[ok].view(np.uint32), yp[ok].view(np.uint32))
+    np.testing.assert_array_equal(w.view(np.uint32), wp.view(np.uint32))
+    return tx
+
+
+def _check_load_data_gpu(sb, tmp_path, text, feats, target, weight):
+    from shifu_tensorflow_b200 import trainer as tr
+    p = str(tmp_path / "part.gz")
+    with gzip.open(p, "wb") as f:
+        f.write(text)
+    a = so.load_data([p], feats, target, weight, 0.0, rng=random.Random(1))
+    b = tr.load_data_gpu(p, feats, target, weight, 0.0, rng=random.Random(1))
+    for k in ("train_data", "train_target", "train_data_sample_weight"):
+        got = b[k].numpy()
+        np.testing.assert_array_equal(np.asarray(a[k], np.float32).reshape(got.shape).view(np.uint32), got.view(np.uint32),
+                                      err_msg=k)
+
+
+def _edge_text(rnd, targets, F=3):
+    """lines 'y|f0..f{F-1}|pad|w' whose newlines land exactly at the absolute byte offsets `targets` (the skipped pad
+    column takes up the difference)"""
+    out = b""
+    for pos in targets:
+        head = ("%d|" % rnd.randrange(2) + "|".join("%.6f" % rnd.gauss(0, 1) for _ in range(F)) + "|").encode()
+        tail = ("|%.3f" % rnd.uniform(-1, 3)).encode()
+        pad = pos - len(out) - len(head) - len(tail)
+        assert pad >= 0, (pos, len(out))
+        out += head + b"x" * pad + tail + b"\n"
+        assert len(out) - 1 == pos
+    return out
+
+
+EDGE_MAP = [COL_TARGET, 0, 1, 2, COL_SKIP, COL_WEIGHT]
+
+
+@pytest.mark.gpu
+def test_gpu_cfg2_width_lines_cross_every_chunk(sb, tmp_path):
+    """2000 features at %.6f: ~18 KB lines, longer than a 16 KB chunk, so some chunks hold no newline at all"""
+    F, rows = 2000, 24
+    rng = np.random.RandomState(7)
+    lines = []
+    for i in range(rows):
+        cells = ["%d" % (i & 1)] + ["%.6f" % v for v in rng.randn(F) * 10] + ["%.2f" % (rng.rand() * 4 - 1)]
+        lines.append("|".join(cells))
+    text = ("\n".join(lines) + "\n").encode()
+    assert min(len(l) for l in lines) > CHUNK
+    col_map = [COL_TARGET] + list(range(F)) + [COL_WEIGHT]
+    _check_gpu_text(sb, text, col_map, F)
+    _check_load_data_gpu(sb, tmp_path, text, list(range(1, F + 1)), 0, F + 1)
+
+
+@pytest.mark.gpu
+def test_gpu_newlines_on_chunk_and_window_edges(sb, tmp_path):
+    rnd = random.Random(11)
+    targets = [CHUNK - 1, 2 * CHUNK, 3 * CHUNK + 1, 4 * CHUNK + 64 * 5 - 1, 4 * CHUNK + 64 * 6, 4 * CHUNK + 64 * 7 + 1,
+               5 * CHUNK + 63, 6 * CHUNK - 1]
+    text = _edge_text(rnd, targets)
+    assert len(text) == 6 * CHUNK                              # ends exactly on a chunk boundary
+    _check_gpu_text(sb, text, EDGE_MAP, 3)
+    _check_load_data_gpu(sb, tmp_path, text, [1, 2, 3], 0, 5)
+
+
+@pytest.mark.gpu
+def test_gpu_text_of_exact_chunk_multiple(sb):
+    rnd = random.Random(12)
+    for n in (1, 2):
+        text = _edge_text(rnd, [CHUNK * k // 4 - 1 for k in range(1, 4 * n + 1)])
+        assert len(text) == n * CHUNK
+        _check_gpu_text(sb, text, EDGE_MAP, 3)
+
+
+@pytest.mark.gpu
+def test_gpu_four_byte_lines(sb):
+    """'d|d\\n': 16 lines per 64-byte thread window, 4096 per chunk"""
+    rnd = random.Random(13)
+    text = b"".join(b"%d|%d\n" % (rnd.randrange(2), rnd.randrange(10)) for _ in range(3 * 4096 + 5))
+    assert len(text) == 4 * (3 * 4096 + 5)
+    _check_gpu_text(sb, text, [COL_TARGET, 0], 1)
+
+
+@pytest.mark.gpu
+def test_gpu_crlf_last_line_without_newline_and_weights(sb, tmp_path):
+    """CRLF endings; a last line without '\\n'; a weight column with zeros, -0, negatives (-> 1) and missing (-> 1)"""
+    rnd = random.Random(14)
+    wcells = ["0", "-0", "-2.5", "0.75", "3", None]
+    lines = []
+    for i in range(3000):
+        cells = ["%d" % (i & 1)] + ["%.5f" % rnd.gauss(0, 1) for _ in range(4)]
+        wc = wcells[i % len(wcells)]
+        if wc is not None:
+            cells.append(wc)
+        lines.append("|".join(cells))
+    col_map = [COL_TARGET, 0, 1, 2, 3, COL_WEIGHT]
+    text = "\r\n".join(lines).encode()                       # CRLF, and no newline after the last line
+    tx = _check_gpu_text(sb, text, col_map, 4)
+    assert tx == text + b"\n"
+    _, _, w, _, _ = sb.capi.text_parse(text, col_map, 4)
+    want = np.array([[0.0, -0.0, 1.0, 0.75, 3.0, 1.0][i % 6] for i in range(3000)], np.float32)
+    np.testing.assert_array_equal(w.view(np.uint32), want.view(np.uint32))
+    _check_load_data_gpu(sb, tmp_path, text, [1, 2, 3, 4], 0, 5)
+
+
+@pytest.mark.gpu
+def test_gpu_empty_line_is_flagged_at_its_row(sb, tmp_path):
+    from shifu_tensorflow_b200 import trainer as tr
+    rnd = random.Random(15)
+    lines = ["%d|%.4f|%.4f" % (i & 1, rnd.gauss(0, 1), rnd.gauss(0, 1)) for i in range(900)]
+    lines[517] = ""
+    text = ("\n".join(lines) + "\n").encode()
+    _check_gpu_text(sb, text, [COL_TARGET, 0, 1], 2, want_bad=[517])
+    X, y, w, flags, _ = sb.capi.text_parse(text, [COL_TARGET, 0, 1], 2)
+    assert sorted((f[0], f[1]) for f in flags) == [(517, -100), (517, COL_TARGET)]   # the empty target cell, and the line
+    for r in (516, 518):                                      # the neighbours are intact
+        c = lines[r].split("|")
+        assert (y[r], X[r, 0], X[r, 1]) == (np.float32(float(c[0])), np.float32(float(c[1])), np.float32(float(c[2])))
+    p = str(tmp_path / "part.gz")
+    with gzip.open(p, "wb") as f:
+        f.write(text)
+    with pytest.raises(ValueError, match="line 517 "):
+        tr.load_data_gpu(p, [1, 2], 0, -1, 0.0, rng=random.Random(1))
