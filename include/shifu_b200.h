@@ -57,10 +57,17 @@ typedef enum { SB_LOSS_MSE = 0, SB_LOSS_SIGMOID_CE = 1 } sb_loss;
  *   ADADELTA  accum = 0, accum_update = 0     ADAM     m = 0, v = 0         SGD   -
  *   MOMENTUM  accum = 0                       ADAGRAD  accum = initial_accumulator
  *   RMSPROP   ms = 1 (TF's ones initializer), mom = 0                     FTRL  accum = initial_accumulator, linear = 0
+ *   RPROP     prev = 0, step = learning_rate
  * FTRL sets a parameter to exactly 0 while |linear| <= l1 (also with l1 = 0 and linear = 0, e.g. a zero gradient from
- * the start), as TF does. */
+ * the start), as TF does.
+ * RPROP: resilient propagation in its iRPROP- form (Igel and Huesken), for full-batch gradients such as the
+ * sync_replicas schedule's one update per epoch.  It uses only the sign of each gradient and computes exactly what
+ * torch.optim.Rprop(lr, etas=(0.5, 1.2), step_sizes=(1e-6, 50)) computes, in fp32:
+ *   p = g prev;  step = min(max(step * (p > 0 ? 1.2 : p < 0 ? 0.5 : 1), 1e-6), 50)
+ *   g = p < 0 ? 0 : g;  theta -= sign(g) step  (g = +-0: theta keeps its bits);  prev = g
+ * learning_rate is only the start value of step; the value 7 is not an optimizer. */
 typedef enum { SB_OPT_ADADELTA = 0, SB_OPT_ADAM = 1, SB_OPT_SGD = 2, SB_OPT_MOMENTUM = 3, SB_OPT_ADAGRAD = 4,
-               SB_OPT_RMSPROP = 5, SB_OPT_FTRL = 6 } sb_optimizer;
+               SB_OPT_RMSPROP = 5, SB_OPT_FTRL = 6, SB_OPT_RPROP = 8 } sb_optimizer;
 /* SB_PREC_FP32: fp32 operands and fp32 accumulation end to end (what TF-CPU computes) - parity mode (CUDA cores).
  * SB_PREC_BF16: bf16 operands on the tensor cores (wgmma), fp32 accumulation, fp32 master
  *               weights and optimizer state - performance mode.
@@ -87,7 +94,7 @@ typedef struct {
   int32_t precision;               /* sb_precision                                                     */
 } sb_net_desc;
 /* Optimizer fields each optimizer reads (the others are ignored, whatever they hold):
- *   ADADELTA rho, epsilon    ADAM beta1, beta2, epsilon    SGD -    MOMENTUM momentum
+ *   ADADELTA rho, epsilon    ADAM beta1, beta2, epsilon    SGD -    MOMENTUM momentum    RPROP -
  *   RMSPROP  rho (decay, in [0, 1]), momentum (>= 0), epsilon (>= 0); a value out of range is SB_ERR_INVALID, found
  *            before any device work
  *   ADAGRAD  initial_accumulator, FTRL initial_accumulator, l1, l2: sb_trainer_set_optimizer_params (TF's defaults
@@ -523,7 +530,7 @@ int sb_debug_exchange_layout(sb_trainer_t* t, int32_t* info, int32_t info_cap, i
  * epoch + 1), then the optimizer over the raw gradient buffer - tail = 0: one launch over the whole work table, as
  * sb_trainer_apply_accumulated and a step without the split tail queue it; tail = 1: the step's split tail (layer 0's
  * runs on the main stream, the others on the side stream, then the join).  *lr_t_out (nullable) receives lr_t, route
- * (route_cap bytes) the launches, "+"-joined, each as "optimizer<base|ext>@<main|side>[first run,end run)".  A bad
+ * (route_cap bytes) the launches, "+"-joined, each as "optimizer<base|ext|rprop>@<main|side>[first run,end run)".  A bad
  * gscale or tail, or tail = 1 with one hidden layer, is SB_ERR_INVALID; world > 1 is SB_ERR_STATE; both are found before
  * any device work. */
 int sb_debug_optimizer(sb_trainer_t* t, float gscale, int32_t tail, float* lr_t_out, char* route, int32_t route_cap);

@@ -1,12 +1,12 @@
 """In-graph span and bandwidth of layer 0's optimizer pass (`opt`) and of the other layers' (`opt_side`) on cfg2's shapes,
-for each of the seven optimizers (run on the GPU box).  The span is read from the step trace (SB_STEP_TRACE: %globaltimer
+for each of the eight optimizers (run on the GPU box).  The span is read from the step trace (SB_STEP_TRACE: %globaltimer
 of the kernel's dependency wait to the last block's exit) of several resident steps; bandwidth = the bytes the update
 needs over that span.
 
     python scripts/bench_optimizer.py [out.json]
 
 Bytes per parameter: theta read + write 8, gradient read 4, each state stream read + write 8 (Momentum and Adagrad 1,
-Adam, Adadelta, RMSProp and FTRL 2), bf16 shadow write 2 for the hidden-layer weights."""
+Adam, Adadelta, RMSProp, FTRL and RPROP 2), bf16 shadow write 2 for the hidden-layer weights."""
 import json
 import os
 import sys
@@ -20,8 +20,8 @@ from oracle import tf_optimizers as tfo
 
 B, F, HIDDEN = 8192, 2000, [1024, 512, 256]   # cfg2
 OPTS = {"adadelta": so.OPT_ADADELTA, "adam": so.OPT_ADAM, "sgd": so.OPT_SGD, "momentum": so.OPT_MOMENTUM,
-        "adagrad": tfo.OPT_ADAGRAD, "rmsprop": tfo.OPT_RMSPROP, "ftrl": tfo.OPT_FTRL}
-STATE_STREAMS = {"adadelta": 2, "adam": 2, "sgd": 0, "momentum": 1, "adagrad": 1, "rmsprop": 2, "ftrl": 2}
+        "adagrad": tfo.OPT_ADAGRAD, "rmsprop": tfo.OPT_RMSPROP, "ftrl": tfo.OPT_FTRL, "rprop": sb.OPT_RPROP}
+STATE_STREAMS = {"adadelta": 2, "adam": 2, "sgd": 0, "momentum": 1, "adagrad": 1, "rmsprop": 2, "ftrl": 2, "rprop": 2}
 
 
 def op_bytes(name, n_weights, n_other):

@@ -11,7 +11,7 @@ from . import _capi as capi  # noqa: F401
 from ._capi import (Trainer, Model, NetDesc, make_desc, ShifuB200Error,  # noqa: F401
                     ACT_SIGMOID, ACT_TANH, ACT_RELU, ACT_LEAKYRELU, ACT_NONE,
                     LOSS_MSE, LOSS_SIGMOID_CE, OPT_ADADELTA, OPT_ADAM, OPT_SGD, OPT_MOMENTUM,
-                    OPT_ADAGRAD, OPT_RMSPROP, OPT_FTRL,
+                    OPT_ADAGRAD, OPT_RMSPROP, OPT_FTRL, OPT_RPROP,
                     PREC_FP32, PREC_BF16, PREC_FP32_TC, PREC_BF16X2)
 
 __all__ = ["capi", "Trainer", "Model", "NetDesc", "make_desc", "ShifuB200Error"]

@@ -24,6 +24,7 @@ SB_NCCL_ID_BYTES = 128
 ACT_SIGMOID, ACT_TANH, ACT_RELU, ACT_LEAKYRELU, ACT_NONE = 0, 1, 2, 3, -1
 LOSS_MSE, LOSS_SIGMOID_CE = 0, 1
 OPT_ADADELTA, OPT_ADAM, OPT_SGD, OPT_MOMENTUM, OPT_ADAGRAD, OPT_RMSPROP, OPT_FTRL = 0, 1, 2, 3, 4, 5, 6
+OPT_RPROP = 8                   # iRPROP-: learning_rate is the start step size (7 is not an optimizer)
 # TF 1.x defaults of the hyperparameters make_desc fills in when the caller passes none: RMSPropOptimizer's (decay,
 # epsilon, momentum) differ from the values every other optimizer gets
 _RMSPROP_DEFAULTS = dict(rho=0.9, epsilon=1e-10, momentum=0.0)

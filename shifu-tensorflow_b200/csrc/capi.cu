@@ -266,22 +266,22 @@ static int enqueue_allreduce(sb_trainer* t, float* buf) {
   return SB_OK;
 }
 
-// route (nullable, sb_debug_optimizer): appends "+"-joined "optimizer<base|ext>@<main|side>[w0,w1)" for the launch
+// route (nullable, sb_debug_optimizer): appends "+"-joined "optimizer<base|ext|rprop>@<main|side>[w0,w1)" for the launch
 static int enqueue_optimizer(sb_trainer* t, const StepIn& in, const float* g, int w0 = 0, int w1 = -1, cudaStream_t st = nullptr,
                              bool publish_scalars = false, bool pdl = false, std::string* route = nullptr) {
   Net& n = t->net;
   if (w1 < 0) w1 = n.n_work;
   if (!st) st = n.stream;
   if (w1 <= w0) return SB_OK;
-  const bool ext = opt_ext(t->hyper.kind);
+  const bool ext = opt_ext(t->hyper.kind), rp = t->hyper.kind == SB_OPT_RPROP;
   // pdl = false: plain dependency (runs after a stream join / on the comm stream)
-  SB_TRY(launch_kernel(ext ? optimizer_kernel<true> : optimizer_kernel<false>, dim3(static_cast<unsigned>(w1 - w0)), dim3(256), 0, st, pdl, n.work + w0, in.desc, t->hyper,
+  SB_TRY(launch_kernel(rp ? optimizer_kernel<true, true> : ext ? optimizer_kernel<true> : optimizer_kernel<false>, dim3(static_cast<unsigned>(w1 - w0)), dim3(256), 0, st, pdl, n.work + w0, in.desc, t->hyper,
                        n.theta, g, n.s1, n.s2, in.scal, publish_scalars ? t->d_hscal : static_cast<float*>(nullptr),
                        n.next_trace(st == n.stream ? "opt" : "opt_side")));
   n.mark("optimizer");
   if (route) {
     char r[64];
-    snprintf(r, sizeof(r), "%soptimizer<%s>@%s[%d,%d)", route->empty() ? "" : "+", ext ? "ext" : "base",
+    snprintf(r, sizeof(r), "%soptimizer<%s>@%s[%d,%d)", route->empty() ? "" : "+", rp ? "rprop" : ext ? "ext" : "base",
              st == n.stream ? "main" : "side", w0, w1);
     *route += r;
   }
@@ -334,22 +334,23 @@ static int xchg_grid(const sb_trainer* t, int slot_mask, bool alone) {
   return grid;
 }
 
-// the exchange kernel of the world size and optimizer group (opt_ext); *kernel names it (the same name for both groups)
-template <bool EXT>
+// the exchange kernel of the world size and optimizer group (opt_ext; RPROP's own); *kernel names it (the same name for
+// every group)
+template <bool EXT, bool RP = false>
 static int launch_xchg(sb_trainer* t, const XchgParams& p, dim3 g, dim3 b, cudaStream_t st, bool pdl, const char** kernel) {
   // plain bf16: the LL protocol (flags inside the data) needs fewer fabric round trips than the flag-and-pull kernel
   if (t->ll_ready) {
     LLParams lp;
     lp.x = p; lp.llg_off = t->llg_off; lp.lls_off = t->lls_off; lp.n4 = t->xch_n4;
-    if (t->world <= 2) { SB_TRY(launch_kernel(xchg_ll_kernel<2, EXT>, g, b, 0, st, pdl, lp)); *kernel = "xchg_ll<2>"; }
-    else if (t->world <= 4) { SB_TRY(launch_kernel(xchg_ll_kernel<4, EXT>, g, b, 0, st, pdl, lp)); *kernel = "xchg_ll<4>"; }
-    else if (t->world <= 8) { SB_TRY(launch_kernel(xchg_ll_kernel<8, EXT>, g, b, 0, st, pdl, lp)); *kernel = "xchg_ll<8>"; }
-    else { SB_TRY(launch_kernel(xchg_ll_kernel<16, EXT>, g, b, 0, st, pdl, lp)); *kernel = "xchg_ll<16>"; }
+    if (t->world <= 2) { SB_TRY(launch_kernel(xchg_ll_kernel<2, EXT, RP>, g, b, 0, st, pdl, lp)); *kernel = "xchg_ll<2>"; }
+    else if (t->world <= 4) { SB_TRY(launch_kernel(xchg_ll_kernel<4, EXT, RP>, g, b, 0, st, pdl, lp)); *kernel = "xchg_ll<4>"; }
+    else if (t->world <= 8) { SB_TRY(launch_kernel(xchg_ll_kernel<8, EXT, RP>, g, b, 0, st, pdl, lp)); *kernel = "xchg_ll<8>"; }
+    else { SB_TRY(launch_kernel(xchg_ll_kernel<16, EXT, RP>, g, b, 0, st, pdl, lp)); *kernel = "xchg_ll<16>"; }
   } else
-  if (t->world <= 2) { SB_TRY(launch_kernel(xchg_update_kernel<2, EXT>, g, b, 0, st, pdl, p)); *kernel = "xchg_update<2>"; }
-  else if (t->world <= 4) { SB_TRY(launch_kernel(xchg_update_kernel<4, EXT>, g, b, 0, st, pdl, p)); *kernel = "xchg_update<4>"; }
-  else if (t->world <= 8) { SB_TRY(launch_kernel(xchg_update_kernel<8, EXT>, g, b, 0, st, pdl, p)); *kernel = "xchg_update<8>"; }
-  else { SB_TRY(launch_kernel(xchg_update_kernel<16, EXT>, g, b, 0, st, pdl, p)); *kernel = "xchg_update<16>"; }
+  if (t->world <= 2) { SB_TRY(launch_kernel(xchg_update_kernel<2, EXT, RP>, g, b, 0, st, pdl, p)); *kernel = "xchg_update<2>"; }
+  else if (t->world <= 4) { SB_TRY(launch_kernel(xchg_update_kernel<4, EXT, RP>, g, b, 0, st, pdl, p)); *kernel = "xchg_update<4>"; }
+  else if (t->world <= 8) { SB_TRY(launch_kernel(xchg_update_kernel<8, EXT, RP>, g, b, 0, st, pdl, p)); *kernel = "xchg_update<8>"; }
+  else { SB_TRY(launch_kernel(xchg_update_kernel<16, EXT, RP>, g, b, 0, st, pdl, p)); *kernel = "xchg_update<16>"; }
   return SB_OK;
 }
 
@@ -370,7 +371,8 @@ static int enqueue_xchg(sb_trainer* t, const StepIn& in, int slot_mask, cudaStre
   if (grid <= 0) grid = xchg_grid(t, slot_mask, alone);
   const dim3 g(static_cast<unsigned>(grid)), b(256);
   const char* kernel;
-  if (opt_ext(t->hyper.kind)) SB_TRY(launch_xchg<true>(t, p, g, b, st, pdl, &kernel));
+  if (t->hyper.kind == SB_OPT_RPROP) SB_TRY((launch_xchg<true, true>(t, p, g, b, st, pdl, &kernel)));
+  else if (opt_ext(t->hyper.kind)) SB_TRY(launch_xchg<true>(t, p, g, b, st, pdl, &kernel));
   else SB_TRY(launch_xchg<false>(t, p, g, b, st, pdl, &kernel));
   n.mark(kernel);
   t->master_stale = true;
@@ -863,11 +865,17 @@ int sb_nccl_unique_id(void* out128) {
 }
 
 // Optimizer state that does not start at 0 (the arena's value): Adagrad's and FTRL's accum start at initial_accumulator,
-// RMSProp's ms at 1 (TF's RMSPropOptimizer creates its `rms` slot with a ones initializer).  Every rank fills its whole
-// state, so the runs a rank owns in the peer exchange start there as well.
+// RMSProp's ms at 1 (TF's RMSPropOptimizer creates its `rms` slot with a ones initializer), RPROP's step size at the
+// learning rate (torch.optim.Rprop's lr).  Every rank fills its whole state, so the runs a rank owns in the peer exchange
+// start there as well.
 static int fill_initial_state(sb_trainer* t) {
   Net& n = t->net;
   const int k = t->hyper.kind;
+  if (k == SB_OPT_RPROP) {
+    fill_kernel<<<static_cast<unsigned>((n.n_params + 255) / 256), 256, 0, n.stream>>>(n.s2, t->lr, n.n_params);
+    SB_CUDA(cudaGetLastError());
+    return SB_OK;
+  }
   if (k != SB_OPT_ADAGRAD && k != SB_OPT_FTRL && k != SB_OPT_RMSPROP) return SB_OK;
   const float v = k == SB_OPT_RMSPROP ? 1.f : t->initial_accumulator;
   fill_kernel<<<static_cast<unsigned>((n.n_params + 255) / 256), 256, 0, n.stream>>>(n.s1, v, n.n_params);
@@ -935,6 +943,7 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
   cudaFuncSetAttribute(set_batch_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   cudaFuncSetAttribute(optimizer_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   cudaFuncSetAttribute(optimizer_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  cudaFuncSetAttribute(optimizer_kernel<true, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   cudaFuncSetAttribute(axpy_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   Net& n = t->net;
   // streams and events of the step schedule; the side stream's CTAs are scheduled behind the main chain's
@@ -1034,6 +1043,14 @@ static int preload_exchange_kernels() {
   SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<4, true>));
   SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<8, true>));
   SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<16, true>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<2, true, true>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<4, true, true>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<8, true, true>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<16, true, true>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<2, true, true>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<4, true, true>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<8, true, true>));
+  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<16, true, true>));
   SB_CUDA(cudaFuncGetAttributes(&a, gather_master_kernel));
   SB_CUDA(cudaFuncGetAttributes(&a, set_batch_kernel));
   SB_CUDA(cudaFuncGetAttributes(&a, scale_kernel));

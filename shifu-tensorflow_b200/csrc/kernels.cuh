@@ -503,8 +503,9 @@ out_layer_rows_kernel(const OutLayerParams p, int rows_per_block) {
 // ------------------------------------------------------------------------------------------------
 // K7 fused multi-tensor optimizer over the flat parameter vector (TF 1.x kernel forms: ApplyAdadelta
 // res/ssgd_monitor.py:138, ApplyAdam res/ssgd.py:57, ApplyGradientDescent res/ssgd_monitor_bk.py:81,
-// ApplyMomentum, ApplyAdagrad, ApplyRMSProp, ApplyFtrl).  Reads the (all-reduced) gradient once, updates fp32 master
-// weights + state, and in bf16 mode refreshes the bf16 shadow of every hidden-layer weight matrix in the same pass.
+// ApplyMomentum, ApplyAdagrad, ApplyRMSProp, ApplyFtrl; and iRPROP- as torch.optim.Rprop computes it).  Reads the
+// (all-reduced) gradient once, updates fp32 master weights + state, and in bf16 mode refreshes the bf16 shadow of every
+// hidden-layer weight matrix in the same pass.
 // ------------------------------------------------------------------------------------------------
 struct OptHyper {
   int kind;
@@ -512,13 +513,15 @@ struct OptHyper {
   float l1, l2;                             // FTRL
 };
 
-// EXT: Adagrad, RMSProp or FTRL.  Every kernel that applies the update is instantiated once per group and launched for the
-// optimizer's group, so the reference's four run without the three later cases in their switch: with one switch of all
-// seven, the larger update cost the peer exchange kernels spills (ptxas -v, DESIGN.md section 5).
+// EXT: Adagrad, RMSProp, FTRL or RPROP.  Every kernel that applies the update is instantiated once per group and launched
+// for the optimizer's group, so the reference's four run without the later cases in their switch: with one switch of all
+// seven, the larger update cost the peer exchange kernels spills (ptxas -v, DESIGN.md section 5).  RPROP (RP = true, with
+// EXT) has instantiations of its own as well: as a fourth case of the EXT switch it slowed FTRL's optimizer pass at cfg2
+// from 21.0 to 24.3 us and RMSProp's from 19.5 to 21.1 (scripts/bench_optimizer.py, H100 SXM 80 GB at 700 W).
 __host__ __device__ __forceinline__ bool opt_ext(int kind) { return kind >= SB_OPT_ADAGRAD; }
 
 // the state streams each optimizer has (HBM-bound passes touch only those): SGD none, Momentum and Adagrad s1, the others
-// s1 + s2
+// (RPROP included) s1 + s2
 template <bool EXT>
 __device__ __forceinline__ bool opt_uses_s1(int kind) { return EXT || kind != SB_OPT_SGD; }
 template <bool EXT>
@@ -527,8 +530,15 @@ __device__ __forceinline__ bool opt_uses_s2(int kind) {
 }
 
 // correctly rounded sqrtf and true divisions throughout (no rsqrtf, no fast-math): the fp32 oracle bounds stay tight
-template <bool EXT>
+template <bool EXT, bool RP = false>
 __device__ __forceinline__ float opt_update(const OptHyper& h, float lr_t, float theta, float g, float& s1, float& s2) {
+  if constexpr (RP) {   // SB_OPT_RPROP, iRPROP- in torch.optim.Rprop's order: s1 = prev (the last gradient, 0 after a sign
+                        // flip), s2 = step size; lr_t is unused (the learning rate is only s2's start value)
+    const float p = g * s1;   // a product that underflows to 0 counts as no change, as in torch
+    s2 = fminf(fmaxf(s2 * (p > 0.f ? 1.2f : (p < 0.f ? 0.5f : 1.f)), 1e-6f), 50.f);
+    s1 = p < 0.f ? 0.f : g;   // a sign flip: no move this step, and no flip next step
+    return s1 > 0.f ? theta - s2 : (s1 < 0.f ? theta + s2 : theta);   // g = +-0: theta keeps its bits
+  }
   if constexpr (EXT) {
     switch (h.kind) {
       case SB_OPT_ADAGRAD:   // s1 = accum
@@ -594,7 +604,7 @@ __device__ __forceinline__ void shadow_store1(const OptWork& wk, long long at, f
   for (int part = 0; part < wk.np; ++part) wk.Wn[part * wk.part_stride + at] = __float2bfloat16_rn(bf16_residual(t, part));
 }
 
-template <bool EXT>
+template <bool EXT, bool RP = false>
 static __global__ void __launch_bounds__(256)
 optimizer_kernel(const OptWork* __restrict__ work, const BatchDesc* __restrict__ desc, OptHyper h,
                  float* __restrict__ theta, const float* __restrict__ grad, float* __restrict__ s1, float* __restrict__ s2,
@@ -626,10 +636,10 @@ optimizer_kernel(const OptWork* __restrict__ work, const BatchDesc* __restrict__
       float4 a = use_s1 ? *reinterpret_cast<const float4*>(s1 + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
       float4 b = use_s2 ? *reinterpret_cast<const float4*>(s2 + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
       float4 t;
-      t.x = opt_update<EXT>(h, lr_t, th.x, g.x * gs, a.x, b.x);
-      t.y = opt_update<EXT>(h, lr_t, th.y, g.y * gs, a.y, b.y);
-      t.z = opt_update<EXT>(h, lr_t, th.z, g.z * gs, a.z, b.z);
-      t.w = opt_update<EXT>(h, lr_t, th.w, g.w * gs, a.w, b.w);
+      t.x = opt_update<EXT, RP>(h, lr_t, th.x, g.x * gs, a.x, b.x);
+      t.y = opt_update<EXT, RP>(h, lr_t, th.y, g.y * gs, a.y, b.y);
+      t.z = opt_update<EXT, RP>(h, lr_t, th.z, g.z * gs, a.z, b.z);
+      t.w = opt_update<EXT, RP>(h, lr_t, th.w, g.w * gs, a.w, b.w);
       *reinterpret_cast<float4*>(theta + idx) = t;
       if (use_s1) *reinterpret_cast<float4*>(s1 + idx) = a;
       if (use_s2) *reinterpret_cast<float4*>(s2 + idx) = b;
@@ -648,7 +658,7 @@ optimizer_kernel(const OptWork* __restrict__ work, const BatchDesc* __restrict__
     if (e < wk.count) {
       const long long idx = wk.off + e;
       float a = use_s1 ? s1[idx] : 0.f, b = use_s2 ? s2[idx] : 0.f;
-      const float t = opt_update<EXT>(h, lr_t, theta[idx], grad[idx] * gs, a, b);
+      const float t = opt_update<EXT, RP>(h, lr_t, theta[idx], grad[idx] * gs, a, b);
       theta[idx] = t;
       if (use_s1) s1[idx] = a;
       if (use_s2) s2[idx] = b;

@@ -131,7 +131,8 @@ int validate_desc(const sb_net_desc* d) {
   SB_CHECK(d->max_batch > 0, SB_ERR_INVALID, "max_batch must be > 0");
   SB_CHECK(d->precision >= SB_PREC_FP32 && d->precision <= SB_PREC_BF16X2, SB_ERR_INVALID, "precision invalid");
   SB_CHECK(d->loss == SB_LOSS_MSE || d->loss == SB_LOSS_SIGMOID_CE, SB_ERR_INVALID, "loss invalid");
-  SB_CHECK(d->optimizer >= SB_OPT_ADADELTA && d->optimizer <= SB_OPT_FTRL, SB_ERR_INVALID, "optimizer invalid");
+  SB_CHECK((d->optimizer >= SB_OPT_ADADELTA && d->optimizer <= SB_OPT_FTRL) || d->optimizer == SB_OPT_RPROP, SB_ERR_INVALID,
+           "optimizer invalid");
   if (d->optimizer == SB_OPT_RMSPROP) {   // (only the optimizer that reads them: other descriptors may leave them at 0)
     SB_CHECK(d->rho >= 0.f && d->rho <= 1.f, SB_ERR_INVALID, "RMSProp decay (rho) must be in [0, 1] (got %g)", d->rho);
     SB_CHECK(d->momentum >= 0.f, SB_ERR_INVALID, "RMSProp momentum must be >= 0 (got %g)", d->momentum);

@@ -138,7 +138,7 @@ __device__ __forceinline__ bool xchg_wait(const unsigned int* slots, int world, 
 // whole SM (registers and shared memory), so an exchange overlaps a GEMM on the SMs that GEMM's grid leaves free.
 // The chain arrive -> loads -> stores + fence -> done costs several P2P round trips however little data moves: the
 // schedule (capi.cu) hides it behind GEMMs.
-template <int W, bool EXT>
+template <int W, bool EXT, bool RP = false>
 static __global__ void __launch_bounds__(256, W <= 8 ? 3 : 2)
 xchg_update_kernel(const XchgParams p) {
   constexpr int U = W <= 2 ? 2 : 1;       // runs per block iteration: U x (W + 3) sixteen-byte loads per thread in flight
@@ -222,10 +222,10 @@ xchg_update_kernel(const XchgParams p) {
                 if (q < p.world) { acc.x += g[u][q].x; acc.y += g[u][q].y; acc.z += g[u][q].z; acc.w += g[u][q].w; }
               const long long idx = wk.off + e;
               float4 a = sa[u], b = sb[u], t;
-              t.x = opt_update<EXT>(p.hyper, lr_t, th[u].x, acc.x * gs, a.x, b.x);
-              t.y = opt_update<EXT>(p.hyper, lr_t, th[u].y, acc.y * gs, a.y, b.y);
-              t.z = opt_update<EXT>(p.hyper, lr_t, th[u].z, acc.z * gs, a.z, b.z);
-              t.w = opt_update<EXT>(p.hyper, lr_t, th[u].w, acc.w * gs, a.w, b.w);
+              t.x = opt_update<EXT, RP>(p.hyper, lr_t, th[u].x, acc.x * gs, a.x, b.x);
+              t.y = opt_update<EXT, RP>(p.hyper, lr_t, th[u].y, acc.y * gs, a.y, b.y);
+              t.z = opt_update<EXT, RP>(p.hyper, lr_t, th[u].z, acc.z * gs, a.z, b.z);
+              t.w = opt_update<EXT, RP>(p.hyper, lr_t, th[u].w, acc.w * gs, a.w, b.w);
               *reinterpret_cast<float4*>(theta + idx) = t;
               // the owner keeps the reduced gradient of its runs (nobody else reads this part of my buffer): parity hook
               *reinterpret_cast<float4*>(my_grad + idx) = acc;
@@ -253,7 +253,7 @@ xchg_update_kernel(const XchgParams p) {
                 float acc = 0.f;
                 for (int q = 0; q < p.world; ++q) acc += ld_peer_f1(reinterpret_cast<const float*>(p.peers->base[q] + p.grad_off) + idx);
                 float a = use_s1 ? s1[idx] : 0.f, b = use_s2 ? s2[idx] : 0.f;
-                const float t = opt_update<EXT>(p.hyper, lr_t, theta[idx], acc * gs, a, b);
+                const float t = opt_update<EXT, RP>(p.hyper, lr_t, theta[idx], acc * gs, a, b);
                 theta[idx] = t;
                 my_grad[idx] = acc;
                 if (use_s1) s1[idx] = a;
@@ -472,7 +472,7 @@ __device__ __forceinline__ int run_owner(int w, int sb, int se, int world) {
 
 // plain-bf16 nets only (one shadow part).  One block per SM at most: no block ever waits for another block of its own
 // grid, but it does wait for the peers' blocks, which must all be able to become resident beside whatever GEMM is running.
-template <int W, bool EXT>
+template <int W, bool EXT, bool RP = false>
 static __global__ void __launch_bounds__(256, W <= 8 ? 3 : 2)
 xchg_ll_kernel(const LLParams lp) {
   const XchgParams& p = lp.x;
@@ -627,10 +627,10 @@ xchg_ll_kernel(const LLParams lp) {
           }
           if (alive) {
             float4 t;
-            t.x = opt_update<EXT>(p.hyper, lr_t, th.x, acc.x * gs, a.x, b.x);
-            t.y = opt_update<EXT>(p.hyper, lr_t, th.y, acc.y * gs, a.y, b.y);
-            t.z = opt_update<EXT>(p.hyper, lr_t, th.z, acc.z * gs, a.z, b.z);
-            t.w = opt_update<EXT>(p.hyper, lr_t, th.w, acc.w * gs, a.w, b.w);
+            t.x = opt_update<EXT, RP>(p.hyper, lr_t, th.x, acc.x * gs, a.x, b.x);
+            t.y = opt_update<EXT, RP>(p.hyper, lr_t, th.y, acc.y * gs, a.y, b.y);
+            t.z = opt_update<EXT, RP>(p.hyper, lr_t, th.z, acc.z * gs, a.z, b.z);
+            t.w = opt_update<EXT, RP>(p.hyper, lr_t, th.w, acc.w * gs, a.w, b.w);
             *reinterpret_cast<float4*>(theta + idx) = t;
             *reinterpret_cast<float4*>(my_grad + idx) = acc;      // the owner keeps the reduced gradient of its runs (parity hook)
             if (use_s1) *reinterpret_cast<float4*>(s1 + idx) = a;
@@ -675,7 +675,7 @@ xchg_ll_kernel(const LLParams lp) {
           }
           if (!alive) break;
           float a = use_s1 ? s1[idx] : 0.f, b = use_s2 ? s2[idx] : 0.f;
-          const float t = opt_update<EXT>(p.hyper, lr_t, theta[idx], acc * gs, a, b);
+          const float t = opt_update<EXT, RP>(p.hyper, lr_t, theta[idx], acc * gs, a, b);
           theta[idx] = t;
           my_grad[idx] = acc;
           if (use_s1) s1[idx] = a;

@@ -21,6 +21,9 @@ Optional ModelConfig train.params the reference does not have (defaults = refere
   Optimizer  "adadelta" (default) | "adam" | "sgd" | "momentum" | "adagrad" | "rmsprop" | "ftrl", each with the TF 1.x
              defaults of its other hyperparameters (Adagrad initial_accumulator 0.1; RMSProp decay 0.9, momentum 0,
              epsilon 1e-10, not centered; FTRL learning_rate_power -0.5, initial_accumulator 0.1, l1 = l2 = 0)
+             | "rprop": resilient propagation (iRPROP-, torch.optim.Rprop's defaults: step sizes grow by 1.2 while a
+             gradient keeps its sign and shrink by 0.5 when it flips, within [1e-6, 50]), made for full-batch gradients
+             such as sync_replicas' one update per epoch; LearningRate is the start step size.  Names in any case
   Loss       "squared" (default: MSE on the sigmoid output, ssgd_monitor.py:129) | "log" (sigmoid cross-entropy)
   Precision  "bf16" (default) | "fp32" (CUDA-core parity mode) | "fp32_tc" (fp32-class accuracy on the tensor cores:
              three bf16 parts per value) | "bf16x2" (two parts)
@@ -82,7 +85,7 @@ DELIMITER = '|'
 BATCH_SIZE = 100
 
 _OPT = {"adadelta": capi.OPT_ADADELTA, "adam": capi.OPT_ADAM, "sgd": capi.OPT_SGD, "momentum": capi.OPT_MOMENTUM,
-        "adagrad": capi.OPT_ADAGRAD, "rmsprop": capi.OPT_RMSPROP, "ftrl": capi.OPT_FTRL}
+        "adagrad": capi.OPT_ADAGRAD, "rmsprop": capi.OPT_RMSPROP, "ftrl": capi.OPT_FTRL, "rprop": capi.OPT_RPROP}
 _LOSS = {"squared": capi.LOSS_MSE, "log": capi.LOSS_SIGMOID_CE}
 
 
