@@ -266,6 +266,24 @@ static int enqueue_allreduce(sb_trainer* t, float* buf) {
   return SB_OK;
 }
 
+// The update kernels of every optimizer group (opt_group) and, for the exchange, world size: every launch, the carveout
+// setting and the preload read these tables.
+static void (*const optimizer_kernels[OPT_GROUPS])(const OptWork*, const BatchDesc*, OptHyper, float*, const float*, float*, float*,
+                                                   const float*, float*, unsigned long long*) = {
+    optimizer_kernel<OPT_BASE>, optimizer_kernel<OPT_EXT>, optimizer_kernel<OPT_RPROP>};
+static const char* const opt_group_names[OPT_GROUPS] = {"base", "ext", "rprop"};
+enum { XCHG_WORLDS = 4 };   // world <= 2 / 4 / 8 / 16
+static void (*const xchg_update_kernels[OPT_GROUPS][XCHG_WORLDS])(const XchgParams) = {
+    {xchg_update_kernel<2, OPT_BASE>, xchg_update_kernel<4, OPT_BASE>, xchg_update_kernel<8, OPT_BASE>, xchg_update_kernel<16, OPT_BASE>},
+    {xchg_update_kernel<2, OPT_EXT>, xchg_update_kernel<4, OPT_EXT>, xchg_update_kernel<8, OPT_EXT>, xchg_update_kernel<16, OPT_EXT>},
+    {xchg_update_kernel<2, OPT_RPROP>, xchg_update_kernel<4, OPT_RPROP>, xchg_update_kernel<8, OPT_RPROP>, xchg_update_kernel<16, OPT_RPROP>}};
+static void (*const xchg_ll_kernels[OPT_GROUPS][XCHG_WORLDS])(const LLParams) = {
+    {xchg_ll_kernel<2, OPT_BASE>, xchg_ll_kernel<4, OPT_BASE>, xchg_ll_kernel<8, OPT_BASE>, xchg_ll_kernel<16, OPT_BASE>},
+    {xchg_ll_kernel<2, OPT_EXT>, xchg_ll_kernel<4, OPT_EXT>, xchg_ll_kernel<8, OPT_EXT>, xchg_ll_kernel<16, OPT_EXT>},
+    {xchg_ll_kernel<2, OPT_RPROP>, xchg_ll_kernel<4, OPT_RPROP>, xchg_ll_kernel<8, OPT_RPROP>, xchg_ll_kernel<16, OPT_RPROP>}};
+static const char* const xchg_update_names[XCHG_WORLDS] = {"xchg_update<2>", "xchg_update<4>", "xchg_update<8>", "xchg_update<16>"};
+static const char* const xchg_ll_names[XCHG_WORLDS] = {"xchg_ll<2>", "xchg_ll<4>", "xchg_ll<8>", "xchg_ll<16>"};
+
 // route (nullable, sb_debug_optimizer): appends "+"-joined "optimizer<base|ext|rprop>@<main|side>[w0,w1)" for the launch
 static int enqueue_optimizer(sb_trainer* t, const StepIn& in, const float* g, int w0 = 0, int w1 = -1, cudaStream_t st = nullptr,
                              bool publish_scalars = false, bool pdl = false, std::string* route = nullptr) {
@@ -273,15 +291,15 @@ static int enqueue_optimizer(sb_trainer* t, const StepIn& in, const float* g, in
   if (w1 < 0) w1 = n.n_work;
   if (!st) st = n.stream;
   if (w1 <= w0) return SB_OK;
-  const bool ext = opt_ext(t->hyper.kind), rp = t->hyper.kind == SB_OPT_RPROP;
+  const int grp = opt_group(t->hyper.kind);
   // pdl = false: plain dependency (runs after a stream join / on the comm stream)
-  SB_TRY(launch_kernel(rp ? optimizer_kernel<true, true> : ext ? optimizer_kernel<true> : optimizer_kernel<false>, dim3(static_cast<unsigned>(w1 - w0)), dim3(256), 0, st, pdl, n.work + w0, in.desc, t->hyper,
+  SB_TRY(launch_kernel(optimizer_kernels[grp], dim3(static_cast<unsigned>(w1 - w0)), dim3(256), 0, st, pdl, n.work + w0, in.desc, t->hyper,
                        n.theta, g, n.s1, n.s2, in.scal, publish_scalars ? t->d_hscal : static_cast<float*>(nullptr),
                        n.next_trace(st == n.stream ? "opt" : "opt_side")));
   n.mark("optimizer");
   if (route) {
     char r[64];
-    snprintf(r, sizeof(r), "%soptimizer<%s>@%s[%d,%d)", route->empty() ? "" : "+", rp ? "rprop" : ext ? "ext" : "base",
+    snprintf(r, sizeof(r), "%soptimizer<%s>@%s[%d,%d)", route->empty() ? "" : "+", opt_group_names[grp],
              st == n.stream ? "main" : "side", w0, w1);
     *route += r;
   }
@@ -334,23 +352,19 @@ static int xchg_grid(const sb_trainer* t, int slot_mask, bool alone) {
   return grid;
 }
 
-// the exchange kernel of the world size and optimizer group (opt_ext; RPROP's own); *kernel names it (the same name for
-// every group)
-template <bool EXT, bool RP = false>
+// the exchange kernel of the world size and optimizer group; *kernel names it (the same name for every group)
 static int launch_xchg(sb_trainer* t, const XchgParams& p, dim3 g, dim3 b, cudaStream_t st, bool pdl, const char** kernel) {
+  const int grp = opt_group(t->hyper.kind), wi = t->world <= 2 ? 0 : t->world <= 4 ? 1 : t->world <= 8 ? 2 : 3;
   // plain bf16: the LL protocol (flags inside the data) needs fewer fabric round trips than the flag-and-pull kernel
   if (t->ll_ready) {
     LLParams lp;
     lp.x = p; lp.llg_off = t->llg_off; lp.lls_off = t->lls_off; lp.n4 = t->xch_n4;
-    if (t->world <= 2) { SB_TRY(launch_kernel(xchg_ll_kernel<2, EXT, RP>, g, b, 0, st, pdl, lp)); *kernel = "xchg_ll<2>"; }
-    else if (t->world <= 4) { SB_TRY(launch_kernel(xchg_ll_kernel<4, EXT, RP>, g, b, 0, st, pdl, lp)); *kernel = "xchg_ll<4>"; }
-    else if (t->world <= 8) { SB_TRY(launch_kernel(xchg_ll_kernel<8, EXT, RP>, g, b, 0, st, pdl, lp)); *kernel = "xchg_ll<8>"; }
-    else { SB_TRY(launch_kernel(xchg_ll_kernel<16, EXT, RP>, g, b, 0, st, pdl, lp)); *kernel = "xchg_ll<16>"; }
-  } else
-  if (t->world <= 2) { SB_TRY(launch_kernel(xchg_update_kernel<2, EXT, RP>, g, b, 0, st, pdl, p)); *kernel = "xchg_update<2>"; }
-  else if (t->world <= 4) { SB_TRY(launch_kernel(xchg_update_kernel<4, EXT, RP>, g, b, 0, st, pdl, p)); *kernel = "xchg_update<4>"; }
-  else if (t->world <= 8) { SB_TRY(launch_kernel(xchg_update_kernel<8, EXT, RP>, g, b, 0, st, pdl, p)); *kernel = "xchg_update<8>"; }
-  else { SB_TRY(launch_kernel(xchg_update_kernel<16, EXT, RP>, g, b, 0, st, pdl, p)); *kernel = "xchg_update<16>"; }
+    SB_TRY(launch_kernel(xchg_ll_kernels[grp][wi], g, b, 0, st, pdl, lp));
+    *kernel = xchg_ll_names[wi];
+  } else {
+    SB_TRY(launch_kernel(xchg_update_kernels[grp][wi], g, b, 0, st, pdl, p));
+    *kernel = xchg_update_names[wi];
+  }
   return SB_OK;
 }
 
@@ -371,9 +385,7 @@ static int enqueue_xchg(sb_trainer* t, const StepIn& in, int slot_mask, cudaStre
   if (grid <= 0) grid = xchg_grid(t, slot_mask, alone);
   const dim3 g(static_cast<unsigned>(grid)), b(256);
   const char* kernel;
-  if (t->hyper.kind == SB_OPT_RPROP) SB_TRY((launch_xchg<true, true>(t, p, g, b, st, pdl, &kernel)));
-  else if (opt_ext(t->hyper.kind)) SB_TRY(launch_xchg<true>(t, p, g, b, st, pdl, &kernel));
-  else SB_TRY(launch_xchg<false>(t, p, g, b, st, pdl, &kernel));
+  SB_TRY(launch_xchg(t, p, g, b, st, pdl, &kernel));
   n.mark(kernel);
   t->master_stale = true;
   t->grad_sharded = true;
@@ -871,7 +883,7 @@ int sb_nccl_unique_id(void* out128) {
 static int fill_initial_state(sb_trainer* t) {
   Net& n = t->net;
   const int k = t->hyper.kind;
-  if (k == SB_OPT_RPROP) {
+  if (opt_group(k) == OPT_RPROP) {
     fill_kernel<<<static_cast<unsigned>((n.n_params + 255) / 256), 256, 0, n.stream>>>(n.s2, t->lr, n.n_params);
     SB_CUDA(cudaGetLastError());
     return SB_OK;
@@ -941,9 +953,7 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
   SB_TRY(t->net.init(desc, device, true));
   // see Net::init: no L1 / shared-memory re-partition between the kernels of a step
   cudaFuncSetAttribute(set_batch_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  cudaFuncSetAttribute(optimizer_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  cudaFuncSetAttribute(optimizer_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  cudaFuncSetAttribute(optimizer_kernel<true, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  for (auto k : optimizer_kernels) cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   cudaFuncSetAttribute(axpy_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   Net& n = t->net;
   // streams and events of the step schedule; the side stream's CTAs are scheduled behind the main chain's
@@ -1027,30 +1037,10 @@ int sb_trainer_ipc_handle(sb_trainer_t* t, void* out64) {
 // with it the thread - would never return.  Everything a non-captured path launches around an exchange is loaded up front.
 static int preload_exchange_kernels() {
   cudaFuncAttributes a;
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<2, false>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<4, false>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<8, false>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<16, false>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<2, false>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<4, false>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<8, false>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<16, false>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<2, true>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<4, true>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<8, true>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<16, true>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<2, true>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<4, true>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<8, true>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<16, true>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<2, true, true>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<4, true, true>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<8, true, true>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_update_kernel<16, true, true>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<2, true, true>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<4, true, true>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<8, true, true>));
-  SB_CUDA(cudaFuncGetAttributes(&a, xchg_ll_kernel<16, true, true>));
+  for (const auto& row : xchg_update_kernels)
+    for (auto k : row) SB_CUDA(cudaFuncGetAttributes(&a, k));
+  for (const auto& row : xchg_ll_kernels)
+    for (auto k : row) SB_CUDA(cudaFuncGetAttributes(&a, k));
   SB_CUDA(cudaFuncGetAttributes(&a, gather_master_kernel));
   SB_CUDA(cudaFuncGetAttributes(&a, set_batch_kernel));
   SB_CUDA(cudaFuncGetAttributes(&a, scale_kernel));

@@ -513,33 +513,36 @@ struct OptHyper {
   float l1, l2;                             // FTRL
 };
 
-// EXT: Adagrad, RMSProp, FTRL or RPROP.  Every kernel that applies the update is instantiated once per group and launched
-// for the optimizer's group, so the reference's four run without the later cases in their switch: with one switch of all
-// seven, the larger update cost the peer exchange kernels spills (ptxas -v, DESIGN.md section 5).  RPROP (RP = true, with
-// EXT) has instantiations of its own as well: as a fourth case of the EXT switch it slowed FTRL's optimizer pass at cfg2
-// from 21.0 to 24.3 us and RMSProp's from 19.5 to 21.1 (scripts/bench_optimizer.py, H100 SXM 80 GB at 700 W).
-__host__ __device__ __forceinline__ bool opt_ext(int kind) { return kind >= SB_OPT_ADAGRAD; }
+// Optimizer groups: every kernel that applies the update is instantiated once per group and launched for the optimizer's
+// group, so the reference's four run without the later cases in their switch: with one switch of all seven, the larger
+// update cost the peer exchange kernels spills (ptxas -v, DESIGN.md section 5).  RPROP has a group of its own: as a fourth
+// case of the EXT switch it slowed FTRL's optimizer pass at cfg2 from 21.0 to 24.3 us and RMSProp's from 19.5 to 21.1
+// (scripts/bench_optimizer.py, H100 SXM 80 GB at 700 W).
+enum OptGroup { OPT_BASE = 0, OPT_EXT = 1, OPT_RPROP = 2, OPT_GROUPS = 3 };
+inline int opt_group(int kind) {   // the one place that maps an sb_optimizer to its group
+  return kind == SB_OPT_RPROP ? OPT_RPROP : kind >= SB_OPT_ADAGRAD ? OPT_EXT : OPT_BASE;
+}
 
 // the state streams each optimizer has (HBM-bound passes touch only those): SGD none, Momentum and Adagrad s1, the others
 // (RPROP included) s1 + s2
-template <bool EXT>
-__device__ __forceinline__ bool opt_uses_s1(int kind) { return EXT || kind != SB_OPT_SGD; }
-template <bool EXT>
+template <int G>
+__device__ __forceinline__ bool opt_uses_s1(int kind) { return G != OPT_BASE || kind != SB_OPT_SGD; }
+template <int G>
 __device__ __forceinline__ bool opt_uses_s2(int kind) {
-  return EXT ? kind != SB_OPT_ADAGRAD : (kind == SB_OPT_ADAM || kind == SB_OPT_ADADELTA);
+  return G != OPT_BASE ? kind != SB_OPT_ADAGRAD : (kind == SB_OPT_ADAM || kind == SB_OPT_ADADELTA);
 }
 
 // correctly rounded sqrtf and true divisions throughout (no rsqrtf, no fast-math): the fp32 oracle bounds stay tight
-template <bool EXT, bool RP = false>
+template <int G>
 __device__ __forceinline__ float opt_update(const OptHyper& h, float lr_t, float theta, float g, float& s1, float& s2) {
-  if constexpr (RP) {   // SB_OPT_RPROP, iRPROP- in torch.optim.Rprop's order: s1 = prev (the last gradient, 0 after a sign
-                        // flip), s2 = step size; lr_t is unused (the learning rate is only s2's start value)
+  if constexpr (G == OPT_RPROP) {   // iRPROP- in torch.optim.Rprop's order: s1 = prev (the last gradient, 0 after a sign
+                                     // flip), s2 = step size; lr_t is unused (the learning rate is only s2's start value)
     const float p = g * s1;   // a product that underflows to 0 counts as no change, as in torch
     s2 = fminf(fmaxf(s2 * (p > 0.f ? 1.2f : (p < 0.f ? 0.5f : 1.f)), 1e-6f), 50.f);
     s1 = p < 0.f ? 0.f : g;   // a sign flip: no move this step, and no flip next step
     return s1 > 0.f ? theta - s2 : (s1 < 0.f ? theta + s2 : theta);   // g = +-0: theta keeps its bits
   }
-  if constexpr (EXT) {
+  if constexpr (G == OPT_EXT) {
     switch (h.kind) {
       case SB_OPT_ADAGRAD:   // s1 = accum
         s1 = s1 + g * g;
@@ -586,10 +589,26 @@ struct OptWork {
   int out_dim;            // > 0: run lies in a weight matrix with this many columns
   long long mat_off;      // flat offset of that matrix
   __nv_bfloat16* Wn;      // shadow base (nullptr: no shadow)
-  int ld_out;
+  int ld_out;             // a multiple of 4 (Net::build_work): the 16-byte path's shadow stores are 8-byte aligned
   int np;                 // bf16 parts of the shadow (split-precision modes; 1 = plain)
   long long part_stride;  // elements between parts
 };
+
+// A run takes the 16-byte path (one thread = 4 consecutive parameters) when its parameters, and the elements of its shadow,
+// come in aligned fours: 4 consecutive elements of a shadow-backed run never straddle a row (out_dim % 4 == 0).
+// optimizer_kernel tests the macro: the bool an inlined function returns stays a value the kernel branches on (byte moves,
+// another block layout), which made its Adagrad / RMSProp / FTRL / RPROP passes over the other layers ~0.8 us slower.  The
+// exchange kernels test it through run_is_vec, whose kept value leaves them fewer registers and spills than the macro
+// (xchg_ll<2, *>: 70-74 registers instead of 78-80).
+#define SB_RUN_IS_VEC(wk) \
+  (((wk).off & 3) == 0 && ((wk).count & 3) == 0 && ((wk).Wn == nullptr || (((wk).out_dim & 3) == 0 && (((wk).off - (wk).mat_off) & 3) == 0)))
+__device__ __forceinline__ bool run_is_vec(const OptWork& wk) { return SB_RUN_IS_VEC(wk); }
+// element offset inside one part of the shadow of flat parameter idx of a shadow-backed run
+__device__ __forceinline__ long long shadow_at(const OptWork& wk, long long idx) {
+  const long long m = idx - wk.mat_off;
+  const long long r = m / wk.out_dim;
+  return r * wk.ld_out + (m - r * wk.out_dim);
+}
 
 // store 4 / 1 updated weights into the bf16 shadow (all of its parts)
 __device__ __forceinline__ void shadow_store4(const OptWork& wk, long long at, const float4& t) {
@@ -604,7 +623,45 @@ __device__ __forceinline__ void shadow_store1(const OptWork& wk, long long at, f
   for (int part = 0; part < wk.np; ++part) wk.Wn[part * wk.part_stride + at] = __float2bfloat16_rn(bf16_residual(t, part));
 }
 
-template <bool EXT, bool RP = false>
+// The update of parameter idx (opt_apply1) or of the 4 from idx (opt_apply4, 16-byte path) and its write-back: theta, the
+// state streams the optimizer has and every part of the shadow.  th, g, a, b are the loaded theta, the unscaled gradient (or
+// the sum over ranks), s1 and s2 (0 where the optimizer has no such stream).  Returns the new theta.
+template <int G>
+__device__ __forceinline__ float4 opt_apply4(const OptHyper& h, float lr_t, float gs, const OptWork& wk, long long idx, float4 th,
+                                             float4 g, float4 a, float4 b, float* theta, float* s1, float* s2) {
+  float4 t;
+  t.x = opt_update<G>(h, lr_t, th.x, g.x * gs, a.x, b.x);
+  t.y = opt_update<G>(h, lr_t, th.y, g.y * gs, a.y, b.y);
+  t.z = opt_update<G>(h, lr_t, th.z, g.z * gs, a.z, b.z);
+  t.w = opt_update<G>(h, lr_t, th.w, g.w * gs, a.w, b.w);
+  *reinterpret_cast<float4*>(theta + idx) = t;
+  if (opt_uses_s1<G>(h.kind)) *reinterpret_cast<float4*>(s1 + idx) = a;
+  if (opt_uses_s2<G>(h.kind)) *reinterpret_cast<float4*>(s2 + idx) = b;
+  if (wk.Wn != nullptr) shadow_store4(wk, shadow_at(wk, idx), t);
+  return t;
+}
+template <int G>
+__device__ __forceinline__ float opt_apply1(const OptHyper& h, float lr_t, float gs, const OptWork& wk, long long idx, float th,
+                                            float g, float a, float b, float* theta, float* s1, float* s2) {
+  const float t = opt_update<G>(h, lr_t, th, g * gs, a, b);
+  theta[idx] = t;
+  if (opt_uses_s1<G>(h.kind)) s1[idx] = a;
+  if (opt_uses_s2<G>(h.kind)) s2[idx] = b;
+  if (wk.Wn != nullptr) shadow_store1(wk, shadow_at(wk, idx), t);
+  return t;
+}
+
+// The last kernel of a step publishes the step scalars (loss sum, n_nz) and the step's loss-history slot straight into
+// mapped pinned host memory: a posted PCIe write off the critical path instead of a D2H copy node between two steps.
+__device__ __forceinline__ void publish_step_scalars(const float* scal, float* host_scal, const BatchDesc* desc) {
+  if (host_scal != nullptr && blockIdx.x == 0 && threadIdx.x < SCAL_COUNT) {
+    host_scal[threadIdx.x] = scal[threadIdx.x];
+    if (threadIdx.x == 0 && desc->hist != nullptr) *desc->hist = make_float2(scal[SCAL_LOSS_SUM], scal[SCAL_NNZ]);   // loss curve
+    __threadfence_system();
+  }
+}
+
+template <int G>
 static __global__ void __launch_bounds__(256)
 optimizer_kernel(const OptWork* __restrict__ work, const BatchDesc* __restrict__ desc, OptHyper h,
                  float* __restrict__ theta, const float* __restrict__ grad, float* __restrict__ s1, float* __restrict__ s2,
@@ -614,40 +671,22 @@ optimizer_kernel(const OptWork* __restrict__ work, const BatchDesc* __restrict__
   pdl_wait();
   pdl_launch_dependents();
   if (trace != nullptr && blockIdx.x == 0 && threadIdx.x == 0) trace[2] = globaltimer_ns();   // dependencies resolved
-  // last kernel of a step: publish the step scalars (loss sum, n_nz) straight into mapped pinned host memory - a posted
-  // PCIe write off the critical path instead of a D2H copy node between two steps
-  if (host_scal != nullptr && blockIdx.x == 0 && threadIdx.x < SCAL_COUNT) {
-    host_scal[threadIdx.x] = scal[threadIdx.x];
-    if (threadIdx.x == 0 && desc->hist != nullptr) *desc->hist = make_float2(scal[SCAL_LOSS_SUM], scal[SCAL_NNZ]);   // loss curve
-    __threadfence_system();
-  }
+  publish_step_scalars(scal, host_scal, desc);
   const OptWork wk = work[blockIdx.x];
   const float lr_t = desc->lr_t, gs = desc->gscale;
   // HBM-bound: only touch the state streams the optimizer actually has
-  const bool use_s1 = opt_uses_s1<EXT>(h.kind);
-  const bool use_s2 = opt_uses_s2<EXT>(h.kind);
-  if ((wk.off & 3) == 0 && (wk.count & 3) == 0 && (wk.Wn == nullptr || ((wk.out_dim & 3) == 0 && ((wk.off - wk.mat_off) & 3) == 0))) {
-    // 16-byte path: one thread = 4 consecutive parameters (a full 1024-run = 256 threads x float4)
+  const bool use_s1 = opt_uses_s1<G>(h.kind);
+  const bool use_s2 = opt_uses_s2<G>(h.kind);
+  if (SB_RUN_IS_VEC(wk)) {
+    // one thread = 4 consecutive parameters (a full 1024-run = 256 threads x float4)
     const int e = threadIdx.x * 4;
     if (e < wk.count) {
       const long long idx = wk.off + e;
       const float4 th = *reinterpret_cast<const float4*>(theta + idx);
       const float4 g = *reinterpret_cast<const float4*>(grad + idx);
-      float4 a = use_s1 ? *reinterpret_cast<const float4*>(s1 + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
-      float4 b = use_s2 ? *reinterpret_cast<const float4*>(s2 + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
-      float4 t;
-      t.x = opt_update<EXT, RP>(h, lr_t, th.x, g.x * gs, a.x, b.x);
-      t.y = opt_update<EXT, RP>(h, lr_t, th.y, g.y * gs, a.y, b.y);
-      t.z = opt_update<EXT, RP>(h, lr_t, th.z, g.z * gs, a.z, b.z);
-      t.w = opt_update<EXT, RP>(h, lr_t, th.w, g.w * gs, a.w, b.w);
-      *reinterpret_cast<float4*>(theta + idx) = t;
-      if (use_s1) *reinterpret_cast<float4*>(s1 + idx) = a;
-      if (use_s2) *reinterpret_cast<float4*>(s2 + idx) = b;
-      if (wk.Wn != nullptr) {
-        const long long m = idx - wk.mat_off;
-        const long long r = m / wk.out_dim;     // 4 consecutive elements never straddle a row (out_dim % 4 == 0)
-        shadow_store4(wk, r * wk.ld_out + (m - r * wk.out_dim), t);
-      }
+      const float4 a = use_s1 ? *reinterpret_cast<const float4*>(s1 + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
+      const float4 b = use_s2 ? *reinterpret_cast<const float4*>(s2 + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
+      opt_apply4<G>(h, lr_t, gs, wk, idx, th, g, a, b, theta, s1, s2);
     }
     trace_end(trace);
     return;
@@ -657,16 +696,8 @@ optimizer_kernel(const OptWork* __restrict__ work, const BatchDesc* __restrict__
     const int e = threadIdx.x + 256 * i;
     if (e < wk.count) {
       const long long idx = wk.off + e;
-      float a = use_s1 ? s1[idx] : 0.f, b = use_s2 ? s2[idx] : 0.f;
-      const float t = opt_update<EXT, RP>(h, lr_t, theta[idx], grad[idx] * gs, a, b);
-      theta[idx] = t;
-      if (use_s1) s1[idx] = a;
-      if (use_s2) s2[idx] = b;
-      if (wk.Wn != nullptr) {
-        const long long m = idx - wk.mat_off;
-        const long long r = m / wk.out_dim;
-        shadow_store1(wk, r * wk.ld_out + (m - r * wk.out_dim), t);
-      }
+      const float a = use_s1 ? s1[idx] : 0.f, b = use_s2 ? s2[idx] : 0.f;
+      opt_apply1<G>(h, lr_t, gs, wk, idx, theta[idx], grad[idx], a, b, theta, s1, s2);
     }
   }
   trace_end(trace);
@@ -682,9 +713,7 @@ shadow_refresh_kernel(const OptWork* __restrict__ work, const float* __restrict_
     const int e = threadIdx.x + 256 * i;
     if (e < wk.count) {
       const long long idx = wk.off + e;
-      const long long m = idx - wk.mat_off;
-      const long long r = m / wk.out_dim;
-      shadow_store1(wk, r * wk.ld_out + (m - r * wk.out_dim), theta[idx]);
+      shadow_store1(wk, shadow_at(wk, idx), theta[idx]);
     }
   }
 }

@@ -250,7 +250,8 @@ int Net::init(const sb_net_desc* d, int device_, bool training_) {
 
   // optimizer / shadow-refresh work table: runs of <= 1024 consecutive parameters
   const std::vector<char> all(static_cast<size_t>(L + 1), 1);
-  const std::vector<OptWork> wk = build_work(all, all, &work_begin, &work_end);
+  std::vector<OptWork> wk;
+  SB_TRY(build_work(all, all, &wk, &work_begin, &work_end));
   n_work = static_cast<int>(wk.size());
   SB_TRY(dalloc(&work, wk.size()));
   SB_CUDA(cudaMemcpyAsync(work, wk.data(), wk.size() * sizeof(OptWork), cudaMemcpyHostToDevice, stream));
@@ -357,9 +358,10 @@ int Net::enqueue_embed(int rows, bool scatter, float* grad, cudaStream_t st) {
 // The runs of every parameter that trains (w_trains[l] / b_trains[l]: W_l / b_l of layer l = 0..L), layer by layer; the
 // range of layer l goes to [(*begin)[l], (*end)[l]).  A tensor-core net keeps W_l (shadow-backed) and b_l in separate
 // runs; fp32 mode puts W_l and b_l, which lie next to each other, into one stretch of runs when both train.
-std::vector<OptWork> Net::build_work(const std::vector<char>& w_trains, const std::vector<char>& b_trains, std::vector<int>* begin,
-                                     std::vector<int>* end) const {
-  std::vector<OptWork> wk;
+int Net::build_work(const std::vector<char>& w_trains, const std::vector<char>& b_trains, std::vector<OptWork>* out,
+                    std::vector<int>* begin, std::vector<int>* end) const {
+  std::vector<OptWork>& wk = *out;
+  wk.clear();
   auto add_runs = [&](long long o, long long n, const Layer* mat) {
     for (long long s = 0; s < n; s += 1024) {
       OptWork w = {};
@@ -376,6 +378,8 @@ std::vector<OptWork> Net::build_work(const std::vector<char>& w_trains, const st
   for (int l = 0; l <= L; ++l) {
     const Layer& ly = layers[l];
     const long long nw = static_cast<long long>(ly.in) * ly.out;
+    // the 16-byte path (SB_RUN_IS_VEC) stores 4 shadow elements at once: they are 8-byte aligned only when ld_out % 4 == 0
+    SB_CHECK(!tc() || l == L || ly.ld_out % 4 == 0, SB_ERR_STATE, "layer %d: shadow row pitch %d is not a multiple of 4", l, ly.ld_out);
     (*begin)[l] = static_cast<int>(wk.size());
     if (tc() && l < L) {
       if (w_trains[l]) add_runs(ly.w_off, nw, &ly);
@@ -388,12 +392,13 @@ std::vector<OptWork> Net::build_work(const std::vector<char>& w_trains, const st
     }
     (*end)[l] = static_cast<int>(wk.size());
   }
-  return wk;
+  return SB_OK;
 }
 
 int Net::set_trainable(const std::vector<char>& w_trains, const std::vector<char>& b_trains) {
   SB_CUDA(cudaSetDevice(device));
-  const std::vector<OptWork> wk = build_work(w_trains, b_trains, &work_begin, &work_end);
+  std::vector<OptWork> wk;
+  SB_TRY(build_work(w_trains, b_trains, &wk, &work_begin, &work_end));
   n_work = static_cast<int>(wk.size());
   const bool every = std::all_of(w_trains.begin(), w_trains.end(), [](char c) { return c != 0; }) &&
                      std::all_of(b_trains.begin(), b_trains.end(), [](char c) { return c != 0; });

@@ -79,8 +79,8 @@ struct Net {
   OptWork* work_all = nullptr;
   int n_work_all = 0;
   OptWork* work_part = nullptr;            // the table's storage once set_trainable left parameters out
-  std::vector<OptWork> build_work(const std::vector<char>& w_trains, const std::vector<char>& b_trains, std::vector<int>* begin,
-                                  std::vector<int>* end) const;
+  int build_work(const std::vector<char>& w_trains, const std::vector<char>& b_trains, std::vector<OptWork>* wk,
+                 std::vector<int>* begin, std::vector<int>* end) const;
   // Freeze parameters (fine-tuning, sb_trainer_set_fixed_layers): the work table and work_begin / work_end keep only the runs
   // of W_l where w_trains[l] and of b_l where b_trains[l] (l = 0..L).  Frozen runs are never updated or shadow-refreshed by
   // a step.

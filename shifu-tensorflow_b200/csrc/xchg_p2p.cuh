@@ -102,6 +102,31 @@ __device__ __forceinline__ float ld_peer_f1(const float* p) {
 __host__ __device__ inline int xchg_share(int b, int e, int r, int world) {
   return b + static_cast<int>((static_cast<long long>(e - b) * r) / world);
 }
+// the rank whose share of [sb, se) holds run w: estimate, then fix up
+__device__ __forceinline__ int run_owner(int w, int sb, int se, int world) {
+  int q = static_cast<int>((static_cast<long long>(w - sb) * world) / (se - sb));
+  while (q + 1 < world && w >= xchg_share(sb, se, q + 1, world)) ++q;
+  while (q > 0 && w < xchg_share(sb, se, q, world)) --q;
+  return q;
+}
+// the j-th run of [sb, se) outside this rank's share [w0, w1)
+__device__ __forceinline__ int other_run(int j, int sb, int w0, int w1) { return sb + j + ((sb + j >= w0) ? (w1 - w0) : 0); }
+
+// The slow half of every spin loop, after each poll that found its flags short of the step: on every (mask + 1)-th call, give
+// up if another thread of the block has, or once the wait has lasted p.timeout_ns (0 = wait forever); a timeout records
+// 1 + 16 * slot + missing() (the rank waited for) in the host's error word.
+template <class Missing>
+__device__ __forceinline__ bool xchg_give_up(unsigned int& spins, unsigned int mask, unsigned long long& t0, const XchgParams& p,
+                                             int slot, const unsigned int* sh_fail, Missing missing) {
+  if ((++spins & mask) != 0) return false;
+  if (*reinterpret_cast<const volatile unsigned int*>(sh_fail)) return true;
+  if (p.timeout_ns == 0) return false;
+  const unsigned long long now = globaltimer_ns();
+  if (t0 == 0) { t0 = now; return false; }
+  if (now - t0 <= p.timeout_ns) return false;
+  if (p.host_err != nullptr) { atomicCAS(p.host_err, 0u, 1u + 16u * slot + missing()); __threadfence_system(); }
+  return true;
+}
 
 // Block-wide wait until slots[q] >= epoch for every q < world.  Returns false after a timeout (error recorded).
 __device__ __forceinline__ bool xchg_wait(const unsigned int* slots, int world, unsigned int epoch, const XchgParams& p, int seg,
@@ -112,20 +137,8 @@ __device__ __forceinline__ bool xchg_wait(const unsigned int* slots, int world, 
     if (lane < world) {
       unsigned long long t0 = 0;
       unsigned int spins = 0;
-      while (static_cast<int>(ld_acquire_sys(slots + lane) - epoch) < 0) {
-        if ((++spins & 0x3FFu) == 0) {
-          if (*reinterpret_cast<volatile unsigned int*>(sh_fail)) { ok = false; break; }
-          if (p.timeout_ns != 0) {
-            const unsigned long long now = globaltimer_ns();
-            if (t0 == 0) t0 = now;
-            else if (now - t0 > p.timeout_ns) {
-              if (p.host_err != nullptr) { atomicCAS(p.host_err, 0u, 1u + 16u * seg + lane); __threadfence_system(); }
-              ok = false;
-              break;
-            }
-          }
-        }
-      }
+      while (static_cast<int>(ld_acquire_sys(slots + lane) - epoch) < 0)
+        if (xchg_give_up(spins, 0x3FFu, t0, p, seg, sh_fail, [&] { return lane; })) { ok = false; break; }
     }
     if (!__all_sync(0xffffffffu, ok) && lane == 0) *sh_fail = 1u;
   }
@@ -138,7 +151,7 @@ __device__ __forceinline__ bool xchg_wait(const unsigned int* slots, int world, 
 // whole SM (registers and shared memory), so an exchange overlaps a GEMM on the SMs that GEMM's grid leaves free.
 // The chain arrive -> loads -> stores + fence -> done costs several P2P round trips however little data moves: the
 // schedule (capi.cu) hides it behind GEMMs.
-template <int W, bool EXT, bool RP = false>
+template <int W, int G>
 static __global__ void __launch_bounds__(256, W <= 8 ? 3 : 2)
 xchg_update_kernel(const XchgParams p) {
   constexpr int U = W <= 2 ? 2 : 1;       // runs per block iteration: U x (W + 3) sixteen-byte loads per thread in flight
@@ -156,14 +169,10 @@ xchg_update_kernel(const XchgParams p) {
   char* const my_base = p.peers->base[p.rank];
   float* const theta = reinterpret_cast<float*>(my_base);
   P2PFlags* mine = reinterpret_cast<P2PFlags*>(my_base + p.flags_off);
-  if (p.host_scal != nullptr && blockIdx.x == 0 && threadIdx.x < SCAL_COUNT) {
-    p.host_scal[threadIdx.x] = p.scal[threadIdx.x];     // loss sum / n_nz of this rank's mini-batch (see optimizer_kernel)
-    if (threadIdx.x == 0 && p.desc->hist != nullptr) *p.desc->hist = make_float2(p.scal[SCAL_LOSS_SUM], p.scal[SCAL_NNZ]);
-    __threadfence_system();
-  }
+  publish_step_scalars(p.scal, p.host_scal, p.desc);     // loss sum / n_nz of this rank's mini-batch
   const float lr_t = p.desc->lr_t, gs = p.desc->gscale;
-  const bool use_s1 = opt_uses_s1<EXT>(p.hyper.kind);
-  const bool use_s2 = opt_uses_s2<EXT>(p.hyper.kind);
+  const bool use_s1 = opt_uses_s1<G>(p.hyper.kind);
+  const bool use_s2 = opt_uses_s2<G>(p.hyper.kind);
   float* const s1 = reinterpret_cast<float*>(my_base + p.s1_off);
   float* const s2 = reinterpret_cast<float*>(my_base + p.s2_off);
   float* const my_grad = reinterpret_cast<float*>(my_base + p.grad_off);
@@ -195,10 +204,8 @@ xchg_update_kernel(const XchgParams p) {
           if (wb + u < w1) {
             const OptWork& wk = p.work[wb + u];
             const long long off = wk.off;
-            const int cnt = wk.count;
-            vec[u] = (off & 3) == 0 && (cnt & 3) == 0 &&
-                     (wk.Wn == nullptr || ((wk.out_dim & 3) == 0 && ((off - wk.mat_off) & 3) == 0 && (wk.ld_out & 3) == 0));
-            on[u] = vec[u] && e < cnt;
+            vec[u] = run_is_vec(wk);
+            on[u] = vec[u] && e < wk.count;
             if (on[u]) {
 #pragma unroll
               for (int q = 0; q < W; ++q)
@@ -213,7 +220,6 @@ xchg_update_kernel(const XchgParams p) {
         for (int u = 0; u < U; ++u) {
           if (wb + u >= w1) continue;
           const OptWork wk = p.work[wb + u];
-          const long long shadow_rel = wk.Wn != nullptr ? reinterpret_cast<char*>(wk.Wn) - my_base : 0;
           if (vec[u]) {
             if (on[u]) {
               float4 acc = g[u][0];               // fixed rank order -> the same bits wherever a sum is computed
@@ -221,27 +227,9 @@ xchg_update_kernel(const XchgParams p) {
               for (int q = 1; q < W; ++q)
                 if (q < p.world) { acc.x += g[u][q].x; acc.y += g[u][q].y; acc.z += g[u][q].z; acc.w += g[u][q].w; }
               const long long idx = wk.off + e;
-              float4 a = sa[u], b = sb[u], t;
-              t.x = opt_update<EXT, RP>(p.hyper, lr_t, th[u].x, acc.x * gs, a.x, b.x);
-              t.y = opt_update<EXT, RP>(p.hyper, lr_t, th[u].y, acc.y * gs, a.y, b.y);
-              t.z = opt_update<EXT, RP>(p.hyper, lr_t, th[u].z, acc.z * gs, a.z, b.z);
-              t.w = opt_update<EXT, RP>(p.hyper, lr_t, th[u].w, acc.w * gs, a.w, b.w);
-              *reinterpret_cast<float4*>(theta + idx) = t;
               // the owner keeps the reduced gradient of its runs (nobody else reads this part of my buffer): parity hook
               *reinterpret_cast<float4*>(my_grad + idx) = acc;
-              if (use_s1) *reinterpret_cast<float4*>(s1 + idx) = a;
-              if (use_s2) *reinterpret_cast<float4*>(s2 + idx) = b;
-              if (wk.Wn != nullptr) {
-                const long long m = idx - wk.mat_off;
-                const long long r = m / wk.out_dim;     // 4 consecutive elements never straddle a row
-                const long long rel = shadow_rel + (r * wk.ld_out + (m - r * wk.out_dim)) * 2;
-                for (int part = 0; part < wk.np; ++part) {      // split-precision modes: every part of the shadow
-                  uint2 o;
-                  o.x = pack_bf16x2(bf16_residual(t.x, part), bf16_residual(t.y, part));
-                  o.y = pack_bf16x2(bf16_residual(t.z, part), bf16_residual(t.w, part));
-                  *reinterpret_cast<uint2*>(my_base + rel + part * wk.part_stride * 2) = o;     // peers pull it in phase 2
-                }
-              }
+              opt_apply4<G>(p.hyper, lr_t, gs, wk, idx, th[u], acc, sa[u], sb[u], theta, s1, s2);   // peers pull the shadow in phase 2
             }
           } else {
             // unaligned run (odd widths): scalar path, 4 elements per thread strided by 256
@@ -252,21 +240,9 @@ xchg_update_kernel(const XchgParams p) {
                 const long long idx = wk.off + es;
                 float acc = 0.f;
                 for (int q = 0; q < p.world; ++q) acc += ld_peer_f1(reinterpret_cast<const float*>(p.peers->base[q] + p.grad_off) + idx);
-                float a = use_s1 ? s1[idx] : 0.f, b = use_s2 ? s2[idx] : 0.f;
-                const float t = opt_update<EXT, RP>(p.hyper, lr_t, theta[idx], acc * gs, a, b);
-                theta[idx] = t;
+                const float a = use_s1 ? s1[idx] : 0.f, b = use_s2 ? s2[idx] : 0.f;
+                opt_apply1<G>(p.hyper, lr_t, gs, wk, idx, theta[idx], acc, a, b, theta, s1, s2);
                 my_grad[idx] = acc;
-                if (use_s1) s1[idx] = a;
-                if (use_s2) s2[idx] = b;
-                if (wk.Wn != nullptr) {
-                  const long long m = idx - wk.mat_off;
-                  const long long r = m / wk.out_dim;
-                  const long long rel = shadow_rel + (r * wk.ld_out + (m - r * wk.out_dim)) * 2;
-                  for (int part = 0; part < wk.np; ++part) {
-                    const __nv_bfloat16 hv = __float2bfloat16_rn(bf16_residual(t, part));
-                    *reinterpret_cast<__nv_bfloat16*>(my_base + rel + part * wk.part_stride * 2) = hv;
-                  }
-                }
               }
             }
           }
@@ -326,21 +302,14 @@ xchg_update_kernel(const XchgParams p) {
           dst[u] = -1; is_sh[u] = false;
           const int j = i0 + u;
           if (j >= n_other) continue;
-          const int w = sb + j + ((sb + j >= w0) ? (w1 - w0) : 0);
-          int q = static_cast<int>((static_cast<long long>(w - sb) * p.world) / (se - sb));     // owner of run w: estimate, then fix up
-          while (q + 1 < p.world && w >= xchg_share(sb, se, q + 1, p.world)) ++q;
-          while (q > 0 && w < xchg_share(sb, se, q, p.world)) --q;
+          const int w = other_run(j, sb, w0, w1);
           const OptWork& wk = p.work[w];
-          const bool vec = (wk.off & 3) == 0 && (wk.count & 3) == 0 &&
-                           (wk.Wn == nullptr || ((wk.out_dim & 3) == 0 && ((wk.off - wk.mat_off) & 3) == 0 && (wk.ld_out & 3) == 0));
-          const char* ob = p.peers->base[q];
-          if (vec && wk.np == 1) {
+          const char* ob = p.peers->base[run_owner(w, sb, se, p.world)];
+          if (run_is_vec(wk) && wk.np == 1) {
             if (e < wk.count) {
               const long long idx = wk.off + e;
               if (wk.Wn != nullptr) {
-                const long long m = idx - wk.mat_off;
-                const long long r = m / wk.out_dim;
-                dst[u] = (reinterpret_cast<char*>(wk.Wn) - my_base) + (r * wk.ld_out + (m - r * wk.out_dim)) * 2;
+                dst[u] = (reinterpret_cast<char*>(wk.Wn) - my_base) + shadow_at(wk, idx) * 2;
                 is_sh[u] = true;
                 asm volatile("ld.relaxed.sys.global.v2.u32 {%0, %1}, [%2];" : "=r"(sh[u].x), "=r"(sh[u].y) : "l"(ob + dst[u]) : "memory");
               } else {
@@ -355,9 +324,7 @@ xchg_update_kernel(const XchgParams p) {
               if (es >= wk.count) continue;
               const long long idx = wk.off + es;
               if (wk.Wn != nullptr) {
-                const long long m = idx - wk.mat_off;
-                const long long r = m / wk.out_dim;
-                const long long rel = (reinterpret_cast<char*>(wk.Wn) - my_base) + (r * wk.ld_out + (m - r * wk.out_dim)) * 2;
+                const long long rel = (reinterpret_cast<char*>(wk.Wn) - my_base) + shadow_at(wk, idx) * 2;
                 for (int part = 0; part < wk.np; ++part) {
                   unsigned short hv;
                   asm volatile("ld.relaxed.sys.global.u16 %0, [%1];" : "=h"(hv) : "l"(ob + rel + part * wk.part_stride * 2) : "memory");
@@ -413,66 +380,24 @@ __device__ __forceinline__ void ll_store2(char* dst, unsigned int d0, unsigned i
 __device__ __forceinline__ void ll_store1(char* dst, unsigned int d0, unsigned int ep) {
   asm volatile("st.relaxed.sys.global.v2.u32 [%0], {%1, %2};" ::"l"(dst), "r"(d0), "r"(ep) : "memory");
 }
-// poll one 16-byte LL pair until both halves carry `ep`; false after a timeout / failure elsewhere in the block
-__device__ __forceinline__ bool ll_poll2(const char* src, unsigned int ep, unsigned int& d0, unsigned int& d1, const XchgParams& p,
-                                         int slot, int from, unsigned int* sh_fail) {
-  unsigned int f0, f1, spins = 0;
+// poll one LL unit (8 bytes {d0, ep}) or, pair = true, one 16-byte pair {d0, ep, d1, ep} until it carries `ep`; false after a
+// timeout / failure elsewhere in the block
+__device__ __forceinline__ bool ll_poll(const char* src, bool pair, unsigned int ep, unsigned int& d0, unsigned int& d1,
+                                        const XchgParams& p, int slot, int from, unsigned int* sh_fail) {
+  unsigned int f0, f1 = ep, spins = 0;
   unsigned long long t0 = 0;
   for (;;) {
-    asm volatile("ld.relaxed.sys.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(d0), "=r"(f0), "=r"(d1), "=r"(f1) : "l"(src) : "memory");
+    if (pair) asm volatile("ld.relaxed.sys.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(d0), "=r"(f0), "=r"(d1), "=r"(f1) : "l"(src) : "memory");
+    else asm volatile("ld.relaxed.sys.global.v2.u32 {%0, %1}, [%2];" : "=r"(d0), "=r"(f0) : "l"(src) : "memory");
     if (f0 == ep && f1 == ep) return true;
     __nanosleep(40);          // (a tight poll loop on every thread takes L2 bandwidth from the GEMM that shares the SM)
-    if ((++spins & 0xFFFu) == 0) {
-      if (*reinterpret_cast<volatile unsigned int*>(sh_fail)) return false;
-      if (p.timeout_ns != 0) {
-        const unsigned long long now = globaltimer_ns();
-        if (t0 == 0) t0 = now;
-        else if (now - t0 > p.timeout_ns) {
-          if (p.host_err != nullptr) { atomicCAS(p.host_err, 0u, 1u + 16u * slot + from); __threadfence_system(); }
-          *sh_fail = 1u;
-          return false;
-        }
-      }
-    }
+    if (xchg_give_up(spins, 0xFFFu, t0, p, slot, sh_fail, [&] { return from; })) { *sh_fail = 1u; return false; }
   }
-}
-__device__ __forceinline__ bool ll_poll1(const char* src, unsigned int ep, unsigned int& d0, const XchgParams& p, int slot, int from,
-                                         unsigned int* sh_fail) {
-  unsigned int f0, spins = 0;
-  unsigned long long t0 = 0;
-  for (;;) {
-    asm volatile("ld.relaxed.sys.global.v2.u32 {%0, %1}, [%2];" : "=r"(d0), "=r"(f0) : "l"(src) : "memory");
-    if (f0 == ep) return true;
-    __nanosleep(40);
-    if ((++spins & 0xFFFu) == 0) {
-      if (*reinterpret_cast<volatile unsigned int*>(sh_fail)) return false;
-      if (p.timeout_ns != 0) {
-        const unsigned long long now = globaltimer_ns();
-        if (t0 == 0) t0 = now;
-        else if (now - t0 > p.timeout_ns) {
-          if (p.host_err != nullptr) { atomicCAS(p.host_err, 0u, 1u + 16u * slot + from); __threadfence_system(); }
-          *sh_fail = 1u;
-          return false;
-        }
-      }
-    }
-  }
-}
-
-__device__ __forceinline__ bool run_is_vec(const OptWork& wk) {
-  return (wk.off & 3) == 0 && (wk.count & 3) == 0 &&
-         (wk.Wn == nullptr || ((wk.out_dim & 3) == 0 && ((wk.off - wk.mat_off) & 3) == 0 && (wk.ld_out & 3) == 0));
-}
-__device__ __forceinline__ int run_owner(int w, int sb, int se, int world) {
-  int q = static_cast<int>((static_cast<long long>(w - sb) * world) / (se - sb));
-  while (q + 1 < world && w >= xchg_share(sb, se, q + 1, world)) ++q;
-  while (q > 0 && w < xchg_share(sb, se, q, world)) --q;
-  return q;
 }
 
 // plain-bf16 nets only (one shadow part).  One block per SM at most: no block ever waits for another block of its own
 // grid, but it does wait for the peers' blocks, which must all be able to become resident beside whatever GEMM is running.
-template <int W, bool EXT, bool RP = false>
+template <int W, int G>
 static __global__ void __launch_bounds__(256, W <= 8 ? 3 : 2)
 xchg_ll_kernel(const LLParams lp) {
   const XchgParams& p = lp.x;
@@ -485,14 +410,10 @@ xchg_ll_kernel(const LLParams lp) {
   const unsigned int ep = p.desc->epoch;
   char* const my_base = p.peers->base[p.rank];
   float* const theta = reinterpret_cast<float*>(my_base);
-  if (p.host_scal != nullptr && blockIdx.x == 0 && threadIdx.x < SCAL_COUNT) {
-    p.host_scal[threadIdx.x] = p.scal[threadIdx.x];
-    if (threadIdx.x == 0 && p.desc->hist != nullptr) *p.desc->hist = make_float2(p.scal[SCAL_LOSS_SUM], p.scal[SCAL_NNZ]);
-    __threadfence_system();
-  }
+  publish_step_scalars(p.scal, p.host_scal, p.desc);
   const float lr_t = p.desc->lr_t, gs = p.desc->gscale;
-  const bool use_s1 = opt_uses_s1<EXT>(p.hyper.kind);
-  const bool use_s2 = opt_uses_s2<EXT>(p.hyper.kind);
+  const bool use_s1 = opt_uses_s1<G>(p.hyper.kind);
+  const bool use_s2 = opt_uses_s2<G>(p.hyper.kind);
   float* const s1 = reinterpret_cast<float*>(my_base + p.s1_off);
   float* const s2 = reinterpret_cast<float*>(my_base + p.s2_off);
   float* const my_grad = reinterpret_cast<float*>(my_base + p.grad_off);
@@ -521,7 +442,7 @@ xchg_ll_kernel(const LLParams lp) {
         dst[u] = nullptr;
         const int j = i0 + u;
         if (j >= n_other) continue;
-        const int w = sb + j + ((sb + j >= w0) ? (w1 - w0) : 0);
+        const int w = other_run(j, sb, w0, w1);
         const int q = run_owner(w, sb, se, p.world);
         const OptWork& wk = p.work[w];
         char* qb = p.peers->base[q] + lp.llg_off + p.rank * g_stride;
@@ -560,15 +481,16 @@ xchg_ll_kernel(const LLParams lp) {
     const int w0 = xchg_share(sb, se, p.rank, p.world), w1 = xchg_share(sb, se, p.rank + 1, p.world);
 #pragma unroll 1
     for (int w = w0 + static_cast<int>(blockIdx.x); w < w1 && alive; w += static_cast<int>(gridDim.x)) {
-      const OptWork wk = p.work[w];
-      const long long shadow_rel = wk.Wn != nullptr ? reinterpret_cast<char*>(wk.Wn) - my_base : 0;
+      // (a reference: the run's fields are read again after the poll instead of being held in registers across it, which
+      // spilled at the 80-register bound of W = 4 / 8)
+      const OptWork& wk = p.work[w];
       if (run_is_vec(wk)) {
         if (e < wk.count) {
           const long long idx = wk.off + e;
           const float4 own = *reinterpret_cast<const float4*>(my_grad + idx);
           const float4 th = *reinterpret_cast<const float4*>(theta + idx);
-          float4 a = use_s1 ? *reinterpret_cast<const float4*>(s1 + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
-          float4 b = use_s2 ? *reinterpret_cast<const float4*>(s2 + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
+          const float4 a = use_s1 ? *reinterpret_cast<const float4*>(s1 + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
+          const float4 b = use_s2 ? *reinterpret_cast<const float4*>(s2 + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
           float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
           const char* src = my_base + lp.llg_off + (idx >> 2) * 16;
           // the peers' entries are polled four ranks at a time with all loads of an attempt in flight together (one L2
@@ -589,31 +511,20 @@ xchg_ll_kernel(const LLParams lp) {
                   asm volatile("ld.relaxed.sys.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(hi[k].x), "=r"(hi[k].y), "=r"(hi[k].z), "=r"(hi[k].w) : "l"(src + q * g_stride + hi_plane) : "memory");
                 }
               }
+              auto ready = [&](int k) { return lo[k].y == ep && lo[k].w == ep && hi[k].y == ep && hi[k].w == ep; };
 #pragma unroll
               for (int k = 0; k < 4; ++k) {
                 const int q = q0 + k;
-                if (q < W && q < p.world && q != p.rank) ok = ok && lo[k].y == ep && lo[k].w == ep && hi[k].y == ep && hi[k].w == ep;
+                if (q < W && q < p.world && q != p.rank) ok = ok && ready(k);
               }
               if (ok) break;
               __nanosleep(40);
-              if ((++spins & 0xFFFu) == 0) {
-                if (*reinterpret_cast<volatile unsigned int*>(&sh_fail)) { alive = false; break; }
-                if (p.timeout_ns != 0) {
-                  const unsigned long long now = globaltimer_ns();
-                  if (t0 == 0) t0 = now;
-                  else if (now - t0 > p.timeout_ns) {
-                    int missing = q0;
-                    for (int k = 0; k < 4; ++k) {
-                      const int q = q0 + k;
-                      if (q < W && q < p.world && q != p.rank && !(lo[k].y == ep && lo[k].w == ep && hi[k].y == ep && hi[k].w == ep)) { missing = q; break; }
-                    }
-                    if (p.host_err != nullptr) { atomicCAS(p.host_err, 0u, 1u + 16u * slot + missing); __threadfence_system(); }
-                    sh_fail = 1u;
-                    alive = false;
-                    break;
-                  }
-                }
-              }
+              auto missing = [&] {      // the first rank of the four whose entry is not there
+                for (int k = 0; k < 4; ++k)
+                  if (q0 + k < W && q0 + k < p.world && q0 + k != p.rank && !ready(k)) return q0 + k;
+                return q0;
+              };
+              if (xchg_give_up(spins, 0xFFFu, t0, p, slot, &sh_fail, missing)) { sh_fail = 1u; alive = false; break; }
             }
             if (!alive) break;
 #pragma unroll
@@ -626,26 +537,14 @@ xchg_ll_kernel(const LLParams lp) {
             }
           }
           if (alive) {
-            float4 t;
-            t.x = opt_update<EXT, RP>(p.hyper, lr_t, th.x, acc.x * gs, a.x, b.x);
-            t.y = opt_update<EXT, RP>(p.hyper, lr_t, th.y, acc.y * gs, a.y, b.y);
-            t.z = opt_update<EXT, RP>(p.hyper, lr_t, th.z, acc.z * gs, a.z, b.z);
-            t.w = opt_update<EXT, RP>(p.hyper, lr_t, th.w, acc.w * gs, a.w, b.w);
-            *reinterpret_cast<float4*>(theta + idx) = t;
+            const float4 t = opt_apply4<G>(p.hyper, lr_t, gs, wk, idx, th, acc, a, b, theta, s1, s2);
             *reinterpret_cast<float4*>(my_grad + idx) = acc;      // the owner keeps the reduced gradient of its runs (parity hook)
-            if (use_s1) *reinterpret_cast<float4*>(s1 + idx) = a;
-            if (use_s2) *reinterpret_cast<float4*>(s2 + idx) = b;
             const long long sent = lp.lls_off + (idx >> 2) * 16;
             if (wk.Wn != nullptr) {
-              const long long m = idx - wk.mat_off;
-              const long long r = m / wk.out_dim;
-              uint2 o;
-              o.x = pack_bf16x2(t.x, t.y);
-              o.y = pack_bf16x2(t.z, t.w);
-              *reinterpret_cast<uint2*>(my_base + shadow_rel + (r * wk.ld_out + (m - r * wk.out_dim)) * 2) = o;
+              const unsigned int o0 = pack_bf16x2(t.x, t.y), o1 = pack_bf16x2(t.z, t.w);
 #pragma unroll
               for (int q = 0; q < W; ++q)
-                if (q < p.world && q != p.rank) ll_store2(p.peers->base[q] + sent, o.x, o.y, ep);
+                if (q < p.world && q != p.rank) ll_store2(p.peers->base[q] + sent, o0, o1, ep);
             } else {
 #pragma unroll
               for (int q = 0; q < W; ++q)
@@ -667,27 +566,17 @@ xchg_ll_kernel(const LLParams lp) {
           for (int q = 0; q < p.world; ++q) {
             float v = my_grad[idx];
             if (q != p.rank) {
-              unsigned int d0;
-              if (!ll_poll1(my_base + lp.llg_off + q * g_stride + uoff, ep, d0, p, slot, q, &sh_fail)) { alive = false; break; }
+              unsigned int d0, d1;
+              if (!ll_poll(my_base + lp.llg_off + q * g_stride + uoff, false, ep, d0, d1, p, slot, q, &sh_fail)) { alive = false; break; }
               v = __uint_as_float(d0);
             }
             acc = (q == 0) ? v : acc + v;
           }
           if (!alive) break;
-          float a = use_s1 ? s1[idx] : 0.f, b = use_s2 ? s2[idx] : 0.f;
-          const float t = opt_update<EXT, RP>(p.hyper, lr_t, theta[idx], acc * gs, a, b);
-          theta[idx] = t;
+          const float a = use_s1 ? s1[idx] : 0.f, b = use_s2 ? s2[idx] : 0.f;
+          const float t = opt_apply1<G>(p.hyper, lr_t, gs, wk, idx, theta[idx], acc, a, b, theta, s1, s2);
           my_grad[idx] = acc;
-          if (use_s1) s1[idx] = a;
-          if (use_s2) s2[idx] = b;
-          unsigned int bits = __float_as_uint(t);
-          if (wk.Wn != nullptr) {
-            const long long m = idx - wk.mat_off;
-            const long long r = m / wk.out_dim;
-            const __nv_bfloat16 hv = __float2bfloat16_rn(t);
-            *reinterpret_cast<__nv_bfloat16*>(my_base + shadow_rel + (r * wk.ld_out + (m - r * wk.out_dim)) * 2) = hv;
-            bits = static_cast<unsigned int>(*reinterpret_cast<const unsigned short*>(&hv));
-          }
+          const unsigned int bits = wk.Wn != nullptr ? static_cast<unsigned int>(__bfloat16_as_ushort(__float2bfloat16_rn(t))) : __float_as_uint(t);
           for (int q = 0; q < p.world; ++q)
             if (q != p.rank) ll_store1(p.peers->base[q] + lp.lls_off + uoff, bits, ep);
         }
@@ -705,22 +594,19 @@ xchg_ll_kernel(const LLParams lp) {
     const int n_other = (se - sb) - (w1 - w0);
 #pragma unroll 1
     for (int j = static_cast<int>(blockIdx.x); j < n_other && alive; j += static_cast<int>(gridDim.x)) {
-      const int w = sb + j + ((sb + j >= w0) ? (w1 - w0) : 0);
+      const int w = other_run(j, sb, w0, w1);
       const int q = run_owner(w, sb, se, p.world);
       const OptWork wk = p.work[w];
-      const long long shadow_rel = wk.Wn != nullptr ? reinterpret_cast<char*>(wk.Wn) - my_base : 0;
       if (run_is_vec(wk)) {
         if (e < wk.count) {
           const long long idx = wk.off + e;
           const char* src = my_base + lp.lls_off + (idx >> 2) * 16;
           unsigned int d0, d1, d2, d3;
-          if (!ll_poll2(src, ep, d0, d1, p, slot, q, &sh_fail)) { alive = false; break; }
+          if (!ll_poll(src, true, ep, d0, d1, p, slot, q, &sh_fail)) { alive = false; break; }
           if (wk.Wn != nullptr) {
-            const long long m = idx - wk.mat_off;
-            const long long r = m / wk.out_dim;
-            *reinterpret_cast<uint2*>(my_base + shadow_rel + (r * wk.ld_out + (m - r * wk.out_dim)) * 2) = make_uint2(d0, d1);
+            *reinterpret_cast<uint2*>(wk.Wn + shadow_at(wk, idx)) = make_uint2(d0, d1);
           } else {
-            if (!ll_poll2(src + hi_plane, ep, d2, d3, p, slot, q, &sh_fail)) { alive = false; break; }
+            if (!ll_poll(src + hi_plane, true, ep, d2, d3, p, slot, q, &sh_fail)) { alive = false; break; }
             *reinterpret_cast<float4*>(theta + idx) = make_float4(__uint_as_float(d0), __uint_as_float(d1), __uint_as_float(d2), __uint_as_float(d3));
           }
         }
@@ -729,12 +615,10 @@ xchg_ll_kernel(const LLParams lp) {
           const int es = threadIdx.x + 256 * i;
           if (es >= wk.count) continue;
           const long long idx = wk.off + es;
-          unsigned int d0;
-          if (!ll_poll1(my_base + lp.lls_off + unit_off(idx), ep, d0, p, slot, q, &sh_fail)) { alive = false; break; }
+          unsigned int d0, d1;
+          if (!ll_poll(my_base + lp.lls_off + unit_off(idx), false, ep, d0, d1, p, slot, q, &sh_fail)) { alive = false; break; }
           if (wk.Wn != nullptr) {
-            const long long m = idx - wk.mat_off;
-            const long long r = m / wk.out_dim;
-            *reinterpret_cast<unsigned short*>(my_base + shadow_rel + (r * wk.ld_out + (m - r * wk.out_dim)) * 2) = static_cast<unsigned short>(d0);
+            *reinterpret_cast<unsigned short*>(wk.Wn + shadow_at(wk, idx)) = static_cast<unsigned short>(d0);
           } else {
             theta[idx] = __uint_as_float(d0);
           }
@@ -754,12 +638,8 @@ gather_master_kernel(const XchgParams p, int what) {
   const int w = blockIdx.x;
   float* const theta = reinterpret_cast<float*>(p.peers->base[p.rank]);
   int owner = -1;
-  for (int slot = 0; slot < p.n_slots; ++slot) {
-    if (w >= p.slot_begin[slot] && w < p.slot_end[slot]) {
-      for (int r = 0; r < p.world; ++r)
-        if (w >= xchg_share(p.slot_begin[slot], p.slot_end[slot], r, p.world) && w < xchg_share(p.slot_begin[slot], p.slot_end[slot], r + 1, p.world)) owner = r;
-    }
-  }
+  for (int slot = 0; slot < p.n_slots; ++slot)
+    if (w >= p.slot_begin[slot] && w < p.slot_end[slot]) owner = run_owner(w, p.slot_begin[slot], p.slot_end[slot], p.world);
   if (owner < 0 || owner == p.rank) return;
   const OptWork wk = p.work[w];
   char* const my_base = p.peers->base[p.rank];

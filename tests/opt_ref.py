@@ -48,7 +48,7 @@ NPARTS = {FP32: 1, BF16: 1, FP32_TC: 3, BF16X2: 2}
 ADADELTA, ADAM, SGD, MOMENTUM, ADAGRAD, RMSPROP, FTRL = 0, 1, 2, 3, 4, 5, 6
 ONAME = {ADADELTA: "adadelta", ADAM: "adam", SGD: "sgd", MOMENTUM: "momentum", ADAGRAD: "adagrad", RMSPROP: "rmsprop",
          FTRL: "ftrl"}
-EXT = (ADAGRAD, RMSPROP, FTRL)          # opt_ext: the rules of the <true> instantiations
+EXT = (ADAGRAD, RMSPROP, FTRL)          # opt_group: the rules of the OPT_EXT instantiations
 U = 2.0 ** -24
 C_BOUND = 16.0
 RHO, EPS, BETA1, BETA2, MOM = 0.95, 1e-8, 0.9, 0.999, 0.9

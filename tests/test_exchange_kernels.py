@@ -29,7 +29,7 @@ Co-residency: every exchange block of every rank must be resident at once (they 
 exchange kernels runs here, so W x grid <= SM count is asserted before each launch; W >= 5 runs at most 8 blocks per
 rank.  The kernel each launch ran ("xchg_ll<4>", "xchg_update<16>", ...) is checked against the instantiation the world
 size selects, and the case matrix reaches both kernels at W = 2, 4, 8 and 16 with the reference's four rules
-(<W, false>) and at W = 2 and 3 (U = 2 and U = 1 update loops) with Adagrad, RMSProp and FTRL (<W, true>)."""
+(<W, OPT_BASE>) and at W = 2 and 3 (U = 2 and U = 1 update loops) with Adagrad, RMSProp and FTRL (<W, OPT_EXT>)."""
 import ctypes as C
 import zlib
 
@@ -315,7 +315,7 @@ def _cases():
         out.append((16, prec, MOMENTUM, "tiny", "each", -2, 0.0, False))
     for W, prec, net in ((3, FP32, "odd"), (5, BF16, "m8"), (2, FP32_TC, "odd"), (16, BF16, "odd")):   # no rounding anywhere
         out.append((W, prec, SGD, net, "all", 0 if W <= 4 else -2, 0.25, True))
-    for opt in EXT:                                             # the <W, true> instantiations: U = 2 and U = 1, both protocols
+    for opt in EXT:                                             # the <W, OPT_EXT> instantiations: U = 2 and U = 1, both protocols
         for W, prec, net, plan in ((2, BF16, "m8", "all"), (3, BF16, "odd", "each"), (2, FP32, "odd", "each"),
                                    (3, FP32, "m8", "all"), (3, FP32_TC, "odd", "all"), (2, BF16X2, "m8", "step")):
             out.append((W, prec, opt, net, plan, 0, 0.0, False))
@@ -356,7 +356,7 @@ def test_exchange_against_float64(sb, monkeypatch, case):
 
 
 def test_case_matrix_reaches_every_instantiation():
-    # kernel_name names both optimizer groups alike: <W, false> for the reference's four rules, <W, true> for the others
+    # kernel_name names both optimizer groups alike: <W, OPT_BASE> for the reference's four rules, <W, OPT_EXT> for the others
     routes = {(kernel_name(c[0], c[1]), c[2] in EXT) for c in CASES}
     want = {("xchg_%s<%d>" % (k, w), False) for k in ("ll", "update") for w in (2, 4, 8, 16)}
     want |= {("xchg_%s<%d>" % (k, w), True) for k in ("ll", "update") for w in (2, 4)}

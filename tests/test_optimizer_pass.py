@@ -1,4 +1,4 @@
-"""Kernel-level checks of the single-GPU optimizer pass (optimizer_kernel<false / true> in csrc/kernels.cuh) and of the
+"""Kernel-level checks of the single-GPU optimizer pass (optimizer_kernel<OPT_BASE / OPT_EXT> in csrc/kernels.cuh) and of the
 bf16 shadow refresh (shadow_refresh_kernel), through the trainer's own launch code.
 
 Each pass case builds a world-1 trainer, writes its raw arena buffers (sb_debug_trainer_buffer): theta, s1 and s2, every

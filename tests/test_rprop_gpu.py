@@ -79,7 +79,7 @@ def test_state_starts_at_zero_and_the_learning_rate(sb, prec):
             t.close()
 
 
-# ---- the single-GPU pass (optimizer_kernel<true>) ----
+# ---- the single-GPU pass (optimizer_kernel<OPT_RPROP>) ----
 def _pass_cases():
     out = []
     for prec in PRECS:
@@ -149,7 +149,7 @@ def test_optimizer_pass_is_the_rule_bit_for_bit(sb, case):
         t.close()
 
 
-# ---- the peer exchange (xchg_update_kernel<W, true>, xchg_ll_kernel<W, true>) ----
+# ---- the peer exchange (xchg_update_kernel<W, OPT_RPROP>, xchg_ll_kernel<W, OPT_RPROP>) ----
 @pytest.mark.parametrize("plan", ["all", "each"])
 @pytest.mark.parametrize("net", ["m8", "odd"])
 @pytest.mark.parametrize("prec", [FP32, BF16], ids=lambda p: PNAME[p])
