@@ -108,6 +108,8 @@ const char* sb_version(void);
 const char* sb_last_error(void);
 /* number of visible CUDA devices with compute capability 10.x; <0 on error */
 int sb_device_count(void);
+/* free and total device memory of `device` (cudaMemGetInfo), e.g. to tell beforehand whether a set will fit in HBM */
+int sb_device_mem_info(int device, uint64_t* free_bytes, uint64_t* total_bytes);
 /* pinned host memory for callers that want true async H2D (JNI direct buffers) */
 int sb_host_alloc(void** ptr, uint64_t bytes);
 int sb_host_free(void* ptr);
@@ -211,8 +213,17 @@ int sb_trainer_apply_accumulated_mean(sb_trainer_t* t, int64_t total_pushes);
 
 /* HBM-resident training set: load_data + np.array_split (ssgd_monitor.py:186-192) keep the whole
  * set in RAM and slice mini-batches from it; here the set lives in HBM and each step reads its
- * rows [row_offset, row_offset+rows) from there.  Calling load again replaces the set. */
+ * rows [row_offset, row_offset+rows) from there.  Calling load again replaces the set.
+ * Placement: X goes to HBM when it fits in the free device memory beside a reserve (16 bytes per row for y, w, the n_nz
+ * prefix counts and a row order, the conversion windows, and as much again as the trainer's step buffers).  A set that
+ * does not fit is kept in mapped pinned host memory in the same layout (tensor-core modes: the bf16 parts, bit for bit
+ * what HBM would hold; fp32 mode: the fp32 rows); y, w and the prefix counts stay in HBM.  Steps over a host set read
+ * their batch's rows over PCIe first (tensor-core modes: gather_batch_kernel into the step's batch buffer; fp32 mode:
+ * the host-batch load kernel), and compute exactly what they compute over the same set in HBM.  If the pinned
+ * allocation fails the call returns SB_ERR_CUDA with the byte count it asked for, and no set is loaded. */
 int sb_trainer_load_dataset(sb_trainer_t* t, const float* X, const float* y, const float* w, int64_t n_rows);
+/* 1 when the loaded set's X lives in pinned host memory, 0 when it is in HBM or no set is loaded */
+int sb_trainer_dataset_on_host(const sb_trainer_t* t);
 /* (X / y / w of sb_trainer_load_dataset, sb_trainer_eval_loss and sb_trainer_predict may be HOST or DEVICE pointers on the
  * trainer's device: sb_text_parse_device hands the parsed set over without a host round trip.) */
 int sb_trainer_step_resident(sb_trainer_t* t, int64_t row_offset, int32_t rows, float* loss_out);
@@ -477,7 +488,7 @@ int sb_debug_embed(int32_t precision, int32_t scatter, const float* We, const in
  *   SB_DEBUG_BUF_BATCH_X: layer 0's batch operand.  Tensor-core modes: Xb as uint16 bits [np, max_batch, ldx] with
  *     ldx = round_up(F, 8), or round_up(n_dense, 8) once sb_trainer_set_sparse was called; fp32 mode: Xf [max_batch, F].
  *   SB_DEBUG_BUF_BATCH_Y / _W: float[max_batch], the labels / weights a step's descriptor points at: ordY / ordW of
- *     ordered steps while a row order is set, else the host staging buffers (a host step without w reads ones instead).
+ *     ordered steps while a row order is set or the bf16 set is in host memory, else the host staging buffers (a host step without w reads ones instead).
  *   SB_DEBUG_BUF_SCAL: float[4], the step scalars of descriptor slot (0, 0) (loss sum, n_nz, 2 unused).
  *   SB_DEBUG_BUF_DS_X: the resident set: uint16 bits [np, ds_rows, round_up(F, 8)] (tensor-core modes) or float
  *     [ds_rows, F] (fp32 mode); _DS_Y / _DS_W: float[ds_rows]; _DS_P: int32[ds_rows + 1], the prefix counts of the
@@ -508,6 +519,9 @@ int sb_debug_trainer_buffer(sb_trainer_t* t, int32_t which, void* host, int64_t 
  * bf16-resident batch, whose descriptor write publishes n_nz and layer 0 reads the set in place.  Changes neither the step count nor any captured step.  Read the results with sb_debug_trainer_buffer. */
 int sb_debug_first_kernel(sb_trainer_t* t, const float* X, const float* y, const float* w, const int32_t* idx, int64_t row_offset,
                           int32_t rows, int32_t clear, char* route, int32_t route_cap);
+/* on = 1: the next sb_trainer_load_dataset places the set in pinned host memory whatever its size (0: by size, the
+ * default), so that the host-memory path can be compared with the same set in HBM.  A test hook, not an option. */
+int sb_debug_force_host_set(sb_trainer_t* t, int32_t on);
 /* Queue one exchange of the slots in slot_mask exactly as a step does, and return without waiting: the descriptor of
  * the next update (global step + 1 and its lr_t, gradient scale `gscale` (0: 1 / world), epoch + 1), then the step's
  * exchange launch on the trainer's stream - its slot and work tables, grid rule (alone: as the last launch of a step)

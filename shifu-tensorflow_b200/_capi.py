@@ -6,6 +6,7 @@ import fails loudly - there is no Python / CPU fallback.
 from __future__ import annotations
 
 import ctypes as C
+import logging
 import os
 from typing import Optional, Sequence
 
@@ -92,6 +93,7 @@ PROTOTYPES = {
     "sb_version": (C.c_char_p, []),
     "sb_last_error": (C.c_char_p, []),
     "sb_device_count": (C.c_int, []),
+    "sb_device_mem_info": (C.c_int, [C.c_int, _P(C.c_uint64), _P(C.c_uint64)]),
     "sb_host_alloc": (C.c_int, [_P(_vp), C.c_uint64]),
     "sb_host_free": (C.c_int, [_vp]),
     "sb_nccl_unique_id": (C.c_int, [_vp]),
@@ -122,6 +124,7 @@ PROTOTYPES = {
     "sb_trainer_loss_resident": (C.c_int, [_vp, C.c_int64, C.c_int32, _f32p]),
     "sb_trainer_broadcast_state": (C.c_int, [_vp, C.c_int32]),
     "sb_trainer_load_dataset": (C.c_int, [_vp, _f32p, _f32p, _f32p, C.c_int64]),
+    "sb_trainer_dataset_on_host": (C.c_int, [_vp]),
     "sb_trainer_step_resident": (C.c_int, [_vp, C.c_int64, C.c_int32, _f32p]),
     "sb_trainer_step_resident_async": (C.c_int, [_vp, C.c_int64, C.c_int32]),
     "sb_trainer_run_resident": (C.c_int, [_vp, C.POINTER(C.c_int64), C.c_int32, C.c_int32]),
@@ -184,6 +187,7 @@ PROTOTYPES = {
     "sb_debug_trainer_buffer": (C.c_int, [_vp, C.c_int32, _vp, C.c_int64, C.c_int32]),
     "sb_debug_first_kernel": (C.c_int, [_vp, _f32p, _f32p, _f32p, _P(C.c_int32), C.c_int64, C.c_int32, C.c_int32, C.c_char_p,
                                         C.c_int32]),
+    "sb_debug_force_host_set": (C.c_int, [_vp, C.c_int32]),
     "sb_debug_exchange": (C.c_int, [_vp, C.c_int32, C.c_float, C.c_int32, C.c_int32, _f32p, _P(C.c_int32), C.c_char_p,
                                     C.c_int32]),
     "sb_debug_exchange_layout": (C.c_int, [_vp, _P(C.c_int32), C.c_int32, _P(C.c_int64), C.c_int64, _P(C.c_int32)]),
@@ -474,6 +478,17 @@ class Trainer:
         X, y, w, rows = self._xyw(X, y, w)
         check(lib().sb_trainer_load_dataset(self._h, _ptr(X), _ptr(y), _ptr(w), rows))
         self.dataset_rows = rows
+        logging.info("resident set: %d rows placed in %s" % (rows, "pinned host memory (each step reads its rows over PCIe)"
+                                                              if self.dataset_on_host else "HBM"))
+
+    @property
+    def dataset_on_host(self) -> bool:
+        """True when the loaded set did not fit in device memory and lives in pinned host memory (load_dataset)"""
+        return lib().sb_trainer_dataset_on_host(self._h) == 1
+
+    def debug_force_host_set(self, on: bool = True):
+        """test hook: the next load_dataset places the set in pinned host memory whatever its size"""
+        check(lib().sb_debug_force_host_set(self._h, int(bool(on))))
 
     def step_resident(self, row_offset: int, rows: int) -> float:
         loss = C.c_float()
@@ -714,6 +729,13 @@ def nccl_unique_id() -> bytes:
 
 def device_count() -> int:
     return int(lib().sb_device_count())
+
+
+def device_mem_info(device: int = 0):
+    """-> (free, total) bytes of device memory (cudaMemGetInfo)"""
+    f, t = C.c_uint64(), C.c_uint64()
+    check(lib().sb_device_mem_info(int(device), C.byref(f), C.byref(t)))
+    return int(f.value), int(t.value)
 
 
 def savedmodel_write(export_dir: str, desc: NetDesc, flat_params) -> None:

@@ -63,11 +63,24 @@ struct sb_trainer {
   float2* h_hist = nullptr;
   float2* d_hist = nullptr;
   float2* hist_slot(long long step) { return d_hist ? d_hist + (step % HIST) : nullptr; }
-  // HBM-resident training set
+  // Resident training set.  dsX / dsXb live in HBM, or, when the set does not fit there (or force_host, the test hook
+  // sb_debug_force_host_set), in mapped pinned host memory (ds_host) that the steps read over PCIe; y, w and P are always
+  // in HBM.
   float *dsX = nullptr, *dsY = nullptr, *dsW = nullptr;   // dsX only in fp32 mode
   __nv_bfloat16* dsXb = nullptr;                           // bf16 mode: the set in GEMM-operand form [ds_rows, ldF]
   int* dsP = nullptr;                                      // prefix counts of non-zero weights [ds_rows + 1]
   long long ds_rows = 0;
+  bool ds_host = false, force_host = false;
+  int* ds_iota = nullptr;   // bf16 set in host memory: the identity order its steps gather through without a row order
+  // Streamed steps (a bf16 set in host memory): step k of a graph computes from batch buffer k & 1 - Xb / ordY / ordW
+  // (k even) or Xb2 / ordY2 / ordW2 (k odd).  Inside a run_resident graph the rows of step k + 1 are fetched on
+  // fetch_stream into the other buffer while step k runs, on fetch_ctas CTAs, with step k's GEMM grids planned for the
+  // remaining SMs.
+  __nv_bfloat16* Xb2 = nullptr;
+  float *ordY2 = nullptr, *ordW2 = nullptr;
+  cudaStream_t fetch_stream = nullptr;
+  cudaEvent_t ev_fork = nullptr, ev_fetched = nullptr;
+  int fetch_ctas = 16;
   // row order of the resident set (sb_trainer_set_row_order): the resident entry points address logical row r as row
   // ord[r] (int32 on the device, the only per-row memory an order costs); ord_n == 0: physical order
   int* ord = nullptr;
@@ -145,12 +158,14 @@ struct sb_trainer {
     destroy_event(ev_join);
     destroy_event(ev_da_done);
     for (int i = 0; i < SB_XCHG_SLOTS; ++i) { destroy_event(ev_x[i]); destroy_event(ev_c[i]); }
+    destroy_event(ev_fork);
+    destroy_event(ev_fetched);
     for (int i = 0; i < 2; ++i) {
       destroy_event(ev_copied[i]); destroy_event(ev_consumed[i]);
       destroy_event(ev_prep[i]); destroy_event(ev_pos[i]);
     }
     if (prep) cudaStreamSynchronize(prep);
-    for (cudaStream_t s : {xstream[0], xstream[1], side, prep, copy_stream}) if (s) cudaStreamDestroy(s);
+    for (cudaStream_t s : {xstream[0], xstream[1], side, prep, copy_stream, fetch_stream}) if (s) cudaStreamDestroy(s);
     if (h_scal) cudaFreeHost(h_scal);
     if (h_err) cudaFreeHost(h_err);
     if (h_hist) cudaFreeHost(h_hist);
@@ -165,8 +180,11 @@ struct sb_trainer {
     graphs.clear();
   }
   void free_dataset() {
-    if (dsX) cudaFree(dsX);
-    if (dsXb) cudaFree(dsXb);
+    void* x = dsXb ? static_cast<void*>(dsXb) : static_cast<void*>(dsX);
+    if (x) { if (ds_host) cudaFreeHost(x); else cudaFree(x); }
+    ds_host = false;
+    if (ds_iota) cudaFree(ds_iota);
+    ds_iota = nullptr;
     if (dsP) cudaFree(dsP);
     if (dsY) cudaFree(dsY);
     if (dsW) cudaFree(dsW);
@@ -179,8 +197,14 @@ struct sb_trainer {
     ord_n = ord_cap = 0;
   }
   long long resident_len() const { return ord_n > 0 ? ord_n : ds_rows; }   // what resident offsets are checked against
-  // the feed of a resident step: the fp32 set is read in place through the host-batch graph
-  Feed resident_feed() const { return ord_n > 0 ? Feed::ORDERED : dsXb ? Feed::RESIDENT : Feed::HOST; }
+  // resident steps gather their batch into Xb / Xf first: through the row order, or, from a bf16 set in host memory, whose
+  // rows layer 0's GEMMs cannot read by TMA, through the row order or the identity order ds_iota
+  bool streamed() const { return ds_host && dsXb; }
+  bool gathers() const { return ord_n > 0 || streamed(); }
+  // the feed of a resident step: the fp32 set (in HBM or host memory) is read in place through the host-batch graph
+  Feed resident_feed() const {
+    return streamed() ? Feed::STREAMED : ord_n > 0 ? Feed::ORDERED : dsXb ? Feed::RESIDENT : Feed::HOST;
+  }
   void close_peer_mappings() {
     for (void* p : peer_bases) cudaIpcCloseMemHandle(p);
     peer_bases.clear();
@@ -241,9 +265,10 @@ static int resident_batch(const sb_trainer* t, long long off, int rows, int step
   *b = Batch{};
   b->feed = t->resident_feed();
   b->rows = rows;
-  if (b->feed == Feed::ORDERED) {   // gather_batch_kernel counts n_nz and fills ordY / ordW
+  if (b->feed == Feed::ORDERED || b->feed == Feed::STREAMED) {   // gather_batch_kernel counts n_nz and fills ordY / ordW
+    // (a streamed step of a run_resident graph reads buffer k & 1: stream_buffer)
     b->y = t->ordY; b->w = t->ordW;
-    b->order = t->ord + off;
+    b->order = (t->ord_n > 0 ? t->ord : t->ds_iota) + off;
     return SB_OK;
   }
   b->y = t->dsY + off; b->w = t->dsW + off;
@@ -611,22 +636,28 @@ static int enqueue_step_backward(sb_trainer* t, const StepIn& in, int rows, int 
 
 // first kernel of an ordered step, in load_batch_kernel's place: the batch's rows of the resident set through the order
 // slice in.desc->order into Xb / Xf, ordY / ordW and the step scalars; clears clear[0, clear_n) on the way
-static int enqueue_gather(sb_trainer* t, const StepIn& in, int rows, float* clear, long long clear_n) {
+// buf: batch buffer 0 (Xb / ordY / ordW) or 1 (a streamed step's second buffer); on stream st (null: the main stream,
+// PDL-chained, at most 16 blocks per SM), else on st with at most `ctas` blocks
+static int enqueue_gather(sb_trainer* t, const StepIn& in, int rows, float* clear, long long clear_n, int buf = 0,
+                          cudaStream_t st = nullptr, int ctas = 0) {
   Net& n = t->net;
   GatherParams p = {};
   p.desc = in.desc;
   p.rows = rows; p.F = n.F; p.ldF = n.ldF; p.np = n.nparts;
-  p.src_b = t->dsXb; p.src_ps = n.resident_ps; p.Xb = n.Xb; p.Xb_ps = n.Xb_ps;
+  p.src_b = t->dsXb; p.src_ps = n.resident_ps; p.Xb = buf ? t->Xb2 : n.Xb; p.Xb_ps = n.Xb_ps;
   p.src_f = t->dsX; p.Xf = n.Xf;
-  p.src_y = t->dsY; p.src_w = t->dsW; p.y = t->ordY; p.w = t->ordW;
+  p.src_y = t->dsY; p.src_w = t->dsW; p.y = buf ? t->ordY2 : t->ordY; p.w = buf ? t->ordW2 : t->ordW;
   p.scal = in.scal;
   p.zero_buf = clear; p.zero_n = clear_n;
-  p.trace = n.next_trace("gather_batch");
+  p.trace = n.next_trace(st ? "fetch_batch" : "gather_batch");
   const long long units = static_cast<long long>(rows) * (n.tc() ? n.ldF / 8 : (n.F + 3) / 4);
-  const long long blocks = std::max(1LL, std::min((units + 255) / 256, static_cast<long long>(n.num_sms) * 16));
+  const long long cap = st ? ctas : static_cast<long long>(n.num_sms) * 16;
+  const long long blocks = std::max(1LL, std::min((units + 255) / 256, cap));
   const dim3 g(static_cast<unsigned>(blocks));
-  if (n.tc()) SB_TRY(launch_kernel(gather_batch_kernel<true>, g, dim3(256), 0, n.stream, true, p));
-  else SB_TRY(launch_kernel(gather_batch_kernel<false>, g, dim3(256), 0, n.stream, true, p));
+  const bool pdl = st == nullptr;
+  if (!st) st = n.stream;
+  if (n.tc()) SB_TRY(launch_kernel(gather_batch_kernel<true>, g, dim3(256), 0, st, pdl, p));
+  else SB_TRY(launch_kernel(gather_batch_kernel<false>, g, dim3(256), 0, st, pdl, p));
   n.mark(n.tc() ? "gather_batch<bf16>" : "gather_batch<fp32>");
   return SB_OK;
 }
@@ -636,8 +667,24 @@ static int enqueue_gather(sb_trainer* t, const StepIn& in, int rows, float* clea
 // clear[0, clear_n) on the way.
 static int enqueue_first(Net& n, sb_trainer* t, const StepIn& in, int rows, float* clear, long long clear_n) {
   if (in.feed == Feed::RESIDENT) return SB_OK;
-  if (in.feed == Feed::ORDERED) return enqueue_gather(t, in, rows, clear, clear_n);
+  if (in.feed == Feed::ORDERED || in.feed == Feed::STREAMED) return enqueue_gather(t, in, rows, clear, clear_n);
   return n.enqueue_load(in, rows, clear, clear_n);
+}
+
+// A streamed step k of a graph of `steps` reads batch buffer k & 1.  Step 0's rows are fetched first, on the main stream
+// with the whole GPU; the rows of step k + 1 are fetched on fetch_stream while step k runs (forked behind step k - 1,
+// the last reader of that buffer), and step k + 1 waits for them.  The fetch clears no gradient: step k still
+// accumulates into it.
+static int enqueue_streamed_fetch(sb_trainer* t, int set, int k, int steps, int rows) {
+  Net& n = t->net;
+  if (k == 0) SB_TRY(enqueue_gather(t, t->slot(set, 0, Feed::STREAMED), rows, nullptr, 0));
+  else SB_CUDA(cudaStreamWaitEvent(n.stream, t->ev_fetched, 0));
+  if (k + 1 < steps) {
+    SB_TRY(join_streams(t->fetch_stream, n.stream, t->ev_fork));
+    SB_TRY(enqueue_gather(t, t->slot(set, k + 1, Feed::STREAMED), rows, nullptr, 0, (k + 1) & 1, t->fetch_stream, t->fetch_ctas));
+    SB_CUDA(cudaEventRecord(t->ev_fetched, t->fetch_stream));
+  }
+  return SB_OK;
 }
 
 // the body of one step as a sequence of stream operations (captured into a CUDA graph)
@@ -646,7 +693,7 @@ static int enqueue_step_body(sb_trainer* t, const StepIn& in, int rows, int kind
   n.trace_k = 0;
   float4* clear = nullptr;
   long long clear_n4 = 0;
-  if (in.feed == Feed::RESIDENT) {
+  if (in.feed == Feed::RESIDENT || in.feed == Feed::STREAMED) {
     // no first kernel to clear the gradient buffer.  It is first written by the last forward layer's epilogue, so with
     // more than one hidden layer the layer-0 forward GEMM clears it (its producer warpgroup's idle warps, beside the main
     // loop) instead of a memset node at the head of the chain.
@@ -657,7 +704,7 @@ static int enqueue_step_body(sb_trainer* t, const StepIn& in, int rows, int kind
       SB_CUDA(cudaMemsetAsync(t->grad, 0, sizeof(float) * n.n_params, n.stream));
     }
   }
-  SB_TRY(enqueue_first(n, t, in, rows, t->grad, n.n_params));   // also clears the step scalars
+  if (in.feed != Feed::STREAMED) SB_TRY(enqueue_first(n, t, in, rows, t->grad, n.n_params));   // also clears the step scalars
   bool fused_out = false;
   SB_TRY(n.enqueue_hidden_forward(in, rows, t->grad, &fused_out, clear, clear_n4));
   if (!fused_out) SB_TRY(n.enqueue_out(in, rows, true, true, nullptr, t->grad));
@@ -673,12 +720,23 @@ static int get_graph(sb_trainer* t, const GraphKey& key, cudaGraphExec_t* out) {
   cudaGraph_t g = nullptr;
   SB_CUDA(cudaStreamBeginCapture(n.stream, cudaStreamCaptureModeThreadLocal));
   int s = SB_OK;
+  // a streamed graph of several steps overlaps each fetch with the previous step: its GEMM grids leave fetch_ctas SMs free
+  const int sms = n.num_sms;
+  const bool overlap = key.feed == Feed::STREAMED && key.steps > 1;
+  if (overlap) n.num_sms = sms - t->fetch_ctas;
+  __nv_bfloat16* const xb0 = n.Xb;
   for (int k = 0; k < key.steps && s == SB_OK; ++k) {
     // (SB_STEP_TRACE: of a run, an interior step is the one traced - it starts behind the previous step's tail, as most
     // steps of a run do)
     n.trace_on = key.steps == 1 || k == 1;
-    s = enqueue_step_body(t, t->slot(key.set, k, key.feed), key.rows, key.kind);
+    if (key.feed == Feed::STREAMED) {
+      s = enqueue_streamed_fetch(t, key.set, k, key.steps, key.rows);
+      n.Xb = (k & 1) ? t->Xb2 : xb0;     // the buffer layer 0's forward and dW GEMMs read
+    }
+    if (s == SB_OK) s = enqueue_step_body(t, t->slot(key.set, k, key.feed), key.rows, key.kind);
   }
+  n.Xb = xb0;
+  n.num_sms = sms;
   n.trace_on = true;
   cudaError_t e = cudaStreamEndCapture(n.stream, &g);
   if (s != SB_OK) { if (g) cudaGraphDestroy(g); return s; }
@@ -731,7 +789,7 @@ static int run_step(sb_trainer* t, const Batch& b, int kind) {
   t->started = true;
   SB_CHECK(b.rows > 0 && b.rows <= n.max_batch, SB_ERR_INVALID, "rows=%d outside (0, max_batch=%d]", b.rows, n.max_batch);
   SB_CUDA(cudaSetDevice(n.device));
-  const bool prefetch = b.feed == Feed::RESIDENT || b.feed == Feed::ORDERED;
+  const bool prefetch = b.feed == Feed::RESIDENT || b.feed == Feed::ORDERED || b.feed == Feed::STREAMED;
   const int set = prefetch ? static_cast<int>(t->prefetches & 1) : 0;
   cudaGraphExec_t ge = nullptr;
   SB_TRY(get_graph(t, GraphKey{b.rows, kind, b.feed, 1, set}, &ge));
@@ -853,6 +911,15 @@ int sb_device_count(void) {
     if (cudaGetDeviceProperties(&p, i) == cudaSuccess && p.major == 9 && p.minor == 0) ++ok;
   }
   return ok;
+}
+
+int sb_device_mem_info(int device, uint64_t* free_bytes, uint64_t* total_bytes) {
+  SB_CHECK(free_bytes && total_bytes, SB_ERR_INVALID, "null argument");
+  SB_CUDA(cudaSetDevice(device));
+  size_t f = 0, t = 0;
+  SB_CUDA(cudaMemGetInfo(&f, &t));
+  *free_bytes = f; *total_bytes = t;
+  return SB_OK;
 }
 
 int sb_host_alloc(void** ptr, uint64_t bytes) {
@@ -985,6 +1052,11 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
   memset(t->h_err, 0, sizeof(unsigned int) * 4);
   if (const char* e = getenv("SB_XCHG_TIMEOUT_S")) t->xchg_timeout_ns = static_cast<unsigned long long>(atof(e) * 1e9);
   if (const char* e = getenv("SB_XCHG_BLOCKS")) t->xchg_blocks = atoi(e);
+  // CTAs of a streamed step's overlapped fetch (DESIGN §6e measures the choice); a value outside [1, SMs / 2] keeps it
+  if (const char* e = getenv("SB_FETCH_CTAS")) {
+    const int k = atoi(e);
+    if (k >= 1 && k <= t->net.num_sms / 2) t->fetch_ctas = k;
+  }
   t->w_trains.assign(static_cast<size_t>(n.L + 1), 1);
   t->b_trains.assign(static_cast<size_t>(n.L + 1), 1);
   set_exchange_slots(t.get());
@@ -1425,6 +1497,20 @@ static int apply_accumulated_impl(sb_trainer_t* t, int64_t total_pushes) {
   return SB_OK;
 }
 
+// Where sb_trainer_load_dataset puts the set's rows (X in GEMM-operand form; y, w and the prefix counts always go to HBM):
+// in HBM if they fit beside what the trainer still allocates after the load, else in mapped pinned host memory.  The
+// reserve counts, besides the set's 12 bytes per row of y, w and P: a row order of every row (4 bytes per row), the
+// conversion windows, ordY / ordW, and once more what the net allocated for its step buffers - the margin for what is
+// sized like them later (the deterministic workspaces, graph instantiation, the validation forward's chunks).
+static int place_dataset(sb_trainer* t, int64_t n_rows, size_t x_bytes, size_t win_bytes, bool* host) {
+  const Net& n = t->net;
+  size_t free_b = 0, total_b = 0;
+  SB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  const size_t reserve = 16 * static_cast<size_t>(n_rows) + win_bytes + 8 * static_cast<size_t>(n.max_batch) + n.dalloc_bytes;
+  *host = t->force_host || x_bytes + reserve > free_b;
+  return SB_OK;
+}
+
 int sb_trainer_load_dataset(sb_trainer_t* t, const float* X, const float* y, const float* w, int64_t n_rows) {
   SB_CHECK(t && X && y, SB_ERR_INVALID, "null argument");
   SB_CHECK(n_rows > 0 && n_rows < (1ll << 31), SB_ERR_INVALID, "n_rows must be in (0, 2^31)");
@@ -1433,6 +1519,29 @@ int sb_trainer_load_dataset(sb_trainer_t* t, const float* X, const float* y, con
   SB_CUDA(cudaStreamSynchronize(n.stream));
   t->drop_step_graphs();   // captured steps carry tensor maps of the old set
   t->free_dataset();
+  // X is converted through a bounded fp32 window (and, for a set in host memory, a bf16 window) so that a 100+ GB set
+  // never needs a second full copy
+  const int64_t win = 32768, wrows = win < n_rows ? win : n_rows;
+  const size_t part_elems = static_cast<size_t>(n_rows) * n.ldF;
+  const size_t x_bytes = n.tc() ? sizeof(__nv_bfloat16) * part_elems * n.nparts : sizeof(float) * static_cast<size_t>(n_rows) * n.F;
+  const size_t win_bytes = n.tc() ? static_cast<size_t>(wrows) * (sizeof(float) * n.F + sizeof(__nv_bfloat16) * n.ldF * n.nparts) : 0;
+  bool host = false;
+  SB_TRY(place_dataset(t, n_rows, x_bytes, win_bytes, &host));
+  void* xs = nullptr;
+  if (host) {
+    // mapped + portable: with unified addressing the host address is also the address kernels read it at
+    const cudaError_t e = cudaHostAlloc(&xs, x_bytes, cudaHostAllocMapped | cudaHostAllocPortable);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      return set_error(SB_ERR_CUDA, "the resident set does not fit in device memory and %zu bytes of pinned host memory for its "
+                       "%lld rows could not be allocated: %s", x_bytes, (long long)n_rows, cudaGetErrorString(e));
+    }
+  } else {
+    SB_CUDA(cudaMalloc(&xs, x_bytes));
+  }
+  t->ds_host = host;
+  if (n.tc()) t->dsXb = static_cast<__nv_bfloat16*>(xs);
+  else t->dsX = static_cast<float*>(xs);
   SB_CUDA(cudaMalloc(&t->dsY, sizeof(float) * n_rows));
   SB_CUDA(cudaMalloc(&t->dsW, sizeof(float) * n_rows));
   SB_CUDA(cudaMemcpyAsync(t->dsY, y, sizeof(float) * n_rows, cudaMemcpyDefault, n.stream));
@@ -1443,23 +1552,30 @@ int sb_trainer_load_dataset(sb_trainer_t* t, const float* X, const float* y, con
     SB_CUDA(cudaGetLastError());
   }
   if (n.tc()) {
-    // keep the set in HBM in the form the layer-0 GEMMs consume (bf16, row pitch ldF; split modes: nparts such arrays):
-    // converted once here, read by TMA every step.  Converted through a bounded fp32 window so a 100+ GB set never needs
-    // a second full copy.
-    const size_t part_elems = static_cast<size_t>(n_rows) * n.ldF;
-    SB_CUDA(cudaMalloc(&t->dsXb, sizeof(__nv_bfloat16) * part_elems * n.nparts));
-    SB_CUDA(cudaMemsetAsync(t->dsXb, 0, sizeof(__nv_bfloat16) * part_elems * n.nparts, n.stream));
+    // keep the set in the form the layer-0 GEMMs consume (bf16, row pitch ldF; split modes: nparts such arrays),
+    // converted once here.  In HBM it is read by TMA every step; in host memory gather_batch_kernel copies each batch's
+    // rows into Xb.  A host set is converted in a device window and copied out part by part, so it holds the same bits.
     n.resident_ps = static_cast<long long>(part_elems);
-    const int64_t win = 32768;
     DevBuf<float> tmp;
-    SB_TRY(tmp.alloc(static_cast<size_t>(win < n_rows ? win : n_rows) * n.F));
+    DevBuf<__nv_bfloat16> wb;
+    SB_TRY(tmp.alloc(static_cast<size_t>(wrows) * n.F));
+    const long long wps = host ? wrows * n.ldF : n.resident_ps;   // part stride of the cast's destination
+    if (host) {
+      SB_TRY(wb.alloc(static_cast<size_t>(wps) * n.nparts));
+      SB_CUDA(cudaMemsetAsync(wb.p, 0, sizeof(__nv_bfloat16) * wps * n.nparts, n.stream));   // pad columns (never written)
+    } else {
+      SB_CUDA(cudaMemsetAsync(t->dsXb, 0, x_bytes, n.stream));
+    }
     for (int64_t r0 = 0; r0 < n_rows; r0 += win) {
       const int64_t c = n_rows - r0 < win ? n_rows - r0 : win;
       SB_CUDA(cudaMemcpyAsync(tmp.p, X + r0 * n.F, sizeof(float) * c * n.F, cudaMemcpyDefault, n.stream));
+      __nv_bfloat16* dst = host ? wb.p : t->dsXb + r0 * n.ldF;
       cast_bf16_kernel<<<static_cast<unsigned>((c * n.F + 255) / 256), 256, 0, n.stream>>>(tmp.p, static_cast<int>(c), n.F,
-                                                                                           t->dsXb + r0 * n.ldF, n.ldF, n.nparts,
-                                                                                           n.resident_ps);
+                                                                                           dst, n.ldF, n.nparts, wps);
       SB_CUDA(cudaGetLastError());
+      for (int k = 0; host && k < n.nparts; ++k)
+        SB_CUDA(cudaMemcpyAsync(t->dsXb + k * n.resident_ps + r0 * n.ldF, wb.p + k * wps, sizeof(__nv_bfloat16) * c * n.ldF,
+                                cudaMemcpyDefault, n.stream));
       SB_CUDA(cudaStreamSynchronize(n.stream));   // X may be pageable: the window is reused
     }
     std::vector<int> prefix(static_cast<size_t>(n_rows) + 1);
@@ -1475,16 +1591,39 @@ int sb_trainer_load_dataset(sb_trainer_t* t, const float* X, const float* y, con
     SB_CUDA(cudaMalloc(&t->dsP, sizeof(int) * (n_rows + 1)));
     SB_CUDA(cudaMemcpyAsync(t->dsP, prefix.data(), sizeof(int) * (n_rows + 1), cudaMemcpyHostToDevice, n.stream));
     SB_CUDA(cudaStreamSynchronize(n.stream));
-    n.resident_Xb = t->dsXb;
-    n.resident_rows = n_rows;
+    if (host) {
+      if (!t->ordY) SB_TRY(n.dalloc(&t->ordY, n.max_batch));
+      if (!t->ordW) SB_TRY(n.dalloc(&t->ordW, n.max_batch));
+      // (4 bytes per row, inside the reserve's row order)
+      for (int64_t i = 0; i < n_rows; ++i) prefix[i] = static_cast<int>(i);
+      SB_CUDA(cudaMalloc(&t->ds_iota, sizeof(int) * n_rows));
+      SB_CUDA(cudaMemcpy(t->ds_iota, prefix.data(), sizeof(int) * n_rows, cudaMemcpyHostToDevice));
+      // the streamed steps' second batch buffer (kept once made, like ordY / ordW) and the fetch branch
+      if (!t->Xb2) SB_TRY(n.dalloc(&t->Xb2, static_cast<size_t>(n.Xb_ps) * n.nparts));
+      if (!t->ordY2) SB_TRY(n.dalloc(&t->ordY2, n.max_batch));
+      if (!t->ordW2) SB_TRY(n.dalloc(&t->ordW2, n.max_batch));
+      if (!t->fetch_stream) SB_CUDA(cudaStreamCreateWithFlags(&t->fetch_stream, cudaStreamNonBlocking));
+      SB_TRY(create_event(&t->ev_fork));
+      SB_TRY(create_event(&t->ev_fetched));
+    }
+    n.resident_Xb = host ? nullptr : t->dsXb;
+    n.resident_rows = host ? 0 : n_rows;
   } else {
-    SB_CUDA(cudaMalloc(&t->dsX, sizeof(float) * n_rows * n.F));
     SB_CUDA(cudaMemcpyAsync(t->dsX, X, sizeof(float) * n_rows * n.F, cudaMemcpyDefault, n.stream));
   }
   SB_CUDA(cudaStreamSynchronize(n.stream));
   t->ds_rows = n_rows;
   return SB_OK;
 }
+
+int sb_debug_force_host_set(sb_trainer_t* t, int32_t on) {
+  SB_CHECK(t, SB_ERR_INVALID, "null trainer");
+  SB_CHECK(on == 0 || on == 1, SB_ERR_INVALID, "on = %d: 0 or 1", on);
+  t->force_host = on != 0;
+  return SB_OK;
+}
+
+int sb_trainer_dataset_on_host(const sb_trainer_t* t) { return t && t->ds_rows > 0 && t->ds_host ? 1 : 0; }
 
 static int resident_step(sb_trainer_t* t, int64_t row_offset, int32_t rows, int kind) {
   SB_CHECK(t, SB_ERR_INVALID, "null trainer");
@@ -1515,6 +1654,7 @@ int sb_trainer_run_resident(sb_trainer_t* t, const int64_t* row_offsets, int32_t
       SB_TRY(prefetch_begin(t, set));
       for (int k = 0; k < S; ++k) {
         SB_TRY(resident_batch(t, row_offsets[i + k], rows, i + k, &b));
+        if (feed == Feed::STREAMED && (k & 1)) { b.y = t->ordY2; b.w = t->ordW2; }   // step k reads buffer k & 1
         const float lr_t = begin_update(t);
         SB_TRY(write_desc(t->prep, t->slot(set, k), &b, lr_t, gscale, t->epoch, t->hist_slot(t->global_step)));
       }
@@ -2075,8 +2215,8 @@ static int input_buffer(sb_trainer* t, int which, void* host, int64_t count, boo
         rs.push_back({n.Xf, static_cast<long long>(n.max_batch) * n.F});
       }
       break;
-    case SB_DEBUG_BUF_BATCH_Y: rs.push_back({t->ord_n > 0 ? t->ordY : n.stY, n.max_batch}); break;
-    case SB_DEBUG_BUF_BATCH_W: rs.push_back({t->ord_n > 0 ? t->ordW : n.stW, n.max_batch}); break;
+    case SB_DEBUG_BUF_BATCH_Y: rs.push_back({t->gathers() ? t->ordY : n.stY, n.max_batch}); break;
+    case SB_DEBUG_BUF_BATCH_W: rs.push_back({t->gathers() ? t->ordW : n.stW, n.max_batch}); break;
     case SB_DEBUG_BUF_SCAL: rs.push_back({t->slot(0, 0).scal, SCAL_COUNT}); break;
     case SB_DEBUG_BUF_DS_X:
       if (bf) {
@@ -2101,8 +2241,9 @@ static int input_buffer(sb_trainer* t, int which, void* host, int64_t count, boo
   char* h = static_cast<char*>(host);
   for (const Range& r : rs) {
     const size_t bytes = esz * static_cast<size_t>(r.elems);
+    // (cudaMemcpyDefault: the resident set may be in host memory)
     if (write) SB_CUDA(cudaMemcpyAsync(r.dev, h, bytes, cudaMemcpyHostToDevice, n.stream));
-    else SB_CUDA(cudaMemcpyAsync(h, r.dev, bytes, cudaMemcpyDeviceToHost, n.stream));
+    else SB_CUDA(cudaMemcpyAsync(h, r.dev, bytes, cudaMemcpyDefault, n.stream));
     h += bytes;
   }
   SB_CUDA(cudaStreamSynchronize(n.stream));

@@ -24,7 +24,9 @@ struct Layer {
 //   SPARSE    wide+deep: dense block + index matrix, hidden layer 0's one-hot block via the embedding
 //   RESIDENT  layer 0's GEMMs read their A operand by TMA from resident_Xb at row offset desc->row0
 //   ORDERED   resident rows through the row order: gather_batch_kernel fills Xb / Xf, layer 0 reads them
-enum class Feed { HOST, SPARSE, RESIDENT, ORDERED };
+//   STREAMED  rows of a bf16 set in mapped host memory: gather_batch_kernel fetches them over PCIe into one of two batch
+//             buffers, in a run_resident graph one step ahead, beside the previous step's GEMMs (capi.cu, DESIGN §6e)
+enum class Feed { HOST, SPARSE, RESIDENT, ORDERED, STREAMED };
 
 // What one step's launches read: its descriptor / scalar slot and its feed.  The trainer takes the slots of its captured
 // steps from a ring of descriptor sets (capi.cu).
@@ -113,10 +115,12 @@ struct Net {
   }
 
   std::vector<void*> allocs;
+  size_t dalloc_bytes = 0;   // what dalloc allocated so far
   template <typename T> int dalloc(T** p, size_t n) {
     void* q = nullptr;
     SB_CUDA(cudaMalloc(&q, n * sizeof(T) + 256));
     allocs.push_back(q);
+    dalloc_bytes += n * sizeof(T) + 256;
     SB_CUDA(cudaMemsetAsync(q, 0, n * sizeof(T) + 256, stream));
     *p = reinterpret_cast<T*>(q);
     return SB_OK;

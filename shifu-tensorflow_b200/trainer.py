@@ -198,10 +198,14 @@ def model(feature_count: int, model_conf: Optional[dict], max_batch: int) -> cap
         learning_rate = 0.003
     opt = _OPT[str(params.get('Optimizer', 'adadelta')).lower()]
     loss = _LOSS[str(params.get('Loss', 'squared')).lower()]
-    prec = {'fp32': capi.PREC_FP32, 'fp32_tc': capi.PREC_FP32_TC, 'bf16x2': capi.PREC_BF16X2}.get(
-        str(params.get('Precision', 'bf16')).lower(), capi.PREC_BF16)
     return capi.make_desc(feature_count, hidden, acts, loss=loss, optimizer=opt, learning_rate=learning_rate,
-                          max_batch=max_batch, precision=prec)
+                          max_batch=max_batch, precision=precision_requested(params))
+
+
+def precision_requested(params: dict) -> int:
+    """ModelConfig `Precision` -> capi.PREC_* (bf16 unless fp32, fp32_tc or bf16x2 is named)"""
+    return {'fp32': capi.PREC_FP32, 'fp32_tc': capi.PREC_FP32_TC, 'bf16x2': capi.PREC_BF16X2}.get(
+        str(params.get('Precision', 'bf16')).lower(), capi.PREC_BF16)
 
 
 class _Fs:
@@ -303,13 +307,82 @@ def load_data(data_file: str, feature_column_nums: Optional[List[int]], target_c
     return out
 
 
+_PARTS = {capi.PREC_FP32: 0, capi.PREC_BF16: 1, capi.PREC_FP32_TC: 3, capi.PREC_BF16X2: 2}
+HOST_PARSE_CHUNK = 1 << 30      # bytes of text per sb_text_parse call when the set is parsed to host memory
+
+
+def gpu_load_footprint(text_bytes: int, n_lines: int, n_feat: int, precision: int, shards: int = 1) -> int:
+    """Device bytes that parsing on the GPU and then loading the set into HBM hold at once: the text, the parsed fp32 set
+    with y and w, and beside it the trainer's copy of the set (tensor-core modes: the bf16 parts at a row pitch of
+    round_up(n_feat, 8); fp32 mode: the fp32 rows).  With `shards` local ranks (SB_ROW_SHARD) every rank parses the
+    whole text but keeps only its share of the rows."""
+    parsed = n_lines * (n_feat + 2) * 4
+    ld = (n_feat + 7) // 8 * 8
+    rows = n_lines // shards
+    copy = rows * ld * 2 * _PARTS[precision] if precision != capi.PREC_FP32 else rows * n_feat * 4
+    return text_bytes + parsed + copy
+
+
+def parse_on_host_side(footprint: int, free_bytes: int) -> bool:
+    """parse to host memory (and let load_dataset keep the set there) when the GPU load would not fit in free HBM"""
+    return footprint > free_bytes
+
+
+def _parse_to_host(text: bytes, col_map: Sequence[int], n_feat: int, n_lines: int, device: int, chunk: int):
+    """sb_text_parse over line-aligned pieces of at most `chunk` bytes (it stages its whole input and output on the
+    device) into host arrays X [n_lines, n_feat], y, w; cells the fast path declines are resolved with float() as in
+    load_data_gpu"""
+    X = np.empty((n_lines, n_feat), np.float32)
+    y = np.empty(n_lines, np.float32)
+    w = np.empty(n_lines, np.float32)
+    pos = row0 = 0
+    while pos < len(text):
+        end = len(text) if len(text) - pos <= chunk else text.rfind(b"\n", pos, pos + chunk) + 1
+        if end <= pos:                               # one line longer than a piece: take it whole
+            end = text.index(b"\n", pos) + 1
+        Xc, yc, wc, flags, piece = capi.text_parse(text[pos:end], col_map, n_feat, DELIMITER, device=device)
+        bad = [row for row, slot, _, _ in flags if slot == -100]
+        if bad:
+            raise ValueError("line %d does not have the selected columns" % (row0 + min(bad)))
+        for row, slot, off, ln in flags:
+            v = float(piece[off:off + ln].decode('utf-8').strip('\n'))
+            if slot >= 0:
+                Xc[row, slot] = v
+            elif slot == capi.COL_TARGET:
+                yc[row] = v
+            else:
+                wc[row] = 1.0 if v < 0.0 else v
+        n = len(yc)
+        X[row0:row0 + n], y[row0:row0 + n], w[row0:row0 + n] = Xc, yc, wc
+        row0 += n
+        pos = end
+    return X[:row0], y[:row0], w[:row0]
+
+
+def _split_in_place(X, y, w, coins):
+    """(train rows, valid rows) of X / y / w by the per-line coins; the train rows are moved to the front of the parsed
+    arrays in place, so the host holds the set once"""
+    va = np.flatnonzero(~coins)
+    valid = (X[va], y[va], w[va])
+    tr = np.flatnonzero(coins)
+    step = 65536
+    for i in range(0, len(tr), step):           # destination index <= source index: front to back never overwrites a source
+        r = tr[i:i + step]
+        X[i:i + len(r)], y[i:i + len(r)], w[i:i + len(r)] = X[r], y[r], w[r]
+    n = len(tr)
+    return (X[:n], y[:n], w[:n]), valid
+
+
 def load_data_gpu(data_file: str, feature_column_nums: Optional[List[int]], target_column_num: int,
-                  sample_weight_column_num: int, valid_ratio: float, rng=random, device: int = 0) -> Dict[str, object]:
+                  sample_weight_column_num: int, valid_ratio: float, rng=random, device: int = 0,
+                  precision: int = capi.PREC_BF16, shards: int = 1) -> Dict[str, object]:
     """load_data with the per-cell float() loop moved to the GPU (sb_text_parse): the host only gunzips and draws the
     train/valid coin per line (same `rng.random() >= ratio -> train` stream, ssgd_monitor.py:396); cells the exact
     fast path declines come back as a list and are resolved with float() here, exactly like the reference would.
     Returns capi.DeviceArray objects under the same keys as load_data: the parsed set never visits the host (the trainer's
-    load_dataset / eval_loss take device pointers)."""
+    load_dataset / eval_loss take device pointers).
+    A set whose GPU load (gpu_load_footprint) exceeds the free device memory is parsed into host arrays instead, in
+    line-aligned pieces, and returned as numpy arrays: load_dataset then keeps it in pinned host memory."""
     chunks = []
     for current_file in data_file.split(","):
         data = gzip.GzipFile(fileobj=io.BytesIO(_Fs.read_bytes(current_file))).read()
@@ -329,6 +402,20 @@ def load_data_gpu(data_file: str, feature_column_nums: Optional[List[int]], targ
     if sample_weight_column_num >= 0:
         col_map[sample_weight_column_num] = capi.COL_WEIGHT
     n_feat = len(feature_column_nums)
+    n_lines = text.count(b"\n")
+    need = gpu_load_footprint(len(text), n_lines, n_feat, precision, shards)
+    free = capi.device_mem_info(device)[0]
+    if parse_on_host_side(need, free):
+        logging.info("training set: %d lines need about %.1f GB of device memory to load, %.1f GB are free: parsing to host "
+                     "memory, the trainer keeps the set in pinned host memory and reads each batch over PCIe"
+                     % (n_lines, need / 1e9, free / 1e9))
+        X, y, w = _parse_to_host(text, col_map, n_feat, n_lines, device, HOST_PARSE_CHUNK)
+        coins = np.fromiter((rng.random() >= valid_ratio for _ in range(len(y))), dtype=bool, count=len(y))
+        (tx, ty, tw), (vx, vy, vw) = _split_in_place(X, y, w, coins)
+        return {"feature_count": n_feat, "train_data": tx, "train_target": ty, "train_data_sample_weight": tw,
+                "valid_data": vx, "valid_target": vy, "valid_data_sample_weight": vw}
+    logging.info("training set: %d lines, about %.1f GB of device memory to load (%.1f GB free): the set is kept in HBM"
+                 % (n_lines, need / 1e9, free / 1e9))
     X, y, w, flags, text, _kernel_ms = capi.text_parse_device(text, col_map, n_feat, DELIMITER, device=device)
     # a line without the selected columns is reported by number before any of its cells is resolved (an empty line also
     # flags its empty target cell, and the flags arrive in no fixed order)
@@ -657,7 +744,8 @@ def main(_=None, env=None, rng=random) -> int:
                             valid_ratio, rng=rng)
     else:
         context = load_data_gpu(training_data_path, feature_column_nums, target_column_num, sample_weight_column_num,
-                                valid_ratio, rng=rng, device=device)
+                                valid_ratio, rng=rng, device=device, precision=precision_requested(params),
+                                shards=int(env["SB_ROW_SHARD"].split("/")[1]) if env.get("SB_ROW_SHARD") else 1)
     on_device = isinstance(context["train_data"], capi.DeviceArray)
     if on_device:
         train_x, train_y, train_w = context["train_data"], context["train_target"], context["train_data_sample_weight"]
@@ -717,6 +805,7 @@ def main(_=None, env=None, rng=random) -> int:
     logging.info("Training set size: %d" % len(train_x))
 
     # split data into batch (ssgd_monitor.py:189-192): int(N / BATCH_SIZE) near-equal batches
+    n_train = len(train_x)
     total_batch = max(1, int(len(train_x) / batch_size))
     bounds = [b[0] for b in np.array_split(np.arange(len(train_x)), total_batch)] + [len(train_x)]
     max_rows = max(bounds[i + 1] - bounds[i] for i in range(total_batch))
@@ -768,7 +857,11 @@ def main(_=None, env=None, rng=random) -> int:
             logging.info("wide+deep trains with one update per mini-batch (Schedule=batch); the sync-replicas accumulator is not wired for sparse steps")
             per_batch_update = True
     else:
-        trainer.load_dataset(train_x, train_y, train_w)
+        trainer.load_dataset(train_x, train_y, train_w)     # (logs where the library placed the set)
+        if not on_device:
+            # the trainer holds its own copy of the set (in HBM or pinned host memory): drop the parsed host arrays, which
+            # for a set larger than HBM are as large as that copy
+            context = train_x = train_y = train_w = None
 
     # replicas_to_aggregate (ssgd_monitor.py:139): accepted pushes per global update, over all workers
     R = max(1, int(total_training_data_number * (1 - valid_ratio) / batch_size * REPLICAS_TO_AGGREGATE_RATIO))
@@ -788,7 +881,7 @@ def main(_=None, env=None, rng=random) -> int:
         start = time.time()
         l = 0.0
         if shuffle:
-            perm = pass_order(shuffle_seed, task_index, trainer.global_step, len(train_x))
+            perm = pass_order(shuffle_seed, task_index, trainer.global_step, n_train)
             if wide_deep:
                 sparse_rows = (train_x[perm], train_idx[perm], train_y[perm], train_w[perm])
             else:
