@@ -68,16 +68,19 @@ struct sb_trainer {
   // in HBM.
   float *dsX = nullptr, *dsY = nullptr, *dsW = nullptr;   // dsX only in fp32 mode
   __nv_bfloat16* dsXb = nullptr;                           // bf16 mode: the set in GEMM-operand form [ds_rows, ldF]
+  long long ds_ps = 0;                                     // part stride of dsXb (elements)
   int* dsP = nullptr;                                      // prefix counts of non-zero weights [ds_rows + 1]
   long long ds_rows = 0;
   bool ds_host = false, force_host = false;
   int* ds_iota = nullptr;   // bf16 set in host memory: the identity order its steps gather through without a row order
-  // Streamed steps (a bf16 set in host memory): step k of a graph computes from batch buffer k & 1 - Xb / ordY / ordW
-  // (k even) or Xb2 / ordY2 / ordW2 (k odd).  Inside a run_resident graph the rows of step k + 1 are fetched on
-  // fetch_stream into the other buffer while step k runs, on fetch_ctas CTAs, with step k's GEMM grids planned for the
-  // remaining SMs.
-  __nv_bfloat16* Xb2 = nullptr;
-  float *ordY2 = nullptr, *ordW2 = nullptr;
+  // Batch buffers: where gather_batch_kernel puts a step's rows (Xb; fp32 mode: the net's Xf), labels and weights.  Entry
+  // 0's Xb is the net's own.  Entry 1 exists for a bf16 set in host memory only: inside a run_resident graph its streamed
+  // steps fetch the rows of step k + 1 on fetch_stream into the other buffer while step k runs, on fetch_ctas CTAs, with
+  // step k's GEMM grids planned for the remaining SMs.  Step k of a captured graph (k = 0 outside graphs) reads buffer
+  // k & 1 if its feed is STREAMED and buffer 0 otherwise; a RESIDENT step reads the set itself at desc->row0 (slot).
+  struct BatchBuf { __nv_bfloat16* Xb = nullptr; float *y = nullptr, *w = nullptr; };
+  BatchBuf bufs[2];
+  const BatchBuf& batch_buf(Feed feed, int k) const { return bufs[feed == Feed::STREAMED ? (k & 1) : 0]; }
   cudaStream_t fetch_stream = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_fetched = nullptr;
   int fetch_ctas = 16;
@@ -85,7 +88,6 @@ struct sb_trainer {
   // ord[r] (int32 on the device, the only per-row memory an order costs); ord_n == 0: physical order
   int* ord = nullptr;
   long long ord_n = 0, ord_cap = 0;
-  float *ordY = nullptr, *ordW = nullptr;   // [max_batch] labels / weights of an ordered step's batch (gather_batch_kernel)
   std::map<GraphKey, cudaGraphExec_t> graphs;
   std::map<std::pair<int, Feed>, int> kernels_per_step;   // (rows, feed) of a captured single G_STEP step
   // peer-memory exchange (xchg_p2p.cuh): the net's parameter arena [theta | s1 | s2 | shadows | gradient | P2PFlags] is
@@ -147,7 +149,20 @@ struct sb_trainer {
   bool started = false;    // a step ran or was captured: sb_trainer_set_deterministic is refused from here on
   bool have_pos = false;   // ev_pos[] of the previous prefetched launch is valid (no step on set 0 since)
   int last_set = 0;        // the set of the last prefetched launch
-  StepIn slot(int set, int k, Feed feed = Feed::HOST) const { return StepIn{ring_desc[set][k], ring_scal[set][k], feed}; }
+  StepIn slot(int set, int k, Feed feed = Feed::HOST) const {
+    const Operand0 x0 = feed == Feed::RESIDENT ? Operand0{dsXb, ds_ps, static_cast<int>(ds_rows), true}
+                                               : Operand0{batch_buf(feed, k).Xb, net.Xb_ps};
+    return StepIn{ring_desc[set][k], ring_scal[set][k], feed, x0};
+  }
+  // y / w of batch buffer 0 and, for a bf16 set in host memory (`streamed`), all of buffer 1; kept once made
+  int alloc_batch_bufs(bool streamed) {
+    for (int i = 0; i < (streamed ? 2 : 1); ++i) {
+      if (i == 1 && !bufs[1].Xb) SB_TRY(net.dalloc(&bufs[1].Xb, static_cast<size_t>(net.Xb_ps) * net.nparts));
+      if (!bufs[i].y) SB_TRY(net.dalloc(&bufs[i].y, net.max_batch));
+      if (!bufs[i].w) SB_TRY(net.dalloc(&bufs[i].w, net.max_batch));
+    }
+    return SB_OK;
+  }
 
   // Releases what the trainer created.  Pointers into the net's allocations (ring_desc, ring_scal, grad, flags, xch, s1,
   // s2, acc, st2*) are freed by `net`, the first member and so the last destroyed.
@@ -250,9 +265,9 @@ static Batch host_batch(const Net& n, const float* X, const float* y, const floa
   return b;
 }
 
-// rows [off, off + rows) of the resident set, through the row order if one is set.  step >= 0 names the step of a run
-// in the error message.
-static int resident_batch(const sb_trainer* t, long long off, int rows, int step, Batch* b) {
+// rows [off, off + rows) of the resident set, through the row order if one is set, for step k of a graph.  step >= 0
+// names the step of a run in the error message.
+static int resident_batch(const sb_trainer* t, long long off, int rows, int step, int k, Batch* b) {
   SB_CHECK(t->ds_rows > 0, SB_ERR_STATE, "no resident dataset loaded");
   const long long len = t->resident_len();
   if (off < 0 || rows <= 0 || off + rows > len) {
@@ -265,9 +280,8 @@ static int resident_batch(const sb_trainer* t, long long off, int rows, int step
   *b = Batch{};
   b->feed = t->resident_feed();
   b->rows = rows;
-  if (b->feed == Feed::ORDERED || b->feed == Feed::STREAMED) {   // gather_batch_kernel counts n_nz and fills ordY / ordW
-    // (a streamed step of a run_resident graph reads buffer k & 1: stream_buffer)
-    b->y = t->ordY; b->w = t->ordW;
+  if (b->feed == Feed::ORDERED || b->feed == Feed::STREAMED) {   // gather_batch_kernel counts n_nz and fills y / w
+    b->y = t->batch_buf(b->feed, k).y; b->w = t->batch_buf(b->feed, k).w;
     b->order = (t->ord_n > 0 ? t->ord : t->ds_iota) + off;
     return SB_OK;
   }
@@ -635,18 +649,17 @@ static int enqueue_step_backward(sb_trainer* t, const StepIn& in, int rows, int 
 }
 
 // first kernel of an ordered step, in load_batch_kernel's place: the batch's rows of the resident set through the order
-// slice in.desc->order into Xb / Xf, ordY / ordW and the step scalars; clears clear[0, clear_n) on the way
-// buf: batch buffer 0 (Xb / ordY / ordW) or 1 (a streamed step's second buffer); on stream st (null: the main stream,
-// PDL-chained, at most 16 blocks per SM), else on st with at most `ctas` blocks
-static int enqueue_gather(sb_trainer* t, const StepIn& in, int rows, float* clear, long long clear_n, int buf = 0,
-                          cudaStream_t st = nullptr, int ctas = 0) {
+// slice in.desc->order into batch buffer bb (fp32 mode: X into Xf) and the step scalars; clears clear[0, clear_n) on the
+// way.  On stream st (null: the main stream, PDL-chained, at most 16 blocks per SM), else on st with at most `ctas` blocks
+static int enqueue_gather(sb_trainer* t, const StepIn& in, const sb_trainer::BatchBuf& bb, int rows, float* clear,
+                          long long clear_n, cudaStream_t st = nullptr, int ctas = 0) {
   Net& n = t->net;
   GatherParams p = {};
   p.desc = in.desc;
   p.rows = rows; p.F = n.F; p.ldF = n.ldF; p.np = n.nparts;
-  p.src_b = t->dsXb; p.src_ps = n.resident_ps; p.Xb = buf ? t->Xb2 : n.Xb; p.Xb_ps = n.Xb_ps;
+  p.src_b = t->dsXb; p.src_ps = t->ds_ps; p.Xb = bb.Xb; p.Xb_ps = n.Xb_ps;
   p.src_f = t->dsX; p.Xf = n.Xf;
-  p.src_y = t->dsY; p.src_w = t->dsW; p.y = buf ? t->ordY2 : t->ordY; p.w = buf ? t->ordW2 : t->ordW;
+  p.src_y = t->dsY; p.src_w = t->dsW; p.y = bb.y; p.w = bb.w;
   p.scal = in.scal;
   p.zero_buf = clear; p.zero_n = clear_n;
   p.trace = n.next_trace(st ? "fetch_batch" : "gather_batch");
@@ -662,12 +675,12 @@ static int enqueue_gather(sb_trainer* t, const StepIn& in, int rows, float* clea
   return SB_OK;
 }
 
-// The first kernel of a step or forward, by feed: HOST / SPARSE load_batch_kernel, ORDERED gather_batch_kernel (t: its
-// trainer), RESIDENT none (layer 0 reads the set by TMA; set_batch_kernel already published n_nz).  Clears
-// clear[0, clear_n) on the way.
+// The first kernel of a step or forward, by feed: HOST / SPARSE load_batch_kernel, ORDERED (and a streamed forward)
+// gather_batch_kernel into batch buffer 0 (t: its trainer), RESIDENT none (layer 0 reads the set by TMA; set_batch_kernel
+// already published n_nz).  Clears clear[0, clear_n) on the way.
 static int enqueue_first(Net& n, sb_trainer* t, const StepIn& in, int rows, float* clear, long long clear_n) {
   if (in.feed == Feed::RESIDENT) return SB_OK;
-  if (in.feed == Feed::ORDERED || in.feed == Feed::STREAMED) return enqueue_gather(t, in, rows, clear, clear_n);
+  if (in.feed == Feed::ORDERED || in.feed == Feed::STREAMED) return enqueue_gather(t, in, t->bufs[0], rows, clear, clear_n);
   return n.enqueue_load(in, rows, clear, clear_n);
 }
 
@@ -677,11 +690,12 @@ static int enqueue_first(Net& n, sb_trainer* t, const StepIn& in, int rows, floa
 // accumulates into it.
 static int enqueue_streamed_fetch(sb_trainer* t, int set, int k, int steps, int rows) {
   Net& n = t->net;
-  if (k == 0) SB_TRY(enqueue_gather(t, t->slot(set, 0, Feed::STREAMED), rows, nullptr, 0));
+  if (k == 0) SB_TRY(enqueue_gather(t, t->slot(set, 0, Feed::STREAMED), t->batch_buf(Feed::STREAMED, 0), rows, nullptr, 0));
   else SB_CUDA(cudaStreamWaitEvent(n.stream, t->ev_fetched, 0));
   if (k + 1 < steps) {
     SB_TRY(join_streams(t->fetch_stream, n.stream, t->ev_fork));
-    SB_TRY(enqueue_gather(t, t->slot(set, k + 1, Feed::STREAMED), rows, nullptr, 0, (k + 1) & 1, t->fetch_stream, t->fetch_ctas));
+    SB_TRY(enqueue_gather(t, t->slot(set, k + 1, Feed::STREAMED), t->batch_buf(Feed::STREAMED, k + 1), rows, nullptr, 0,
+                          t->fetch_stream, t->fetch_ctas));
     SB_CUDA(cudaEventRecord(t->ev_fetched, t->fetch_stream));
   }
   return SB_OK;
@@ -724,18 +738,13 @@ static int get_graph(sb_trainer* t, const GraphKey& key, cudaGraphExec_t* out) {
   const int sms = n.num_sms;
   const bool overlap = key.feed == Feed::STREAMED && key.steps > 1;
   if (overlap) n.num_sms = sms - t->fetch_ctas;
-  __nv_bfloat16* const xb0 = n.Xb;
   for (int k = 0; k < key.steps && s == SB_OK; ++k) {
     // (SB_STEP_TRACE: of a run, an interior step is the one traced - it starts behind the previous step's tail, as most
     // steps of a run do)
     n.trace_on = key.steps == 1 || k == 1;
-    if (key.feed == Feed::STREAMED) {
-      s = enqueue_streamed_fetch(t, key.set, k, key.steps, key.rows);
-      n.Xb = (k & 1) ? t->Xb2 : xb0;     // the buffer layer 0's forward and dW GEMMs read
-    }
+    if (key.feed == Feed::STREAMED) s = enqueue_streamed_fetch(t, key.set, k, key.steps, key.rows);
     if (s == SB_OK) s = enqueue_step_body(t, t->slot(key.set, k, key.feed), key.rows, key.kind);
   }
-  n.Xb = xb0;
   n.num_sms = sms;
   n.trace_on = true;
   cudaError_t e = cudaStreamEndCapture(n.stream, &g);
@@ -1018,6 +1027,7 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
   }
   // from here on, a failed step returns and `t` releases whatever exists
   SB_TRY(t->net.init(desc, device, true));
+  t->bufs[0].Xb = t->net.Xb;
   // see Net::init: no L1 / shared-memory re-partition between the kernels of a step
   cudaFuncSetAttribute(set_batch_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   for (auto k : optimizer_kernels) cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
@@ -1500,7 +1510,7 @@ static int apply_accumulated_impl(sb_trainer_t* t, int64_t total_pushes) {
 // Where sb_trainer_load_dataset puts the set's rows (X in GEMM-operand form; y, w and the prefix counts always go to HBM):
 // in HBM if they fit beside what the trainer still allocates after the load, else in mapped pinned host memory.  The
 // reserve counts, besides the set's 12 bytes per row of y, w and P: a row order of every row (4 bytes per row), the
-// conversion windows, ordY / ordW, and once more what the net allocated for its step buffers - the margin for what is
+// conversion windows, batch y / w, and once more what the net allocated for its step buffers - the margin for what is
 // sized like them later (the deterministic workspaces, graph instantiation, the validation forward's chunks).
 static int place_dataset(sb_trainer* t, int64_t n_rows, size_t x_bytes, size_t win_bytes, bool* host) {
   const Net& n = t->net;
@@ -1555,11 +1565,11 @@ int sb_trainer_load_dataset(sb_trainer_t* t, const float* X, const float* y, con
     // keep the set in the form the layer-0 GEMMs consume (bf16, row pitch ldF; split modes: nparts such arrays),
     // converted once here.  In HBM it is read by TMA every step; in host memory gather_batch_kernel copies each batch's
     // rows into Xb.  A host set is converted in a device window and copied out part by part, so it holds the same bits.
-    n.resident_ps = static_cast<long long>(part_elems);
+    t->ds_ps = static_cast<long long>(part_elems);
     DevBuf<float> tmp;
     DevBuf<__nv_bfloat16> wb;
     SB_TRY(tmp.alloc(static_cast<size_t>(wrows) * n.F));
-    const long long wps = host ? wrows * n.ldF : n.resident_ps;   // part stride of the cast's destination
+    const long long wps = host ? wrows * n.ldF : t->ds_ps;   // part stride of the cast's destination
     if (host) {
       SB_TRY(wb.alloc(static_cast<size_t>(wps) * n.nparts));
       SB_CUDA(cudaMemsetAsync(wb.p, 0, sizeof(__nv_bfloat16) * wps * n.nparts, n.stream));   // pad columns (never written)
@@ -1574,7 +1584,7 @@ int sb_trainer_load_dataset(sb_trainer_t* t, const float* X, const float* y, con
                                                                                            dst, n.ldF, n.nparts, wps);
       SB_CUDA(cudaGetLastError());
       for (int k = 0; host && k < n.nparts; ++k)
-        SB_CUDA(cudaMemcpyAsync(t->dsXb + k * n.resident_ps + r0 * n.ldF, wb.p + k * wps, sizeof(__nv_bfloat16) * c * n.ldF,
+        SB_CUDA(cudaMemcpyAsync(t->dsXb + k * t->ds_ps + r0 * n.ldF, wb.p + k * wps, sizeof(__nv_bfloat16) * c * n.ldF,
                                 cudaMemcpyDefault, n.stream));
       SB_CUDA(cudaStreamSynchronize(n.stream));   // X may be pageable: the window is reused
     }
@@ -1592,22 +1602,16 @@ int sb_trainer_load_dataset(sb_trainer_t* t, const float* X, const float* y, con
     SB_CUDA(cudaMemcpyAsync(t->dsP, prefix.data(), sizeof(int) * (n_rows + 1), cudaMemcpyHostToDevice, n.stream));
     SB_CUDA(cudaStreamSynchronize(n.stream));
     if (host) {
-      if (!t->ordY) SB_TRY(n.dalloc(&t->ordY, n.max_batch));
-      if (!t->ordW) SB_TRY(n.dalloc(&t->ordW, n.max_batch));
       // (4 bytes per row, inside the reserve's row order)
       for (int64_t i = 0; i < n_rows; ++i) prefix[i] = static_cast<int>(i);
       SB_CUDA(cudaMalloc(&t->ds_iota, sizeof(int) * n_rows));
       SB_CUDA(cudaMemcpy(t->ds_iota, prefix.data(), sizeof(int) * n_rows, cudaMemcpyHostToDevice));
-      // the streamed steps' second batch buffer (kept once made, like ordY / ordW) and the fetch branch
-      if (!t->Xb2) SB_TRY(n.dalloc(&t->Xb2, static_cast<size_t>(n.Xb_ps) * n.nparts));
-      if (!t->ordY2) SB_TRY(n.dalloc(&t->ordY2, n.max_batch));
-      if (!t->ordW2) SB_TRY(n.dalloc(&t->ordW2, n.max_batch));
+      // the streamed steps' batch buffers and the fetch branch
+      SB_TRY(t->alloc_batch_bufs(true));
       if (!t->fetch_stream) SB_CUDA(cudaStreamCreateWithFlags(&t->fetch_stream, cudaStreamNonBlocking));
       SB_TRY(create_event(&t->ev_fork));
       SB_TRY(create_event(&t->ev_fetched));
     }
-    n.resident_Xb = host ? nullptr : t->dsXb;
-    n.resident_rows = host ? 0 : n_rows;
   } else {
     SB_CUDA(cudaMemcpyAsync(t->dsX, X, sizeof(float) * n_rows * n.F, cudaMemcpyDefault, n.stream));
   }
@@ -1628,7 +1632,7 @@ int sb_trainer_dataset_on_host(const sb_trainer_t* t) { return t && t->ds_rows >
 static int resident_step(sb_trainer_t* t, int64_t row_offset, int32_t rows, int kind) {
   SB_CHECK(t, SB_ERR_INVALID, "null trainer");
   Batch b;
-  SB_TRY(resident_batch(t, row_offset, rows, -1, &b));
+  SB_TRY(resident_batch(t, row_offset, rows, -1, 0, &b));
   return run_step(t, b, kind);
 }
 
@@ -1639,7 +1643,7 @@ int sb_trainer_run_resident(sb_trainer_t* t, const int64_t* row_offsets, int32_t
   Net& n = t->net;
   SB_CHECK(rows > 0 && rows <= n.max_batch, SB_ERR_INVALID, "rows=%d outside (0, max_batch=%d]", rows, n.max_batch);
   Batch b;
-  for (int i = 0; i < n_steps; ++i) SB_TRY(resident_batch(t, row_offsets[i], rows, i, &b));
+  for (int i = 0; i < n_steps; ++i) SB_TRY(resident_batch(t, row_offsets[i], rows, i, 0, &b));
   constexpr int S = sb_trainer::RUN_S;
   int i = 0;
   SB_TRY(check_det_exchange(t));
@@ -1653,8 +1657,7 @@ int sb_trainer_run_resident(sb_trainer_t* t, const int64_t* row_offsets, int32_t
       SB_TRY(get_graph(t, GraphKey{rows, G_STEP, feed, S, set}, &ge));
       SB_TRY(prefetch_begin(t, set));
       for (int k = 0; k < S; ++k) {
-        SB_TRY(resident_batch(t, row_offsets[i + k], rows, i + k, &b));
-        if (feed == Feed::STREAMED && (k & 1)) { b.y = t->ordY2; b.w = t->ordW2; }   // step k reads buffer k & 1
+        SB_TRY(resident_batch(t, row_offsets[i + k], rows, i + k, k, &b));
         const float lr_t = begin_update(t);
         SB_TRY(write_desc(t->prep, t->slot(set, k), &b, lr_t, gscale, t->epoch, t->hist_slot(t->global_step)));
       }
@@ -1681,11 +1684,11 @@ int sb_trainer_accumulate_resident(sb_trainer_t* t, int64_t row_offset, int32_t 
 int sb_trainer_loss_resident(sb_trainer_t* t, int64_t row_offset, int32_t rows, float* loss_out) {
   SB_CHECK(t && loss_out, SB_ERR_INVALID, "null argument");
   Batch b;
-  SB_TRY(resident_batch(t, row_offset, rows, -1, &b));
+  SB_TRY(resident_batch(t, row_offset, rows, -1, 0, &b));
   Net& n = t->net;
   SB_CUDA(cudaSetDevice(n.device));
   t->have_pos = false;
-  const StepIn in = t->slot(0, 0);      // (see forward_chunks)
+  const StepIn in = t->slot(0, 0, b.feed);      // (see forward_chunks)
   SB_TRY(enqueue_forward(n, t, in, b, t->epoch, true, nullptr));
   float h[SCAL_COUNT];
   SB_CUDA(cudaMemcpyAsync(h, in.scal, sizeof(h), cudaMemcpyDeviceToHost, n.stream));
@@ -1768,12 +1771,11 @@ int sb_trainer_set_row_order(sb_trainer_t* t, const int64_t* rows, int64_t n) {
   }
   Net& net = t->net;
   SB_CUDA(cudaSetDevice(net.device));
-  // steps already queued read the current order (and ordY / ordW) when they run; the graphs read the order through the
+  // steps already queued read the current order (and batch buffer 0) when they run; the graphs read the order through the
   // descriptor, so neither a new buffer nor new contents need a new capture
   SB_CUDA(cudaStreamSynchronize(net.stream));
   if (n == 0) { t->drop_row_order(); return SB_OK; }
-  if (!t->ordY) SB_TRY(net.dalloc(&t->ordY, net.max_batch));
-  if (!t->ordW) SB_TRY(net.dalloc(&t->ordW, net.max_batch));
+  SB_TRY(t->alloc_batch_bufs(false));
   if (n > t->ord_cap) {
     t->drop_row_order();
     SB_CUDA(cudaMalloc(&t->ord, sizeof(int) * n));
@@ -2215,13 +2217,13 @@ static int input_buffer(sb_trainer* t, int which, void* host, int64_t count, boo
         rs.push_back({n.Xf, static_cast<long long>(n.max_batch) * n.F});
       }
       break;
-    case SB_DEBUG_BUF_BATCH_Y: rs.push_back({t->gathers() ? t->ordY : n.stY, n.max_batch}); break;
-    case SB_DEBUG_BUF_BATCH_W: rs.push_back({t->gathers() ? t->ordW : n.stW, n.max_batch}); break;
+    case SB_DEBUG_BUF_BATCH_Y: rs.push_back({t->gathers() ? t->bufs[0].y : n.stY, n.max_batch}); break;
+    case SB_DEBUG_BUF_BATCH_W: rs.push_back({t->gathers() ? t->bufs[0].w : n.stW, n.max_batch}); break;
     case SB_DEBUG_BUF_SCAL: rs.push_back({t->slot(0, 0).scal, SCAL_COUNT}); break;
     case SB_DEBUG_BUF_DS_X:
       if (bf) {
         esz = sizeof(uint16_t);
-        for (int k = 0; k < n.nparts; ++k) rs.push_back({t->dsXb + k * n.resident_ps, ds * n.ldF});
+        for (int k = 0; k < n.nparts; ++k) rs.push_back({t->dsXb + k * t->ds_ps, ds * n.ldF});
       } else {
         rs.push_back({t->dsX, ds * n.F});
       }
@@ -2300,7 +2302,7 @@ int sb_debug_first_kernel(sb_trainer_t* t, const float* X, const float* y, const
   Net& n = t->net;
   Batch b;
   if (X == nullptr) {
-    SB_TRY(resident_batch(t, row_offset, rows, -1, &b));
+    SB_TRY(resident_batch(t, row_offset, rows, -1, 0, &b));
   } else if (n.n_cat > 0) {   // as sb_trainer_step_sparse
     SB_TRY(stage_sparse_batch(n, X, idx, y, w, rows));
     b = host_batch(n, n.stX, n.stY, w ? n.stW : nullptr, rows, Feed::SPARSE);

@@ -452,10 +452,7 @@ int Net::enqueue_hidden_forward(const StepIn& in, int rows, float* grad, bool* f
     if (tc()) {
       // Z = A_{l-1}[rows,in] (K-major) x W_l[in,out] (MN-major B operand: n contiguous)
       TmapSet tm;
-      const bool res0 = (l == 0) && in.feed == Feed::RESIDENT;
-      const __nv_bfloat16* src = (l == 0) ? (res0 ? resident_Xb : Xb) : A[l - 1];
-      const long long src_ps = (l == 0) ? (res0 ? resident_ps : Xb_ps) : A_ps[l - 1];
-      const int src_rows = res0 ? static_cast<int>(resident_rows) : rows;
+      const Operand0 a = (l == 0) ? layer0(in, rows) : Operand0{A[l - 1], A_ps[l - 1], rows};
       SB_TRY(make_tmaps_bf16(tm.b, ly.Wn, Wn_ps[l], nparts, k_in, ly.out, ly.ld_out, 64));
       GemmTcParams p = {};
       set_part_pairs(&p, nparts);
@@ -463,11 +460,11 @@ int Net::enqueue_hidden_forward(const StepIn& in, int rows, float* grad, bool* f
       if (sp0) { p.addend = E; p.ld_add = ly.ld_out; }
       p.bias = theta + ly.b_off; p.act = ly.act;
       p.out = A[l]; p.ld_out = ly.ld_out; p.out_ps = A_ps[l];
-      p.a_rows = res0 ? in.desc : nullptr;
+      p.a_rows = a.at_row0 ? in.desc : nullptr;
       if (l == L - 1 && grad != nullptr && training && ly.out <= FWD_OUT_MAX_N && p.addend == nullptr) {
         // K2 + K3 + K4 + output backward in one kernel (gemm_fwd_out.cuh): 64-row tiles of whole rows of A_L
         FwdOutTmaps ft;
-        SB_TRY(make_tmaps_bf16(ft.a, src, src_ps, nparts, src_rows, k_in, ld_k, 64));
+        SB_TRY(make_tmaps_bf16(ft.a, a.p, a.ps, nparts, a.rows, k_in, ld_k, 64));
         for (int i = 0; i < 3; ++i) ft.b[i] = tm.b[i];
         SB_TRY(make_tmaps_bf16(ft.o, dZ[l], A_ps[l], nparts, rows, ly.out, ly.ld_out, 64));
         const int tiles = (rows + 63) / 64;
@@ -488,7 +485,7 @@ int Net::enqueue_hidden_forward(const StepIn& in, int rows, float* grad, bool* f
       if (nparts == 1 && p.addend == nullptr) {    // plain bf16: the ping-pong kernel
         const PpPlan pp = plan_gemm_pp(rows, ly.out, k_in, num_sms, true);
         PpTmaps pt;
-        SB_TRY(make_tmap_bf16(&pt.a, src, src_rows, k_in, ld_k, pp.bm_wg));
+        SB_TRY(make_tmap_bf16(&pt.a, a.p, a.rows, k_in, ld_k, pp.bm_wg));
         pt.b = tm.b[0];
         SB_TRY(make_tmap_bf16(&pt.o, A[l], rows, ly.out, ly.ld_out, pp.bm_wg));
         if (pp.bn == 256) {
@@ -500,7 +497,7 @@ int Net::enqueue_hidden_forward(const StepIn& in, int rows, float* grad, bool* f
         }
       } else {
         const GemmPlan pl = plan_gemm(rows, ly.out, round_up(k_in, 64) * pairs_of(nparts), num_sms, false);
-        SB_TRY(make_tmaps_bf16(tm.a, src, src_ps, nparts, src_rows, k_in, ld_k, 128));
+        SB_TRY(make_tmaps_bf16(tm.a, a.p, a.ps, nparts, a.rows, k_in, ld_k, 128));
         SB_TRY((launch_gemm_tc<EPI_FWD, false, true>(pl, tm, p, stream, true)));
         mark(pl.bn == 64 ? "gemm_tc<64,FWD,GENERIC>" : "gemm_tc<128,FWD,GENERIC>");
       }
@@ -598,20 +595,18 @@ int Net::enqueue_dw(const StepIn& in, int l, int rows, float* grad, cudaStream_t
     return SB_OK;
   }
   // dW_l[in,out] += sum_rows A_{l-1}[rows,in] (MN-major A) * dZ_l[rows,out] (MN-major B), split-K over rows
-  const bool res0 = (l == 0) && in.feed == Feed::RESIDENT;
   const int ld_k = sp0 ? ldD : ly.ld_in;
-  const __nv_bfloat16* ap = (l == 0) ? (res0 ? resident_Xb : Xb) : A[l - 1];
-  const long long ap_ps = (l == 0) ? (res0 ? resident_ps : Xb_ps) : A_ps[l - 1];
+  const Operand0 a = (l == 0) ? layer0(in, rows) : Operand0{A[l - 1], A_ps[l - 1], rows};
   const GemmPlan pl = plan_gemm(r1 - r0, ly.out, round_up(rows, 64) * pairs_of(nparts), sms, true, dw_max_split());
   TmapSet tm;
   // resident set: rows past the batch end are real rows of other batches; the B operand (dZ_l, extent = rows) is
   // zero-filled there, so they contribute nothing
-  SB_TRY(make_tmaps_bf16(tm.a, ap + r0, ap_ps, nparts, res0 ? static_cast<int>(resident_rows) : rows, r1 - r0, ld_k, 64));
+  SB_TRY(make_tmaps_bf16(tm.a, a.p + r0, a.ps, nparts, a.rows, r1 - r0, ld_k, 64));
   SB_TRY(make_tmaps_bf16(tm.b, dZ[l], A_ps[l], nparts, rows, ly.out, ly.ld_out, 64));
   GemmTcParams p = {};
   set_part_pairs(&p, nparts);
   p.M = r1 - r0; p.N = ly.out; p.K = rows;
-  p.a_rows = res0 ? in.desc : nullptr;
+  p.a_rows = a.at_row0 ? in.desc : nullptr;
   p.accum = grad + ly.w_off + static_cast<long long>(r0) * ly.out; p.ld_acc = ly.out;
   p.acc_vec4 = (ly.out % 4 == 0 && ly.w_off % 4 == 0) ? 1 : 0;
   p.trace = next_trace("dW", l, r1 - r0, ly.out, rows, chunk);
@@ -939,14 +934,14 @@ int sb_debug_gemm_layer(int32_t kind, int32_t precision, const float* A, const f
   hd.row0 = row0;
   SB_CUDA(cudaMemcpy(net.desc, &hd, sizeof(hd), cudaMemcpyHostToDevice));
   // the batch operand of layer 0: the staged batch, or the resident set
+  StepIn in{net.desc, net.scal, resident ? Feed::RESIDENT : addend ? Feed::SPARSE : Feed::HOST};
   if (kind != DA) {
     const int cols = kind == FWD ? K : M;
     if (resident) {
-      net.resident_ps = static_cast<long long>(a_rows) * net.ldF;
-      net.resident_rows = a_rows;
-      SB_TRY(alloc_filled(&res, static_cast<size_t>(net.resident_ps) * np));
-      SB_TRY(upload_parts(res.p, A, a_rows, cols, net.ldF, np, net.resident_ps));
-      net.resident_Xb = res.p;
+      const long long ps = static_cast<long long>(a_rows) * net.ldF;
+      SB_TRY(alloc_filled(&res, static_cast<size_t>(ps) * np));
+      SB_TRY(upload_parts(res.p, A, a_rows, cols, net.ldF, np, ps));
+      in.x0 = Operand0{res.p, ps, a_rows, true};
     } else if (tc) {
       SB_TRY(upload_parts(net.Xb, A, rows, cols, addend ? net.ldD : net.ldF, np, net.Xb_ps));
     } else {
@@ -999,8 +994,6 @@ int sb_debug_gemm_layer(int32_t kind, int32_t precision, const float* A, const f
   if (clear_n4 > 0) SB_TRY(alloc_filled(&clr, clr_n, 0x7f));
   SB_CUDA(cudaDeviceSynchronize());     // the uploads above ran on the legacy stream, the net launches on its own
 
-  StepIn in;
-  in.desc = net.desc; in.scal = net.scal; in.feed = resident ? Feed::RESIDENT : addend ? Feed::SPARSE : Feed::HOST;
   SB_TRY(net.refresh_shadows());
   net.launches = 0;
   if (kind == FWD) SB_TRY(net.enqueue_hidden_forward(in, M, nullptr, nullptr, reinterpret_cast<float4*>(clr.p), clear_n4));

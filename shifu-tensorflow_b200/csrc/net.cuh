@@ -22,18 +22,23 @@ struct Layer {
 // Where layer 0 of a step gets its batch:
 //   HOST      fp32 rows at desc->X (the staging area, or the fp32 resident set): load_batch_kernel fills Xb / Xf
 //   SPARSE    wide+deep: dense block + index matrix, hidden layer 0's one-hot block via the embedding
-//   RESIDENT  layer 0's GEMMs read their A operand by TMA from resident_Xb at row offset desc->row0
+//   RESIDENT  layer 0's GEMMs read their A operand by TMA from the resident set (StepIn::x0) at row offset desc->row0
 //   ORDERED   resident rows through the row order: gather_batch_kernel fills Xb / Xf, layer 0 reads them
 //   STREAMED  rows of a bf16 set in mapped host memory: gather_batch_kernel fetches them over PCIe into one of two batch
 //             buffers, in a run_resident graph one step ahead, beside the previous step's GEMMs (capi.cu, DESIGN §6e)
 enum class Feed { HOST, SPARSE, RESIDENT, ORDERED, STREAMED };
 
-// What one step's launches read: its descriptor / scalar slot and its feed.  The trainer takes the slots of its captured
-// steps from a ring of descriptor sets (capi.cu).
+// Layer 0's bf16 A operand in tensor-core modes: nparts arrays `ps` elements apart, whose tensor maps span `rows` rows
+// (0: the batch rows).  at_row0: the TMA row coordinate is offset by desc->row0 (the resident set, read in place).
+struct Operand0 { const __nv_bfloat16* p = nullptr; long long ps = 0; int rows = 0; bool at_row0 = false; };
+
+// What one step's launches read: its descriptor / scalar slot, its feed and layer 0's operand (unset: the net's own Xb,
+// Net::layer0).  The trainer takes the slots of its captured steps from a ring of descriptor sets (capi.cu).
 struct StepIn {
   BatchDesc* desc = nullptr;
   float* scal = nullptr;
   Feed feed = Feed::HOST;
+  Operand0 x0;
 };
 
 inline int pairs_of(int np) { return np == 3 ? 6 : (np == 2 ? 3 : 1); }
@@ -52,7 +57,6 @@ struct Net {
   bool tc() const { return precision != SB_PREC_FP32; }
   long long Xb_ps = 0;                       // part strides (elements)
   std::vector<long long> A_ps, Wn_ps;        // A_ps[l] also applies to dZ[l]
-  long long resident_ps = 0;
   int max_batch = 0, ldB = 0, ldF = 0;
   bool training = false;
 
@@ -147,9 +151,10 @@ struct Net {
   float* E = nullptr;                        // [max_batch, ld_out_0] embedding sums
   int set_sparse(int n_dense_, int n_onehot_, int n_cat_);
   int enqueue_embed(int rows, bool scatter, float* grad, cudaStream_t st);
-  // bf16 HBM-resident training set (trainer), read by steps with Feed::RESIDENT
-  const __nv_bfloat16* resident_Xb = nullptr;
-  long long resident_rows = 0;
+  // layer 0's A operand of a step over `rows` batch rows: in.x0, or, unset, Xb
+  Operand0 layer0(const StepIn& in, int rows) const {
+    return in.x0.p ? Operand0{in.x0.p, in.x0.ps, in.x0.rows ? in.x0.rows : rows, in.x0.at_row0} : Operand0{Xb, Xb_ps, rows};
+  }
   int enqueue_out(const StepIn& in, int rows, bool do_loss, bool do_bwd, float* yhat_dst, float* grad);
   // Backward pass, one GEMM per call; the trainer's step schedule (enqueue_step_backward, capi.cu) puts them on streams.
   // dW_l[r0, r1) rows of W_l (r1 < 0: all) += A_{l-1}^T dZ_l on `st`, its grid capped at `sms` (tensor-core modes; `pdl`:

@@ -1,5 +1,5 @@
 """Where a training step gets its batch (its feed): a host batch, the bf16 or fp32 resident set, the resident set through a
-row order, or a wide+deep sparse batch.
+row order, a bf16 set in host memory streamed batch by batch, or a wide+deep sparse batch.
 
 Every entry point describes its batch once and hands that description to the one descriptor writer, the one descriptor
 ring and the one graph cache of csrc/capi.cu.  These tests pin what that must keep:
@@ -38,6 +38,9 @@ EXPECTED = {
     "ordered_fp32": (9,
         ['gather_batch', 'out_layer', 'opt'],
         ['gather_batch', 'out_layer', 'opt']),
+    "streamed_bf16": (9,
+        ['fwd0@256x96x120', 'fwd_out1@256x64x96', 'dW1@96x64x256', 'dA1@256x96x64', 'dW0@120x96x256', 'opt', 'opt_side'],
+        ['fwd0@256x96x120', 'fwd_out1@256x64x96', 'dW1@96x64x256', 'dA1@256x96x64', 'dW0@120x96x256', 'opt', 'opt_side']),
     "sparse": (None,
         ['fwd0@130x40x21', 'fwd_out1@130x24x40', 'dW1@40x24x130', 'dA1@130x40x24', 'dW0@21x40x130', 'opt', 'opt_side'],
         None),
@@ -64,6 +67,8 @@ def observe(sb, feed):
         t.init_xavier(1)
         if feed != "host":
             X, y, w = so.synth_batch(N_ROWS, F, 3, weights="mixed")
+            if feed.startswith("streamed"):
+                t.debug_force_host_set(True)
             t.load_dataset(X, y, w)
             if feed.startswith("ordered"):
                 t.set_row_order(np.random.RandomState(5).permutation(N_ROWS))
@@ -86,7 +91,8 @@ def _h100_sxm(sb, monkeypatch):
     monkeypatch.setenv("SB_STEP_TRACE", "1")
 
 
-@pytest.mark.parametrize("feed", ["host", "resident_bf16", "resident_fp32", "ordered_bf16", "ordered_fp32", "sparse"])
+@pytest.mark.parametrize("feed", ["host", "resident_bf16", "resident_fp32", "ordered_bf16", "ordered_fp32", "streamed_bf16",
+                                  "sparse"])
 def test_step_launches_per_feed(sb, _h100_sxm, feed):
     kps, names, run_names = observe(sb, feed)
     assert (kps, names, run_names) == EXPECTED[feed]
