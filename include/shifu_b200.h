@@ -313,6 +313,12 @@ enum { SB_DEBUG_MSTAT_BATCHES = 0, SB_DEBUG_MSTAT_ROWS = 1, SB_DEBUG_MSTAT_MAX_F
 int sb_debug_model_batch_stats(sb_model_t* m, int64_t* stats, int32_t n_stats);
 /* The next compute() batch waits until k rows are queued or timeout_ms have passed (k = 0: no wait). */
 int sb_debug_model_hold(sb_model_t* m, int32_t k, int32_t timeout_ms);
+/* The kernels the model's last forward launched, "+"-joined into out (cap bytes, truncated to fit): "score_rows" for
+ * an fp32 batch of up to 128 rows, otherwise the batch load, one GEMM per hidden layer and the output layer, e.g.
+ * "load_batch<bf16>+gemm_wide+gemm_wide+gemm_pp<FWD>+out_layer_rows<1>"; "none" before the first forward.  Every
+ * scoring entry point runs its rows in forwards of at most max_batch rows (16384 in fp32, 65536 in bf16, 32768 in the
+ * split modes), so after a call this names the launches of its last piece. */
+int sb_debug_model_routes(sb_model_t* m, char* out, int32_t cap);
 
 /* ---- text ingest: the per-cell float() loop of load_data (ssgd_monitor.py:387-419) on the GPU ----
  * text: the gunzipped, delim-separated lines (must end with '\n'), HOST memory.  col_map[c] gives the role of text

@@ -153,6 +153,7 @@ PROTOTYPES = {
     "sb_model_stream": (C.c_void_p, [_vp]),
     "sb_debug_model_batch_stats": (C.c_int, [_vp, _P(C.c_int64), C.c_int32]),
     "sb_debug_model_hold": (C.c_int, [_vp, C.c_int32, C.c_int32]),
+    "sb_debug_model_routes": (C.c_int, [_vp, C.c_char_p, C.c_int32]),
     "sb_text_parse": (C.c_int, [_cp, C.c_int64, C.c_char, _P(C.c_int32), C.c_int32, C.c_int32, _f32p, _f32p, _f32p, C.c_int64,
                                 _P(C.c_int64), _P(CellFlag), C.c_int64, _P(C.c_int64), C.c_int]),
     "sb_text_parse_device": (C.c_int, [_cp, C.c_int64, C.c_char, _P(C.c_int32), C.c_int32, C.c_int32, _P(_f32p), _P(_f32p), _P(_f32p),
@@ -204,6 +205,8 @@ SCAL_LOSS_SUM, SCAL_NNZ, SCAL_COUNT = 0, 1, 4
 DEBUG_XINFO_WORDS, DEBUG_XWORK_WORDS = 24, 8
 DEBUG_MSTAT_WORDS = 6
 SMALL_ROWS = 128        # score_rows.cuh: an fp32 model scores batches of up to this many rows in one launch
+# capi.cu model_from_desc: a model runs every scoring call in forwards of at most this many rows (its max_batch)
+MODEL_CHUNK_ROWS = {PREC_FP32: 16384, PREC_BF16: 65536, PREC_FP32_TC: 32768, PREC_BF16X2: 32768}
 
 
 def lib():
@@ -719,6 +722,12 @@ class Model:
     def hold(self, k: int, timeout_ms: int):
         """the next compute() batch waits until k rows are queued or timeout_ms have passed (sb_debug_model_hold)"""
         check(lib().sb_debug_model_hold(self._h, int(k), int(timeout_ms)))
+
+    def routes(self) -> str:
+        """the kernels of the last forward, "+"-joined (sb_debug_model_routes)"""
+        buf = C.create_string_buffer(256)
+        check(lib().sb_debug_model_routes(self._h, buf, len(buf)))
+        return buf.value.decode()
 
 
 def nccl_unique_id() -> bytes:

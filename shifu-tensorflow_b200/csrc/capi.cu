@@ -1914,6 +1914,7 @@ struct sb_model {
   int hold_k = 0, hold_ms = 0;                // sb_debug_model_hold
   cudaGraphExec_t mb_graph = nullptr;         // tensor-core modes: the forward of MB_ROWS staged rows
   std::atomic<long long> st[SB_DEBUG_MSTAT_WORDS] = {};
+  std::string routes;         // the launches of the last model_forward, "+"-joined (sb_debug_model_routes; guarded by mu)
   ~sb_model() {
     if (!net.stream) return;
     cudaSetDevice(net.device);
@@ -1954,10 +1955,10 @@ static int model_from_desc(sb_net_desc d, const float* flat, int64_t n, int devi
   return SB_OK;
 }
 
-// The forward of `rows` (<= max_batch) device rows dX -> scores dOut (device), queued on the model's stream: every scoring
-// path of a model comes through here.  An fp32 batch of <= SMALL_ROWS rows is one score_rows_kernel launch; any other
-// batch runs the layer-by-layer launches.  Both give the same bits.  Called with m->mu held.
-static int model_forward(sb_model* m, const float* dX, int rows, float* dOut) {
+// The forward of `rows` (<= max_batch) device rows dX -> scores dOut (device), queued on the model's stream.  An fp32 batch
+// of <= SMALL_ROWS rows is one score_rows_kernel launch; any other batch runs the layer-by-layer launches.  Both give the
+// same bits.
+static int enqueue_model_forward(sb_model* m, const float* dX, int rows, float* dOut) {
   Net& n = m->net;
   if (!n.tc() && rows <= SMALL_ROWS) {
     ScoreRowsParams p = {};
@@ -1970,10 +1971,22 @@ static int model_forward(sb_model* m, const float* dX, int rows, float* dOut) {
     const int clusters = (rows + SR_ROWS - 1) / SR_ROWS;
     score_rows_kernel<<<clusters * SR_CLUSTER, SR_THREADS, SR_SMEM, n.stream>>>(p);
     SB_CUDA(cudaGetLastError());
+    n.mark("score_rows");
     ++m->st[SB_DEBUG_MSTAT_SMALL_LAUNCHES];
     return SB_OK;
   }
   return enqueue_forward(n, nullptr, StepIn{n.desc, n.scal}, host_batch(n, dX, nullptr, nullptr, rows), 0, false, dOut);
+}
+
+// Every scoring path of a model comes through here; its launches are kept for sb_debug_model_routes.  Called with m->mu
+// held.
+static int model_forward(sb_model* m, const float* dX, int rows, float* dOut) {
+  Net& n = m->net;
+  m->routes.clear();
+  n.marks = &m->routes;
+  const int s = enqueue_model_forward(m, dX, rows, dOut);
+  n.marks = nullptr;
+  return s;
 }
 
 // tensor-core modes: model_forward of MB_ROWS rows of the staging area, captured once, so a micro-batch is one launch
@@ -2160,6 +2173,14 @@ int sb_debug_model_batch_stats(sb_model_t* m, int64_t* stats, int32_t n_stats) {
   SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
   SB_CHECK(stats && n_stats >= SB_DEBUG_MSTAT_WORDS, SB_ERR_INVALID, "stats needs %d words, got %d", SB_DEBUG_MSTAT_WORDS, n_stats);
   for (int i = 0; i < SB_DEBUG_MSTAT_WORDS; ++i) stats[i] = m->st[i].load();
+  return SB_OK;
+}
+
+int sb_debug_model_routes(sb_model_t* m, char* out, int32_t cap) {
+  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
+  SB_CHECK(out && cap > 0, SB_ERR_INVALID, "route buffer of %d bytes", cap);
+  std::lock_guard<std::mutex> lk(m->mu);
+  snprintf(out, static_cast<size_t>(cap), "%s", m->routes.empty() ? "none" : m->routes.c_str());
   return SB_OK;
 }
 

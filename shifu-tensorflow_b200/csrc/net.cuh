@@ -112,7 +112,8 @@ struct Net {
   }
   // every launch of an enqueue_* routine: `kernel` names the kernel and tile it launched (sb_debug_gemm_layer reports it)
   const char* last_kernel = nullptr;
-  std::string* marks = nullptr;   // non-null: every launch's name is appended, "+"-joined (sb_debug_first_kernel)
+  std::string* marks = nullptr;   // non-null: every launch's name is appended, "+"-joined (sb_debug_first_kernel,
+                                  // sb_debug_model_routes)
   void mark(const char* kernel) {
     ++launches; last_kernel = kernel;
     if (marks) { if (!marks->empty()) *marks += '+'; *marks += kernel; }

@@ -45,15 +45,16 @@ def act_grad(a, act):
     return np.ones_like(a)
 
 
-def output_layer(a, e_a, wo, bo, y, w, act, loss, d, kink=None):
+def output_layer(a, e_a, wo, bo, y, w, act, loss, d, kink=None, e_z_add=0.0):
     """float64 values and bounds (module docstring) of every output of the layer on a [M, H] (float64) within e_a:
-    y_hat, g = dZ_L and e_g, and (value, bound) of db_L, dw_o, db_o and the loss sum for a reduction depth d"""
+    y_hat, g = dZ_L and e_g, and (value, bound) of db_L, dw_o, db_o and the loss sum for a reduction depth d.
+    e_z_add [M]: a bound on z the caller derived itself, added to e_z"""
     f64 = np.float64
     wo64 = wo.astype(f64)
     H = a.shape[1]
     aw = a * wo64
     z = aw.sum(axis=1) + f64(bo)
-    e_z = e_a @ np.abs(wo64) + (H + 4) * U * (np.abs(aw).sum(axis=1) + abs(f64(bo)))
+    e_z = e_a @ np.abs(wo64) + (H + 4) * U * (np.abs(aw).sum(axis=1) + abs(f64(bo))) + e_z_add
     yh = 1.0 / (1.0 + np.exp(-z))
     y64, w64 = y.astype(f64), w.astype(f64)
     nnz = np.count_nonzero(w)

@@ -33,6 +33,7 @@ import numpy as np
 import pytest
 
 from conftest import bf16_round
+from score_ref import contraction_c
 
 FP32, BF16, FP32_TC, BF16X2 = 0, 1, 2, 3
 PREC = {"fp32": FP32, "bf16": BF16, "fp32_tc": FP32_TC, "bf16x2": BF16X2}
@@ -66,7 +67,7 @@ def _note(name, err, tol):
 
 
 def _c(prec, K):
-    return (K + 2) * U if prec == FP32 else {1: 3e-6, 2: 2e-5, 3: 3e-6}[NPARTS[prec]]
+    return contraction_c(prec, K)
 
 
 def _act(z, act):

@@ -241,4 +241,5 @@ def test_debug_hooks_reject_a_null_handle(sb):
     st = (ctypes.c_int64 * sb.capi.DEBUG_MSTAT_WORDS)()
     assert lib.sb_debug_model_batch_stats(None, st, sb.capi.DEBUG_MSTAT_WORDS) == sb.capi.SB_ERR_STATE
     assert lib.sb_debug_model_hold(None, 4, 10) == sb.capi.SB_ERR_STATE
+    assert lib.sb_debug_model_routes(None, ctypes.create_string_buffer(64), 64) == sb.capi.SB_ERR_STATE
     assert b"not initialized" in lib.sb_last_error()
