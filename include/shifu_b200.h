@@ -302,6 +302,30 @@ int sb_model_score_row_f64(sb_model_t* m, const double* row, int32_t n, double* 
 /* device-resident scoring (X, out are DEVICE pointers on the model's device), asynchronous on the
  * model's stream; sb_model_sync waits. */
 int sb_model_score_device(sb_model_t* m, const float* dX, int64_t rows, float* dOut);
+/* Column sensitivity (varsel filterBy SE / ST, per-row reason codes).  With s(x) the score sb_model_score computes in
+ * the model's precision mode, for row r and list position k:
+ *   d[r,k] = s(x_r) - s(x_r with column cols[k] set to values[k])
+ *   sum_sq[k] = sum_r w_r d^2,  sum[k] = sum_r w_r d,  *w_sum = sum_r w_r.
+ * cols == NULL && n_cols == 0: every column in order; otherwise n_cols >= 1 columns in [0, n_features), in any order,
+ * repeats allowed; outputs follow list positions.  values: NULL (every value 0, the mean of a ZSCALE-normalised column)
+ * or one finite value per list position.  w: NULL weighs every row 1.  deltas: nullable, row-major [rows, n_cols].
+ * X, w and deltas may be host or device pointers on the model's device; sum_sq, sum (n_cols each) and w_sum are host
+ * memory.  Synchronous; takes the model's device lock, so it is safe beside compute() callers on the same handle.
+ * Guarantees:
+ *   - same bits on repeat: every output is bit-identical across calls with the same inputs, and the sums do not depend
+ *     on whether deltas was requested or on whether X / w are host or device pointers;
+ *   - zero when nothing changes: d is exactly +0 wherever x[r, cols[k]] == values[k] (the base score each delta is
+ *     taken against comes out of the same launches as the perturbed scores);
+ *   - fixed-order sums: accumulated in fp64, over rows in a fixed tree per row chunk and over row chunks in order.
+ * Layer 0's pre-activation z0 is computed once per row; each (row, column) pair is the rank-1 update
+ * z0 + (v - x_c) W0[c, :] followed by layers 1..L.  The scores are s within the model's precision (not bit-identical to
+ * sb_model_score's: z0 is kept in fp32 and updated before the activation).  Rows go in chunks of
+ * R = clamp(max_batch / (n_cols + 1), 64, max_batch / 2) rows; a chunk's list positions in pieces of up to
+ * max_batch / R - 1 columns, each one forward of R (columns + 1) pair rows.
+ * Errors, all reported before any device work: a null model SB_ERR_STATE; null X / sum_sq / sum / w_sum, rows < 0, a bad
+ * cols / n_cols pair, a column out of range or a non-finite value SB_ERR_INVALID.  rows = 0 returns zeros. */
+int sb_model_sensitivity(sb_model_t* m, const float* X, const float* w, int64_t rows, const int32_t* cols, int32_t n_cols,
+                         const float* values, double* sum_sq, double* sum, double* w_sum, float* deltas);
 int sb_model_sync(sb_model_t* m);
 void* sb_model_stream(sb_model_t* m);
 /* Test hooks of the scorer.  stats[SB_DEBUG_MSTAT_WORDS] since creation = {compute() batches run, rows they scored,
@@ -317,7 +341,9 @@ int sb_debug_model_hold(sb_model_t* m, int32_t k, int32_t timeout_ms);
  * an fp32 batch of up to 128 rows, otherwise the batch load, one GEMM per hidden layer and the output layer, e.g.
  * "load_batch<bf16>+gemm_wide+gemm_wide+gemm_pp<FWD>+out_layer_rows<1>"; "none" before the first forward.  Every
  * scoring entry point runs its rows in forwards of at most max_batch rows (16384 in fp32, 65536 in bf16, 32768 in the
- * split modes), so after a call this names the launches of its last piece. */
+ * split modes), so after a call this names the launches of its last piece.  After sb_model_sensitivity: the launches
+ * of its last row chunk's z0 and last piece, e.g.
+ * "load_batch<bf16>+gemm_tc<128,F32>+sens_perturb<bf16>+gemm_pp<FWD>+gemm_pp<FWD>+out_layer_rows<1>+sens_reduce". */
 int sb_debug_model_routes(sb_model_t* m, char* out, int32_t cap);
 
 /* ---- text ingest: the per-cell float() loop of load_data (ssgd_monitor.py:387-419) on the GPU ----

@@ -149,6 +149,7 @@ PROTOTYPES = {
     "sb_model_score": (C.c_int, [_vp, _f32p, C.c_int64, _f32p]),
     "sb_model_score_row_f64": (C.c_int, [_vp, _f64p, C.c_int32, _f64p]),
     "sb_model_score_device": (C.c_int, [_vp, _vp, C.c_int64, _vp]),
+    "sb_model_sensitivity": (C.c_int, [_vp, _vp, _vp, C.c_int64, _P(C.c_int32), C.c_int32, _f32p, _f64p, _f64p, _f64p, _vp]),
     "sb_model_sync": (C.c_int, [_vp]),
     "sb_model_stream": (C.c_void_p, [_vp]),
     "sb_debug_model_batch_stats": (C.c_int, [_vp, _P(C.c_int64), C.c_int32]),
@@ -244,6 +245,22 @@ def _ptr(a):
     if hasattr(a, "ptr") and not isinstance(a, np.ndarray):      # DeviceArray
         return a.ptr
     return a.ctypes.data_as(_f32p)
+
+
+def _in_ptr(a):
+    """-> (void pointer, shape) of a numpy array (host), a DeviceArray or a CUDA tensor (device); numpy arrays must be
+    C-contiguous fp32, anything else is converted to one"""
+    if isinstance(a, DeviceArray):
+        return C.c_void_p(C.cast(a.ptr, _vp).value), a.shape
+    if hasattr(a, "data_ptr") and getattr(a, "is_cuda", False):
+        if not a.is_contiguous() or str(a.dtype) != "torch.float32":
+            raise ValueError("a device tensor must be contiguous float32")
+        return C.c_void_p(a.data_ptr()), tuple(a.shape)
+    if hasattr(a, "numpy") and not isinstance(a, np.ndarray):
+        a = a.numpy()
+    if not (isinstance(a, np.ndarray) and a.dtype == np.float32 and a.flags.c_contiguous):
+        raise ValueError("a host array must be C-contiguous float32 (it is read in place)")
+    return a.ctypes.data_as(_vp), a.shape
 
 
 class DeviceArray:
@@ -704,6 +721,39 @@ class Model:
 
     def score_device(self, dX_ptr: int, rows: int, dOut_ptr: int):
         check(lib().sb_model_score_device(self._h, C.c_void_p(dX_ptr), rows, C.c_void_p(dOut_ptr)))
+
+    def sensitivity(self, X, w=None, cols=None, values=None, deltas=False) -> dict:
+        """Column sensitivity (sb_model_sensitivity): for each list position k, d[r, k] = s(X[r]) - s(X[r] with column
+        cols[k] set to values[k]).  -> {"sum_sq": sum_r w d^2, "sum": sum_r w d (float64 [n_cols]), "w_sum": sum_r w,
+        "deltas": d [rows, n_cols] or None}.
+        X / w: numpy arrays (host) or CUDA tensors / DeviceArrays on the model's device.  cols: None for every column in
+        order.  values: None for 0 at every position.  deltas: False (not computed), True (returned as a host array) or a
+        device buffer of rows * n_cols floats to write them into."""
+        xp, shape = _in_ptr(X)
+        if len(shape) != 2 or shape[1] != self.n_features:
+            raise ValueError("X must be [rows, %d]" % self.n_features)
+        rows = int(shape[0])
+        wp, wshape = _in_ptr(w) if w is not None else (None, (rows,))
+        if int(np.prod(wshape)) != rows:
+            raise ValueError("w must hold one weight per row")
+        cl = None if cols is None else np.ascontiguousarray(cols, dtype=np.int32).reshape(-1)
+        n_cols = self.n_features if cl is None else cl.size
+        vl = None if values is None else _f32(values).reshape(-1)
+        if vl is not None and vl.size != n_cols:
+            raise ValueError("values must hold one value per list position (%d)" % n_cols)
+        sum_sq, total, w_sum = np.zeros(n_cols), np.zeros(n_cols), C.c_double()
+        if deltas is True:
+            d_out = np.empty((rows, n_cols), np.float32)
+            dp = d_out.ctypes.data_as(_vp)
+        elif deltas is False or deltas is None:
+            d_out, dp = None, None
+        else:
+            d_out = deltas
+            dp = _in_ptr(deltas)[0]
+        check(lib().sb_model_sensitivity(self._h, xp, wp, rows, None if cl is None else cl.ctypes.data_as(_P(C.c_int32)),
+                                         0 if cl is None else cl.size, None if vl is None else _ptr(vl),
+                                         sum_sq.ctypes.data_as(_f64p), total.ctypes.data_as(_f64p), C.byref(w_sum), dp))
+        return {"sum_sq": sum_sq, "sum": total, "w_sum": float(w_sum.value), "deltas": d_out}
 
     def sync(self):
         check(lib().sb_model_sync(self._h))

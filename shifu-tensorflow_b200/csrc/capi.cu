@@ -14,6 +14,7 @@
 #include "net.cuh"
 #include "savedmodel.h"
 #include "score_rows.cuh"
+#include "sensitivity.cuh"
 #include "xchg_p2p.cuh"
 
 using namespace sb;
@@ -1915,6 +1916,13 @@ struct sb_model {
   cudaGraphExec_t mb_graph = nullptr;         // tensor-core modes: the forward of MB_ROWS staged rows
   std::atomic<long long> st[SB_DEBUG_MSTAT_WORDS] = {};
   std::string routes;         // the launches of the last model_forward, "+"-joined (sb_debug_model_routes; guarded by mu)
+  // sb_model_sensitivity's buffers (guarded by mu), allocated by its first call and grown when a call needs more
+  DevBuf<float> sens_z;       // layer 0's pre-activations of a row chunk [R, ld_out_0]
+  DevBuf<double> sens_acc;    // running sums [list position][w d^2, w d], then sum w
+  DevBuf<int> sens_cols;      // the column list and its values
+  DevBuf<float> sens_vals;
+  DevBuf<float> sens_d;       // the deltas of one piece [R, piece columns] (max_batch)
+  size_t sens_z_n = 0, sens_list_n = 0;
   ~sb_model() {
     if (!net.stream) return;
     cudaSetDevice(net.device);
@@ -2159,6 +2167,141 @@ int sb_model_score_device(sb_model_t* m, const float* dX, int64_t rows, float* d
     const int c = static_cast<int>(rows - r0 < n.max_batch ? rows - r0 : n.max_batch);
     SB_TRY(model_forward(m, dX + r0 * n.F, c, dOut + r0));
   }
+  return SB_OK;
+}
+
+}  // extern "C"
+
+// Rows per row chunk for C list positions: max_batch / (C + 1), so that a row chunk's pairs fit one piece, but at least 64
+// (more columns go in several pieces) and at most max_batch / 2
+static int sens_chunk_rows(int max_batch, int C) {
+  long long r = max_batch / (static_cast<long long>(C) + 1);
+  if (r < 64) r = 64;
+  if (r > max_batch / 2) r = max_batch / 2;
+  return static_cast<int>(r > 0 ? r : 1);
+}
+
+static int sens_grow(DevBuf<float>* b, size_t* cap, size_t n) {
+  if (n <= *cap) return SB_OK;
+  *b = DevBuf<float>();
+  SB_TRY(b->alloc(n));
+  *cap = n;
+  return SB_OK;
+}
+
+// Column sensitivity (sensitivity.cuh, DESIGN §6f), called with m->mu held.  Rows go in row chunks of R rows
+// (sens_chunk_rows); a row chunk's z0 is computed once, and its list positions go in pieces of up to max_batch / R - 1
+// columns, each piece one forward of R (columns + 1) pair rows through layers 1..L and the output unit.
+static int sens_forward(sb_model* m, const float* X, const float* w, int64_t rows, int C, float* deltas) {
+  Net& n = m->net;
+  const Layer& l0 = n.layers[0];
+  const int R = sens_chunk_rows(n.max_batch, C);
+  const int Cp = n.max_batch / R - 1;
+  SB_TRY(sens_grow(&m->sens_z, &m->sens_z_n, static_cast<size_t>(R) * l0.ld_out));
+  if (!m->sens_d.p) SB_TRY(m->sens_d.alloc(static_cast<size_t>(n.max_batch)));
+  const StepIn in{n.desc, n.scal};
+  SensParams sp = {};
+  sp.F = n.F; sp.N = l0.out; sp.ld = l0.ld_out;
+  sp.X = n.stX;
+  sp.z = m->sens_z.p;
+  sp.act = l0.act;
+  if (n.tc()) {
+    sp.bias = n.theta + l0.b_off;
+    sp.Wn = l0.Wn; sp.w_ps = n.Wn_ps[0];
+    sp.out = n.A[0]; sp.out_ps = n.A_ps[0];
+  } else {
+    sp.W32 = n.theta + l0.w_off;
+    sp.out32 = n.Af[0];
+  }
+  using PerturbFn = void (*)(SensParams);
+  const PerturbFn perturb = !n.tc() ? sens_perturb_kernel<false, 1>
+                                    : n.nparts == 3 ? sens_perturb_kernel<true, 3>
+                                    : n.nparts == 2 ? sens_perturb_kernel<true, 2> : sens_perturb_kernel<true, 1>;
+  const char* perturb_name = !n.tc() ? "sens_perturb<fp32>"
+                             : n.nparts == 3 ? "sens_perturb<bf16x3>"
+                             : n.nparts == 2 ? "sens_perturb<bf16x2>" : "sens_perturb<bf16>";
+  const size_t row_bytes = sizeof(float) * n.F;
+  for (int64_t r0 = 0; r0 < rows; r0 += R) {
+    const int rc = static_cast<int>(rows - r0 < R ? rows - r0 : R);
+    SB_CUDA(cudaMemcpyAsync(n.stX, X + r0 * n.F, row_bytes * rc, cudaMemcpyDefault, n.stream));
+    if (w) SB_CUDA(cudaMemcpyAsync(n.stW, w + r0, sizeof(float) * rc, cudaMemcpyDefault, n.stream));
+    const float* wd = w ? n.stW : n.ones;
+    m->routes.clear();
+    const Batch b = host_batch(n, n.stX, nullptr, wd, rc);
+    SB_TRY(write_desc(n.stream, in, &b, 0.f, 1.f, 0, nullptr));
+    SB_TRY(enqueue_first(n, nullptr, in, rc, nullptr, 0));
+    SB_TRY(n.enqueue_layer0_pre(in, rc, m->sens_z.p, l0.ld_out));
+    const std::string prefix = m->routes;
+    sp.R = rc;
+    for (int k0 = 0; k0 < C; k0 += Cp) {
+      const int ck = C - k0 < Cp ? C - k0 : Cp;
+      const int pairs = rc * (ck + 1);
+      m->routes = prefix;
+      sp.cols = m->sens_cols.p + k0; sp.vals = m->sens_vals.p + k0;
+      const dim3 grid(static_cast<unsigned>((l0.out + 255) / 256), static_cast<unsigned>(ck + 1),
+                      static_cast<unsigned>((rc + SENS_ROWS - 1) / SENS_ROWS));
+      SB_TRY(launch_kernel(perturb, grid, dim3(32, 8), 0, n.stream, false, sp));
+      n.mark(perturb_name);
+      SB_TRY(n.enqueue_hidden_forward(in, pairs, nullptr, nullptr, nullptr, 0, 1));
+      SB_TRY(n.enqueue_out(in, pairs, false, false, n.yhat, nullptr));
+      SB_TRY(launch_kernel(sens_reduce_kernel, dim3(static_cast<unsigned>(ck + 1)), dim3(SENS_REDUCE_THREADS), 0, n.stream, false,
+                           static_cast<const float*>(n.yhat), wd, rc, ck, k0, deltas ? m->sens_d.p : nullptr, ck, m->sens_acc.p,
+                           k0 == 0 ? 1 : 0, 2LL * C));
+      n.mark("sens_reduce");
+      if (deltas)
+        SB_CUDA(cudaMemcpy2DAsync(deltas + r0 * C + k0, sizeof(float) * C, m->sens_d.p, sizeof(float) * ck, sizeof(float) * ck, rc,
+                                  cudaMemcpyDefault, n.stream));
+    }
+  }
+  return SB_OK;
+}
+
+extern "C" {
+
+int sb_model_sensitivity(sb_model_t* m, const float* X, const float* w, int64_t rows, const int32_t* cols, int32_t n_cols,
+                         const float* values, double* sum_sq, double* sum, double* w_sum, float* deltas) {
+  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
+  SB_CHECK(X && sum_sq && sum && w_sum, SB_ERR_INVALID, "null argument");
+  SB_CHECK(rows >= 0, SB_ERR_INVALID, "rows = %lld < 0", static_cast<long long>(rows));
+  SB_CHECK((cols == nullptr && n_cols == 0) || (cols != nullptr && n_cols >= 1), SB_ERR_INVALID,
+           "cols / n_cols: a list of n_cols >= 1 columns, or NULL and 0 for every column (got %s and %d)", cols ? "a list" : "NULL",
+           n_cols);
+  Net& n = m->net;
+  const int C = cols ? n_cols : n.F;
+  std::vector<int32_t> cl(static_cast<size_t>(C));
+  std::vector<float> vl(static_cast<size_t>(C));
+  for (int k = 0; k < C; ++k) {
+    cl[k] = cols ? cols[k] : k;
+    SB_CHECK(cl[k] >= 0 && cl[k] < n.F, SB_ERR_INVALID, "cols[%d] = %d outside [0, %d)", k, cl[k], n.F);
+    vl[k] = values ? values[k] : 0.f;
+    SB_CHECK(std::isfinite(vl[k]), SB_ERR_INVALID, "values[%d] = %g is not finite", k, static_cast<double>(vl[k]));
+  }
+  for (int k = 0; k < C; ++k) sum_sq[k] = sum[k] = 0.0;
+  *w_sum = 0.0;
+  if (rows == 0) return SB_OK;
+  std::lock_guard<std::mutex> lk(m->mu);
+  SB_CUDA(cudaSetDevice(n.device));
+  const size_t list_n = static_cast<size_t>(C);
+  if (list_n > m->sens_list_n) {
+    m->sens_acc = DevBuf<double>(); m->sens_cols = DevBuf<int>(); m->sens_vals = DevBuf<float>();
+    m->sens_list_n = 0;
+    SB_TRY(m->sens_acc.alloc(2 * list_n + 1));
+    SB_TRY(m->sens_cols.alloc(list_n));
+    SB_TRY(m->sens_vals.alloc(list_n));
+    m->sens_list_n = list_n;
+  }
+  SB_CUDA(cudaMemcpyAsync(m->sens_cols.p, cl.data(), sizeof(int32_t) * list_n, cudaMemcpyHostToDevice, n.stream));
+  SB_CUDA(cudaMemcpyAsync(m->sens_vals.p, vl.data(), sizeof(float) * list_n, cudaMemcpyHostToDevice, n.stream));
+  SB_CUDA(cudaMemsetAsync(m->sens_acc.p, 0, sizeof(double) * (2 * list_n + 1), n.stream));
+  n.marks = &m->routes;
+  const int s = sens_forward(m, X, w, rows, C, deltas);
+  n.marks = nullptr;
+  SB_TRY(s);
+  std::vector<double> acc(2 * list_n + 1);
+  SB_CUDA(cudaMemcpyAsync(acc.data(), m->sens_acc.p, sizeof(double) * acc.size(), cudaMemcpyDeviceToHost, n.stream));
+  SB_CUDA(cudaStreamSynchronize(n.stream));
+  for (int k = 0; k < C; ++k) { sum_sq[k] = acc[2 * k]; sum[k] = acc[2 * k + 1]; }
+  *w_sum = acc[2 * list_n];
   return SB_OK;
 }
 

@@ -442,9 +442,10 @@ int Net::enqueue_load(const StepIn& in, int rows, float* clear, long long clear_
   return SB_OK;
 }
 
-int Net::enqueue_hidden_forward(const StepIn& in, int rows, float* grad, bool* fused_out, float4* clear, long long clear_n4) {
+int Net::enqueue_hidden_forward(const StepIn& in, int rows, float* grad, bool* fused_out, float4* clear, long long clear_n4,
+                                int first) {
   if (fused_out) *fused_out = false;
-  for (int l = 0; l < L; ++l) {
+  for (int l = first; l < L; ++l) {
     Layer& ly = layers[l];
     const bool sp0 = (l == 0) && in.feed == Feed::SPARSE;       // wide+deep: contract the dense columns only, add the embedding sums
     const int k_in = sp0 ? n_dense : ly.in;
@@ -570,6 +571,37 @@ int Net::enqueue_out(const StepIn& in, int rows, bool do_loss, bool do_bwd, floa
   }
   SB_CUDA(cudaGetLastError());
   mark(kernel);
+  return SB_OK;
+}
+
+int Net::enqueue_layer0_pre(const StepIn& in, int rows, float* z, int ld_z) {
+  const Layer& ly = layers[0];
+  if (!tc()) {
+    GemmF32Params p = {};
+    p.M = rows; p.N = ly.out; p.K = ly.in;
+    p.A = Xf; p.sAm = ly.in; p.sAk = 1;
+    p.B = theta + ly.w_off; p.sBk = ly.out; p.sBn = 1;
+    p.bias = theta + ly.b_off; p.act = SB_ACT_NONE;
+    p.out = z; p.ld_out = ld_z;
+    SB_TRY(launch_gemm_f32<EPI_FWD>(p, 1, stream));
+    mark("gemm_f32<FWD>");
+    return SB_OK;
+  }
+  if (!f32_attrs) {
+    SB_TRY((set_gemm_tc_attrs<EPI_F32, false, true>()));
+    f32_attrs = true;
+  }
+  const Operand0 a = layer0(in, rows);
+  const GemmPlan pl = plan_gemm(rows, ly.out, round_up(ly.in, 64) * pairs_of(nparts), num_sms, false);
+  TmapSet tm;
+  SB_TRY(make_tmaps_bf16(tm.a, a.p, a.ps, nparts, a.rows, ly.in, ly.ld_in, 128));
+  SB_TRY(make_tmaps_bf16(tm.b, ly.Wn, Wn_ps[0], nparts, ly.in, ly.out, ly.ld_out, 64));
+  GemmTcParams p = {};
+  set_part_pairs(&p, nparts);
+  p.M = rows; p.N = ly.out; p.K = ly.in;
+  p.accum = z; p.ld_acc = ld_z;
+  SB_TRY((launch_gemm_tc<EPI_F32, false, true>(pl, tm, p, stream, true)));
+  mark(pl.bn == 64 ? "gemm_tc<64,F32>" : "gemm_tc<128,F32>");
   return SB_OK;
 }
 

@@ -141,9 +141,11 @@ struct Net {
   int enqueue_load(const StepIn& in, int rows, float* clear = nullptr, long long clear_n = 0);
   // grad != nullptr (training step): the last hidden layer's GEMM also runs the output layer, the loss and the output
   // backward in its epilogue when h_L <= 128; *fused_out tells the caller whether enqueue_out is still needed.  clear
-  // (resident steps): the layer-0 GEMM's idle producer warps clear clear[0, clear_n4) beside its main loop.
+  // (resident steps): the layer-0 GEMM's idle producer warps clear clear[0, clear_n4) beside its main loop.  first > 0
+  // starts at hidden layer `first`, whose input A_{first-1} the caller has written (sb_model_sensitivity: layer 0's
+  // rank-1 updates).
   int enqueue_hidden_forward(const StepIn& in, int rows, float* grad = nullptr, bool* fused_out = nullptr, float4* clear = nullptr,
-                             long long clear_n4 = 0);
+                             long long clear_n4 = 0, int first = 0);
   // wide+deep first layer (oracle/wide_deep.py): hidden layer 0 = [n_dense numeric columns | n_onehot one-hot columns of
   // n_cat categorical columns]; a SPARSE step feeds (dense block, index matrix) and evaluates the one-hot block as an
   // embedding gather / scatter-add.  F = n_dense + n_onehot, the parameters are those of the dense net.
@@ -157,6 +159,11 @@ struct Net {
     return in.x0.p ? Operand0{in.x0.p, in.x0.ps, in.x0.rows ? in.x0.rows : rows, in.x0.at_row0} : Operand0{Xb, Xb_ps, rows};
   }
   int enqueue_out(const StepIn& in, int rows, bool do_loss, bool do_bwd, float* yhat_dst, float* grad);
+  // layer 0's pre-activation of the batch's rows to fp32 z [rows, ld_z] (sb_model_sensitivity): tensor-core modes
+  // X W0 from the bf16 parts by the fp32-store GEMM (every part pair, fp32 accumulator stored as it is, no bias), fp32
+  // mode X W0 + b0 by the fp32 GEMM
+  int enqueue_layer0_pre(const StepIn& in, int rows, float* z, int ld_z);
+  bool f32_attrs = false;                  // the fp32-store GEMM's shared-memory opt-in is done
   // Backward pass, one GEMM per call; the trainer's step schedule (enqueue_step_backward, capi.cu) puts them on streams.
   // dW_l[r0, r1) rows of W_l (r1 < 0: all) += A_{l-1}^T dZ_l on `st`, its grid capped at `sms` (tensor-core modes; `pdl`:
   // launched with programmatic dependent launch); layer 0 of a sparse step also scatter-adds the embedding rows' gradient.

@@ -108,6 +108,22 @@ class TensorflowModel:
         X = np.asarray(rows, dtype=np.float64).astype(np.float32)     # the same double -> float cast, vectorised
         return self._model.score(X).astype(np.float64)
 
+    # -- new: column sensitivity (varsel filterBy SE / ST): each column replaced by a value, over the whole table --
+    def computeSensitivity(self, rows, weights=None, columns=None, values=None) -> dict:
+        """-> {"sum_sq", "sum": per-column sums of w d^2 and w d, "w_sum", "mse" = sum_sq / w_sum, "mean" = sum / w_sum},
+        with d = compute(row) - compute(row with the column set to its value); columns None: every column; values None:
+        0 per column (the mean of a ZSCALE-normalised column)"""
+        if not self.initiate or self._model is None:
+            raise IllegalStateException("TF model not initialized.")
+        X = np.asarray(rows, dtype=np.float64).astype(np.float32)     # the same double -> float cast as computeBatch
+        w = None if weights is None else np.asarray(weights, dtype=np.float64).astype(np.float32)
+        vals = None if values is None else np.asarray(values, dtype=np.float64).astype(np.float32)
+        r = self._model.sensitivity(X, w=w, cols=columns, values=vals)
+        ws = r["w_sum"]
+        with np.errstate(invalid="ignore", divide="ignore"):
+            mse, mean = r["sum_sq"] / ws, r["sum"] / ws
+        return {"sum_sq": r["sum_sq"], "sum": r["sum"], "w_sum": ws, "mse": mse, "mean": mean}
+
     def releaseResource(self) -> None:
         """The reference never closes its bundle (TensorflowModel.java:175-176); here device memory is returned."""
         if self._model is not None:
