@@ -326,6 +326,24 @@ int sb_model_score_device(sb_model_t* m, const float* dX, int64_t rows, float* d
  * cols / n_cols pair, a column out of range or a non-finite value SB_ERR_INVALID.  rows = 0 returns zeros. */
 int sb_model_sensitivity(sb_model_t* m, const float* X, const float* w, int64_t rows, const int32_t* cols, int32_t n_cols,
                          const float* values, double* sum_sq, double* sum, double* w_sum, float* deltas);
+/* Per-row reason codes: for each row, the k list positions whose deltas rank first, computed on the GPU without
+ * materialising the [rows, n_cols] deltas.  d[r,j] is sb_model_sensitivity's delta, with the same cols / n_cols / values
+ * rules.  Ranking order (total, so the result is unique): the key is d for SB_REASON_RAISE (the values that push the
+ * score up the most), -d for SB_REASON_LOWER and |d| for SB_REASON_MAGNITUDE; a larger key ranks first; keys compare as
+ * floats (-0 == +0); a NaN key ranks after every other key; equal keys rank by the smaller list position.
+ * Outputs, row-major: pos [rows, k] int32, the list positions best first; d [rows, k] their deltas; scores (nullable)
+ * [rows] the base score s(x_r) the deltas are taken against.  That score is computed as this call computes it (z0 kept
+ * in fp32), so it is not bit-identical to sb_model_score's.
+ * Every returned d[r,i] is bit-identical to deltas[r, pos[r,i]] of sb_model_sensitivity on the same model and inputs:
+ * the call runs the same row chunks, pieces and launches up to the pair scores, and merges each piece's deltas into a
+ * running top k per row on the device.
+ * X, pos, d and scores may be host or device pointers on the model's device.  Synchronous; takes the model's device
+ * lock, so it is safe beside compute() callers on the same handle.  rows = 0 returns SB_OK and writes nothing.
+ * Errors, all reported before any device work: a null model SB_ERR_STATE; null X / pos / d, rows < 0, a bad cols / n_cols
+ * pair, a column out of range, a non-finite value, k < 1, k > min(n_cols, 32) or an unknown order SB_ERR_INVALID. */
+enum { SB_REASON_RAISE = 0, SB_REASON_LOWER = 1, SB_REASON_MAGNITUDE = 2 };
+int sb_model_reason_codes(sb_model_t* m, const float* X, int64_t rows, const int32_t* cols, int32_t n_cols, const float* values,
+                          int32_t k, int32_t order, int32_t* pos, float* d, float* scores);
 int sb_model_sync(sb_model_t* m);
 void* sb_model_stream(sb_model_t* m);
 /* Test hooks of the scorer.  stats[SB_DEBUG_MSTAT_WORDS] since creation = {compute() batches run, rows they scored,
@@ -343,7 +361,8 @@ int sb_debug_model_hold(sb_model_t* m, int32_t k, int32_t timeout_ms);
  * scoring entry point runs its rows in forwards of at most max_batch rows (16384 in fp32, 65536 in bf16, 32768 in the
  * split modes), so after a call this names the launches of its last piece.  After sb_model_sensitivity: the launches
  * of its last row chunk's z0 and last piece, e.g.
- * "load_batch<bf16>+gemm_tc<128,F32>+sens_perturb<bf16>+gemm_pp<FWD>+gemm_pp<FWD>+out_layer_rows<1>+sens_reduce". */
+ * "load_batch<bf16>+gemm_tc<128,F32>+sens_perturb<bf16>+gemm_pp<FWD>+gemm_pp<FWD>+out_layer_rows<1>+sens_reduce".
+ * After sb_model_reason_codes: the same, ending in "sens_topk" instead of "sens_reduce". */
 int sb_debug_model_routes(sb_model_t* m, char* out, int32_t cap);
 
 /* ---- text ingest: the per-cell float() loop of load_data (ssgd_monitor.py:387-419) on the GPU ----

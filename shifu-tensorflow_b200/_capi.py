@@ -32,6 +32,8 @@ _RMSPROP_DEFAULTS = dict(rho=0.9, epsilon=1e-10, momentum=0.0)
 _OTHER_DEFAULTS = dict(rho=0.95, epsilon=1e-8, momentum=0.9)
 INITIAL_ACCUMULATOR, L1, L2 = 0.1, 0.0, 0.0     # Adagrad / FTRL (Trainer(initial_accumulator=, l1=, l2=))
 PREC_FP32, PREC_BF16, PREC_FP32_TC, PREC_BF16X2 = 0, 1, 2, 3
+SB_REASON_RAISE, SB_REASON_LOWER, SB_REASON_MAGNITUDE = 0, 1, 2
+REASON_ORDERS = {"raise": SB_REASON_RAISE, "lower": SB_REASON_LOWER, "magnitude": SB_REASON_MAGNITUDE}
 SB_OK, SB_ERR_INVALID, SB_ERR_CUDA, SB_ERR_NCCL, SB_ERR_IO, SB_ERR_STATE, SB_ERR_FORMAT = 0, -1, -2, -3, -4, -5, -6
 
 
@@ -150,6 +152,8 @@ PROTOTYPES = {
     "sb_model_score_row_f64": (C.c_int, [_vp, _f64p, C.c_int32, _f64p]),
     "sb_model_score_device": (C.c_int, [_vp, _vp, C.c_int64, _vp]),
     "sb_model_sensitivity": (C.c_int, [_vp, _vp, _vp, C.c_int64, _P(C.c_int32), C.c_int32, _f32p, _f64p, _f64p, _f64p, _vp]),
+    "sb_model_reason_codes": (C.c_int, [_vp, _vp, C.c_int64, _P(C.c_int32), C.c_int32, _f32p, C.c_int32, C.c_int32, _vp, _vp,
+                                        _vp]),
     "sb_model_sync": (C.c_int, [_vp]),
     "sb_model_stream": (C.c_void_p, [_vp]),
     "sb_debug_model_batch_stats": (C.c_int, [_vp, _P(C.c_int64), C.c_int32]),
@@ -247,19 +251,20 @@ def _ptr(a):
     return a.ctypes.data_as(_f32p)
 
 
-def _in_ptr(a):
+def _in_ptr(a, dtype=np.float32):
     """-> (void pointer, shape) of a numpy array (host), a DeviceArray or a CUDA tensor (device); numpy arrays must be
-    C-contiguous fp32, anything else is converted to one"""
+    C-contiguous `dtype` (fp32 by default), anything else is converted to one"""
+    name = np.dtype(dtype).name
     if isinstance(a, DeviceArray):
         return C.c_void_p(C.cast(a.ptr, _vp).value), a.shape
     if hasattr(a, "data_ptr") and getattr(a, "is_cuda", False):
-        if not a.is_contiguous() or str(a.dtype) != "torch.float32":
-            raise ValueError("a device tensor must be contiguous float32")
+        if not a.is_contiguous() or str(a.dtype) != "torch." + name:
+            raise ValueError("a device tensor must be contiguous " + name)
         return C.c_void_p(a.data_ptr()), tuple(a.shape)
     if hasattr(a, "numpy") and not isinstance(a, np.ndarray):
         a = a.numpy()
-    if not (isinstance(a, np.ndarray) and a.dtype == np.float32 and a.flags.c_contiguous):
-        raise ValueError("a host array must be C-contiguous float32 (it is read in place)")
+    if not (isinstance(a, np.ndarray) and a.dtype == dtype and a.flags.c_contiguous):
+        raise ValueError("a host array must be C-contiguous %s (it is read in place)" % name)
     return a.ctypes.data_as(_vp), a.shape
 
 
@@ -754,6 +759,40 @@ class Model:
                                          0 if cl is None else cl.size, None if vl is None else _ptr(vl),
                                          sum_sq.ctypes.data_as(_f64p), total.ctypes.data_as(_f64p), C.byref(w_sum), dp))
         return {"sum_sq": sum_sq, "sum": total, "w_sum": float(w_sum.value), "deltas": d_out}
+
+    def reason_codes(self, X, k, cols=None, values=None, order="raise", scores=False, pos=None, d=None) -> dict:
+        """Per-row reason codes (sb_model_reason_codes): for each row, the k list positions whose deltas
+        d = s(X[r]) - s(X[r] with column cols[j] set to values[j]) rank first in `order` ("raise": largest d first,
+        "lower": smallest d first, "magnitude": largest |d| first; NaN last, ties to the smaller position).
+        -> {"pos": int32 [rows, k], "d": their deltas float32 [rows, k], "scores": the base scores [rows] or None}.
+        X: a numpy array (host) or a CUDA tensor / DeviceArray on the model's device.  cols / values as in sensitivity.
+        pos / d: None (returned as host arrays) or a buffer of rows * k int32 / float32 to write into; scores: False (not
+        computed), True (a host array) or a buffer of rows floats."""
+        xp, shape = _in_ptr(X)
+        if len(shape) != 2 or shape[1] != self.n_features:
+            raise ValueError("X must be [rows, %d]" % self.n_features)
+        rows = int(shape[0])
+        cl = None if cols is None else np.ascontiguousarray(cols, dtype=np.int32).reshape(-1)
+        n_cols = self.n_features if cl is None else cl.size
+        vl = None if values is None else _f32(values).reshape(-1)
+        if vl is not None and vl.size != n_cols:
+            raise ValueError("values must hold one value per list position (%d)" % n_cols)
+        if order not in REASON_ORDERS:
+            raise ValueError("order must be one of %s" % sorted(REASON_ORDERS))
+
+        def out(buf, dtype, shape):
+            if buf is None or buf is True:
+                a = np.empty(shape, dtype)
+                return a, a.ctypes.data_as(_vp)
+            return buf, _in_ptr(buf, dtype)[0]
+
+        p_out, pp = out(pos, np.int32, (rows, k))
+        d_out, dp = out(d, np.float32, (rows, k))
+        s_out, sp = out(scores, np.float32, (rows,)) if scores is not False and scores is not None else (None, None)
+        check(lib().sb_model_reason_codes(self._h, xp, rows, None if cl is None else cl.ctypes.data_as(_P(C.c_int32)),
+                                          0 if cl is None else cl.size, None if vl is None else _ptr(vl), int(k),
+                                          REASON_ORDERS[order], pp, dp, sp))
+        return {"pos": p_out, "d": d_out, "scores": s_out}
 
     def sync(self):
         check(lib().sb_model_sync(self._h))

@@ -1923,6 +1923,10 @@ struct sb_model {
   DevBuf<float> sens_vals;
   DevBuf<float> sens_d;       // the deltas of one piece [R, piece columns] (max_batch)
   size_t sens_z_n = 0, sens_list_n = 0;
+  // sb_model_reason_codes' running top k of a row chunk [R, k], best first (guarded by mu; allocated and grown as above)
+  DevBuf<float> reason_d;
+  DevBuf<int> reason_pos;
+  size_t reason_d_n = 0, reason_pos_n = 0;
   ~sb_model() {
     if (!net.stream) return;
     cudaSetDevice(net.device);
@@ -2181,24 +2185,27 @@ static int sens_chunk_rows(int max_batch, int C) {
   return static_cast<int>(r > 0 ? r : 1);
 }
 
-static int sens_grow(DevBuf<float>* b, size_t* cap, size_t n) {
+template <typename T>
+static int sens_grow(DevBuf<T>* b, size_t* cap, size_t n) {
   if (n <= *cap) return SB_OK;
-  *b = DevBuf<float>();
+  *b = DevBuf<T>();
   SB_TRY(b->alloc(n));
   *cap = n;
   return SB_OK;
 }
 
-// Column sensitivity (sensitivity.cuh, DESIGN §6f), called with m->mu held.  Rows go in row chunks of R rows
+// Column sensitivity's pieces (sensitivity.cuh, DESIGN §6f), called with m->mu held.  Rows go in row chunks of R rows
 // (sens_chunk_rows); a row chunk's z0 is computed once, and its list positions go in pieces of up to max_batch / R - 1
-// columns, each piece one forward of R (columns + 1) pair rows through layers 1..L and the output unit.
-static int sens_forward(sb_model* m, const float* X, const float* w, int64_t rows, int C, float* deltas) {
+// columns, each piece one forward of R (columns + 1) pair rows through layers 1..L and the output unit.  After each
+// forward, piece(r0, rc, k0, ck, wd) consumes the piece's pair scores in n.yhat (pair p = slot * rc + r; wd: the chunk's
+// weights): sb_model_sensitivity's sums and deltas, or sb_model_reason_codes' top-k merge.
+template <typename Piece>
+static int sens_forward(sb_model* m, const float* X, const float* w, int64_t rows, int C, const Piece& piece) {
   Net& n = m->net;
   const Layer& l0 = n.layers[0];
   const int R = sens_chunk_rows(n.max_batch, C);
   const int Cp = n.max_batch / R - 1;
   SB_TRY(sens_grow(&m->sens_z, &m->sens_z_n, static_cast<size_t>(R) * l0.ld_out));
-  if (!m->sens_d.p) SB_TRY(m->sens_d.alloc(static_cast<size_t>(n.max_batch)));
   const StepIn in{n.desc, n.scal};
   SensParams sp = {};
   sp.F = n.F; sp.N = l0.out; sp.ld = l0.ld_out;
@@ -2244,44 +2251,34 @@ static int sens_forward(sb_model* m, const float* X, const float* w, int64_t row
       n.mark(perturb_name);
       SB_TRY(n.enqueue_hidden_forward(in, pairs, nullptr, nullptr, nullptr, 0, 1));
       SB_TRY(n.enqueue_out(in, pairs, false, false, n.yhat, nullptr));
-      SB_TRY(launch_kernel(sens_reduce_kernel, dim3(static_cast<unsigned>(ck + 1)), dim3(SENS_REDUCE_THREADS), 0, n.stream, false,
-                           static_cast<const float*>(n.yhat), wd, rc, ck, k0, deltas ? m->sens_d.p : nullptr, ck, m->sens_acc.p,
-                           k0 == 0 ? 1 : 0, 2LL * C));
-      n.mark("sens_reduce");
-      if (deltas)
-        SB_CUDA(cudaMemcpy2DAsync(deltas + r0 * C + k0, sizeof(float) * C, m->sens_d.p, sizeof(float) * ck, sizeof(float) * ck, rc,
-                                  cudaMemcpyDefault, n.stream));
+      SB_TRY(piece(r0, rc, k0, ck, wd));
     }
   }
   return SB_OK;
 }
 
-extern "C" {
-
-int sb_model_sensitivity(sb_model_t* m, const float* X, const float* w, int64_t rows, const int32_t* cols, int32_t n_cols,
-                         const float* values, double* sum_sq, double* sum, double* w_sum, float* deltas) {
-  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
-  SB_CHECK(X && sum_sq && sum && w_sum, SB_ERR_INVALID, "null argument");
-  SB_CHECK(rows >= 0, SB_ERR_INVALID, "rows = %lld < 0", static_cast<long long>(rows));
+// cols / n_cols / values as sb_model_sensitivity takes them -> the column list and its values (cl, vl)
+static int sens_list(const Net& n, const int32_t* cols, int32_t n_cols, const float* values, std::vector<int32_t>* cl,
+                     std::vector<float>* vl) {
   SB_CHECK((cols == nullptr && n_cols == 0) || (cols != nullptr && n_cols >= 1), SB_ERR_INVALID,
            "cols / n_cols: a list of n_cols >= 1 columns, or NULL and 0 for every column (got %s and %d)", cols ? "a list" : "NULL",
            n_cols);
-  Net& n = m->net;
   const int C = cols ? n_cols : n.F;
-  std::vector<int32_t> cl(static_cast<size_t>(C));
-  std::vector<float> vl(static_cast<size_t>(C));
+  cl->resize(static_cast<size_t>(C));
+  vl->resize(static_cast<size_t>(C));
   for (int k = 0; k < C; ++k) {
-    cl[k] = cols ? cols[k] : k;
-    SB_CHECK(cl[k] >= 0 && cl[k] < n.F, SB_ERR_INVALID, "cols[%d] = %d outside [0, %d)", k, cl[k], n.F);
-    vl[k] = values ? values[k] : 0.f;
-    SB_CHECK(std::isfinite(vl[k]), SB_ERR_INVALID, "values[%d] = %g is not finite", k, static_cast<double>(vl[k]));
+    (*cl)[k] = cols ? cols[k] : k;
+    SB_CHECK((*cl)[k] >= 0 && (*cl)[k] < n.F, SB_ERR_INVALID, "cols[%d] = %d outside [0, %d)", k, (*cl)[k], n.F);
+    (*vl)[k] = values ? values[k] : 0.f;
+    SB_CHECK(std::isfinite((*vl)[k]), SB_ERR_INVALID, "values[%d] = %g is not finite", k, static_cast<double>((*vl)[k]));
   }
-  for (int k = 0; k < C; ++k) sum_sq[k] = sum[k] = 0.0;
-  *w_sum = 0.0;
-  if (rows == 0) return SB_OK;
-  std::lock_guard<std::mutex> lk(m->mu);
-  SB_CUDA(cudaSetDevice(n.device));
-  const size_t list_n = static_cast<size_t>(C);
+  return SB_OK;
+}
+
+// the column list and its values to the device (with m->mu held); the running sums are sized with them
+static int sens_upload_list(sb_model* m, const std::vector<int32_t>& cl, const std::vector<float>& vl) {
+  Net& n = m->net;
+  const size_t list_n = cl.size();
   if (list_n > m->sens_list_n) {
     m->sens_acc = DevBuf<double>(); m->sens_cols = DevBuf<int>(); m->sens_vals = DevBuf<float>();
     m->sens_list_n = 0;
@@ -2292,9 +2289,43 @@ int sb_model_sensitivity(sb_model_t* m, const float* X, const float* w, int64_t 
   }
   SB_CUDA(cudaMemcpyAsync(m->sens_cols.p, cl.data(), sizeof(int32_t) * list_n, cudaMemcpyHostToDevice, n.stream));
   SB_CUDA(cudaMemcpyAsync(m->sens_vals.p, vl.data(), sizeof(float) * list_n, cudaMemcpyHostToDevice, n.stream));
+  return SB_OK;
+}
+
+extern "C" {
+
+int sb_model_sensitivity(sb_model_t* m, const float* X, const float* w, int64_t rows, const int32_t* cols, int32_t n_cols,
+                         const float* values, double* sum_sq, double* sum, double* w_sum, float* deltas) {
+  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
+  SB_CHECK(X && sum_sq && sum && w_sum, SB_ERR_INVALID, "null argument");
+  SB_CHECK(rows >= 0, SB_ERR_INVALID, "rows = %lld < 0", static_cast<long long>(rows));
+  Net& n = m->net;
+  std::vector<int32_t> cl;
+  std::vector<float> vl;
+  SB_TRY(sens_list(n, cols, n_cols, values, &cl, &vl));
+  const int C = static_cast<int>(cl.size());
+  for (int k = 0; k < C; ++k) sum_sq[k] = sum[k] = 0.0;
+  *w_sum = 0.0;
+  if (rows == 0) return SB_OK;
+  std::lock_guard<std::mutex> lk(m->mu);
+  SB_CUDA(cudaSetDevice(n.device));
+  const size_t list_n = static_cast<size_t>(C);
+  SB_TRY(sens_upload_list(m, cl, vl));
   SB_CUDA(cudaMemsetAsync(m->sens_acc.p, 0, sizeof(double) * (2 * list_n + 1), n.stream));
+  if (!m->sens_d.p) SB_TRY(m->sens_d.alloc(static_cast<size_t>(n.max_batch)));
+  // per piece: d and the sums (sens_reduce_kernel), and the piece's deltas copied out when asked
+  const auto reduce = [&](int64_t r0, int rc, int k0, int ck, const float* wd) -> int {
+    SB_TRY(launch_kernel(sens_reduce_kernel, dim3(static_cast<unsigned>(ck + 1)), dim3(SENS_REDUCE_THREADS), 0, n.stream, false,
+                         static_cast<const float*>(n.yhat), wd, rc, ck, k0, deltas ? m->sens_d.p : nullptr, ck, m->sens_acc.p,
+                         k0 == 0 ? 1 : 0, 2LL * C));
+    n.mark("sens_reduce");
+    if (deltas)
+      SB_CUDA(cudaMemcpy2DAsync(deltas + r0 * C + k0, sizeof(float) * C, m->sens_d.p, sizeof(float) * ck, sizeof(float) * ck, rc,
+                                cudaMemcpyDefault, n.stream));
+    return SB_OK;
+  };
   n.marks = &m->routes;
-  const int s = sens_forward(m, X, w, rows, C, deltas);
+  const int s = sens_forward(m, X, w, rows, C, reduce);
   n.marks = nullptr;
   SB_TRY(s);
   std::vector<double> acc(2 * list_n + 1);
@@ -2302,6 +2333,50 @@ int sb_model_sensitivity(sb_model_t* m, const float* X, const float* w, int64_t 
   SB_CUDA(cudaStreamSynchronize(n.stream));
   for (int k = 0; k < C; ++k) { sum_sq[k] = acc[2 * k]; sum[k] = acc[2 * k + 1]; }
   *w_sum = acc[2 * list_n];
+  return SB_OK;
+}
+
+int sb_model_reason_codes(sb_model_t* m, const float* X, int64_t rows, const int32_t* cols, int32_t n_cols, const float* values,
+                          int32_t k, int32_t order, int32_t* pos, float* d, float* scores) {
+  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
+  SB_CHECK(X && pos && d, SB_ERR_INVALID, "null argument");
+  SB_CHECK(rows >= 0, SB_ERR_INVALID, "rows = %lld < 0", static_cast<long long>(rows));
+  Net& n = m->net;
+  std::vector<int32_t> cl;
+  std::vector<float> vl;
+  SB_TRY(sens_list(n, cols, n_cols, values, &cl, &vl));
+  const int C = static_cast<int>(cl.size());
+  SB_CHECK(k >= 1 && k <= C && k <= SENS_TOPK_MAX_K, SB_ERR_INVALID, "k = %d outside [1, min(%d list positions, %d)]", k, C,
+           SENS_TOPK_MAX_K);
+  SB_CHECK(order == SB_REASON_RAISE || order == SB_REASON_LOWER || order == SB_REASON_MAGNITUDE, SB_ERR_INVALID,
+           "order = %d is not SB_REASON_RAISE, SB_REASON_LOWER or SB_REASON_MAGNITUDE", order);
+  if (rows == 0) return SB_OK;
+  std::lock_guard<std::mutex> lk(m->mu);
+  SB_CUDA(cudaSetDevice(n.device));
+  SB_TRY(sens_upload_list(m, cl, vl));
+  const size_t run_n = static_cast<size_t>(sens_chunk_rows(n.max_batch, C)) * k;
+  SB_TRY(sens_grow(&m->reason_d, &m->reason_d_n, run_n));
+  SB_TRY(sens_grow(&m->reason_pos, &m->reason_pos_n, run_n));
+  // per piece: merge its deltas into each row's running top k (reset by the chunk's first piece); after the chunk's last
+  // piece, copy the chunk's top k and base scores out
+  const auto merge = [&](int64_t r0, int rc, int k0, int ck, const float*) -> int {
+    const unsigned warps = static_cast<unsigned>(std::min((ck + 31) / 32, SENS_TOPK_WARPS));
+    SB_TRY(launch_kernel(sens_topk_kernel, dim3(static_cast<unsigned>(rc)), dim3(32, warps), 0, n.stream, false,
+                         static_cast<const float*>(n.yhat), rc, ck, k0, static_cast<int>(k), static_cast<int>(order), k0 == 0 ? 1 : 0,
+                         m->reason_d.p, m->reason_pos.p));
+    n.mark("sens_topk");
+    if (k0 + ck < C) return SB_OK;
+    const size_t out_n = static_cast<size_t>(rc) * k;
+    SB_CUDA(cudaMemcpyAsync(pos + r0 * k, m->reason_pos.p, sizeof(int32_t) * out_n, cudaMemcpyDefault, n.stream));
+    SB_CUDA(cudaMemcpyAsync(d + r0 * k, m->reason_d.p, sizeof(float) * out_n, cudaMemcpyDefault, n.stream));
+    if (scores) SB_CUDA(cudaMemcpyAsync(scores + r0, n.yhat, sizeof(float) * rc, cudaMemcpyDefault, n.stream));
+    return SB_OK;
+  };
+  n.marks = &m->routes;
+  const int s = sens_forward(m, X, nullptr, rows, C, merge);
+  n.marks = nullptr;
+  SB_TRY(s);
+  SB_CUDA(cudaStreamSynchronize(n.stream));
   return SB_OK;
 }
 

@@ -8,6 +8,7 @@
 // as the perturbed scores, so a pair whose column already holds the value gets exactly the base row's score.
 //   sens_perturb_kernel  z0 (fp32, [R, ld_z]) -> A0' of every pair, stored as layer 0's forward epilogue stores A0
 //   sens_reduce_kernel   the pair scores -> d = s(base) - s(pair) per (row, column), and the fp64 sums of w d^2 and w d
+//   sens_topk_kernel     the pair scores -> each row's running top k of d (sb_model_reason_codes, DESIGN §6g)
 #pragma once
 #include "common.cuh"
 #include "kernels.cuh"
@@ -186,6 +187,93 @@ sens_reduce_kernel(const float* __restrict__ yhat, const float* __restrict__ w, 
     } else {
       acc[w_slot] += s1[0];
     }
+  }
+}
+
+constexpr int SENS_TOPK_MAX_K = 32;      // one running entry per lane
+constexpr int SENS_TOPK_WARPS = 8;       // most warps per row
+
+// The reason-code order as one unsigned 64-bit key, larger = ranks first: the high word maps the float key (d, -d or
+// |d| for SB_REASON_RAISE / LOWER / MAGNITUDE) to an order-preserving integer with -0 made +0 and NaN below -inf; the
+// low word is ~pos, so equal keys rank by the smaller list position.  Every entry is > 0; 0 is an empty slot.
+__device__ __forceinline__ unsigned long long topk_key(float d, int order, int pos) {
+  const float f = order == SB_REASON_RAISE ? d : order == SB_REASON_LOWER ? -d : fabsf(d);
+  unsigned u = __float_as_uint(f);
+  if ((u << 1) == 0u) u = 0u;                                   // -0 -> +0
+  u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+  if (f != f) u = 0u;
+  return (static_cast<unsigned long long>(u) << 32) | (0xFFFFFFFFu - static_cast<unsigned>(pos));
+}
+
+// one compare-exchange of a warp bitonic network with the lane `lane ^ s`: this lane keeps the larger (key, d) entry when
+// keep_max, else the smaller.  Keys are distinct unless both are empty.
+__device__ __forceinline__ void topk_cx(unsigned long long& key, float& d, int s, bool keep_max) {
+  const unsigned long long pk = __shfl_xor_sync(0xFFFFFFFFu, key, s);
+  const float pd = __shfl_xor_sync(0xFFFFFFFFu, d, s);
+  if (keep_max ? pk > key : pk < key) { key = pk; d = pd; }
+}
+
+// a bitonic sequence over the warp's lanes -> sorted, largest key in lane 0
+__device__ __forceinline__ void topk_bitonic_merge(unsigned long long& key, float& d, int lane) {
+#pragma unroll
+  for (int s = 16; s > 0; s >>= 1) topk_cx(key, d, s, (lane & s) == 0);
+}
+
+// `key` (sorted, lane 0 first) := the 32 largest of itself and the sorted list `ok` / `od` (lane 0 first), sorted
+__device__ __forceinline__ void topk_merge(unsigned long long& key, float& d, unsigned long long ok, float od, int lane) {
+  ok = __shfl_sync(0xFFFFFFFFu, ok, 31 - lane);                 // ascending: max(key[i], ok[31 - i]) is bitonic and holds
+  od = __shfl_sync(0xFFFFFFFFu, od, 31 - lane);                 // the 32 largest of the union
+  if (ok > key) { key = ok; d = od; }
+  topk_bitonic_merge(key, d, lane);
+}
+
+// grid (R), block (32, W), W <= SENS_TOPK_WARPS: block r merges the piece's C deltas d = yhat[r] - yhat[(j + 1) R + r]
+// (j < C, list position k0 + j; the fp32 expression of sens_reduce_kernel) into row r's running top k, run_d / run_pos
+// [R, k] sorted best first (first: the running list starts empty).  Warp w takes columns w * 32 + lane, w * 32 + 32 W +
+// lane, ...; a batch of 32 whose best key does not beat the warp's k-th is skipped, otherwise it is sorted by a warp
+// bitonic network and merged into the warp's list.  Warp 0 then merges the other warps' lists from shared memory.  The
+// order is total and each merge keeps the k best of the union, so the result does not depend on the piece boundaries or
+// on the order the columns are taken in.
+__global__ void __launch_bounds__(32 * SENS_TOPK_WARPS)
+sens_topk_kernel(const float* __restrict__ yhat, int R, int C, int k0, int k, int order, int first, float* __restrict__ run_d,
+                 int* __restrict__ run_pos) {
+  __shared__ unsigned long long s_key[SENS_TOPK_WARPS][32];
+  __shared__ float s_d[SENS_TOPK_WARPS][32];
+  const int r = blockIdx.x, lane = threadIdx.x, wp = threadIdx.y, W = blockDim.y;
+  const size_t o = static_cast<size_t>(r) * k + lane;
+  unsigned long long key = 0;
+  float d = 0.f;
+  if (wp == 0 && !first && lane < k) {
+    d = run_d[o];
+    key = topk_key(d, order, run_pos[o]);
+  }
+  const float base = yhat[r];
+  for (int j0 = wp * 32; j0 < C; j0 += 32 * W) {
+    const int j = j0 + lane;
+    unsigned long long ck = 0;
+    float cd = 0.f;
+    if (j < C) {
+      cd = base - yhat[static_cast<size_t>(j + 1) * R + r];
+      ck = topk_key(cd, order, k0 + j);
+    }
+    const unsigned long long kth = __shfl_sync(0xFFFFFFFFu, key, k - 1);
+    if (!__any_sync(0xFFFFFFFFu, ck > kth)) continue;
+#pragma unroll
+    for (int size = 2; size <= 32; size <<= 1)                  // sort the batch, largest key in lane 0
+#pragma unroll
+      for (int s = size / 2; s > 0; s >>= 1) topk_cx(ck, cd, s, ((lane & s) == 0) == ((lane & size) == 0));
+    topk_merge(key, d, ck, cd, lane);
+  }
+  if (W > 1) {
+    s_key[wp][lane] = key;
+    s_d[wp][lane] = d;
+    __syncthreads();
+    if (wp != 0) return;
+    for (int v = 1; v < W; ++v) topk_merge(key, d, s_key[v][lane], s_d[v][lane], lane);
+  }
+  if (lane < k) {
+    run_d[o] = d;
+    run_pos[o] = static_cast<int>(0xFFFFFFFFu - static_cast<unsigned>(key));
   }
 }
 

@@ -124,6 +124,20 @@ class TensorflowModel:
             mse, mean = r["sum_sq"] / ws, r["sum"] / ws
         return {"sum_sq": r["sum_sq"], "sum": r["sum"], "w_sum": ws, "mse": mse, "mean": mean}
 
+    # -- new: per-row reason codes: the columns whose replacement moves each row's score the most --
+    def computeReasonCodes(self, rows, k, columns=None, values=None, order="raise") -> dict:
+        """-> {"columns": int32 [rows, k] the k columns that rank first per row, "deltas": their d = compute(row) -
+        compute(row with the column set to its value), "scores": compute(row) as the call computes it}; order "raise"
+        (largest d first: the values that push the score up the most), "lower" or "magnitude"; columns None: every
+        column; values None: 0 per column (the mean of a ZSCALE-normalised column)"""
+        if not self.initiate or self._model is None:
+            raise IllegalStateException("TF model not initialized.")
+        X = np.asarray(rows, dtype=np.float64).astype(np.float32)     # the same double -> float cast as computeBatch
+        vals = None if values is None else np.asarray(values, dtype=np.float64).astype(np.float32)
+        cl = np.arange(X.shape[1], dtype=np.int32) if columns is None else np.asarray(columns, dtype=np.int32).reshape(-1)
+        r = self._model.reason_codes(X, k, cols=columns, values=vals, order=order, scores=True)
+        return {"columns": cl[r["pos"]], "deltas": r["d"], "scores": r["scores"]}
+
     def releaseResource(self) -> None:
         """The reference never closes its bundle (TensorflowModel.java:175-176); here device memory is returned."""
         if self._model is not None:
