@@ -364,6 +364,58 @@ int sb_debug_model_hold(sb_model_t* m, int32_t k, int32_t timeout_ms);
  * "load_batch<bf16>+gemm_tc<128,F32>+sens_perturb<bf16>+gemm_pp<FWD>+gemm_pp<FWD>+out_layer_rows<1>+sens_reduce".
  * After sb_model_reason_codes: the same, ending in "sens_topk" instead of "sens_reduce". */
 int sb_debug_model_routes(sb_model_t* m, char* out, int32_t cap);
+/* the device bytes the model allocated for its network, workspace and staging (a test hook) */
+int sb_debug_model_bytes(sb_model_t* m, int64_t* out);
+
+/* ---- bagged models: Shifu trains train.baggingNum models per run (models/model0 .. model{K-1}) and `shifu eval` scores
+ * every one of them per row and reports their mean, max, min and median beside the members' scores.  An ensemble is K
+ * member models on one device and one stream that share one staged copy of the rows: each chunk of rows is copied in and
+ * converted to the GEMM operand (load_batch_kernel) once, and every member's forward reads it.
+ * Members must share n_features and precision; their hidden widths, depths and activations may differ.  Each member
+ * scores each chunk with its own launches at its own max_batch, the one sb_model_score uses at that precision, and the
+ * ensemble chunks rows at that size, so member g's scores are bit-identical to what an sb_model_t of the same member
+ * computes from the same rows through sb_model_score / sb_model_score_device.
+ * The statistics, per row, over the K member scores s_0 .. s_{K-1}:
+ *   mean    ((s_0 + s_1) + ...) + s_{K-1} summed in fp32 in member order, then divided by (float)K
+ *   max     the largest value (of equal values, the first in member order); min likewise
+ *   median  with the values sorted (equal values in member order): K odd the middle value; K even (a + b) / 2 in fp32 of
+ *           the two middle values a <= b.  The reference scorer's sources are not part of this project, so this even-K
+ *           convention is defined here, not taken from Shifu.
+ *   If any member's score is NaN, all four statistics are the quiet NaN 0x7fc00000.
+ * Errors, all found before any device work: k < 1 or k > SB_ENSEMBLE_MAX, a null argument, members whose n_features
+ * differ, descriptors whose precision differs, a parameter count that does not fit its descriptor, both outputs null,
+ * rows < 0, or a row length != n_features in sb_ensemble_score_row_f64 are SB_ERR_INVALID; a null handle SB_ERR_STATE;
+ * sb_ensemble_load reports a member's load errors exactly as sb_model_load does.  rows = 0 returns SB_OK and writes
+ * nothing. ---- */
+#define SB_ENSEMBLE_MAX 32
+typedef struct sb_ensemble sb_ensemble_t;
+/* K SavedModel directories, each loaded as sb_model_load loads one (SavedModelBundle.load per models/model<g>), every
+ * member at `precision` */
+int sb_ensemble_load(const char* const* dirs, int32_t k, const char* input_name, const char* output_name, const char* tag,
+                     int device, int precision, sb_ensemble_t** out);
+/* K topologies + flat parameter vectors, each as sb_model_create takes one */
+int sb_ensemble_create(const sb_net_desc* descs, const float* const* flats, const int64_t* n_params, int32_t k, int device,
+                       sb_ensemble_t** out);
+int sb_ensemble_destroy(sb_ensemble_t* e);
+int32_t sb_ensemble_size(const sb_ensemble_t* e);
+/* K compute() calls per row plus the statistics: X [rows, n_features] fp32, host or device; scores [rows, k] (member
+ * order) and stats [rows, 4] = {mean, max, min, median}, host or device; either output may be NULL, not both.
+ * Synchronous, like sb_model_score. */
+int sb_ensemble_score(sb_ensemble_t* e, const float* X, int64_t rows, float* scores, float* stats);
+/* the same with DEVICE pointers, asynchronous on the ensemble's stream, like sb_model_score_device; sb_ensemble_sync waits */
+int sb_ensemble_score_device(sb_ensemble_t* e, const float* dX, int64_t rows, float* dScores, float* dStats);
+/* compute(MLData) of every member: one row of doubles -> out[k + 4] doubles (the k member scores, then mean, max, min,
+ * median).  Concurrent calls on one handle share device batches of up to 128 rows, as sb_model_score_row_f64's do; a
+ * lone call is scored at once. */
+int sb_ensemble_score_row_f64(sb_ensemble_t* e, const double* row, int32_t n, double* out);
+int sb_ensemble_sync(sb_ensemble_t* e);
+void* sb_ensemble_stream(sb_ensemble_t* e);
+/* Test hooks.  routes: the launches of the ensemble's last chunk, "+"-joined, e.g. for two bf16 members
+ * "load_batch<bf16>+gemm_wide+gemm_pp<FWD>+out_layer_rows<1>+gemm_pp<FWD>+out_layer_rows<1>+ensemble_stats", for an
+ * fp32 chunk of up to 128 rows "score_rows+score_rows+ensemble_stats"; "none" before the first.  bytes: the device bytes
+ * the ensemble allocated (every member's network and workspace, the one input staging, the member score slots). */
+int sb_debug_ensemble_routes(sb_ensemble_t* e, char* out, int32_t cap);
+int sb_debug_ensemble_bytes(sb_ensemble_t* e, int64_t* out);
 
 /* ---- text ingest: the per-cell float() loop of load_data (ssgd_monitor.py:387-419) on the GPU ----
  * text: the gunzipped, delim-separated lines (must end with '\n'), HOST memory.  col_map[c] gives the role of text

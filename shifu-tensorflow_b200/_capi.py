@@ -159,6 +159,18 @@ PROTOTYPES = {
     "sb_debug_model_batch_stats": (C.c_int, [_vp, _P(C.c_int64), C.c_int32]),
     "sb_debug_model_hold": (C.c_int, [_vp, C.c_int32, C.c_int32]),
     "sb_debug_model_routes": (C.c_int, [_vp, C.c_char_p, C.c_int32]),
+    "sb_debug_model_bytes": (C.c_int, [_vp, _P(C.c_int64)]),
+    "sb_ensemble_load": (C.c_int, [_P(_cp), C.c_int32, _cp, _cp, _cp, C.c_int, C.c_int, _P(_vp)]),
+    "sb_ensemble_create": (C.c_int, [_P(NetDesc), _P(_f32p), _P(C.c_int64), C.c_int32, C.c_int, _P(_vp)]),
+    "sb_ensemble_destroy": (C.c_int, [_vp]),
+    "sb_ensemble_size": (C.c_int32, [_vp]),
+    "sb_ensemble_score": (C.c_int, [_vp, _vp, C.c_int64, _vp, _vp]),
+    "sb_ensemble_score_device": (C.c_int, [_vp, _vp, C.c_int64, _vp, _vp]),
+    "sb_ensemble_score_row_f64": (C.c_int, [_vp, _f64p, C.c_int32, _f64p]),
+    "sb_ensemble_sync": (C.c_int, [_vp]),
+    "sb_ensemble_stream": (C.c_void_p, [_vp]),
+    "sb_debug_ensemble_routes": (C.c_int, [_vp, C.c_char_p, C.c_int32]),
+    "sb_debug_ensemble_bytes": (C.c_int, [_vp, _P(C.c_int64)]),
     "sb_text_parse": (C.c_int, [_cp, C.c_int64, C.c_char, _P(C.c_int32), C.c_int32, C.c_int32, _f32p, _f32p, _f32p, C.c_int64,
                                 _P(C.c_int64), _P(CellFlag), C.c_int64, _P(C.c_int64), C.c_int]),
     "sb_text_parse_device": (C.c_int, [_cp, C.c_int64, C.c_char, _P(C.c_int32), C.c_int32, C.c_int32, _P(_f32p), _P(_f32p), _P(_f32p),
@@ -209,6 +221,8 @@ DEBUG_BUF_DS_X, DEBUG_BUF_DS_Y, DEBUG_BUF_DS_W, DEBUG_BUF_DS_P = (DEBUG_BUF_BATC
 SCAL_LOSS_SUM, SCAL_NNZ, SCAL_COUNT = 0, 1, 4
 DEBUG_XINFO_WORDS, DEBUG_XWORK_WORDS = 24, 8
 DEBUG_MSTAT_WORDS = 6
+ENSEMBLE_MAX = 32       # SB_ENSEMBLE_MAX: members of one ensemble
+ENSEMBLE_STATS = ("mean", "max", "min", "median")     # sb_ensemble_score's stats columns
 SMALL_ROWS = 128        # score_rows.cuh: an fp32 model scores batches of up to this many rows in one launch
 # capi.cu model_from_desc: a model runs every scoring call in forwards of at most this many rows (its max_batch)
 MODEL_CHUNK_ROWS = {PREC_FP32: 16384, PREC_BF16: 65536, PREC_FP32_TC: 32768, PREC_BF16X2: 32768}
@@ -817,6 +831,106 @@ class Model:
         buf = C.create_string_buffer(256)
         check(lib().sb_debug_model_routes(self._h, buf, len(buf)))
         return buf.value.decode()
+
+    def device_bytes(self) -> int:
+        """the device bytes the model allocated (sb_debug_model_bytes)"""
+        out = C.c_int64()
+        check(lib().sb_debug_model_bytes(self._h, C.byref(out)))
+        return int(out.value)
+
+
+class Ensemble:
+    """Owns one sb_ensemble_t: K bagged member models scored from one staged copy of the rows, with each row's mean,
+    max, min and median of the member scores formed on the GPU."""
+
+    def __init__(self, handle, n_features: int):
+        self._h = handle
+        self.n_features = int(n_features)
+        self.k = int(lib().sb_ensemble_size(self._h))
+
+    @classmethod
+    def load(cls, saved_model_dirs: Sequence[str], input_name: str, output_name: str, tag: str = "serve", device: int = 0,
+             precision: int = PREC_FP32) -> "Ensemble":
+        enc = lambda s: None if s is None else s.encode()
+        dirs = (_cp * max(len(saved_model_dirs), 1))(*[enc(d) for d in saved_model_dirs])
+        h = C.c_void_p()
+        check(lib().sb_ensemble_load(dirs, len(saved_model_dirs), enc(input_name), enc(output_name), enc(tag), device,
+                                     precision, C.byref(h)))
+        e = cls(h, 0)
+        e.n_features = savedmodel_read(saved_model_dirs[0], input_name, output_name, tag)[0]
+        return e
+
+    @classmethod
+    def create(cls, descs: Sequence[NetDesc], flats, device: int = 0) -> "Ensemble":
+        k = len(descs)
+        flats = [_f32(f).reshape(-1) for f in flats]
+        if len(flats) != k:
+            raise ValueError("one flat parameter vector per descriptor")
+        d_arr = (NetDesc * max(k, 1))(*descs)
+        f_arr = (_f32p * max(k, 1))(*[_ptr(f) for f in flats])
+        n_arr = (C.c_int64 * max(k, 1))(*[f.size for f in flats])
+        h = C.c_void_p()
+        check(lib().sb_ensemble_create(d_arr, f_arr, n_arr, k, device, C.byref(h)))
+        return cls(h, descs[0].n_features)
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and self._h:
+            lib().sb_ensemble_destroy(self._h)
+            self._h = None
+
+    __del__ = close
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def score(self, X, scores: bool = True, stats: bool = True):
+        """-> (scores [rows, k] in member order or None, stats [rows, 4] = mean, max, min, median or None).  X: a numpy
+        array (host) or a CUDA tensor / DeviceArray on the ensemble's device."""
+        if isinstance(X, np.ndarray) or not (hasattr(X, "data_ptr") or isinstance(X, DeviceArray)):
+            X = _f32(X)
+        xp, shape = _in_ptr(X)
+        if len(shape) != 2 or shape[1] != self.n_features:
+            raise ValueError("X must be [rows, %d]" % self.n_features)
+        rows = int(shape[0])
+        s = np.empty((rows, self.k), np.float32) if scores else None
+        t = np.empty((rows, 4), np.float32) if stats else None
+        check(lib().sb_ensemble_score(self._h, xp, rows, None if s is None else s.ctypes.data_as(_vp),
+                                      None if t is None else t.ctypes.data_as(_vp)))
+        return s, t
+
+    def score_device(self, dX_ptr: int, rows: int, dScores_ptr: Optional[int], dStats_ptr: Optional[int]):
+        """device pointers, asynchronous on the ensemble's stream (sync() waits); either output pointer may be None"""
+        check(lib().sb_ensemble_score_device(self._h, C.c_void_p(dX_ptr), rows, C.c_void_p(dScores_ptr) if dScores_ptr else None,
+                                             C.c_void_p(dStats_ptr) if dStats_ptr else None))
+
+    def score_row_f64(self, row) -> np.ndarray:
+        """compute() of every member: -> float64 [k + 4] (the k member scores, then mean, max, min, median)"""
+        row = np.ascontiguousarray(row, dtype=np.float64).reshape(-1)
+        out = np.empty(self.k + 4, np.float64)
+        check(lib().sb_ensemble_score_row_f64(self._h, row.ctypes.data_as(_f64p), row.size, out.ctypes.data_as(_f64p)))
+        return out
+
+    def sync(self):
+        check(lib().sb_ensemble_sync(self._h))
+
+    @property
+    def stream(self) -> int:
+        return int(lib().sb_ensemble_stream(self._h) or 0)
+
+    def routes(self) -> str:
+        """the kernels of the last chunk, "+"-joined (sb_debug_ensemble_routes)"""
+        buf = C.create_string_buffer(16384)
+        check(lib().sb_debug_ensemble_routes(self._h, buf, len(buf)))
+        return buf.value.decode()
+
+    def device_bytes(self) -> int:
+        """the device bytes the ensemble allocated (sb_debug_ensemble_bytes)"""
+        out = C.c_int64()
+        check(lib().sb_debug_ensemble_bytes(self._h, C.byref(out)))
+        return int(out.value)
 
 
 def nccl_unique_id() -> bytes:

@@ -9,8 +9,10 @@
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
+#include <functional>
 #include <memory>
 #include <random>
+#include "ensemble.cuh"
 #include "net.cuh"
 #include "savedmodel.h"
 #include "score_rows.cuh"
@@ -1889,10 +1891,108 @@ static const int MB_ROWS = 128;
 static_assert(SMALL_ROWS >= MB_ROWS, "an fp32 micro-batch is one score_rows_kernel launch");
 
 struct RowWaiter {            // one compute() call, on its caller's stack
-  float value = 0.f;
+  float* out = nullptr;       // its result, RowQueue::words floats
   int status = SB_OK;
   std::string err;            // the leader's error text, re-raised in the caller's thread
   bool done = false;
+};
+
+// The compute() queue of a model (one score per row) or an ensemble (K scores and four statistics per row): concurrent
+// callers on one handle share device batches of up to MB_ROWS rows.  No thread of its own: the first caller that finds
+// no batch in flight leads, running every queued row in batches until the queue is empty; the others wait for their
+// result.  A batch is run by the owner's run(b, rows): the rows of stage[b] -> res[b] [rows, words].
+struct RowQueue {
+  using Run = std::function<int(int, int)>;
+  int F = 0, words = 1;
+  std::mutex q_mu;
+  std::condition_variable q_cv;
+  float* stage[2] = {nullptr, nullptr};       // pinned [MB_ROWS, F]: one buffer fills while the other's batch runs
+  float* res[2] = {nullptr, nullptr};         // pinned [MB_ROWS, words]
+  RowWaiter* waiters[2][MB_ROWS] = {};
+  int fill[2] = {0, 0};       // rows queued in a buffer
+  int writers[2] = {0, 0};    // callers still converting their row into it
+  int cur = 0;                // the buffer that takes new rows
+  bool leading = false;
+  int hold_k = 0, hold_ms = 0;                // sb_debug_model_hold
+  std::atomic<long long> batches{0}, rows{0}, max_fill{0};   // since creation: batches run, their rows, the largest
+
+  int alloc(int F_, int words_) {
+    F = F_; words = words_;
+    for (int b = 0; b < 2; ++b) {
+      SB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&stage[b]), sizeof(float) * MB_ROWS * F, cudaHostAllocDefault));
+      SB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&res[b]), sizeof(float) * MB_ROWS * words, cudaHostAllocDefault));
+    }
+    return SB_OK;
+  }
+  ~RowQueue() {
+    for (int b = 0; b < 2; ++b) {
+      if (stage[b]) cudaFreeHost(stage[b]);
+      if (res[b]) cudaFreeHost(res[b]);
+    }
+  }
+
+  // one row of F doubles (cast to float as TensorflowModel.java:64-68 casts it) -> out[words]
+  int submit(const double* row, float* out, const Run& run) {
+    RowWaiter me;
+    me.out = out;
+    std::unique_lock<std::mutex> lk(q_mu);
+    q_cv.wait(lk, [&] { return fill[cur] < MB_ROWS; });
+    const int b = cur, slot = fill[b]++;
+    waiters[b][slot] = &me;
+    ++writers[b];
+    lk.unlock();
+    float* f = stage[b] + static_cast<size_t>(slot) * F;
+    for (int i = 0; i < F; ++i) f[i] = static_cast<float>(row[i]);
+    lk.lock();
+    if (--writers[b] == 0) q_cv.notify_all();
+    while (!me.done) {
+      if (!leading) {           // no batch in flight: lead (a lone caller is scored at once)
+        leading = true;
+        lead(lk, run);
+        leading = false;
+        q_cv.notify_all();
+      } else {
+        q_cv.wait(lk);
+      }
+    }
+    lk.unlock();
+    if (me.status != SB_OK) return set_error(me.status, "%s", me.err.c_str());
+    return SB_OK;
+  }
+
+ private:
+  // The leader (q_mu held through lk): runs the queued rows in batches until the queue is empty, and publishes each
+  // caller's result and status.
+  void lead(std::unique_lock<std::mutex>& lk, const Run& run) {
+    while (fill[cur] > 0) {
+      if (hold_k > 0) {         // sb_debug_model_hold: this batch waits for hold_k rows or the timeout
+        const int k = hold_k;
+        hold_k = 0;
+        q_cv.wait_until(lk, std::chrono::steady_clock::now() + std::chrono::milliseconds(hold_ms), [&] { return fill[cur] >= k; });
+      }
+      const int b = cur;
+      q_cv.wait(lk, [&] { return writers[b] == 0; });
+      const int n = fill[b];
+      cur ^= 1;                 // new rows go to the other buffer (empty: its batch was published before this one began)
+      q_cv.notify_all();
+      lk.unlock();
+      const int s = run(b, n);
+      const std::string err = s == SB_OK ? std::string() : last_error_ref();
+      lk.lock();
+      for (int i = 0; i < n; ++i) {
+        RowWaiter* w = waiters[b][i];
+        w->status = s;
+        if (s == SB_OK) memcpy(w->out, res[b] + static_cast<size_t>(i) * words, sizeof(float) * words);
+        else w->err = err;
+        w->done = true;
+      }
+      fill[b] = 0;
+      ++batches;
+      rows += n;
+      if (n > max_fill) max_fill = n;
+      q_cv.notify_all();
+    }
+  }
 };
 
 struct sb_model {
@@ -1901,20 +2001,9 @@ struct sb_model {
   std::mutex mu;              // device work on the model's stream
   DevBuf<float> sr_act;       // fp32: score_rows_kernel's two activation buffers [SMALL_ROWS, sr_ld]
   int sr_ld = 0;
-  // compute() queue (guarded by q_mu).  No thread of its own: the first caller that finds no batch in flight leads,
-  // running every queued row in batches until the queue is empty; the others wait for their result.
-  std::mutex q_mu;
-  std::condition_variable q_cv;
-  float* stage[2] = {nullptr, nullptr};       // pinned [MB_ROWS, F]: one buffer fills while the other's batch runs
-  float* res[2] = {nullptr, nullptr};         // pinned [MB_ROWS] scores
-  RowWaiter* waiters[2][MB_ROWS] = {};
-  int fill[2] = {0, 0};       // rows queued in a buffer
-  int writers[2] = {0, 0};    // callers still converting their row into it
-  int cur = 0;                // the buffer that takes new rows
-  bool leading = false;
-  int hold_k = 0, hold_ms = 0;                // sb_debug_model_hold
+  RowQueue q;                 // compute() (not allocated for an ensemble's members)
   cudaGraphExec_t mb_graph = nullptr;         // tensor-core modes: the forward of MB_ROWS staged rows
-  std::atomic<long long> st[SB_DEBUG_MSTAT_WORDS] = {};
+  std::atomic<long long> st[SB_DEBUG_MSTAT_WORDS] = {};   // (the first three words are the queue's)
   std::string routes;         // the launches of the last model_forward, "+"-joined (sb_debug_model_routes; guarded by mu)
   // sb_model_sensitivity's buffers (guarded by mu), allocated by its first call and grown when a call needs more
   DevBuf<float> sens_z;       // layer 0's pre-activations of a row chunk [R, ld_out_0]
@@ -1932,21 +2021,25 @@ struct sb_model {
     cudaSetDevice(net.device);
     cudaStreamSynchronize(net.stream);
     if (mb_graph) cudaGraphExecDestroy(mb_graph);
-    for (int b = 0; b < 2; ++b) {
-      if (stage[b]) cudaFreeHost(stage[b]);
-      if (res[b]) cudaFreeHost(res[b]);
-    }
   }
 };
 
 static const int MODEL_CHUNK_ROWS = 16384;        // fp32 parity mode
 static const int MODEL_CHUNK_ROWS_BF16 = 65536;   // bf16: bigger GEMMs per launch (workspace ~0.8 GB at 2000 cols)
 
-static int model_from_desc(sb_net_desc d, const float* flat, int64_t n, int device, sb_model_t** out) {
-  d.max_batch = d.precision == SB_PREC_FP32 ? MODEL_CHUNK_ROWS : (d.precision == SB_PREC_BF16 ? MODEL_CHUNK_ROWS_BF16 : MODEL_CHUNK_ROWS_BF16 / 2);
+static int model_chunk_rows(int precision) {
+  return precision == SB_PREC_FP32 ? MODEL_CHUNK_ROWS : (precision == SB_PREC_BF16 ? MODEL_CHUNK_ROWS_BF16 : MODEL_CHUNK_ROWS_BF16 / 2);
+}
+
+// A model, or (member) an ensemble's member: no compute() queue, and with input_from set it runs on that net's stream and
+// reads its input staging.
+static int model_from_desc(sb_net_desc d, const float* flat, int64_t n, int device, sb_model_t** out, bool member = false,
+                           const Net* input_from = nullptr) {
+  d.max_batch = model_chunk_rows(d.precision);
   std::unique_ptr<sb_model> m(new sb_model());
   m->desc = d;
   Net& net = m->net;
+  net.input_from = input_from;
   SB_TRY(net.init(&d, device, false));
   SB_CHECK(n == net.n_params, SB_ERR_INVALID, "expected %lld params, got %lld", (long long)net.n_params, (long long)n);
   SB_CUDA(cudaMemcpyAsync(net.theta, flat, sizeof(float) * n, cudaMemcpyHostToDevice, net.stream));
@@ -1958,10 +2051,7 @@ static int model_from_desc(sb_net_desc d, const float* flat, int64_t n, int devi
     SB_TRY(m->sr_act.alloc(static_cast<size_t>(2) * SMALL_ROWS * m->sr_ld));
     SB_TRY(set_max_smem(score_rows_kernel, SR_SMEM));
   }
-  for (int b = 0; b < 2; ++b) {
-    SB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&m->stage[b]), sizeof(float) * MB_ROWS * net.F, cudaHostAllocDefault));
-    SB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&m->res[b]), sizeof(float) * MB_ROWS, cudaHostAllocDefault));
-  }
+  if (!member) SB_TRY(m->q.alloc(net.F, 1));
   SB_CUDA(cudaStreamSynchronize(net.stream));
   *out = m.release();
   return SB_OK;
@@ -2001,30 +2091,32 @@ static int model_forward(sb_model* m, const float* dX, int rows, float* dOut) {
   return s;
 }
 
-// tensor-core modes: model_forward of MB_ROWS rows of the staging area, captured once, so a micro-batch is one launch
-static int capture_micro_batch(sb_model* m) {
-  Net& n = m->net;
+// tensor-core modes: the forward of one compute() batch (fwd(), MB_ROWS rows of the staging area) captured once into
+// *graph, so a micro-batch is one launch
+template <typename Fwd>
+static int capture_micro_batch(cudaStream_t st, const Fwd& fwd, cudaGraphExec_t* graph) {
   cudaGraph_t g = nullptr;
-  SB_CUDA(cudaStreamBeginCapture(n.stream, cudaStreamCaptureModeThreadLocal));
-  const int s = model_forward(m, n.stX, MB_ROWS, n.yhat);
-  const cudaError_t e = cudaStreamEndCapture(n.stream, &g);
+  SB_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+  const int s = fwd();
+  const cudaError_t e = cudaStreamEndCapture(st, &g);
   if (s != SB_OK) { if (g) cudaGraphDestroy(g); return s; }
   SB_CHECK(e == cudaSuccess, SB_ERR_CUDA, "cudaStreamEndCapture failed: %s", cudaGetErrorString(e));
-  const cudaError_t ei = cudaGraphInstantiate(&m->mb_graph, g, 0);
+  const cudaError_t ei = cudaGraphInstantiate(graph, g, 0);
   cudaGraphDestroy(g);
   SB_CHECK(ei == cudaSuccess, SB_ERR_CUDA, "cudaGraphInstantiate failed: %s", cudaGetErrorString(ei));
   return SB_OK;
 }
 
-// one compute() batch: rows of staging buffer b -> m->res[b].  A tensor-core batch runs at MB_ROWS rows, its pad rows
+// one compute() batch: rows of staging buffer b -> m->q.res[b].  A tensor-core batch runs at MB_ROWS rows, its pad rows
 // zero-filled; only the real rows are copied back.
 static int run_micro_batch(sb_model* m, int b, int rows) {
   std::lock_guard<std::mutex> lk(m->mu);
   Net& n = m->net;
   SB_CUDA(cudaSetDevice(n.device));
-  if (n.tc() && !m->mb_graph) SB_TRY(capture_micro_batch(m));
+  if (n.tc() && !m->mb_graph)
+    SB_TRY(capture_micro_batch(n.stream, [&] { return model_forward(m, n.stX, MB_ROWS, n.yhat); }, &m->mb_graph));
   const size_t row_bytes = sizeof(float) * n.F;
-  SB_CUDA(cudaMemcpyAsync(n.stX, m->stage[b], row_bytes * rows, cudaMemcpyHostToDevice, n.stream));
+  SB_CUDA(cudaMemcpyAsync(n.stX, m->q.stage[b], row_bytes * rows, cudaMemcpyHostToDevice, n.stream));
   if (n.tc()) {
     if (rows < MB_ROWS) SB_CUDA(cudaMemsetAsync(n.stX + static_cast<size_t>(rows) * n.F, 0, row_bytes * (MB_ROWS - rows), n.stream));
     SB_CUDA(cudaGraphLaunch(m->mb_graph, n.stream));
@@ -2033,43 +2125,29 @@ static int run_micro_batch(sb_model* m, int b, int rows) {
     SB_TRY(model_forward(m, n.stX, rows, n.yhat));
     ++m->st[SB_DEBUG_MSTAT_SMALL];
   }
-  SB_CUDA(cudaMemcpyAsync(m->res[b], n.yhat, sizeof(float) * rows, cudaMemcpyDeviceToHost, n.stream));
+  SB_CUDA(cudaMemcpyAsync(m->q.res[b], n.yhat, sizeof(float) * rows, cudaMemcpyDeviceToHost, n.stream));
   SB_CUDA(cudaStreamSynchronize(n.stream));
   return SB_OK;
 }
 
-// The leader (q_mu held through lk): runs the queued rows in batches until the queue is empty, and publishes each
-// caller's result and status.
-static void lead_batches(sb_model* m, std::unique_lock<std::mutex>& lk) {
-  while (m->fill[m->cur] > 0) {
-    if (m->hold_k > 0) {      // sb_debug_model_hold: this batch waits for hold_k rows or the timeout
-      const int k = m->hold_k;
-      m->hold_k = 0;
-      m->q_cv.wait_until(lk, std::chrono::steady_clock::now() + std::chrono::milliseconds(m->hold_ms),
-                         [&] { return m->fill[m->cur] >= k; });
-    }
-    const int b = m->cur;
-    m->q_cv.wait(lk, [&] { return m->writers[b] == 0; });
-    const int rows = m->fill[b];
-    m->cur ^= 1;              // new rows go to the other buffer (empty: its batch was published before this one began)
-    m->q_cv.notify_all();
-    lk.unlock();
-    const int s = run_micro_batch(m, b, rows);
-    const std::string err = s == SB_OK ? std::string() : last_error_ref();
-    lk.lock();
-    for (int i = 0; i < rows; ++i) {
-      RowWaiter* w = m->waiters[b][i];
-      w->status = s;
-      if (s == SB_OK) w->value = m->res[b][i];
-      else w->err = err;
-      w->done = true;
-    }
-    m->fill[b] = 0;
-    ++m->st[SB_DEBUG_MSTAT_BATCHES];
-    m->st[SB_DEBUG_MSTAT_ROWS] += rows;
-    if (rows > m->st[SB_DEBUG_MSTAT_MAX_FILL]) m->st[SB_DEBUG_MSTAT_MAX_FILL] = rows;
-    m->q_cv.notify_all();
-  }
+// A SavedModel directory -> the topology (at `precision`) and flat parameters of a scoring model; host work only.  The
+// null checks mirror TensorflowModel.init (TensorflowModel.java:147-166).
+static int read_scoring_model(const char* saved_model_dir, const char* input_name, const char* output_name, const char* tag,
+                              int precision, sb_net_desc* d, std::vector<float>* flat) {
+  SB_CHECK(saved_model_dir && saved_model_dir[0], SB_ERR_INVALID, "Model path is null");
+  SB_CHECK(input_name && input_name[0], SB_ERR_INVALID, "Input names is null");
+  SB_CHECK(output_name && output_name[0], SB_ERR_INVALID, "Output names is null");
+  SB_CHECK(tag && tag[0], SB_ERR_INVALID, "Tags is null");
+  memset(d, 0, sizeof(*d));
+  int32_t out_act = SB_ACT_SIGMOID;
+  int64_t np = 0;
+  SB_TRY(sb_savedmodel_read(saved_model_dir, input_name, output_name, tag, d, &out_act, nullptr, 0, &np));
+  SB_CHECK(out_act == SB_ACT_SIGMOID, SB_ERR_FORMAT, "output layer must be a sigmoid unit");
+  flat->assign(static_cast<size_t>(np), 0.f);
+  SB_TRY(sb_savedmodel_read(saved_model_dir, input_name, output_name, tag, d, &out_act, flat->data(), np, &np));
+  d->precision = precision;
+  d->max_batch = 1;
+  return SB_OK;
 }
 
 extern "C" {
@@ -2087,22 +2165,10 @@ int sb_model_load(const char* saved_model_dir, const char* input_name, const cha
                   int device, int precision, sb_model_t** out) {
   SB_CHECK(out, SB_ERR_INVALID, "out is null");
   *out = nullptr;
-  // the null checks mirror TensorflowModel.init (TensorflowModel.java:147-166)
-  SB_CHECK(saved_model_dir && saved_model_dir[0], SB_ERR_INVALID, "Model path is null");
-  SB_CHECK(input_name && input_name[0], SB_ERR_INVALID, "Input names is null");
-  SB_CHECK(output_name && output_name[0], SB_ERR_INVALID, "Output names is null");
-  SB_CHECK(tag && tag[0], SB_ERR_INVALID, "Tags is null");
   sb_net_desc d;
-  memset(&d, 0, sizeof(d));
-  int32_t out_act = SB_ACT_SIGMOID;
-  int64_t np = 0;
-  SB_TRY(sb_savedmodel_read(saved_model_dir, input_name, output_name, tag, &d, &out_act, nullptr, 0, &np));
-  SB_CHECK(out_act == SB_ACT_SIGMOID, SB_ERR_FORMAT, "output layer must be a sigmoid unit");
-  std::vector<float> flat(static_cast<size_t>(np));
-  SB_TRY(sb_savedmodel_read(saved_model_dir, input_name, output_name, tag, &d, &out_act, flat.data(), np, &np));
-  d.precision = precision;
-  d.max_batch = 1;
-  return model_from_desc(d, flat.data(), np, device, out);
+  std::vector<float> flat;
+  SB_TRY(read_scoring_model(saved_model_dir, input_name, output_name, tag, precision, &d, &flat));
+  return model_from_desc(d, flat.data(), static_cast<int64_t>(flat.size()), device, out);
 }
 
 int sb_model_destroy(sb_model_t* m) {
@@ -2134,30 +2200,9 @@ int sb_model_score_row_f64(sb_model_t* m, const double* row, int32_t n, double* 
   SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
   SB_CHECK(row && out, SB_ERR_INVALID, "null argument");
   SB_CHECK(n == m->net.F, SB_ERR_INVALID, "expected %d features, got %d", m->net.F, n);
-  RowWaiter me;
-  std::unique_lock<std::mutex> lk(m->q_mu);
-  m->q_cv.wait(lk, [&] { return m->fill[m->cur] < MB_ROWS; });
-  const int b = m->cur, slot = m->fill[b]++;
-  m->waiters[b][slot] = &me;
-  ++m->writers[b];
-  lk.unlock();
-  float* f = m->stage[b] + static_cast<size_t>(slot) * n;
-  for (int i = 0; i < n; ++i) f[i] = static_cast<float>(row[i]);  // TensorflowModel.java:64-68
-  lk.lock();
-  if (--m->writers[b] == 0) m->q_cv.notify_all();
-  while (!me.done) {
-    if (!m->leading) {        // no batch in flight: lead (a lone caller is scored at once)
-      m->leading = true;
-      lead_batches(m, lk);
-      m->leading = false;
-      m->q_cv.notify_all();
-    } else {
-      m->q_cv.wait(lk);
-    }
-  }
-  lk.unlock();
-  if (me.status != SB_OK) return set_error(me.status, "%s", me.err.c_str());
-  *out = static_cast<double>(me.value);
+  float v = 0.f;
+  SB_TRY(m->q.submit(row, &v, [m](int b, int rows) { return run_micro_batch(m, b, rows); }));
+  *out = static_cast<double>(v);
   return SB_OK;
 }
 
@@ -2391,6 +2436,9 @@ int sb_debug_model_batch_stats(sb_model_t* m, int64_t* stats, int32_t n_stats) {
   SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
   SB_CHECK(stats && n_stats >= SB_DEBUG_MSTAT_WORDS, SB_ERR_INVALID, "stats needs %d words, got %d", SB_DEBUG_MSTAT_WORDS, n_stats);
   for (int i = 0; i < SB_DEBUG_MSTAT_WORDS; ++i) stats[i] = m->st[i].load();
+  stats[SB_DEBUG_MSTAT_BATCHES] = m->q.batches.load();
+  stats[SB_DEBUG_MSTAT_ROWS] = m->q.rows.load();
+  stats[SB_DEBUG_MSTAT_MAX_FILL] = m->q.max_fill.load();
   return SB_OK;
 }
 
@@ -2406,9 +2454,281 @@ int sb_debug_model_hold(sb_model_t* m, int32_t k, int32_t timeout_ms) {
   SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
   SB_CHECK(k >= 0 && k <= MB_ROWS && timeout_ms >= 0, SB_ERR_INVALID, "k = %d outside [0, %d] or timeout_ms = %d < 0", k, MB_ROWS,
            timeout_ms);
-  std::lock_guard<std::mutex> lk(m->q_mu);
-  m->hold_k = k;
-  m->hold_ms = timeout_ms;
+  std::lock_guard<std::mutex> lk(m->q.q_mu);
+  m->q.hold_k = k;
+  m->q.hold_ms = timeout_ms;
+  return SB_OK;
+}
+
+int sb_debug_model_bytes(sb_model_t* m, int64_t* out) {
+  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
+  SB_CHECK(out, SB_ERR_INVALID, "null argument");
+  *out = static_cast<int64_t>(m->net.dalloc_bytes);
+  return SB_OK;
+}
+
+}  // extern "C"
+
+// ================================================================================================
+// ensemble: K member models on one stream that share one staged copy of the rows (DESIGN §6h)
+// ================================================================================================
+struct sb_ensemble {
+  // Member 0 owns the stream and the input staging (stX, Xb / Xf); members 1 .. K-1 are created with input_from = its net
+  // and allocate neither.  Destroyed in reverse order, member 0 last.
+  std::vector<sb_model*> members;
+  int K = 0;
+  std::mutex mu;              // device work on the ensemble's stream
+  float* slots = nullptr;     // [K, max_batch]: member g's scores of a chunk at slots + g * max_batch (member 0's net)
+  float* d_scores = nullptr;  // [max_batch, K] and [max_batch, 4]: the outputs of sb_ensemble_score and compute() batches
+  float* d_stats = nullptr;
+  RowQueue q;                 // compute(): K + 4 words per row
+  cudaGraphExec_t mb_graph = nullptr;         // tensor-core modes: the ensemble forward of MB_ROWS staged rows
+  std::string routes;         // the launches of the last chunk, "+"-joined (sb_debug_ensemble_routes; guarded by mu)
+  Net& lead() { return members[0]->net; }
+  ~sb_ensemble() {
+    if (!members.empty() && members[0]->net.stream) {
+      cudaSetDevice(lead().device);
+      cudaStreamSynchronize(lead().stream);
+    }
+    if (mb_graph) cudaGraphExecDestroy(mb_graph);
+    while (!members.empty()) {
+      delete members.back();
+      members.pop_back();
+    }
+  }
+};
+
+// the flat parameter count of a topology (what Net::init lays out)
+static long long desc_param_count(const sb_net_desc& d) {
+  long long np = 0;
+  int prev = d.n_features;
+  for (int l = 0; l <= d.n_hidden; ++l) {
+    const int out = l < d.n_hidden ? d.hidden[l] : 1;
+    np += static_cast<long long>(prev) * out + out;
+    prev = out;
+  }
+  return np;
+}
+
+// K checked descriptors (n_features and precision shared) and their parameters -> an ensemble
+static int ensemble_from_descs(const std::vector<sb_net_desc>& ds, const float* const* flats, const int64_t* n_params, int device,
+                               sb_ensemble_t** out) {
+  std::unique_ptr<sb_ensemble> e(new sb_ensemble());
+  e->K = static_cast<int>(ds.size());
+  for (int g = 0; g < e->K; ++g) {
+    sb_model* m = nullptr;
+    SB_TRY(model_from_desc(ds[g], flats[g], n_params[g], device, &m, true, g > 0 ? &e->lead() : nullptr));
+    e->members.push_back(m);
+  }
+  Net& n0 = e->lead();
+  SB_TRY(n0.dalloc(&e->slots, static_cast<size_t>(e->K) * n0.max_batch));
+  SB_TRY(n0.dalloc(&e->d_scores, static_cast<size_t>(n0.max_batch) * e->K));
+  SB_TRY(n0.dalloc(&e->d_stats, static_cast<size_t>(n0.max_batch) * 4));
+  SB_TRY(e->q.alloc(n0.F, e->K + 4));
+  SB_CUDA(cudaStreamSynchronize(n0.stream));
+  *out = e.release();
+  return SB_OK;
+}
+
+// The members' forwards and the statistics of `rows` (<= max_batch) device rows dX, queued on the ensemble's stream.
+// Tensor-core modes and fp32 chunks of more than SMALL_ROWS rows load the rows once (member 0's descriptor and
+// load_batch_kernel into the shared Xb / Xf), then run each member's hidden-layer and output launches, which read that
+// operand; an fp32 chunk of up to SMALL_ROWS rows is one score_rows_kernel launch per member, reading dX.  Scoring reads
+// no descriptor field or step scalar besides what the load reads (the output layer runs without the loss), so the other
+// members need no descriptor of their own.  Each member's launches are the ones enqueue_model_forward runs for the same
+// rows, minus the load.  Then ensemble_stats_kernel: slots -> dScores / dStats (either may be null).
+static int enqueue_ensemble_forward(sb_ensemble* e, const float* dX, int rows, float* dScores, float* dStats) {
+  Net& n0 = e->lead();
+  const bool layered = n0.tc() || rows > SMALL_ROWS;
+  if (layered) {
+    const StepIn in{n0.desc, n0.scal};
+    const Batch b = host_batch(n0, dX, nullptr, nullptr, rows);
+    SB_TRY(write_desc(n0.stream, in, &b, 0.f, 1.f, 0, nullptr));
+    SB_TRY(n0.enqueue_load(in, rows));
+  }
+  for (int g = 0; g < e->K; ++g) {
+    sb_model* m = e->members[g];
+    Net& n = m->net;
+    float* slot = e->slots + static_cast<size_t>(g) * n0.max_batch;
+    if (!layered) {
+      SB_TRY(enqueue_model_forward(m, dX, rows, slot));
+      continue;
+    }
+    const StepIn in{n.desc, n.scal};
+    SB_TRY(n.enqueue_hidden_forward(in, rows));
+    SB_TRY(n.enqueue_out(in, rows, false, false, slot, nullptr));
+  }
+  SB_TRY(launch_kernel(ensemble_stats_kernel, dim3(static_cast<unsigned>((rows + ENS_THREADS - 1) / ENS_THREADS)), dim3(ENS_THREADS), 0,
+                       n0.stream, false, static_cast<const float*>(e->slots), static_cast<long long>(n0.max_batch), e->K, rows,
+                       dScores, dStats));
+  n0.mark("ensemble_stats");
+  return SB_OK;
+}
+
+// Every scoring path of an ensemble comes through here; its launches are kept for sb_debug_ensemble_routes.  Called with
+// e->mu held.
+static int ensemble_forward(sb_ensemble* e, const float* dX, int rows, float* dScores, float* dStats) {
+  e->routes.clear();
+  for (sb_model* m : e->members) m->net.marks = &e->routes;
+  const int s = enqueue_ensemble_forward(e, dX, rows, dScores, dStats);
+  for (sb_model* m : e->members) m->net.marks = nullptr;
+  return s;
+}
+
+// one compute() batch: rows of staging buffer b -> e->q.res[b] [rows, K + 4].  A tensor-core batch runs the captured
+// forward of MB_ROWS rows (one load, K members, the statistics), its pad rows zero-filled.
+static int run_ensemble_micro_batch(sb_ensemble* e, int b, int rows) {
+  std::lock_guard<std::mutex> lk(e->mu);
+  Net& n = e->lead();
+  SB_CUDA(cudaSetDevice(n.device));
+  if (n.tc() && !e->mb_graph)
+    SB_TRY(capture_micro_batch(n.stream, [&] { return ensemble_forward(e, n.stX, MB_ROWS, e->d_scores, e->d_stats); }, &e->mb_graph));
+  const size_t row_bytes = sizeof(float) * n.F;
+  SB_CUDA(cudaMemcpyAsync(n.stX, e->q.stage[b], row_bytes * rows, cudaMemcpyHostToDevice, n.stream));
+  if (n.tc()) {
+    if (rows < MB_ROWS) SB_CUDA(cudaMemsetAsync(n.stX + static_cast<size_t>(rows) * n.F, 0, row_bytes * (MB_ROWS - rows), n.stream));
+    SB_CUDA(cudaGraphLaunch(e->mb_graph, n.stream));
+  } else {
+    SB_TRY(ensemble_forward(e, n.stX, rows, e->d_scores, e->d_stats));
+  }
+  const size_t pitch = sizeof(float) * (e->K + 4);
+  SB_CUDA(cudaMemcpy2DAsync(e->q.res[b], pitch, e->d_scores, sizeof(float) * e->K, sizeof(float) * e->K, rows, cudaMemcpyDeviceToHost,
+                            n.stream));
+  SB_CUDA(cudaMemcpy2DAsync(e->q.res[b] + e->K, pitch, e->d_stats, sizeof(float) * 4, sizeof(float) * 4, rows, cudaMemcpyDeviceToHost,
+                            n.stream));
+  SB_CUDA(cudaStreamSynchronize(n.stream));
+  return SB_OK;
+}
+
+static int check_ensemble_k(int32_t k) {
+  SB_CHECK(k >= 1 && k <= SB_ENSEMBLE_MAX, SB_ERR_INVALID, "k = %d members outside [1, %d]", k, SB_ENSEMBLE_MAX);
+  return SB_OK;
+}
+
+static int check_ensemble_members(const std::vector<sb_net_desc>& ds) {
+  for (size_t g = 1; g < ds.size(); ++g) {
+    SB_CHECK(ds[g].n_features == ds[0].n_features, SB_ERR_INVALID, "member %d has %d features, member 0 has %d", static_cast<int>(g),
+             ds[g].n_features, ds[0].n_features);
+    SB_CHECK(ds[g].precision == ds[0].precision, SB_ERR_INVALID, "member %d has precision %d, member 0 has %d", static_cast<int>(g),
+             ds[g].precision, ds[0].precision);
+  }
+  return SB_OK;
+}
+
+extern "C" {
+
+int sb_ensemble_create(const sb_net_desc* descs, const float* const* flats, const int64_t* n_params, int32_t k, int device,
+                       sb_ensemble_t** out) {
+  SB_CHECK(out, SB_ERR_INVALID, "out is null");
+  *out = nullptr;
+  SB_TRY(check_ensemble_k(k));
+  SB_CHECK(descs && flats && n_params, SB_ERR_INVALID, "null argument");
+  std::vector<sb_net_desc> ds(descs, descs + k);
+  for (int g = 0; g < k; ++g) {
+    SB_CHECK(flats[g], SB_ERR_INVALID, "flats[%d] is null", g);
+    if (ds[g].max_batch <= 0) ds[g].max_batch = 1;
+    SB_TRY(validate_desc(&ds[g]));
+    const long long np = desc_param_count(ds[g]);
+    SB_CHECK(n_params[g] == np, SB_ERR_INVALID, "member %d: expected %lld params, got %lld", g, np, static_cast<long long>(n_params[g]));
+  }
+  SB_TRY(check_ensemble_members(ds));
+  return ensemble_from_descs(ds, flats, n_params, device, out);
+}
+
+int sb_ensemble_load(const char* const* dirs, int32_t k, const char* input_name, const char* output_name, const char* tag,
+                     int device, int precision, sb_ensemble_t** out) {
+  SB_CHECK(out, SB_ERR_INVALID, "out is null");
+  *out = nullptr;
+  SB_TRY(check_ensemble_k(k));
+  SB_CHECK(dirs, SB_ERR_INVALID, "dirs is null");
+  std::vector<sb_net_desc> ds(static_cast<size_t>(k));
+  std::vector<std::vector<float>> flat(static_cast<size_t>(k));
+  for (int g = 0; g < k; ++g) SB_TRY(read_scoring_model(dirs[g], input_name, output_name, tag, precision, &ds[g], &flat[g]));
+  SB_TRY(check_ensemble_members(ds));
+  std::vector<const float*> fp(static_cast<size_t>(k));
+  std::vector<int64_t> np(static_cast<size_t>(k));
+  for (int g = 0; g < k; ++g) { fp[g] = flat[g].data(); np[g] = static_cast<int64_t>(flat[g].size()); }
+  return ensemble_from_descs(ds, fp.data(), np.data(), device, out);
+}
+
+int sb_ensemble_destroy(sb_ensemble_t* e) {
+  delete e;
+  return SB_OK;
+}
+
+int32_t sb_ensemble_size(const sb_ensemble_t* e) { return e ? e->K : 0; }
+
+// the argument checks every scoring entry point shares
+static int check_ensemble_score(const sb_ensemble* e, const float* X, int64_t rows, const float* scores, const float* stats) {
+  SB_CHECK(e, SB_ERR_STATE, "TF ensemble not initialized.");
+  SB_CHECK(X, SB_ERR_INVALID, "X is null");
+  SB_CHECK(scores || stats, SB_ERR_INVALID, "scores and stats are both null");
+  SB_CHECK(rows >= 0, SB_ERR_INVALID, "rows = %lld < 0", static_cast<long long>(rows));
+  return SB_OK;
+}
+
+int sb_ensemble_score(sb_ensemble_t* e, const float* X, int64_t rows, float* scores, float* stats) {
+  SB_TRY(check_ensemble_score(e, X, rows, scores, stats));
+  if (rows == 0) return SB_OK;
+  std::lock_guard<std::mutex> lk(e->mu);
+  Net& n = e->lead();
+  const int K = e->K;
+  SB_CUDA(cudaSetDevice(n.device));
+  for (int64_t r0 = 0; r0 < rows; r0 += n.max_batch) {
+    const int c = static_cast<int>(rows - r0 < n.max_batch ? rows - r0 : n.max_batch);
+    SB_CUDA(cudaMemcpyAsync(n.stX, X + r0 * n.F, sizeof(float) * c * static_cast<size_t>(n.F), cudaMemcpyDefault, n.stream));
+    SB_TRY(ensemble_forward(e, n.stX, c, scores ? e->d_scores : nullptr, stats ? e->d_stats : nullptr));
+    if (scores) SB_CUDA(cudaMemcpyAsync(scores + r0 * K, e->d_scores, sizeof(float) * c * K, cudaMemcpyDefault, n.stream));
+    if (stats) SB_CUDA(cudaMemcpyAsync(stats + r0 * 4, e->d_stats, sizeof(float) * c * 4, cudaMemcpyDefault, n.stream));
+    SB_CUDA(cudaStreamSynchronize(n.stream));
+  }
+  return SB_OK;
+}
+
+int sb_ensemble_score_device(sb_ensemble_t* e, const float* dX, int64_t rows, float* dScores, float* dStats) {
+  SB_TRY(check_ensemble_score(e, dX, rows, dScores, dStats));
+  std::lock_guard<std::mutex> lk(e->mu);
+  Net& n = e->lead();
+  SB_CUDA(cudaSetDevice(n.device));
+  for (int64_t r0 = 0; r0 < rows; r0 += n.max_batch) {
+    const int c = static_cast<int>(rows - r0 < n.max_batch ? rows - r0 : n.max_batch);
+    SB_TRY(ensemble_forward(e, dX + r0 * n.F, c, dScores ? dScores + r0 * e->K : nullptr, dStats ? dStats + r0 * 4 : nullptr));
+  }
+  return SB_OK;
+}
+
+int sb_ensemble_score_row_f64(sb_ensemble_t* e, const double* row, int32_t n, double* out) {
+  SB_CHECK(e, SB_ERR_STATE, "TF ensemble not initialized.");
+  SB_CHECK(row && out, SB_ERR_INVALID, "null argument");
+  SB_CHECK(n == e->q.F, SB_ERR_INVALID, "expected %d features, got %d", e->q.F, n);
+  float v[SB_ENSEMBLE_MAX + 4];
+  SB_TRY(e->q.submit(row, v, [e](int b, int rows) { return run_ensemble_micro_batch(e, b, rows); }));
+  for (int i = 0; i < e->K + 4; ++i) out[i] = static_cast<double>(v[i]);
+  return SB_OK;
+}
+
+int sb_ensemble_sync(sb_ensemble_t* e) {
+  SB_CHECK(e, SB_ERR_STATE, "TF ensemble not initialized.");
+  SB_CUDA(cudaStreamSynchronize(e->lead().stream));
+  return SB_OK;
+}
+
+void* sb_ensemble_stream(sb_ensemble_t* e) { return e ? reinterpret_cast<void*>(e->lead().stream) : nullptr; }
+
+int sb_debug_ensemble_routes(sb_ensemble_t* e, char* out, int32_t cap) {
+  SB_CHECK(e, SB_ERR_STATE, "TF ensemble not initialized.");
+  SB_CHECK(out && cap > 0, SB_ERR_INVALID, "route buffer of %d bytes", cap);
+  std::lock_guard<std::mutex> lk(e->mu);
+  snprintf(out, static_cast<size_t>(cap), "%s", e->routes.empty() ? "none" : e->routes.c_str());
+  return SB_OK;
+}
+
+int sb_debug_ensemble_bytes(sb_ensemble_t* e, int64_t* out) {
+  SB_CHECK(e, SB_ERR_STATE, "TF ensemble not initialized.");
+  SB_CHECK(out, SB_ERR_INVALID, "null argument");
+  long long b = 0;
+  for (const sb_model* m : e->members) b += static_cast<long long>(m->net.dalloc_bytes);
+  *out = b;
   return SB_OK;
 }
 

@@ -165,9 +165,15 @@ int Net::init(const sb_net_desc* d, int device_, bool training_) {
   const bool want_trace = getenv("SB_STEP_TRACE") != nullptr;
   // the main chain is the critical path: its CTAs are scheduled ahead of the trainer's side stream's (dW GEMMs, second
   // optimizer)
-  int prio_least = 0, prio_greatest = 0;
-  SB_CUDA(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));
-  SB_CUDA(cudaStreamCreateWithPriority(&stream, cudaStreamNonBlocking, prio_greatest));
+  if (input_from) {
+    SB_CHECK(input_from->F == d->n_features && input_from->max_batch == d->max_batch && input_from->device == device_,
+             SB_ERR_INVALID, "a net that borrows input staging needs the lender's features, max_batch and device");
+    stream = input_from->stream;
+  } else {
+    int prio_least = 0, prio_greatest = 0;
+    SB_CUDA(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));
+    SB_CUDA(cudaStreamCreateWithPriority(&stream, cudaStreamNonBlocking, prio_greatest));
+  }
   F = d->n_features;
   L = d->n_hidden;
   precision = d->precision;
@@ -224,14 +230,16 @@ int Net::init(const sb_net_desc* d, int device_, bool training_) {
   if (want_trace) SB_TRY(dalloc(&step_trace, 32 * 16));
   SB_TRY(dalloc(&yhat, max_batch));
   SB_TRY(dalloc(&ones, max_batch));
-  SB_TRY(dalloc(&stX, static_cast<size_t>(max_batch) * F));
+  if (input_from) stX = input_from->stX;
+  else SB_TRY(dalloc(&stX, static_cast<size_t>(max_batch) * F));
   SB_TRY(dalloc(&stY, max_batch));
   SB_TRY(dalloc(&stW, max_batch));
   fill_kernel<<<(max_batch + 255) / 256, 256, 0, stream>>>(ones, 1.f, max_batch);
 
   if (bf) {
     Xb_ps = static_cast<long long>(max_batch) * ldF;
-    SB_TRY(dalloc(&Xb, static_cast<size_t>(Xb_ps) * nparts));
+    if (input_from) Xb = input_from->Xb;
+    else SB_TRY(dalloc(&Xb, static_cast<size_t>(Xb_ps) * nparts));
     A.assign(L, nullptr); dZ.assign(L, nullptr); A_ps.assign(L, 0);
     for (int l = 0; l < L; ++l) {
       Layer& ly = layers[l];
@@ -240,7 +248,8 @@ int Net::init(const sb_net_desc* d, int device_, bool training_) {
       if (training) SB_TRY(dalloc(&dZ[l], static_cast<size_t>(A_ps[l]) * nparts));
     }
   } else {
-    SB_TRY(dalloc(&Xf, static_cast<size_t>(max_batch) * F));
+    if (input_from) Xf = input_from->Xf;
+    else SB_TRY(dalloc(&Xf, static_cast<size_t>(max_batch) * F));
     Af.assign(L, nullptr); dZf.assign(L, nullptr);
     for (int l = 0; l < L; ++l) {
       SB_TRY(dalloc(&Af[l], static_cast<size_t>(max_batch) * layers[l].out));
@@ -283,7 +292,7 @@ Net::~Net() {
   cudaSetDevice(device);
   if (stream) cudaStreamSynchronize(stream);
   for (void* p : allocs) cudaFree(p);
-  if (stream) cudaStreamDestroy(stream);
+  if (stream && !input_from) cudaStreamDestroy(stream);
 }
 
 int check_sparse_idx(const int32_t* idx, long long n, int n_onehot) {

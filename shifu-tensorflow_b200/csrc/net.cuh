@@ -65,6 +65,9 @@ struct Net {
   // is set by the trainer BEFORE init(): room for its gradient buffer and flag block behind the parameters.
   char* arena = nullptr;
   size_t arena_bytes = 0, arena_extra_bytes = 0;
+  // Set BEFORE init() on an ensemble member (capi.cu sb_ensemble): the net runs on input_from's stream and uses its input
+  // staging (stX, Xb / Xf) instead of creating its own; input_from must have the same F and max_batch and outlive it.
+  const Net* input_from = nullptr;
   size_t s1_off = 0, s2_off = 0, shadow_off = 0, extra_off = 0;   // byte offsets inside the arena (theta at 0)
   float* theta = nullptr;
   float *s1 = nullptr, *s2 = nullptr;      // optimizer state (training only)

@@ -8,6 +8,7 @@ JNI is java/ml/shifu/shifu/tensorflow/B200Model.java (INTEGRATION.md).
               "properties": {"modelpath": "/path/to/saved_model_dir", "outputnames": "shifu_output_0",
                              "tags": ["serve"], "algorithm": "tensorflow", "normtype": "ZSCALE"}}
     m = TensorflowModel(); m.init(config); score = m.compute(row_of_doubles)
+    e = TensorflowEnsemble(); e.init([config_of_model0, ..., config_of_model4]); r = e.compute(row_of_doubles)
 """
 from __future__ import annotations
 
@@ -55,6 +56,14 @@ class TensorflowModel:
     def init(self, config) -> None:
         if self.initiate:                                   # idempotent (:114-116)
             return
+        self.init_config(config)
+        self._model = capi.Model.load(self.modelPath, self.inputNames[0], self.outputNames, tag=self.tags[0],
+                                      device=self._device, precision=self._precision)
+        self.initiate = True
+
+    def init_config(self, config) -> None:
+        """init's reading and checking of the GenericModelConfig, without loading the model (TensorflowEnsemble checks
+        each member's config this way)"""
         if config is None:
             raise RuntimeError("Config is null")
         self.config = config
@@ -90,9 +99,6 @@ class TensorflowModel:
         # True / non-zero (training branch: dropout active) or any other type -> rejected here, at init.
         for name in self.inputNames[1:]:
             check_phase_switch(name, self.properties.get(name))
-        self._model = capi.Model.load(self.modelPath, self.inputNames[0], self.outputNames, tag=self.tags[0],
-                                      device=self._device, precision=self._precision)
-        self.initiate = True
 
     # -- Computable.compute (TensorflowModel.java:53-94): double[] -> float[] -> [1,n] forward -> double --
     def compute(self, input) -> float:
@@ -143,4 +149,66 @@ class TensorflowModel:
         if self._model is not None:
             self._model.close()
             self._model = None
+        self.initiate = False
+
+
+class TensorflowEnsemble:
+    """The bagged form of TensorflowModel: `shifu eval` over a run's models/model0 .. model{K-1} (train.baggingNum
+    members), each row scored by every member, with the members' mean, max, min and median.  init takes one
+    GenericModelConfig per member, checked as TensorflowModel.init checks one; the members are scored together on one
+    device from one staged copy of the rows (sb_ensemble_*)."""
+
+    def __init__(self, device: int = 0, precision: int = capi.PREC_FP32):
+        self.initiate = False
+        self.members: List[TensorflowModel] = []
+        self._ensemble: Optional[capi.Ensemble] = None
+        self._device, self._precision = device, precision
+
+    def init(self, configs: Sequence[Any]) -> None:
+        if self.initiate:
+            return
+        if configs is None or len(configs) == 0:
+            raise RuntimeError("Configs is null")
+        members = []
+        for config in configs:
+            m = TensorflowModel(self._device, self._precision)
+            m.init_config(config)
+            members.append(m)
+        names = {(m.inputNames[0], m.outputNames, m.tags[0]) for m in members}
+        if len(names) != 1:
+            raise IllegalArgumentException("Every member must have the same input name, output name and tag.")
+        inp, outp, tag = names.pop()
+        self._ensemble = capi.Ensemble.load([m.modelPath for m in members], inp, outp, tag=tag, device=self._device,
+                                            precision=self._precision)
+        self.members = members
+        self.initiate = True
+
+    def _check(self) -> capi.Ensemble:
+        if not self.initiate or self._ensemble is None:
+            raise IllegalStateException("TF ensemble not initialized.")
+        return self._ensemble
+
+    # -- compute() of every member: double[] -> {"scores": [K] in member order, "mean", "max", "min", "median"} --
+    def compute(self, input) -> dict:
+        e = self._check()
+        data = input.getData() if hasattr(input, "getData") else input
+        r = e.score_row_f64(np.asarray(data, dtype=np.float64))
+        out = {"scores": r[:e.k]}
+        out.update({name: float(r[e.k + i]) for i, name in enumerate(capi.ENSEMBLE_STATS)})
+        return out
+
+    # -- the whole table in one call: {"scores": [rows, K], "mean" .. "median": [rows]} as float64 --
+    def computeBatch(self, rows) -> dict:
+        e = self._check()
+        X = np.asarray(rows, dtype=np.float64).astype(np.float32)     # the same double -> float cast as compute()
+        s, t = e.score(X)
+        out = {"scores": s.astype(np.float64)}
+        out.update({name: t[:, i].astype(np.float64) for i, name in enumerate(capi.ENSEMBLE_STATS)})
+        return out
+
+    def releaseResource(self) -> None:
+        if self._ensemble is not None:
+            self._ensemble.close()
+            self._ensemble = None
+        self.members = []
         self.initiate = False
