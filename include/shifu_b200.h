@@ -417,6 +417,76 @@ void* sb_ensemble_stream(sb_ensemble_t* e);
 int sb_debug_ensemble_routes(sb_ensemble_t* e, char* out, int32_t cap);
 int sb_debug_ensemble_bytes(sb_ensemble_t* e, int64_t* out);
 
+/* ---- model performance: what `shifu eval` reports about a scored set (ROC AUC, PR AUC, KS, and the gains / ROC / PR /
+ * score-bucket lists), computed on the GPU from one radix sort of the scores.  Shifu's evaluator is not part of this
+ * project, so the quantities are defined here.
+ * Rows.  Each added row has a score s (fp32), a target y and a weight w.  y must be exactly 0 or 1 (-0 counts as 0); w must
+ * be finite and >= 0, and is 1 for every row when the caller passes no weights.  A row whose s is NaN, whose y is any other
+ * value, or whose w is negative, NaN or +-inf is invalid.  +-inf scores are valid; -0 and +0 are the same score.
+ * Thresholds.  t_1 > t_2 > ... > t_m are the distinct scores; run j is the set of rows with s = t_j.  p_j, n_j count its
+ * positives and negatives, wp_j, wn_j are their weight sums in fp64.  TP_j = sum_{i<=j} p_i, and likewise FP_j, WTP_j and
+ * WFP_j: the rows flagged at threshold t_j (s >= t_j).  P, N, Wp and Wn are the totals.  Every row counts once in the
+ * unweighted metrics, rows with w = 0 included.
+ * Metrics (sb_perf_summary):
+ *   auc    A2 / (2 P N), A2 = sum_j n_j (2 TP_{j-1} + p_j): the Mann-Whitney statistic with ties counted half.  A2 and
+ *          2 P N are exact int64 values and the result is one fp64 division of their fp64 values; up to 1.34e8 rows both
+ *          are below 2^53, so auc is the correctly rounded value of the exact fraction.
+ *   w_auc  sum_j wn_j (WTP_{j-1} + wp_j / 2) / (Wp Wn) in fp64.
+ *   ap     average precision (area under the PR curve): sum_j (p_j / P) TP_j / (TP_j + FP_j); w_ap the same with the
+ *          weighted values (a run with wp_j = 0 adds 0).
+ *   ks     max_j |TP_j N - FP_j P| / (P N): the numerator is exact in int64 (so is the argmax), and the value is one fp64
+ *          division of the two int64 values; ks_score is t_j of the first j (the highest threshold) that attains it.
+ *          w_ks / w_ks_score: the same in fp64 with the weighted values and the same tie-break.
+ *   A metric whose denominator is 0 is the quiet NaN (a single-class set; a zero weight total for the weighted ones), and
+ *   so is its ks_score.  An empty handle's summary has zero counts and NaN metrics.
+ * Guarantees: every result depends only on the rows and their arrival order, not on how they were split into adds, on
+ * whether the pointers were host or device, or on timing.  The sort is stable and every fp64 sum runs in a fixed order, so
+ * results are bit-identical on repeat.  WTP_j and WFP_j never decrease along the table.  At most 2^31 - 1 rows per handle.
+ * Memory: the handle holds each row's 32-bit key and payload, their sort double buffer and the run table: at most 53 device
+ * bytes per row of capacity (every score distinct), plus 13 MB (12 MB of it the host-row staging, allocated at the first add
+ * that reads host memory, and 48 bytes per level of the largest sb_perf_points call).  The capacity is allocated at the first add (or by reserve_rows), grows to
+ * max(rows held, 1.5 x capacity) rounded up to 4096 rows, and is freed by sb_perf_destroy.
+ * Errors: a null handle is SB_ERR_STATE.  Null scores or y, rows < 0, score_stride < 1, a row total over 2^31 - 1, an unknown
+ * axis, a level out of range, a NaN level or n < 0 are SB_ERR_INVALID, reported before any device work.  Invalid rows are
+ * counted on the device; while the handle holds any, sb_perf_summary_get, sb_perf_points and sb_debug_perf_runs return
+ * SB_ERR_INVALID with the three counts in the message, until sb_perf_reset. ---- */
+typedef struct sb_perf sb_perf_t;
+/* no device: SB_ERR_CUDA.  reserve_rows (0 .. 2^31 - 1) pre-sizes the row capacity. */
+int sb_perf_create(int device, int64_t reserve_rows, sb_perf_t** out);
+int sb_perf_destroy(sb_perf_t* p);
+/* forget every row (and every invalid-row count), keep the allocations */
+int sb_perf_reset(sb_perf_t* p);
+/* Append rows: scores[r * score_stride], y[r], w[r] (w NULL: 1).  With score_stride = 4 a caller can pass the mean column
+ * of sb_ensemble_score_device's stats; with stride K, member g's scores.  Host or device pointers on p's device.  When all
+ * of them are device pointers the call is queued on p's stream, after the work that was queued on after_stream (nullable,
+ * e.g. sb_model_stream(m)) at the time of the call, with no host synchronise.  Otherwise it returns once the rows have been
+ * read.  rows = 0 adds nothing.  The sort runs when a result is asked for after new rows arrived. */
+int sb_perf_add(sb_perf_t* p, const float* scores, int32_t score_stride, const float* y, const float* w, int64_t rows,
+                void* after_stream);
+typedef struct {
+  int64_t rows, pos, neg, n_distinct;   /* rows held, P, N, m */
+  double w_pos, w_neg;                  /* Wp, Wn */
+  double auc, w_auc, ap, w_ap, ks, w_ks;
+  float ks_score, w_ks_score;
+} sb_perf_summary;
+/* synchronous */
+int sb_perf_summary_get(sb_perf_t* p, sb_perf_summary* out);
+/* Operating points, one per level (synchronous).  For SB_PERF_ACTION_RATE, SB_PERF_RECALL and SB_PERF_FPR a level l lies in
+ * [0, 1]: the point is the first run j (the highest threshold) whose axis value reaches l, the axis values being
+ * (TP_j + FP_j) / (P + N), TP_j / P and FP_j / N as fp64 divisions (weighted != 0: (WTP_j + WFP_j) / (Wp + Wn), WTP_j / Wp,
+ * WFP_j / Wn); an axis whose denominator is 0 is SB_ERR_INVALID.  These give Shifu's gains, ROC and PR lists.  For
+ * SB_PERF_SCORE, l is any non-NaN value: the point is the last run with t_j >= l (the score-bucket list), or, when there is
+ * none, the empty point {threshold +inf, all counts 0}.  Each point is {t_j, TP_j, FP_j, WTP_j, WFP_j}. */
+enum { SB_PERF_ACTION_RATE = 0, SB_PERF_RECALL = 1, SB_PERF_FPR = 2, SB_PERF_SCORE = 3 };
+typedef struct { float threshold; int64_t tp, fp; double w_tp, w_fp; } sb_perf_point;
+int sb_perf_points(sb_perf_t* p, int32_t axis, int32_t weighted, const double* levels, int32_t n, sb_perf_point* out);
+int sb_perf_sync(sb_perf_t* p);
+void* sb_perf_stream(sb_perf_t* p);
+/* Test hooks: the first min(cap, m) rows of the run table (t_j and the cumulative TP / FP / WTP / WFP; any output may be
+ * NULL) with *n_runs = m, and the device bytes the handle holds. */
+int sb_debug_perf_runs(sb_perf_t* p, float* t, int64_t* tp, int64_t* fp, double* wtp, double* wfp, int64_t cap, int64_t* n_runs);
+int sb_debug_perf_bytes(sb_perf_t* p, int64_t* out);
+
 /* ---- text ingest: the per-cell float() loop of load_data (ssgd_monitor.py:387-419) on the GPU ----
  * text: the gunzipped, delim-separated lines (must end with '\n'), HOST memory.  col_map[c] gives the role of text
  * column c: >= 0 feature index (into X [rows, n_feat] row-major), SB_COL_TARGET, SB_COL_WEIGHT, SB_COL_SKIP; columns

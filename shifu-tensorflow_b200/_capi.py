@@ -80,6 +80,17 @@ class CellFlag(C.Structure):
 COL_SKIP, COL_TARGET, COL_WEIGHT = -1, -2, -3
 
 
+class PerfSummary(C.Structure):
+    _fields_ = [("rows", C.c_int64), ("pos", C.c_int64), ("neg", C.c_int64), ("n_distinct", C.c_int64),
+                ("w_pos", C.c_double), ("w_neg", C.c_double), ("auc", C.c_double), ("w_auc", C.c_double),
+                ("ap", C.c_double), ("w_ap", C.c_double), ("ks", C.c_double), ("w_ks", C.c_double),
+                ("ks_score", C.c_float), ("w_ks_score", C.c_float)]
+
+
+class PerfPoint(C.Structure):
+    _fields_ = [("threshold", C.c_float), ("tp", C.c_int64), ("fp", C.c_int64), ("w_tp", C.c_double), ("w_fp", C.c_double)]
+
+
 class ShifuB200Error(RuntimeError):
     def __init__(self, code: int, msg: str):
         super().__init__("[%d] %s" % (code, msg))
@@ -171,6 +182,16 @@ PROTOTYPES = {
     "sb_ensemble_stream": (C.c_void_p, [_vp]),
     "sb_debug_ensemble_routes": (C.c_int, [_vp, C.c_char_p, C.c_int32]),
     "sb_debug_ensemble_bytes": (C.c_int, [_vp, _P(C.c_int64)]),
+    "sb_perf_create": (C.c_int, [C.c_int, C.c_int64, _P(_vp)]),
+    "sb_perf_destroy": (C.c_int, [_vp]),
+    "sb_perf_reset": (C.c_int, [_vp]),
+    "sb_perf_add": (C.c_int, [_vp, _vp, C.c_int32, _vp, _vp, C.c_int64, _vp]),
+    "sb_perf_summary_get": (C.c_int, [_vp, _P(PerfSummary)]),
+    "sb_perf_points": (C.c_int, [_vp, C.c_int32, C.c_int32, _f64p, C.c_int32, _P(PerfPoint)]),
+    "sb_perf_sync": (C.c_int, [_vp]),
+    "sb_perf_stream": (C.c_void_p, [_vp]),
+    "sb_debug_perf_runs": (C.c_int, [_vp, _f32p, _P(C.c_int64), _P(C.c_int64), _f64p, _f64p, C.c_int64, _P(C.c_int64)]),
+    "sb_debug_perf_bytes": (C.c_int, [_vp, _P(C.c_int64)]),
     "sb_text_parse": (C.c_int, [_cp, C.c_int64, C.c_char, _P(C.c_int32), C.c_int32, C.c_int32, _f32p, _f32p, _f32p, C.c_int64,
                                 _P(C.c_int64), _P(CellFlag), C.c_int64, _P(C.c_int64), C.c_int]),
     "sb_text_parse_device": (C.c_int, [_cp, C.c_int64, C.c_char, _P(C.c_int32), C.c_int32, C.c_int32, _P(_f32p), _P(_f32p), _P(_f32p),
@@ -223,6 +244,9 @@ DEBUG_XINFO_WORDS, DEBUG_XWORK_WORDS = 24, 8
 DEBUG_MSTAT_WORDS = 6
 ENSEMBLE_MAX = 32       # SB_ENSEMBLE_MAX: members of one ensemble
 ENSEMBLE_STATS = ("mean", "max", "min", "median")     # sb_ensemble_score's stats columns
+PERF_ACTION_RATE, PERF_RECALL, PERF_FPR, PERF_SCORE = 0, 1, 2, 3
+PERF_AXES = {"action_rate": PERF_ACTION_RATE, "recall": PERF_RECALL, "fpr": PERF_FPR, "score": PERF_SCORE}
+PERF_MAX_ROWS = 2**31 - 1     # rows one performance handle holds
 SMALL_ROWS = 128        # score_rows.cuh: an fp32 model scores batches of up to this many rows in one launch
 # capi.cu model_from_desc: a model runs every scoring call in forwards of at most this many rows (its max_batch)
 MODEL_CHUNK_ROWS = {PREC_FP32: 16384, PREC_BF16: 65536, PREC_FP32_TC: 32768, PREC_BF16X2: 32768}
@@ -930,6 +954,92 @@ class Ensemble:
         """the device bytes the ensemble allocated (sb_debug_ensemble_bytes)"""
         out = C.c_int64()
         check(lib().sb_debug_ensemble_bytes(self._h, C.byref(out)))
+        return int(out.value)
+
+
+class Performance:
+    """Owns one sb_perf_t: exact ROC AUC, PR AUC (average precision), KS and operating points of scored rows, each
+    weighted and unweighted, computed on the GPU from one radix sort of the scores (include/shifu_b200.h defines them)."""
+
+    def __init__(self, device: int = 0, reserve_rows: int = 0):
+        h = C.c_void_p()
+        check(lib().sb_perf_create(device, int(reserve_rows), C.byref(h)))
+        self._h = h
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and self._h:
+            lib().sb_perf_destroy(self._h)
+            self._h = None
+
+    __del__ = close
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def add(self, scores, y, w=None, stride: int = 1):
+        """numpy rows: scores[r * stride] (float32), y[r] (0 / 1), w[r] (None: 1); returns once the rows have been read"""
+        y = _f32(y).reshape(-1)
+        s = _f32(scores).reshape(-1)
+        rows = y.size
+        if rows and s.size < (rows - 1) * stride + 1:
+            raise ValueError("scores must hold (rows - 1) * stride + 1 values")
+        if w is not None:
+            w = _f32(w).reshape(-1)
+            if w.size != rows:
+                raise ValueError("w must hold one weight per row")
+        check(lib().sb_perf_add(self._h, s.ctypes.data_as(_vp), int(stride), y.ctypes.data_as(_vp),
+                                None if w is None else w.ctypes.data_as(_vp), rows, None))
+
+    def add_device(self, ptr: int, y_ptr: int, w_ptr: Optional[int], rows: int, stride: int = 1,
+                   after_stream: Optional[int] = None):
+        """device pointers (ints): queued on the handle's stream behind the work queued on after_stream so far"""
+        check(lib().sb_perf_add(self._h, C.c_void_p(ptr), int(stride), C.c_void_p(y_ptr), C.c_void_p(w_ptr) if w_ptr else None,
+                                int(rows), C.c_void_p(after_stream) if after_stream else None))
+
+    def summary(self) -> dict:
+        s = PerfSummary()
+        check(lib().sb_perf_summary_get(self._h, C.byref(s)))
+        return {name: getattr(s, name) for name, _ in PerfSummary._fields_}
+
+    def points(self, axis, levels, weighted: bool = False) -> dict:
+        """-> {"threshold" float32, "tp", "fp" int64, "w_tp", "w_fp" float64}, one entry per level.  axis: "action_rate",
+        "recall", "fpr", "score" or its PERF_* number"""
+        ax = PERF_AXES[axis] if isinstance(axis, str) else int(axis)
+        lv = np.ascontiguousarray(levels, dtype=np.float64).reshape(-1)
+        out = (PerfPoint * max(lv.size, 1))()
+        check(lib().sb_perf_points(self._h, ax, 1 if weighted else 0, lv.ctypes.data_as(_f64p), lv.size, out))
+        a = np.frombuffer(out, dtype=np.dtype([("threshold", "<f4"), ("tp", "<i8"), ("fp", "<i8"), ("w_tp", "<f8"),
+                                               ("w_fp", "<f8")], align=True), count=lv.size)
+        return {name: a[name].copy() for name in a.dtype.names}
+
+    def reset(self):
+        check(lib().sb_perf_reset(self._h))
+
+    def sync(self):
+        check(lib().sb_perf_sync(self._h))
+
+    @property
+    def stream(self) -> int:
+        return int(lib().sb_perf_stream(self._h) or 0)
+
+    def runs(self) -> dict:
+        """the whole run table (sb_debug_perf_runs): t, tp, fp, w_tp, w_fp per distinct score, highest first"""
+        n = C.c_int64()
+        check(lib().sb_debug_perf_runs(self._h, None, None, None, None, None, 0, C.byref(n)))
+        m = int(n.value)
+        t, tp, fp = np.empty(m, np.float32), np.empty(m, np.int64), np.empty(m, np.int64)
+        wtp, wfp = np.empty(m, np.float64), np.empty(m, np.float64)
+        check(lib().sb_debug_perf_runs(self._h, _ptr(t), tp.ctypes.data_as(_P(C.c_int64)), fp.ctypes.data_as(_P(C.c_int64)),
+                                       wtp.ctypes.data_as(_f64p), wfp.ctypes.data_as(_f64p), m, C.byref(n)))
+        return {"t": t, "tp": tp, "fp": fp, "w_tp": wtp, "w_fp": wfp}
+
+    def device_bytes(self) -> int:
+        """the device bytes the handle holds (sb_debug_perf_bytes)"""
+        out = C.c_int64()
+        check(lib().sb_debug_perf_bytes(self._h, C.byref(out)))
         return int(out.value)
 
 

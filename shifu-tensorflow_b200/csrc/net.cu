@@ -141,8 +141,7 @@ int validate_desc(const sb_net_desc* d) {
   return SB_OK;
 }
 
-// makes `device` current if it is an sm_90 device
-static int check_device(int device, int* num_sms) {
+int check_device(int device, int* num_sms) {
   int n = 0;
   cudaError_t e = cudaGetDeviceCount(&n);
   SB_CHECK(e == cudaSuccess && n > 0, SB_ERR_CUDA, "no CUDA device available (%s); this library has no CPU fallback",

@@ -187,6 +187,8 @@ struct Net {
 };
 
 int validate_desc(const sb_net_desc* d);
+// makes `device` current if it is an sm_90 device (SB_ERR_CUDA when there is none)
+int check_device(int device, int* num_sms);
 // a wide+deep index matrix of n entries: each a one-hot column in [0, n_onehot) or -1 (missing); anything else is
 // SB_ERR_INVALID (a negative index other than -1 is not "missing", and a numpy caller would read it as a row from the end)
 int check_sparse_idx(const int32_t* idx, long long n, int n_onehot);

@@ -40,6 +40,44 @@ def check_phase_switch(name: str, value: Any) -> None:
                                    "honoured." % (name, type(value).__name__))
 
 
+# computePerformance's tables: Shifu's gains, ROC and PR lists, each the operating points at fixed levels of one axis
+PERF_TABLES = (("gains", "action_rate"), ("roc", "fpr"), ("pr", "recall"))
+
+
+def _perf_table(pts: dict, pos: float, neg: float, weighted: bool) -> dict:
+    """operating points -> the table entries with their ratios formed from the counts (NaN where a ratio's denominator is 0)"""
+    tp, fp = (pts["w_tp"], pts["w_fp"]) if weighted else (pts["tp"].astype(np.float64), pts["fp"].astype(np.float64))
+    with np.errstate(invalid="ignore", divide="ignore"):
+        precision = tp / (tp + fp)
+        out = dict(pts, recall=tp / pos, precision=precision, fpr=fp / neg, lift=precision / (pos / (pos + neg)))
+    return out
+
+
+def _performance(perf: capi.Performance, buckets: int, weighted: bool) -> dict:
+    """summary and tables of the rows added to `perf`: {"summary", "gains", "roc", "pr"} and, when weighted,
+    "weighted_gains" / "weighted_roc" / "weighted_pr"; a table whose axis is undefined (its total is 0) is None"""
+    if buckets < 1:
+        raise ValueError("buckets must be >= 1")
+    summ = perf.summary()
+    levels = np.arange(1, buckets + 1, dtype=np.float64) / buckets
+    out = {"summary": summ}
+    for w in ((False, True) if weighted else (False,)):
+        pos, neg = (summ["w_pos"], summ["w_neg"]) if w else (float(summ["pos"]), float(summ["neg"]))
+        for name, axis in PERF_TABLES:
+            den = {"action_rate": pos + neg, "recall": pos, "fpr": neg}[axis]
+            key = ("weighted_" if w else "") + name
+            out[key] = _perf_table(perf.points(axis, levels, weighted=w), pos, neg, w) if den > 0 else None
+    return out
+
+
+def _targets(targets, weights, rows: int):
+    y = np.asarray(targets, dtype=np.float64).astype(np.float32).reshape(-1)
+    w = None if weights is None else np.asarray(weights, dtype=np.float64).astype(np.float32).reshape(-1)
+    if y.size != rows or (w is not None and w.size != rows):
+        raise ValueError("one target (and weight) per row")
+    return y, w
+
+
 class TensorflowModel:
     def __init__(self, device: int = 0, precision: int = capi.PREC_FP32):
         self.properties: Dict[str, Any] = {}
@@ -144,6 +182,18 @@ class TensorflowModel:
         r = self._model.reason_codes(X, k, cols=columns, values=vals, order=order, scores=True)
         return {"columns": cl[r["pos"]], "deltas": r["d"], "scores": r["scores"]}
 
+    # -- new: how good the model is on a scored set (what `shifu eval` reports), computed on the GPU --
+    def computePerformance(self, rows, targets, weights=None, buckets=10) -> dict:
+        """Scores the rows as computeBatch does and evaluates them against targets (0 / 1) and weights (None: 1):
+        -> {"summary": AUC, average precision, KS, ... (include/shifu_b200.h, sb_perf_summary), "gains" / "roc" / "pr":
+        the operating points at action rate / FPR / recall (1 .. buckets) / buckets, each entry with its threshold,
+        counts, recall, precision, fpr and lift; with weights also "weighted_gains" / "weighted_roc" / "weighted_pr"}"""
+        scores = self.computeBatch(rows).astype(np.float32)
+        y, w = _targets(targets, weights, scores.size)
+        with capi.Performance(self._device, scores.size) as perf:
+            perf.add(scores, y, w)
+            return _performance(perf, buckets, w is not None)
+
     def releaseResource(self) -> None:
         """The reference never closes its bundle (TensorflowModel.java:175-176); here device memory is returned."""
         if self._model is not None:
@@ -205,6 +255,43 @@ class TensorflowEnsemble:
         out = {"scores": s.astype(np.float64)}
         out.update({name: t[:, i].astype(np.float64) for i, name in enumerate(capi.ENSEMBLE_STATS)})
         return out
+
+    # -- how good one column is on a scored set: score = "mean" | "max" | "min" | "median" or a member index --
+    def computePerformance(self, rows, targets, weights=None, buckets=10, score="mean") -> dict:
+        """TensorflowModel.computePerformance for one column of the ensemble's output.  The rows are scored in chunks
+        into device memory and the column is read there in place (sb_perf_add's score_stride): the scores never come
+        back to the host."""
+        e = self._check()
+        X = np.asarray(rows, dtype=np.float64).astype(np.float32)
+        if X.ndim != 2 or X.shape[1] != e.n_features:
+            raise ValueError("rows must be [rows, %d]" % e.n_features)
+        n = X.shape[0]
+        y, w = _targets(targets, weights, n)
+        if isinstance(score, str):
+            if score not in capi.ENSEMBLE_STATS:
+                raise ValueError("score must be one of %s or a member index" % (capi.ENSEMBLE_STATS,))
+            col, stride = capi.ENSEMBLE_STATS.index(score), 4
+        else:
+            col, stride = int(score), e.k
+            if not 0 <= col < e.k:
+                raise ValueError("member index %d outside [0, %d)" % (col, e.k))
+        chunk = min(max(n, 1), 1 << 20)
+        buf = capi.DeviceArray.empty((chunk, stride), self._device)
+        try:
+            base = capi.C.cast(buf.ptr, capi.C.c_void_p).value
+            with capi.Performance(self._device, n) as perf:
+                for r0 in range(0, n, chunk):
+                    c = min(chunk, n - r0)
+                    xc = np.ascontiguousarray(X[r0:r0 + c])
+                    out = capi.C.c_void_p(base)
+                    capi.check(capi.lib().sb_ensemble_score(e._h, xc.ctypes.data_as(capi.C.c_void_p), c,
+                                                            None if isinstance(score, str) else out,
+                                                            out if isinstance(score, str) else None))
+                    perf.add_device(base + 4 * col, y[r0:r0 + c].ctypes.data, None if w is None else w[r0:r0 + c].ctypes.data,
+                                    c, stride=stride)
+                return _performance(perf, buckets, w is not None)
+        finally:
+            buf.free()
 
     def releaseResource(self) -> None:
         if self._ensemble is not None:
