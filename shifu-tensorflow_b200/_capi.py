@@ -248,7 +248,7 @@ PERF_ACTION_RATE, PERF_RECALL, PERF_FPR, PERF_SCORE = 0, 1, 2, 3
 PERF_AXES = {"action_rate": PERF_ACTION_RATE, "recall": PERF_RECALL, "fpr": PERF_FPR, "score": PERF_SCORE}
 PERF_MAX_ROWS = 2**31 - 1     # rows one performance handle holds
 SMALL_ROWS = 128        # score_rows.cuh: an fp32 model scores batches of up to this many rows in one launch
-# capi.cu model_from_desc: a model runs every scoring call in forwards of at most this many rows (its max_batch)
+# score.cu model_chunk_rows: a model runs every scoring call in forwards of at most this many rows (its max_batch)
 MODEL_CHUNK_ROWS = {PREC_FP32: 16384, PREC_BF16: 65536, PREC_FP32_TC: 32768, PREC_BF16X2: 32768}
 
 

@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libshifu_b200.so")
-SOURCES = ["net.cu", "capi.cu", "text_ingest.cu", "savedmodel.cpp"]
+SOURCES = ["net.cu", "capi.cu", "score.cu", "perf.cu", "text_ingest.cu", "savedmodel.cpp"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function",

@@ -1,24 +1,16 @@
-// extern "C" surface of libshifu_b200.so: trainer, scorer, rendezvous, step-trace hook (the kernel-level test hooks are
-// in net.cu).
+// extern "C" surface of libshifu_b200.so: the trainer, its step-trace and exchange test hooks, and the library-wide calls
+// (version, devices, host allocation, NCCL id).  The scorers are in score.cu, the performance handle in perf.cu, and the
+// kernel-level test hooks in net.cu.
 // See include/shifu_b200.h for the contract and the reference call each entry point replaces.
 #include <math.h>
 #include <stdlib.h>
 #include <cmath>
 #include <string.h>
 #include <algorithm>
-#include <atomic>
-#include <chrono>
-#include <condition_variable>
-#include <functional>
-#include <limits>
 #include <memory>
 #include <random>
-#include "ensemble.cuh"
 #include "net.cuh"
-#include "perf.cuh"
 #include "savedmodel.h"
-#include "score_rows.cuh"
-#include "sensitivity.cuh"
 #include "xchg_p2p.cuh"
 
 using namespace sb;
@@ -37,16 +29,6 @@ struct GraphKey {
   bool operator<(const GraphKey& o) const {
     return std::tie(rows, kind, feed, steps, set) < std::tie(o.rows, o.kind, o.feed, o.steps, o.set);
   }
-};
-
-// One step's batch: everything set_batch_kernel reads besides the update's scalars (write_desc)
-struct Batch {
-  Feed feed = Feed::HOST;
-  const float *X = nullptr, *y = nullptr, *w = nullptr;
-  int row0 = 0;                     // RESIDENT: first row in the resident set
-  const int* nz_prefix = nullptr;   // RESIDENT: n_nz is published from the set's prefix counts
-  const int* order = nullptr;       // ORDERED: the batch's slice of the row order
-  int rows = 0;
 };
 
 struct sb_trainer {
@@ -249,25 +231,6 @@ static float begin_update(sb_trainer* t) {
   ++t->global_step;
   ++t->epoch;
   return lr_for_step(t, t->global_step);
-}
-
-// The only writer of a step descriptor: batch `b` (nullptr: an update without a batch), the update's scalars and the
-// step's slot in the loss history, into slot `in` on stream `st`
-static int write_desc(cudaStream_t st, const StepIn& in, const Batch* b, float lr_t, float gscale, unsigned int epoch,
-                      float2* hist) {
-  static const Batch none{};
-  const Batch& x = b ? *b : none;
-  return launch_kernel(set_batch_kernel, dim3(1), dim3(1), 0, st, false, in.desc, x.X, x.y, x.w, lr_t, gscale, epoch, x.row0,
-                       x.nz_prefix, x.rows, in.scal, hist, x.order);
-}
-
-// a batch of fp32 rows on the device (the staging area, or the fp32 resident set); w == nullptr weighs every row 1
-static Batch host_batch(const Net& n, const float* X, const float* y, const float* w, int rows, Feed feed = Feed::HOST) {
-  Batch b;
-  b.feed = feed;
-  b.X = X; b.y = y; b.w = w ? w : n.ones;
-  b.rows = rows;
-  return b;
 }
 
 // rows [off, off + rows) of the resident set, through the row order if one is set, for step k of a graph.  step >= 0
@@ -826,8 +789,7 @@ static int run_step(sb_trainer* t, const Batch& b, int kind) {
 }
 
 // The forward of one batch on the main stream: its descriptor into slot `in`, the feed's first kernel, the hidden layers and
-// the output layer (do_loss: + the loss sum into in.scal), scores to yhat_dst (nullable).  t: the trainer of an ORDERED
-// batch (the scorer has none).
+// the output layer (do_loss: + the loss sum into in.scal), scores to yhat_dst (nullable).
 static int enqueue_forward(Net& n, sb_trainer* t, StepIn in, const Batch& b, unsigned int epoch, bool do_loss, float* yhat_dst) {
   in.feed = b.feed;
   SB_TRY(write_desc(n.stream, in, &b, 0.f, 1.f, epoch, nullptr));
@@ -841,7 +803,8 @@ static int enqueue_forward(Net& n, sb_trainer* t, StepIn in, const Batch& b, uns
 // (Slot set 0: these host-driven paths are not captured.  A step queues its descriptor writes ahead of its graph on the
 // main stream, and every forward path synchronises that stream before it returns, so no descriptor prefetch overlaps them.)
 template <typename Stage>
-static int forward_chunks(Net& n, int64_t rows, Stage stage, float* out, double* loss_sum, double* nnz) {
+static int forward_chunks(sb_trainer* t, int64_t rows, Stage stage, float* out, double* loss_sum, double* nnz) {
+  Net& n = t->net;
   SB_CUDA(cudaSetDevice(n.device));
   const StepIn in{n.desc, n.scal};
   float h[SCAL_COUNT];
@@ -849,7 +812,7 @@ static int forward_chunks(Net& n, int64_t rows, Stage stage, float* out, double*
     const int c = static_cast<int>(rows - r0 < n.max_batch ? rows - r0 : n.max_batch);
     Batch b;
     SB_TRY(stage(r0, c, &b));
-    SB_TRY(enqueue_forward(n, nullptr, in, b, 0, loss_sum != nullptr, n.yhat));
+    SB_TRY(enqueue_forward(n, t, in, b, 0, loss_sum != nullptr, n.yhat));
     if (out) SB_CUDA(cudaMemcpyAsync(out + r0, n.yhat, sizeof(float) * c, cudaMemcpyDefault, n.stream));
     if (loss_sum) SB_CUDA(cudaMemcpyAsync(h, in.scal, sizeof(h), cudaMemcpyDeviceToHost, n.stream));
     SB_CUDA(cudaStreamSynchronize(n.stream));
@@ -889,15 +852,6 @@ static int finish_loss(sb_trainer* t, float* loss_out) {
     *loss_out = nnz > 0.f ? t->h_scal[SCAL_LOSS_SUM] / nnz : 0.f;
   }
   return SB_OK;
-}
-
-// X / y / w of load_dataset, eval_loss and predict may be HOST or DEVICE pointers (unified addressing: the copies use
-// cudaMemcpyDefault); the GPU text ingest hands over device arrays so that the parsed set never visits the host
-static bool is_device_ptr(const void* p) {
-  if (!p) return false;
-  cudaPointerAttributes at;
-  if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return false; }
-  return at.type == cudaMemoryTypeDevice;
 }
 
 static int stage_host_batch(sb_trainer* t, const float* X, const float* y, const float* w, int rows) {
@@ -1034,7 +988,7 @@ int sb_trainer_create(const sb_net_desc* desc, int device, const void* nccl_id, 
   SB_TRY(t->net.init(desc, device, true));
   t->bufs[0].Xb = t->net.Xb;
   // see Net::init: no L1 / shared-memory re-partition between the kernels of a step
-  cudaFuncSetAttribute(set_batch_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  write_desc_max_shared();
   for (auto k : optimizer_kernels) cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   cudaFuncSetAttribute(axpy_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   Net& n = t->net;
@@ -1129,7 +1083,7 @@ static int preload_exchange_kernels() {
   for (const auto& row : xchg_ll_kernels)
     for (auto k : row) SB_CUDA(cudaFuncGetAttributes(&a, k));
   SB_CUDA(cudaFuncGetAttributes(&a, gather_master_kernel));
-  SB_CUDA(cudaFuncGetAttributes(&a, set_batch_kernel));
+  SB_TRY(write_desc_preload());
   SB_CUDA(cudaFuncGetAttributes(&a, scale_kernel));
   SB_CUDA(cudaFuncGetAttributes(&a, zero_f32_kernel));
   SB_CUDA(cudaFuncGetAttributes(&a, axpy_kernel));
@@ -1406,9 +1360,10 @@ int sb_trainer_step_sparse(sb_trainer_t* t, const float* Xd, const int32_t* idx,
 }
 
 // forward (+ loss: y != nullptr) over any number of sparse rows; out / loss accumulators nullable
-static int forward_sparse(Net& n, const float* Xd, const int32_t* idx, const float* y, const float* w, int64_t rows, float* out,
-                          double* loss_sum, double* nnz) {
-  return forward_chunks(n, rows, [&](int64_t r0, int c, Batch* b) -> int {
+static int forward_sparse(sb_trainer* t, const float* Xd, const int32_t* idx, const float* y, const float* w, int64_t rows,
+                          float* out, double* loss_sum, double* nnz) {
+  Net& n = t->net;
+  return forward_chunks(t, rows, [&](int64_t r0, int c, Batch* b) -> int {
     SB_TRY(stage_sparse_batch(n, Xd + r0 * n.n_dense, idx + r0 * n.n_cat, y ? y + r0 : nullptr, (y && w) ? w + r0 : nullptr, c));
     *b = host_batch(n, n.stX, n.stY, (y && w) ? n.stW : nullptr, c, Feed::SPARSE);
     return SB_OK;
@@ -1417,14 +1372,14 @@ static int forward_sparse(Net& n, const float* Xd, const int32_t* idx, const flo
 
 int sb_trainer_predict_sparse(sb_trainer_t* t, const float* Xd, const int32_t* idx, int64_t rows, float* out) {
   SB_CHECK(t && out, SB_ERR_INVALID, "null argument");
-  return forward_sparse(t->net, Xd, idx, nullptr, nullptr, rows, out, nullptr, nullptr);
+  return forward_sparse(t, Xd, idx, nullptr, nullptr, rows, out, nullptr, nullptr);
 }
 
 int sb_trainer_eval_loss_sparse(sb_trainer_t* t, const float* Xd, const int32_t* idx, const float* y, const float* w, int64_t rows,
                                 float* loss_out) {
   SB_CHECK(t && y && loss_out && rows > 0, SB_ERR_INVALID, "bad argument");
   double ls = 0, nz = 0;
-  SB_TRY(forward_sparse(t->net, Xd, idx, y, w, rows, nullptr, &ls, &nz));
+  SB_TRY(forward_sparse(t, Xd, idx, y, w, rows, nullptr, &ls, &nz));
   *loss_out = nz > 0 ? static_cast<float>(ls / nz) : 0.f;
   return SB_OK;
 }
@@ -1526,6 +1481,8 @@ static int place_dataset(sb_trainer* t, int64_t n_rows, size_t x_bytes, size_t w
   return SB_OK;
 }
 
+// X / y / w of load_dataset, eval_loss and predict may be HOST or DEVICE pointers (unified addressing: the copies use
+// cudaMemcpyDefault); the GPU text ingest hands over device arrays so that the parsed set never visits the host
 int sb_trainer_load_dataset(sb_trainer_t* t, const float* X, const float* y, const float* w, int64_t n_rows) {
   SB_CHECK(t && X && y, SB_ERR_INVALID, "null argument");
   SB_CHECK(n_rows > 0 && n_rows < (1ll << 31), SB_ERR_INVALID, "n_rows must be in (0, 2^31)");
@@ -1597,7 +1554,7 @@ int sb_trainer_load_dataset(sb_trainer_t* t, const float* X, const float* y, con
     prefix[0] = 0;
     std::vector<float> w_host;
     const float* wh = w;
-    if (is_device_ptr(w)) {      // 4 bytes per row: the only part of a device-resident set the host looks at
+    if (ptr_device(w) >= 0) {    // 4 bytes per row: the only part of a device-resident set the host looks at
       w_host.resize(static_cast<size_t>(n_rows));
       SB_CUDA(cudaMemcpy(w_host.data(), w, sizeof(float) * n_rows, cudaMemcpyDeviceToHost));
       wh = w_host.data();
@@ -1793,9 +1750,10 @@ int sb_trainer_set_row_order(sb_trainer_t* t, const int64_t* rows, int64_t n) {
 }
 
 // forward (+ loss: y != nullptr) over any number of host or device rows; out / loss accumulators nullable
-static int forward_rows(Net& n, const float* X, const float* y, const float* w, int64_t rows, float* out, double* loss_sum,
-                        double* nnz) {
-  return forward_chunks(n, rows, [&](int64_t r0, int c, Batch* b) -> int {
+static int forward_rows(sb_trainer* t, const float* X, const float* y, const float* w, int64_t rows, float* out,
+                        double* loss_sum, double* nnz) {
+  Net& n = t->net;
+  return forward_chunks(t, rows, [&](int64_t r0, int c, Batch* b) -> int {
     SB_CUDA(cudaMemcpyAsync(n.stX, X + r0 * n.F, sizeof(float) * c * static_cast<size_t>(n.F), cudaMemcpyDefault, n.stream));
     if (y) {
       SB_CUDA(cudaMemcpyAsync(n.stY, y + r0, sizeof(float) * c, cudaMemcpyDefault, n.stream));
@@ -1810,7 +1768,7 @@ int sb_trainer_eval_loss(sb_trainer_t* t, const float* X, const float* y, const 
   SB_CHECK(t && X && y && loss_out, SB_ERR_INVALID, "null argument");
   SB_CHECK(rows > 0, SB_ERR_INVALID, "rows must be > 0");
   double ls = 0, nz = 0;
-  SB_TRY(forward_rows(t->net, X, y, w, rows, nullptr, &ls, &nz));
+  SB_TRY(forward_rows(t, X, y, w, rows, nullptr, &ls, &nz));
   *loss_out = nz > 0 ? static_cast<float>(ls / nz) : 0.f;
   return SB_OK;
 }
@@ -1818,7 +1776,7 @@ int sb_trainer_eval_loss(sb_trainer_t* t, const float* X, const float* y, const 
 int sb_trainer_predict(sb_trainer_t* t, const float* X, int64_t rows, float* out) {
   SB_CHECK(t && X && out, SB_ERR_INVALID, "null argument");
   SB_CHECK(rows > 0, SB_ERR_INVALID, "rows must be > 0");
-  return forward_rows(t->net, X, nullptr, nullptr, rows, out, nullptr, nullptr);
+  return forward_rows(t, X, nullptr, nullptr, rows, out, nullptr, nullptr);
 }
 
 // ---- checkpoint: flat blob {magic, version, n_params, global_step, optimizer, theta, s1, s2} ----
@@ -1878,1235 +1836,6 @@ int sb_trainer_export_savedmodel(sb_trainer_t* t, const char* export_dir) {
   std::vector<float> flat(static_cast<size_t>(t->net.n_params));
   SB_TRY(sb_trainer_get_params(t, flat.data(), t->net.n_params));
   return sb_savedmodel_write(export_dir, &t->desc, flat.data(), t->net.n_params);
-}
-
-// ================================================================================================
-// scorer
-// ================================================================================================
-}  // extern "C"
-
-// compute() (sb_model_score_row_f64) callers on one handle share device batches of up to MB_ROWS rows: the tensor-core
-// kernels' tile height.  plan_gemm / plan_gemm_pp depend on M only through ceil(M / 128) and the grid size, so every GEMM
-// plan of <= 128 rows is the one-row plan, and rows never interact in the forward GEMMs, the load or the output kernels:
-// a row's score does not depend on which rows shared its batch.
-static const int MB_ROWS = 128;
-static_assert(SMALL_ROWS >= MB_ROWS, "an fp32 micro-batch is one score_rows_kernel launch");
-
-struct RowWaiter {            // one compute() call, on its caller's stack
-  float* out = nullptr;       // its result, RowQueue::words floats
-  int status = SB_OK;
-  std::string err;            // the leader's error text, re-raised in the caller's thread
-  bool done = false;
-};
-
-// The compute() queue of a model (one score per row) or an ensemble (K scores and four statistics per row): concurrent
-// callers on one handle share device batches of up to MB_ROWS rows.  No thread of its own: the first caller that finds
-// no batch in flight leads, running every queued row in batches until the queue is empty; the others wait for their
-// result.  A batch is run by the owner's run(b, rows): the rows of stage[b] -> res[b] [rows, words].
-struct RowQueue {
-  using Run = std::function<int(int, int)>;
-  int F = 0, words = 1;
-  std::mutex q_mu;
-  std::condition_variable q_cv;
-  float* stage[2] = {nullptr, nullptr};       // pinned [MB_ROWS, F]: one buffer fills while the other's batch runs
-  float* res[2] = {nullptr, nullptr};         // pinned [MB_ROWS, words]
-  RowWaiter* waiters[2][MB_ROWS] = {};
-  int fill[2] = {0, 0};       // rows queued in a buffer
-  int writers[2] = {0, 0};    // callers still converting their row into it
-  int cur = 0;                // the buffer that takes new rows
-  bool leading = false;
-  int hold_k = 0, hold_ms = 0;                // sb_debug_model_hold
-  std::atomic<long long> batches{0}, rows{0}, max_fill{0};   // since creation: batches run, their rows, the largest
-
-  int alloc(int F_, int words_) {
-    F = F_; words = words_;
-    for (int b = 0; b < 2; ++b) {
-      SB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&stage[b]), sizeof(float) * MB_ROWS * F, cudaHostAllocDefault));
-      SB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&res[b]), sizeof(float) * MB_ROWS * words, cudaHostAllocDefault));
-    }
-    return SB_OK;
-  }
-  ~RowQueue() {
-    for (int b = 0; b < 2; ++b) {
-      if (stage[b]) cudaFreeHost(stage[b]);
-      if (res[b]) cudaFreeHost(res[b]);
-    }
-  }
-
-  // one row of F doubles (cast to float as TensorflowModel.java:64-68 casts it) -> out[words]
-  int submit(const double* row, float* out, const Run& run) {
-    RowWaiter me;
-    me.out = out;
-    std::unique_lock<std::mutex> lk(q_mu);
-    q_cv.wait(lk, [&] { return fill[cur] < MB_ROWS; });
-    const int b = cur, slot = fill[b]++;
-    waiters[b][slot] = &me;
-    ++writers[b];
-    lk.unlock();
-    float* f = stage[b] + static_cast<size_t>(slot) * F;
-    for (int i = 0; i < F; ++i) f[i] = static_cast<float>(row[i]);
-    lk.lock();
-    if (--writers[b] == 0) q_cv.notify_all();
-    while (!me.done) {
-      if (!leading) {           // no batch in flight: lead (a lone caller is scored at once)
-        leading = true;
-        lead(lk, run);
-        leading = false;
-        q_cv.notify_all();
-      } else {
-        q_cv.wait(lk);
-      }
-    }
-    lk.unlock();
-    if (me.status != SB_OK) return set_error(me.status, "%s", me.err.c_str());
-    return SB_OK;
-  }
-
- private:
-  // The leader (q_mu held through lk): runs the queued rows in batches until the queue is empty, and publishes each
-  // caller's result and status.
-  void lead(std::unique_lock<std::mutex>& lk, const Run& run) {
-    while (fill[cur] > 0) {
-      if (hold_k > 0) {         // sb_debug_model_hold: this batch waits for hold_k rows or the timeout
-        const int k = hold_k;
-        hold_k = 0;
-        q_cv.wait_until(lk, std::chrono::steady_clock::now() + std::chrono::milliseconds(hold_ms), [&] { return fill[cur] >= k; });
-      }
-      const int b = cur;
-      q_cv.wait(lk, [&] { return writers[b] == 0; });
-      const int n = fill[b];
-      cur ^= 1;                 // new rows go to the other buffer (empty: its batch was published before this one began)
-      q_cv.notify_all();
-      lk.unlock();
-      const int s = run(b, n);
-      const std::string err = s == SB_OK ? std::string() : last_error_ref();
-      lk.lock();
-      for (int i = 0; i < n; ++i) {
-        RowWaiter* w = waiters[b][i];
-        w->status = s;
-        if (s == SB_OK) memcpy(w->out, res[b] + static_cast<size_t>(i) * words, sizeof(float) * words);
-        else w->err = err;
-        w->done = true;
-      }
-      fill[b] = 0;
-      ++batches;
-      rows += n;
-      if (n > max_fill) max_fill = n;
-      q_cv.notify_all();
-    }
-  }
-};
-
-struct sb_model {
-  Net net;
-  sb_net_desc desc;
-  std::mutex mu;              // device work on the model's stream
-  DevBuf<float> sr_act;       // fp32: score_rows_kernel's two activation buffers [SMALL_ROWS, sr_ld]
-  int sr_ld = 0;
-  RowQueue q;                 // compute() (not allocated for an ensemble's members)
-  cudaGraphExec_t mb_graph = nullptr;         // tensor-core modes: the forward of MB_ROWS staged rows
-  std::atomic<long long> st[SB_DEBUG_MSTAT_WORDS] = {};   // (the first three words are the queue's)
-  std::string routes;         // the launches of the last model_forward, "+"-joined (sb_debug_model_routes; guarded by mu)
-  // sb_model_sensitivity's buffers (guarded by mu), allocated by its first call and grown when a call needs more
-  DevBuf<float> sens_z;       // layer 0's pre-activations of a row chunk [R, ld_out_0]
-  DevBuf<double> sens_acc;    // running sums [list position][w d^2, w d], then sum w
-  DevBuf<int> sens_cols;      // the column list and its values
-  DevBuf<float> sens_vals;
-  DevBuf<float> sens_d;       // the deltas of one piece [R, piece columns] (max_batch)
-  size_t sens_z_n = 0, sens_list_n = 0;
-  // sb_model_reason_codes' running top k of a row chunk [R, k], best first (guarded by mu; allocated and grown as above)
-  DevBuf<float> reason_d;
-  DevBuf<int> reason_pos;
-  size_t reason_d_n = 0, reason_pos_n = 0;
-  ~sb_model() {
-    if (!net.stream) return;
-    cudaSetDevice(net.device);
-    cudaStreamSynchronize(net.stream);
-    if (mb_graph) cudaGraphExecDestroy(mb_graph);
-  }
-};
-
-static const int MODEL_CHUNK_ROWS = 16384;        // fp32 parity mode
-static const int MODEL_CHUNK_ROWS_BF16 = 65536;   // bf16: bigger GEMMs per launch (workspace ~0.8 GB at 2000 cols)
-
-static int model_chunk_rows(int precision) {
-  return precision == SB_PREC_FP32 ? MODEL_CHUNK_ROWS : (precision == SB_PREC_BF16 ? MODEL_CHUNK_ROWS_BF16 : MODEL_CHUNK_ROWS_BF16 / 2);
-}
-
-// A model, or (member) an ensemble's member: no compute() queue, and with input_from set it runs on that net's stream and
-// reads its input staging.
-static int model_from_desc(sb_net_desc d, const float* flat, int64_t n, int device, sb_model_t** out, bool member = false,
-                           const Net* input_from = nullptr) {
-  d.max_batch = model_chunk_rows(d.precision);
-  std::unique_ptr<sb_model> m(new sb_model());
-  m->desc = d;
-  Net& net = m->net;
-  net.input_from = input_from;
-  SB_TRY(net.init(&d, device, false));
-  SB_CHECK(n == net.n_params, SB_ERR_INVALID, "expected %lld params, got %lld", (long long)net.n_params, (long long)n);
-  SB_CUDA(cudaMemcpyAsync(net.theta, flat, sizeof(float) * n, cudaMemcpyHostToDevice, net.stream));
-  SB_TRY(net.refresh_shadows());
-  if (!net.tc()) {
-    int widest = 1;
-    for (int l = 0; l < net.L; ++l) widest = std::max(widest, net.layers[l].out);
-    m->sr_ld = round_up(widest, 4);
-    SB_TRY(m->sr_act.alloc(static_cast<size_t>(2) * SMALL_ROWS * m->sr_ld));
-    SB_TRY(set_max_smem(score_rows_kernel, SR_SMEM));
-  }
-  if (!member) SB_TRY(m->q.alloc(net.F, 1));
-  SB_CUDA(cudaStreamSynchronize(net.stream));
-  *out = m.release();
-  return SB_OK;
-}
-
-// The forward of `rows` (<= max_batch) device rows dX -> scores dOut (device), queued on the model's stream.  An fp32 batch
-// of <= SMALL_ROWS rows is one score_rows_kernel launch; any other batch runs the layer-by-layer launches.  Both give the
-// same bits.
-static int enqueue_model_forward(sb_model* m, const float* dX, int rows, float* dOut) {
-  Net& n = m->net;
-  if (!n.tc() && rows <= SMALL_ROWS) {
-    ScoreRowsParams p = {};
-    p.rows = rows; p.F = n.F; p.L = n.L;
-    p.X = dX; p.theta = n.theta;
-    p.act[0] = m->sr_act.p; p.act[1] = m->sr_act.p + static_cast<size_t>(SMALL_ROWS) * m->sr_ld; p.ld_act = m->sr_ld;
-    p.yhat = dOut;
-    for (int l = 0; l < n.L; ++l) { p.out[l] = n.layers[l].out; p.act_fn[l] = n.layers[l].act; }
-    for (int l = 0; l <= n.L; ++l) { p.w_off[l] = n.layers[l].w_off; p.b_off[l] = n.layers[l].b_off; }
-    const int clusters = (rows + SR_ROWS - 1) / SR_ROWS;
-    score_rows_kernel<<<clusters * SR_CLUSTER, SR_THREADS, SR_SMEM, n.stream>>>(p);
-    SB_CUDA(cudaGetLastError());
-    n.mark("score_rows");
-    ++m->st[SB_DEBUG_MSTAT_SMALL_LAUNCHES];
-    return SB_OK;
-  }
-  return enqueue_forward(n, nullptr, StepIn{n.desc, n.scal}, host_batch(n, dX, nullptr, nullptr, rows), 0, false, dOut);
-}
-
-// Every scoring path of a model comes through here; its launches are kept for sb_debug_model_routes.  Called with m->mu
-// held.
-static int model_forward(sb_model* m, const float* dX, int rows, float* dOut) {
-  Net& n = m->net;
-  m->routes.clear();
-  n.marks = &m->routes;
-  const int s = enqueue_model_forward(m, dX, rows, dOut);
-  n.marks = nullptr;
-  return s;
-}
-
-// tensor-core modes: the forward of one compute() batch (fwd(), MB_ROWS rows of the staging area) captured once into
-// *graph, so a micro-batch is one launch
-template <typename Fwd>
-static int capture_micro_batch(cudaStream_t st, const Fwd& fwd, cudaGraphExec_t* graph) {
-  cudaGraph_t g = nullptr;
-  SB_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-  const int s = fwd();
-  const cudaError_t e = cudaStreamEndCapture(st, &g);
-  if (s != SB_OK) { if (g) cudaGraphDestroy(g); return s; }
-  SB_CHECK(e == cudaSuccess, SB_ERR_CUDA, "cudaStreamEndCapture failed: %s", cudaGetErrorString(e));
-  const cudaError_t ei = cudaGraphInstantiate(graph, g, 0);
-  cudaGraphDestroy(g);
-  SB_CHECK(ei == cudaSuccess, SB_ERR_CUDA, "cudaGraphInstantiate failed: %s", cudaGetErrorString(ei));
-  return SB_OK;
-}
-
-// one compute() batch: rows of staging buffer b -> m->q.res[b].  A tensor-core batch runs at MB_ROWS rows, its pad rows
-// zero-filled; only the real rows are copied back.
-static int run_micro_batch(sb_model* m, int b, int rows) {
-  std::lock_guard<std::mutex> lk(m->mu);
-  Net& n = m->net;
-  SB_CUDA(cudaSetDevice(n.device));
-  if (n.tc() && !m->mb_graph)
-    SB_TRY(capture_micro_batch(n.stream, [&] { return model_forward(m, n.stX, MB_ROWS, n.yhat); }, &m->mb_graph));
-  const size_t row_bytes = sizeof(float) * n.F;
-  SB_CUDA(cudaMemcpyAsync(n.stX, m->q.stage[b], row_bytes * rows, cudaMemcpyHostToDevice, n.stream));
-  if (n.tc()) {
-    if (rows < MB_ROWS) SB_CUDA(cudaMemsetAsync(n.stX + static_cast<size_t>(rows) * n.F, 0, row_bytes * (MB_ROWS - rows), n.stream));
-    SB_CUDA(cudaGraphLaunch(m->mb_graph, n.stream));
-    ++m->st[SB_DEBUG_MSTAT_GRAPH];
-  } else {
-    SB_TRY(model_forward(m, n.stX, rows, n.yhat));
-    ++m->st[SB_DEBUG_MSTAT_SMALL];
-  }
-  SB_CUDA(cudaMemcpyAsync(m->q.res[b], n.yhat, sizeof(float) * rows, cudaMemcpyDeviceToHost, n.stream));
-  SB_CUDA(cudaStreamSynchronize(n.stream));
-  return SB_OK;
-}
-
-// A SavedModel directory -> the topology (at `precision`) and flat parameters of a scoring model; host work only.  The
-// null checks mirror TensorflowModel.init (TensorflowModel.java:147-166).
-static int read_scoring_model(const char* saved_model_dir, const char* input_name, const char* output_name, const char* tag,
-                              int precision, sb_net_desc* d, std::vector<float>* flat) {
-  SB_CHECK(saved_model_dir && saved_model_dir[0], SB_ERR_INVALID, "Model path is null");
-  SB_CHECK(input_name && input_name[0], SB_ERR_INVALID, "Input names is null");
-  SB_CHECK(output_name && output_name[0], SB_ERR_INVALID, "Output names is null");
-  SB_CHECK(tag && tag[0], SB_ERR_INVALID, "Tags is null");
-  memset(d, 0, sizeof(*d));
-  int32_t out_act = SB_ACT_SIGMOID;
-  int64_t np = 0;
-  SB_TRY(sb_savedmodel_read(saved_model_dir, input_name, output_name, tag, d, &out_act, nullptr, 0, &np));
-  SB_CHECK(out_act == SB_ACT_SIGMOID, SB_ERR_FORMAT, "output layer must be a sigmoid unit");
-  flat->assign(static_cast<size_t>(np), 0.f);
-  SB_TRY(sb_savedmodel_read(saved_model_dir, input_name, output_name, tag, d, &out_act, flat->data(), np, &np));
-  d->precision = precision;
-  d->max_batch = 1;
-  return SB_OK;
-}
-
-extern "C" {
-
-int sb_model_create(const sb_net_desc* desc, const float* flat_params, int64_t n, int device, sb_model_t** out) {
-  SB_CHECK(out && flat_params, SB_ERR_INVALID, "null argument");
-  *out = nullptr;
-  sb_net_desc d = *desc;
-  if (d.max_batch <= 0) d.max_batch = 1;
-  SB_TRY(validate_desc(&d));
-  return model_from_desc(d, flat_params, n, device, out);
-}
-
-int sb_model_load(const char* saved_model_dir, const char* input_name, const char* output_name, const char* tag,
-                  int device, int precision, sb_model_t** out) {
-  SB_CHECK(out, SB_ERR_INVALID, "out is null");
-  *out = nullptr;
-  sb_net_desc d;
-  std::vector<float> flat;
-  SB_TRY(read_scoring_model(saved_model_dir, input_name, output_name, tag, precision, &d, &flat));
-  return model_from_desc(d, flat.data(), static_cast<int64_t>(flat.size()), device, out);
-}
-
-int sb_model_destroy(sb_model_t* m) {
-  delete m;
-  return SB_OK;
-}
-
-int32_t sb_model_n_features(const sb_model_t* m) { return m ? m->net.F : 0; }
-int32_t sb_model_n_layers(const sb_model_t* m) { return m ? m->net.L + 1 : 0; }
-
-int sb_model_score(sb_model_t* m, const float* X, int64_t rows, float* out) {
-  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
-  SB_CHECK(X && out, SB_ERR_INVALID, "null argument");
-  if (rows <= 0) return SB_OK;
-  std::lock_guard<std::mutex> lk(m->mu);
-  Net& n = m->net;
-  SB_CUDA(cudaSetDevice(n.device));
-  for (int64_t r0 = 0; r0 < rows; r0 += n.max_batch) {
-    const int c = static_cast<int>(rows - r0 < n.max_batch ? rows - r0 : n.max_batch);
-    SB_CUDA(cudaMemcpyAsync(n.stX, X + r0 * n.F, sizeof(float) * c * static_cast<size_t>(n.F), cudaMemcpyDefault, n.stream));
-    SB_TRY(model_forward(m, n.stX, c, n.yhat));
-    SB_CUDA(cudaMemcpyAsync(out + r0, n.yhat, sizeof(float) * c, cudaMemcpyDefault, n.stream));
-    SB_CUDA(cudaStreamSynchronize(n.stream));
-  }
-  return SB_OK;
-}
-
-int sb_model_score_row_f64(sb_model_t* m, const double* row, int32_t n, double* out) {
-  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
-  SB_CHECK(row && out, SB_ERR_INVALID, "null argument");
-  SB_CHECK(n == m->net.F, SB_ERR_INVALID, "expected %d features, got %d", m->net.F, n);
-  float v = 0.f;
-  SB_TRY(m->q.submit(row, &v, [m](int b, int rows) { return run_micro_batch(m, b, rows); }));
-  *out = static_cast<double>(v);
-  return SB_OK;
-}
-
-int sb_model_score_device(sb_model_t* m, const float* dX, int64_t rows, float* dOut) {
-  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
-  SB_CHECK(dX && dOut, SB_ERR_INVALID, "null argument");
-  std::lock_guard<std::mutex> lk(m->mu);
-  Net& n = m->net;
-  SB_CUDA(cudaSetDevice(n.device));
-  for (int64_t r0 = 0; r0 < rows; r0 += n.max_batch) {
-    const int c = static_cast<int>(rows - r0 < n.max_batch ? rows - r0 : n.max_batch);
-    SB_TRY(model_forward(m, dX + r0 * n.F, c, dOut + r0));
-  }
-  return SB_OK;
-}
-
-}  // extern "C"
-
-// Rows per row chunk for C list positions: max_batch / (C + 1), so that a row chunk's pairs fit one piece, but at least 64
-// (more columns go in several pieces) and at most max_batch / 2
-static int sens_chunk_rows(int max_batch, int C) {
-  long long r = max_batch / (static_cast<long long>(C) + 1);
-  if (r < 64) r = 64;
-  if (r > max_batch / 2) r = max_batch / 2;
-  return static_cast<int>(r > 0 ? r : 1);
-}
-
-template <typename T>
-static int sens_grow(DevBuf<T>* b, size_t* cap, size_t n) {
-  if (n <= *cap) return SB_OK;
-  *b = DevBuf<T>();
-  SB_TRY(b->alloc(n));
-  *cap = n;
-  return SB_OK;
-}
-
-// Column sensitivity's pieces (sensitivity.cuh, DESIGN §6f), called with m->mu held.  Rows go in row chunks of R rows
-// (sens_chunk_rows); a row chunk's z0 is computed once, and its list positions go in pieces of up to max_batch / R - 1
-// columns, each piece one forward of R (columns + 1) pair rows through layers 1..L and the output unit.  After each
-// forward, piece(r0, rc, k0, ck, wd) consumes the piece's pair scores in n.yhat (pair p = slot * rc + r; wd: the chunk's
-// weights): sb_model_sensitivity's sums and deltas, or sb_model_reason_codes' top-k merge.
-template <typename Piece>
-static int sens_forward(sb_model* m, const float* X, const float* w, int64_t rows, int C, const Piece& piece) {
-  Net& n = m->net;
-  const Layer& l0 = n.layers[0];
-  const int R = sens_chunk_rows(n.max_batch, C);
-  const int Cp = n.max_batch / R - 1;
-  SB_TRY(sens_grow(&m->sens_z, &m->sens_z_n, static_cast<size_t>(R) * l0.ld_out));
-  const StepIn in{n.desc, n.scal};
-  SensParams sp = {};
-  sp.F = n.F; sp.N = l0.out; sp.ld = l0.ld_out;
-  sp.X = n.stX;
-  sp.z = m->sens_z.p;
-  sp.act = l0.act;
-  if (n.tc()) {
-    sp.bias = n.theta + l0.b_off;
-    sp.Wn = l0.Wn; sp.w_ps = n.Wn_ps[0];
-    sp.out = n.A[0]; sp.out_ps = n.A_ps[0];
-  } else {
-    sp.W32 = n.theta + l0.w_off;
-    sp.out32 = n.Af[0];
-  }
-  using PerturbFn = void (*)(SensParams);
-  const PerturbFn perturb = !n.tc() ? sens_perturb_kernel<false, 1>
-                                    : n.nparts == 3 ? sens_perturb_kernel<true, 3>
-                                    : n.nparts == 2 ? sens_perturb_kernel<true, 2> : sens_perturb_kernel<true, 1>;
-  const char* perturb_name = !n.tc() ? "sens_perturb<fp32>"
-                             : n.nparts == 3 ? "sens_perturb<bf16x3>"
-                             : n.nparts == 2 ? "sens_perturb<bf16x2>" : "sens_perturb<bf16>";
-  const size_t row_bytes = sizeof(float) * n.F;
-  for (int64_t r0 = 0; r0 < rows; r0 += R) {
-    const int rc = static_cast<int>(rows - r0 < R ? rows - r0 : R);
-    SB_CUDA(cudaMemcpyAsync(n.stX, X + r0 * n.F, row_bytes * rc, cudaMemcpyDefault, n.stream));
-    if (w) SB_CUDA(cudaMemcpyAsync(n.stW, w + r0, sizeof(float) * rc, cudaMemcpyDefault, n.stream));
-    const float* wd = w ? n.stW : n.ones;
-    m->routes.clear();
-    const Batch b = host_batch(n, n.stX, nullptr, wd, rc);
-    SB_TRY(write_desc(n.stream, in, &b, 0.f, 1.f, 0, nullptr));
-    SB_TRY(enqueue_first(n, nullptr, in, rc, nullptr, 0));
-    SB_TRY(n.enqueue_layer0_pre(in, rc, m->sens_z.p, l0.ld_out));
-    const std::string prefix = m->routes;
-    sp.R = rc;
-    for (int k0 = 0; k0 < C; k0 += Cp) {
-      const int ck = C - k0 < Cp ? C - k0 : Cp;
-      const int pairs = rc * (ck + 1);
-      m->routes = prefix;
-      sp.cols = m->sens_cols.p + k0; sp.vals = m->sens_vals.p + k0;
-      const dim3 grid(static_cast<unsigned>((l0.out + 255) / 256), static_cast<unsigned>(ck + 1),
-                      static_cast<unsigned>((rc + SENS_ROWS - 1) / SENS_ROWS));
-      SB_TRY(launch_kernel(perturb, grid, dim3(32, 8), 0, n.stream, false, sp));
-      n.mark(perturb_name);
-      SB_TRY(n.enqueue_hidden_forward(in, pairs, nullptr, nullptr, nullptr, 0, 1));
-      SB_TRY(n.enqueue_out(in, pairs, false, false, n.yhat, nullptr));
-      SB_TRY(piece(r0, rc, k0, ck, wd));
-    }
-  }
-  return SB_OK;
-}
-
-// cols / n_cols / values as sb_model_sensitivity takes them -> the column list and its values (cl, vl)
-static int sens_list(const Net& n, const int32_t* cols, int32_t n_cols, const float* values, std::vector<int32_t>* cl,
-                     std::vector<float>* vl) {
-  SB_CHECK((cols == nullptr && n_cols == 0) || (cols != nullptr && n_cols >= 1), SB_ERR_INVALID,
-           "cols / n_cols: a list of n_cols >= 1 columns, or NULL and 0 for every column (got %s and %d)", cols ? "a list" : "NULL",
-           n_cols);
-  const int C = cols ? n_cols : n.F;
-  cl->resize(static_cast<size_t>(C));
-  vl->resize(static_cast<size_t>(C));
-  for (int k = 0; k < C; ++k) {
-    (*cl)[k] = cols ? cols[k] : k;
-    SB_CHECK((*cl)[k] >= 0 && (*cl)[k] < n.F, SB_ERR_INVALID, "cols[%d] = %d outside [0, %d)", k, (*cl)[k], n.F);
-    (*vl)[k] = values ? values[k] : 0.f;
-    SB_CHECK(std::isfinite((*vl)[k]), SB_ERR_INVALID, "values[%d] = %g is not finite", k, static_cast<double>((*vl)[k]));
-  }
-  return SB_OK;
-}
-
-// the column list and its values to the device (with m->mu held); the running sums are sized with them
-static int sens_upload_list(sb_model* m, const std::vector<int32_t>& cl, const std::vector<float>& vl) {
-  Net& n = m->net;
-  const size_t list_n = cl.size();
-  if (list_n > m->sens_list_n) {
-    m->sens_acc = DevBuf<double>(); m->sens_cols = DevBuf<int>(); m->sens_vals = DevBuf<float>();
-    m->sens_list_n = 0;
-    SB_TRY(m->sens_acc.alloc(2 * list_n + 1));
-    SB_TRY(m->sens_cols.alloc(list_n));
-    SB_TRY(m->sens_vals.alloc(list_n));
-    m->sens_list_n = list_n;
-  }
-  SB_CUDA(cudaMemcpyAsync(m->sens_cols.p, cl.data(), sizeof(int32_t) * list_n, cudaMemcpyHostToDevice, n.stream));
-  SB_CUDA(cudaMemcpyAsync(m->sens_vals.p, vl.data(), sizeof(float) * list_n, cudaMemcpyHostToDevice, n.stream));
-  return SB_OK;
-}
-
-extern "C" {
-
-int sb_model_sensitivity(sb_model_t* m, const float* X, const float* w, int64_t rows, const int32_t* cols, int32_t n_cols,
-                         const float* values, double* sum_sq, double* sum, double* w_sum, float* deltas) {
-  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
-  SB_CHECK(X && sum_sq && sum && w_sum, SB_ERR_INVALID, "null argument");
-  SB_CHECK(rows >= 0, SB_ERR_INVALID, "rows = %lld < 0", static_cast<long long>(rows));
-  Net& n = m->net;
-  std::vector<int32_t> cl;
-  std::vector<float> vl;
-  SB_TRY(sens_list(n, cols, n_cols, values, &cl, &vl));
-  const int C = static_cast<int>(cl.size());
-  for (int k = 0; k < C; ++k) sum_sq[k] = sum[k] = 0.0;
-  *w_sum = 0.0;
-  if (rows == 0) return SB_OK;
-  std::lock_guard<std::mutex> lk(m->mu);
-  SB_CUDA(cudaSetDevice(n.device));
-  const size_t list_n = static_cast<size_t>(C);
-  SB_TRY(sens_upload_list(m, cl, vl));
-  SB_CUDA(cudaMemsetAsync(m->sens_acc.p, 0, sizeof(double) * (2 * list_n + 1), n.stream));
-  if (!m->sens_d.p) SB_TRY(m->sens_d.alloc(static_cast<size_t>(n.max_batch)));
-  // per piece: d and the sums (sens_reduce_kernel), and the piece's deltas copied out when asked
-  const auto reduce = [&](int64_t r0, int rc, int k0, int ck, const float* wd) -> int {
-    SB_TRY(launch_kernel(sens_reduce_kernel, dim3(static_cast<unsigned>(ck + 1)), dim3(SENS_REDUCE_THREADS), 0, n.stream, false,
-                         static_cast<const float*>(n.yhat), wd, rc, ck, k0, deltas ? m->sens_d.p : nullptr, ck, m->sens_acc.p,
-                         k0 == 0 ? 1 : 0, 2LL * C));
-    n.mark("sens_reduce");
-    if (deltas)
-      SB_CUDA(cudaMemcpy2DAsync(deltas + r0 * C + k0, sizeof(float) * C, m->sens_d.p, sizeof(float) * ck, sizeof(float) * ck, rc,
-                                cudaMemcpyDefault, n.stream));
-    return SB_OK;
-  };
-  n.marks = &m->routes;
-  const int s = sens_forward(m, X, w, rows, C, reduce);
-  n.marks = nullptr;
-  SB_TRY(s);
-  std::vector<double> acc(2 * list_n + 1);
-  SB_CUDA(cudaMemcpyAsync(acc.data(), m->sens_acc.p, sizeof(double) * acc.size(), cudaMemcpyDeviceToHost, n.stream));
-  SB_CUDA(cudaStreamSynchronize(n.stream));
-  for (int k = 0; k < C; ++k) { sum_sq[k] = acc[2 * k]; sum[k] = acc[2 * k + 1]; }
-  *w_sum = acc[2 * list_n];
-  return SB_OK;
-}
-
-int sb_model_reason_codes(sb_model_t* m, const float* X, int64_t rows, const int32_t* cols, int32_t n_cols, const float* values,
-                          int32_t k, int32_t order, int32_t* pos, float* d, float* scores) {
-  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
-  SB_CHECK(X && pos && d, SB_ERR_INVALID, "null argument");
-  SB_CHECK(rows >= 0, SB_ERR_INVALID, "rows = %lld < 0", static_cast<long long>(rows));
-  Net& n = m->net;
-  std::vector<int32_t> cl;
-  std::vector<float> vl;
-  SB_TRY(sens_list(n, cols, n_cols, values, &cl, &vl));
-  const int C = static_cast<int>(cl.size());
-  SB_CHECK(k >= 1 && k <= C && k <= SENS_TOPK_MAX_K, SB_ERR_INVALID, "k = %d outside [1, min(%d list positions, %d)]", k, C,
-           SENS_TOPK_MAX_K);
-  SB_CHECK(order == SB_REASON_RAISE || order == SB_REASON_LOWER || order == SB_REASON_MAGNITUDE, SB_ERR_INVALID,
-           "order = %d is not SB_REASON_RAISE, SB_REASON_LOWER or SB_REASON_MAGNITUDE", order);
-  if (rows == 0) return SB_OK;
-  std::lock_guard<std::mutex> lk(m->mu);
-  SB_CUDA(cudaSetDevice(n.device));
-  SB_TRY(sens_upload_list(m, cl, vl));
-  const size_t run_n = static_cast<size_t>(sens_chunk_rows(n.max_batch, C)) * k;
-  SB_TRY(sens_grow(&m->reason_d, &m->reason_d_n, run_n));
-  SB_TRY(sens_grow(&m->reason_pos, &m->reason_pos_n, run_n));
-  // per piece: merge its deltas into each row's running top k (reset by the chunk's first piece); after the chunk's last
-  // piece, copy the chunk's top k and base scores out
-  const auto merge = [&](int64_t r0, int rc, int k0, int ck, const float*) -> int {
-    const unsigned warps = static_cast<unsigned>(std::min((ck + 31) / 32, SENS_TOPK_WARPS));
-    SB_TRY(launch_kernel(sens_topk_kernel, dim3(static_cast<unsigned>(rc)), dim3(32, warps), 0, n.stream, false,
-                         static_cast<const float*>(n.yhat), rc, ck, k0, static_cast<int>(k), static_cast<int>(order), k0 == 0 ? 1 : 0,
-                         m->reason_d.p, m->reason_pos.p));
-    n.mark("sens_topk");
-    if (k0 + ck < C) return SB_OK;
-    const size_t out_n = static_cast<size_t>(rc) * k;
-    SB_CUDA(cudaMemcpyAsync(pos + r0 * k, m->reason_pos.p, sizeof(int32_t) * out_n, cudaMemcpyDefault, n.stream));
-    SB_CUDA(cudaMemcpyAsync(d + r0 * k, m->reason_d.p, sizeof(float) * out_n, cudaMemcpyDefault, n.stream));
-    if (scores) SB_CUDA(cudaMemcpyAsync(scores + r0, n.yhat, sizeof(float) * rc, cudaMemcpyDefault, n.stream));
-    return SB_OK;
-  };
-  n.marks = &m->routes;
-  const int s = sens_forward(m, X, nullptr, rows, C, merge);
-  n.marks = nullptr;
-  SB_TRY(s);
-  SB_CUDA(cudaStreamSynchronize(n.stream));
-  return SB_OK;
-}
-
-int sb_model_sync(sb_model_t* m) {
-  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
-  SB_CUDA(cudaStreamSynchronize(m->net.stream));
-  return SB_OK;
-}
-void* sb_model_stream(sb_model_t* m) { return m ? reinterpret_cast<void*>(m->net.stream) : nullptr; }
-
-int sb_debug_model_batch_stats(sb_model_t* m, int64_t* stats, int32_t n_stats) {
-  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
-  SB_CHECK(stats && n_stats >= SB_DEBUG_MSTAT_WORDS, SB_ERR_INVALID, "stats needs %d words, got %d", SB_DEBUG_MSTAT_WORDS, n_stats);
-  for (int i = 0; i < SB_DEBUG_MSTAT_WORDS; ++i) stats[i] = m->st[i].load();
-  stats[SB_DEBUG_MSTAT_BATCHES] = m->q.batches.load();
-  stats[SB_DEBUG_MSTAT_ROWS] = m->q.rows.load();
-  stats[SB_DEBUG_MSTAT_MAX_FILL] = m->q.max_fill.load();
-  return SB_OK;
-}
-
-int sb_debug_model_routes(sb_model_t* m, char* out, int32_t cap) {
-  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
-  SB_CHECK(out && cap > 0, SB_ERR_INVALID, "route buffer of %d bytes", cap);
-  std::lock_guard<std::mutex> lk(m->mu);
-  snprintf(out, static_cast<size_t>(cap), "%s", m->routes.empty() ? "none" : m->routes.c_str());
-  return SB_OK;
-}
-
-int sb_debug_model_hold(sb_model_t* m, int32_t k, int32_t timeout_ms) {
-  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
-  SB_CHECK(k >= 0 && k <= MB_ROWS && timeout_ms >= 0, SB_ERR_INVALID, "k = %d outside [0, %d] or timeout_ms = %d < 0", k, MB_ROWS,
-           timeout_ms);
-  std::lock_guard<std::mutex> lk(m->q.q_mu);
-  m->q.hold_k = k;
-  m->q.hold_ms = timeout_ms;
-  return SB_OK;
-}
-
-int sb_debug_model_bytes(sb_model_t* m, int64_t* out) {
-  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
-  SB_CHECK(out, SB_ERR_INVALID, "null argument");
-  *out = static_cast<int64_t>(m->net.dalloc_bytes);
-  return SB_OK;
-}
-
-}  // extern "C"
-
-// ================================================================================================
-// ensemble: K member models on one stream that share one staged copy of the rows (DESIGN §6h)
-// ================================================================================================
-struct sb_ensemble {
-  // Member 0 owns the stream and the input staging (stX, Xb / Xf); members 1 .. K-1 are created with input_from = its net
-  // and allocate neither.  Destroyed in reverse order, member 0 last.
-  std::vector<sb_model*> members;
-  int K = 0;
-  std::mutex mu;              // device work on the ensemble's stream
-  float* slots = nullptr;     // [K, max_batch]: member g's scores of a chunk at slots + g * max_batch (member 0's net)
-  float* d_scores = nullptr;  // [max_batch, K] and [max_batch, 4]: the outputs of sb_ensemble_score and compute() batches
-  float* d_stats = nullptr;
-  RowQueue q;                 // compute(): K + 4 words per row
-  cudaGraphExec_t mb_graph = nullptr;         // tensor-core modes: the ensemble forward of MB_ROWS staged rows
-  std::string routes;         // the launches of the last chunk, "+"-joined (sb_debug_ensemble_routes; guarded by mu)
-  Net& lead() { return members[0]->net; }
-  ~sb_ensemble() {
-    if (!members.empty() && members[0]->net.stream) {
-      cudaSetDevice(lead().device);
-      cudaStreamSynchronize(lead().stream);
-    }
-    if (mb_graph) cudaGraphExecDestroy(mb_graph);
-    while (!members.empty()) {
-      delete members.back();
-      members.pop_back();
-    }
-  }
-};
-
-// the flat parameter count of a topology (what Net::init lays out)
-static long long desc_param_count(const sb_net_desc& d) {
-  long long np = 0;
-  int prev = d.n_features;
-  for (int l = 0; l <= d.n_hidden; ++l) {
-    const int out = l < d.n_hidden ? d.hidden[l] : 1;
-    np += static_cast<long long>(prev) * out + out;
-    prev = out;
-  }
-  return np;
-}
-
-// K checked descriptors (n_features and precision shared) and their parameters -> an ensemble
-static int ensemble_from_descs(const std::vector<sb_net_desc>& ds, const float* const* flats, const int64_t* n_params, int device,
-                               sb_ensemble_t** out) {
-  std::unique_ptr<sb_ensemble> e(new sb_ensemble());
-  e->K = static_cast<int>(ds.size());
-  for (int g = 0; g < e->K; ++g) {
-    sb_model* m = nullptr;
-    SB_TRY(model_from_desc(ds[g], flats[g], n_params[g], device, &m, true, g > 0 ? &e->lead() : nullptr));
-    e->members.push_back(m);
-  }
-  Net& n0 = e->lead();
-  SB_TRY(n0.dalloc(&e->slots, static_cast<size_t>(e->K) * n0.max_batch));
-  SB_TRY(n0.dalloc(&e->d_scores, static_cast<size_t>(n0.max_batch) * e->K));
-  SB_TRY(n0.dalloc(&e->d_stats, static_cast<size_t>(n0.max_batch) * 4));
-  SB_TRY(e->q.alloc(n0.F, e->K + 4));
-  SB_CUDA(cudaStreamSynchronize(n0.stream));
-  *out = e.release();
-  return SB_OK;
-}
-
-// The members' forwards and the statistics of `rows` (<= max_batch) device rows dX, queued on the ensemble's stream.
-// Tensor-core modes and fp32 chunks of more than SMALL_ROWS rows load the rows once (member 0's descriptor and
-// load_batch_kernel into the shared Xb / Xf), then run each member's hidden-layer and output launches, which read that
-// operand; an fp32 chunk of up to SMALL_ROWS rows is one score_rows_kernel launch per member, reading dX.  Scoring reads
-// no descriptor field or step scalar besides what the load reads (the output layer runs without the loss), so the other
-// members need no descriptor of their own.  Each member's launches are the ones enqueue_model_forward runs for the same
-// rows, minus the load.  Then ensemble_stats_kernel: slots -> dScores / dStats (either may be null).
-static int enqueue_ensemble_forward(sb_ensemble* e, const float* dX, int rows, float* dScores, float* dStats) {
-  Net& n0 = e->lead();
-  const bool layered = n0.tc() || rows > SMALL_ROWS;
-  if (layered) {
-    const StepIn in{n0.desc, n0.scal};
-    const Batch b = host_batch(n0, dX, nullptr, nullptr, rows);
-    SB_TRY(write_desc(n0.stream, in, &b, 0.f, 1.f, 0, nullptr));
-    SB_TRY(n0.enqueue_load(in, rows));
-  }
-  for (int g = 0; g < e->K; ++g) {
-    sb_model* m = e->members[g];
-    Net& n = m->net;
-    float* slot = e->slots + static_cast<size_t>(g) * n0.max_batch;
-    if (!layered) {
-      SB_TRY(enqueue_model_forward(m, dX, rows, slot));
-      continue;
-    }
-    const StepIn in{n.desc, n.scal};
-    SB_TRY(n.enqueue_hidden_forward(in, rows));
-    SB_TRY(n.enqueue_out(in, rows, false, false, slot, nullptr));
-  }
-  SB_TRY(launch_kernel(ensemble_stats_kernel, dim3(static_cast<unsigned>((rows + ENS_THREADS - 1) / ENS_THREADS)), dim3(ENS_THREADS), 0,
-                       n0.stream, false, static_cast<const float*>(e->slots), static_cast<long long>(n0.max_batch), e->K, rows,
-                       dScores, dStats));
-  n0.mark("ensemble_stats");
-  return SB_OK;
-}
-
-// Every scoring path of an ensemble comes through here; its launches are kept for sb_debug_ensemble_routes.  Called with
-// e->mu held.
-static int ensemble_forward(sb_ensemble* e, const float* dX, int rows, float* dScores, float* dStats) {
-  e->routes.clear();
-  for (sb_model* m : e->members) m->net.marks = &e->routes;
-  const int s = enqueue_ensemble_forward(e, dX, rows, dScores, dStats);
-  for (sb_model* m : e->members) m->net.marks = nullptr;
-  return s;
-}
-
-// one compute() batch: rows of staging buffer b -> e->q.res[b] [rows, K + 4].  A tensor-core batch runs the captured
-// forward of MB_ROWS rows (one load, K members, the statistics), its pad rows zero-filled.
-static int run_ensemble_micro_batch(sb_ensemble* e, int b, int rows) {
-  std::lock_guard<std::mutex> lk(e->mu);
-  Net& n = e->lead();
-  SB_CUDA(cudaSetDevice(n.device));
-  if (n.tc() && !e->mb_graph)
-    SB_TRY(capture_micro_batch(n.stream, [&] { return ensemble_forward(e, n.stX, MB_ROWS, e->d_scores, e->d_stats); }, &e->mb_graph));
-  const size_t row_bytes = sizeof(float) * n.F;
-  SB_CUDA(cudaMemcpyAsync(n.stX, e->q.stage[b], row_bytes * rows, cudaMemcpyHostToDevice, n.stream));
-  if (n.tc()) {
-    if (rows < MB_ROWS) SB_CUDA(cudaMemsetAsync(n.stX + static_cast<size_t>(rows) * n.F, 0, row_bytes * (MB_ROWS - rows), n.stream));
-    SB_CUDA(cudaGraphLaunch(e->mb_graph, n.stream));
-  } else {
-    SB_TRY(ensemble_forward(e, n.stX, rows, e->d_scores, e->d_stats));
-  }
-  const size_t pitch = sizeof(float) * (e->K + 4);
-  SB_CUDA(cudaMemcpy2DAsync(e->q.res[b], pitch, e->d_scores, sizeof(float) * e->K, sizeof(float) * e->K, rows, cudaMemcpyDeviceToHost,
-                            n.stream));
-  SB_CUDA(cudaMemcpy2DAsync(e->q.res[b] + e->K, pitch, e->d_stats, sizeof(float) * 4, sizeof(float) * 4, rows, cudaMemcpyDeviceToHost,
-                            n.stream));
-  SB_CUDA(cudaStreamSynchronize(n.stream));
-  return SB_OK;
-}
-
-static int check_ensemble_k(int32_t k) {
-  SB_CHECK(k >= 1 && k <= SB_ENSEMBLE_MAX, SB_ERR_INVALID, "k = %d members outside [1, %d]", k, SB_ENSEMBLE_MAX);
-  return SB_OK;
-}
-
-static int check_ensemble_members(const std::vector<sb_net_desc>& ds) {
-  for (size_t g = 1; g < ds.size(); ++g) {
-    SB_CHECK(ds[g].n_features == ds[0].n_features, SB_ERR_INVALID, "member %d has %d features, member 0 has %d", static_cast<int>(g),
-             ds[g].n_features, ds[0].n_features);
-    SB_CHECK(ds[g].precision == ds[0].precision, SB_ERR_INVALID, "member %d has precision %d, member 0 has %d", static_cast<int>(g),
-             ds[g].precision, ds[0].precision);
-  }
-  return SB_OK;
-}
-
-extern "C" {
-
-int sb_ensemble_create(const sb_net_desc* descs, const float* const* flats, const int64_t* n_params, int32_t k, int device,
-                       sb_ensemble_t** out) {
-  SB_CHECK(out, SB_ERR_INVALID, "out is null");
-  *out = nullptr;
-  SB_TRY(check_ensemble_k(k));
-  SB_CHECK(descs && flats && n_params, SB_ERR_INVALID, "null argument");
-  std::vector<sb_net_desc> ds(descs, descs + k);
-  for (int g = 0; g < k; ++g) {
-    SB_CHECK(flats[g], SB_ERR_INVALID, "flats[%d] is null", g);
-    if (ds[g].max_batch <= 0) ds[g].max_batch = 1;
-    SB_TRY(validate_desc(&ds[g]));
-    const long long np = desc_param_count(ds[g]);
-    SB_CHECK(n_params[g] == np, SB_ERR_INVALID, "member %d: expected %lld params, got %lld", g, np, static_cast<long long>(n_params[g]));
-  }
-  SB_TRY(check_ensemble_members(ds));
-  return ensemble_from_descs(ds, flats, n_params, device, out);
-}
-
-int sb_ensemble_load(const char* const* dirs, int32_t k, const char* input_name, const char* output_name, const char* tag,
-                     int device, int precision, sb_ensemble_t** out) {
-  SB_CHECK(out, SB_ERR_INVALID, "out is null");
-  *out = nullptr;
-  SB_TRY(check_ensemble_k(k));
-  SB_CHECK(dirs, SB_ERR_INVALID, "dirs is null");
-  std::vector<sb_net_desc> ds(static_cast<size_t>(k));
-  std::vector<std::vector<float>> flat(static_cast<size_t>(k));
-  for (int g = 0; g < k; ++g) SB_TRY(read_scoring_model(dirs[g], input_name, output_name, tag, precision, &ds[g], &flat[g]));
-  SB_TRY(check_ensemble_members(ds));
-  std::vector<const float*> fp(static_cast<size_t>(k));
-  std::vector<int64_t> np(static_cast<size_t>(k));
-  for (int g = 0; g < k; ++g) { fp[g] = flat[g].data(); np[g] = static_cast<int64_t>(flat[g].size()); }
-  return ensemble_from_descs(ds, fp.data(), np.data(), device, out);
-}
-
-int sb_ensemble_destroy(sb_ensemble_t* e) {
-  delete e;
-  return SB_OK;
-}
-
-int32_t sb_ensemble_size(const sb_ensemble_t* e) { return e ? e->K : 0; }
-
-// the argument checks every scoring entry point shares
-static int check_ensemble_score(const sb_ensemble* e, const float* X, int64_t rows, const float* scores, const float* stats) {
-  SB_CHECK(e, SB_ERR_STATE, "TF ensemble not initialized.");
-  SB_CHECK(X, SB_ERR_INVALID, "X is null");
-  SB_CHECK(scores || stats, SB_ERR_INVALID, "scores and stats are both null");
-  SB_CHECK(rows >= 0, SB_ERR_INVALID, "rows = %lld < 0", static_cast<long long>(rows));
-  return SB_OK;
-}
-
-int sb_ensemble_score(sb_ensemble_t* e, const float* X, int64_t rows, float* scores, float* stats) {
-  SB_TRY(check_ensemble_score(e, X, rows, scores, stats));
-  if (rows == 0) return SB_OK;
-  std::lock_guard<std::mutex> lk(e->mu);
-  Net& n = e->lead();
-  const int K = e->K;
-  SB_CUDA(cudaSetDevice(n.device));
-  for (int64_t r0 = 0; r0 < rows; r0 += n.max_batch) {
-    const int c = static_cast<int>(rows - r0 < n.max_batch ? rows - r0 : n.max_batch);
-    SB_CUDA(cudaMemcpyAsync(n.stX, X + r0 * n.F, sizeof(float) * c * static_cast<size_t>(n.F), cudaMemcpyDefault, n.stream));
-    SB_TRY(ensemble_forward(e, n.stX, c, scores ? e->d_scores : nullptr, stats ? e->d_stats : nullptr));
-    if (scores) SB_CUDA(cudaMemcpyAsync(scores + r0 * K, e->d_scores, sizeof(float) * c * K, cudaMemcpyDefault, n.stream));
-    if (stats) SB_CUDA(cudaMemcpyAsync(stats + r0 * 4, e->d_stats, sizeof(float) * c * 4, cudaMemcpyDefault, n.stream));
-    SB_CUDA(cudaStreamSynchronize(n.stream));
-  }
-  return SB_OK;
-}
-
-int sb_ensemble_score_device(sb_ensemble_t* e, const float* dX, int64_t rows, float* dScores, float* dStats) {
-  SB_TRY(check_ensemble_score(e, dX, rows, dScores, dStats));
-  std::lock_guard<std::mutex> lk(e->mu);
-  Net& n = e->lead();
-  SB_CUDA(cudaSetDevice(n.device));
-  for (int64_t r0 = 0; r0 < rows; r0 += n.max_batch) {
-    const int c = static_cast<int>(rows - r0 < n.max_batch ? rows - r0 : n.max_batch);
-    SB_TRY(ensemble_forward(e, dX + r0 * n.F, c, dScores ? dScores + r0 * e->K : nullptr, dStats ? dStats + r0 * 4 : nullptr));
-  }
-  return SB_OK;
-}
-
-int sb_ensemble_score_row_f64(sb_ensemble_t* e, const double* row, int32_t n, double* out) {
-  SB_CHECK(e, SB_ERR_STATE, "TF ensemble not initialized.");
-  SB_CHECK(row && out, SB_ERR_INVALID, "null argument");
-  SB_CHECK(n == e->q.F, SB_ERR_INVALID, "expected %d features, got %d", e->q.F, n);
-  float v[SB_ENSEMBLE_MAX + 4];
-  SB_TRY(e->q.submit(row, v, [e](int b, int rows) { return run_ensemble_micro_batch(e, b, rows); }));
-  for (int i = 0; i < e->K + 4; ++i) out[i] = static_cast<double>(v[i]);
-  return SB_OK;
-}
-
-int sb_ensemble_sync(sb_ensemble_t* e) {
-  SB_CHECK(e, SB_ERR_STATE, "TF ensemble not initialized.");
-  SB_CUDA(cudaStreamSynchronize(e->lead().stream));
-  return SB_OK;
-}
-
-void* sb_ensemble_stream(sb_ensemble_t* e) { return e ? reinterpret_cast<void*>(e->lead().stream) : nullptr; }
-
-int sb_debug_ensemble_routes(sb_ensemble_t* e, char* out, int32_t cap) {
-  SB_CHECK(e, SB_ERR_STATE, "TF ensemble not initialized.");
-  SB_CHECK(out && cap > 0, SB_ERR_INVALID, "route buffer of %d bytes", cap);
-  std::lock_guard<std::mutex> lk(e->mu);
-  snprintf(out, static_cast<size_t>(cap), "%s", e->routes.empty() ? "none" : e->routes.c_str());
-  return SB_OK;
-}
-
-int sb_debug_ensemble_bytes(sb_ensemble_t* e, int64_t* out) {
-  SB_CHECK(e, SB_ERR_STATE, "TF ensemble not initialized.");
-  SB_CHECK(out, SB_ERR_INVALID, "null argument");
-  long long b = 0;
-  for (const sb_model* m : e->members) b += static_cast<long long>(m->net.dalloc_bytes);
-  *out = b;
-  return SB_OK;
-}
-
-}  // extern "C"
-
-// ================================================================================================
-// performance: exact ranking metrics of scored rows from one radix sort (DESIGN §6i, kernels in perf.cuh)
-// ================================================================================================
-constexpr long long PERF_MAX_ROWS = 2147483647LL;   // 2^31 - 1 rows per handle: every count fits the int64 formulas
-constexpr long long PERF_STAGE_ROWS = 1 << 20;      // host rows go through a device staging of this many (s, y, w)
-
-struct sb_perf {
-  int device = -1, sms = 0;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev_after = nullptr;      // the point of after_stream an add is queued behind
-  long long rows = 0, cap = 0;         // rows held; pair capacity (a multiple of PERF_TILE)
-  long long sorted = 0, m = 0;         // rows the run table describes, its runs
-  long long P = 0, N = 0;              // the table's totals (its last row)
-  double Wp = 0.0, Wn = 0.0;
-  int cur = 0;                         // keys[cur] / pay[cur] hold the rows; the other pair is the sort's double buffer
-  uint32_t* keys[2] = {nullptr, nullptr};
-  uint32_t* pay[2] = {nullptr, nullptr};
-  unsigned long long* status = nullptr;   // [cap / PERF_TILE][256]: the sort's look-back words
-  PerfTile* tiles = nullptr;              // [cap / PERF_TILE]
-  long long run_cap = 0;
-  float* rt = nullptr;                    // the run table [run_cap]
-  long long *rtp = nullptr, *rfp = nullptr;
-  double *rwtp = nullptr, *rwfp = nullptr;
-  unsigned int* hist = nullptr;           // [4][256] digit counts of every key held
-  unsigned long long* bad = nullptr;      // [3] invalid rows: NaN score, bad label, bad weight
-  unsigned int* tile_ctr = nullptr;
-  PerfPart* parts = nullptr;              // [PERF_SUM_BLOCKS]
-  PerfResult* result = nullptr;
-  PerfTile* total = nullptr;
-  float* stage = nullptr;                 // [3][PERF_STAGE_ROWS], at the first add that reads host memory
-  long long pt_cap = 0;                   // sb_perf_points' levels and points on the device
-  double* d_levels = nullptr;
-  sb_perf_point* d_points = nullptr;
-  long long bytes = 0;                    // device bytes held (sb_debug_perf_bytes)
-
-  // stream-ordered allocations, so that growing on an asynchronous add needs no host synchronise
-  template <typename T> int alloc(T** p, long long n) {
-    void* q = nullptr;
-    SB_CUDA(cudaMallocAsync(&q, sizeof(T) * static_cast<size_t>(n), stream));
-    *p = static_cast<T*>(q);
-    bytes += static_cast<long long>(sizeof(T)) * n;
-    return SB_OK;
-  }
-  template <typename T> void release(T** p, long long n) {
-    if (*p == nullptr) return;
-    cudaFreeAsync(*p, stream);
-    bytes -= static_cast<long long>(sizeof(T)) * n;
-    *p = nullptr;
-  }
-  void release_runs() {
-    release(&rt, run_cap); release(&rtp, run_cap); release(&rfp, run_cap); release(&rwtp, run_cap); release(&rwfp, run_cap);
-    run_cap = 0;
-  }
-  ~sb_perf() {
-    if (!stream) return;
-    cudaSetDevice(device);
-    const long long nt = cap / PERF_TILE;
-    for (int b = 0; b < 2; ++b) { release(&keys[b], cap); release(&pay[b], cap); }
-    release(&status, nt * 256); release(&tiles, nt);
-    release_runs();
-    release(&hist, 4 * 256); release(&bad, 3); release(&tile_ctr, 1); release(&parts, PERF_SUM_BLOCKS);
-    release(&result, 1); release(&total, 1); release(&stage, 3 * PERF_STAGE_ROWS);
-    release(&d_levels, pt_cap); release(&d_points, pt_cap);
-    cudaStreamSynchronize(stream);
-    if (ev_after) cudaEventDestroy(ev_after);
-    cudaStreamDestroy(stream);
-  }
-};
-
-// capacity for `need` rows: grows by half at least, keeps the rows held (copied into the new pair 0)
-static int perf_reserve(sb_perf* p, long long need) {
-  if (need <= p->cap) return SB_OK;
-  long long c = std::max(need, p->cap + p->cap / 2);
-  c = (c + PERF_TILE - 1) / PERF_TILE * PERF_TILE;
-  const long long nt = c / PERF_TILE, old_nt = p->cap / PERF_TILE;
-  sb_perf q;                           // the new buffers, owned by q until they are swapped in
-  q.stream = p->stream;
-  q.device = p->device;
-  int s = SB_OK;
-  for (int b = 0; b < 2 && s == SB_OK; ++b) {
-    s = q.alloc(&q.keys[b], c);
-    if (s == SB_OK) s = q.alloc(&q.pay[b], c);
-  }
-  if (s == SB_OK) s = q.alloc(&q.status, nt * 256);
-  if (s == SB_OK) s = q.alloc(&q.tiles, nt);
-  if (s == SB_OK && p->rows > 0) {
-    const size_t b = sizeof(uint32_t) * static_cast<size_t>(p->rows);
-    if (cudaMemcpyAsync(q.keys[0], p->keys[p->cur], b, cudaMemcpyDeviceToDevice, p->stream) != cudaSuccess ||
-        cudaMemcpyAsync(q.pay[0], p->pay[p->cur], b, cudaMemcpyDeviceToDevice, p->stream) != cudaSuccess)
-      s = set_error(SB_ERR_CUDA, "copying %lld rows into the grown buffers failed", p->rows);
-  }
-  if (s != SB_OK) {
-    for (int b = 0; b < 2; ++b) { q.release(&q.keys[b], c); q.release(&q.pay[b], c); }
-    q.release(&q.status, nt * 256); q.release(&q.tiles, nt);
-    q.stream = nullptr;                // q's destructor must not tear down p's stream
-    return s;
-  }
-  for (int b = 0; b < 2; ++b) {
-    p->release(&p->keys[b], p->cap); p->release(&p->pay[b], p->cap);
-    std::swap(p->keys[b], q.keys[b]); std::swap(p->pay[b], q.pay[b]);
-  }
-  p->release(&p->status, old_nt * 256); p->release(&p->tiles, old_nt);
-  std::swap(p->status, q.status); std::swap(p->tiles, q.tiles);
-  p->bytes += q.bytes;
-  q.stream = nullptr;
-  p->cur = 0;
-  p->cap = c;
-  return SB_OK;
-}
-
-// Synchronous: refuses a handle that holds invalid rows, then sorts the rows and builds the run table if rows arrived
-// since the last time
-static int perf_prepare(sb_perf* p) {
-  SB_CUDA(cudaSetDevice(p->device));
-  unsigned long long bad[3];
-  SB_CUDA(cudaMemcpyAsync(bad, p->bad, sizeof(bad), cudaMemcpyDeviceToHost, p->stream));
-  SB_CUDA(cudaStreamSynchronize(p->stream));
-  SB_CHECK(bad[0] + bad[1] + bad[2] == 0, SB_ERR_INVALID,
-           "the handle holds invalid rows: %llu with a NaN score, %llu with a label other than 0 or 1, %llu with a negative "
-           "or non-finite weight (sb_perf_reset forgets them)", bad[0], bad[1], bad[2]);
-  if (p->sorted == p->rows) return SB_OK;
-  const long long n = p->rows;
-  const long long nt = (n + PERF_TILE - 1) / PERF_TILE;
-  unsigned int hist[4 * 256];
-  SB_CUDA(cudaMemcpyAsync(hist, p->hist, sizeof(hist), cudaMemcpyDeviceToHost, p->stream));
-  SB_CUDA(cudaStreamSynchronize(p->stream));
-  for (int d = 0; d < 4; ++d) {
-    bool one_bin = false;
-    for (int b = 0; b < 256; ++b) one_bin |= hist[d * 256 + b] == static_cast<unsigned int>(n);
-    if (one_bin) continue;             // this digit leaves the order as it is
-    SB_CUDA(cudaMemsetAsync(p->status, 0, sizeof(unsigned long long) * 256 * static_cast<size_t>(nt), p->stream));
-    SB_CUDA(cudaMemsetAsync(p->tile_ctr, 0, sizeof(unsigned int), p->stream));
-    SB_TRY(launch_kernel(perf_sort_pass_kernel, dim3(static_cast<unsigned>(nt)), dim3(PERF_THREADS), 0, p->stream, false,
-                         static_cast<const uint32_t*>(p->keys[p->cur]), static_cast<const uint32_t*>(p->pay[p->cur]),
-                         p->keys[p->cur ^ 1], p->pay[p->cur ^ 1], n, 8 * d, static_cast<const unsigned int*>(p->hist + 256 * d),
-                         p->status, p->tile_ctr));
-    p->cur ^= 1;
-  }
-  if (p->run_cap < p->cap) {
-    p->release_runs();
-    SB_TRY(p->alloc(&p->rt, p->cap)); SB_TRY(p->alloc(&p->rtp, p->cap)); SB_TRY(p->alloc(&p->rfp, p->cap));
-    SB_TRY(p->alloc(&p->rwtp, p->cap)); SB_TRY(p->alloc(&p->rwfp, p->cap));
-    p->run_cap = p->cap;
-  }
-  const uint32_t* k = p->keys[p->cur];
-  const uint32_t* w = p->pay[p->cur];
-  SB_TRY(launch_kernel(perf_runs_kernel<false>, dim3(static_cast<unsigned>(nt)), dim3(PERF_THREADS), 0, p->stream, false, k, w, n,
-                       p->tiles, p->rt, p->rtp, p->rfp, p->rwtp, p->rwfp));
-  SB_TRY(launch_kernel(perf_tile_scan_kernel, dim3(1), dim3(PERF_THREADS), 0, p->stream, false, p->tiles, nt, p->total));
-  SB_TRY(launch_kernel(perf_runs_kernel<true>, dim3(static_cast<unsigned>(nt)), dim3(PERF_THREADS), 0, p->stream, false, k, w, n,
-                       p->tiles, p->rt, p->rtp, p->rfp, p->rwtp, p->rwfp));
-  PerfTile tot;
-  SB_CUDA(cudaMemcpyAsync(&tot, p->total, sizeof(tot), cudaMemcpyDeviceToHost, p->stream));
-  SB_CUDA(cudaStreamSynchronize(p->stream));
-  p->m = tot.heads;
-  p->P = p->N = 0;
-  p->Wp = p->Wn = 0.0;
-  if (p->m > 0) {                      // the totals are the table's last row (the metrics' denominators)
-    const long long j = p->m - 1;
-    SB_CUDA(cudaMemcpyAsync(&p->P, p->rtp + j, sizeof(long long), cudaMemcpyDeviceToHost, p->stream));
-    SB_CUDA(cudaMemcpyAsync(&p->N, p->rfp + j, sizeof(long long), cudaMemcpyDeviceToHost, p->stream));
-    SB_CUDA(cudaMemcpyAsync(&p->Wp, p->rwtp + j, sizeof(double), cudaMemcpyDeviceToHost, p->stream));
-    SB_CUDA(cudaMemcpyAsync(&p->Wn, p->rwfp + j, sizeof(double), cudaMemcpyDeviceToHost, p->stream));
-    SB_CUDA(cudaStreamSynchronize(p->stream));
-  }
-  p->sorted = n;
-  return SB_OK;
-}
-
-// the device a pointer lives on, or -1 for host memory (pageable, pinned or managed: read through a staging copy)
-static int perf_ptr_device(const void* ptr) {
-  cudaPointerAttributes at;
-  if (cudaPointerGetAttributes(&at, ptr) != cudaSuccess) { cudaGetLastError(); return -1; }
-  return at.type == cudaMemoryTypeDevice ? at.device : -1;
-}
-
-extern "C" {
-
-int sb_perf_create(int device, int64_t reserve_rows, sb_perf_t** out) {
-  SB_CHECK(out, SB_ERR_INVALID, "out is null");
-  *out = nullptr;
-  SB_CHECK(reserve_rows >= 0 && reserve_rows <= PERF_MAX_ROWS, SB_ERR_INVALID, "reserve_rows = %lld outside [0, 2^31 - 1]",
-           static_cast<long long>(reserve_rows));
-  std::unique_ptr<sb_perf> p(new sb_perf());
-  SB_TRY(check_device(device, &p->sms));
-  p->device = device;
-  SB_CUDA(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
-  SB_CUDA(cudaEventCreateWithFlags(&p->ev_after, cudaEventDisableTiming));
-  SB_TRY(p->alloc(&p->hist, 4 * 256));
-  SB_TRY(p->alloc(&p->bad, 3));
-  SB_TRY(p->alloc(&p->tile_ctr, 1));
-  SB_TRY(p->alloc(&p->parts, PERF_SUM_BLOCKS));
-  SB_TRY(p->alloc(&p->result, 1));
-  SB_TRY(p->alloc(&p->total, 1));
-  SB_CUDA(cudaMemsetAsync(p->hist, 0, sizeof(unsigned int) * 4 * 256, p->stream));
-  SB_CUDA(cudaMemsetAsync(p->bad, 0, sizeof(unsigned long long) * 3, p->stream));
-  SB_TRY(perf_reserve(p.get(), reserve_rows));
-  SB_CUDA(cudaStreamSynchronize(p->stream));
-  *out = p.release();
-  return SB_OK;
-}
-
-int sb_perf_destroy(sb_perf_t* p) {
-  delete p;
-  return SB_OK;
-}
-
-int sb_perf_reset(sb_perf_t* p) {
-  SB_CHECK(p, SB_ERR_STATE, "performance handle not initialized.");
-  SB_CUDA(cudaSetDevice(p->device));
-  SB_CUDA(cudaMemsetAsync(p->hist, 0, sizeof(unsigned int) * 4 * 256, p->stream));
-  SB_CUDA(cudaMemsetAsync(p->bad, 0, sizeof(unsigned long long) * 3, p->stream));
-  p->rows = p->sorted = p->m = p->P = p->N = 0;
-  p->Wp = p->Wn = 0.0;
-  return SB_OK;
-}
-
-int sb_perf_add(sb_perf_t* p, const float* scores, int32_t score_stride, const float* y, const float* w, int64_t rows,
-                void* after_stream) {
-  SB_CHECK(p, SB_ERR_STATE, "performance handle not initialized.");
-  SB_CHECK(scores && y, SB_ERR_INVALID, "scores and y must not be null");
-  SB_CHECK(rows >= 0, SB_ERR_INVALID, "rows = %lld < 0", static_cast<long long>(rows));
-  SB_CHECK(score_stride >= 1, SB_ERR_INVALID, "score_stride = %d < 1", score_stride);
-  SB_CHECK(rows <= PERF_MAX_ROWS - p->rows, SB_ERR_INVALID, "%lld rows held + %lld added exceed 2^31 - 1 rows per handle", p->rows,
-           static_cast<long long>(rows));
-  if (rows == 0) return SB_OK;
-  const int ds = perf_ptr_device(scores), dy = perf_ptr_device(y), dw = w ? perf_ptr_device(w) : p->device;
-  for (int d : {ds, dy, dw})
-    SB_CHECK(d < 0 || d == p->device, SB_ERR_INVALID, "a device pointer on device %d, the handle is on device %d", d, p->device);
-  const bool on_device = ds >= 0 && dy >= 0 && dw >= 0;
-  SB_CUDA(cudaSetDevice(p->device));
-  if (after_stream) {
-    SB_CUDA(cudaEventRecord(p->ev_after, static_cast<cudaStream_t>(after_stream)));
-    SB_CUDA(cudaStreamWaitEvent(p->stream, p->ev_after, 0));
-  }
-  SB_TRY(perf_reserve(p, p->rows + rows));
-  const long long sp = score_stride;
-  auto add = [&](const float* s, long long stride, const float* yy, const float* ww, long long r0, long long c) {
-    const long long grid = std::min<long long>((c + PERF_ADD_THREADS - 1) / PERF_ADD_THREADS, 4LL * p->sms);
-    return launch_kernel(perf_add_kernel, dim3(static_cast<unsigned>(grid)), dim3(PERF_ADD_THREADS), 0, p->stream, false, s, stride,
-                         yy, ww, c, p->keys[p->cur] + p->rows + r0, p->pay[p->cur] + p->rows + r0, p->hist, p->bad);
-  };
-  if (on_device) {
-    SB_TRY(add(scores, sp, y, w, 0, rows));
-  } else {
-    if (!p->stage) SB_TRY(p->alloc(&p->stage, 3 * PERF_STAGE_ROWS));
-    float* ss = p->stage;
-    float* sy = ss + PERF_STAGE_ROWS;
-    float* sw = sy + PERF_STAGE_ROWS;
-    for (long long r0 = 0; r0 < rows; r0 += PERF_STAGE_ROWS) {
-      const long long c = std::min<long long>(rows - r0, PERF_STAGE_ROWS);
-      SB_CUDA(cudaMemcpy2DAsync(ss, sizeof(float), scores + r0 * sp, sizeof(float) * sp, sizeof(float), static_cast<size_t>(c),
-                                cudaMemcpyDefault, p->stream));
-      SB_CUDA(cudaMemcpyAsync(sy, y + r0, sizeof(float) * c, cudaMemcpyDefault, p->stream));
-      if (w) SB_CUDA(cudaMemcpyAsync(sw, w + r0, sizeof(float) * c, cudaMemcpyDefault, p->stream));
-      SB_TRY(add(ss, 1, sy, w ? sw : nullptr, r0, c));
-    }
-    SB_CUDA(cudaStreamSynchronize(p->stream));
-  }
-  p->rows += rows;
-  return SB_OK;
-}
-
-int sb_perf_summary_get(sb_perf_t* p, sb_perf_summary* out) {
-  SB_CHECK(p, SB_ERR_STATE, "performance handle not initialized.");
-  SB_CHECK(out, SB_ERR_INVALID, "out is null");
-  SB_TRY(perf_prepare(p));
-  const double qnan = std::numeric_limits<double>::quiet_NaN();
-  sb_perf_summary s;
-  s.rows = p->rows; s.pos = p->P; s.neg = p->N; s.n_distinct = p->m; s.w_pos = p->Wp; s.w_neg = p->Wn;
-  s.auc = s.w_auc = s.ap = s.w_ap = s.ks = s.w_ks = qnan;
-  s.ks_score = s.w_ks_score = std::numeric_limits<float>::quiet_NaN();
-  if (p->m > 0) {
-    const int G = static_cast<int>(std::min<long long>(PERF_SUM_BLOCKS, (p->m + PERF_THREADS - 1) / PERF_THREADS));
-    SB_TRY(launch_kernel(perf_summary_kernel, dim3(G), dim3(PERF_THREADS), 0, p->stream, false, static_cast<const long long*>(p->rtp),
-                         static_cast<const long long*>(p->rfp), static_cast<const double*>(p->rwtp),
-                         static_cast<const double*>(p->rwfp), p->m, p->parts));
-    SB_TRY(launch_kernel(perf_summary_final_kernel, dim3(1), dim3(1), 0, p->stream, false, static_cast<const PerfPart*>(p->parts), G,
-                         static_cast<const float*>(p->rt), p->result));
-    PerfResult r;
-    SB_CUDA(cudaMemcpyAsync(&r, p->result, sizeof(r), cudaMemcpyDeviceToHost, p->stream));
-    SB_CUDA(cudaStreamSynchronize(p->stream));
-    const long long pn = p->P * p->N;
-    const double wpn = p->Wp * p->Wn;
-    if (pn > 0) {
-      s.auc = static_cast<double>(r.a.a2) / static_cast<double>(2 * pn);
-      s.ks = static_cast<double>(r.a.ks) / static_cast<double>(pn);
-      s.ks_score = r.ks_t;
-    }
-    if (p->P > 0) s.ap = r.a.ap / static_cast<double>(p->P);
-    if (wpn > 0.0) {
-      s.w_auc = r.a.wauc / wpn;
-      s.w_ks = r.a.wks / wpn;
-      s.w_ks_score = r.wks_t;
-    }
-    if (p->Wp > 0.0) s.w_ap = r.a.wap / p->Wp;
-  }
-  *out = s;
-  return SB_OK;
-}
-
-int sb_perf_points(sb_perf_t* p, int32_t axis, int32_t weighted, const double* levels, int32_t n, sb_perf_point* out) {
-  SB_CHECK(p, SB_ERR_STATE, "performance handle not initialized.");
-  SB_CHECK(axis >= SB_PERF_ACTION_RATE && axis <= SB_PERF_SCORE, SB_ERR_INVALID, "unknown axis %d", axis);
-  SB_CHECK(n >= 0, SB_ERR_INVALID, "n = %d < 0", n);
-  SB_CHECK(n == 0 || (levels && out), SB_ERR_INVALID, "levels and out must not be null");
-  for (int i = 0; i < n; ++i) {
-    SB_CHECK(!std::isnan(levels[i]), SB_ERR_INVALID, "level %d is NaN", i);
-    SB_CHECK(axis == SB_PERF_SCORE || (levels[i] >= 0.0 && levels[i] <= 1.0), SB_ERR_INVALID, "level %d = %g outside [0, 1]", i,
-             levels[i]);
-  }
-  SB_TRY(perf_prepare(p));
-  if (n == 0) return SB_OK;
-  double den = 1.0;
-  if (axis != SB_PERF_SCORE) {
-    den = weighted ? (axis == SB_PERF_ACTION_RATE ? p->Wp + p->Wn : axis == SB_PERF_RECALL ? p->Wp : p->Wn)
-                   : static_cast<double>(axis == SB_PERF_ACTION_RATE ? p->P + p->N : axis == SB_PERF_RECALL ? p->P : p->N);
-    SB_CHECK(den > 0.0, SB_ERR_INVALID, "the %s%s total is 0: the axis is undefined", weighted ? "weighted " : "",
-             axis == SB_PERF_ACTION_RATE ? "row" : axis == SB_PERF_RECALL ? "positive" : "negative");
-  }
-  if (p->m == 0) {                     // score axis of an empty handle: every point is the empty point
-    for (int i = 0; i < n; ++i) out[i] = sb_perf_point{std::numeric_limits<float>::infinity(), 0, 0, 0.0, 0.0};
-    return SB_OK;
-  }
-  if (n > p->pt_cap) {                 // kept for the next call: an allocation here would synchronise the device
-    p->release(&p->d_levels, p->pt_cap); p->release(&p->d_points, p->pt_cap);
-    p->pt_cap = 0;
-    SB_TRY(p->alloc(&p->d_levels, n)); SB_TRY(p->alloc(&p->d_points, n));
-    p->pt_cap = n;
-  }
-  SB_CUDA(cudaMemcpyAsync(p->d_levels, levels, sizeof(double) * n, cudaMemcpyHostToDevice, p->stream));
-  SB_TRY(launch_kernel(perf_points_kernel, dim3(static_cast<unsigned>((n + 127) / 128)), dim3(128), 0, p->stream, false,
-                       static_cast<const float*>(p->rt), static_cast<const long long*>(p->rtp), static_cast<const long long*>(p->rfp),
-                       static_cast<const double*>(p->rwtp), static_cast<const double*>(p->rwfp), p->m, static_cast<int>(axis),
-                       weighted ? 1 : 0, den, static_cast<const double*>(p->d_levels), static_cast<int>(n), p->d_points));
-  SB_CUDA(cudaMemcpyAsync(out, p->d_points, sizeof(sb_perf_point) * n, cudaMemcpyDeviceToHost, p->stream));
-  SB_CUDA(cudaStreamSynchronize(p->stream));
-  return SB_OK;
-}
-
-int sb_perf_sync(sb_perf_t* p) {
-  SB_CHECK(p, SB_ERR_STATE, "performance handle not initialized.");
-  SB_CUDA(cudaSetDevice(p->device));
-  SB_CUDA(cudaStreamSynchronize(p->stream));
-  return SB_OK;
-}
-
-void* sb_perf_stream(sb_perf_t* p) { return p ? reinterpret_cast<void*>(p->stream) : nullptr; }
-
-int sb_debug_perf_runs(sb_perf_t* p, float* t, int64_t* tp, int64_t* fp, double* wtp, double* wfp, int64_t cap, int64_t* n_runs) {
-  SB_CHECK(p, SB_ERR_STATE, "performance handle not initialized.");
-  SB_CHECK(n_runs && cap >= 0, SB_ERR_INVALID, "null n_runs or cap < 0");
-  SB_TRY(perf_prepare(p));
-  const size_t c = static_cast<size_t>(std::min<long long>(cap, p->m));
-  if (c > 0) {
-    if (t) SB_CUDA(cudaMemcpyAsync(t, p->rt, sizeof(float) * c, cudaMemcpyDeviceToHost, p->stream));
-    if (tp) SB_CUDA(cudaMemcpyAsync(tp, p->rtp, sizeof(int64_t) * c, cudaMemcpyDeviceToHost, p->stream));
-    if (fp) SB_CUDA(cudaMemcpyAsync(fp, p->rfp, sizeof(int64_t) * c, cudaMemcpyDeviceToHost, p->stream));
-    if (wtp) SB_CUDA(cudaMemcpyAsync(wtp, p->rwtp, sizeof(double) * c, cudaMemcpyDeviceToHost, p->stream));
-    if (wfp) SB_CUDA(cudaMemcpyAsync(wfp, p->rwfp, sizeof(double) * c, cudaMemcpyDeviceToHost, p->stream));
-    SB_CUDA(cudaStreamSynchronize(p->stream));
-  }
-  *n_runs = p->m;
-  return SB_OK;
-}
-
-int sb_debug_perf_bytes(sb_perf_t* p, int64_t* out) {
-  SB_CHECK(p, SB_ERR_STATE, "performance handle not initialized.");
-  SB_CHECK(out, SB_ERR_INVALID, "null argument");
-  *out = p->bytes;
-  return SB_OK;
 }
 
 // ================================================================================================

@@ -156,6 +156,13 @@ int check_device(int device, int* num_sms) {
   return SB_OK;
 }
 
+int ptr_device(const void* p) {
+  if (!p) return -1;
+  cudaPointerAttributes at;
+  if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return -1; }
+  return at.type == cudaMemoryTypeDevice ? at.device : -1;
+}
+
 int Net::init(const sb_net_desc* d, int device_, bool training_) {
   SB_TRY(validate_desc(d));
   SB_TRY(check_device(device_, &num_sms));
@@ -426,6 +433,31 @@ int Net::refresh_shadows() {
   shadow_refresh_kernel<<<n_work_all, 256, 0, stream>>>(work_all, theta);
   SB_CUDA(cudaGetLastError());
   return SB_OK;
+}
+
+int write_desc(cudaStream_t st, const StepIn& in, const Batch* b, float lr_t, float gscale, unsigned int epoch, float2* hist) {
+  static const Batch none{};
+  const Batch& x = b ? *b : none;
+  return launch_kernel(set_batch_kernel, dim3(1), dim3(1), 0, st, false, in.desc, x.X, x.y, x.w, lr_t, gscale, epoch, x.row0,
+                       x.nz_prefix, x.rows, in.scal, hist, x.order);
+}
+
+void write_desc_max_shared() {
+  cudaFuncSetAttribute(set_batch_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+}
+
+int write_desc_preload() {
+  cudaFuncAttributes a;
+  SB_CUDA(cudaFuncGetAttributes(&a, set_batch_kernel));
+  return SB_OK;
+}
+
+Batch host_batch(const Net& n, const float* X, const float* y, const float* w, int rows, Feed feed) {
+  Batch b;
+  b.feed = feed;
+  b.X = X; b.y = y; b.w = w ? w : n.ones;
+  b.rows = rows;
+  return b;
 }
 
 int Net::enqueue_load(const StepIn& in, int rows, float* clear, long long clear_n) {

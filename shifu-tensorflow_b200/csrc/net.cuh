@@ -41,6 +41,16 @@ struct StepIn {
   Operand0 x0;
 };
 
+// One step's batch: everything set_batch_kernel reads besides the update's scalars (write_desc)
+struct Batch {
+  Feed feed = Feed::HOST;
+  const float *X = nullptr, *y = nullptr, *w = nullptr;
+  int row0 = 0;                     // RESIDENT: first row in the resident set
+  const int* nz_prefix = nullptr;   // RESIDENT: n_nz is published from the set's prefix counts
+  const int* order = nullptr;       // ORDERED: the batch's slice of the row order
+  int rows = 0;
+};
+
 inline int pairs_of(int np) { return np == 3 ? 6 : (np == 2 ? 3 : 1); }
 
 struct Net {
@@ -65,7 +75,7 @@ struct Net {
   // is set by the trainer BEFORE init(): room for its gradient buffer and flag block behind the parameters.
   char* arena = nullptr;
   size_t arena_bytes = 0, arena_extra_bytes = 0;
-  // Set BEFORE init() on an ensemble member (capi.cu sb_ensemble): the net runs on input_from's stream and uses its input
+  // Set BEFORE init() on an ensemble member (score.cu sb_ensemble): the net runs on input_from's stream and uses its input
   // staging (stX, Xb / Xf) instead of creating its own; input_from must have the same F and max_batch and outlive it.
   const Net* input_from = nullptr;
   size_t s1_off = 0, s2_off = 0, shadow_off = 0, extra_off = 0;   // byte offsets inside the arena (theta at 0)
@@ -186,9 +196,21 @@ struct Net {
   int dw_max_split() const { return det ? 2 : 0; }
 };
 
+// The only writer of a step descriptor: batch `b` (nullptr: an update without a batch), the update's scalars and the
+// step's slot in the loss history, into slot `in` on stream `st`
+int write_desc(cudaStream_t st, const StepIn& in, const Batch* b, float lr_t, float gscale, unsigned int epoch, float2* hist);
+// set_batch_kernel is static (one copy per translation unit): these reach the copy write_desc launches.  The trainer keeps
+// it in the step's shared-memory carve-out (see Net::init) and loads it before an exchange (preload_exchange_kernels).
+void write_desc_max_shared();
+int write_desc_preload();
+// a batch of fp32 rows on the device (the staging area, or the fp32 resident set); w == nullptr weighs every row 1
+Batch host_batch(const Net& n, const float* X, const float* y, const float* w, int rows, Feed feed = Feed::HOST);
+
 int validate_desc(const sb_net_desc* d);
 // makes `device` current if it is an sm_90 device (SB_ERR_CUDA when there is none)
 int check_device(int device, int* num_sms);
+// the device a pointer lives on, or -1 for host memory (pageable, pinned or managed) and for nullptr
+int ptr_device(const void* p);
 // a wide+deep index matrix of n entries: each a one-hot column in [0, n_onehot) or -1 (missing); anything else is
 // SB_ERR_INVALID (a negative index other than -1 is not "missing", and a numpy caller would read it as a row from the end)
 int check_sparse_idx(const int32_t* idx, long long n, int n_onehot);

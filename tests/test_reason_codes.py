@@ -30,7 +30,7 @@ SENTINEL = 0x7FCDCDCD
 
 
 def expected_reason_routes(prec, F, hidden, rows, n_cols, sms):
-    """the launches of a call's last row chunk's z0 and last piece (capi.cu sens_forward, then sens_topk_kernel)"""
+    """the launches of a call's last row chunk's z0 and last piece (score.cu sens_forward, then sens_topk_kernel)"""
     r = expected_sens_routes(prec, F, hidden, rows, n_cols, sms)
     assert r.endswith("+sens_reduce")
     return r[:-len("sens_reduce")] + "sens_topk"

@@ -84,7 +84,7 @@ def _wide(M, N, K, sms):
 
 
 def expected_routes(prec, F, hidden, rows, sms):
-    """the launches of a model's forward of `rows` rows (capi.cu model_forward, Net::enqueue_*)"""
+    """the launches of a model's forward of `rows` rows (score.cu ScoreCore::forward, Net::enqueue_*)"""
     if prec == FP32 and rows <= SMALL_ROWS:
         return "score_rows"
     r = ["load_batch<fp32>" if prec == FP32 else "load_batch<bf16>"]

@@ -26,7 +26,7 @@ NPARTS = {FP32: 1, BF16: 1, FP32_TC: 3, BF16X2: 2}
 
 
 def chunk_rows(prec, n_cols):
-    """rows per row chunk (capi.cu sens_chunk_rows)"""
+    """rows per row chunk (score.cu sens_chunk_rows)"""
     mb = CHUNK[prec]
     return min(mb // 2, max(64, mb // (n_cols + 1)))
 
@@ -39,7 +39,7 @@ def _next_prime(n):
 
 
 def expected_sens_routes(prec, F, hidden, rows, n_cols, sms):
-    """the launches of a call's last row chunk's z0 and last piece (capi.cu sens_forward)"""
+    """the launches of a call's last row chunk's z0 and last piece (score.cu sens_forward)"""
     R = chunk_rows(prec, n_cols)
     rc = rows - R * ((rows - 1) // R)
     cp = CHUNK[prec] // R - 1
