@@ -21,7 +21,7 @@ carry; e_a includes 2u |a| where the kernel rebuilds A_L from its bf16 parts in 
 import numpy as np
 
 from conftest import bf16_round
-from out_layer_ref import ACTS, U, activation, output_layer
+from out_layer_ref import ACTS, MSE, U, activation, output_layer
 
 FP32, BF16, FP32_TC, BF16X2 = 0, 1, 2, 3
 NPARTS = {FP32: 1, BF16: 1, FP32_TC: 3, BF16X2: 2}
@@ -59,19 +59,31 @@ def _carried(e, W):
     return KAPPA * np.sqrt((e * e) @ (W * W))
 
 
-def hidden_forward(X, layers, acts, prec, exact=None):
+def stored_inputs(X, prec):
+    """the rows as layer 0 reads them: bf16 in BF16, else fp32 (float64)"""
+    return (bf16_round(X) if prec == BF16 else np.asarray(X, np.float32)).astype(np.float64)
+
+
+def pre_activation(a, e, W, b, prec):
+    """-> (z, e_z) float64: a W + b of inputs a within e (None: exact) and its bound (module docstring)"""
+    Wm = (bf16_round(W) if prec == BF16 else W).astype(np.float64)
+    b64 = b.astype(np.float64)
+    z = a @ Wm + b64
+    e_z = contraction_c(prec, W.shape[0]) * (np.abs(a) @ np.abs(Wm)) + 4 * U * (np.abs(z) + np.abs(b64))
+    if e is not None:
+        e_z += _carried(e, Wm)
+    return z, e_z
+
+
+def hidden_forward(X, layers, acts, prec, exact=None, z0=None):
     """-> (A_L, e_a) float64 [M, H_L]: the last hidden layer as the kernels store it, and its bound (module docstring).
-    exact (a list): receives each BF16 layer's fraction of elements known exactly"""
+    exact (a list): receives each BF16 layer's fraction of elements known exactly.  z0: (z, e_z) of layer 0's
+    pre-activation, where the caller evaluates it itself (wide_deep_ref.py); X is then not read"""
     bf = prec == BF16
-    a = (bf16_round(X) if bf else np.asarray(X, np.float32)).astype(np.float64)
+    a = None if z0 is not None else stored_inputs(X, prec)
     e = None                                         # the inputs are exact
-    for (W, b), act in zip(layers[:-1], acts):
-        Wm = (bf16_round(W) if bf else W).astype(np.float64)
-        b64 = b.astype(np.float64)
-        z = a @ Wm + b64
-        e_z = contraction_c(prec, W.shape[0]) * (np.abs(a) @ np.abs(Wm)) + 4 * U * (np.abs(z) + np.abs(b64))
-        if e is not None:
-            e_z += _carried(e, Wm)
+    for l, ((W, b), act) in enumerate(zip(layers[:-1], acts)):
+        z, e_z = z0 if (l == 0 and z0 is not None) else pre_activation(a, e, W, b, prec)
         v = activation(z, act)
         if bf:
             with np.errstate(over="ignore"):         # exp of a saturated sigmoid's argument
@@ -97,9 +109,29 @@ def out_unit(a, e_a, wo, bo, y, w, act, loss, d):
                             e_z_add=_carried(e_a, np.asarray(wo, np.float64)[:, None])[:, 0])
 
 
-def score(X, layers, acts, prec, exact=None):
-    """-> (y_hat, e_yhat) float64 [M] of the rows X [M, F] (fp32) in precision mode prec"""
-    a, e = hidden_forward(X, layers, acts, prec, exact)
+def validation_loss(a, e_a, wo, bo, y, w, act, B, depth):
+    """-> (loss, bound) of a validation pass (Trainer.eval_loss, eval_loss_sparse) over A_L = a within e_a: the MSE sums of
+    output_layer over pieces of at most B rows, added up and divided by n_nz.  depth(m): the reduction depth of the
+    output-layer launch over a piece of m rows.  A set without a non-zero weight: (0, 0)"""
+    n, nnz = len(y), np.count_nonzero(w)
+    if nnz == 0:
+        return 0.0, 0.0
+    total, bound = 0.0, 0.0
+    for r0 in range(0, n, B):
+        s = slice(r0, min(n, r0 + B))
+        ref = out_unit(a[s], e_a[s], wo, bo, y[s], w[s], act, MSE, depth(s.stop - s.start))
+        total += ref["loss"][0]
+        bound += ref["loss"][1] + ref["d"] * U * abs(ref["loss"][0])
+    return total / nnz, bound / nnz + 2 * U * abs(total / nnz)
+
+
+def scores(a, e, layers, acts):
+    """-> (y_hat, e_yhat) float64 [M] of the output unit on A_L = a within e"""
     M = a.shape[0]
     wo, bo = layers[-1]
     return out_unit(a, e, wo, bo, np.zeros(M, np.float32), np.ones(M, np.float32), acts[-1], 0, 1)["yhat"]
+
+
+def score(X, layers, acts, prec, exact=None):
+    """-> (y_hat, e_yhat) float64 [M] of the rows X [M, F] (fp32) in precision mode prec"""
+    return scores(*hidden_forward(X, layers, acts, prec, exact), layers, acts)

@@ -13,8 +13,8 @@ outside E's batch columns or W_e's gradient rows."""
 import numpy as np
 import pytest
 
-from conftest import bf16_round
 from oracle import wide_deep as wd
+from wide_deep_ref import stored_parts
 
 FP32, BF16, FP32_TC, BF16X2 = 0, 1, 2, 3
 PRECS = {"fp32": FP32, "bf16": BF16, "fp32tc": FP32_TC, "bf16x2": BF16X2}
@@ -33,18 +33,6 @@ def _report_worst():
     yield
     if _worst:
         print("\nworst error / bound: " + ", ".join("%s %.3g" % (k, _worst[k]) for k in OUTS if k in _worst))
-
-
-def _stored(x, prec):
-    """x as the step stores it: [np, ...] float64 of the bf16 parts (bf16_residual), or the fp32 values"""
-    if prec == FP32:
-        return x.astype(np.float64)[None]
-    r, parts = x.astype(np.float32), []
-    for _ in range(NP[prec]):
-        p = bf16_round(r)
-        parts.append(p.astype(np.float64))
-        r = (r - p).astype(np.float32)
-    return np.stack(parts)
 
 
 def _index(rows, n_cat, seed, hot=None):
@@ -70,7 +58,7 @@ def _gather(sb, prec, idx, n_onehot, H, seed):
     E, guard = sb.capi.debug_embed(prec, idx, n_onehot, H, We=We)
     assert guard == 0, "%d guard elements around E changed" % guard
     O = wd.onehot_matrix(idx, n_onehot, np.float64)
-    parts = _stored(We, prec)
+    parts = stored_parts(We, prec)
     want = O @ parts.sum(axis=0)
     tol = idx.shape[1] * NP[prec] * U * (O @ np.abs(parts).sum(axis=0))
     err = np.abs(E - want)
@@ -86,7 +74,7 @@ def _scatter(sb, prec, idx, n_onehot, H, seed):
     got, guard = sb.capi.debug_embed(prec, idx, n_onehot, H, dZ=dZ, grad=init)
     assert guard == 0, "%d guard elements around W_e's gradient rows changed" % guard
     O = wd.onehot_matrix(idx, n_onehot, np.float64)
-    parts = _stored(dZ, prec)
+    parts = stored_parts(dZ, prec)
     count = O.sum(axis=0)[:, None]
     gain = O.T @ parts.sum(axis=0)
     tol = (count + NP[prec]) * U * (O.T @ np.abs(parts).sum(axis=0) + np.abs(init))

@@ -17,8 +17,8 @@ import zlib
 import numpy as np
 import pytest
 
-from out_layer_ref import ACTS, MSE, U
-from score_ref import BF16, BF16X2, FP32, FP32_TC, hidden_forward, out_unit, score, unflatten
+from out_layer_ref import ACTS
+from score_ref import BF16, BF16X2, FP32, FP32_TC, hidden_forward, score, unflatten, validation_loss
 from test_out_layer import _depth, expected_route
 
 PRECS = {"fp32": FP32, "bf16": BF16, "fp32_tc": FP32_TC, "bf16x2": BF16X2}
@@ -394,15 +394,7 @@ def test_validation_pass(sb, prec):
     _check(pred, score(X, layers, _acts(acts), p), p, "predict %s" % prec)
     a, e_a = hidden_forward(X, layers, _acts(acts), p)
     route = expected_route(p, hidden[-1], False, "eval")
-    total, bound = 0.0, 0.0
-    for r0 in range(0, n, B):
-        s = slice(r0, min(n, r0 + B))
-        ref = out_unit(a[s], e_a[s], layers[-1][0], layers[-1][1], y[s], w[s], ACTS[acts[-1]], MSE,
-                       _depth(route, s.stop - s.start, 0))
-        total += ref["loss"][0]
-        bound += ref["loss"][1] + ref["d"] * U * abs(ref["loss"][0])
-    nnz = np.count_nonzero(w)
-    want, tol = total / nnz, bound / nnz + 2 * U * abs(total / nnz)
+    want, tol = validation_loss(a, e_a, layers[-1][0], layers[-1][1], y, w, ACTS[acts[-1]], B, lambda m: _depth(route, m, 0))
     _notes["validation %s loss error / bound" % prec] = "%.3g" % (abs(loss - want) / tol)
     assert abs(loss - want) <= tol, (loss, want, tol)
 
