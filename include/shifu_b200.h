@@ -416,6 +416,31 @@ void* sb_ensemble_stream(sb_ensemble_t* e);
  * the ensemble allocated (every member's network and workspace, the one input staging, the member score slots). */
 int sb_debug_ensemble_routes(sb_ensemble_t* e, char* out, int32_t cap);
 int sb_debug_ensemble_bytes(sb_ensemble_t* e, int64_t* out);
+/* Explaining the ensemble's score (DESIGN §6j): column sensitivity and per-row reason codes of one statistic of the
+ * members' scores.  With s_g(x) member g's score as sb_model_sensitivity computes it for that member alone (z0 in fp32,
+ * the rank-1 update, layers 1..L) and S(x) the statistic `stat` of s_0 .. s_{K-1} under exactly the rules above (fp32
+ * mean in member order, first-wins max / min, the even-K median (a + b) * 0.5f, a NaN giving the quiet NaN):
+ *   d[r,k] = S(x_r) - S(x_r with column cols[k] set to values[k]).
+ * Every other rule is sb_model_sensitivity's / sb_model_reason_codes': cols / n_cols / values, w, the sums, deltas, k,
+ * order, the outputs and where they may live, and their guarantees (the same bits on repeat; sums that do not depend on
+ * deltas or on the pointer kinds; d exactly +0 wherever x[r, cols[k]] == values[k]; fp64 sums added in a fixed order;
+ * every reason-code d bit-identical to sb_ensemble_sensitivity's delta at its position; scores = S(x_r) as the call
+ * computes it).  Rows go in the chunks and pieces sb_model_sensitivity uses at the members' shared max_batch: each row
+ * chunk is loaded once and each member computes its own z0; per piece every member runs its perturbation and forward
+ * into its score slot, so member g's pair scores are bit-identical to those of an sb_model_t of member g, and one launch
+ * forms S of every pair.  A one-member ensemble gives sb_model_sensitivity's bits for every stat.
+ * Synchronous; takes the ensemble's device lock, so it is safe beside sb_ensemble_score_row_f64 callers.
+ * Errors, all found before any device work: a null handle SB_ERR_STATE; a stat outside 0..3 SB_ERR_INVALID; otherwise
+ * as the model functions report them.  The routes after a call: the last row chunk's load and every member's z0 GEMM,
+ * then per member in member order its sens_perturb, its layers and its output unit, then "ensemble_stat", then
+ * "sens_reduce" or "sens_topk". */
+enum { SB_STAT_MEAN = 0, SB_STAT_MAX = 1, SB_STAT_MIN = 2, SB_STAT_MEDIAN = 3 };
+int sb_ensemble_sensitivity(sb_ensemble_t* e, int32_t stat, const float* X, const float* w, int64_t rows,
+                            const int32_t* cols, int32_t n_cols, const float* values,
+                            double* sum_sq, double* sum, double* w_sum, float* deltas);
+int sb_ensemble_reason_codes(sb_ensemble_t* e, int32_t stat, const float* X, int64_t rows, const int32_t* cols,
+                             int32_t n_cols, const float* values, int32_t k, int32_t order,
+                             int32_t* pos, float* d, float* scores);
 
 /* ---- model performance: what `shifu eval` reports about a scored set (ROC AUC, PR AUC, KS, and the gains / ROC / PR /
  * score-bucket lists), computed on the GPU from one radix sort of the scores.  Shifu's evaluator is not part of this

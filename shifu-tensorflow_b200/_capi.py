@@ -182,6 +182,10 @@ PROTOTYPES = {
     "sb_ensemble_stream": (C.c_void_p, [_vp]),
     "sb_debug_ensemble_routes": (C.c_int, [_vp, C.c_char_p, C.c_int32]),
     "sb_debug_ensemble_bytes": (C.c_int, [_vp, _P(C.c_int64)]),
+    "sb_ensemble_sensitivity": (C.c_int, [_vp, C.c_int32, _vp, _vp, C.c_int64, _P(C.c_int32), C.c_int32, _f32p, _f64p, _f64p, _f64p,
+                                          _vp]),
+    "sb_ensemble_reason_codes": (C.c_int, [_vp, C.c_int32, _vp, C.c_int64, _P(C.c_int32), C.c_int32, _f32p, C.c_int32, C.c_int32,
+                                           _vp, _vp, _vp]),
     "sb_perf_create": (C.c_int, [C.c_int, C.c_int64, _P(_vp)]),
     "sb_perf_destroy": (C.c_int, [_vp]),
     "sb_perf_reset": (C.c_int, [_vp]),
@@ -712,6 +716,64 @@ class Trainer:
         check(lib().sb_trainer_export_savedmodel(self._h, export_dir.encode()))
 
 
+def _sensitivity(n_features, call, X, w, cols, values, deltas) -> dict:
+    """Model.sensitivity / Ensemble.sensitivity: the arguments checked and converted, then call(X, w, rows, cols, n_cols,
+    values, sum_sq, sum, w_sum, deltas) of the C entry point"""
+    xp, shape = _in_ptr(X)
+    if len(shape) != 2 or shape[1] != n_features:
+        raise ValueError("X must be [rows, %d]" % n_features)
+    rows = int(shape[0])
+    wp, wshape = _in_ptr(w) if w is not None else (None, (rows,))
+    if int(np.prod(wshape)) != rows:
+        raise ValueError("w must hold one weight per row")
+    cl = None if cols is None else np.ascontiguousarray(cols, dtype=np.int32).reshape(-1)
+    n_cols = n_features if cl is None else cl.size
+    vl = None if values is None else _f32(values).reshape(-1)
+    if vl is not None and vl.size != n_cols:
+        raise ValueError("values must hold one value per list position (%d)" % n_cols)
+    sum_sq, total, w_sum = np.zeros(n_cols), np.zeros(n_cols), C.c_double()
+    if deltas is True:
+        d_out = np.empty((rows, n_cols), np.float32)
+        dp = d_out.ctypes.data_as(_vp)
+    elif deltas is False or deltas is None:
+        d_out, dp = None, None
+    else:
+        d_out = deltas
+        dp = _in_ptr(deltas)[0]
+    check(call(xp, wp, rows, None if cl is None else cl.ctypes.data_as(_P(C.c_int32)), 0 if cl is None else cl.size,
+               None if vl is None else _ptr(vl), sum_sq.ctypes.data_as(_f64p), total.ctypes.data_as(_f64p), C.byref(w_sum), dp))
+    return {"sum_sq": sum_sq, "sum": total, "w_sum": float(w_sum.value), "deltas": d_out}
+
+
+def _reason_codes(n_features, call, X, k, cols, values, order, scores, pos, d) -> dict:
+    """Model.reason_codes / Ensemble.reason_codes: the arguments checked and converted, then call(X, rows, cols, n_cols,
+    values, k, order, pos, d, scores) of the C entry point"""
+    xp, shape = _in_ptr(X)
+    if len(shape) != 2 or shape[1] != n_features:
+        raise ValueError("X must be [rows, %d]" % n_features)
+    rows = int(shape[0])
+    cl = None if cols is None else np.ascontiguousarray(cols, dtype=np.int32).reshape(-1)
+    n_cols = n_features if cl is None else cl.size
+    vl = None if values is None else _f32(values).reshape(-1)
+    if vl is not None and vl.size != n_cols:
+        raise ValueError("values must hold one value per list position (%d)" % n_cols)
+    if order not in REASON_ORDERS:
+        raise ValueError("order must be one of %s" % sorted(REASON_ORDERS))
+
+    def out(buf, dtype, shape):
+        if buf is None or buf is True:
+            a = np.empty(shape, dtype)
+            return a, a.ctypes.data_as(_vp)
+        return buf, _in_ptr(buf, dtype)[0]
+
+    p_out, pp = out(pos, np.int32, (rows, k))
+    d_out, dp = out(d, np.float32, (rows, k))
+    s_out, sp = out(scores, np.float32, (rows,)) if scores is not False and scores is not None else (None, None)
+    check(call(xp, rows, None if cl is None else cl.ctypes.data_as(_P(C.c_int32)), 0 if cl is None else cl.size,
+               None if vl is None else _ptr(vl), int(k), REASON_ORDERS[order], pp, dp, sp))
+    return {"pos": p_out, "d": d_out, "scores": s_out}
+
+
 class Model:
     """Owns one sb_model_t (batched scorer)."""
 
@@ -772,31 +834,7 @@ class Model:
         X / w: numpy arrays (host) or CUDA tensors / DeviceArrays on the model's device.  cols: None for every column in
         order.  values: None for 0 at every position.  deltas: False (not computed), True (returned as a host array) or a
         device buffer of rows * n_cols floats to write them into."""
-        xp, shape = _in_ptr(X)
-        if len(shape) != 2 or shape[1] != self.n_features:
-            raise ValueError("X must be [rows, %d]" % self.n_features)
-        rows = int(shape[0])
-        wp, wshape = _in_ptr(w) if w is not None else (None, (rows,))
-        if int(np.prod(wshape)) != rows:
-            raise ValueError("w must hold one weight per row")
-        cl = None if cols is None else np.ascontiguousarray(cols, dtype=np.int32).reshape(-1)
-        n_cols = self.n_features if cl is None else cl.size
-        vl = None if values is None else _f32(values).reshape(-1)
-        if vl is not None and vl.size != n_cols:
-            raise ValueError("values must hold one value per list position (%d)" % n_cols)
-        sum_sq, total, w_sum = np.zeros(n_cols), np.zeros(n_cols), C.c_double()
-        if deltas is True:
-            d_out = np.empty((rows, n_cols), np.float32)
-            dp = d_out.ctypes.data_as(_vp)
-        elif deltas is False or deltas is None:
-            d_out, dp = None, None
-        else:
-            d_out = deltas
-            dp = _in_ptr(deltas)[0]
-        check(lib().sb_model_sensitivity(self._h, xp, wp, rows, None if cl is None else cl.ctypes.data_as(_P(C.c_int32)),
-                                         0 if cl is None else cl.size, None if vl is None else _ptr(vl),
-                                         sum_sq.ctypes.data_as(_f64p), total.ctypes.data_as(_f64p), C.byref(w_sum), dp))
-        return {"sum_sq": sum_sq, "sum": total, "w_sum": float(w_sum.value), "deltas": d_out}
+        return _sensitivity(self.n_features, lambda *a: lib().sb_model_sensitivity(self._h, *a), X, w, cols, values, deltas)
 
     def reason_codes(self, X, k, cols=None, values=None, order="raise", scores=False, pos=None, d=None) -> dict:
         """Per-row reason codes (sb_model_reason_codes): for each row, the k list positions whose deltas
@@ -806,31 +844,8 @@ class Model:
         X: a numpy array (host) or a CUDA tensor / DeviceArray on the model's device.  cols / values as in sensitivity.
         pos / d: None (returned as host arrays) or a buffer of rows * k int32 / float32 to write into; scores: False (not
         computed), True (a host array) or a buffer of rows floats."""
-        xp, shape = _in_ptr(X)
-        if len(shape) != 2 or shape[1] != self.n_features:
-            raise ValueError("X must be [rows, %d]" % self.n_features)
-        rows = int(shape[0])
-        cl = None if cols is None else np.ascontiguousarray(cols, dtype=np.int32).reshape(-1)
-        n_cols = self.n_features if cl is None else cl.size
-        vl = None if values is None else _f32(values).reshape(-1)
-        if vl is not None and vl.size != n_cols:
-            raise ValueError("values must hold one value per list position (%d)" % n_cols)
-        if order not in REASON_ORDERS:
-            raise ValueError("order must be one of %s" % sorted(REASON_ORDERS))
-
-        def out(buf, dtype, shape):
-            if buf is None or buf is True:
-                a = np.empty(shape, dtype)
-                return a, a.ctypes.data_as(_vp)
-            return buf, _in_ptr(buf, dtype)[0]
-
-        p_out, pp = out(pos, np.int32, (rows, k))
-        d_out, dp = out(d, np.float32, (rows, k))
-        s_out, sp = out(scores, np.float32, (rows,)) if scores is not False and scores is not None else (None, None)
-        check(lib().sb_model_reason_codes(self._h, xp, rows, None if cl is None else cl.ctypes.data_as(_P(C.c_int32)),
-                                          0 if cl is None else cl.size, None if vl is None else _ptr(vl), int(k),
-                                          REASON_ORDERS[order], pp, dp, sp))
-        return {"pos": p_out, "d": d_out, "scores": s_out}
+        return _reason_codes(self.n_features, lambda *a: lib().sb_model_reason_codes(self._h, *a), X, k, cols, values, order,
+                             scores, pos, d)
 
     def sync(self):
         check(lib().sb_model_sync(self._h))
@@ -936,6 +951,27 @@ class Ensemble:
         out = np.empty(self.k + 4, np.float64)
         check(lib().sb_ensemble_score_row_f64(self._h, row.ctypes.data_as(_f64p), row.size, out.ctypes.data_as(_f64p)))
         return out
+
+    def _stat(self, stat: str) -> int:
+        if stat not in ENSEMBLE_STATS:
+            raise ValueError("stat must be one of %s" % (ENSEMBLE_STATS,))
+        return ENSEMBLE_STATS.index(stat)
+
+    def sensitivity(self, X, w=None, cols=None, values=None, deltas=False, stat="mean") -> dict:
+        """Column sensitivity of one statistic S of the member scores (sb_ensemble_sensitivity): for each list position
+        k, d[r, k] = S(X[r]) - S(X[r] with column cols[k] set to values[k]), stat one of ENSEMBLE_STATS.  Arguments and
+        result as Model.sensitivity."""
+        st = self._stat(stat)
+        return _sensitivity(self.n_features, lambda *a: lib().sb_ensemble_sensitivity(self._h, st, *a), X, w, cols, values,
+                            deltas)
+
+    def reason_codes(self, X, k, cols=None, values=None, order="raise", stat="mean", scores=False, pos=None, d=None) -> dict:
+        """Per-row reason codes of one statistic S of the member scores (sb_ensemble_reason_codes): the k list positions
+        whose deltas d = S(X[r]) - S(X[r] with column cols[j] set to values[j]) rank first in `order`, stat one of
+        ENSEMBLE_STATS; scores: S(X[r]).  Arguments and result as Model.reason_codes."""
+        st = self._stat(stat)
+        return _reason_codes(self.n_features, lambda *a: lib().sb_ensemble_reason_codes(self._h, st, *a), X, k, cols, values,
+                             order, scores, pos, d)
 
     def sync(self):
         check(lib().sb_ensemble_sync(self._h))

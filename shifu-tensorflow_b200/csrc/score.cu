@@ -1,6 +1,7 @@
 // extern "C" surface of the scorers: the model (sb_model_*: scores, compute(), column sensitivity, reason codes) and the
-// bagged ensemble (sb_ensemble_*, DESIGN §6h).  Both hold a ScoreCore: their members' nets, one forward of the members,
-// the chunk loops, the compute() queue and the launch routes.  See include/shifu_b200.h for the contract.
+// bagged ensemble (sb_ensemble_*, DESIGN §6h / §6j).  Both hold a ScoreCore: their members' nets, one forward of the
+// members, the chunk loops, the compute() queue, the sensitivity loop and the launch routes.  See include/shifu_b200.h
+// for the contract.
 #include <string.h>
 #include <algorithm>
 #include <atomic>
@@ -196,6 +197,22 @@ struct Member {
   }
 };
 
+// Column sensitivity's and reason codes' buffers (guarded by ScoreCore::mu), allocated by the first call and grown when a
+// call needs more.  Only z is per member; the rest serves every member.
+struct SensBufs {
+  std::vector<DevBuf<float>> z;   // member g's layer-0 pre-activations of a row chunk [R, ld_out_0(g)]
+  std::vector<size_t> z_n;
+  DevBuf<double> acc;         // running sums [list position][w d^2, w d], then sum w
+  DevBuf<int> cols;           // the column list and its values
+  DevBuf<float> vals;
+  DevBuf<float> d;            // the deltas of one piece [R, piece columns] (max_batch)
+  DevBuf<float> stat;         // ensemble: the statistic of a piece's pair scores [max_batch], laid out like a model's yhat
+  size_t acc_n = 0, cols_n = 0, vals_n = 0;
+  DevBuf<float> reason_d;     // reason codes' running top k of a row chunk [R, k], best first
+  DevBuf<int> reason_pos;
+  size_t reason_d_n = 0, reason_pos_n = 0;
+};
+
 // What a model and an ensemble share.  Member 0 owns the stream and the input staging (stX, Xb / Xf); members 1 .. K-1
 // borrow both (Net::input_from).  A chunk's results are outs[i] [max_batch, outs[i].words] on the device: a model's
 // scores (1 word per row), or an ensemble's scores (K words) and statistics (4 words); a compute() row gets the words of
@@ -211,6 +228,7 @@ struct ScoreCore {
   cudaGraphExec_t mb_graph = nullptr;         // tensor-core modes: the forward of MB_ROWS staged rows
   std::atomic<long long> st[SB_DEBUG_MSTAT_WORDS] = {};   // a model's counters (the first three words are the queue's)
   std::string routes;         // the launches of the last forward, "+"-joined (sb_debug_*_routes; guarded by mu)
+  SensBufs sens;              // sensitivity and reason codes (freed after the destructor's wait)
 
   Net& lead() { return members[0]->net; }
   const Net& lead() const { return members[0]->net; }
@@ -368,20 +386,7 @@ struct ScoreCore {
 // ================================================================================================
 // model
 // ================================================================================================
-struct sb_model : ScoreCore {
-  // sb_model_sensitivity's buffers (guarded by mu), allocated by its first call and grown when a call needs more
-  DevBuf<float> sens_z;       // layer 0's pre-activations of a row chunk [R, ld_out_0]
-  DevBuf<double> sens_acc;    // running sums [list position][w d^2, w d], then sum w
-  DevBuf<int> sens_cols;      // the column list and its values
-  DevBuf<float> sens_vals;
-  DevBuf<float> sens_d;       // the deltas of one piece [R, piece columns] (max_batch)
-  size_t sens_z_n = 0, sens_acc_n = 0, sens_cols_n = 0, sens_vals_n = 0;
-  // sb_model_reason_codes' running top k of a row chunk [R, k], best first (guarded by mu; allocated and grown as above)
-  DevBuf<float> reason_d;
-  DevBuf<int> reason_pos;
-  size_t reason_d_n = 0, reason_pos_n = 0;
-  ~sb_model() { wait(); }     // (the buffers above are freed before the core's destructor runs)
-};
+struct sb_model : ScoreCore {};
 
 static int model_from_desc(const sb_net_desc& d, const float* flat, int64_t n, int device, sb_model_t** out) {
   std::unique_ptr<sb_model> m(new sb_model());
@@ -486,39 +491,53 @@ static int sens_grow(DevBuf<T>* b, size_t* cap, size_t n) {
   return SB_OK;
 }
 
-// Column sensitivity's pieces (sensitivity.cuh, DESIGN §6f), called with m->mu held.  Rows go in row chunks of R rows
-// (sens_chunk_rows); a row chunk's z0 is computed once, and its list positions go in pieces of up to max_batch / R - 1
-// columns, each piece one forward of R (columns + 1) pair rows through layers 1..L and the output unit.  After each
-// forward, piece(r0, rc, k0, ck, wd) consumes the piece's pair scores in n.yhat (pair p = slot * rc + r; wd: the chunk's
-// weights): sb_model_sensitivity's sums and deltas, or sb_model_reason_codes' top-k merge.
+// Column sensitivity's pieces (sensitivity.cuh, DESIGN §6f / §6j), called with m->mu held.  Rows go in row chunks of R rows
+// (sens_chunk_rows); a row chunk is loaded once through member 0 and each member's z0 is computed once, and its list
+// positions go in pieces of up to max_batch / R - 1 columns.  A piece is, per member in member order, one forward of
+// R (columns + 1) pair rows through its layers 1..L and output unit; a model's pair scores land in n.yhat, an
+// ensemble's in its slots, of which ensemble_stat_kernel forms statistic `stat` as one column.  After each piece,
+// piece(y, r0, rc, k0, ck, wd) consumes that column (pair p = slot * rc + r; wd: the chunk's weights): the sums and
+// deltas of sensitivity, or the top-k merge of reason codes.
 template <typename Piece>
-static int sens_forward(sb_model* m, const float* X, const float* w, int64_t rows, int C, const Piece& piece) {
+static int sens_forward(ScoreCore* m, int stat, const float* X, const float* w, int64_t rows, int C, const Piece& piece) {
   Net& n = m->lead();
-  const Layer& l0 = n.layers[0];
+  const int K = static_cast<int>(m->members.size());
   const int R = sens_chunk_rows(n.max_batch, C);
   const int Cp = n.max_batch / R - 1;
-  SB_TRY(sens_grow(&m->sens_z, &m->sens_z_n, static_cast<size_t>(R) * l0.ld_out));
-  const StepIn in{n.desc, n.scal};
-  SensParams sp = {};
-  sp.F = n.F; sp.N = l0.out; sp.ld = l0.ld_out;
-  sp.X = n.stX;
-  sp.z = m->sens_z.p;
-  sp.act = l0.act;
-  if (n.tc()) {
-    sp.bias = n.theta + l0.b_off;
-    sp.Wn = l0.Wn; sp.w_ps = n.Wn_ps[0];
-    sp.out = n.A[0]; sp.out_ps = n.A_ps[0];
-  } else {
-    sp.W32 = n.theta + l0.w_off;
-    sp.out32 = n.Af[0];
-  }
+  SensBufs& sb = m->sens;
+  sb.z.resize(static_cast<size_t>(K));
+  sb.z_n.resize(static_cast<size_t>(K));
   using PerturbFn = void (*)(SensParams);
-  const PerturbFn perturb = !n.tc() ? sens_perturb_kernel<false, 1>
-                                    : n.nparts == 3 ? sens_perturb_kernel<true, 3>
-                                    : n.nparts == 2 ? sens_perturb_kernel<true, 2> : sens_perturb_kernel<true, 1>;
-  const char* perturb_name = !n.tc() ? "sens_perturb<fp32>"
-                             : n.nparts == 3 ? "sens_perturb<bf16x3>"
-                             : n.nparts == 2 ? "sens_perturb<bf16x2>" : "sens_perturb<bf16>";
+  std::vector<SensParams> sp(static_cast<size_t>(K));
+  std::vector<PerturbFn> perturb(static_cast<size_t>(K));
+  std::vector<const char*> perturb_name(static_cast<size_t>(K));
+  for (int g = 0; g < K; ++g) {
+    Net& ng = m->members[g]->net;
+    const Layer& l0 = ng.layers[0];
+    SB_TRY(sens_grow(&sb.z[g], &sb.z_n[g], static_cast<size_t>(R) * l0.ld_out));
+    SensParams& p = sp[g];
+    p = {};
+    p.F = ng.F; p.N = l0.out; p.ld = l0.ld_out;
+    p.X = n.stX;
+    p.z = sb.z[g].p;
+    p.act = l0.act;
+    if (ng.tc()) {
+      p.bias = ng.theta + l0.b_off;
+      p.Wn = l0.Wn; p.w_ps = ng.Wn_ps[0];
+      p.out = ng.A[0]; p.out_ps = ng.A_ps[0];
+    } else {
+      p.W32 = ng.theta + l0.w_off;
+      p.out32 = ng.Af[0];
+    }
+    perturb[g] = !ng.tc() ? sens_perturb_kernel<false, 1>
+                 : ng.nparts == 3 ? sens_perturb_kernel<true, 3>
+                 : ng.nparts == 2 ? sens_perturb_kernel<true, 2> : sens_perturb_kernel<true, 1>;
+    perturb_name[g] = !ng.tc() ? "sens_perturb<fp32>"
+                      : ng.nparts == 3 ? "sens_perturb<bf16x3>"
+                      : ng.nparts == 2 ? "sens_perturb<bf16x2>" : "sens_perturb<bf16>";
+  }
+  if (m->slots && !sb.stat.p) SB_TRY(sb.stat.alloc(static_cast<size_t>(n.max_batch)));
+  float* const y = m->slots ? sb.stat.p : n.yhat;
   const size_t row_bytes = sizeof(float) * n.F;
   for (int64_t r0 = 0; r0 < rows; r0 += R) {
     const int rc = static_cast<int>(rows - r0 < R ? rows - r0 : R);
@@ -527,21 +546,34 @@ static int sens_forward(sb_model* m, const float* X, const float* w, int64_t row
     const float* wd = w ? n.stW : n.ones;
     m->routes.clear();
     SB_TRY(load_rows(n, n.stX, wd, rc));
-    SB_TRY(n.enqueue_layer0_pre(in, rc, m->sens_z.p, l0.ld_out));
+    for (int g = 0; g < K; ++g) {
+      Net& ng = m->members[g]->net;
+      SB_TRY(ng.enqueue_layer0_pre(StepIn{ng.desc, ng.scal}, rc, sb.z[g].p, ng.layers[0].ld_out));
+      sp[g].R = rc;
+    }
     const std::string prefix = m->routes;
-    sp.R = rc;
     for (int k0 = 0; k0 < C; k0 += Cp) {
       const int ck = C - k0 < Cp ? C - k0 : Cp;
       const int pairs = rc * (ck + 1);
       m->routes = prefix;
-      sp.cols = m->sens_cols.p + k0; sp.vals = m->sens_vals.p + k0;
-      const dim3 grid(static_cast<unsigned>((l0.out + 255) / 256), static_cast<unsigned>(ck + 1),
-                      static_cast<unsigned>((rc + SENS_ROWS - 1) / SENS_ROWS));
-      SB_TRY(launch_kernel(perturb, grid, dim3(32, 8), 0, n.stream, false, sp));
-      n.mark(perturb_name);
-      SB_TRY(n.enqueue_hidden_forward(in, pairs, nullptr, nullptr, nullptr, 0, 1));
-      SB_TRY(n.enqueue_out(in, pairs, false, false, n.yhat, nullptr));
-      SB_TRY(piece(r0, rc, k0, ck, wd));
+      for (int g = 0; g < K; ++g) {
+        Net& ng = m->members[g]->net;
+        const StepIn in{ng.desc, ng.scal};
+        sp[g].cols = sb.cols.p + k0; sp[g].vals = sb.vals.p + k0;
+        const dim3 grid(static_cast<unsigned>((sp[g].N + 255) / 256), static_cast<unsigned>(ck + 1),
+                        static_cast<unsigned>((rc + SENS_ROWS - 1) / SENS_ROWS));
+        SB_TRY(launch_kernel(perturb[g], grid, dim3(32, 8), 0, ng.stream, false, sp[g]));
+        ng.mark(perturb_name[g]);
+        SB_TRY(ng.enqueue_hidden_forward(in, pairs, nullptr, nullptr, nullptr, 0, 1));
+        SB_TRY(ng.enqueue_out(in, pairs, false, false, m->slots ? m->slots + static_cast<size_t>(g) * n.max_batch : n.yhat, nullptr));
+      }
+      if (m->slots) {
+        SB_TRY(launch_kernel(ensemble_stat_kernel, dim3(static_cast<unsigned>((pairs + ENS_THREADS - 1) / ENS_THREADS)),
+                             dim3(ENS_THREADS), 0, n.stream, false, static_cast<const float*>(m->slots),
+                             static_cast<long long>(n.max_batch), K, pairs, stat, y));
+        n.mark("ensemble_stat");
+      }
+      SB_TRY(piece(static_cast<const float*>(y), r0, rc, k0, ck, wd));
     }
   }
   return SB_OK;
@@ -566,22 +598,21 @@ static int sens_list(const Net& n, const int32_t* cols, int32_t n_cols, const fl
 }
 
 // the column list and its values to the device (with m->mu held); the running sums are sized with them
-static int sens_upload_list(sb_model* m, const std::vector<int32_t>& cl, const std::vector<float>& vl) {
+static int sens_upload_list(ScoreCore* m, const std::vector<int32_t>& cl, const std::vector<float>& vl) {
   Net& n = m->lead();
+  SensBufs& sb = m->sens;
   const size_t list_n = cl.size();
-  SB_TRY(sens_grow(&m->sens_acc, &m->sens_acc_n, 2 * list_n + 1));
-  SB_TRY(sens_grow(&m->sens_cols, &m->sens_cols_n, list_n));
-  SB_TRY(sens_grow(&m->sens_vals, &m->sens_vals_n, list_n));
-  SB_CUDA(cudaMemcpyAsync(m->sens_cols.p, cl.data(), sizeof(int32_t) * list_n, cudaMemcpyHostToDevice, n.stream));
-  SB_CUDA(cudaMemcpyAsync(m->sens_vals.p, vl.data(), sizeof(float) * list_n, cudaMemcpyHostToDevice, n.stream));
+  SB_TRY(sens_grow(&sb.acc, &sb.acc_n, 2 * list_n + 1));
+  SB_TRY(sens_grow(&sb.cols, &sb.cols_n, list_n));
+  SB_TRY(sens_grow(&sb.vals, &sb.vals_n, list_n));
+  SB_CUDA(cudaMemcpyAsync(sb.cols.p, cl.data(), sizeof(int32_t) * list_n, cudaMemcpyHostToDevice, n.stream));
+  SB_CUDA(cudaMemcpyAsync(sb.vals.p, vl.data(), sizeof(float) * list_n, cudaMemcpyHostToDevice, n.stream));
   return SB_OK;
 }
 
-extern "C" {
-
-int sb_model_sensitivity(sb_model_t* m, const float* X, const float* w, int64_t rows, const int32_t* cols, int32_t n_cols,
-                         const float* values, double* sum_sq, double* sum, double* w_sum, float* deltas) {
-  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
+// sb_model_sensitivity / sb_ensemble_sensitivity after the handle's checks (stat: an ensemble's statistic)
+static int sensitivity(ScoreCore* m, int stat, const float* X, const float* w, int64_t rows, const int32_t* cols, int32_t n_cols,
+                       const float* values, double* sum_sq, double* sum, double* w_sum, float* deltas) {
   SB_CHECK(X && sum_sq && sum && w_sum, SB_ERR_INVALID, "null argument");
   SB_CHECK(rows >= 0, SB_ERR_INVALID, "rows = %lld < 0", static_cast<long long>(rows));
   Net& n = m->lead();
@@ -594,33 +625,33 @@ int sb_model_sensitivity(sb_model_t* m, const float* X, const float* w, int64_t 
   if (rows == 0) return SB_OK;
   std::lock_guard<std::mutex> lk(m->mu);
   SB_CUDA(cudaSetDevice(n.device));
+  SensBufs& sb = m->sens;
   const size_t list_n = static_cast<size_t>(C);
   SB_TRY(sens_upload_list(m, cl, vl));
-  SB_CUDA(cudaMemsetAsync(m->sens_acc.p, 0, sizeof(double) * (2 * list_n + 1), n.stream));
-  if (!m->sens_d.p) SB_TRY(m->sens_d.alloc(static_cast<size_t>(n.max_batch)));
+  SB_CUDA(cudaMemsetAsync(sb.acc.p, 0, sizeof(double) * (2 * list_n + 1), n.stream));
+  if (!sb.d.p) SB_TRY(sb.d.alloc(static_cast<size_t>(n.max_batch)));
   // per piece: d and the sums (sens_reduce_kernel), and the piece's deltas copied out when asked
-  const auto reduce = [&](int64_t r0, int rc, int k0, int ck, const float* wd) -> int {
-    SB_TRY(launch_kernel(sens_reduce_kernel, dim3(static_cast<unsigned>(ck + 1)), dim3(SENS_REDUCE_THREADS), 0, n.stream, false,
-                         static_cast<const float*>(n.yhat), wd, rc, ck, k0, deltas ? m->sens_d.p : nullptr, ck, m->sens_acc.p,
-                         k0 == 0 ? 1 : 0, 2LL * C));
+  const auto reduce = [&](const float* y, int64_t r0, int rc, int k0, int ck, const float* wd) -> int {
+    SB_TRY(launch_kernel(sens_reduce_kernel, dim3(static_cast<unsigned>(ck + 1)), dim3(SENS_REDUCE_THREADS), 0, n.stream, false, y,
+                         wd, rc, ck, k0, deltas ? sb.d.p : nullptr, ck, sb.acc.p, k0 == 0 ? 1 : 0, 2LL * C));
     n.mark("sens_reduce");
     if (deltas)
-      SB_CUDA(cudaMemcpy2DAsync(deltas + r0 * C + k0, sizeof(float) * C, m->sens_d.p, sizeof(float) * ck, sizeof(float) * ck, rc,
+      SB_CUDA(cudaMemcpy2DAsync(deltas + r0 * C + k0, sizeof(float) * C, sb.d.p, sizeof(float) * ck, sizeof(float) * ck, rc,
                                 cudaMemcpyDefault, n.stream));
     return SB_OK;
   };
-  SB_TRY(m->routed([&] { return sens_forward(m, X, w, rows, C, reduce); }));
+  SB_TRY(m->routed([&] { return sens_forward(m, stat, X, w, rows, C, reduce); }));
   std::vector<double> acc(2 * list_n + 1);
-  SB_CUDA(cudaMemcpyAsync(acc.data(), m->sens_acc.p, sizeof(double) * acc.size(), cudaMemcpyDeviceToHost, n.stream));
+  SB_CUDA(cudaMemcpyAsync(acc.data(), sb.acc.p, sizeof(double) * acc.size(), cudaMemcpyDeviceToHost, n.stream));
   SB_CUDA(cudaStreamSynchronize(n.stream));
   for (int k = 0; k < C; ++k) { sum_sq[k] = acc[2 * k]; sum[k] = acc[2 * k + 1]; }
   *w_sum = acc[2 * list_n];
   return SB_OK;
 }
 
-int sb_model_reason_codes(sb_model_t* m, const float* X, int64_t rows, const int32_t* cols, int32_t n_cols, const float* values,
-                          int32_t k, int32_t order, int32_t* pos, float* d, float* scores) {
-  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
+// sb_model_reason_codes / sb_ensemble_reason_codes after the handle's checks (stat: an ensemble's statistic)
+static int reason_codes(ScoreCore* m, int stat, const float* X, int64_t rows, const int32_t* cols, int32_t n_cols,
+                        const float* values, int32_t k, int32_t order, int32_t* pos, float* d, float* scores) {
   SB_CHECK(X && pos && d, SB_ERR_INVALID, "null argument");
   SB_CHECK(rows >= 0, SB_ERR_INVALID, "rows = %lld < 0", static_cast<long long>(rows));
   Net& n = m->lead();
@@ -635,28 +666,42 @@ int sb_model_reason_codes(sb_model_t* m, const float* X, int64_t rows, const int
   if (rows == 0) return SB_OK;
   std::lock_guard<std::mutex> lk(m->mu);
   SB_CUDA(cudaSetDevice(n.device));
+  SensBufs& sb = m->sens;
   SB_TRY(sens_upload_list(m, cl, vl));
   const size_t run_n = static_cast<size_t>(sens_chunk_rows(n.max_batch, C)) * k;
-  SB_TRY(sens_grow(&m->reason_d, &m->reason_d_n, run_n));
-  SB_TRY(sens_grow(&m->reason_pos, &m->reason_pos_n, run_n));
+  SB_TRY(sens_grow(&sb.reason_d, &sb.reason_d_n, run_n));
+  SB_TRY(sens_grow(&sb.reason_pos, &sb.reason_pos_n, run_n));
   // per piece: merge its deltas into each row's running top k (reset by the chunk's first piece); after the chunk's last
   // piece, copy the chunk's top k and base scores out
-  const auto merge = [&](int64_t r0, int rc, int k0, int ck, const float*) -> int {
+  const auto merge = [&](const float* y, int64_t r0, int rc, int k0, int ck, const float*) -> int {
     const unsigned warps = static_cast<unsigned>(std::min((ck + 31) / 32, SENS_TOPK_WARPS));
-    SB_TRY(launch_kernel(sens_topk_kernel, dim3(static_cast<unsigned>(rc)), dim3(32, warps), 0, n.stream, false,
-                         static_cast<const float*>(n.yhat), rc, ck, k0, static_cast<int>(k), static_cast<int>(order), k0 == 0 ? 1 : 0,
-                         m->reason_d.p, m->reason_pos.p));
+    SB_TRY(launch_kernel(sens_topk_kernel, dim3(static_cast<unsigned>(rc)), dim3(32, warps), 0, n.stream, false, y, rc, ck, k0,
+                         static_cast<int>(k), static_cast<int>(order), k0 == 0 ? 1 : 0, sb.reason_d.p, sb.reason_pos.p));
     n.mark("sens_topk");
     if (k0 + ck < C) return SB_OK;
     const size_t out_n = static_cast<size_t>(rc) * k;
-    SB_CUDA(cudaMemcpyAsync(pos + r0 * k, m->reason_pos.p, sizeof(int32_t) * out_n, cudaMemcpyDefault, n.stream));
-    SB_CUDA(cudaMemcpyAsync(d + r0 * k, m->reason_d.p, sizeof(float) * out_n, cudaMemcpyDefault, n.stream));
-    if (scores) SB_CUDA(cudaMemcpyAsync(scores + r0, n.yhat, sizeof(float) * rc, cudaMemcpyDefault, n.stream));
+    SB_CUDA(cudaMemcpyAsync(pos + r0 * k, sb.reason_pos.p, sizeof(int32_t) * out_n, cudaMemcpyDefault, n.stream));
+    SB_CUDA(cudaMemcpyAsync(d + r0 * k, sb.reason_d.p, sizeof(float) * out_n, cudaMemcpyDefault, n.stream));
+    if (scores) SB_CUDA(cudaMemcpyAsync(scores + r0, y, sizeof(float) * rc, cudaMemcpyDefault, n.stream));
     return SB_OK;
   };
-  SB_TRY(m->routed([&] { return sens_forward(m, X, nullptr, rows, C, merge); }));
+  SB_TRY(m->routed([&] { return sens_forward(m, stat, X, nullptr, rows, C, merge); }));
   SB_CUDA(cudaStreamSynchronize(n.stream));
   return SB_OK;
+}
+
+extern "C" {
+
+int sb_model_sensitivity(sb_model_t* m, const float* X, const float* w, int64_t rows, const int32_t* cols, int32_t n_cols,
+                         const float* values, double* sum_sq, double* sum, double* w_sum, float* deltas) {
+  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
+  return sensitivity(m, SB_STAT_MEAN, X, w, rows, cols, n_cols, values, sum_sq, sum, w_sum, deltas);
+}
+
+int sb_model_reason_codes(sb_model_t* m, const float* X, int64_t rows, const int32_t* cols, int32_t n_cols, const float* values,
+                          int32_t k, int32_t order, int32_t* pos, float* d, float* scores) {
+  SB_CHECK(m, SB_ERR_STATE, "TF model not initialized.");
+  return reason_codes(m, SB_STAT_MEAN, X, rows, cols, n_cols, values, k, order, pos, d, scores);
 }
 
 int sb_model_sync(sb_model_t* m) {
@@ -823,6 +868,25 @@ int sb_ensemble_score_row_f64(sb_ensemble_t* e, const double* row, int32_t n, do
   SB_TRY(e->submit(row, v));
   for (int i = 0; i < e->q.words; ++i) out[i] = static_cast<double>(v[i]);
   return SB_OK;
+}
+
+static int check_ensemble_stat(const sb_ensemble* e, int32_t stat) {
+  SB_CHECK(e, SB_ERR_STATE, "TF ensemble not initialized.");
+  SB_CHECK(stat >= SB_STAT_MEAN && stat <= SB_STAT_MEDIAN, SB_ERR_INVALID,
+           "stat = %d is not SB_STAT_MEAN, SB_STAT_MAX, SB_STAT_MIN or SB_STAT_MEDIAN", stat);
+  return SB_OK;
+}
+
+int sb_ensemble_sensitivity(sb_ensemble_t* e, int32_t stat, const float* X, const float* w, int64_t rows, const int32_t* cols,
+                            int32_t n_cols, const float* values, double* sum_sq, double* sum, double* w_sum, float* deltas) {
+  SB_TRY(check_ensemble_stat(e, stat));
+  return sensitivity(e, stat, X, w, rows, cols, n_cols, values, sum_sq, sum, w_sum, deltas);
+}
+
+int sb_ensemble_reason_codes(sb_ensemble_t* e, int32_t stat, const float* X, int64_t rows, const int32_t* cols, int32_t n_cols,
+                             const float* values, int32_t k, int32_t order, int32_t* pos, float* d, float* scores) {
+  SB_TRY(check_ensemble_stat(e, stat));
+  return reason_codes(e, stat, X, rows, cols, n_cols, values, k, order, pos, d, scores);
 }
 
 int sb_ensemble_sync(sb_ensemble_t* e) {

@@ -78,6 +78,27 @@ def _targets(targets, weights, rows: int):
     return y, w
 
 
+def _sensitivity(fn, rows, weights, columns, values, **kw) -> dict:
+    """computeSensitivity through fn (Model.sensitivity or Ensemble.sensitivity; kw: its further arguments)"""
+    X = np.asarray(rows, dtype=np.float64).astype(np.float32)     # the same double -> float cast as computeBatch
+    w = None if weights is None else np.asarray(weights, dtype=np.float64).astype(np.float32)
+    vals = None if values is None else np.asarray(values, dtype=np.float64).astype(np.float32)
+    r = fn(X, w=w, cols=columns, values=vals, **kw)
+    ws = r["w_sum"]
+    with np.errstate(invalid="ignore", divide="ignore"):
+        mse, mean = r["sum_sq"] / ws, r["sum"] / ws
+    return {"sum_sq": r["sum_sq"], "sum": r["sum"], "w_sum": ws, "mse": mse, "mean": mean}
+
+
+def _reason_codes(fn, rows, k, columns, values, order, **kw) -> dict:
+    """computeReasonCodes through fn (Model.reason_codes or Ensemble.reason_codes; kw: its further arguments)"""
+    X = np.asarray(rows, dtype=np.float64).astype(np.float32)     # the same double -> float cast as computeBatch
+    vals = None if values is None else np.asarray(values, dtype=np.float64).astype(np.float32)
+    cl = np.arange(X.shape[1], dtype=np.int32) if columns is None else np.asarray(columns, dtype=np.int32).reshape(-1)
+    r = fn(X, k, cols=columns, values=vals, order=order, scores=True, **kw)
+    return {"columns": cl[r["pos"]], "deltas": r["d"], "scores": r["scores"]}
+
+
 class TensorflowModel:
     def __init__(self, device: int = 0, precision: int = capi.PREC_FP32):
         self.properties: Dict[str, Any] = {}
@@ -159,14 +180,7 @@ class TensorflowModel:
         0 per column (the mean of a ZSCALE-normalised column)"""
         if not self.initiate or self._model is None:
             raise IllegalStateException("TF model not initialized.")
-        X = np.asarray(rows, dtype=np.float64).astype(np.float32)     # the same double -> float cast as computeBatch
-        w = None if weights is None else np.asarray(weights, dtype=np.float64).astype(np.float32)
-        vals = None if values is None else np.asarray(values, dtype=np.float64).astype(np.float32)
-        r = self._model.sensitivity(X, w=w, cols=columns, values=vals)
-        ws = r["w_sum"]
-        with np.errstate(invalid="ignore", divide="ignore"):
-            mse, mean = r["sum_sq"] / ws, r["sum"] / ws
-        return {"sum_sq": r["sum_sq"], "sum": r["sum"], "w_sum": ws, "mse": mse, "mean": mean}
+        return _sensitivity(self._model.sensitivity, rows, weights, columns, values)
 
     # -- new: per-row reason codes: the columns whose replacement moves each row's score the most --
     def computeReasonCodes(self, rows, k, columns=None, values=None, order="raise") -> dict:
@@ -176,11 +190,7 @@ class TensorflowModel:
         column; values None: 0 per column (the mean of a ZSCALE-normalised column)"""
         if not self.initiate or self._model is None:
             raise IllegalStateException("TF model not initialized.")
-        X = np.asarray(rows, dtype=np.float64).astype(np.float32)     # the same double -> float cast as computeBatch
-        vals = None if values is None else np.asarray(values, dtype=np.float64).astype(np.float32)
-        cl = np.arange(X.shape[1], dtype=np.int32) if columns is None else np.asarray(columns, dtype=np.int32).reshape(-1)
-        r = self._model.reason_codes(X, k, cols=columns, values=vals, order=order, scores=True)
-        return {"columns": cl[r["pos"]], "deltas": r["d"], "scores": r["scores"]}
+        return _reason_codes(self._model.reason_codes, rows, k, columns, values, order)
 
     # -- new: how good the model is on a scored set (what `shifu eval` reports), computed on the GPU --
     def computePerformance(self, rows, targets, weights=None, buckets=10) -> dict:
@@ -255,6 +265,25 @@ class TensorflowEnsemble:
         out = {"scores": s.astype(np.float64)}
         out.update({name: t[:, i].astype(np.float64) for i, name in enumerate(capi.ENSEMBLE_STATS)})
         return out
+
+    def _stat(self, score) -> str:
+        if not isinstance(score, str) or score not in capi.ENSEMBLE_STATS:
+            raise ValueError("score must be one of %s" % (capi.ENSEMBLE_STATS,))
+        return score
+
+    # -- column sensitivity of the shipped score: score = "mean" | "max" | "min" | "median" of the member scores --
+    def computeSensitivity(self, rows, weights=None, columns=None, values=None, score="mean") -> dict:
+        """TensorflowModel.computeSensitivity with d = S(row) - S(row with the column set to its value), S the
+        statistic `score` of the members' scores"""
+        e = self._check()
+        return _sensitivity(e.sensitivity, rows, weights, columns, values, stat=self._stat(score))
+
+    # -- per-row reason codes of the shipped score --
+    def computeReasonCodes(self, rows, k, columns=None, values=None, order="raise", score="mean") -> dict:
+        """TensorflowModel.computeReasonCodes with d = S(row) - S(row with the column set to its value) and "scores" =
+        S(row), S the statistic `score` of the members' scores"""
+        e = self._check()
+        return _reason_codes(e.reason_codes, rows, k, columns, values, order, stat=self._stat(score))
 
     # -- how good one column is on a scored set: score = "mean" | "max" | "min" | "median" or a member index --
     def computePerformance(self, rows, targets, weights=None, buckets=10, score="mean") -> dict:
